@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Headline benchmark of the Mega-NeRF rendering hot path on B200 (BASELINE.json metric).
+"""Headline benchmark of the Mega-NeRF rendering hot path on H100 (BASELINE.json metric).
 
-  python bench.py --gpus N --steps K --warmup W            # this repo's sm_100a path
+  python bench.py --gpus N --steps K --warmup W            # this repo's sm_90a path
   python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm on host CPU cores
 
 A "step" is one render_rays() pass over one batch of synthetic rays: BASELINE.json configs[1]
@@ -13,8 +13,8 @@ With N > 1 the per-GPU batch is BASELINE configs[2]'s shard (65 536 rays / 8 = 8
 
 Prints ONE JSON line on rank 0 (see the task contract): value = ray-samples/s with inputs resident in HBM
 (device-timed with CUDA events), e2e = the same through the public API from pinned host buffers including
-H2D/D2H, roofline for the dominant (MLP) kernel, cpu_baseline = the UNMODIFIED reference (baseline/_ref, see
-baseline/README.md; `kind: "reference"`) timed on the host cores - the oracle port (`kind: "port"`) when _ref is absent.
+H2D/D2H, roofline for the dominant (MLP) kernel, cpu_baseline = the UNMODIFIED reference (oracle/_ref, see
+oracle/make_ref.py; `kind: "reference"`) timed on the host cores - the oracle port (`kind: "port"`) when _ref is absent.
 """
 from __future__ import annotations
 
@@ -40,14 +40,14 @@ MARGIN = 1.15
 # for diagnostics only (python bench.py --workload c4); their lines carry the same keys.
 WORKLOADS = {
     'c2': dict(desc='BASELINE configs[1]: mega-nerf 8-submodule 256-ch', rays=4096, spec={}, grid=(2, 4), sh_deg=None,
-               kernel='tc_mlp_tp_kernel'),
+               kernel='tc_mlp_wg_kernel'),
     # configs[2]: 65 536 rays per iteration over 8 GPUs = 8192 rays per GPU; the default when N > 1
     'c3': dict(desc='BASELINE configs[2] shard: mega-nerf 8-submodule 256-ch, 65536 rays / 8 GPUs', rays=8192, spec={}, grid=(2, 4),
-               sh_deg=None, kernel='tc_mlp_tp_kernel'),
+               sh_deg=None, kernel='tc_mlp_wg_kernel'),
     'c4': dict(desc='BASELINE configs[3] shape: mega-nerf 25-submodule 512-ch', rays=4096, spec=dict(layer_dim=512), grid=(5, 5),
-               sh_deg=None, kernel='tc_mlp_wide_kernel'),
+               sh_deg=None, kernel='tc_mlp_wg_kernel'),
     'c5': dict(desc='BASELINE configs[4]: mega-nerf-sh-3 (SH degree 2 head) 8-submodule 256-ch', rays=8192,
-               spec=dict(pos_dir_dim=0, rgb_dim=27), grid=(2, 4), sh_deg=2, kernel='tc_mlp_tp_kernel'),
+               spec=dict(pos_dir_dim=0, rgb_dim=27), grid=(2, 4), sh_deg=2, kernel='tc_mlp_wg_kernel'),
 }
 WL = WORKLOADS['c2']
 
@@ -64,11 +64,12 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(tflops=d['bf16_tflops'], tflops_sustained=d.get('bf16_tflops_sustained'), hbm=d['hbm_gbs'], src='measured')
-    return dict(tflops=1590.0, tflops_sustained=1400.0, hbm=6650.0, src='fallback')
+    # H100 SXM data sheet (dense fp16 / bf16 tensor rate, HBM3 bandwidth at a 700 W power limit); not measured
+    return dict(tflops=989.0, tflops_sustained=None, hbm=3350.0, src='datasheet')
 
 
 # ------------------------------------------------------------------------------------------------
-# The unmodified reference (baseline/_ref/mega_nerf, a copy of /root/reference/mega_nerf made by baseline/make_ref.py)
+# The unmodified reference (oracle/_ref/mega_nerf, a copy of the reference package made by oracle/make_ref.py)
 # ------------------------------------------------------------------------------------------------
 _REF = None
 
@@ -78,7 +79,7 @@ def load_reference():
     global _REF
     if _REF is not None:
         return _REF or None
-    ref_root = os.path.join(ROOT, 'baseline', '_ref')
+    ref_root = os.path.join(ROOT, 'oracle', '_ref')
     if os.environ.get('MN_BENCH_NO_REF') == '1' or not os.path.isdir(os.path.join(ref_root, 'mega_nerf')):
         _REF = False
         return None
@@ -92,7 +93,7 @@ def load_reference():
         _REF = Namespace(render_rays=render_rays, NeRF=NeRF, ShiftedSoftplus=ShiftedSoftplus, MegaNeRF=MegaNeRF,
                          Cascade=Cascade, path=os.path.dirname(mega_nerf.__file__))
     except Exception as e:  # noqa: BLE001
-        log(f'baseline/_ref present but not importable ({e!r}); falling back to the oracle port')
+        log(f'oracle/_ref present but not importable ({e!r}); falling back to the oracle port')
         _REF = False
     finally:
         if ref_root in sys.path:
@@ -120,26 +121,12 @@ def reference_net(R, net, device='cpu'):
 
 
 def cpu_renderer(O, net, opts):
-    """-> (fn(rays, idx) -> results, kind): the reference itself when baseline/_ref is there, else the oracle port."""
+    """-> (fn(rays, idx) -> results, kind): the reference itself when oracle/_ref is there, else the oracle port."""
     R = load_reference()
     if R is not None:
         rnet, hp = reference_net(R, net), Namespace(**vars(opts))
         return (lambda r, i: R.render_rays(rnet, None, r, i, hp, None, None, True, False, False)[0]), 'reference'
     return (lambda r, i: O.render_rays(net, None, r, i, opts, None, None, True, False, False)[0]), 'port'
-
-
-def kernel_traffic(kernel: str, workload_name: str, precision: str):
-    """DRAM traffic per launch of `kernel` from the committed ncu capture of this workload (profiles/kernel_traffic.json)."""
-    p = os.path.join(ROOT, 'profiles', 'kernel_traffic.json')
-    if not os.path.exists(p):
-        return None
-    try:
-        for e in json.load(open(p)):
-            if e['kernel'] == kernel and e['workload'] == workload_name and e['precision'] == precision:
-                return e
-    except Exception:  # noqa: BLE001
-        pass
-    return None
 
 
 def workload(seed_shift: int = 0):
@@ -177,7 +164,7 @@ def flops_per_row(spec) -> int:
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -240,7 +227,7 @@ def cpu_rays_per_sec(render, rays, idx, n_probe: int = 64) -> float:
 
 def run_reference(args, rank: int):
     """The reference's own CPU implementation of the path on the host cores: the unmodified mega_nerf.rendering.render_rays
-    + mega_nerf.models from baseline/_ref (kind "reference"); the oracle port of it (oracle/mn_oracle.py, kind "port") only
+    + mega_nerf.models from oracle/_ref (kind "reference"); the oracle port of it (oracle/mn_oracle.py, kind "port") only
     when _ref is absent."""
     if rank != 0:
         return
@@ -268,8 +255,8 @@ def run_reference(args, rank: int):
         'config': {'workload': workload_string(), 'cpu_sample': f'each CPU step renders a {sample}-ray sample of it'},
         'cpu_baseline': {'value': value, 'unit': 'samples/s', 'cores': torch.get_num_threads(), 'kind': kind,
                          'sample': f'{sample} of {N_RAYS} rays per step, {args.steps} steps',
-                         'what': ('unmodified mega_nerf.rendering.render_rays + mega_nerf.models (baseline/_ref), torch CPU fp32, '
-                                  'inference_mode' if kind == 'reference' else 'oracle port (baseline/_ref absent)')},
+                         'what': ('unmodified mega_nerf.rendering.render_rays + mega_nerf.models (oracle/_ref), torch CPU fp32, '
+                                  'inference_mode' if kind == 'reference' else 'oracle port (oracle/_ref absent)')},
         'e2e': {'value': value, 'unit': 'samples/s', 'h2d_bytes_per_step': 0, 'd2h_bytes_per_step': 0},
         'gpu_launches': 0,
     }
@@ -277,13 +264,13 @@ def run_reference(args, rank: int):
 
 
 def gpu_incumbent(O, net, rays_d, idx_d, opts, dev, steps: int = 5):
-    """SURVEY.md §8d "GPU incumbent": the UNMODIFIED reference (baseline/_ref: mega_nerf.rendering.render_rays over
-    mega_nerf.models, i.e. cuBLAS GEMMs + ~10^3 ATen elementwise launches per step) through torch-CUDA on the SAME B200
+    """SURVEY.md §8d "GPU incumbent": the UNMODIFIED reference (oracle/_ref: mega_nerf.rendering.render_rays over
+    mega_nerf.models, i.e. cuBLAS GEMMs + ~10^3 ATen elementwise launches per step) through torch-CUDA on the SAME GPU
     in the three precisions it can run in - fp32, TF32, and autocast fp16 (its default, runner.py:243); the oracle
     restatement moved to CUDA when _ref is absent.  A baseline leg like cpu_baseline: reported next to the product's
     number, never on the product path.  Any failure is reported, not raised."""
     R = load_reference()
-    out = {'kind': 'reference (baseline/_ref under torch-CUDA eager, same GPU)' if R is not None else
+    out = {'kind': 'reference (oracle/_ref under torch-CUDA eager, same GPU)' if R is not None else
                    'port (oracle restatement under torch-CUDA eager, same GPU)', 'unit': 'samples/s', 'steps': steps}
     try:
         n = rays_d.shape[0]
@@ -317,6 +304,29 @@ def gpu_incumbent(O, net, rays_d, idx_d, opts, dev, steps: int = 5):
     except Exception as e:  # noqa: BLE001
         out['error'] = repr(e)[:300]
     return out
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, res: dict, gathered=None) -> None:
+    """Write each result array of one render step as out_dir/<key>.npy in float32 (gathered: the all-gathered buffer).
+    Arrays beyond the 64 MiB budget are replaced by a fixed, seeded sample of their rows (<key>.rows.npy holds the indices)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v for k, v in res.items() if torch.is_tensor(v)}
+    if gathered is not None:
+        arrays['gathered'] = gathered
+    total = sum(v.numel() * 4 for v in arrays.values())
+    for k, v in sorted(arrays.items()):
+        a = v.detach().float().cpu()
+        if total > DUMP_LIMIT_BYTES and a.dim() > 0:
+            keep = max(1, int(a.shape[0] * DUMP_LIMIT_BYTES / total))
+            rows = torch.randperm(a.shape[0], generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            a = a[rows]
+            np.save(os.path.join(out_dir, f'{k}.rows.npy'), rows.numpy())
+        np.save(os.path.join(out_dir, f'{k}.npy'), a.numpy())
+    log(f'dumped {len(arrays)} arrays to {out_dir}')
 
 
 def log(msg):
@@ -414,7 +424,7 @@ def run_train(args, rank, local_rank, world):
         'config': {'workload': f'{WL["desc"]}, {N_RAYS} rays x ({COARSE} coarse + {FINE} fine), train() mode (jitter, density '
                                f'noise, random resampling), boundary_margin {MARGIN} (m = {mult:.3f}), MSE vs random colours, Adam',
                    'parallelism': 'single GPU',
-                   'precision': ('tc_f16: recording forward, data gradients and weight gradients on tcgen05 (fp16 operands, fp32 accumulate)'
+                   'precision': ('tc_f16: recording forward, data gradients and weight gradients on wgmma (fp16 operands, fp32 accumulate)'
                                  if on_tc else 'fp32 (CUDA-core kernels, the parity mode)'),
                    'fp32_parity_mode_ms_per_step': other,
                    'launch': 'eager', 'l2': f'flushed between timed iterations ({L2_FLUSH_BYTES >> 20} MiB write)'},
@@ -422,7 +432,7 @@ def run_train(args, rank, local_rank, world):
                 'h2d_bytes_per_step': (rays_pin.numel() + idx_pin.numel() + rgbs_pin.numel()) * 4, 'd2h_bytes_per_step': 4},
         'gpu_launches': int(launches_per_step * args.steps),
         'clocks': clocks,
-        'roofline': {'bound': 'tensor', 'kernel': ('tc_mlp_pp_kernel<TRAIN_FWD> + tc_mlp_pp_kernel<DGRAD> + tc_wgrad_kernel' if on_tc else
+        'roofline': {'bound': 'tensor', 'kernel': ('tc_mlp_wg_kernel<TRAIN_FWD> + tc_mlp_wg_kernel<DGRAD> + tc_wgrad_kernel' if on_tc else
                                                     'mlp_simt_kernel<SAVE> + mlp_bwd_data_kernel + mlp_bwd_weight_kernel'),
                      'achieved': achieved, 'peak': pk['tflops'], 'unit': 'TFLOP/s', 'frac': achieved / pk['tflops'],
                      'peak_source': pk['src'], 'traffic': None, 'kernel_ms_per_step': kms,
@@ -437,7 +447,7 @@ def run_cluster(args, local_rank):
     centroids of the C2 grid: rays/s of mn_cluster_min_dist_ratios, device-timed, next to the restatement on the host cores
     (bounded sample).  The kernel reads 32 B/ray and writes (4K + K) B/ray, so HBM is irrelevant (a few GB/s): the work is
     S x K distance evaluations per ray (sqrt + div each), i.e. it is bound by the fp32 / SFU issue rate; `roofline`
-    reports distance evaluations per second against 148 SMs x 128 lanes x clock / ~12 issue slots per evaluation."""
+    reports distance evaluations per second against SMs x 128 lanes x clock / ~12 issue slots per evaluation."""
     import mega_nerf_b200 as M  # noqa: F401
     from mega_nerf_b200 import cluster_masks as CM
     from oracle import mn_oracle as O
@@ -485,8 +495,8 @@ def run_cluster(args, local_rank):
         O.cluster_min_dist_ratios(rays_h[:n_cpu], zs, cent, True)
         dt = time.perf_counter() - t0
     evals = n * S * 8
-    sm_mhz = clocks.get('sm_mhz') or 1965.0
-    peak = 148 * 128 * sm_mhz * 1e6 / 12.0
+    sm_mhz = clocks.get('sm_mhz') or clocks.get('sm_max_mhz') or 1980.0
+    peak = torch.cuda.get_device_properties(dev).multi_processor_count * 128 * sm_mhz * 1e6 / 12.0
     line = {'metric': 'cluster-mask rays/sec (1000 samples x 8 centroids per ray)', 'value': n / (ms * 1e-3), 'unit': 'rays/s',
             'n_gpus': 1, 'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': ms, 'higher_is_better': True, 'scaling': 'weak',
             'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
@@ -528,11 +538,17 @@ def main():
                          "'peer' = one kernel of ours storing into every rank's symmetric buffer over NVLink (mega_nerf_b200.dist.PeerGather)")
     ap.add_argument('--train-precision', default='tc_f16', choices=['fp32', 'tc_f16'], help="--mode train: arithmetic of the recording forward "
                     "and the backward pass ('fp32' = CUDA-core parity mode)")
+    ap.add_argument('--dump-outputs', default=None, metavar='DIR',
+                    help="after the timed steps, write the arrays the timed render path returned in its last step to DIR/<name>.npy "
+                         "(float32; rank 0; with N > 1 also the all-gathered [rays, 4] buffer as gathered.npy); inputs are seeded, so "
+                         "two builds can be compared output for output")
     ap.add_argument('--mode', default='render', choices=['render', 'train', 'cluster'],
                     help="'render' = the graded line; 'train' = one optimisation step (forward + backward + Adam) of the same "
                          "workload through the recording path (SURVEY.md §8f-1); 'cluster' = the cluster-mask kernel on one "
                          "48k-ray chunk x 1000 samples (SURVEY.md §8f-3); both diagnostics only")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != 'b200' or args.mode != 'render'):
+        ap.error('--dump-outputs applies to the render path (--impl b200 --mode render)')
     rank = int(os.environ.get('RANK', '0'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))
     world = int(os.environ.get('WORLD_SIZE', '1'))
@@ -600,12 +616,16 @@ def main():
         exchange(res)
         return res
 
+    last = {}           # result of the most recent resident step (--dump-outputs)
+
     def step_resident():
         if graphed is None:
-            return step_eager()
-        res = graphed(rays_d, idx_d)                 # device-resident inputs -> static buffers (D2D) -> graph replay
-        if graphed.post is None:
-            exchange(res)
+            res = step_eager()
+        else:
+            res = graphed(rays_d, idx_d)             # device-resident inputs -> static buffers (D2D) -> graph replay
+            if graphed.post is None:
+                exchange(res)
+        last['res'] = res
         return res
 
     def step_e2e():
@@ -670,6 +690,8 @@ def main():
     if rank == 0:
         sampler.start()
     ms_total = timed(step_resident, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last['res'], (pg.buf if pg is not None else gather_buf) if world > 1 else None)
     launches = launches_per_step * args.steps
     samples_per_step = N_RAYS * (COARSE + FINE) * world
     value = samples_per_step * args.steps / (ms_total * 1e-3)
@@ -707,10 +729,7 @@ def main():
     kernel_ms_per_step = tot_ms.value / args.steps
     achieved = flops_step / (kernel_ms_per_step * 1e-3) / 1e12 if kernel_ms_per_step > 0 else 0.0
     passes = {'fp32': 1, 'tc_f16': 1, 'tc_f16x3': 3}[args.precision]
-    kernel_name = {'fp32': 'mlp_simt_kernel', 'tc_f16': WL['kernel'], 'tc_f16x3': 'tc_mlp_kernel<split>'}[args.precision]
-    if kernel_name == 'tc_mlp_tp_kernel' and os.environ.get('MN_TC_TP', '1') == '0':
-        kernel_name = 'tc_mlp_pp_kernel'          # A/B switch of libmn_b200.so: the shared-memory ping-pong kernel
-    traffic = kernel_traffic(kernel_name, args.workload if world == 1 else 'c3', args.precision)
+    kernel_name = {'fp32': 'mlp_simt_kernel', 'tc_f16': WL['kernel'], 'tc_f16x3': 'tc_mlp_wg_kernel<split>'}[args.precision]
 
     log(f'mlp kernel: {kernel_ms_per_step:.3f} ms/step, m={mult:.3f}')
     # ---- parity against the CPU checker (not timed).  Every rank checks (a) the first N_PAR of its own rays through the
@@ -750,7 +769,7 @@ def main():
         log(f'parity: rgb {par_rgb:.2e} depth {par_depth:.2e}' + (f' gathered rgb {par_g_rgb:.2e} depth {par_g_depth:.2e}' if world > 1 else ''))
         cpu = None
         if world == 1 and not args.no_cpu_baseline:
-            # the reference's own CPU path (baseline/_ref; oracle port when absent) on a bounded sample of the same batch
+            # the reference's own CPU path (oracle/_ref; oracle port when absent) on a bounded sample of the same batch
             torch.set_num_threads(usable_cpus())
             render_cpu, cpu_kind = cpu_renderer(O, net, opts)
             rate = cpu_rays_per_sec(render_cpu, rays_h, idx_h)
@@ -793,11 +812,9 @@ def main():
                          'achieved': achieved, 'peak': pk['tflops'], 'unit': 'TFLOP/s', 'frac': achieved / pk['tflops'],
                          'frac_of_sustained_peak': achieved / pk['tflops_sustained'] if pk['tflops_sustained'] else None,
                          'peak_source': pk['src'],
-                         # dram__bytes_read.sum + dram__bytes_write.sum per launch of this kernel on this workload, from the committed
-                         # `ncu --set full` capture (profiles/kernel_traffic.json, written by scripts/ncu_extract.py from the
-                         # .ncu-rep next to it); null when no capture of this (kernel, workload, precision) is committed
-                         'traffic': traffic['dram_bytes'] if traffic else None,
-                         'traffic_detail': traffic,
+                         # DRAM traffic of the kernel is not measured (no hardware-counter profiler on the benchmark machines)
+                         'traffic': None,
+                         'traffic_detail': None,
                          'algorithmic_flops_per_row': fl_row, 'mma_passes_per_algorithmic': passes,
                          'kernel_ms_per_step': kernel_ms_per_step, 'launches_per_step': n_l.value / args.steps},
             'parity': {'max_rel_rgb_vs_oracle': par_rgb, 'max_rel_depth_vs_oracle': par_depth, 'rays_checked_per_rank': N_PAR,

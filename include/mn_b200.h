@@ -1,5 +1,5 @@
 /*
- * mn_b200.h — C ABI of the B200-native Mega-NeRF rendering hot path (libmn_b200.so).
+ * mn_b200.h — C ABI of the Mega-NeRF rendering hot path for H100 (sm_90a; libmn_b200.so).
  *
  * The reference (cmusatyalab/mega-nerf @76d8d76b) is pure Python/PyTorch and has NO FFI / plugin
  * boundary of its own (SURVEY.md §8b); this header defines the boundary underneath the Python call
@@ -42,8 +42,8 @@ enum {
 /* Arithmetic of the MLP stage. */
 enum {
     MN_PREC_FP32 = 0,      /* CUDA-core fp32 FMA, parity mode (<= 1e-5 of the fp32 oracle)              */
-    MN_PREC_TC_F16 = 1,    /* tcgen05 kind::f16, fp16 operands, fp32 TMEM accumulate, 1 MMA pass        */
-    MN_PREC_TC_F16X3 = 2   /* tcgen05, hi/lo fp16 split of both operands, 3 MMA passes per algorithmic  */
+    MN_PREC_TC_F16 = 1,    /* wgmma, fp16 operands, fp32 register accumulate, 1 MMA pass                */
+    MN_PREC_TC_F16X3 = 2   /* wgmma, hi/lo fp16 split of both operands, 3 MMA passes per algorithmic    */
 };
 
 typedef struct mn_ctx mn_ctx;
@@ -296,7 +296,7 @@ int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const
  * What the reference does on a GPU: Linear layers in fp16 with fp32 accumulation under autocast, gradients scaled into
  * fp16 range (runner.py:243-274, opts.py:99).  Forward = the tc_f16 inference kernel writing every layer's fp16
  * activations to the tape; backward = data gradients on transposed fp16 weight images (ReLU masks from the tape, gradient
- * images scaled by a power of two chosen from max|grad_out|), weight gradients as tcgen05 contractions of the two tapes
+ * images scaled by a power of two chosen from max|grad_out|), weight gradients as wgmma contractions of the two tapes
  * over the slot axis, fp32 accumulation, fp32 atomics into param_grads_d.  Same argument meaning as the fp32 entry points
  * above; covers layer_dim 256 with a direction / appearance head and rgb_dim 3 (mn_model_train_tc_supported), everything
  * else returns MN_ERR_UNSUPPORTED - use the fp32 entry points.  Gradients agree with the fp32 path to ~1e-2 of each
@@ -311,17 +311,21 @@ int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, co
                          size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream);
 
 /* ---- test hook (host only, no CUDA call) ---------------------------------------------------------------------------
- * The role tables of the default inference MLP kernel (csrc/mn_mlp_tp.cuh) for one network shape: `desc` as for
- * mn_model_create (only the per-sub-module fields matter).  table_out receives up to cap_entries 16-byte entries - first the
- * MMA issuers' block entries, then the TMA producer's stage entries - and info[8] = {issuer entries, issuer entries of a
- * sigma_only call, producer entries, producer entries of a sigma_only call, bytes of one sub-module's weight image, ring stages,
- * shared-memory bytes, feature-tile bytes}.  Returns MN_ERR_UNSUPPORTED for shapes this kernel does not run (layer_dim 512,
- * fp32-only shapes).  Used by tests/test_tp_program.py to check the tables' invariants without a GPU. */
+ * The stage program of the tensor-core MLP kernel (csrc/mn_mlp_wg.cuh, precision tc_f16) for one network shape: `desc` as for
+ * mn_model_create (only the per-sub-module fields matter).  The producer and both consumer warpgroups walk this program, one
+ * entry per weight-ring stage of one 128-row tile.  table_out receives up to cap_entries entries of 8 unsigned ints: weight
+ * byte offset in the sub-module's pack, weight bytes, B rows (N), K columns, first K column of the A operand, feature-segment
+ * byte offset and bytes (first stage of a feature segment, else 0), flags | GEMM << 8 | N-chunk << 16 (flags: 1 A from the
+ * feature buffer, 2 first / 4 last stage of a feature segment, 8 lo planes, 16 first / 32 last stage of an accumulator).
+ * info[8] = {entries, entries of a sigma_only call, bytes of one weight plane of a sub-module, ring stages, shared-memory bytes,
+ * feature-tile bytes, ring-stage bytes, K columns per stage}.  Returns MN_ERR_UNSUPPORTED for shapes only the fp32 kernels
+ * run, MN_ERR_WORKSPACE when cap_entries is too small.  Used by tests/test_tp_program.py and tests/tp_protocol_sim.py. */
 int mn_debug_tp_program(const mn_model_desc* desc, unsigned int* table_out, int cap_entries, int* info8);
-/* In-kernel timeline of CTA 0 of the shared-memory ping-pong MLP kernel and the SM clock during the last MLP launch; recorded
- * only when the process runs with MN_TC_TRACE=1 (scripts/tc_trace.py).  out: [2][2048] (tag, globaltimer ns) pairs of the MMA
- * issuer / epilogue warp 0, counts[2] their numbers, reset != 0 clears them; out4 = {clock64, globaltimer} at kernel start and
- * end.  Both synchronise the device. */
+/* ---- debug hooks ----------------------------------------------------------------------------------------------------
+ * SM clock during the last tensor-core MLP launch, recorded only when the process runs with MN_TC_TRACE=1: out4 = {clock64,
+ * globaltimer} at kernel start and end.  mn_debug_read_trace returns the in-kernel event buffer ([2][2048] (tag, globaltimer ns)
+ * pairs, counts[2] their numbers, reset != 0 clears them); the current MLP kernel records no events into it.  Both synchronise
+ * the device. */
 int mn_debug_read_trace(unsigned long long* out, unsigned int* counts, int reset);
 int mn_debug_read_clock(unsigned long long* out4);
 

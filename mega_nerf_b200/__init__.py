@@ -1,7 +1,7 @@
-"""B200-native drop-in for the Mega-NeRF rendering hot path.
+"""H100-native drop-in for the Mega-NeRF rendering hot path.
 
 Mirrors the reference's Python call surface (mega_nerf/rendering.py, ray_utils.py, models/*.py) on top
-of libmn_b200.so (hand-written sm_100a CUDA behind the C ABI in include/mn_b200.h).
+of libmn_b200.so (hand-written sm_90a CUDA behind the C ABI in include/mn_b200.h).
 """
 from .modules import (Embedding, ShiftedSoftplus, NeRF, MegaNeRF, Cascade, get_nerf, get_bg_nerf,  # noqa: F401
                       set_precision, get_precision, set_train_precision, get_train_precision)

@@ -132,7 +132,7 @@ def lib():
 def ctx(device: torch.device) -> int:
     """Per-device native context."""
     if device.type != 'cuda':
-        raise RuntimeError('mega_nerf_b200 runs on CUDA (sm_100a) tensors only; there is no CPU path')
+        raise RuntimeError('mega_nerf_b200 runs on CUDA (sm_90a) tensors only; there is no CPU path')
     idx = device.index if device.index is not None else torch.cuda.current_device()
     with _lock:
         h = _ctx.get(idx)

@@ -3,8 +3,8 @@
 
 Gradient flow is the reference's: per-sample (rgb, sigma) receive gradients from the composited colour
 and from bg_lambda; depth / depth_variance / weights are outputs without gradient (rendering.py:381,
-:215); sample positions, directions and image indices are inputs without gradient.  Only fp32 (CUDA-core)
-kernels exist for the backward pass in this round, so a recording forward always runs in fp32 whatever
+:215); sample positions, directions and image indices are inputs without gradient.  A recording forward runs in the
+arithmetic of `set_train_precision` ('fp32' CUDA-core kernels by default, or 'tc_f16' on the tensor cores) whatever
 `set_precision` says.
 """
 from __future__ import annotations

@@ -215,8 +215,8 @@ int mn_create(mn_ctx** out, int device) {
     cudaDeviceProp prop;
     MN_CUDA(c, cudaGetDeviceProperties(&prop, device));
     c->sm_count = prop.multiProcessorCount;
-    if (prop.major != 10) {
-        c->err = std::string("libmn_b200 is built for sm_100a only; found ") + prop.name;
+    if (prop.major != 9 || prop.minor != 0) {
+        c->err = std::string("libmn_b200 is built for sm_90a (Hopper) only; found ") + prop.name;
         return MN_ERR_UNSUPPORTED;
     }
     MN_CUDA(c, cudaMalloc(&c->status_d, sizeof(unsigned int)));
@@ -319,8 +319,6 @@ void mn_model_destroy(mn_model* m) {
     if (m->counters_d) cudaFree(m->counters_d);
     if (m->tc_packed) cudaFree(m->tc_packed);
     if (m->tc_dgrad) cudaFree(m->tc_dgrad);
-    if (m->tc_tp) cudaFree(m->tc_tp);
-    if (m->tp_prog) cudaFree(m->tp_prog);
     delete m;
 }
 

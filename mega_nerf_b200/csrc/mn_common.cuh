@@ -33,7 +33,7 @@ struct PackOp {
 
 struct mn_ctx {
     int device = 0;
-    int sm_count = 148;
+    int sm_count = 132;
     std::string err;
     unsigned int* status_d = nullptr;
     long long launches = 0;             // kernels launched through this context (bench: gpu_launches)

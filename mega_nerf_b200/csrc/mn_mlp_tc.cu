@@ -1,17 +1,17 @@
-// MN_PREC_TC_F16 / MN_PREC_TC_F16X3: the NeRF MLP (models/nerf.py:115-160) on the 5th-gen tensor cores.
+// MN_PREC_TC_F16 / MN_PREC_TC_F16X3: the NeRF MLP (models/nerf.py:115-160) on the Hopper tensor cores.
 //
 //   tc_encode_kernel   sample rows -> fp16 feature tiles (positional encodings of xyz / dir, appearance
 //                      embedding) written in the exact shared-memory operand image, one 128-row tile
 //                      per CTA, coalesced 16-byte stores.
-//   tc_mlp_kernel      persistent, warp-specialised: warp 0 = TMA producer (cp.async.bulk of weight
-//                      K-slabs through an mbarrier ring and of the feature tiles), warp 1 = single-thread
-//                      tcgen05.mma issuer (accumulators in TMEM), warps 2-5 = epilogue (tcgen05.ld ->
-//                      bias/ReLU -> fp16 -> next layer's A operand in shared memory; heads -> HBM).
+//   tc_mlp_wg_kernel   persistent, warp-specialised (mn_mlp_wg.cuh): one producer thread (cp.async.bulk of
+//                      weight K-slabs through an mbarrier ring and of the feature tiles), two consumer
+//                      warpgroups issuing wgmma.mma_async (accumulators in registers) and running the
+//                      epilogue (bias/ReLU -> fp16 -> next layer's A operand in shared memory; heads -> HBM).
 //                      Activations never leave the SM between layers.
 //
 // Operand layout (both A tiles and packed weights): K-major, no swizzle, "interleaved" core matrices:
 //   element (row r, col k) of an R-row operand lives at byte (k/8)*(R*16) + r*16 + (k%8)*2,
-// i.e. [K/8][R][8] fp16.  UMMA descriptor: LBO = R*16 (next 8-column chunk), SBO = 128 (next 8-row group).
+// i.e. [K/8][R][8] fp16.  wgmma descriptor: LBO = R*16 (next 8-column chunk), SBO = 128 (next 8-row group).
 // The epilogue's per-row 16-byte stores and the packer's images are contiguous in this layout, any K that
 // is a multiple of 16 works, and no TMA tensor map is needed (plain 1-D bulk copies).
 #include <cuda_fp16.h>
@@ -27,19 +27,9 @@ namespace {
 
 constexpr int kTileM = 128;
 
-// Optional in-kernel timeline (MN_TC_TRACE=1): CTA 0 records (event, tile-slot, gemm, clock) tuples.
+// In-kernel event buffer read by mn_debug_read_trace (the current MLP kernel records no events into it).
 __device__ unsigned long long g_trace[4 * 4096];
 __device__ unsigned int g_trace_n[2];
-__device__ __forceinline__ void trace_ev(int on, int who, int ev, int sl, int gi) {
-    if (!(on & 1) || blockIdx.x != 0) return;
-    const unsigned int i = atomicAdd(&g_trace_n[who], 1u);
-    if (i < 2048) {
-        unsigned long long t;
-        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-        g_trace[(who * 2048 + i) * 2 + 0] = ((unsigned long long)ev << 32) | ((unsigned long long)sl << 16) | (unsigned long long)gi;
-        g_trace[(who * 2048 + i) * 2 + 1] = t;
-    }
-}
 // SM clock during the kernel (MN_TC_TRACE=1): thread 0 of CTA 0 stamps (clock64, globaltimer) at kernel start and end.
 __device__ unsigned long long g_clk[4];
 __device__ __forceinline__ void clk_stamp(int on, int which) {
@@ -49,24 +39,13 @@ __device__ __forceinline__ void clk_stamp(int on, int which) {
     g_clk[2 * which] = (unsigned long long)clock64();
     g_clk[2 * which + 1] = t;
 }
-constexpr int kMaxStages = 4;
-// weight ring geometry: single pass = 3 stages x 64 K-columns (32 KiB); split mode (H holds hi+lo planes) = 4 x 32 columns
-__host__ __device__ constexpr int ring_slab_cols(bool split) { return split ? 32 : 64; }
-__host__ __device__ constexpr int ring_stage_bytes(bool split) { return ring_slab_cols(split) * 256 * 2; }
 constexpr int kMaxGemm = 16;
-constexpr int kThreads = 576;   // producer warp, MMA warp, 16 epilogue warps
-constexpr int kEpiWarps = 16;
-// Warps 0..15 = epilogue (TMEM lane quarter = warp % 4), 16 = TMA producer, 17 = MMA issuer.  The scheduler favours the
-// highest warp id on an SM sub-partition, so the latency-critical single-thread roles get the top ids.
-constexpr int kWarpProd = 16;
-constexpr int kWarpMma = 17;
-constexpr int kPPThreads = kThreads;
 
 enum { SRC_H = 0, SRC_XPE = 1, SRC_XAUX = 2 };
 enum { EPI_RELU = 0, EPI_RELU_SIGMA = 1, EPI_LINEAR = 2, EPI_RGB = 3,
        // data-gradient chain (training, mn_train_tc.cuh): plain copy, ReLU mask from the activation tape, mask + sigma-head term
        EPI_D_LINEAR = 4, EPI_D_MASK = 5, EPI_D_MASK_SIGMA = 6 };
-// kernel modes of tc_mlp_pp_kernel
+// kernel modes of tc_mlp_wg_kernel
 enum { PP_INFER = 0, PP_TRAIN_FWD = 1, PP_DGRAD = 2 };
 
 struct TcGemm {
@@ -164,15 +143,13 @@ __device__ __forceinline__ bool mbar_try(uint64_t* bar, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Bounded wait: a protocol bug becomes a trap (launch failure) instead of a hung GPU.
+// Bounded wait: a protocol bug becomes a trap (launch failure) instead of a hung GPU.  No printf here: a function call
+// between an asynchronous warpgroup MMA and its wait makes the compiler serialise every wgmma.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     if (mbar_try(bar, parity)) return;
     const long long t0 = clock64();
     while (!mbar_try(bar, parity)) {
-        if (clock64() - t0 > 4000000000ll) {
-            printf("mn_mlp_tc: mbarrier timeout block %d thread %d\n", (int)blockIdx.x, (int)threadIdx.x);
-            __trap();
-        }
+        if (clock64() - t0 > 4000000000ll) __trap();
     }
 }
 __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, uint32_t bytes, uint64_t* bar) {
@@ -182,125 +159,12 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                  : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-           (1ull << 46);
-}
-__device__ __forceinline__ uint32_t make_idesc(int n) {
-    // kind::f16: D=f32 (bit 4), A=B=f16 (0), K-major A and B, N>>3 at [17,23), M>>4 at [24,29)
-    return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred;
-    asm volatile(
-        "{\n\t.reg .pred P;\n\t"
-        "elect.sync _|P, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, P;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
 
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
     const __half2 h = __floats2half2_rn(a, b);
     return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// One 16-column piece of the epilogue for one accumulator row: TMEM -> +bias -> (ReLU) -> fp16 (hi [, lo]) ->
-// two 16-byte stores into the next layer's A operand.  Returns the partial sigma dot product if kSigma.
-template <bool kSplit, bool kRelu, bool kSigma>
-__device__ __forceinline__ float epi_piece16(uint32_t taddr, const float* __restrict__ bias16, const float* __restrict__ sw16,
-                                             unsigned char* dst, size_t lo_off, bool store, unsigned char* gdst = nullptr) {
-    uint32_t v[16];
-    tmem_ld16(taddr, v);
-    const float4* b4 = reinterpret_cast<const float4*>(bias16);
-    const float4 b0 = b4[0], b1 = b4[1], b2 = b4[2], b3 = b4[3];
-    const float b[16] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w, b2.x, b2.y, b2.z, b2.w, b3.x, b3.y, b3.z, b3.w};
-    tmem_ld_wait();
-    float f[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[i]) + b[i];
-    float sacc = 0.0f;
-    if (kSigma || kSplit) {
-        if (kRelu) {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) f[i] = fmaxf(f[i], 0.0f);
-        }
-    }
-    if (kSigma) {
-        const float4* s4 = reinterpret_cast<const float4*>(sw16);
-        const float4 s0 = s4[0], s1 = s4[1], s2 = s4[2], s3 = s4[3];
-        const float sw[16] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w, s2.x, s2.y, s2.z, s2.w, s3.x, s3.y, s3.z, s3.w};
-#pragma unroll
-        for (int i = 0; i < 16; ++i) sacc = fmaf(f[i], sw[i], sacc);
-    }
-    if (store) {
-        uint32_t hi[8];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) hi[e] = pack_h2(f[2 * e], f[2 * e + 1]);
-        if (kRelu && !(kSigma || kSplit)) {
-            // ReLU after the fp16 rounding (max(round(x),0) == round(max(x,0))): one HMNMX2 per pair
-            const __half2 z = __float2half2_rn(0.0f);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                __half2 h = __hmax2(*reinterpret_cast<__half2*>(&hi[e]), z);
-                hi[e] = *reinterpret_cast<const uint32_t*>(&h);
-            }
-        }
-        *reinterpret_cast<uint4*>(dst) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        *reinterpret_cast<uint4*>(dst + kTileM * 16) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-        if (gdst) {     // training forward: the same two 16-byte pieces go to the activation tape (same image layout)
-            *reinterpret_cast<uint4*>(gdst) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            *reinterpret_cast<uint4*>(gdst + kTileM * 16) = make_uint4(hi[4], hi[5], hi[6], hi[7]);
-        }
-        if (kSplit) {
-            uint32_t lo[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const float2 back = __half22float2(*reinterpret_cast<const __half2*>(&hi[e]));
-                lo[e] = pack_h2(f[2 * e] - back.x, f[2 * e + 1] - back.y);
-            }
-            *reinterpret_cast<uint4*>(dst + lo_off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-            *reinterpret_cast<uint4*>(dst + lo_off + kTileM * 16) = make_uint4(lo[4], lo[5], lo[6], lo[7]);
-        }
-    }
-    return sacc;
-}
 
 // rgb head epilogue shared by the tensor-core kernels (nerf.py:152-160): bias, optional per-image affine appearance
 // transform (3x4 matrix = affine(embedding_a[idx]), nerf.py:156-158), sigmoid when rgb_dim == 3, blend weight.
@@ -535,107 +399,6 @@ __global__ void __launch_bounds__(kTileM) tc_encode_fast_kernel(const MlpArgs a,
     }
 }
 
-// ---- lean primitives for the MMA-issuing warp (raw shared-memory addresses, no per-slab descriptor rebuild) ----
-__device__ __forceinline__ void mbar_wait_a(uint32_t bar_addr, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(bar_addr), "r"(parity) : "memory");
-    if (ok) return;
-    const long long t0 = clock64();
-    while (true) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok) : "r"(bar_addr), "r"(parity) : "memory");
-        if (ok) return;
-        if (clock64() - t0 > 4000000000ll) {
-            printf("mn_mlp_tc: mbarrier timeout (mma) block %d\n", (int)blockIdx.x);
-            __trap();
-        }
-    }
-}
-// Non-blocking look-ahead probe (mbarrier.test_wait): issued BEFORE the current stage's work so that its ~100-cycle latency
-// overlaps that work instead of heading the next stage's dependent chain.  A single thread pays ~260 cycles per ring stage
-// for wait -> issue -> signal when these are strictly sequential (scripts/probes/l2_stream_probe.cu: throughput of a
-// one-thread TMA ring is proportional to the stage size and independent of its depth) - as long as two 128-cycle MMAs.
-__device__ __forceinline__ uint32_t mbar_test_a(uint32_t bar_addr, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(bar_addr), "r"(parity) : "memory");
-    return ok;
-}
-// one ring stage worth of MMAs (one or two K=16 steps) + the commit that releases the stage, issued by one
-// elected lane; everything is predicated, no branches.
-__device__ __forceinline__ void mma_stage(uint32_t d_tmem, uint64_t ad, uint64_t bd, uint64_t ad2, uint64_t bd2, uint32_t idesc,
-                                          uint32_t accum, uint32_t two, uint32_t empty_bar_addr) {
-    asm volatile(
-        "{\n\t.reg .pred e, p, q;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "setp.ne.and.b32 q, %7, 0, e;\n\t"
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %5, p;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], %3, %4, %5, 1;\n\t"
-        "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%8];\n\t}"
-        ::"r"(d_tmem), "l"(ad), "l"(bd), "l"(ad2), "l"(bd2), "r"(idesc), "r"(accum), "r"(two), "r"(empty_bar_addr)
-        : "memory");
-}
-// Two consecutive ring stages of one GEMM in one issue block: up to four K=16 MMAs (A contiguous in the activation buffer,
-// B in stage a then stage b), each stage released by its own commit.  n_b = MMAs of the second stage (1 or 2).
-__device__ __forceinline__ void mma_stage2(uint32_t d_tmem, uint64_t ad, uint64_t a_step, uint64_t bda, uint64_t bdb, uint64_t b_step,
-                                           uint32_t idesc, uint32_t accum, uint32_t n_b, uint32_t empty_a, uint32_t empty_b) {
-    asm volatile(
-        "{\n\t.reg .pred e, p, q;\n\t.reg .b64 a1, a2, a3, b1, b3;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %7, 0;\n\t"
-        "setp.gt.and.u32 q, %8, 1, e;\n\t"
-        "add.u64 a1, %1, %2;\n\tadd.u64 a2, a1, %2;\n\tadd.u64 a3, a2, %2;\n\t"
-        "add.u64 b1, %3, %5;\n\tadd.u64 b3, %4, %5;\n\t"
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %3, %6, p;\n\t"
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%0], a1, b1, %6, 1;\n\t"
-        "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%9];\n\t"
-        "@e tcgen05.mma.cta_group::1.kind::f16 [%0], a2, %4, %6, 1;\n\t"
-        "@q tcgen05.mma.cta_group::1.kind::f16 [%0], a3, b3, %6, 1;\n\t"
-        "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%10];\n\t}"
-        ::"r"(d_tmem), "l"(ad), "l"(a_step), "l"(bda), "l"(bdb), "l"(b_step), "r"(idesc), "r"(accum), "r"(n_b), "r"(empty_a), "r"(empty_b)
-        : "memory");
-}
-__device__ __forceinline__ void commit_elect(uint32_t bar_addr) {
-    asm volatile(
-        "{\n\t.reg .pred e;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t}"
-        ::"r"(bar_addr) : "memory");
-}
-
-
-// up to four K=16 steps against one ring stage (A from shared memory: descriptor + a_step per step); one elected lane issues,
-// then releases the stage.
-__device__ __forceinline__ void ts_stage_smem(uint32_t d_tmem, uint64_t ad, uint64_t a_step, uint64_t bd, uint64_t b_step,
-                                              uint32_t idesc, uint32_t accum, int nk, uint32_t empty_bar) {
-    asm volatile(
-        "{\n\t.reg .pred e, p, q1, q2, q3;\n\t.reg .b64 a1, a2, a3, b1, b2, b3;\n\t"
-        "elect.sync _|e, 0xffffffff;\n\t"
-        "setp.ne.b32 p, %6, 0;\n\t"
-        "setp.gt.and.s32 q1, %7, 1, e;\n\t"
-        "setp.gt.and.s32 q2, %7, 2, e;\n\t"
-        "setp.gt.and.s32 q3, %7, 3, e;\n\t"
-        "add.u64 a1, %1, %2;\n\tadd.u64 a2, a1, %2;\n\tadd.u64 a3, a2, %2;\n\t"
-        "add.u64 b1, %3, %4;\n\tadd.u64 b2, b1, %4;\n\tadd.u64 b3, b2, %4;\n\t"
-        "@e  tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %3, %5, p;\n\t"
-        "@q1 tcgen05.mma.cta_group::1.kind::f16 [%0], a1, b1, %5, 1;\n\t"
-        "@q2 tcgen05.mma.cta_group::1.kind::f16 [%0], a2, b2, %5, 1;\n\t"
-        "@q3 tcgen05.mma.cta_group::1.kind::f16 [%0], a3, b3, %5, 1;\n\t"
-        "@e  tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%8];\n\t}"
-        ::"r"(d_tmem), "l"(ad), "l"(a_step), "l"(bd), "l"(b_step), "r"(idesc), "r"(accum), "r"(nk), "r"(empty_bar)
-        : "memory");
-}
 
 
 // ------------------------------------------------------------------------------------------------
@@ -661,799 +424,23 @@ struct TcArgs {
     const float* scale;           // PP_DGRAD: device scalar S (power of two): gradient images hold S * dZ
     int64_t act_tile_bytes;       // bytes of one tile's record in tape_act / tape_dz
     int layers;
-    // ---- TMEM ping-pong kernel (mn_mlp_tp.cuh): half-major weight images and the two role tables
-    const unsigned char* tpack;
-    size_t tp_sub_bytes;
-    const uint4* tp_prog;
-    int tp_n[4];
-};
-
-struct SmemLayout {
-    // byte offsets inside dynamic shared memory
-    int ring, h, xa, f32, sigp, bars, total, stages;
 };
 
 constexpr int kSmemMax = 227 * 1024;
 
-__host__ __device__ inline SmemLayout smem_layout(const TcPlan& p, bool split) {
-    SmemLayout s;
-    const int kx = p.kpe > p.kaux ? p.kpe : p.kaux;
-    const int fixed = p.L * kTileM * 2 * (split ? 2 : 1) + kx * kTileM * 2 + ((p.f32_floats * 4 + 15) / 16) * 16 + 2048 + 256;
-    int st = (kSmemMax - fixed) / ring_stage_bytes(split);
-    if (st > kMaxStages) st = kMaxStages;
-    s.stages = st;
-    s.ring = 0;
-    s.h = s.ring + st * ring_stage_bytes(split);
-    s.xa = s.h + p.L * kTileM * 2 * (split ? 2 : 1);   // split: hi plane then lo plane
-    s.f32 = s.xa + kx * kTileM * 2;
-    s.sigp = s.f32 + ((p.f32_floats * 4 + 15) / 16) * 16;
-    s.bars = s.sigp + 2048;
-    s.total = s.bars + 256;
-    return s;
+#include "mn_mlp_wg.cuh"
+
+template <int kMode, bool kSplit, bool kWide>
+int wg_launch(mn_ctx* ctx, const TcArgs& A, int64_t n_tiles128, cudaStream_t st) {
+    const WgLayout WL = wg_layout(A.plan, kSplit);
+    if (WL.total > kSmemMax || WL.stages < 2) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: shared-memory budget exceeded");
+    MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_wg_kernel<kMode, kSplit, kWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, WL.total));
+    const unsigned grid = (unsigned)(n_tiles128 < ctx->sm_count ? n_tiles128 : ctx->sm_count);
+    tc_mlp_wg_kernel<kMode, kSplit, kWide><<<grid, kWgmmaThreads, WL.total, st>>>(A);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
 }
 
-// Warp roles: 0 = TMA producer, 1 = MMA issuer, 2..9 = epilogue.  Epilogue warp w owns TMEM lanes
-// 32*(w%4).. (hardware rule) and, within every 64-column slab of the accumulator, the 32-column half
-// (w-2)/4; a slab of the next layer's A operand is published (mbarrier hready[slab]) as soon as all eight
-// warps have written their part, so the next layer's MMAs trail the epilogue slab by slab while the
-// other accumulator buffer is still being drained.
-template <bool kSplit>
-__global__ void __launch_bounds__(kThreads, 1) tc_mlp_kernel(const TcArgs A) {
-    constexpr int kSlabCols = ring_slab_cols(kSplit);
-    constexpr int kStageBytes = ring_stage_bytes(kSplit);
-    extern __shared__ __align__(1024) unsigned char smem[];
-    const TcPlan& P = A.plan;
-    const SmemLayout SL = smem_layout(P, kSplit);
-    const int kStages = SL.stages;
-    unsigned char* ring = smem + SL.ring;
-    unsigned char* Hs = smem + SL.h;
-    unsigned char* XA = smem + SL.xa;
-    float* F32 = reinterpret_cast<float*>(smem + SL.f32);
-    float* SIGP = reinterpret_cast<float*>(smem + SL.sigp);   // [4][128] partial sigma dot products
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SL.bars);
-    uint64_t* full = bars;                  // [kMaxStages]
-    uint64_t* empty = bars + kMaxStages;    // [kMaxStages]
-    uint64_t* xa_full = bars + 2 * kMaxStages;
-    uint64_t* xa_empty = xa_full + 1;
-    uint64_t* acc_full = xa_full + 2;       // [2]
-    uint64_t* hready = xa_full + 4;         // [4]
-    uint64_t* f32_full = xa_full + 8;
-    uint64_t* f32_empty = xa_full + 9;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(xa_full + 10);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t n_slots = A.m.counters ? A.m.counters[CNT_NSLOTS] : A.m.B;
-    const int64_t n_tiles = (n_slots + kTileM - 1) / kTileM;
-    const int n_gemm = A.m.sigma_only ? P.n_trunk : P.n_gemm;
-
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        mbar_init(xa_full, 1);
-        mbar_init(xa_empty, 1);
-        mbar_init(&acc_full[0], 1);
-        mbar_init(&acc_full[1], 1);
-        for (int i = 0; i < 4; ++i) mbar_init(&hready[i], kEpiWarps);
-        mbar_init(f32_full, 1);
-        mbar_init(f32_empty, kEpiWarps);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == kWarpProd) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    auto sub_of = [&](int64_t tile) -> int {
-        int sub = A.m.fixed_sub;
-        if (A.m.counters) {
-            sub = 0;
-            const int64_t s0 = tile * kTileM;
-            while (sub + 1 < A.m.n_sub && s0 >= A.m.counters[CNT_START + sub + 1]) ++sub;
-        }
-        return sub;
-    };
-    constexpr int npass = kSplit ? 3 : 1;
-
-    if (warp == kWarpProd) {
-        // =========================== TMA producer ===========================
-        if (lane == 0) {
-            int stage = 0;
-            uint32_t phase = 0, xphase = 0, fphase = 0;
-            const uint32_t f32_bytes = (uint32_t)(((P.f32_floats * 4 + 15) / 16) * 16);
-            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const int sub = sub_of(tile);
-                const unsigned char* wsub = A.wpack + (size_t)sub * P.sub_bytes;
-                const size_t f32_off = (size_t)P.plane_bytes * 2;   // both planes are always packed
-                // biases + sigma weights of this tile's sub-module
-                mbar_wait(f32_empty, fphase ^ 1);
-                mbar_expect_tx(f32_full, f32_bytes);
-                bulk_g2s(F32, wsub + f32_off, f32_bytes, f32_full);
-                fphase ^= 1;
-                for (int gi = 0; gi < n_gemm; ++gi) {
-                    const TcGemm& g = P.g[gi];
-                    for (int pass = 0; pass < npass; ++pass) {
-                        // pass 0: A_hi * W_hi, pass 1: A_hi * W_lo, pass 2: A_lo * W_hi
-                        const unsigned char* wimg = wsub + (pass == 1 ? (size_t)P.plane_bytes : 0) + g.w_off;
-                        int kbase = 0;
-                        for (int sgi = 0; sgi < g.nseg; ++sgi) {
-                            const int kseg = g.k[sgi];
-                            if (g.src[sgi] != SRC_H) {
-                                const __half* xt = A.ximg + (pass == 2 ? A.x_plane_halves : 0) +
-                                                   tile * (int64_t)(P.kpe + P.kaux) * kTileM +
-                                                   (g.src[sgi] == SRC_XAUX ? (int64_t)P.kpe * kTileM : 0);
-                                mbar_wait(xa_empty, xphase ^ 1);
-                                mbar_expect_tx(xa_full, (uint32_t)(kseg * kTileM * 2));
-                                bulk_g2s(XA, xt, (uint32_t)(kseg * kTileM * 2), xa_full);
-                                xphase ^= 1;
-                            }
-                            for (int k0 = 0; k0 < kseg; k0 += kSlabCols) {
-                                const int kc = min(kSlabCols, kseg - k0);
-                                const uint32_t bytes = (uint32_t)(kc * g.n * 2);
-                                mbar_wait(&empty[stage], phase ^ 1);
-                                mbar_expect_tx(&full[stage], bytes);
-                                bulk_g2s(ring + (size_t)stage * kStageBytes, wimg + (size_t)(kbase + k0) * g.n * 2, bytes,
-                                         &full[stage]);
-                                if (++stage == kStages) { stage = 0; phase ^= 1; }
-                            }
-                            kbase += kseg;
-                        }
-                    }
-                }
-            }
-        }
-    } else if (warp == kWarpMma) {
-        // =========================== MMA issuer ===========================
-        // The whole warp runs the loop (so addresses/descriptors stay in uniform registers); one elected lane
-        // issues tcgen05.mma / tcgen05.commit.
-        {
-            int stage = 0;
-            uint32_t phase = 0, xphase = 0, gidx = 0;
-            uint32_t hph0 = 0, hph1 = 0, hph2 = 0, hph3 = 0;
-            const uint32_t h_base = smem_u32(Hs), xa_base = smem_u32(XA), ring_base = smem_u32(ring);
-            const uint64_t a_step = (uint64_t)((2 * kTileM * 16) >> 4);           // +16 K-columns of A (descriptor address field)
-            for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                for (int gi = 0; gi < n_gemm; ++gi, ++gidx) {
-                    const TcGemm& g = P.g[gi];
-                    const uint32_t idesc = make_idesc(g.n);
-                    const uint32_t d_tmem = tmem_base + (gidx & 1u) * 256u;
-                    const uint64_t b_step = (uint64_t)((2 * g.n * 16) >> 4);      // +16 K-columns of B
-                    uint32_t accum = 0;
-                    for (int pass = 0; pass < npass; ++pass) {
-                        for (int sgi = 0; sgi < g.nseg; ++sgi) {
-                            const int kseg = g.k[sgi];
-                            const bool from_x = g.src[sgi] != SRC_H;
-                            // lo plane of H lives right after the hi plane in the H buffer (split mode)
-                            const uint32_t a_base = from_x ? xa_base : h_base + (pass == 2 ? (uint32_t)(P.L * kTileM * 2) : 0u);
-                            if (from_x) {
-                                mbar_wait(xa_full, xphase);
-                                xphase ^= 1;
-                            }
-                            for (int k0 = 0; k0 < kseg; k0 += kSlabCols) {
-                                const int kc = min(kSlabCols, kseg - k0);
-                                if (!from_x && pass == 0 && (k0 & 63) == 0) {
-                                    // the previous GEMM's epilogue has published this 64-column slab of H
-                                    const int hs = k0 >> 6;
-                                    if (hs == 0) { mbar_wait(&hready[0], hph0); hph0 ^= 1; }
-                                    else if (hs == 1) { mbar_wait(&hready[1], hph1); hph1 ^= 1; }
-                                    else if (hs == 2) { mbar_wait(&hready[2], hph2); hph2 ^= 1; }
-                                    else { mbar_wait(&hready[3], hph3); hph3 ^= 1; }
-                                }
-                                mbar_wait(&full[stage], phase);
-                                tc_fence_after();
-                                uint64_t ad = make_desc(a_base + (uint32_t)(k0 / 8) * (kTileM * 16), kTileM * 16, 128);
-                                uint64_t bd = make_desc(ring_base + (uint32_t)stage * kStageBytes, (uint32_t)g.n * 16, 128);
-                                // up to four MMAs and the commit that frees the ring stage, one predicated straight-line block
-                                ts_stage_smem(d_tmem, ad, a_step, bd, b_step, idesc, accum, kc >> 4, smem_u32(&empty[stage]));
-                                accum = 1;
-                                if (++stage == kStages) { stage = 0; phase ^= 1; }
-                            }
-                            if (from_x && elect_one()) tc_commit(xa_empty);
-                            __syncwarp();
-                        }
-                    }
-                    if (elect_one()) tc_commit(&acc_full[gidx & 1u]);
-                    __syncwarp();
-                }
-            }
-        }
-    } else {
-        // =========================== epilogue (16 warps) ===========================
-        const int q = warp & 3;                      // TMEM lane quarter this warp may access
-        const int part = warp >> 2;            // which 16-column piece of every 64-column slab
-        const int r = q * 32 + lane;                 // row of the tile == TMEM lane
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-        uint32_t acc_phase0 = 0, acc_phase1 = 0, fphase = 0, gidx = 0;
-        const int L = P.L;
-        const size_t lo_off = (size_t)L * kTileM * 2;
-        for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const int64_t slot = tile * kTileM + r;
-            int64_t row = -1;
-            if (slot < n_slots) row = A.m.slot_row ? (int64_t)A.m.slot_row[slot] : slot;
-            mbar_wait(f32_full, fphase);
-            fphase ^= 1;
-            float sigma = 0.0f;
-            for (int gi = 0; gi < n_gemm; ++gi, ++gidx) {
-                const TcGemm& g = P.g[gi];
-                const uint32_t ab = gidx & 1u;
-                if (ab) { mbar_wait(&acc_full[1], acc_phase1); acc_phase1 ^= 1; }
-                else    { mbar_wait(&acc_full[0], acc_phase0); acc_phase0 ^= 1; }
-                tc_fence_after();
-                const uint32_t t_acc = t_lane + ab * 256u;
-                const float* bias = F32 + g.bias_off;
-                if (g.epi == EPI_RGB) {
-                    if (part == 0) {
-                        uint32_t v[32];
-                        tmem_ld32(t_acc, v);
-                        tmem_ld_wait();
-                        if (row >= 0) tc_emit_rgb(A.m, A.m.nd.affine ? sub_of(tile) : 0, row, slot, v, bias, sigma);
-                    }
-                    tc_fence_before();
-                } else {
-                    const bool want_sigma = g.epi == EPI_RELU_SIGMA;
-                    const bool publish = !(want_sigma && A.m.sigma_only);   // nobody reads H after the last trunk layer
-                    const float* sw = F32 + P.sigma_w_off;
-                    float sacc = 0.0f;
-                    const int nslab = (g.n + 63) >> 6;
-                    for (int j = 0; j < nslab; ++j) {
-                        const int c0 = 64 * j + 16 * part;
-                        if (c0 < g.n) {
-                            unsigned char* dst = Hs + (size_t)(c0 >> 3) * (kTileM * 16) + (size_t)r * 16;
-                            if (g.epi == EPI_RELU)
-                                epi_piece16<kSplit, true, false>(t_acc + (uint32_t)c0, bias + c0, sw + c0, dst, lo_off, true);
-                            else if (g.epi == EPI_LINEAR)
-                                epi_piece16<kSplit, false, false>(t_acc + (uint32_t)c0, bias + c0, sw + c0, dst, lo_off, true);
-                            else
-                                sacc += epi_piece16<kSplit, true, true>(t_acc + (uint32_t)c0, bias + c0, sw + c0, dst, lo_off, publish);
-                            if (publish) fence_proxy_async();   // generic-proxy stores to H -> visible to the tensor core
-                        }
-                        if (publish) {
-                            tc_fence_before();
-                            __syncwarp();
-                            if (lane == 0) mbar_arrive(&hready[j]);
-                        }
-                    }
-                    if (want_sigma) {
-                        SIGP[part * kTileM + r] = sacc;
-                        asm volatile("bar.sync 1, 512;" ::: "memory");
-                        if (part == 0) {
-                            // sigma bias is stored right after sigma_w
-                            float s = ((SIGP[r] + SIGP[kTileM + r]) + (SIGP[2 * kTileM + r] + SIGP[3 * kTileM + r])) + sw[L];
-                            if (A.m.sigma_noise && row >= 0) s = s + A.m.sigma_noise[row];
-                            sigma = A.m.nd.softplus ? mn_softplus_shifted(s) : fmaxf(s, 0.0f);
-                            if (A.m.sigma_only && row >= 0) {
-                                const int64_t o = (A.m.scatter ? row : slot) * A.m.out_cols;
-                                A.m.out[o] = A.m.slot_w ? sigma * A.m.slot_w[slot] : sigma;
-                            }
-                        }
-                        tc_fence_before();
-                    }
-                }
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(f32_empty);
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == kWarpProd) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-    }
-}
-
-
-
-// ------------------------------------------------------------------------------------------------
-// Ping-pong variant (single-pass fp16): two 128-row tiles per CTA, each with its own activation buffer
-// and TMEM accumulator.  GEMMs are issued X_l, Y_l, X_l+1, Y_l+1, ...: the epilogue of X_l (16 warps)
-// runs entirely under the MMAs of Y_l and vice versa, so the tensor pipe only idles at pipeline fill.
-// ------------------------------------------------------------------------------------------------
-// A ring stage (16 KiB) carries either 32 K-columns of weights (activation segment: A operand = the tile's H buffer,
-// two K=16 MMAs) or, for the feature segments (PE / direction+appearance tiles), 16 K-columns of weights (<= 8 KiB) PLUS
-// the matching 16 K-columns x 128 rows of the tile's feature image (4 KiB at +8 KiB, one MMA): the features travel in
-// the same stream as the weights, so there is no separate feature buffer and no producer stall waiting for it.
-constexpr int kPPMaxStages = 8;
-constexpr int kPPSlabCols = 32;
-constexpr int kPPStageBytes = kPPSlabCols * 256 * 2;
-constexpr int kPPXCols = 16;
-constexpr int kPPXOff = 8192;
-
-struct PPLayout {
-    int ring, h, f32, f32_stride, sigp, bars, prog, total, stages;
-};
-// Stage program of the ping-pong kernel: ONE 16-byte entry per ring stage of a tile pair, shared by the TMA producer and the
-// MMA issuer, so that both single-thread roles run a flat loop (no nested GEMM / segment / K loops, no address arithmetic
-// beyond one add): their per-stage dependent chain is what paces the kernel (see the probe notes at mbar_test_a).
-//   x = weight byte offset inside the sub-module image   y = weight bytes | (feature offset / 16, 0xFFFF = none) << 16
-//   z = flags | MMA N << 8                               w = activation-operand offset >> 4 (descriptor units)
-constexpr int kPPMaxProg = 208;
-enum { PF_SLOT1 = 1, PF_FIRST = 2, PF_LAST = 4, PF_FROM_X = 8, PF_TWO = 16, PF_PAIR = 32 };   // PF_PAIR: this and the next entry are consecutive activation stages of one GEMM - the MMA warp issues them together
-
-__host__ __device__ inline PPLayout pp_layout(const TcPlan& p) {
-    PPLayout s;
-    s.f32_stride = ((p.f32_floats * 4 + 15) / 16) * 16;
-    const int fixed = 2 * p.L * kTileM * 2 + s.f32_stride + 2048 + 256 + kPPMaxProg * 16;
-    int kPPStages = (kSmemMax - fixed) / kPPStageBytes;
-    if (kPPStages > kPPMaxStages) kPPStages = kPPMaxStages;
-    s.stages = kPPStages;
-    s.ring = 0;
-    s.h = kPPStages * kPPStageBytes;
-    s.f32 = s.h + 2 * p.L * kTileM * 2;
-    s.sigp = s.f32 + s.f32_stride;    // ONE fp32 block: both tiles of a pair belong to the same sub-module
-    s.bars = s.sigp + 2048;
-    s.prog = s.bars + 256;
-    s.total = s.prog + kPPMaxProg * 16;
-    return s;
-}
-
-__host__ __device__ inline int pp_gemm_stages(const TcGemm& g) {
-    int n = 0;
-    for (int sgi = 0; sgi < g.nseg; ++sgi)
-        n += g.src[sgi] != SRC_H ? (g.k[sgi] + kPPXCols - 1) / kPPXCols : (g.k[sgi] + kPPSlabCols - 1) / kPPSlabCols;
-    return n;
-}
-__host__ __device__ inline int pp_prog_entries(const TcPlan& p, int n_gemm) {
-    int n = 0;
-    for (int gi = 0; gi < n_gemm; ++gi) n += 2 * pp_gemm_stages(p.g[gi]);
-    return n;
-}
-
-// Ping-pong kernel (see the header of this section).  Warps 0..15 epilogue, 16 TMA producer, 17 MMA issuer.
-template <int kMode>
-__global__ void __launch_bounds__(kPPThreads, 1) tc_mlp_pp_kernel(const TcArgs A) {
-    extern __shared__ __align__(1024) unsigned char smem[];
-    const TcPlan& P = A.plan;
-    const PPLayout SL = pp_layout(P);
-    const int kPPStages = SL.stages;
-    unsigned char* ring = smem + SL.ring;
-    unsigned char* Hs = smem + SL.h;
-    float* F32 = reinterpret_cast<float*>(smem + SL.f32);
-    float* SIGP = reinterpret_cast<float*>(smem + SL.sigp);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + SL.bars);
-    uint64_t* full = bars;            // [<=8]
-    uint64_t* empty = bars + 8;       // [<=8]
-    uint64_t* acc_full = bars + 16;   // [2] per tile slot
-    uint64_t* epi_done = bars + 18;   // [2]
-    uint64_t* f32_full = bars + 20;   // [2]
-    uint64_t* f32_empty = bars + 22;  // [2]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 24);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t n_slots = A.m.counters ? A.m.counters[CNT_NSLOTS] : A.m.B;
-    const int64_t n_tiles = (n_slots + kTileM - 1) / kTileM;
-    const int n_gemm = A.m.sigma_only ? P.n_trunk : P.n_gemm;
-    const int h_bytes = P.L * kTileM * 2;
-    const float* SW = F32 + P.sigma_w_off;
-    const float* RGBB = F32 + P.g[P.n_gemm - 1].bias_off;
-
-    // ---- stage program (see kPPMaxProg): entries in the order both roles walk a tile pair: GEMM, slot, segment, K
-    uint4* PROG = reinterpret_cast<uint4*>(smem + SL.prog);
-    auto stages_of = [&](const TcGemm& g) -> int { return pp_gemm_stages(g); };
-    const int n_prog = pp_prog_entries(P, n_gemm);       // <= kPPMaxProg: checked by the launcher
-    if (threadIdx.x >= 64 && threadIdx.x < 66) PROG[n_prog + (threadIdx.x - 64)] = make_uint4(0u, 0u, 0u, 0u);   // read-ahead padding
-    if ((int)threadIdx.x < 2 * n_gemm) {
-        const int gi = threadIdx.x >> 1, sl = threadIdx.x & 1;
-        const TcGemm& g = P.g[gi];
-        int e = 0;
-        for (int j = 0; j < gi; ++j) e += 2 * stages_of(P.g[j]);
-        const int total = stages_of(g);
-        e += sl * total;
-        int kbase = 0, cnt = 0;
-        for (int sgi = 0; sgi < g.nseg; ++sgi) {
-            const bool fx = g.src[sgi] != SRC_H;
-            const int kk = g.k[sgi];
-            const int step = fx ? kPPXCols : kPPSlabCols;
-            for (int k0 = 0; k0 < kk; k0 += step, ++cnt, ++e) {
-                const int kc = min(step, kk - k0);
-                const uint32_t xo = fx ? (uint32_t)(((g.src[sgi] == SRC_XAUX ? P.kpe * kTileM * 2 : 0) + k0 * kTileM * 2) >> 4) : 0xFFFFu;
-                const bool pair = !fx && ((k0 / kPPSlabCols) & 1) == 0 && k0 + kPPSlabCols < kk;      // even activation stage with a successor
-                const uint32_t fl = (sl ? PF_SLOT1 : 0) | (cnt == 0 ? PF_FIRST : 0) | (cnt == total - 1 ? PF_LAST : 0) | (fx ? PF_FROM_X : 0) |
-                                    ((!fx && kc == kPPSlabCols) ? PF_TWO : 0) | (pair ? PF_PAIR : 0);
-                PROG[e] = make_uint4((uint32_t)(g.w_off + (kbase + k0) * g.n * 2), (uint32_t)(kc * g.n * 2) | (xo << 16),
-                                     fl | ((uint32_t)g.n << 8), fx ? 0u : (uint32_t)(((k0 >> 3) * (kTileM * 16)) >> 4));
-            }
-            kbase += kk;
-        }
-    }
-    if (threadIdx.x == 0) {
-        for (int i = 0; i < kPPMaxStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&acc_full[i], 1);
-            mbar_init(&epi_done[i], kEpiWarps);
-            mbar_init(&f32_full[i], 1);
-            mbar_init(&f32_empty[i], kEpiWarps);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == kWarpProd) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    clk_stamp(A.desc_swap, 0);
-
-    auto sub_of = [&](int64_t tile) -> int {
-        int sub = A.m.fixed_sub;
-        if (A.m.counters) {
-            sub = 0;
-            const int64_t s0 = tile * kTileM;
-            while (sub + 1 < A.m.n_sub && s0 >= A.m.counters[CNT_START + sub + 1]) ++sub;
-        }
-        return sub;
-    };
-    // a CTA works on PAIRS of adjacent tiles (2p, 2p+1): buckets are 256-row aligned, so both belong to one sub-module
-    const int64_t n_pairs = (n_tiles + 1) / 2;
-
-    if (warp == kWarpProd) {
-        // =========================== TMA producer: table-driven (PROG) ===========================
-        // One thread.  Its per-stage dependent chain (wait -> expect_tx -> copy) is as long as the stage's two MMAs, so the
-        // loop is kept flat: one 16-byte table entry per ring stage, look-ahead probe of the next stage's empty barrier.
-        if (lane == 0) {
-            uint32_t stage = 0, phase = 0, fph_e = 0, ahead = 0;
-            int last_sub = -1;
-            const uint32_t f32_bytes = (uint32_t)SL.f32_stride;
-            const uint32_t empty_pa = smem_u32(empty), full_pa = smem_u32(full), ring_pa = smem_u32(ring);
-            const uint32_t nst = (uint32_t)kPPStages;
-            const int64_t xtile_bytes = (int64_t)(P.kpe + P.kaux) * kTileM * 2;
-            for (int64_t pr = blockIdx.x; pr < n_pairs; pr += gridDim.x) {
-                const int64_t t0 = 2 * pr;
-                const int sub0 = sub_of(t0);
-                const unsigned char* wsub = A.wpack + (size_t)sub0 * P.sub_bytes;
-                const unsigned char* xt0 = reinterpret_cast<const unsigned char*>(A.ximg) + t0 * xtile_bytes;
-                const bool valid1 = t0 + 1 < n_tiles;
-                if (sub0 != last_sub) {
-                    // the bias / sigma block is re-staged only when the sub-module changes (a handful of times per launch):
-                    // the weight stream of consecutive pairs is not interrupted by waiting for the epilogue
-                    if (last_sub >= 0) { mbar_wait(&f32_empty[0], fph_e); fph_e ^= 1; }
-                    const unsigned char* fsrc = wsub + (size_t)P.f32_off;
-                    mbar_expect_tx(&f32_full[0], f32_bytes);
-                    bulk_g2s(reinterpret_cast<unsigned char*>(F32), fsrc, f32_bytes, &f32_full[0]);
-                    last_sub = sub0;
-                }
-                for (int e = 0; e < n_prog; ++e) {
-                    const uint4 E = PROG[e];
-                    const bool slot1 = (E.z & PF_SLOT1) != 0;
-                    if (slot1 && !valid1) continue;
-                    const uint32_t cur = stage;
-                    if (!ahead) mbar_wait_a(empty_pa + 8u * cur, phase ^ 1);
-                    if (++stage == nst) { stage = 0; phase ^= 1; }
-                    ahead = mbar_test_a(empty_pa + 8u * stage, phase ^ 1);       // next stage: latency overlaps the copies below
-                    const uint32_t bar = full_pa + 8u * cur, dst = ring_pa + cur * (uint32_t)kPPStageBytes;
-                    const uint32_t wbytes = E.y & 0xFFFFu, xo = E.y >> 16;
-                    const bool has_x = xo != 0xFFFFu;
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(wbytes + (has_x ? (uint32_t)(kPPXCols * kTileM * 2) : 0u)) : "memory");
-                    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 ::"r"(dst), "l"(wsub + E.x), "r"(wbytes), "r"(bar) : "memory");
-                    if (has_x)
-                        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                     ::"r"(dst + (uint32_t)kPPXOff), "l"(xt0 + (slot1 ? xtile_bytes : 0) + (int64_t)(xo << 4)),
-                                       "r"((uint32_t)(kPPXCols * kTileM * 2)), "r"(bar) : "memory");
-                }
-            }
-        }
-    } else if (warp == kWarpMma) {
-        // =========================== MMA issuer (whole warp, one elected lane issues): table-driven (PROG) ===========================
-        uint32_t stage = 0, phase = 0, eph0 = 0, eph1 = 0;
-        uint32_t ahead = 0;              // the look-ahead probe of the CURRENT stage's full barrier already succeeded
-        // data-gradient mode: the first GEMM of every pair waits for the head stage the epilogue warps run first
-        bool started0 = kMode == PP_DGRAD, started1 = kMode == PP_DGRAD;
-        const uint32_t h_base = smem_u32(Hs), ring_base = smem_u32(ring);
-        const uint32_t full_a = smem_u32(full), empty_a = smem_u32(empty);
-        const uint32_t acc_full_a = smem_u32(acc_full), epi_done_a = smem_u32(epi_done);
-        const uint32_t nst = (uint32_t)kPPStages;
-        const uint64_t xd0 = make_desc(ring_base + (uint32_t)kPPXOff, kTileM * 16, 128);
-        const uint64_t bd_base = make_desc(ring_base, 0, 128);                 // LBO (= N * 16 bytes) is added per entry
-        const uint64_t hd0 = make_desc(h_base, kTileM * 16, 128), hd1 = make_desc(h_base + (uint32_t)h_bytes, kTileM * 16, 128);
-        const uint64_t a_step = (uint64_t)((2 * kTileM * 16) >> 4);
-        const uint64_t st_step = (uint64_t)(kPPStageBytes >> 4);
-        uint32_t accum = 0;
-        for (int64_t pr = blockIdx.x; pr < n_pairs; pr += gridDim.x) {
-            const bool valid1 = 2 * pr + 1 < n_tiles;
-            uint4 E = PROG[0];
-            for (int e = 0; e < n_prog;) {
-                const uint32_t fl = E.z & 0xFFu, N = E.z >> 8;
-                const uint4 E1 = PROG[e + 1], E2 = PROG[e + 2];      // prefetched: the table has two spare entries at its end
-                if ((fl & PF_SLOT1) && !valid1) { ++e; E = E1; continue; }
-                const uint32_t sl = (fl & PF_SLOT1) ? 1u : 0u;
-                if (fl & PF_FIRST) {
-                    // the previous GEMM of this tile slot has been drained from TMEM and its activations are in H[sl]
-                    if (sl == 0) { if (started0) { mbar_wait_a(epi_done_a, eph0); eph0 ^= 1; } started0 = true; }
-                    else         { if (started1) { mbar_wait_a(epi_done_a + 8, eph1); eph1 ^= 1; } started1 = true; }
-                    accum = 0;
-                }
-                const uint32_t cur = stage;
-                if (!ahead) mbar_wait_a(full_a + 8u * cur, phase);
-                if (++stage == nst) { stage = 0; phase ^= 1; }
-                if (fl & PF_PAIR) {
-                    // two activation stages (up to 4 MMAs) per iteration: the loop overhead of this single warp - not the data -
-                    // is what paces the kernel (ncu: it never waits on `full`, it is busy with ~90 instructions per stage)
-                    const uint32_t cur1 = stage;
-                    if (!mbar_test_a(full_a + 8u * cur1, phase)) mbar_wait_a(full_a + 8u * cur1, phase);
-                    tc_fence_after();
-                    if (++stage == nst) { stage = 0; phase ^= 1; }
-                    ahead = mbar_test_a(full_a + 8u * stage, phase);
-                    const uint64_t ad = (sl ? hd1 : hd0) + (uint64_t)E.w;
-                    const uint64_t bb = bd_base + ((uint64_t)N << 16);
-                    mma_stage2(tmem_base + sl * 256u, ad, a_step, bb + (uint64_t)cur * st_step, bb + (uint64_t)cur1 * st_step, (uint64_t)(2u * N),
-                               make_idesc((int)N), accum, ((E1.z & PF_TWO) ? 2u : 1u), empty_a + 8u * cur, empty_a + 8u * cur1);
-                    accum = 1;
-                    if (E1.z & PF_LAST) commit_elect(acc_full_a + 8u * sl);
-                    e += 2;
-                    E = E2;
-                    continue;
-                }
-                tc_fence_after();
-                ahead = mbar_test_a(full_a + 8u * stage, phase);              // next stage, overlapped with the issue below
-                const uint64_t so = (uint64_t)cur * st_step;
-                const uint64_t ad = (fl & PF_FROM_X) ? xd0 + so : (sl ? hd1 : hd0) + (uint64_t)E.w;
-                const uint64_t bd = bd_base + so + ((uint64_t)N << 16);        // LBO field = N * 16 bytes >> 4 = N
-                mma_stage(tmem_base + sl * 256u, ad, bd, ad + a_step, bd + (uint64_t)(2u * N), make_idesc((int)N), accum,
-                          (fl & PF_TWO) ? 1u : 0u, empty_a + 8u * cur);
-                accum = 1;
-                if (fl & PF_LAST) commit_elect(acc_full_a + 8u * sl);
-                ++e;
-                E = E1;
-            }
-        }
-    } else {
-        // =========================== epilogue (16 warps) ===========================
-        const int q = warp & 3;
-        const int part = warp >> 2;
-        const int r = q * 32 + lane;
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-        uint32_t aph0 = 0, aph1 = 0, fph0 = 0;
-        int last_sub = -1;
-        const int L = P.L;
-        for (int64_t pr = blockIdx.x; pr < n_pairs; pr += gridDim.x) {
-            const int64_t t0 = 2 * pr;
-            const bool valid1 = t0 + 1 < n_tiles;
-            {
-                const int sub0 = sub_of(t0);
-                if (sub0 != last_sub) {
-                    if (last_sub >= 0) {            // done with the previous sub-module's block
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&f32_empty[0]);
-                    }
-                    mbar_wait(&f32_full[0], fph0);
-                    fph0 ^= 1;
-                    last_sub = sub0;
-                }
-            }
-            int64_t slot_[2], row_[2] = {-1, -1};
-            float sigma_[2] = {0.0f, 0.0f};
-            for (int sl = 0; sl < 2; ++sl) {
-                if (sl == 1 && !valid1) continue;
-                slot_[sl] = (t0 + sl) * kTileM + r;
-                if (slot_[sl] < n_slots) row_[sl] = A.m.slot_row ? (int64_t)A.m.slot_row[slot_[sl]] : slot_[sl];
-            }
-            float dsig_[2] = {0.0f, 0.0f};       // PP_DGRAD: S * d(sigma pre-activation) of this thread's row, per tile slot
-            if (kMode == PP_DGRAD) {
-                // ---- head stage of the data-gradient chain (nerf.py:132-160 backwards): upstream gradient x blend weight ->
-                // sigmoid' / softplus' -> rgb Linear transposed (3 -> L/2, CUDA cores) -> ReLU mask of dir_a_encoding -> dZ_dira
-                // as the first A operand (columns 0 .. L/2-1 of the activation buffer) and on the gradient tape; per-image sums
-                // of its rows for the appearance-embedding gradient; head pre-activation gradients in fp32 for their own Linears.
-                const float S = *A.scale;
-                const int sub0 = last_sub;
-                const float* Wr = F32 + L;                                  // [3][L/2] rgb weights (fp32 block of the data-gradient plan)
-                for (int sl = 0; sl < 2; ++sl) {
-                    if (sl == 1 && !valid1) continue;
-                    const int64_t tile = t0 + sl;
-                    const int64_t row = row_[sl];
-                    const float* tf = A.tape_f32 + (size_t)tile * 5 * kTileM + r;
-                    float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f, g3 = 0.0f;
-                    if (row >= 0) {
-                        const float4 g = *reinterpret_cast<const float4*>(A.grad_out + row * 4);
-                        const float w = A.m.slot_w ? A.m.slot_w[slot_[sl]] : 1.0f;
-                        g0 = g.x * w; g1 = g.y * w; g2 = g.z * w; g3 = g.w * w;
-                    }
-                    const float c0v = tf[1 * kTileM], c1v = tf[2 * kTileM], c2v = tf[3 * kTileM], pre = tf[0];
-                    const float d0 = (g0 * (1.0f - c0v)) * c0v, d1 = (g1 * (1.0f - c1v)) * c1v, d2 = (g2 * (1.0f - c2v)) * c2v;
-                    float dsp;
-                    if (A.m.nd.softplus) { const float y = pre - 1.0f; dsp = y > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-y)); }
-                    else dsp = pre > 0.0f ? 1.0f : 0.0f;
-                    const float ds = g3 * dsp;
-                    dsig_[sl] = ds * S;
-                    if (part == 0) {
-                        float* tg = A.tape_gf32 + (size_t)tile * 4 * kTileM + r;
-                        tg[0] = ds; tg[1 * kTileM] = d0; tg[2 * kTileM] = d1; tg[3 * kTileM] = d2;
-                    }
-                    const int id = (int)tf[4 * kTileM];
-                    const unsigned char* gimg = A.tape_act + (size_t)tile * A.act_tile_bytes + (size_t)(A.layers + 1) * L * kTileM * 2;
-                    unsigned char* dimg = A.tape_dz + (size_t)tile * A.act_tile_bytes + (size_t)(A.layers + 1) * L * kTileM * 2;
-                    unsigned char* Hsl = Hs + (size_t)sl * h_bytes;
-                    const int half = L / 2, per = half / 4;                 // columns of dZ_dira handled by this thread (32 for L = 256)
-                    for (int kk = 0; kk < per; kk += 8) {
-                        const int k0 = part * per + kk;
-                        const uint4 gm = *reinterpret_cast<const uint4*>(gimg + (size_t)(k0 >> 3) * (kTileM * 16) + (size_t)r * 16);
-                        const __half2* gh = reinterpret_cast<const __half2*>(&gm);
-                        float v[8];
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) {
-                            const int k = k0 + e;
-                            float acc = Wr[k] * d0;
-                            acc = fmaf(Wr[half + k], d1, acc);
-                            acc = fmaf(Wr[2 * half + k], d2, acc);
-                            const float gv = (e & 1) ? __high2float(gh[e >> 1]) : __low2float(gh[e >> 1]);
-                            v[e] = gv > 0.0f ? acc : 0.0f;
-                        }
-                        // appearance-embedding gradient, step 1: per-image sums of dZ_dira rows (fp32, unscaled); the lanes of a warp
-                        // are consecutive slots, i.e. mostly samples of one ray = one image id
-                        if (A.emb_sum) {
-                            unsigned todo = __ballot_sync(0xffffffffu, row >= 0);
-                            while (todo) {
-                                const int leader = __ffs(todo) - 1;
-                                const int cur = __shfl_sync(0xffffffffu, id, leader);
-                                const bool mine = row >= 0 && id == cur;
-#pragma unroll
-                                for (int e = 0; e < 8; ++e) {
-                                    float t = mine ? v[e] : 0.0f;
-#pragma unroll
-                                    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
-                                    if (lane == leader) atomicAdd(A.emb_sum + ((size_t)sub0 * A.m.nd.app_count + cur) * half + k0 + e, t);
-                                }
-                                todo &= ~__ballot_sync(0xffffffffu, mine);
-                            }
-                        }
-                        uint32_t pk[4];
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) pk[e] = pack_h2(v[2 * e] * S, v[2 * e + 1] * S);
-                        const uint4 outv = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-                        *reinterpret_cast<uint4*>(Hsl + (size_t)(k0 >> 3) * (kTileM * 16) + (size_t)r * 16) = outv;
-                        *reinterpret_cast<uint4*>(dimg + (size_t)(k0 >> 3) * (kTileM * 16) + (size_t)r * 16) = outv;
-                    }
-                    fence_proxy_async();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&epi_done[sl]);
-                }
-            }
-            for (int gi = 0; gi < n_gemm; ++gi) {
-                const TcGemm& g = P.g[gi];
-#pragma unroll
-                for (int sl = 0; sl < 2; ++sl) {
-                    if (sl == 1 && !valid1) continue;
-                    if (sl == 0) { mbar_wait(&acc_full[0], aph0); aph0 ^= 1; }
-                    else         { mbar_wait(&acc_full[1], aph1); aph1 ^= 1; }
-                    tc_fence_after();
-                    if (warp == 0 && lane == 0) trace_ev(A.desc_swap, 1, 3, sl, gi);   // epilogue: accumulator ready
-                    const uint32_t t_acc = t_lane + (uint32_t)sl * 256u;
-                    const float* bias = F32 + g.bias_off;
-                    const int64_t row = row_[sl], slot = slot_[sl];
-                    unsigned char* Hsl = Hs + (size_t)sl * h_bytes;
-                    if (kMode == PP_DGRAD) {
-                        // dH = accumulator (scaled by S) [+ S dsigma x w_sigma] -> ReLU mask from the activation tape -> fp16 ->
-                        // next A operand + gradient tape.  g.bias_off holds the image index (the mask image and the target image
-                        // coincide: dZ_l = dH_l where H_l > 0).
-                        const int img = g.bias_off;
-                        const size_t ioff = (size_t)(t0 + sl) * A.act_tile_bytes + (size_t)img * L * kTileM * 2;
-                        const unsigned char* mimg = A.tape_act + ioff;
-                        unsigned char* dimg = A.tape_dz + ioff;
-                        const float dss = dsig_[sl];
-                        const int nslab = (g.n + 63) >> 6;
-                        for (int j = 0; j < nslab; ++j) {
-                            const int c0 = 64 * j + 16 * part;
-                            if (c0 >= g.n) continue;
-                            uint32_t v[16];
-                            tmem_ld16(t_acc + (uint32_t)c0, v);
-                            const size_t po = (size_t)(c0 >> 3) * (kTileM * 16) + (size_t)r * 16;
-                            uint4 m0 = make_uint4(0, 0, 0, 0), m1 = m0;
-                            if (g.epi != EPI_D_LINEAR) {
-                                m0 = *reinterpret_cast<const uint4*>(mimg + po);
-                                m1 = *reinterpret_cast<const uint4*>(mimg + po + kTileM * 16);
-                            }
-                            tmem_ld_wait();
-                            float f[16];
-#pragma unroll
-                            for (int i = 0; i < 16; ++i) f[i] = __uint_as_float(v[i]);
-                            if (g.epi == EPI_D_MASK_SIGMA) {
-#pragma unroll
-                                for (int i = 0; i < 16; ++i) f[i] = fmaf(dss, F32[c0 + i], f[i]);      // F32[0..L) = sigma weights
-                            }
-                            if (g.epi != EPI_D_LINEAR) {
-                                const __half2* h0 = reinterpret_cast<const __half2*>(&m0);
-                                const __half2* h1 = reinterpret_cast<const __half2*>(&m1);
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) {
-                                    const float hv = (i & 1) ? __high2float(h0[i >> 1]) : __low2float(h0[i >> 1]);
-                                    const float hw = (i & 1) ? __high2float(h1[i >> 1]) : __low2float(h1[i >> 1]);
-                                    if (!(hv > 0.0f)) f[i] = 0.0f;
-                                    if (!(hw > 0.0f)) f[8 + i] = 0.0f;
-                                }
-                            }
-                            uint32_t pk[8];
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) pk[e] = pack_h2(f[2 * e], f[2 * e + 1]);
-                            const uint4 o0 = make_uint4(pk[0], pk[1], pk[2], pk[3]), o1 = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-                            *reinterpret_cast<uint4*>(Hsl + po) = o0;
-                            *reinterpret_cast<uint4*>(Hsl + po + kTileM * 16) = o1;
-                            *reinterpret_cast<uint4*>(dimg + po) = o0;
-                            *reinterpret_cast<uint4*>(dimg + po + kTileM * 16) = o1;
-                        }
-                        fence_proxy_async();
-                        tc_fence_before();
-                        __syncwarp();
-                        // the last GEMM's epilogue is followed by this slot's next head stage (same warps): nobody waits for it
-                        if (lane == 0 && gi + 1 < n_gemm) mbar_arrive(&epi_done[sl]);
-                        continue;
-                    }
-                    // training forward: tape image of this GEMM's output (trunk layer gi; then F, then G)
-                    unsigned char* timg = nullptr;
-                    if (kMode == PP_TRAIN_FWD && g.epi != EPI_RGB)
-                        timg = A.tape_act + (size_t)(t0 + sl) * A.act_tile_bytes + (size_t)gi * L * kTileM * 2;
-                    if (g.epi == EPI_RGB) {
-                        if (part == 0) {
-                            uint32_t v[32];
-                            tmem_ld32(t_acc, v);
-                            tmem_ld_wait();
-                            float* tr = kMode == PP_TRAIN_FWD ? A.tape_f32 + (size_t)(t0 + sl) * 5 * kTileM + kTileM + r : nullptr;
-                            if (row >= 0) tc_emit_rgb(A.m, A.m.nd.affine ? sub_of(t0 + sl) : 0, row, slot, v, RGBB, sigma_[sl], tr);
-                            else if (tr) { tr[0] = 0.5f; tr[kTileM] = 0.5f; tr[2 * kTileM] = 0.5f; }
-                        }
-                    } else {
-                        const bool want_sigma = g.epi == EPI_RELU_SIGMA;
-                        const bool publish = !(want_sigma && A.m.sigma_only);
-                        const float* sw = SW;
-                        float sacc = 0.0f;
-                        const int nslab = (g.n + 63) >> 6;
-                        for (int j = 0; j < nslab; ++j) {
-                            const int c0 = 64 * j + 16 * part;
-                            if (c0 < g.n) {
-                                const size_t po = (size_t)(c0 >> 3) * (kTileM * 16) + (size_t)r * 16;
-                                unsigned char* dst = Hsl + po;
-                                unsigned char* gd = timg ? timg + po : nullptr;
-                                if (g.epi == EPI_RELU)
-                                    epi_piece16<false, true, false>(t_acc + (uint32_t)c0, bias + c0, sw + c0, dst, 0, true, gd);
-                                else if (g.epi == EPI_LINEAR)
-                                    epi_piece16<false, false, false>(t_acc + (uint32_t)c0, bias + c0, sw + c0, dst, 0, true, gd);
-                                else
-                                    sacc += epi_piece16<false, true, true>(t_acc + (uint32_t)c0, bias + c0, sw + c0, dst, 0, publish, gd);
-                            }
-                        }
-                        if (publish) fence_proxy_async();
-                        if (want_sigma) {
-                            SIGP[part * kTileM + r] = sacc;
-                            asm volatile("bar.sync 1, 512;" ::: "memory");
-                            if (part == 0) {
-                                float s = ((SIGP[r] + SIGP[kTileM + r]) + (SIGP[2 * kTileM + r] + SIGP[3 * kTileM + r])) + sw[L];
-                                if (A.m.sigma_noise && row >= 0) s = s + A.m.sigma_noise[row];
-                                const float sg = A.m.nd.softplus ? mn_softplus_shifted(s) : fmaxf(s, 0.0f);
-                                sigma_[sl] = sg;
-                                if (kMode == PP_TRAIN_FWD) {
-                                    float* tf = A.tape_f32 + (size_t)(t0 + sl) * 5 * kTileM + r;
-                                    tf[0] = s;                                                  // pre-activation (with the density noise)
-                                    tf[4 * kTileM] = (row >= 0 && A.m.nd.app > 0) ? A.m.src.index(row) : 0.0f;   // image id of the row
-                                }
-                                if (A.m.sigma_only && row >= 0) {
-                                    const int64_t o = (A.m.scatter ? row : slot) * A.m.out_cols;
-                                    A.m.out[o] = A.m.slot_w ? sg * A.m.slot_w[slot] : sg;
-                                }
-                            }
-                            asm volatile("bar.sync 1, 512;" ::: "memory");   // SIGP is reused by the other tile slot
-                        }
-                    }
-                    tc_fence_before();
-                    __syncwarp();
-                    if (warp == 0 && lane == 0) trace_ev(A.desc_swap, 1, 4, sl, gi);   // epilogue: this warp done
-                    if (lane == 0) mbar_arrive(&epi_done[sl]);
-                }
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    clk_stamp(A.desc_swap, 1);
-    if (warp == kWarpProd) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
-    }
-}
-
-#include "mn_mlp_tp.cuh"
-#include "mn_mlp_wide.cuh"
 #include "mn_train_tc.cuh"
 
 }  // namespace
@@ -1466,27 +453,29 @@ size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision)
     return mn_align((size_t)n_tiles128 * P.x_tile_bytes * planes, 1024) + 1024;
 }
 
+
 int mn_mlp_tp_program(const NetDims& nd, unsigned int* table_out, int cap_entries, int* info8) {
     TcPlan P;
-    if (!build_plan(nd, &P) || nd.L > 256) return MN_ERR_UNSUPPORTED;
-    std::vector<uint4> table;
-    int counts[4];
-    if (!tp_build_program(P, &table, counts)) return MN_ERR_UNSUPPORTED;
-    size_t tp_bytes = 0;
-    for (int gi = 0; gi < P.n_gemm; ++gi) tp_bytes += (size_t)tp_gemm_bytes(P.g[gi]);
-    const TPLayout TL = tp_layout(P);
-    const int info[8] = {counts[0], counts[1], counts[2], counts[3], (int)tp_bytes, TL.stages, TL.total, P.x_tile_bytes};
+    if (!build_plan(nd, &P)) return MN_ERR_UNSUPPORTED;
+    const WgLayout L = wg_layout(P, false);
+    int n = 0, n_trunk = 0;
+    for (int gi = 0; gi < P.n_gemm; ++gi) {
+        const int nch = (P.g[gi].n + 255) >> 8;
+        for (int ch = 0; ch < nch; ++ch)
+            wg_walk_chunk(P, gi, ch, 1, L.slab, [&](const WgStage& st) {
+                if (n < cap_entries) {
+                    unsigned int* e = table_out + 8 * (size_t)n;
+                    e[0] = (unsigned)st.w_off; e[1] = (unsigned)st.w_bytes; e[2] = (unsigned)st.nw; e[3] = (unsigned)st.kc;
+                    e[4] = (unsigned)st.a_col; e[5] = (unsigned)st.x_off; e[6] = (unsigned)st.x_bytes;
+                    e[7] = (unsigned)st.flags | ((unsigned)gi << 8) | ((unsigned)ch << 16);
+                }
+                ++n;
+            });
+        if (gi + 1 == P.n_trunk) n_trunk = n;
+    }
+    const int info[8] = {n, n_trunk, P.plane_bytes, L.stages, L.total, P.x_tile_bytes, L.stage_bytes, L.slab};
     for (int i = 0; i < 8; ++i) info8[i] = info[i];
-    int n = 0;
-    for (int i = 0; i < counts[0] && n < cap_entries; ++i, ++n) {
-        const uint4 e = table[i];
-        table_out[4 * n] = e.x; table_out[4 * n + 1] = e.y; table_out[4 * n + 2] = e.z; table_out[4 * n + 3] = e.w;
-    }
-    for (int i = 0; i < counts[2] && n < cap_entries; ++i, ++n) {
-        const uint4 e = table[kTPMaxProg + i];
-        table_out[4 * n] = e.x; table_out[4 * n + 1] = e.y; table_out[4 * n + 2] = e.z; table_out[4 * n + 3] = e.w;
-    }
-    return MN_OK;
+    return n <= cap_entries ? MN_OK : MN_ERR_WORKSPACE;
 }
 
 int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
@@ -1497,7 +486,7 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
     }
     const NetDims& nd = m->nd;
     // per sub-module: [hi plane][lo plane][fp32 block, 256-aligned]
-    // 512-wide network: only the wide kernel runs it; its one image ([N half of 256][K/8][256][8]) lives in the hi plane
+    // 512-wide network (tc_f16 only): its one image per GEMM ([N half of 256][K/8][256][8]) lives in the hi plane
     const bool wide = nd.L > 256;
     const size_t sub_bytes = mn_align((size_t)P.plane_bytes * 2 + (size_t)(((P.f32_floats * 4 + 255) / 256) * 256), 256);
     if (!m->tc_packed) {
@@ -1507,26 +496,6 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
     }
     unsigned char* base = (unsigned char*)m->tc_packed + (size_t)sub * sub_bytes;
     const float* Pk = m->packed + (size_t)sub * m->lay.total;
-    // TMEM ping-pong kernel (layer_dim <= 256): its own weight plane and, once per model, the role tables
-    unsigned char* tp_base = nullptr;
-    size_t tp_woff = 0;
-    if (!wide) {
-        size_t tp_bytes = 0;
-        for (int gi2 = 0; gi2 < P.n_gemm; ++gi2) tp_bytes += (size_t)tp_gemm_bytes(P.g[gi2]);
-        tp_bytes = mn_align(tp_bytes, 256);
-        if (!m->tc_tp) {
-            std::vector<uint4> table;
-            if (tp_build_program(P, &table, m->tp_n)) {
-                MN_CUDA(ctx, cudaMalloc(&m->tc_tp, tp_bytes * m->d.n_sub));
-                MN_CUDA(ctx, cudaMemsetAsync(m->tc_tp, 0, tp_bytes * m->d.n_sub, st));
-                MN_CUDA(ctx, cudaMalloc(&m->tp_prog, table.size() * sizeof(uint4)));
-                MN_CUDA(ctx, cudaMemcpyAsync(m->tp_prog, table.data(), table.size() * sizeof(uint4), cudaMemcpyHostToDevice, st));
-                MN_CUDA(ctx, cudaStreamSynchronize(st));      // `table` is pageable host memory
-                m->tc_tp_sub_bytes = tp_bytes;
-            }
-        }
-        if (m->tc_tp) tp_base = (unsigned char*)m->tc_tp + (size_t)sub * m->tc_tp_sub_bytes;
-    }
     float* f32 = reinterpret_cast<float*>(base + (size_t)P.plane_bytes * 2);
     auto pack = [&](const TcGemm& g, const float* wt, int n_src, int k_src, int k_real0, int k_pad0, const float* bias,
                     int n_bias) -> int {
@@ -1542,11 +511,6 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
         }
         mn_pack_push(ctx, PackOp{wt, hi, lo, (long long)n, PK_TC_IMAGE, {n_src, k_src, g.n, K, k_real0, k_pad0, 0}});
         mn_pack_push(ctx, PackOp{bias, f32 + g.bias_off, nullptr, 256, PK_TC_F32, {n_bias, 0, 0, 0, 0, 0, 0}});
-        if (tp_base) {       // half-major image of the TMEM ping-pong kernel: [N-half][K/8][nw][8]
-            const int nw = g.n < 128 ? g.n : 128, nh = (g.n + 127) / 128;
-            mn_pack_push(ctx, PackOp{wt, tp_base + tp_woff, nullptr, (long long)nh * nw * K, PK_TC_HALF, {n_src, k_src, g.n, K, k_real0, k_pad0, nw}});
-            tp_woff += tp_gemm_bytes(g);
-        }
         return MN_OK;
     };
     int rc, gi = 0;
@@ -1626,29 +590,6 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
     A.ximg = ximg;
     A.x_plane_halves = (int64_t)n_tiles128 * (P.kpe + P.kaux) * kTileM;
 
-    // ---- kernel selection: the ping-pong kernel for layer_dim <= 256 (MN_TC_PINGPONG=0: the single-tile kernel, kept as
-    // the cross-check of the variants test), the wide kernel for 512, the split kernel for tc_f16x3
-    static int use_pp = -1;
-    if (use_pp < 0) {
-        const char* e = getenv("MN_TC_PINGPONG");
-        use_pp = (e && e[0] == '0') ? 0 : 1;
-    }
-    // The TMEM ping-pong kernel (mn_mlp_tp.cuh) is the default inference kernel for layer_dim <= 256; MN_TC_TP=0 selects the
-    // shared-memory ping-pong kernel (which also serves the two training modes) - variants test, A/B runs
-    static int use_tp = -1;
-    if (use_tp < 0) {
-        const char* e = getenv("MN_TC_TP");
-        use_tp = (e && e[0] == '0') ? 0 : 1;
-    }
-    const TPLayout TL = tp_layout(P);
-    const bool run_tp = !split && P.L <= 256 && use_tp && use_pp && m->tc_tp && TL.stages >= 8;
-    A.tpack = (const unsigned char*)m->tc_tp;
-    A.tp_sub_bytes = m->tc_tp_sub_bytes;
-    A.tp_prog = (const uint4*)m->tp_prog;
-    for (int i = 0; i < 4; ++i) A.tp_n[i] = m->tp_n[i];
-    const PPLayout PL = pp_layout(P);
-    const bool run_pp = !split && P.L <= 256 && use_pp && PL.total <= kSmemMax && PL.stages >= 3 &&
-                        pp_prog_entries(P, P.n_gemm) + 2 <= kPPMaxProg;
 
     const size_t enc_sm = (size_t)P.x_tile_bytes * (split ? 2 : 1);
     MN_CUDA(ctx, cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
@@ -1661,73 +602,13 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
         tc_encode_kernel<<<(unsigned)n_tiles128, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split, ximg, A.x_plane_halves);
     MN_LAUNCH_CHECK(ctx);
 
-    if (P.L > 256) {
-        const WLayout WL = w_layout(P);
-        if (WL.total > kSmemMax) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP (512-wide): shared-memory budget exceeded");
-        // MN_TC_CLUSTER=2: clusters of two CTAs share one multicast weight stream (the router's bucket alignment
-        // guarantees that tiles 2p and 2p+1 belong to one sub-module).  Halves the L2 reads but measured 2-3 % SLOWER
-        // on B200: every SM still RECEIVES all weight bytes, and the ~32 B/clk/SM delivery rate is what binds these kernels
-        // (DESIGN.md §7) - multicast saves L2 reads, not deliveries.  The default is one CTA per cluster.
-        static int cs = -1;
-        if (cs < 0) {
-            const char* e = getenv("MN_TC_CLUSTER");
-            cs = (e && e[0] == '2') ? 2 : 1;
-        }
-        mn_prof_begin(ctx, st);
-        if (cs == 2) {
-            MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_wide_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, WL.total));
-            const int64_t groups = (n_tiles128 + 1) / 2;
-            const unsigned ncl = (unsigned)(groups < ctx->sm_count / 2 ? groups : ctx->sm_count / 2);
-            cudaLaunchConfig_t cfg{};
-            cfg.gridDim = dim3(2 * ncl);
-            cfg.blockDim = dim3(kThreads);
-            cfg.dynamicSmemBytes = (size_t)WL.total;
-            cfg.stream = st;
-            cudaLaunchAttribute at[1];
-            at[0].id = cudaLaunchAttributeClusterDimension;
-            at[0].val.clusterDim.x = 2;
-            at[0].val.clusterDim.y = 1;
-            at[0].val.clusterDim.z = 1;
-            cfg.attrs = at;
-            cfg.numAttrs = 1;
-            MN_CUDA(ctx, cudaLaunchKernelEx(&cfg, tc_mlp_wide_kernel<2>, A));
-        } else {
-            MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_wide_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, WL.total));
-            const unsigned grid_w = (unsigned)(n_tiles128 < ctx->sm_count ? n_tiles128 : ctx->sm_count);
-            tc_mlp_wide_kernel<1><<<grid_w, kThreads, WL.total, st>>>(A);
-        }
-        mn_prof_end(ctx, st);
-        MN_LAUNCH_CHECK(ctx);
-        return MN_OK;
-    }
-    const SmemLayout SL = smem_layout(P, split != 0);
-    const int total = SL.total;
-    if (total > kSmemMax || SL.stages < 2) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: shared-memory budget exceeded");
-    const unsigned grid = (unsigned)(n_tiles128 < ctx->sm_count ? n_tiles128 : ctx->sm_count);
-    if (split) {
-        MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, total));
-        mn_prof_begin(ctx, st);
-        tc_mlp_kernel<true><<<grid, kThreads, total, st>>>(A);
-    } else {
-        if (run_tp) {
-            const unsigned grid_tp = (unsigned)((n_tiles128 + 1) / 2 < ctx->sm_count ? (n_tiles128 + 1) / 2 : ctx->sm_count);
-            MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_tp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TL.total));
-            mn_prof_begin(ctx, st);
-            tc_mlp_tp_kernel<<<grid_tp, kTPThreads, TL.total, st>>>(A);
-        } else if (run_pp) {
-            const unsigned grid_pp = (unsigned)((n_tiles128 + 1) / 2 < ctx->sm_count ? (n_tiles128 + 1) / 2 : ctx->sm_count);
-            MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_pp_kernel<PP_INFER>, cudaFuncAttributeMaxDynamicSharedMemorySize, PL.total));
-            mn_prof_begin(ctx, st);
-            tc_mlp_pp_kernel<PP_INFER><<<grid_pp, kPPThreads, PL.total, st>>>(A);
-        } else {
-            MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, total));
-            mn_prof_begin(ctx, st);
-            tc_mlp_kernel<false><<<grid, kThreads, total, st>>>(A);
-        }
-    }
+    mn_prof_begin(ctx, st);
+    int rc;
+    if (split) rc = wg_launch<PP_INFER, true, false>(ctx, A, n_tiles128, st);
+    else if (P.L > 256) rc = wg_launch<PP_INFER, false, true>(ctx, A, n_tiles128, st);
+    else rc = wg_launch<PP_INFER, false, false>(ctx, A, n_tiles128, st);
     mn_prof_end(ctx, st);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return rc;
 }
 
 // =================================================================================================
@@ -1767,16 +648,10 @@ int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n
     if (fast_shape) tc_encode_fast_kernel<3, 12, 4, 48><<<(unsigned)n_tiles128, kTileM, 0, st>>>(a, ximg);
     else tc_encode_kernel<<<(unsigned)n_tiles128, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, 0, ximg, 0);
     MN_LAUNCH_CHECK(ctx);
-    const PPLayout PL = pp_layout(P);
-    if (PL.total > kSmemMax || PL.stages < 3 || pp_prog_entries(P, P.n_gemm) + 2 > kPPMaxProg)
-        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training forward: shared-memory budget exceeded");
-    const unsigned grid = (unsigned)((n_tiles128 + 1) / 2 < ctx->sm_count ? (n_tiles128 + 1) / 2 : ctx->sm_count);
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_pp_kernel<PP_TRAIN_FWD>, cudaFuncAttributeMaxDynamicSharedMemorySize, PL.total));
     mn_prof_begin(ctx, st);
-    tc_mlp_pp_kernel<PP_TRAIN_FWD><<<grid, kPPThreads, PL.total, st>>>(A);
+    const int rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
     mn_prof_end(ctx, st);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return rc;
 }
 
 // backward workspace: [gradient records][head gradients fp32 [n_tiles][4][128]][embedding sums][scale]
@@ -1809,7 +684,6 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     MN_LAUNCH_CHECK(ctx);
 
     // ---- data gradients
-    TcPlan& D = A.plan;
     A.m = MlpArgs{};
     A.m.nd = nd;
     A.m.slot_row = a.slot_row;
@@ -1830,13 +704,10 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     A.scale = scale;
     A.act_tile_bytes = (int64_t)act_tile;
     A.layers = nd.layers;
-    const PPLayout PL = pp_layout(D);
-    if (PL.total > kSmemMax || PL.stages < 3 || pp_prog_entries(D, D.n_gemm) + 2 > kPPMaxProg)
-        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: shared-memory budget exceeded");
-    const unsigned grid = (unsigned)((n_tiles128 + 1) / 2 < ctx->sm_count ? (n_tiles128 + 1) / 2 : ctx->sm_count);
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_pp_kernel<PP_DGRAD>, cudaFuncAttributeMaxDynamicSharedMemorySize, PL.total));
-    tc_mlp_pp_kernel<PP_DGRAD><<<grid, kPPThreads, PL.total, st>>>(A);
-    MN_LAUNCH_CHECK(ctx);
+    {
+        const int rc = wg_launch<PP_DGRAD, false, false>(ctx, A, n_tiles128, st);
+        if (rc != MN_OK) return rc;
+    }
 
     // ---- weight gradients: one item per (Linear input segment, 128-channel output half)
     WgArgs W{};

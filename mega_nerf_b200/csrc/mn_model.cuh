@@ -66,11 +66,6 @@ struct mn_model {
     void* tc_dgrad = nullptr;
     size_t tc_dgrad_sub_bytes = 0;
     int train_tc_ok = 0;
-    // half-major fp16 weight images + role tables of the TMEM ping-pong kernel (mn_mlp_tp.cuh); NULL for layer_dim 512
-    void* tc_tp = nullptr;
-    size_t tc_tp_sub_bytes = 0;
-    void* tp_prog = nullptr;
-    int tp_n[4] = {0, 0, 0, 0};
 };
 
 // counters_d layout (ints)

@@ -2,18 +2,18 @@
 // mn_mlp_tc.cu's anonymous namespace.  SURVEY.md §8f-1; the reference trains exactly this way on a GPU: Linear layers in
 // fp16 with fp32 accumulation under autocast, gradients scaled into fp16 range (runner.py:243-274, opts.py:99).
 //
-//   forward   tc_mlp_pp_kernel<PP_TRAIN_FWD>  the inference kernel + every layer's fp16 activations written to a tape in the
+//   forward   tc_mlp_wg_kernel<PP_TRAIN_FWD>  the inference kernel + every layer's fp16 activations written to a tape in the
 //                                             tile-image layout of the activation buffer ([cols/8][128 slots][8]).
-//   dgrad     tc_mlp_pp_kernel<PP_DGRAD>      the same GEMM pipeline on transposed weight images: head stage on CUDA cores
+//   dgrad     tc_mlp_wg_kernel<PP_DGRAD>      the same GEMM pipeline on transposed weight images: head stage on CUDA cores
 //                                             (sigmoid' / softplus' / rgb Linear transposed), then dH_{l-1} = dZ_l W_l with the
 //                                             ReLU mask read from the activation tape in the epilogue; dZ images (fp16, scaled by
 //                                             a power of two S) go to a gradient tape.
 //   wgrad     tc_wgrad_kernel                 dW_l = dZ_l^T X_l over all slots of a sub-module: both tapes are consumed AS THEY
-//                                             ARE through MN-major UMMA descriptors (the slot axis is the K axis; LBO = 128 B
-//                                             between 8-slot groups, SBO = 2048 B between 8-column groups - verified by
-//                                             scripts/probes/mn_major_probe.cu), M = 128 output channels per CTA, N <= 256 input
-//                                             channels + a 16-column all-ones operand whose product is the bias gradient,
-//                                             accumulated in TMEM over a chunk of tiles and flushed with fp32 atomics.
+//                                             ARE through MN-major wgmma descriptors (the slot axis is the K axis; LBO = 128 B
+//                                             between 8-slot groups, SBO = 2048 B between 8-column groups), M = 128 output
+//                                             channels per CTA (64 per consumer warpgroup), N <= 256 input channels + a 16-column
+//                                             all-ones operand whose product is the bias gradient, accumulated in registers over
+//                                             a chunk of tiles and flushed with fp32 atomics.
 //   heads     tc_heads_wgrad_kernel (sigma / rgb Linears: 1 and 3 output channels - CUDA cores), tc_emb_grad_kernel
 //             (appearance embedding: W_e^T times the per-image sums of dZ_dira rows collected by the dgrad head stage).
 #pragma once
@@ -90,7 +90,7 @@ struct WgArgs {
     const float* scale;
 };
 constexpr int kWgStageBytes = 96 * 1024;
-constexpr int kWgThreads = 192;
+constexpr int kWgThreads = 384;     // warpgroup 0: producer thread; warpgroups 1-2: output channels 0-63 / 64-127 of the item
 
 __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A) {
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -98,10 +98,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
     unsigned char* ones = smem + 2 * kWgStageBytes;               // 6 KiB of fp16 1.0
     uint64_t* bars = reinterpret_cast<uint64_t*>(ones + 6144);
     uint64_t* full = bars;        // [2]
-    uint64_t* empty = bars + 2;   // [2]
-    uint64_t* done = bars + 4;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint64_t* empty = bars + 2;   // [2], one arrival per consumer warpgroup
     const WgItem it = A.item[blockIdx.y];
     int sub = A.fixed_sub;
     int64_t t_lo = 0, t_hi = A.n_tiles;
@@ -116,23 +113,16 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
 
     for (int i = threadIdx.x; i < 6144 / 4; i += kWgThreads) reinterpret_cast<uint32_t*>(ones)[i] = 0x3C003C00u;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 2; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 1); }
-        mbar_init(done, 1);
+        for (int i = 0; i < 2; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     fence_proxy_async();
-    if (warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const uint32_t xbytes = (uint32_t)(it.n / 8) * (kTileM * 16);
 
-    if (warp == 0) {
-        if (lane == 0) {
+    const int wgi = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);     // warp-uniform role
+    if (wgi == 0) {
+        if (threadIdx.x == 0) {
             uint32_t st = 0, ph = 0;
             const unsigned char* xbase = it.x_region ? A.xreg : A.act;
             const int64_t xstride = it.x_region ? A.x_tile_bytes : A.act_tile_bytes;
@@ -144,61 +134,71 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
                 if (++st == 2) { st = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // A = dZ^T (M = 128 channels x K = 16 slots), B = X^T: both MN-major views of the row-major tile images
-        const uint32_t idesc = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(it.n >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
-        const uint32_t idesc1 = (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(16 >> 3) << 17) | ((uint32_t)(kTileM >> 4) << 24);
-        const uint64_t od = make_desc(smem_u32(ones), 128, 2048);
-        uint32_t st = 0, ph = 0, accum = 0;
-        for (int64_t t = t_begin; t < t_end; ++t) {
-            mbar_wait(&full[st], ph);
-            tc_fence_after();
-            const uint32_t base = smem_u32(ring) + st * (uint32_t)kWgStageBytes;
-            if (elect_one()) {
+    } else {
+        // A = dZ^T (M = 64 channels of this warpgroup x K = 16 slots), B = X^T: both MN-major views of the tile images
+        // ([cols/8][128 slots][8]): leading byte offset 128 (next 8 slots), stride byte offset 2048 (next 8 columns).  The
+        // all-ones operand turns the bias gradient into one more N = 16 MMA.
+        const int wg = wgi - 1;
+        const int tid = threadIdx.x & 127, w = tid >> 5, lane = tid & 31, q4 = lane & 3;
+        const int ca = 64 * wg + 16 * w + (lane >> 2), cb = ca + 8;      // output channels of this thread's accumulator rows
+        const uint64_t od = wg_desc(smem_u32(ones), 128, 2048);
+        auto run = [&](auto nm_tag) {
+            constexpr int NM = decltype(nm_tag)::value;
+            float acc[NM / 2], accb[8];
+#pragma unroll
+            for (int i = 0; i < NM / 2; ++i) acc[i] = 0.0f;
+#pragma unroll
+            for (int i = 0; i < 8; ++i) accb[i] = 0.0f;
+            wg_fence_operand<NM / 2>(acc);
+            wg_fence_operand<8>(accb);
+            uint32_t st = 0, ph = 0;
+            int prev = -1;
+            for (int64_t t = t_begin; t < t_end; ++t) {
+                mbar_wait(&full[st], ph);
+                const uint32_t base = smem_u32(ring) + st * (uint32_t)kWgStageBytes;
+                wg_fence();
 #pragma unroll
                 for (int ks = 0; ks < 8; ++ks) {
-                    const uint64_t ad = make_desc(base + (uint32_t)ks * 256u, 128, 2048);
-                    const uint64_t bd = make_desc(base + 32768u + (uint32_t)ks * 256u, 128, 2048);
-                    tc_mma_f16(tmem_base, ad, bd, idesc, accum);
-                    if (it.b_off >= 0) tc_mma_f16(tmem_base + 256u, ad, od, idesc1, accum);
-                    accum = 1;
+                    const uint64_t ad = wg_desc(base + (uint32_t)ks * 256u + (uint32_t)wg * 16384u, 128, 2048);
+                    const uint64_t bd = wg_desc(base + 32768u + (uint32_t)ks * 256u, 128, 2048);
+                    wg_mma<NM, 1, 1>(acc, ad, bd, 1u);
+                    if (it.b_off >= 0) wg_mma<16, 1, 1>(accb, ad, od, 1u);
                 }
-                tc_commit(&empty[st]);
+                wg_commit();
+                if (prev >= 0) {
+                    wg_wait<1>();
+                    if (tid == 0) mbar_arrive(&empty[prev]);
+                }
+                prev = (int)st;
+                if (++st == 2) { st = 0; ph ^= 1; }
             }
-            accum = 1;
-            __syncwarp();
-            if (++st == 2) { st = 0; ph ^= 1; }
-        }
-        if (elect_one()) tc_commit(done);
-        __syncwarp();
-    } else {
-        // ---- flush: lane = output channel, columns = input channels; unscale and accumulate into the fp32 gradient block
-        mbar_wait(done, 0);
-        tc_fence_after();
-        const int q = warp & 3;                                   // TMEM lane quarter of warps 2..5: 2, 3, 0, 1
-        const int r = q * 32 + lane;
-        const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-        const float inv = 1.0f / *A.scale;
-        float* W = A.gw + (size_t)sub * A.sub_stride;
-        for (int c0 = 0; c0 < it.n; c0 += 16) {
-            uint32_t v[16];
-            tmem_ld16(t_lane + (uint32_t)c0, v);
-            tmem_ld_wait();
+            wg_wait<0>();
+            wg_fence_operand<NM / 2>(acc);
+            wg_fence_operand<8>(accb);
+            // ---- flush: unscale and accumulate into the fp32 gradient block ([out][in] rows of the nn.Linear weight)
+            const float inv = 1.0f / *A.scale;
+            float* W = A.gw + (size_t)sub * A.sub_stride;
 #pragma unroll
-            for (int i = 0; i < 16; ++i)
-                if (c0 + i < it.n_real) atomicAdd(W + it.w_off + (size_t)r * it.k_in + c0 + i, __uint_as_float(v[i]) * inv);
-        }
-        if (it.b_off >= 0) {
-            uint32_t v[16];
-            tmem_ld16(t_lane + 256u, v);
-            tmem_ld_wait();
-            atomicAdd(W + it.b_off + r, __uint_as_float(v[0]) * inv);
-        }
-        tc_fence_before();
+            for (int j = 0; j < NM / 8; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int c = 8 * j + 2 * q4 + e;
+                    if (c < it.n_real) {
+                        atomicAdd(W + it.w_off + (size_t)ca * it.k_in + c, acc[4 * j + e] * inv);
+                        atomicAdd(W + it.w_off + (size_t)cb * it.k_in + c, acc[4 * j + 2 + e] * inv);
+                    }
+                }
+            }
+            if (it.b_off >= 0 && q4 == 0) {
+                atomicAdd(W + it.b_off + ca, accb[0] * inv);
+                atomicAdd(W + it.b_off + cb, accb[2] * inv);
+            }
+        };
+        if (it.n > 128) run(std::integral_constant<int, 256>{});
+        else if (it.n > 64) run(std::integral_constant<int, 128>{});
+        else if (it.n > 32) run(std::integral_constant<int, 64>{});
+        else run(std::integral_constant<int, 32>{});
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512));
 }
 
 // sigma Linear (1 x L) and rgb Linear (3 x L/2) weight / bias gradients from the fp32 head gradients and the fp16 tapes.

@@ -1,5 +1,5 @@
 """Alias this package over the reference's module names so that the reference's own
-train.py / eval.py / Runner import the B200 path unchanged:
+train.py / eval.py / Runner import this package's path unchanged:
 
     import mega_nerf_b200; mega_nerf_b200.install()
     from mega_nerf.runner import Runner        # picks up render_rays / get_nerf / get_rays from here

@@ -26,7 +26,7 @@ _precision = os.environ.get('MN_B200_PRECISION', 'tc_f16')
 
 
 def set_precision(name: str) -> None:
-    """'fp32' (CUDA-core parity mode), 'tc_f16' (tcgen05, 1 pass) or 'tc_f16x3' (tcgen05, split)."""
+    """'fp32' (CUDA-core parity mode), 'tc_f16' (wgmma, 1 pass) or 'tc_f16x3' (wgmma, split)."""
     global _precision
     if name not in K.PRECISIONS:
         raise ValueError(f'unknown precision {name!r}; choose from {sorted(K.PRECISIONS)}')

@@ -1,5 +1,5 @@
 """render_rays() with the reference's signature and result dictionary (mega_nerf/rendering.py:15-173),
-orchestrating the sm_100a kernels of libmn_b200.so.  Host syncs happen only where the reference has
+orchestrating the sm_90a kernels of libmn_b200.so.  Host syncs happen only where the reference has
 them too (sphere check :412, background ray selection :37).
 
 When autograd is recording and a network parameter requires grad (the reference's training step,

@@ -9,10 +9,9 @@ arithmetic provider, SURVEY.md §8c), of the algorithm in the reference reposito
 cmusatyalab/mega-nerf @76d8d76b.  Every function cites the reference file:line it follows.
 
 Parity pinning: the reference ships no tests / golden vectors (SURVEY.md §4), so this oracle is
-pinned against outputs of the reference itself, imported read-only in the build container by
+pinned against outputs of the reference itself, imported read-only on the CPU by
 `tests/golden/make_golden.py`; the resulting fixtures are committed under `tests/golden/` and
-`tests/test_oracle_golden.py` re-checks the oracle against them everywhere (and against the live
-reference whenever `/root/reference` exists).
+`tests/test_oracle_golden.py` re-checks the oracle against them everywhere.
 
 Everything is functional: a network is a `NerfSpec` (hyper-parameters) plus a flat dict of
 tensors using the reference's state-dict key names, so both the reference's modules and the

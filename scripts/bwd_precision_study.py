@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """CPU study for the tensor-core backward (DESIGN.md §10 item 4): how large is the parameter-gradient error if the tapes
-and operands are 16-bit, as a tcgen05 backward would keep them?  The chain rule of tests/test_backward_algorithm.py is
+and operands are 16-bit, as the tensor-core backward keeps them?  The chain rule of tests/test_backward_algorithm.py is
 re-run with the operands of every GEMM rounded to fp16 / bf16 (fp32 accumulation, like the MMA) and compared with fp32
 autograd, for upstream gradients of realistic magnitude (render_rays' own dL/d(rgb, sigma) on a grad case) with and
 without a power-of-two loss scale.  Prints the worst per-tensor deviation relative to the tensor's max.

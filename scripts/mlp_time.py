@@ -1,5 +1,5 @@
 """Times the MLP kernel alone on a fixed batch (single sub-module, identity slots): python scripts/mlp_time.py [width] [tiles_per_sm]
-Env switches of mn_mlp_tc.cu (MN_TC_NOFETCH, MN_TC_CLUSTER, MN_TC_PINGPONG ...) apply.  Prints ms, TFLOP/s and the SM clock."""
+MN_B200_PRECISION selects the arithmetic (tc_f16 by default).  Prints ms, TFLOP/s and the SM clock."""
 import ctypes as C
 import os
 import subprocess
@@ -21,7 +21,7 @@ tps = int(sys.argv[2]) if len(sys.argv) > 2 else 32
 dev = torch.device('cuda:0')
 spec = O.NerfSpec(layer_dim=width)
 net = O.make_net('nerf', spec, seed=3)
-n = 148 * 128 * tps
+n = torch.cuda.get_device_properties(dev).multi_processor_count * 128 * tps
 x = Cs.nerf_rows(spec, 4096, 9).repeat(n // 4096 + 1, 1)[:n].contiguous().to(dev)
 p = build_net(net, dev)
 M.set_precision(os.environ.get('MN_B200_PRECISION', 'tc_f16'))

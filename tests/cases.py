@@ -6,8 +6,11 @@ seeding is detected rather than silently compared.
 """
 from __future__ import annotations
 
+import glob
+import io
 import os
 import sys
+import tempfile
 from typing import Dict
 
 import torch
@@ -19,6 +22,65 @@ if ROOT not in sys.path:
 from oracle import mn_oracle as O  # noqa: E402
 
 GOLDEN_PATH = os.path.join(ROOT, 'tests', 'golden', 'hotpath_v1.pt')
+GOLDEN_PART_BYTES = 900 * 1000          # every committed fixture file stays below 1 MB
+
+
+def _parts(path: str):
+    return sorted(glob.glob(path + '.part*'), key=lambda p: int(p.rsplit('.part', 1)[1]))
+
+
+def load_golden(path: str):
+    """A fixture written by save_golden: the dict in `path`, or the union of its key-disjoint parts `path`.partN."""
+    if os.path.exists(path):
+        return torch.load(path, map_location='cpu', weights_only=False)
+    parts = _parts(path)
+    if not parts:
+        raise FileNotFoundError(path)
+    out = {}
+    for p in parts:
+        out.update(torch.load(p, map_location='cpu', weights_only=False))
+    return out
+
+
+def save_golden(G: dict, path: str) -> None:
+    """torch.save(G, path), split by top-level keys into parts `path`.partN of at most GOLDEN_PART_BYTES each."""
+    for p in _parts(path) + ([path] if os.path.exists(path) else []):
+        os.remove(p)
+    parts, cur, cur_bytes = [], {}, 0
+    for k, v in G.items():
+        b = io.BytesIO()
+        torch.save(v, b)
+        if cur and cur_bytes + b.tell() > GOLDEN_PART_BYTES:
+            parts.append(cur)
+            cur, cur_bytes = {}, 0
+        cur[k] = v
+        cur_bytes += b.tell()
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        torch.save(part, f'{path}.part{i}')
+
+
+def join_golden_bytes(path: str) -> str:
+    """A binary fixture stored as byte parts `path`.partN (split_golden_bytes): the path of the reassembled file, written
+    once per process to a temporary directory."""
+    if os.path.exists(path):
+        return path
+    out = os.path.join(tempfile.gettempdir(), f'mn_golden_{os.getpid()}_{os.path.basename(path)}')
+    if not os.path.exists(out):
+        with open(out + '.tmp', 'wb') as f:
+            for p in _parts(path):
+                f.write(open(p, 'rb').read())
+        os.replace(out + '.tmp', out)
+    return out
+
+
+def split_golden_bytes(path: str) -> None:
+    """Replace the file `path` by byte parts `path`.partN of at most GOLDEN_PART_BYTES each."""
+    data = open(path, 'rb').read()
+    for i in range(0, len(data), GOLDEN_PART_BYTES):
+        with open(f'{path}.part{i // GOLDEN_PART_BYTES}', 'wb') as f:
+            f.write(data[i:i + GOLDEN_PART_BYTES])
+    os.remove(path)
 
 
 def checksum(*tensors) -> float:
@@ -174,7 +236,11 @@ def cluster_mask_case() -> dict:
                 near=0.05, far=1.5, cluster_2d=True, boundary_margin=1.15, center_pixels=True)
 
 
-CONTAINER_PATH = os.path.join(ROOT, 'tests', 'golden', 'container_v1.pt')
+CONTAINER_PATH = os.path.join(ROOT, 'tests', 'golden', 'container_v1.pt')     # stored as byte parts: use container_path()
+
+
+def container_path() -> str:
+    return join_golden_bytes(CONTAINER_PATH)
 
 
 def container_nets():

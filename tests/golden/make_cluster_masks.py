@@ -1,6 +1,6 @@
 """Generate tests/golden/cluster_masks_v1.pt by running the UNMODIFIED reference script
 scripts/create_cluster_masks.py (main(), CPU) on a tiny synthetic dataset directory written to a temp dir.
-Run in the build container only:    python tests/golden/make_cluster_masks.py
+Needs a checkout of the reference:    MEGA_NERF_REFERENCE=<path> python tests/golden/make_cluster_masks.py
 Pins oracle/mn_oracle.py::image_cluster_masks / cluster_min_dist_ratios (SURVEY.md §8f-3)."""
 from __future__ import annotations
 

@@ -1,7 +1,7 @@
 """Generate tests/golden/container_v1.pt: a merged TorchScript container exactly as the reference's
 scripts/merge_submodules.py:70-77 writes it (MegaNeRFContainer of reference NeRF sub-modules, scripted),
-with small seeded networks.  Run in the build container only (needs /root/reference):
-    python tests/golden/make_container.py
+with small seeded networks.  Needs a checkout of the reference:
+    MEGA_NERF_REFERENCE=<path> python tests/golden/make_container.py
 The fixture is the on-disk INPUT format of the path (SURVEY.md §8f-4); loading it needs no reference code."""
 from __future__ import annotations
 
@@ -28,7 +28,8 @@ def main():
     torch.jit.save(torch.jit.script(cont.eval()), C.CONTAINER_PATH)
     back = torch.jit.load(C.CONTAINER_PATH, map_location='cpu')
     assert len(back.centroids) == 4 and back.cluster_2d is True
-    print(f'wrote {C.CONTAINER_PATH} ({os.path.getsize(C.CONTAINER_PATH) / 1e6:.2f} MB)')
+    C.split_golden_bytes(C.CONTAINER_PATH)          # committed as byte parts below 1 MB each (C.container_path() joins them)
+    print(f'wrote {C.CONTAINER_PATH}.part*')
 
 
 if __name__ == '__main__':

@@ -1,8 +1,8 @@
 """Generate tests/golden/hotpath_v1.pt by running the UNMODIFIED reference (imported read-only
-from /root/reference) on the seeded cases of tests/cases.py.
+from $MEGA_NERF_REFERENCE) on the seeded cases of tests/cases.py.
 
-Run in the build container only (the GPU box has no /root/reference):
-    python tests/golden/make_golden.py
+Needs a checkout of the reference:
+    MEGA_NERF_REFERENCE=<path> python tests/golden/make_golden.py
 The reference has no tests or golden vectors of its own (SURVEY.md §4); these fixtures are what
 pins the oracle (oracle/mn_oracle.py) and, through it, the CUDA path.
 """
@@ -19,7 +19,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tests'))
-REF = os.environ.get('MEGA_NERF_REFERENCE', '/root/reference')
+REF = os.environ['MEGA_NERF_REFERENCE']     # a checkout of the reference repository
 sys.path.insert(0, REF)
 
 import cases as C  # noqa: E402
@@ -249,8 +249,8 @@ def main():
                                         xsum=C.checksum(rays, idx))
             print(f'render_{rname}: keys={sorted(res)} present={present}')
 
-    torch.save(G, C.GOLDEN_PATH)
-    print(f'wrote {C.GOLDEN_PATH} ({os.path.getsize(C.GOLDEN_PATH) / 1e6:.2f} MB); worst oracle-vs-reference diff {worst:.3e}')
+    C.save_golden(G, C.GOLDEN_PATH)
+    print(f'wrote {C.GOLDEN_PATH}.part*; worst oracle-vs-reference diff {worst:.3e}')
 
 
 if __name__ == '__main__':

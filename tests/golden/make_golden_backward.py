@@ -1,5 +1,5 @@
 """Generate tests/golden/backward_v1.pt: parameter gradients of the UNMODIFIED reference
-(imported read-only from /root/reference) on the seeded cases `GRAD_CASES` of tests/cases.py.
+(imported read-only from the reference checkout) on the seeded cases `GRAD_CASES` of tests/cases.py.
 
 The reference's training step (runner.py:346-378, :265) is `render_rays(..., get_depth=False,
 get_depth_variance=True, get_bg_fg_rgb=False)` followed by `loss.backward()`; here the loss is
@@ -7,7 +7,7 @@ sum_k sum(results[k] * cotangent[k]) over the differentiable outputs with seeded
 modules are in eval() mode (no jitter / sigma noise: those only add random inputs, the gradient
 arithmetic is identical) and gradients are read from `param.grad`.
 
-Run in the build container only:    python tests/golden/make_golden_backward.py
+Needs a checkout of the reference:    MEGA_NERF_REFERENCE=<path> python tests/golden/make_golden_backward.py
 It also asserts that the oracle's autograd (oracle/mn_oracle.py::render_grads) agrees.
 """
 from __future__ import annotations
@@ -73,8 +73,8 @@ def main():
                        xsum=C.checksum(rays, idx, *cot.values()))
         nz = sum(int((g.abs() > 0).any()) for sub in gn for g in sub.values())
         print(f'{name}: keys={sorted(res)}  non-zero grad tensors {nz}/{sum(len(s) for s in gn)}')
-    torch.save(G, C.GRAD_GOLDEN_PATH)
-    print(f'wrote {C.GRAD_GOLDEN_PATH} ({os.path.getsize(C.GRAD_GOLDEN_PATH) / 1e6:.2f} MB); '
+    C.save_golden(G, C.GRAD_GOLDEN_PATH)
+    print(f'wrote {C.GRAD_GOLDEN_PATH}.part*; '
           f'worst oracle-vs-reference gradient diff {worst:.3e}')
 
 

@@ -1,7 +1,7 @@
 """Generate tests/golden/train_mode_v1.pt: the UNMODIFIED reference in train() mode (stratified jitter, density noise,
 random inverse-CDF draws - rendering.py:83,294,321,511) under a fixed torch seed, forward results for several cases and
 parameter gradients for one.  The oracle must consume the global RNG in exactly the reference's order to reproduce them.
-Run in the build container only:    python tests/golden/make_golden_train_mode.py"""
+Needs a checkout of the reference:    MEGA_NERF_REFERENCE=<path> python tests/golden/make_golden_train_mode.py"""
 from __future__ import annotations
 
 import dataclasses

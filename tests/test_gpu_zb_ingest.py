@@ -17,7 +17,7 @@ def test_container_model_matches_oracle():
     m = M()
     m.set_precision('fp32')
     fg, bg, _ = C.container_nets()
-    hp = C.container_hparams(container_path=C.CONTAINER_PATH)
+    hp = C.container_hparams(container_path=C.container_path())
     net = m.get_nerf(hp, 10).to(DEV).eval().requires_grad_(False)
     bnet = m.get_bg_nerf(hp, 10).to(DEV).eval().requires_grad_(False)
     x = C.mega_rows(fg, 500, 77)
@@ -31,14 +31,14 @@ def test_container_render_with_background():
     m = M()
     m.set_precision('fp32')
     fg, bg, _ = C.container_nets()
-    hp = C.container_hparams(container_path=C.CONTAINER_PATH)
+    hp = C.container_hparams(container_path=C.container_path())
     net = m.get_nerf(hp, 10).to(DEV).eval().requires_grad_(False)
     bnet = m.get_bg_nerf(hp, 10).to(DEV).eval().requires_grad_(False)
     rays = O.synthetic_rays(40, seed=4, far=1e5)
     rays[::2, 7] = 0.4
     idx = O.synthetic_indices(40, 10)
     center, radius = torch.tensor([0.05, -0.02, 0.03]), torch.tensor([0.8, 0.9, 1.0])
-    opts = O.RenderOpts(coarse_samples=32, fine_samples=32, container_path=C.CONTAINER_PATH)
+    opts = O.RenderOpts(coarse_samples=32, fine_samples=32, container_path=C.container_path())
     with torch.inference_mode():
         want, wp = O.render_rays(fg, bg, rays, idx, opts, center, radius, True, True, True)
         rp = Namespace(**vars(opts), **{k: v for k, v in vars(hp).items() if k not in vars(opts)})

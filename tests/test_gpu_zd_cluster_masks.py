@@ -3,7 +3,7 @@ reference's own masks.
 
 Every float op of the reference is restated with its own rounding (the accumulators of cdist's matmul path are
 bit-identical to an in-order FMA chain), but torch's vectorised CPU `sqrt` is not correctly rounded: it is 1 ulp off
-IEEE `sqrtf` on ~0.6 % of inputs (measured in the build container: 6141 of 1e6 random inputs; numpy's and CUDA's
+IEEE `sqrtf` on ~0.6 % of inputs (measured on the CPU: 6141 of 1e6 random inputs; numpy's and CUDA's
 agree with the correctly rounded value everywhere).  So the distance ratios may differ from the CPU oracle by an ulp
 or two and are compared to 4 ulp; the boolean masks - the actual output - must be identical wherever the ratio is not
 within 1e-6 of the margin, and identical everywhere on the committed reference fixture."""

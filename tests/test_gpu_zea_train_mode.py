@@ -12,7 +12,6 @@ import cases as C
 from test_gpu_parity import DEV, M, product_net, relerr
 from test_gpu_zc_backward import E2E_TOL, E2E_L2, check_param_grads, global_rel_l2
 
-# (first run on a B200 in round 2: all green, see profiles/r2_staging_tests.log)
 pytestmark = pytest.mark.gpu
 
 

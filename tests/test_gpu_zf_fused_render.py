@@ -8,7 +8,6 @@ import torch
 import cases as C
 from test_gpu_parity import DEV, M, product_net
 
-# (first run on a B200 in round 2: all green, see profiles/r2_staging_tests.log)
 pytestmark = pytest.mark.gpu
 
 

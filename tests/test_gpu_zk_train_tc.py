@@ -1,14 +1,13 @@
 """GPU: the tensor-core training path (`set_train_precision('tc_f16')`: recording forward + data gradients + weight
-gradients on tcgen05, SURVEY.md §8f-1) against the fp32 CUDA-core path of the same library (which
+gradients on the tensor cores (wgmma), SURVEY.md §8f-1) against the fp32 CUDA-core path of the same library (which
 tests/test_gpu_zc_backward.py pins to the reference's own parameter gradients).
 
 Tolerances: the forward equals the tc_f16 inference kernel (same arithmetic); gradients are a 16-bit computation
 (fp16 operands in all three GEMM families, ReLU masks from an fp16 forward) - the regime the reference itself trains in on
 a GPU under autocast.  scripts/bwd_precision_study.py (CPU) puts such a backward at 1-2 % of the whole gradient vector and
-up to ~1e-1 of a tensor's max for the layer-0 weights.  Measured on B200 (first run): whole-vector relative L2 6.6e-4 ... 1.9e-3
-for one sub-module on 640 - 4099 rows, 1.1e-2 for the 8-sub-module mixtures on 3000 rows and for a 48-ray render_rays step;
-worst single tensor 0.6 % ... 25 % of its max (sub-modules that see only a few dozen rows of a small batch: ReLU masks of an
-fp16 forward flip on individual rows).  Bounds: TC_L2 on the whole vector, TC_TENSOR per tensor."""
+up to ~1e-1 of a tensor's max for the layer-0 weights; single tensors of sub-modules that see only a few dozen rows of a
+small batch can be tens of % of their max off (ReLU masks of an fp16 forward flip on individual rows).  Bounds: TC_L2 on the
+whole vector, TC_TENSOR per tensor."""
 from argparse import Namespace
 
 import pytest

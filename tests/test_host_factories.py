@@ -71,7 +71,7 @@ def test_container_ingestion():
     """container_v1.pt was written by the reference's own MegaNeRFContainer + torch.jit.script."""
     m = M()
     fg, bg, cents = C.container_nets()
-    hp = C.container_hparams(container_path=C.CONTAINER_PATH)
+    hp = C.container_hparams(container_path=C.container_path())
     net, bnet = m.get_nerf(hp, 10), m.get_bg_nerf(hp, 10)
     for got, want, real in ((net, fg, False), (bnet, bg, True)):
         assert isinstance(got, m.MegaNeRF) and len(got.sub_modules) == 4

@@ -1,7 +1,8 @@
-"""CPU: the barrier protocol of the default inference MLP kernel (csrc/mn_mlp_tp.cuh) in a discrete-event model driven by the
-kernel's real role tables (tests/tp_protocol_sim.py): no deadlock and no stale read - ring stages, accumulators, A operands -
-under randomised timing, for every network shape the parity tests use, full and sigma_only calls, odd tile counts and the
-smallest ring the launcher accepts.  A ring that cannot hold a block must be reported as a deadlock (the model can fail)."""
+"""CPU: the barrier protocol of the tensor-core MLP kernel (csrc/mn_mlp_wg.cuh) in a discrete-event model driven by the kernel's
+real stage program (tests/tp_protocol_sim.py): no deadlock and no stale read - ring stages, feature buffer - under randomised
+timing, for every network shape the parity tests use, full and sigma_only calls, odd and even tile counts per CTA (the barrier
+phases wrap differently) and the smallest ring the launcher accepts.  A ring too small for the stages a warpgroup keeps in
+flight must be reported as a deadlock (the model can fail)."""
 import pytest
 
 import tp_protocol_sim as S
@@ -11,30 +12,33 @@ from test_tp_program import SHAPES, desc, program
 @pytest.mark.parametrize('name', sorted(SHAPES))
 @pytest.mark.parametrize('odd_tail', [False, True])
 def test_no_deadlock_no_stale_read(name, odd_tail):
-    rc, prog, loads, info = program(desc(**SHAPES[name]))
+    rc, prog, prog_t, info = program(desc(**SHAPES[name]))
     assert rc == 0
-    n_prog_t, n_loads_t, stages = info[1], info[3], info[5]
-    for seed in range(4):
-        S.simulate(prog, loads, stages, n_pairs=3, odd_tail=odd_tail, seed=seed)
-    S.simulate(prog, loads, 8, n_pairs=3, odd_tail=odd_tail, seed=11)                       # smallest ring the launcher accepts
-    S.simulate(prog[:n_prog_t], loads[:n_loads_t], stages, n_pairs=3, odd_tail=odd_tail, seed=5)      # sigma_only: trunk prefix
+    stages = info[3]
+    n_tiles = 3 if odd_tail else 4
+    for seed in range(3):
+        S.simulate(prog, stages, n_tiles=n_tiles, seed=seed)
+    S.simulate(prog, 2, n_tiles=n_tiles, seed=11)                       # smallest ring the launcher accepts
+    S.simulate(prog_t, stages, n_tiles=n_tiles, seed=5)                 # sigma_only: trunk prefix
 
 
 def test_model_reports_a_ring_smaller_than_a_block():
-    rc, prog, loads, info = program(desc())
-    assert rc == 0 and max((z >> 12) & 0xF for _, _, z, _ in prog) == 5
+    """A warpgroup releases a ring stage only after issuing the next stage's MMAs, so it holds two stages at a time: a
+    one-stage ring must deadlock in the model (the launcher requires at least two)."""
+    rc, prog, prog_t, info = program(desc())
+    assert rc == 0 and info[3] >= 2
     with pytest.raises(S.Deadlock):
-        S.simulate(prog, loads, 4, n_pairs=2, odd_tail=False, seed=0)
+        S.simulate(prog, 1, n_tiles=2, seed=0)
 
 
 def test_model_reports_a_missing_release():
-    """Dropping the second release of a ring stage when the pair has one tile (what the odd-tail path of the issuer adds) starves
-    the producer: the model must notice."""
-    rc, prog, loads, info = program(desc())
-    orig = S.MBar.arrive
+    """Dropping the second warpgroup's release of the feature buffer starves the producer at the next feature segment: the model
+    must notice."""
+    rc, prog, prog_t, info = program(desc())
+    orig = S.release
     try:
-        S.MBar.arrive = lambda self, n=1: orig(self, 1)
+        S.release = lambda bar, who: None if who == ('xa', 1) else orig(bar, who)
         with pytest.raises(S.Deadlock):
-            S.simulate(prog, loads, info[5], n_pairs=2, odd_tail=True, seed=0)
+            S.simulate(prog, info[3], n_tiles=2, seed=0)
     finally:
-        S.MBar.arrive = orig
+        S.release = orig

@@ -1,19 +1,16 @@
-"""Discrete-event model of the barrier protocol of the default inference MLP kernel (csrc/mn_mlp_tp.cuh), driven by the REAL role
-tables (mn_debug_tp_program).  Four actors - TMA producer, the two MMA issuers, the epilogue warps (in lockstep) - exchange the
-kernel's mbarriers (full / empty per ring stage, acc_full / d_free / a_ready per tile slot, the issue token); every action takes
-a random time, so many seeds explore many interleavings.  Independent of the barriers, the model tracks WHAT each resource holds
-(which load a ring stage contains, which accumulator half a tile slot's TMEM columns hold and whether it was drained, which
-GEMM's output the A operand is) and asserts that every read sees what the kernel's arithmetic needs.  A deadlock (all actors
-blocked, nothing in flight) or a stale read fails the test.  Test infrastructure only.
-
-With a `timing` dict (clock cycles, see scripts/tp_pipeline_model.py) the same model runs deterministically with a shared tensor
-pipe and a wake-up latency per barrier hand-off, and reports where the time goes - a what-if tool for the kernel's dependency ring,
-calibrated against the ncu captures under profiles/."""
-import collections
+"""Discrete-event model of the barrier protocol of the tensor-core MLP kernel (csrc/mn_mlp_wg.cuh), driven by the kernel's REAL
+stage program (mn_debug_tp_program).  Three actors - the producer thread and the two consumer warpgroups - exchange the kernel's
+mbarriers (full / empty per ring stage, xa_full / xa_empty of the feature buffer); copies land and warpgroup MMAs complete after
+random times, so many seeds explore many interleavings.  A consumer releases a ring stage the way the kernel does: after the
+MMAs of the NEXT stage are issued and `wgmma.wait_group 1` says the stage's own MMAs have completed; at the end of a feature
+segment and of an accumulator it waits for all of them.  Independent of the barriers, the model tracks WHAT each buffer holds
+(which program entry of which tile a ring stage contains, which feature segment the feature buffer holds, how many unfinished
+MMAs read them) and asserts that every MMA reads what the kernel's arithmetic needs and that no copy overwrites a buffer an MMA
+still reads.  A deadlock (every actor blocked, nothing in flight) raises Deadlock.  Test infrastructure only."""
 import heapq
 import random
 
-TF_FIRST, TF_LAST, TF_FROM_X, TF_WAIT_A = 2, 4, 8, 16
+WS_FROM_X, WS_X_FIRST, WS_X_LAST, WS_LO, WS_CHUNK_FIRST, WS_CHUNK_LAST = 1, 2, 4, 8, 16, 32
 
 
 class MBar:
@@ -36,206 +33,149 @@ class Deadlock(AssertionError):
     pass
 
 
-def simulate(prog, loads, n_stages, n_pairs, odd_tail, seed=0, max_events=2_000_000, timing=None, stats=None):
-    """prog / loads: the tables (issuer entries (x, idesc, z, code), producer entries).  odd_tail: the last pair has one tile."""
+def release(bar, who):
+    """One consumer warpgroup's arrival on an `empty` barrier (`who` = ('stage' | 'xa', warpgroup)); tests replace it to model a
+    missing release."""
+    bar.arrive()
+
+
+def simulate(prog, n_stages, n_tiles, seed=0, max_steps=5_000_000):
+    """prog: the stage program of one tile (entries as returned by tests/test_tp_program.py::program)."""
     rnd = random.Random(seed)
     full = [MBar(1, 'full') for _ in range(n_stages)]
     empty = [MBar(2, 'empty') for _ in range(n_stages)]
-    acc_full, d_free, a_ready = [MBar(1, 'acc_full'), MBar(1, 'acc_full')], [MBar(16, 'd_free'), MBar(16, 'd_free')], [MBar(16, 'a_ready'), MBar(16, 'a_ready')]
-    turn = [MBar(1, 'token'), MBar(1, 'token')]
-    T = timing
-    pipe_free = [0.0]                                # timing mode: the tensor pipe executes blocks in issue order
-    if stats is not None:
-        stats.update(tensor_busy=0.0, wait=collections.defaultdict(float))
-    stage_holds = [None] * n_stages                  # (pair, load index) a ring stage contains
-    acc = [dict(state='free', what=None), dict(state='free', what=None)]      # accumulator of a tile slot
-    a_op = [None, None]                              # (pair, gemm) whose output the A operand of a slot holds
-    a_readers = [0, 0]                               # issued, not yet completed blocks that read a slot's A operand
-    stage_readers = [0] * n_stages                   # ... that read a ring stage
-    n_gemm = max(code for _, _, _, code in prog) // 2 + 1
-    halves = {gi: max(code for _, _, _, code in prog if code // 2 == gi) % 2 + 1 for gi in range(n_gemm)}
-    reads_a = {code // 2 for _, _, z, code in prog if not ((z >> 20) & TF_FROM_X)}
+    xa_full, xa_empty = MBar(1, 'xa_full'), MBar(2, 'xa_empty')
+    stage_holds = [None] * n_stages              # (tile, entry) a ring stage contains
+    stage_readers = [0] * n_stages               # issued, unfinished MMAs that read a ring stage
+    xa = dict(holds=None, readers=0)             # (tile, entry of the segment's first stage), unfinished MMAs reading it
+    seg_of = {}
+    cur = None
+    for i, e in enumerate(prog):
+        if e['flags'] & WS_X_FIRST:
+            cur = i
+        if e['flags'] & WS_FROM_X:
+            seg_of[i] = cur
     events, now, seq = [], [0.0], [0]
-    in_flight = [0]
 
     def later(dt, fn):
         seq[0] += 1
-        in_flight[0] += 1
         heapq.heappush(events, (now[0] + dt, seq[0], fn))
 
-    def valid1(pr):
-        return not (odd_tail and pr == n_pairs - 1)
-
-    # ---- actors are generators yielding either ('wait', barrier, parity) or ('sleep', dt)
+    # ---- actors are generators yielding a condition (callable) to wait for, or a float to sleep
     def producer():
-        stage, phase = 0, 0
-        for pr in range(n_pairs):
-            for li in range(len(loads)):
-                yield ('wait', empty[stage], phase ^ 1)
-                s = stage
+        stage, phase, xphase = 0, 0, 0
+        for tile in range(n_tiles):
+            for i, e in enumerate(prog):
+                if e['flags'] & WS_X_FIRST:
+                    yield lambda p=xphase: xa_empty.passed(p ^ 1)
+                    assert xa['readers'] == 0, f'feature copy issued under {xa["readers"]} unfinished MMA(s)'
 
-                def land(s=s, pr=pr, li=li):
-                    assert stage_readers[s] == 0, f'TMA overwrites ring stage {s} under {stage_readers[s]} unfinished block(s)'
-                    stage_holds[s] = (pr, li)
+                    def land_x(tile=tile, i=i):
+                        assert xa['readers'] == 0, 'feature copy lands under an unfinished MMA'
+                        xa['holds'] = (tile, i)
+                        xa_full.arrive()
+                    later(rnd.uniform(0.5, 3.0), land_x)
+                    xphase ^= 1
+                yield lambda s=stage, p=phase: empty[s].passed(p ^ 1)
+                assert stage_readers[stage] == 0, f'copy into ring stage {stage} issued under an unfinished MMA'
+
+                def land(s=stage, tile=tile, i=i):
+                    assert stage_readers[s] == 0, f'copy lands in ring stage {s} under an unfinished MMA'
+                    stage_holds[s] = (tile, i)
                     full[s].arrive()
-                later(T['tma'] if T else rnd.uniform(0.2, 3.0), land)           # TMA in flight
+                later(rnd.uniform(0.5, 3.0), land)
                 stage += 1
                 if stage == n_stages:
                     stage, phase = 0, phase ^ 1
-                yield ('sleep', T['prod_stage'] if T else rnd.uniform(0.05, 0.3))
+                yield rnd.uniform(0.0, 0.3)
 
-    def issuer(sl):
-        stage, phase, dph, aph = 0, 0, 0, 0
-        tph = 0 if sl else 1
-        done_at = [0.0]                                   # completion time of this issuer's last MMA (commits are in order)
-        for pr in range(n_pairs):
-            v1 = valid1(pr)
-            if sl and not v1:
+    def consumer(wg):
+        stage, phase, xphase = 0, 0, 0
+        groups = []                                  # per committed group: [unfinished flag]
+        last_done = [0.0]                            # completion time of the most recently issued group
+
+        def pending():
+            return sum(1 for g in groups if g[0])
+        for tile in range(n_tiles):
+            prev = -1
+            for i, e in enumerate(prog):
+                if e['flags'] & WS_X_FIRST:
+                    yield lambda p=xphase: xa_full.passed(p)
+                    xphase ^= 1
+                yield lambda s=stage, p=phase: full[s].passed(p)
+                assert stage_holds[stage] == (tile, i), f'warpgroup {wg} reads ring stage {stage} = {stage_holds[stage]}, needs {(tile, i)}'
+                fx = bool(e['flags'] & WS_FROM_X)
+                if fx:
+                    assert xa['holds'] == (tile, seg_of[i]), f'warpgroup {wg} reads feature segment {xa["holds"]}, needs {(tile, seg_of[i])}'
+                stage_readers[stage] += 1
+                xa['readers'] += fx
+                g = [True]
+                groups.append(g)
+
+                def done(g=g, s=stage, fx=fx):
+                    g[0] = False
+                    stage_readers[s] -= 1
+                    xa['readers'] -= fx
+                # a warpgroup's MMA groups complete in issue order
+                last_done[0] = max(last_done[0], now[0]) + rnd.uniform(1.0, 4.0) * e['kc'] / 32
+                later(last_done[0] - now[0], done)
+                if prev >= 0:
+                    yield lambda: pending() <= 1                 # wgmma.wait_group 1
+                    release(empty[prev], ('stage', wg))
+                prev = stage
+                stage += 1
+                if stage == n_stages:
+                    stage, phase = 0, phase ^ 1
+                if e['flags'] & WS_X_LAST:
+                    yield lambda: pending() == 0                 # wgmma.wait_group 0
+                    release(empty[prev], ('stage', wg))
+                    release(xa_empty, ('xa', wg))
+                    prev = -1
+                if e['flags'] & WS_CHUNK_LAST:
+                    yield lambda: pending() == 0
+                    if prev >= 0:
+                        release(empty[prev], ('stage', wg))
+                    prev = -1
+                    yield rnd.uniform(0.5, 4.0)                  # epilogue
+                groups[:] = [g for g in groups if g[0]]
+
+    actors = [producer(), consumer(0), consumer(1)]
+    waiting = [None] * len(actors)                   # current condition of each actor; 'sleep' while a wake-up is queued
+    done_ = [False] * len(actors)
+
+    def step(k):
+        """Advance actor k as far as it can go now."""
+        while not done_[k]:
+            w = waiting[k]
+            if w == 'sleep':
                 return
-            li = 0
-            for x, idesc, z, code in prog:
-                ns, fl = (z >> 12) & 0xF, z >> 20
-                gi, h = code // 2, code % 2
-                n_mma = ns if (fl & TF_FROM_X) else 4 * (ns - 1) + ((z >> 16) & 0xF)
-                if T:
-                    yield ('sleep', T['decode'])            # table entry, flags, operand arithmetic
-                if fl & TF_FIRST:
-                    yield ('wait', d_free[sl], dph ^ 1)
-                    dph ^= 1
-                if fl & TF_WAIT_A:
-                    yield ('wait', a_ready[sl], aph)
-                    aph ^= 1
-                blk = []
-                for _ in range(ns):
-                    yield ('wait', full[stage], phase)
-                    blk.append(stage)
-                    stage += 1
-                    if stage == n_stages:
-                        stage, phase = 0, phase ^ 1
-                if v1:
-                    yield ('wait', turn[sl], tph)
-                    tph ^= 1
-                # ---- issue: what the MMAs are about to read / write must be what the arithmetic needs
-                for k, s in enumerate(blk):
-                    assert stage_holds[s] == (pr, li + k), f'slot {sl} pair {pr} block {code}: stage {s} holds {stage_holds[s]}, wants load {li + k}'
-                if fl & TF_FIRST:
-                    assert acc[sl]['state'] == 'free', f'slot {sl} pair {pr} block {code}: accumulator not drained ({acc[sl]})'
-                    acc[sl].update(state='accumulating', what=(pr, gi, h))
-                else:
-                    assert acc[sl] == dict(state='accumulating', what=(pr, gi, h)), f'slot {sl}: accumulates into {acc[sl]}'
-                if not (fl & TF_FROM_X):
-                    assert a_op[sl] == (pr, gi - 1), f'slot {sl} pair {pr} gemm {gi}: A operand holds {a_op[sl]}'
-                li += ns
-                reads_a_op = not (fl & TF_FROM_X)
-                for s in blk:
-                    stage_readers[s] += 1
-                a_readers[sl] += reads_a_op
-                t_issue0 = now[0]
-                yield ('sleep', T['issue_fixed'] + T['issue_mma'] * n_mma if T else rnd.uniform(0.1, 0.6))          # the issue sequence itself
-                if T:
-                    # the pipe starts on the block's first MMA soon after the sequence begins and cannot finish before it ends
-                    start = max(pipe_free[0], t_issue0 + T['first_mma'])
-                    pipe_free[0] = max(start + n_mma * T['mma'], now[0])
-                    done_at[0] = pipe_free[0] + T['commit']
-                    if stats is not None:
-                        stats['tensor_busy'] += n_mma * T['mma']
-                else:
-                    done_at[0] = max(done_at[0], now[0]) + rnd.uniform(0.5, 2.0) * ns     # the tensor pipe executes the block
-
-                def complete(blk=tuple(blk), last=bool(fl & TF_LAST), sl=sl, what=(pr, gi, h), twice=not v1, reads_a_op=reads_a_op):
-                    a_readers[sl] -= reads_a_op
-                    for s in blk:
-                        stage_readers[s] -= 1
-                        empty[s].arrive(2 if twice else 1)
-                    if last:
-                        assert acc[sl]['what'] == what
-                        acc[sl]['state'] = 'complete'
-                        acc_full[sl].arrive()
-                later(done_at[0] - now[0], complete)
-                if v1:
-                    turn[sl ^ 1].arrive()
-
-    def epilogue():
-        aph = [0, 0]
-        for pr in range(n_pairs):
-            slots = [0, 1] if valid1(pr) else [0]
-            for gi in range(n_gemm):
-                for h in range(halves[gi]):
-                    for sl in slots:
-                        yield ('wait', acc_full[sl], aph[sl])
-                        aph[sl] ^= 1
-                        assert acc[sl] == dict(state='complete', what=(pr, gi, h)), f'epilogue pair {pr} gemm {gi}.{h} slot {sl}: {acc[sl]}'
-                        last_h = h == halves[gi] - 1
-                        yield ('sleep', T['ld'] if T else rnd.uniform(0.1, 0.5))      # tcgen05.ld
-                        if T and (last_h or T.get('d_free_late')):
-                            yield ('sleep', T['math'] / 2)          # the second load completes under the first piece's arithmetic
-                        acc[sl].update(state='free', what=None)
-                        d_free[sl].arrive(16)
-                        if T:
-                            yield ('sleep', T['math'] / 2 if (last_h or T.get('d_free_late')) else T['math'])
-                            if last_h and gi in _publishers:
-                                yield ('sleep', T['st'])            # tcgen05.st + wait::st + fence
-                        else:
-                            yield ('sleep', rnd.uniform(0.1, 1.0))      # arithmetic
-                        if h == halves[gi] - 1 and gi in _publishers:
-                            assert a_readers[sl] == 0, f'epilogue overwrites the A operand of slot {sl} under unfinished MMAs'
-                            a_op[sl] = (pr, gi)
-                            a_ready[sl].arrive(16)
-
-    # GEMMs whose output is some later GEMM's A operand (everything but the colour head / a sigma_only call's last trunk layer)
-    _publishers = {g - 1 for g in reads_a if g - 1 >= 0}
-    actors = {'producer': producer(), 'issuer0': issuer(0), 'issuer1': issuer(1), 'epilogue': epilogue()}
-    blocked = {}
-
-    def step(name):
-        gen = actors.get(name)
-        if gen is None:
-            return
-        while True:
+            if w is not None and not w():
+                return
             try:
-                req = next(gen)
+                req = next(actors[k])
             except StopIteration:
-                del actors[name]
+                done_[k] = True
                 return
-            if req[0] == 'sleep':
-                later(req[1], lambda name=name: step(name))
-                return
-            _, bar, parity = req
-            if not bar.passed(parity):
-                blocked[name] = (bar, parity, now[0])
-                return
+            if callable(req):
+                waiting[k] = req
+            else:
+                waiting[k] = 'sleep'
 
-    for name in list(actors):
-        step(name)
-    n_ev = 0
-    while actors:
-        # wake whoever can proceed
-        progressed = False
-        for name, (bar, parity, t0) in list(blocked.items()):
-            if bar.passed(parity):
-                del blocked[name]
-                hop = (T.get('hop_' + name.rstrip('01'), T['hop']) if T else 0.0)      # per-role override: hop_issuer / hop_epilogue / hop_producer
-                if stats is not None:
-                    stats['wait'][(name, bar.name)] += now[0] - t0 + hop
-                if T:
-                    later(hop, lambda name=name: step(name))        # wake-up latency of a barrier hand-off
-                else:
-                    step(name)
-                progressed = True
-        if progressed:
-            continue
+                def wake(k=k):
+                    waiting[k] = None
+                later(req, wake)
+    steps = 0
+    while not all(done_):
+        for k in range(len(actors)):
+            step(k)
+        if all(done_):
+            break
         if not events:
-            raise Deadlock(f'deadlock at t={now[0]:.1f}: blocked {sorted(blocked)}, running {sorted(set(actors) - set(blocked))}')
-        t, _, fn = heapq.heappop(events)
-        now[0] = t
-        in_flight[0] -= 1
-        fn()
-        n_ev += 1
-        assert n_ev < max_events, 'simulation does not terminate'
-    # drain what is still in flight (commits of the last blocks)
-    while events:
+            blocked = [k for k in range(len(actors)) if not done_[k]]
+            raise Deadlock(f'actors {blocked} blocked with nothing in flight at t={now[0]:.1f}')
         t, _, fn = heapq.heappop(events)
         now[0] = t
         fn()
-    assert all(a['state'] == 'free' for a in acc)
-    return now[0]
+        steps += 1
+        if steps > max_steps:
+            raise Deadlock('no progress within the step budget')
