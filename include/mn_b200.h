@@ -321,13 +321,6 @@ int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, co
  * feature-tile bytes, ring-stage bytes, K columns per stage}.  Returns MN_ERR_UNSUPPORTED for shapes only the fp32 kernels
  * run, MN_ERR_WORKSPACE when cap_entries is too small.  Used by tests/test_tp_program.py and tests/tp_protocol_sim.py. */
 int mn_debug_tp_program(const mn_model_desc* desc, unsigned int* table_out, int cap_entries, int* info8);
-/* ---- debug hooks ----------------------------------------------------------------------------------------------------
- * SM clock during the last tensor-core MLP launch, recorded only when the process runs with MN_TC_TRACE=1: out4 = {clock64,
- * globaltimer} at kernel start and end.  mn_debug_read_trace returns the in-kernel event buffer ([2][2048] (tag, globaltimer ns)
- * pairs, counts[2] their numbers, reset != 0 clears them); the current MLP kernel records no events into it.  Both synchronise
- * the device. */
-int mn_debug_read_trace(unsigned long long* out, unsigned int* counts, int reset);
-int mn_debug_read_clock(unsigned long long* out4);
 
 #ifdef __cplusplus
 }

@@ -73,17 +73,13 @@ __global__ void __launch_bounds__(256) pack_ops_kernel(const PackOp* __restrict_
     }
 }
 
-int pack_T(mn_ctx* ctx, const float* src, int N, int K, float* dst, cudaStream_t) {
-    PackOp op{src, dst, nullptr, (long long)N * K, PK_TRANSPOSE, {N, K, 0, 0, 0, 0, 0}};
-    mn_pack_push(ctx, op);
-    return MN_OK;
+void pack_T(mn_ctx* ctx, const float* src, int N, int K, float* dst) {
+    mn_pack_push(ctx, PackOp{src, dst, nullptr, (long long)N * K, PK_TRANSPOSE, {N, K, 0, 0, 0, 0, 0}});
 }
 
-int pack_sub(mn_ctx* ctx, const float* src, int N, int K, int koff, int kw, float* dst, cudaStream_t) {
-    if ((long long)N * kw == 0) return MN_OK;
-    PackOp op{src, dst, nullptr, (long long)N * kw, PK_SUBMATRIX, {N, K, koff, kw, 0, 0, 0}};
-    mn_pack_push(ctx, op);
-    return MN_OK;
+void pack_sub(mn_ctx* ctx, const float* src, int N, int K, int koff, int kw, float* dst) {
+    if ((long long)N * kw == 0) return;
+    mn_pack_push(ctx, PackOp{src, dst, nullptr, (long long)N * kw, PK_SUBMATRIX, {N, K, koff, kw, 0, 0, 0}});
 }
 
 int al4(int x) { return (x + 3) / 4 * 4; }
@@ -353,40 +349,37 @@ int mn_model_set_weights(mn_model* m, int sub, const mn_nerf_weights* w, void* s
     int rc;
     for (int i = 0; i < nd.layers; ++i) {
         if (!w->xyz_w[i] || !w->xyz_b[i]) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_set_weights: missing trunk layer");
-        if ((rc = pack_T(ctx, w->xyz_w[i], nd.L, l.kin[i], P + l.w[i], st))) return rc;
+        pack_T(ctx, w->xyz_w[i], nd.L, l.kin[i], P + l.w[i]);
         if ((rc = copy(P + l.b[i], w->xyz_b[i], nd.L))) return rc;
     }
     if ((rc = copy(P + l.sigma_w, w->sigma_w, nd.L))) return rc;
     if ((rc = copy(P + l.sigma_b, w->sigma_b, 1))) return rc;
     if (nd.has_dir_a) {
         if (!w->final_w || !w->dir_a_w) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_set_weights: missing head");
-        if ((rc = pack_T(ctx, w->final_w, nd.L, nd.L, P + l.final_w, st))) return rc;
+        pack_T(ctx, w->final_w, nd.L, nd.L, P + l.final_w);
         if ((rc = copy(P + l.final_b, w->final_b, nd.L))) return rc;
-        if ((rc = pack_T(ctx, w->dir_a_w, nd.L / 2, nd.L + nd.aux, P + l.dira_w, st))) return rc;
+        pack_T(ctx, w->dir_a_w, nd.L / 2, nd.L + nd.aux, P + l.dira_w);
         if ((rc = copy(P + l.dira_b, w->dir_a_b, nd.L / 2))) return rc;
     }
     if (!w->rgb_w) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_set_weights: missing rgb head");
-    if ((rc = pack_T(ctx, w->rgb_w, nd.rgb_dim, nd.rgb_in, P + l.rgb_w, st))) return rc;
+    pack_T(ctx, w->rgb_w, nd.rgb_dim, nd.rgb_in, P + l.rgb_w);
     if ((rc = copy(P + l.rgb_b, w->rgb_b, nd.rgb_dim))) return rc;
     if (nd.app > 0)
         if ((rc = copy(P + l.emb, w->embedding_a, (size_t)nd.app_count * nd.app))) return rc;
     if (nd.affine) {
         if (!w->affine_w) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_set_weights: missing affine");
-        if ((rc = pack_T(ctx, w->affine_w, 12, nd.app, P + l.aff_w, st))) return rc;
+        pack_T(ctx, w->affine_w, 12, nd.app, P + l.aff_w);
         if ((rc = copy(P + l.aff_b, w->affine_b, 12))) return rc;
     }
     // data-gradient images (BwdLayout): the input columns that carry a gradient, in nn.Linear [out][in] order
     {
         const BwdLayout& bl = m->blay;
         float* Q = m->packed_bwd + (size_t)sub * bl.total;
-        for (int i = 1; i < nd.layers; ++i)
-            if ((rc = pack_sub(ctx, w->xyz_w[i], nd.L, l.kin[i], l.kin[i] - nd.L, nd.L, Q + bl.w[i], st))) return rc;
+        for (int i = 1; i < nd.layers; ++i) pack_sub(ctx, w->xyz_w[i], nd.L, l.kin[i], l.kin[i] - nd.L, nd.L, Q + bl.w[i]);
         if (nd.has_dir_a) {
-            if ((rc = pack_sub(ctx, w->final_w, nd.L, nd.L, 0, nd.L, Q + bl.final_w, st))) return rc;
-            if ((rc = pack_sub(ctx, w->dir_a_w, nd.L / 2, nd.L + nd.aux, 0, nd.L, Q + bl.dira_f, st))) return rc;
-            if (nd.app_in_dira)
-                if ((rc = pack_sub(ctx, w->dir_a_w, nd.L / 2, nd.L + nd.aux, nd.L + nd.in_dir, nd.app, Q + bl.dira_e, st)))
-                    return rc;
+            pack_sub(ctx, w->final_w, nd.L, nd.L, 0, nd.L, Q + bl.final_w);
+            pack_sub(ctx, w->dir_a_w, nd.L / 2, nd.L + nd.aux, 0, nd.L, Q + bl.dira_f);
+            if (nd.app_in_dira) pack_sub(ctx, w->dir_a_w, nd.L / 2, nd.L + nd.aux, nd.L + nd.in_dir, nd.app, Q + bl.dira_e);
         }
     }
     // launch 1: the fp32 layouts; launch 2 (queued by mn_mlp_tc_pack): the fp16 images that read them
@@ -421,9 +414,45 @@ size_t mn_model_workspace_bytes(const mn_model* m, int64_t B, int precision) {
 #define MN_TAPE_HEADER 1024
 static_assert(CNT_TOTAL * sizeof(int) <= MN_TAPE_HEADER, "tape header too small");
 
-static size_t tape_bytes_tc(const mn_model* m, int64_t B);
+// Regions of a training tape, in this order: header, slot_row and slot_w (routed models; slot_w only when blending), then
+// either the fp32 activation tape or the tensor-core records (encoder tiles, activation images, fp32 head blocks).
+struct TapeRegions {
+    int* counters;
+    int* slot_row;
+    float* slot_w;
+    float* act;          // fp32 tape
+    TrainTcTape tc;      // tensor-core tape
+};
 
-// train_tc != 0: recording forward on the tensor cores (precision tc_f16): tape layout of mn_model_tape_bytes_tc
+// Carves the regions of a tape at `base` into *r (base may be null when only the size is wanted) and returns the tape's size.
+static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, TapeRegions* r = nullptr) {
+    const int64_t cap = slot_capacity(m, B);
+    TapeRegions t{};
+    size_t off = 0;
+    auto take = [&](size_t n) -> void* {
+        void* p = base ? (char*)base + off : nullptr;
+        off += mn_align(n);
+        return p;
+    };
+    t.counters = (int*)take(MN_TAPE_HEADER);
+    if (m->d.kind == 2) {
+        t.slot_row = (int*)take((size_t)cap * sizeof(int));
+        if (m->d.boundary_margin > 1.0f) t.slot_w = (float*)take((size_t)cap * sizeof(float));
+    }
+    if (tc) {
+        const int64_t n_tiles = cap / MN_TILE;
+        t.tc.xreg = (unsigned char*)take((size_t)n_tiles * mn_train_tc_x_tile_bytes(m));
+        t.tc.act = (unsigned char*)take((size_t)n_tiles * mn_train_tc_act_tile_bytes(m));
+        t.tc.f32 = (float*)take((size_t)n_tiles * MN_TC_F32_ROWS * MN_TILE * sizeof(float));
+    } else {
+        const int TM = mn_tape_tm(m->nd.L);
+        t.act = (float*)take((size_t)(cap / TM) * m->tape.a_total * TM * sizeof(float));
+    }
+    if (r) *r = t;
+    return off;
+}
+
+// train_tc != 0: recording forward on the tensor cores (precision tc_f16) into the tensor-core tape regions
 static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, int sigma_only,
                               const float* sigma_noise_d, int precision, float* out_d, void* workspace_d,
                               size_t workspace_bytes, void* tape_d, size_t tape_bytes, void* stream, int train_tc = 0) {
@@ -497,14 +526,9 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
     char* ws = (char*)workspace_d;
     auto carve = [&](size_t n) { char* p = ws; ws += mn_align(n); return p; };
     // training forward: the routing tables and the activations outlive the call inside the caller's tape
-    char* tp = (char*)tape_d;
-    auto tcarve = [&](size_t n) { char* p = tp; tp += mn_align(n); return p; };
-    int* tape_counters = nullptr;
-    if (tape_d) {
-        if (tape_bytes < (train_tc ? tape_bytes_tc(m, B) : mn_model_tape_bytes(m, B)))
-            return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward_train: tape too small");
-        tape_counters = (int*)tcarve(MN_TAPE_HEADER);
-    }
+    TapeRegions T{};
+    if (tape_d && tape_bytes < tape_regions(m, B, train_tc != 0, tape_d, &T))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward_train: tape too small");
 
     int rc;
     int* row_slots = nullptr;
@@ -520,12 +544,12 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
             slot_out = (float*)carve((size_t)cap * a.out_cols * sizeof(float));
         }
         if (tape_d) {
-            slot_row = (int*)tcarve((size_t)cap * sizeof(int));
-            if (blend) slot_w = (float*)tcarve((size_t)cap * sizeof(float));
+            slot_row = T.slot_row;
+            slot_w = T.slot_w;
         }
         if ((rc = mn_route_build(ctx, m, src, B, cap, slot_row, slot_w, row_slots, route_scratch, st))) return rc;
         if (tape_d)
-            MN_CUDA(ctx, cudaMemcpyAsync(tape_counters, m->counters_d, CNT_TOTAL * sizeof(int), cudaMemcpyDeviceToDevice, st));
+            MN_CUDA(ctx, cudaMemcpyAsync(T.counters, m->counters_d, CNT_TOTAL * sizeof(int), cudaMemcpyDeviceToDevice, st));
         a.slot_row = slot_row;
         a.slot_w = slot_w;
         a.counters = m->counters_d;
@@ -539,16 +563,12 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
 
     const int64_t n_tiles = cap / MN_TILE;
     if (tape_d && train_tc) {
-        TrainTcTape T;
-        T.xreg = (unsigned char*)tcarve((size_t)n_tiles * mn_train_tc_x_tile_bytes(m));
-        T.act = (unsigned char*)tcarve((size_t)n_tiles * mn_train_tc_act_tile_bytes(m));
-        T.f32 = (float*)tcarve((size_t)n_tiles * 5 * MN_TILE * sizeof(float));
-        if ((rc = mn_mlp_tc_launch_train(ctx, m, a, n_tiles, T, st))) return rc;
+        if ((rc = mn_mlp_tc_launch_train(ctx, m, a, n_tiles, T.tc, st))) return rc;
         if (row_slots) return mn_route_combine(ctx, m, B, row_slots, slot_out, a.out_cols, out_d, st);
         return MN_OK;
     }
     if (tape_d) {
-        a.tape = (float*)tp;
+        a.tape = T.act;
         a.tl = m->tape;
     }
     if (precision == MN_PREC_FP32)
@@ -568,18 +588,7 @@ int mn_model_forward(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, i
 }
 
 // ---- training (SURVEY.md §8f-1) --------------------------------------------------------------------
-size_t mn_model_tape_bytes(const mn_model* m, int64_t B) {
-    if (!m) return 0;
-    const int64_t cap = slot_capacity(m, B);
-    const int TM = mn_tape_tm(m->nd.L);
-    size_t bytes = MN_TAPE_HEADER;
-    if (m->d.kind == 2) {
-        bytes += mn_align((size_t)cap * sizeof(int));
-        if (m->d.boundary_margin > 1.0f) bytes += mn_align((size_t)cap * sizeof(float));
-    }
-    bytes += mn_align((size_t)(cap / TM) * m->tape.a_total * TM * sizeof(float));
-    return bytes;
-}
+size_t mn_model_tape_bytes(const mn_model* m, int64_t B) { return m ? tape_regions(m, B, false, nullptr) : 0; }
 
 int mn_model_forward_train(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse,
                            const float* sigma_noise_d, float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d,
@@ -613,24 +622,15 @@ int mn_model_param_offsets(const mn_model* m, int64_t* out, int n) {
     return MN_OK;
 }
 
-int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const float* grad_out_d, const void* tape_d,
-                      size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream) {
-    if (!ctx || !m || B < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;
-    if (B == 0) return MN_OK;
+// BwdArgs fields common to both backward passes; routed models read the slot mapping and counters the forward pass saved
+// in the tape, the others run every row through one sub-module.
+static BwdArgs bwd_args(const mn_model* m, int64_t B, int use_coarse, const float* grad_out_d, float* param_grads_d,
+                        const TapeRegions& T) {
     const mn_model_desc& d = m->d;
-    if (tape_bytes < mn_model_tape_bytes(m, B)) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward: tape too small");
-    if (!workspace_d || workspace_bytes < mn_model_backward_workspace_bytes(m, B))
-        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward: workspace too small");
-    const int64_t cap = slot_capacity(m, B);
-    const char* tp = (const char*)tape_d;
-    auto tcarve = [&](size_t n) { const char* p = tp; tp += mn_align(n); return p; };
-    const int* counters = (const int*)tcarve(MN_TAPE_HEADER);
-
     BwdArgs a{};
     a.nd = m->nd;
     a.lay = m->lay;
     a.blay = m->blay;
-    a.tl = m->tape;
     a.packed = m->packed;
     a.packed_bwd = m->packed_bwd;
     a.n_sub = d.n_sub;
@@ -639,36 +639,36 @@ int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const
     a.out_cols = m->nd.rgb_dim + 1;
     a.gw = param_grads_d;
     if (d.kind == 2) {
-        a.slot_row = (const int*)tcarve((size_t)cap * sizeof(int));
-        if (d.boundary_margin > 1.0f) a.slot_w = (const float*)tcarve((size_t)cap * sizeof(float));
-        a.counters = counters;
-        a.B = cap;
+        a.slot_row = T.slot_row;
+        a.slot_w = T.slot_w;
+        a.counters = T.counters;
+        a.B = slot_capacity(m, B);
     } else {
         a.fixed_sub = (d.kind == 1) ? (use_coarse ? 0 : 1) : 0;
     }
-    a.act = (const float*)tp;
+    return a;
+}
+
+int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const float* grad_out_d, const void* tape_d,
+                      size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream) {
+    if (!ctx || !m || B < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;
+    if (B == 0) return MN_OK;
+    TapeRegions T;
+    if (tape_bytes < tape_regions(m, B, false, const_cast<void*>(tape_d), &T))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward: tape too small");
+    if (!workspace_d || workspace_bytes < mn_model_backward_workspace_bytes(m, B))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward: workspace too small");
+    BwdArgs a = bwd_args(m, B, use_coarse, grad_out_d, param_grads_d, T);
+    a.tl = m->tape;
+    a.act = T.act;
     a.grad = (float*)workspace_d;
-    return mn_mlp_bwd_launch(ctx, a, cap / MN_TILE, (cudaStream_t)stream);
+    return mn_mlp_bwd_launch(ctx, a, slot_capacity(m, B) / MN_TILE, (cudaStream_t)stream);
 }
 
 // ---- tensor-core training path (precision tc_f16 for the recording forward and the backward pass) ----------------
-static size_t tape_bytes_tc(const mn_model* m, int64_t B) {
-    const int64_t cap = slot_capacity(m, B);
-    const int64_t n_tiles = cap / MN_TILE;
-    size_t bytes = MN_TAPE_HEADER;
-    if (m->d.kind == 2) {
-        bytes += mn_align((size_t)cap * sizeof(int));
-        if (m->d.boundary_margin > 1.0f) bytes += mn_align((size_t)cap * sizeof(float));
-    }
-    bytes += mn_align((size_t)n_tiles * mn_train_tc_x_tile_bytes(m));
-    bytes += mn_align((size_t)n_tiles * mn_train_tc_act_tile_bytes(m));
-    bytes += mn_align((size_t)n_tiles * 5 * MN_TILE * sizeof(float));
-    return bytes;
-}
-
 int mn_model_train_tc_supported(const mn_model* m) { return (m && m->train_tc_ok) ? 1 : 0; }
 
-size_t mn_model_tape_bytes_tc(const mn_model* m, int64_t B) { return m ? tape_bytes_tc(m, B) : 0; }
+size_t mn_model_tape_bytes_tc(const mn_model* m, int64_t B) { return m ? tape_regions(m, B, true, nullptr) : 0; }
 
 int mn_model_forward_train_tc(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse,
                               const float* sigma_noise_d, float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d,
@@ -691,38 +691,12 @@ int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, co
     if (!ctx || !m || B < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;
     if (B == 0) return MN_OK;
     if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_model_backward_tc: unsupported network shape");
-    const mn_model_desc& d = m->d;
-    if (tape_bytes < tape_bytes_tc(m, B)) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward_tc: tape too small");
-    const int64_t cap = slot_capacity(m, B);
-    const int64_t n_tiles = cap / MN_TILE;
-    const char* tp = (const char*)tape_d;
-    auto tcarve = [&](size_t n) { const char* p = tp; tp += mn_align(n); return p; };
-    const int* counters = (const int*)tcarve(MN_TAPE_HEADER);
-    BwdArgs a{};
-    a.nd = m->nd;
-    a.lay = m->lay;
-    a.blay = m->blay;
-    a.packed = m->packed;
-    a.packed_bwd = m->packed_bwd;
-    a.n_sub = d.n_sub;
-    a.B = B;
-    a.grad_out = grad_out_d;
+    TapeRegions T;
+    if (tape_bytes < tape_regions(m, B, true, const_cast<void*>(tape_d), &T))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward_tc: tape too small");
+    BwdArgs a = bwd_args(m, B, use_coarse, grad_out_d, param_grads_d, T);
     a.grad_rows = B;
-    a.out_cols = m->nd.rgb_dim + 1;
-    a.gw = param_grads_d;
-    if (d.kind == 2) {
-        a.slot_row = (const int*)tcarve((size_t)cap * sizeof(int));
-        if (d.boundary_margin > 1.0f) a.slot_w = (const float*)tcarve((size_t)cap * sizeof(float));
-        a.counters = counters;
-        a.B = cap;
-    } else {
-        a.fixed_sub = (d.kind == 1) ? (use_coarse ? 0 : 1) : 0;
-    }
-    TrainTcTape T;
-    T.xreg = (unsigned char*)tcarve((size_t)n_tiles * mn_train_tc_x_tile_bytes(m));
-    T.act = (unsigned char*)tcarve((size_t)n_tiles * mn_train_tc_act_tile_bytes(m));
-    T.f32 = (float*)tcarve((size_t)n_tiles * 5 * MN_TILE * sizeof(float));
-    return mn_train_tc_backward(ctx, m, a, n_tiles, T, workspace_d, workspace_bytes, (cudaStream_t)stream);
+    return mn_train_tc_backward(ctx, m, a, slot_capacity(m, B) / MN_TILE, T.tc, workspace_d, workspace_bytes, (cudaStream_t)stream);
 }
 
 int mn_model_last_stats(mn_ctx* ctx, mn_model* m, int64_t* slots, int64_t* tiles, void* stream) {

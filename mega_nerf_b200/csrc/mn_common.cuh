@@ -129,24 +129,6 @@ __device__ __forceinline__ void mn_pe_sincos(float x, int k, float* s, float* c)
     sincosf(x * mn_pow2f(k), s, c);
 }
 
-// Same value, ~4x cheaper when many bands share one coordinate: reduce the argument ONCE in fp64
-// (xp = x/pi, error ~1e-16 relative), then every band is an exact power-of-two scaling, an exact
-// quadrant split (u = n/2 + w, |w| <= 1/4) and a short sincospi polynomial on w.  The angle error of
-// rounding w to fp32 is <= pi * 2^-27 = 2.4e-8 rad, i.e. below the 1-ulp accuracy of the oracle's own sin/cos.
-__device__ __forceinline__ double mn_pe_prescale(float x) { return (double)x * 0.31830988618379067154; }
-__device__ __forceinline__ void mn_pe_sincos_pi(double xp, int k, float* s, float* c) {
-    const double u = scalbn(xp, k);          // 2^k x / pi, exact scaling
-    const double n = rint(2.0 * u);
-    const float w = (float)(u - 0.5 * n);    // exact difference, then one rounding
-    float sw, cw;
-    sincospif(w, &sw, &cw);
-    const int q = (int)((long long)n & 3);
-    const bool swap = q & 1;
-    const float ss = swap ? cw : sw, cc = swap ? sw : cw;
-    *s = (q & 2) ? -ss : ss;                 // q: 0 (s,c) 1 (c,-s) 2 (-s,-c) 3 (-c,s)
-    *c = ((q + 1) & 2) ? -cc : cc;
-}
-
 __device__ __forceinline__ float mn_softplus_shifted(float x) {
     // F.softplus(x - 1, beta=1, threshold=20)   (models/nerf.py:38-39)
     float y = x - 1.0f;
@@ -154,7 +136,3 @@ __device__ __forceinline__ float mn_softplus_shifted(float x) {
 }
 
 __device__ __forceinline__ float mn_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
-
-__device__ __forceinline__ double mn_shfl_up_d(double v, int delta) {
-    return __shfl_up_sync(0xffffffffu, v, delta);
-}

@@ -16,8 +16,6 @@
 // is a multiple of 16 works, and no TMA tensor map is needed (plain 1-D bulk copies).
 #include <cuda_fp16.h>
 
-#include <cstdlib>
-#include <cstring>
 #include <type_traits>
 #include <vector>
 
@@ -25,20 +23,7 @@
 
 namespace {
 
-constexpr int kTileM = 128;
-
-// In-kernel event buffer read by mn_debug_read_trace (the current MLP kernel records no events into it).
-__device__ unsigned long long g_trace[4 * 4096];
-__device__ unsigned int g_trace_n[2];
-// SM clock during the kernel (MN_TC_TRACE=1): thread 0 of CTA 0 stamps (clock64, globaltimer) at kernel start and end.
-__device__ unsigned long long g_clk[4];
-__device__ __forceinline__ void clk_stamp(int on, int which) {
-    if (!(on & 1) || blockIdx.x != 0 || threadIdx.x != 0) return;
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    g_clk[2 * which] = (unsigned long long)clock64();
-    g_clk[2 * which + 1] = t;
-}
+constexpr int kTileM = MN_TILE;
 constexpr int kMaxGemm = 16;
 
 enum { SRC_H = 0, SRC_XPE = 1, SRC_XAUX = 2 };
@@ -55,6 +40,7 @@ struct TcGemm {
     int k[2];        // padded K columns per segment (multiple of 16)
     int w_off;       // byte offset of the weight image inside one precision plane of a sub-module
     int bias_off;    // float offset inside the sub-module's fp32 block
+    int img;         // data-gradient plan: tape image of the output (ReLU mask read from the activation record, dZ written)
     int epi;
 };
 
@@ -209,13 +195,6 @@ __device__ __forceinline__ void tc_emit_rgb(const MlpArgs& m, int sub, int64_t r
 }
 
 // ------------------------------------------------------------------------------------------------
-// weight packing: nn.Linear weight [N_src][K_src] fp32 -> image [K/8][N][8] fp16 (hi) and the residual (lo)
-// ------------------------------------------------------------------------------------------------
-
-// half-major image for the TS kernel: [N-half][K/8][nw][8] fp16 (nw = min(N,128))
-
-
-// ------------------------------------------------------------------------------------------------
 // feature tiles
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int kpe, int kaux, int split,
@@ -229,9 +208,7 @@ __global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int 
     const int64_t slot0 = tile * kTileM;
     const int64_t n_slots = a.counters ? a.counters[CNT_NSLOTS] : a.B;
     if (slot0 >= n_slots) return;
-    const int64_t slot = slot0 + t;
-    int64_t row = -1;
-    if (slot < n_slots) row = a.slot_row ? (int64_t)a.slot_row[slot] : slot;
+    const int64_t row = a.row_of_slot(slot0 + t, n_slots);
     __half* lo_img = img + (size_t)ktot * kTileM;
     auto put = [&](int col, float v) {
         const int o = (col >> 3) * (kTileM * 8) + t * 8 + (col & 7);
@@ -239,17 +216,12 @@ __global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int 
         img[o] = h;
         if (split) lo_img[o] = __float2half_rn(v - __half2float(h));
     };
-    int sub = a.fixed_sub;
-    if (a.counters) {
-        sub = 0;
-        while (sub + 1 < a.n_sub && slot0 >= a.counters[CNT_START + sub + 1]) ++sub;
-    }
+    const int sub = a.sub_of_tile(tile);
     if (row < 0) {
         for (int c = 0; c < ktot; ++c) put(c, 0.0f);
     } else {
         float x[4];
-        double xp[4];
-        for (int j = 0; j < nd.xyz_dim; ++j) { x[j] = a.src.xyz(row, j); put(j, x[j]); xp[j] = mn_pe_prescale(x[j]); }
+        for (int j = 0; j < nd.xyz_dim; ++j) { x[j] = a.src.xyz(row, j); put(j, x[j]); }
         for (int k = 0; k < nd.nf_xyz; ++k)
             for (int j = 0; j < nd.xyz_dim; ++j) {
                 float s, c;
@@ -264,8 +236,7 @@ __global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int 
             if (!a.sigma_only) {
                 if (nd.nf_dir > 0) {
                     float d[3];
-                    double dp[3];
-                    for (int j = 0; j < 3; ++j) { d[j] = a.src.dir(row, j); put(col + j, d[j]); dp[j] = mn_pe_prescale(d[j]); }
+                    for (int j = 0; j < 3; ++j) { d[j] = a.src.dir(row, j); put(col + j, d[j]); }
                     for (int k = 0; k < nd.nf_dir; ++k)
                         for (int j = 0; j < 3; ++j) {
                             float s, c;
@@ -327,9 +298,7 @@ __global__ void __launch_bounds__(kTileM) tc_encode_fast_kernel(const MlpArgs a,
     const int64_t slot0 = tile * kTileM;
     const int64_t n_slots = a.counters ? a.counters[CNT_NSLOTS] : a.B;
     if (slot0 >= n_slots) return;
-    const int64_t slot = slot0 + t;
-    int64_t row = -1;
-    if (slot < n_slots) row = a.slot_row ? (int64_t)a.slot_row[slot] : slot;
+    const int64_t row = a.row_of_slot(slot0 + t, n_slots);
     uint4* out = reinterpret_cast<uint4*>(ximg + tile * (int64_t)(KPE + KAUX) * kTileM) + t;   // + chunk * kTileM
     {
         float v[KPE];
@@ -374,11 +343,7 @@ __global__ void __launch_bounds__(kTileM) tc_encode_fast_kernel(const MlpArgs a,
                 }
             }
             if (APP > 0) {
-                int sub = a.fixed_sub;
-                if (a.counters) {
-                    sub = 0;
-                    while (sub + 1 < a.n_sub && slot0 >= a.counters[CNT_START + sub + 1]) ++sub;
-                }
+                const int sub = a.sub_of_tile(tile);
                 int id = (int)a.src.index(row);
                 id = min(max(id, 0), a.nd.app_count - 1);
                 const float4* e4 = reinterpret_cast<const float4*>(a.packed + (size_t)sub * a.lay.total + a.lay.emb + (size_t)id * APP);
@@ -411,14 +376,13 @@ struct TcArgs {
     const __half* ximg;           // feature tiles (hi plane; lo plane at +x_plane_halves)
     int64_t x_plane_halves;
     int split;                    // 1: three MMA passes (hi*hi + hi*lo + lo*hi)
-    int desc_swap;                // debug: 1 = record the in-kernel timeline (MN_TC_TRACE)
     int64_t n_tiles_cap;
-    // ---- training (tc_f16 training path, mn_train_tc.cuh).  Tapes hold, per 128-slot tile, fp16 tile images in the layout of
-    // the activation buffer ([cols/8][128][8]): activations H_0 .. H_{layers-1}, F (xyz_encoding_final), G (dir_a_encoding).
+    // ---- training (tc_f16 training path, mn_train_tc.cuh).  Per 128-slot tile, records of fp16 tile images (mn_model.cuh,
+    // mn_tc_img_off) and fp32 head blocks.
     unsigned char* tape_act;      // PP_TRAIN_FWD: written;  PP_DGRAD: read (ReLU masks)
-    float* tape_f32;              // per tile [4][128]: sigma pre-activation, rgb (3)     (written / read)
+    float* tape_f32;              // fp32 head blocks [MN_TC_F32_ROWS][128]     (written / read)
     unsigned char* tape_dz;       // PP_DGRAD: gradient images dZ_0 .. dZ_{layers-1}, dZ_final, dZ_dira (same layout, scaled fp16)
-    float* tape_gf32;             // PP_DGRAD: per tile [4][128]: d sigma pre-activation, d rgb pre-activation (3), UNscaled fp32
+    float* tape_gf32;             // PP_DGRAD: head-gradient blocks [MN_TC_G32_ROWS][128], UNscaled fp32
     const float* grad_out;        // PP_DGRAD: [rows][rgb_dim + 1] upstream gradient
     float* emb_sum;               // PP_DGRAD: [n_sub][app_count][L/2] per-image sums of dZ_dira rows (appearance-embedding gradient)
     const float* scale;           // PP_DGRAD: device scalar S (power of two): gradient images hold S * dZ
@@ -498,7 +462,7 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
     const float* Pk = m->packed + (size_t)sub * m->lay.total;
     float* f32 = reinterpret_cast<float*>(base + (size_t)P.plane_bytes * 2);
     auto pack = [&](const TcGemm& g, const float* wt, int n_src, int k_src, int k_real0, int k_pad0, const float* bias,
-                    int n_bias) -> int {
+                    int n_bias) {
         const int K = g.k[0] + (g.nseg > 1 ? g.k[1] : 0);
         const int64_t n = (int64_t)g.n * K;
         __half* hi = reinterpret_cast<__half*>(base + g.w_off);
@@ -507,24 +471,21 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
         if (wide) {
             mn_pack_push(ctx, PackOp{wt, hi, nullptr, (long long)n, PK_TC_HALF, {n_src, k_src, g.n, K, k_real0, k_pad0, g.n < 256 ? g.n : 256}});
             mn_pack_push(ctx, PackOp{bias, f32 + g.bias_off, nullptr, (long long)P.bstride, PK_TC_F32, {n_bias, 0, 0, 0, 0, 0, 0}});
-            return MN_OK;
+            return;
         }
         mn_pack_push(ctx, PackOp{wt, hi, lo, (long long)n, PK_TC_IMAGE, {n_src, k_src, g.n, K, k_real0, k_pad0, 0}});
         mn_pack_push(ctx, PackOp{bias, f32 + g.bias_off, nullptr, 256, PK_TC_F32, {n_bias, 0, 0, 0, 0, 0, 0}});
-        return MN_OK;
     };
-    int rc, gi = 0;
+    int gi = 0;
     for (int i = 0; i < nd.layers; ++i, ++gi) {
         const bool has_pe = (i == 0) || ((nd.skip_mask >> i) & 1);
-        if ((rc = pack(P.g[gi], Pk + m->lay.w[i], nd.L, m->lay.kin[i], has_pe ? nd.in_xyz : 0, has_pe ? P.kpe : 0,
-                       Pk + m->lay.b[i], nd.L)))
-            return rc;
+        pack(P.g[gi], Pk + m->lay.w[i], nd.L, m->lay.kin[i], has_pe ? nd.in_xyz : 0, has_pe ? P.kpe : 0, Pk + m->lay.b[i], nd.L);
     }
     if (nd.has_dir_a) {
-        if ((rc = pack(P.g[gi++], Pk + m->lay.final_w, nd.L, nd.L, 0, 0, Pk + m->lay.final_b, nd.L))) return rc;
-        if ((rc = pack(P.g[gi++], Pk + m->lay.dira_w, nd.L / 2, nd.L + nd.aux, 0, 0, Pk + m->lay.dira_b, nd.L / 2))) return rc;
+        pack(P.g[gi++], Pk + m->lay.final_w, nd.L, nd.L, 0, 0, Pk + m->lay.final_b, nd.L);
+        pack(P.g[gi++], Pk + m->lay.dira_w, nd.L / 2, nd.L + nd.aux, 0, 0, Pk + m->lay.dira_b, nd.L / 2);
     }
-    if ((rc = pack(P.g[gi++], Pk + m->lay.rgb_w, nd.rgb_dim, nd.rgb_in, 0, 0, Pk + m->lay.rgb_b, nd.rgb_dim))) return rc;
+    pack(P.g[gi++], Pk + m->lay.rgb_w, nd.rgb_dim, nd.rgb_in, 0, 0, Pk + m->lay.rgb_b, nd.rgb_dim);
     // sigma_w [L] + sigma_b
     mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + P.sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
     mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + P.sigma_w_off + nd.L, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
@@ -541,15 +502,14 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
         }
         unsigned char* db = (unsigned char*)m->tc_dgrad + (size_t)sub * D.sub_bytes;
         const float* Q = m->packed_bwd + (size_t)sub * m->blay.total;
-        auto packd = [&](const TcGemm& g, const float* wd, int ld) -> int {
+        auto packd = [&](const TcGemm& g, const float* wd, int ld) {
             mn_pack_push(ctx, PackOp{wd, db + g.w_off, nullptr, (long long)g.n * g.k[0], PK_DGRAD, {ld, g.n, g.k[0], 0, 0, 0, 0}});
-            return MN_OK;
         };
         int di = 0;
-        if ((rc = packd(D.g[di++], Q + m->blay.dira_f, nd.L))) return rc;         // [L/2][L]
-        if ((rc = packd(D.g[di++], Q + m->blay.final_w, nd.L))) return rc;        // [L][L]
+        packd(D.g[di++], Q + m->blay.dira_f, nd.L);         // [L/2][L]
+        packd(D.g[di++], Q + m->blay.final_w, nd.L);        // [L][L]
         for (int l = nd.layers - 1; l >= 1; --l)
-            if ((rc = packd(D.g[di++], Q + m->blay.w[l], nd.L))) return rc;       // [L][L]: hidden-part columns of layer l
+            packd(D.g[di++], Q + m->blay.w[l], nd.L);       // [L][L]: hidden-part columns of layer l
         float* df32 = reinterpret_cast<float*>(db + D.f32_off);
         mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, df32, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
         mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, df32 + nd.L, nullptr, (long long)3 * (nd.L / 2), PK_RGBW, {nd.L / 2, 3, 0, 0, 0, 0, 0}});
@@ -558,10 +518,38 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
     return MN_OK;
 }
 
+// Feature tiles of the first n_tiles128 tiles: the specialised encoder for the common network shape, the generic one otherwise.
+static int tc_encode(mn_ctx* ctx, const mn_model* m, const MlpArgs& a, const TcPlan& P, int64_t n_tiles128, int split,
+                     __half* ximg, int64_t plane_halves, cudaStream_t st) {
+    const size_t enc_sm = (size_t)P.x_tile_bytes * (split ? 2 : 1);
+    MN_CUDA(ctx, cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
+    const NetDims& nd = a.nd;
+    const bool fast_shape = !split && nd.xyz_dim == 3 && nd.nf_xyz == 12 && nd.nf_dir == 4 && nd.app == 48 && nd.app_in_dira &&
+                            (m->lay.emb % 4) == 0;
+    if (fast_shape)
+        tc_encode_fast_kernel<3, 12, 4, 48><<<(unsigned)n_tiles128, kTileM, 0, st>>>(a, ximg);
+    else
+        tc_encode_kernel<<<(unsigned)n_tiles128, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split, ximg, plane_halves);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+// TcArgs fields common to the inference and the recording forward: the plan and the model's packed weights.  False when the
+// network shape has no tensor-core plan or the weights are not packed.
+static bool tc_forward_args(const mn_model* m, const MlpArgs& a, int64_t n_tiles128, TcArgs* A) {
+    *A = TcArgs{};
+    if (!build_plan(a.nd, &A->plan) || !m->tc_ready) return false;
+    A->plan.sub_bytes = (int)m->tc_sub_bytes;
+    A->m = a;
+    A->wpack = (const unsigned char*)m->tc_packed;
+    A->n_tiles_cap = n_tiles128;
+    return true;
+}
+
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws, size_t ws_bytes,
                      cudaStream_t st) {
-    TcArgs A{};
-    if (!build_plan(a.nd, &A.plan) || !m->tc_ready)
+    TcArgs A;
+    if (!tc_forward_args(m, a, n_tiles128, &A))
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "tensor-core MLP path covers layer_dim 64..256 (multiple of 64) or 512 and rgb_dim <= 32; "
                        "use precision 'fp32' for this model");
@@ -569,41 +557,19 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "precision 'tc_f16x3' covers layer_dim <= 256; use 'tc_f16' or 'fp32' for the 512-wide network");
     if (n_tiles128 <= 0) return MN_OK;
-    TcPlan& P = A.plan;
+    const TcPlan& P = A.plan;
     const int split = precision == MN_PREC_TC_F16X3 ? 1 : 0;
-    P.sub_bytes = (int)m->tc_sub_bytes;
-    // the packed layout always holds both planes; tell the kernel where the fp32 block is
-    A.m = a;
-    A.wpack = (const unsigned char*)m->tc_packed;
     A.split = split;
-    static int desc_swap = -1;
-    if (desc_swap < 0) {
-        const char* e = getenv("MN_TC_TRACE");
-        desc_swap = e ? atoi(e) : 0;      // bit 0: in-kernel timeline + SM-clock stamp
-    }
-    A.desc_swap = desc_swap;
-    A.n_tiles_cap = n_tiles128;
     const size_t need = mn_mlp_tc_workspace(m, n_tiles128, precision);
     if (ws_bytes < need || !ws) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
     uintptr_t wp = ((uintptr_t)ws + 1023) / 1024 * 1024;
     __half* ximg = reinterpret_cast<__half*>(wp);
     A.ximg = ximg;
     A.x_plane_halves = (int64_t)n_tiles128 * (P.kpe + P.kaux) * kTileM;
-
-
-    const size_t enc_sm = (size_t)P.x_tile_bytes * (split ? 2 : 1);
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
-    const NetDims& ndE = a.nd;
-    const bool fast_shape = !split && ndE.xyz_dim == 3 && ndE.nf_xyz == 12 && ndE.nf_dir == 4 && ndE.app == 48 && ndE.app_in_dira &&
-                            (m->lay.emb % 4) == 0;
-    if (fast_shape)
-        tc_encode_fast_kernel<3, 12, 4, 48><<<(unsigned)n_tiles128, kTileM, 0, st>>>(a, ximg);
-    else
-        tc_encode_kernel<<<(unsigned)n_tiles128, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split, ximg, A.x_plane_halves);
-    MN_LAUNCH_CHECK(ctx);
+    int rc = tc_encode(ctx, m, a, P, n_tiles128, split, ximg, A.x_plane_halves, st);
+    if (rc) return rc;
 
     mn_prof_begin(ctx, st);
-    int rc;
     if (split) rc = wg_launch<PP_INFER, true, false>(ctx, A, n_tiles128, st);
     else if (P.L > 256) rc = wg_launch<PP_INFER, false, true>(ctx, A, n_tiles128, st);
     else rc = wg_launch<PP_INFER, false, false>(ctx, A, n_tiles128, st);
@@ -620,46 +586,35 @@ size_t mn_train_tc_x_tile_bytes(const mn_model* m) {
 }
 size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
     const NetDims& nd = m->nd;
-    return (size_t)(nd.layers + 1) * nd.L * kTileM * 2 + (size_t)(nd.L / 2) * kTileM * 2;
+    return mn_tc_img_off(nd.layers + 1, nd.L) + mn_tc_img_off(1, nd.L / 2);     // ends with G (L/2 columns)
 }
 
 // recording forward: encoder tiles and every layer's activations land in the caller's tape
 int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
-    TcArgs A{};
-    if (!m->train_tc_ok || !build_plan(a.nd, &A.plan) || !m->tc_ready)
+    TcArgs A;
+    if (!m->train_tc_ok || !tc_forward_args(m, a, n_tiles128, &A))
         return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 with a direction / appearance head and rgb_dim 3; use train precision 'fp32'");
     if (n_tiles128 <= 0) return MN_OK;
-    TcPlan& P = A.plan;
-    P.sub_bytes = (int)m->tc_sub_bytes;
-    A.m = a;
-    A.wpack = (const unsigned char*)m->tc_packed;
     A.ximg = reinterpret_cast<const __half*>(tape.xreg);
     A.x_plane_halves = 0;
-    A.n_tiles_cap = n_tiles128;
     A.tape_act = tape.act;
     A.tape_f32 = tape.f32;
     A.act_tile_bytes = (int64_t)mn_train_tc_act_tile_bytes(m);
     A.layers = a.nd.layers;
-    const size_t enc_sm = (size_t)P.x_tile_bytes;
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
-    const NetDims& ndE = a.nd;
-    const bool fast_shape = ndE.xyz_dim == 3 && ndE.nf_xyz == 12 && ndE.nf_dir == 4 && ndE.app == 48 && ndE.app_in_dira && (m->lay.emb % 4) == 0;
-    __half* ximg = reinterpret_cast<__half*>(tape.xreg);
-    if (fast_shape) tc_encode_fast_kernel<3, 12, 4, 48><<<(unsigned)n_tiles128, kTileM, 0, st>>>(a, ximg);
-    else tc_encode_kernel<<<(unsigned)n_tiles128, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, 0, ximg, 0);
-    MN_LAUNCH_CHECK(ctx);
+    int rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st);
+    if (rc) return rc;
     mn_prof_begin(ctx, st);
-    const int rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
+    rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
     mn_prof_end(ctx, st);
     return rc;
 }
 
-// backward workspace: [gradient records][head gradients fp32 [n_tiles][4][128]][embedding sums][scale]
+// backward workspace: [gradient records][head gradients fp32 [n_tiles][MN_TC_G32_ROWS][128]][embedding sums][scale]
 static size_t train_tc_emb_floats(const mn_model* m) {
     return m->nd.app_in_dira ? (size_t)m->d.n_sub * m->nd.app_count * (m->nd.L / 2) : 0;
 }
 size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
-    return mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m)) + mn_align((size_t)n_tiles128 * 4 * kTileM * sizeof(float)) +
+    return mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m)) + mn_align((size_t)n_tiles128 * MN_TC_G32_ROWS * kTileM * sizeof(float)) +
            mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) + 1024;
 }
 
@@ -673,7 +628,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     const size_t act_tile = mn_train_tc_act_tile_bytes(m);
     char* wp = (char*)(((uintptr_t)ws + 255) / 256 * 256);
     unsigned char* dz = (unsigned char*)wp;               wp += mn_align((size_t)n_tiles128 * act_tile);
-    float* gf32 = (float*)wp;                             wp += mn_align((size_t)n_tiles128 * 4 * kTileM * sizeof(float));
+    float* gf32 = (float*)wp;                             wp += mn_align((size_t)n_tiles128 * MN_TC_G32_ROWS * kTileM * sizeof(float));
     float* emb_sum = (float*)wp;                          wp += mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) - 256;
     float* scale = (float*)wp;
     if (train_tc_emb_floats(m)) MN_CUDA(ctx, cudaMemsetAsync(emb_sum, 0, train_tc_emb_floats(m) * sizeof(float), st));
@@ -712,13 +667,13 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     // ---- weight gradients: one item per (Linear input segment, 128-channel output half)
     WgArgs W{};
     const int L = nd.L;
-    const int img_bytes = L * kTileM * 2;
+    auto img = [&](int i) { return (int)mn_tc_img_off(i, L); };
     TcPlan F;
     build_plan(nd, &F);
     int ni = 0;
     auto item = [&](int dz_img, int half, int x_region, int x_off, int n, int n_real, int w_off, int k_in, int in0, int b_off) {
         WgItem& it = W.item[ni++];
-        it.dz_off = dz_img * img_bytes + half * 16 * (kTileM * 16);
+        it.dz_off = img(dz_img) + half * 16 * (kTileM * 16);
         it.x_region = x_region;
         it.x_off = x_off;
         it.n = n;
@@ -734,13 +689,13 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
             if (i == 0) item(i, h, 1, 0, F.kpe, nd.in_xyz, a.lay.w[i], k_in, 0, a.lay.b[i]);
             else if (skip) {
                 item(i, h, 1, 0, F.kpe, nd.in_xyz, a.lay.w[i], k_in, 0, a.lay.b[i]);                       // cat[PE, h]: PE columns first
-                item(i, h, 0, (i - 1) * img_bytes, L, L, a.lay.w[i], k_in, nd.in_xyz, -1);
-            } else item(i, h, 0, (i - 1) * img_bytes, L, L, a.lay.w[i], k_in, 0, a.lay.b[i]);
+                item(i, h, 0, img(i - 1), L, L, a.lay.w[i], k_in, nd.in_xyz, -1);
+            } else item(i, h, 0, img(i - 1), L, L, a.lay.w[i], k_in, 0, a.lay.b[i]);
         }
     }
-    for (int h = 0; h < L / 128; ++h) item(nd.layers, h, 0, (nd.layers - 1) * img_bytes, L, L, a.lay.final_w, L, 0, a.lay.final_b);
+    for (int h = 0; h < L / 128; ++h) item(nd.layers, h, 0, img(nd.layers - 1), L, L, a.lay.final_w, L, 0, a.lay.final_b);
     // dir_a_encoding: L/2 = 128 output channels (one half); input = cat[final (L), dir PE + embedding (aux)]
-    item(nd.layers + 1, 0, 0, nd.layers * img_bytes, L, L, a.lay.dira_w, L + nd.aux, 0, a.lay.dira_b);
+    item(nd.layers + 1, 0, 0, img(nd.layers), L, L, a.lay.dira_w, L + nd.aux, 0, a.lay.dira_b);
     item(nd.layers + 1, 0, 1, (F.kpe / 8) * (kTileM * 16), F.kaux, nd.aux, a.lay.dira_w, L + nd.aux, L, -1);
     if (ni > kWgMaxItems) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: too many weight-gradient items");
     W.n_items = ni;
@@ -793,21 +748,4 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     }
     mn_prof_end(ctx, st);
     return MN_OK;
-}
-
-extern "C" int mn_debug_read_clock(unsigned long long* out4) {
-    cudaDeviceSynchronize();
-    if (out4) cudaMemcpyFromSymbol(out4, g_clk, sizeof(unsigned long long) * 4);
-    return 0;
-}
-
-extern "C" int mn_debug_read_trace(unsigned long long* out, unsigned int* counts, int reset) {
-    cudaDeviceSynchronize();
-    if (out) cudaMemcpyFromSymbol(out, g_trace, sizeof(unsigned long long) * 4 * 4096);
-    if (counts) cudaMemcpyFromSymbol(counts, g_trace_n, sizeof(unsigned int) * 2);
-    if (reset) {
-        unsigned int z[2] = {0, 0};
-        cudaMemcpyToSymbol(g_trace_n, z, sizeof(z));
-    }
-    return 0;
 }

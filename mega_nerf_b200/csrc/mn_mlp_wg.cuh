@@ -192,17 +192,6 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    clk_stamp(A.desc_swap, 0);
-
-    auto sub_of = [&](int64_t tile) -> int {
-        int sub = A.m.fixed_sub;
-        if (A.m.counters) {
-            sub = 0;
-            const int64_t s0 = tile * kTileM;
-            while (sub + 1 < A.m.n_sub && s0 >= A.m.counters[CNT_START + sub + 1]) ++sub;
-        }
-        return sub;
-    };
 
     const int wgi = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);     // warp-uniform role
     if (wgi == 2) {
@@ -212,7 +201,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
             uint32_t phase = 0, xphase = 0;
             const int64_t xtile_bytes = (int64_t)(P.kpe + P.kaux) * kTileM * 2;
             for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                const unsigned char* wsub = A.wpack + (size_t)sub_of(tile) * P.sub_bytes;
+                const unsigned char* wsub = A.wpack + (size_t)A.m.sub_of_tile(tile) * P.sub_bytes;
                 const unsigned char* xtile = reinterpret_cast<const unsigned char*>(A.ximg) + tile * xtile_bytes;
                 for (int gi = 0; gi < n_gemm; ++gi) {
                     const int nch = (P.g[gi].n + 255) >> 8;
@@ -249,7 +238,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
         uint32_t phase = 0, xphase = 0;
 
         for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-            const int sub = sub_of(tile);
+            const int sub = A.m.sub_of_tile(tile);
             if (sub != cur_sub) {
                 // both warpgroups stage the sub-module's fp32 block (it changes a handful of times per launch): epilogue
                 // operands from shared memory instead of dependent global loads between the activation stores
@@ -260,9 +249,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                 cur_sub = sub;
             }
             const int64_t slot_a = tile * kTileM + ra, slot_b = tile * kTileM + rb;
-            int64_t row_a = -1, row_b = -1;
-            if (slot_a < n_slots) row_a = A.m.slot_row ? (int64_t)A.m.slot_row[slot_a] : slot_a;
-            if (slot_b < n_slots) row_b = A.m.slot_row ? (int64_t)A.m.slot_row[slot_b] : slot_b;
+            const int64_t row_a = A.m.row_of_slot(slot_a, n_slots), row_b = A.m.row_of_slot(slot_b, n_slots);
             float sig_a = 0.0f, sig_b = 0.0f;
 
             if (kMode == PP_DGRAD) {
@@ -274,17 +261,17 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                 const float S = *A.scale;
                 const int hr = 64 * wg + (t & 63), part = t >> 6;
                 const int64_t hslot = tile * kTileM + hr;
-                int64_t hrow = -1;
-                if (hslot < n_slots) hrow = A.m.slot_row ? (int64_t)A.m.slot_row[hslot] : hslot;
+                const int64_t hrow = A.m.row_of_slot(hslot, n_slots);
                 const float* Wr = F32 + L;                                  // [3][L/2] rgb weights (fp32 block of the data-gradient plan)
-                const float* tf = A.tape_f32 + (size_t)tile * 5 * kTileM + hr;
+                const float* tf = A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + hr;
                 float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f, g3 = 0.0f;
                 if (hrow >= 0) {
                     const float4 gv = *reinterpret_cast<const float4*>(A.grad_out + hrow * 4);
                     const float bw = A.m.slot_w ? A.m.slot_w[hslot] : 1.0f;
                     g0 = gv.x * bw; g1 = gv.y * bw; g2 = gv.z * bw; g3 = gv.w * bw;
                 }
-                const float c0v = tf[1 * kTileM], c1v = tf[2 * kTileM], c2v = tf[3 * kTileM], pre = tf[0];
+                const float c0v = tf[MN_TC_F32_RGB * kTileM], c1v = tf[(MN_TC_F32_RGB + 1) * kTileM], c2v = tf[(MN_TC_F32_RGB + 2) * kTileM];
+                const float pre = tf[MN_TC_F32_SIGMA * kTileM];
                 const float d0 = (g0 * (1.0f - c0v)) * c0v, d1 = (g1 * (1.0f - c1v)) * c1v, d2 = (g2 * (1.0f - c2v)) * c2v;
                 float dsp;
                 if (A.m.nd.softplus) { const float y = pre - 1.0f; dsp = y > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-y)); }
@@ -292,12 +279,13 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                 const float ds = g3 * dsp;
                 if (part == 0) {
                     DSIG[hr] = ds * S;
-                    float* tg = A.tape_gf32 + (size_t)tile * 4 * kTileM + hr;
-                    tg[0] = ds; tg[1 * kTileM] = d0; tg[2 * kTileM] = d1; tg[3 * kTileM] = d2;
+                    float* tg = A.tape_gf32 + (size_t)tile * MN_TC_G32_ROWS * kTileM + hr;
+                    tg[MN_TC_G32_SIGMA * kTileM] = ds;
+                    tg[MN_TC_G32_RGB * kTileM] = d0; tg[(MN_TC_G32_RGB + 1) * kTileM] = d1; tg[(MN_TC_G32_RGB + 2) * kTileM] = d2;
                 }
-                const int id = (int)tf[4 * kTileM];
-                const unsigned char* gimg = A.tape_act + (size_t)tile * A.act_tile_bytes + (size_t)(A.layers + 1) * L * kTileM * 2;
-                unsigned char* dimg = A.tape_dz + (size_t)tile * A.act_tile_bytes + (size_t)(A.layers + 1) * L * kTileM * 2;
+                const int id = (int)tf[MN_TC_F32_ID * kTileM];
+                const unsigned char* gimg = A.tape_act + (size_t)tile * A.act_tile_bytes + mn_tc_img_off(A.layers + 1, L);
+                unsigned char* dimg = A.tape_dz + (size_t)tile * A.act_tile_bytes + mn_tc_img_off(A.layers + 1, L);
                 const int half = L / 2, per = half / 2;
                 for (int kk = 0; kk < per; kk += 8) {
                     const int k0 = part * per + kk;
@@ -396,9 +384,8 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                         const int cb = ch * 256;
                         if (kMode == PP_DGRAD) {
                             // dH = accumulator (scaled by S) [+ S dsigma x w_sigma] -> ReLU mask from the activation tape -> fp16 ->
-                            // next A operand + gradient tape.  gm.bias_off holds the image index (the mask image and the target image
-                            // coincide: dZ_l = dH_l where H_l > 0).
-                            const size_t ioff = (size_t)tile * A.act_tile_bytes + (size_t)gm.bias_off * L * kTileM * 2;
+                            // next A operand + gradient tape.  The mask image and the target image coincide: dZ_l = dH_l where H_l > 0.
+                            const size_t ioff = (size_t)tile * A.act_tile_bytes + mn_tc_img_off(gm.img, L);
                             const unsigned char* mimg = A.tape_act + ioff;
                             unsigned char* dimg = A.tape_dz + ioff;
                             const float dsa = DSIG[ra], dsb = DSIG[rb];
@@ -459,14 +446,14 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                             if (q4 < 2) {
                                 const int r = q4 ? rb : ra;
                                 const int64_t row = q4 ? row_b : row_a, slot = q4 ? slot_b : slot_a;
-                                float* tr = kMode == PP_TRAIN_FWD ? A.tape_f32 + (size_t)tile * 5 * kTileM + kTileM + r : nullptr;
+                                float* tr = kMode == PP_TRAIN_FWD ? A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + MN_TC_F32_RGB * kTileM + r : nullptr;
                                 if (row >= 0) tc_emit_rgb(A.m, A.m.nd.affine ? sub : 0, row, slot, q4 ? vb : va, bias, q4 ? sig_b : sig_a, tr);
                                 else if (tr) { tr[0] = 0.5f; tr[kTileM] = 0.5f; tr[2 * kTileM] = 0.5f; }
                             }
                             continue;
                         }
                         // training forward: tape image of this GEMM's output (trunk layer gi; then F, then G)
-                        unsigned char* timg = kMode == PP_TRAIN_FWD ? A.tape_act + (size_t)tile * A.act_tile_bytes + (size_t)gi * L * kTileM * 2 : nullptr;
+                        unsigned char* timg = kMode == PP_TRAIN_FWD ? A.tape_act + (size_t)tile * A.act_tile_bytes + mn_tc_img_off(gi, L) : nullptr;
                         const float* bias = F32 + gm.bias_off + cb;
                         const bool relu = gm.epi != EPI_LINEAR;
                         const bool hold = kWide && nch == 2 && ch == 0;
@@ -539,9 +526,9 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                             const int64_t row = q4 ? row_b : row_a, slot = q4 ? slot_b : slot_a;
                             const float s = q4 ? sb : sa, sg = q4 ? sig_b : sig_a;
                             if (kMode == PP_TRAIN_FWD) {
-                                float* tf = A.tape_f32 + (size_t)tile * 5 * kTileM + r;
-                                tf[0] = s;                                                  // pre-activation (with the density noise)
-                                tf[4 * kTileM] = (row >= 0 && A.m.nd.app > 0) ? A.m.src.index(row) : 0.0f;   // image id of the row
+                                float* tf = A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + r;
+                                tf[MN_TC_F32_SIGMA * kTileM] = s;                           // pre-activation (with the density noise)
+                                tf[MN_TC_F32_ID * kTileM] = (row >= 0 && A.m.nd.app > 0) ? A.m.src.index(row) : 0.0f;
                             }
                             if (A.m.sigma_only && row >= 0) {
                                 const int64_t o = (A.m.scatter ? row : slot) * A.m.out_cols;
@@ -560,5 +547,4 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
         }
     }
     __syncthreads();
-    clk_stamp(A.desc_swap, 1);
 }

@@ -5,7 +5,7 @@
 #define MN_MAX_LAYERS 16
 #define MN_MAX_SUB 64
 #define MN_TILE 128     // rows of one tensor-core MLP tile
-#define MN_BUCKET 512   // slot-space bucket alignment: four consecutive 128-row tiles (two ping-pong slots of a CTA pair) never mix sub-modules
+#define MN_BUCKET 512   // alignment of each sub-module's slot range (a multiple of MN_TILE: no tile mixes sub-modules); sets workspace and tape sizes
 
 // Offsets (in floats) of each packed tensor inside one sub-module's fp32 buffer.  All matrices are
 // stored K-major ("transposed": Wt[k][n] = W[n][k]) so that consecutive output channels are contiguous.
@@ -96,6 +96,23 @@ struct MlpArgs {
     int scatter;              // 1: out index = row, 0: out index = slot
     float* tape;              // activation tape (training forward) or NULL
     TapeLayout tl;
+
+    // sub-module that owns the 128-slot tile `tile` (routed: the bucket it lies in)
+    __device__ __forceinline__ int sub_of_tile(int64_t tile) const {
+        int sub = fixed_sub;
+        if (counters) {
+            sub = 0;
+            const int64_t s0 = tile * MN_TILE;
+            while (sub + 1 < n_sub && s0 >= counters[CNT_START + sub + 1]) ++sub;
+        }
+        return sub;
+    }
+    // row held by `slot`, -1 for padding and for slots at or past n_slots
+    __device__ __forceinline__ int64_t row_of_slot(int64_t slot, int64_t n_slots) const {
+        int64_t row = -1;
+        if (slot < n_slots) row = slot_row ? (int64_t)slot_row[slot] : slot;
+        return row;
+    }
 };
 
 // Arguments of the backward kernels (csrc/mn_backward.cu).
@@ -133,10 +150,19 @@ size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision)
 int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st);
 int mn_mlp_tp_program(const NetDims& nd, unsigned int* table_out, int cap_entries, int* info8);   // host only (test hook)
 // ---- tensor-core training path (csrc/mn_train_tc.cuh): per-tile tape records and the two passes
+// An activation record (and the backward pass's gradient record, same layout) holds fp16 images in the layout of the MLP
+// kernel's activation buffer, [cols/8][128 slots][8], one every L * 128 * 2 bytes: H_0 .. H_{layers-1}, then F
+// (xyz_encoding_final) at image `layers`, then G (dir_a_encoding, L/2 columns) at image `layers + 1`.
+__host__ __device__ __forceinline__ size_t mn_tc_img_off(int img, int L) { return (size_t)img * L * MN_TILE * 2; }
+// rows of the per-tile fp32 head block [MN_TC_F32_ROWS][128]: sigma pre-activation, rgb (3), image id
+enum { MN_TC_F32_SIGMA = 0, MN_TC_F32_RGB = 1, MN_TC_F32_ID = 4, MN_TC_F32_ROWS = 5 };
+// rows of the backward pass's per-tile fp32 head-gradient block [MN_TC_G32_ROWS][128]: d sigma pre-activation, d rgb
+// pre-activation (3)
+enum { MN_TC_G32_SIGMA = 0, MN_TC_G32_RGB = 1, MN_TC_G32_ROWS = 4 };
 struct TrainTcTape {
     unsigned char* xreg;      // encoder feature tiles        [n_tiles][x_tile_bytes]
     unsigned char* act;       // activation records           [n_tiles][act_tile_bytes]
-    float* f32;               // [n_tiles][5][128]: sigma pre-activation, rgb (3), image id
+    float* f32;               // fp32 head blocks             [n_tiles][MN_TC_F32_ROWS][128]
 };
 size_t mn_train_tc_x_tile_bytes(const mn_model* m);
 size_t mn_train_tc_act_tile_bytes(const mn_model* m);

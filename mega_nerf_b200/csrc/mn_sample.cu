@@ -196,43 +196,51 @@ __device__ __forceinline__ void warp_bitonic(float* key, unsigned short* id, int
     }
 }
 
-__device__ __forceinline__ int next_pow2(int v) {
+// ------------------------------------------------------------------------------------------------
+// merge + composite                                                   (rendering.py:336-393)
+// ------------------------------------------------------------------------------------------------
+// Shared memory of one warp (one ray) of the composite kernels, 4 warps per CTA: the float planes [4 warps][2][npad]
+// come first, then the id planes [2][4 warps][npad]; the second id plane (merge scratch, at ids + 4 npad) is only
+// addressed inside composite_merge.
+struct CompositeSmem {
+    float* zs;             // merged depths
+    float* f2;             // merge scratch, then a per-sample float of the kernel
+    unsigned short* ids;   // sample index of each merged position (< S: own sample, else stored sample + S)
+};
+__device__ __forceinline__ CompositeSmem composite_smem(unsigned char* sm_raw, int warp, int npad) {
+    CompositeSmem s;
+    s.zs = reinterpret_cast<float*>(sm_raw) + (size_t)warp * npad * 2;
+    s.f2 = s.zs + npad;
+    s.ids = reinterpret_cast<unsigned short*>(reinterpret_cast<float*>(sm_raw) + (size_t)4 * npad * 2) + (size_t)warp * npad;
+    return s;
+}
+
+int pow2_at_least(int v) {
     int p = 32;
     while (p < v) p <<= 1;
     return p;
 }
 
-// ------------------------------------------------------------------------------------------------
-// merge + composite                                                   (rendering.py:336-393)
-// ------------------------------------------------------------------------------------------------
-struct CompositeArgs {
-    const float* raw;      // [N,S,4]
-    const float* z;        // [N,S]
-    const float* dreal;    // [N,S] or null
-    int S;
-    const float* raw2;     // [N,S2,4] or null
-    const float* z2;
-    const float* dreal2;
-    int S2;
-    const float* last_delta;  // [N]
-    int64_t N;
-    int flip;
-    float *weights, *rgb, *depth, *var, *lambda;
-    int npad;              // shared-memory elements per warp
-};
+// Launches either composite kernel: one warp per ray, 4 rays per CTA, each warp with the buffers of composite_smem.
+template <class Args>
+int composite_launch(mn_ctx* ctx, void (*kernel)(Args), Args a, const char* name, cudaStream_t st) {
+    a.npad = a.S2 > 0 ? pow2_at_least(a.S + a.S2) : (a.S + 31) / 32 * 32;
+    if (a.npad > 4096) return mn_fail(ctx, MN_ERR_UNSUPPORTED, std::string(name) + ": more than 4096 samples per ray");
+    const size_t sm = (size_t)4 * a.npad * (2 * sizeof(float) + 2 * sizeof(unsigned short));
+    MN_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    kernel<<<(unsigned)mn_cdiv(a.N, 4), 128, sm, st>>>(a);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
 
-__global__ void __launch_bounds__(128) composite_kernel(const CompositeArgs a) {
-    extern __shared__ unsigned char sm_raw[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t ray = (int64_t)blockIdx.x * 4 + warp;
-    if (ray >= a.N) return;
+// Loads the ray's own depths and the stored ones into s.zs / s.ids in merged order: (depth, index), own samples first on
+// ties.  The backward pass is only right because it rebuilds exactly this order.  Returns the max over the own depths (the
+// last-delta fix-up).  Args: CompositeArgs or CompositeBwdArgs.
+template <class Args>
+__device__ __forceinline__ float composite_merge(const Args& a, int64_t ray, int lane, const CompositeSmem& s) {
+    float* zs = s.zs;
+    unsigned short* ids = s.ids;
     const int n = a.S + a.S2;
-    float* zs = reinterpret_cast<float*>(sm_raw) + (size_t)warp * a.npad * 2;
-    float* ws = zs + a.npad;
-    unsigned short* ids = reinterpret_cast<unsigned short*>(reinterpret_cast<float*>(sm_raw) + (size_t)4 * a.npad * 2) +
-                          (size_t)warp * a.npad;
-
-    // own depths (+ max for the last-delta fix-up), optional stored coarse depths
     float zmax = -INFINITY;
     for (int i = lane; i < a.S; i += 32) {
         const float v = a.z[ray * a.S + i];
@@ -248,15 +256,15 @@ __global__ void __launch_bounds__(128) composite_kernel(const CompositeArgs a) {
         }
         __syncwarp();
         // Both runs are usually already ordered (deterministic sampling): merge by rank instead of sorting.
-        // Same total order as the bitonic path: (depth, index), own samples first on ties.
+        // Same total order as the bitonic path.
         bool ordered = true;
         for (int i = lane; i + 1 < a.S; i += 32) ordered &= a.flip ? (zs[i] >= zs[i + 1]) : (zs[i] <= zs[i + 1]);
         for (int i = lane; i + 1 < a.S2; i += 32)
             ordered &= a.flip ? (zs[a.S + i] >= zs[a.S + i + 1]) : (zs[a.S + i] <= zs[a.S + i + 1]);
         ordered = __all_sync(0xffffffffu, ordered);
         if (ordered) {
-            float* zm = ws;   // merged depths are built in the (still unused) weights buffer, then swapped in
-            unsigned short* idm = ids + a.npad * 4;   // second id plane (see launch: 2 planes per warp)
+            float* zm = s.f2;
+            unsigned short* idm = ids + a.npad * 4;
             for (int i = lane; i < n; i += 32) {
                 const bool own = i < a.S;
                 const float v = zs[i];
@@ -284,6 +292,45 @@ __global__ void __launch_bounds__(128) composite_kernel(const CompositeArgs a) {
         }
     }
     __syncwarp();
+    return zmax;
+}
+
+// Distance from merged sample p to the next one; the last sample takes the ray's last delta ld.
+__device__ __forceinline__ float sample_delta(const float* zs, int p, int n, int flip, float ld) {
+    const float zz = zs[p];
+    const float znext = (p + 1 < n) ? zs[p + 1] : 0.0f;
+    float delta = flip ? (zz - znext) : (znext - zz);
+    if (p + 1 == n) delta = ld;
+    return delta;
+}
+
+struct CompositeArgs {
+    const float* raw;      // [N,S,4]
+    const float* z;        // [N,S]
+    const float* dreal;    // [N,S] or null
+    int S;
+    const float* raw2;     // [N,S2,4] or null
+    const float* z2;
+    const float* dreal2;
+    int S2;
+    const float* last_delta;  // [N]
+    int64_t N;
+    int flip;
+    float *weights, *rgb, *depth, *var, *lambda;
+    int npad;              // shared-memory elements per warp
+};
+
+__global__ void __launch_bounds__(128) composite_kernel(const CompositeArgs a) {
+    extern __shared__ unsigned char sm_raw[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t ray = (int64_t)blockIdx.x * 4 + warp;
+    if (ray >= a.N) return;
+    const int n = a.S + a.S2;
+    const CompositeSmem sm = composite_smem(sm_raw, warp, a.npad);
+    const float* zs = sm.zs;
+    float* ws = sm.f2;
+    const unsigned short* ids = sm.ids;
+    const float zmax = composite_merge(a, ray, lane, sm);
 
     float ld = a.last_delta[ray];
     if (ld < 1e10f) ld = ld - zmax;   // rendering.py:191-193 / 224-225: max over this pass's own depths
@@ -301,9 +348,7 @@ __global__ void __launch_bounds__(128) composite_kernel(const CompositeArgs a) {
             const float4 v = *reinterpret_cast<const float4*>(rw);
             cr = v.x; cg = v.y; cb = v.z;
             zz = zs[p];
-            const float znext = (p + 1 < n) ? zs[p + 1] : 0.0f;
-            float delta = a.flip ? (zz - znext) : (znext - zz);
-            if (p + 1 == n) delta = ld;
+            const float delta = sample_delta(zs, p, n, a.flip, ld);
             alpha = 1.0f - expf(-delta * v.w);
             x = (1.0f - alpha) + 1e-8f;
             dd = zz;
@@ -603,59 +648,11 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(const CompositeBwdAr
     const int64_t ray = (int64_t)blockIdx.x * 4 + warp;
     if (ray >= a.N) return;
     const int n = a.S + a.S2;
-    float* zs = reinterpret_cast<float*>(sm_raw) + (size_t)warp * a.npad * 2;
-    float* ts = zs + a.npad;   // merge scratch first, then T (exclusive transmittance) per merged position
-    unsigned short* ids = reinterpret_cast<unsigned short*>(reinterpret_cast<float*>(sm_raw) + (size_t)4 * a.npad * 2) +
-                          (size_t)warp * a.npad;
-
-    float zmax = -INFINITY;
-    for (int i = lane; i < a.S; i += 32) {
-        const float v = a.z[ray * a.S + i];
-        zs[i] = v;
-        ids[i] = (unsigned short)i;
-        zmax = fmaxf(zmax, v);
-    }
-    zmax = warp_max(zmax);
-    if (a.S2 > 0) {
-        for (int i = lane; i < a.S2; i += 32) {
-            zs[a.S + i] = a.z2[ray * a.S2 + i];
-            ids[a.S + i] = (unsigned short)(a.S + i);
-        }
-        __syncwarp();
-        bool ordered = true;
-        for (int i = lane; i + 1 < a.S; i += 32) ordered &= a.flip ? (zs[i] >= zs[i + 1]) : (zs[i] <= zs[i + 1]);
-        for (int i = lane; i + 1 < a.S2; i += 32)
-            ordered &= a.flip ? (zs[a.S + i] >= zs[a.S + i + 1]) : (zs[a.S + i] <= zs[a.S + i + 1]);
-        ordered = __all_sync(0xffffffffu, ordered);
-        if (ordered) {
-            float* zm = ts;
-            unsigned short* idm = ids + a.npad * 4;
-            for (int i = lane; i < n; i += 32) {
-                const bool own = i < a.S;
-                const float v = zs[i];
-                const float* other = own ? zs + a.S : zs;
-                const int m = own ? a.S2 : a.S;
-                int lo = 0, hi = m;
-                while (lo < hi) {
-                    const int mid = (lo + hi) >> 1;
-                    const float o = other[mid];
-                    const bool before = a.flip ? (own ? o > v : o >= v) : (own ? o < v : o <= v);
-                    if (before) lo = mid + 1; else hi = mid;
-                }
-                const int pos = (own ? i : i - a.S) + lo;
-                zm[pos] = v;
-                idm[pos] = (unsigned short)i;
-            }
-            __syncwarp();
-            for (int i = lane; i < n; i += 32) { const float v = zm[i]; const unsigned short id = idm[i]; zs[i] = v; ids[i] = id; }
-        } else {
-            const float pad = a.flip ? -INFINITY : INFINITY;
-            for (int i = n + lane; i < a.npad; i += 32) { zs[i] = pad; ids[i] = 0xFFFF; }
-            __syncwarp();
-            warp_bitonic(zs, ids, a.npad, a.flip != 0, lane);
-        }
-    }
-    __syncwarp();
+    const CompositeSmem sm = composite_smem(sm_raw, warp, a.npad);
+    const float* zs = sm.zs;
+    float* ts = sm.f2;   // T (exclusive transmittance) per merged position
+    const unsigned short* ids = sm.ids;
+    const float zmax = composite_merge(a, ray, lane, sm);
 
     float ld = a.last_delta[ray];
     if (ld < 1e10f) ld = ld - zmax;
@@ -670,10 +667,7 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(const CompositeBwdAr
         if (ok) {
             const int id = ids[p];
             const float sg = (id < a.S) ? a.raw[(ray * a.S + id) * 4 + 3] : a.raw2[(ray * a.S2 + (id - a.S)) * 4 + 3];
-            const float zz = zs[p];
-            const float znext = (p + 1 < n) ? zs[p + 1] : 0.0f;
-            float delta = a.flip ? (zz - znext) : (znext - zz);
-            if (p + 1 == n) delta = ld;
+            const float delta = sample_delta(zs, p, n, a.flip, ld);
             const float alpha = 1.0f - expf(-delta * sg);
             x = (1.0f - alpha) + 1e-8f;
         }
@@ -703,10 +697,7 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(const CompositeBwdAr
             id = ids[p];
             const float* rw = (id < a.S) ? a.raw + (ray * a.S + id) * 4 : a.raw2 + (ray * a.S2 + (id - a.S)) * 4;
             const float4 v = *reinterpret_cast<const float4*>(rw);
-            const float zz = zs[p];
-            const float znext = (p + 1 < n) ? zs[p + 1] : 0.0f;
-            delta = a.flip ? (zz - znext) : (znext - zz);
-            if (p + 1 == n) delta = ld;
+            delta = sample_delta(zs, p, n, a.flip, ld);
             ex = expf(-delta * v.w);
             const float alpha = 1.0f - ex;
             x = (1.0f - alpha) + 1e-8f;
@@ -864,12 +855,6 @@ int mn_sample_pdf(mn_ctx* ctx, const float* z_coarse_d, const float* weights_d, 
     return MN_OK;
 }
 
-static int pow2_at_least(int v) {
-    int p = 32;
-    while (p < v) p <<= 1;
-    return p;
-}
-
 int mn_sort_cat(mn_ctx* ctx, const float* a_d, int na, const float* b_d, int nb, int64_t N, int descending, float* out_d,
                 void* stream) {
     if (!ctx || !a_d || (nb > 0 && !b_d) || !out_d) return MN_ERR_INVALID;
@@ -896,13 +881,7 @@ int mn_composite(mn_ctx* ctx, const float* raw_d, const float* z_d, const float*
     a.raw2 = raw2_d; a.z2 = z2_d; a.dreal2 = depth_real2_d; a.S2 = S2;
     a.last_delta = last_delta_d; a.N = N; a.flip = flip;
     a.weights = weights_out_d; a.rgb = rgb_out_d; a.depth = depth_out_d; a.var = depth_var_out_d; a.lambda = bg_lambda_out_d;
-    a.npad = S2 > 0 ? pow2_at_least(S + S2) : (S + 31) / 32 * 32;
-    if (a.npad > 4096) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_composite: more than 4096 samples per ray");
-    const size_t sm = (size_t)4 * a.npad * (2 * sizeof(float) + 2 * sizeof(unsigned short));
-    MN_CUDA(ctx, cudaFuncSetAttribute(composite_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    composite_kernel<<<(unsigned)mn_cdiv(N, 4), 128, sm, (cudaStream_t)stream>>>(a);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return composite_launch(ctx, composite_kernel, a, "mn_composite", (cudaStream_t)stream);
 }
 
 int mn_composite_backward(mn_ctx* ctx, const float* raw_d, const float* z_d, int S, const float* raw2_d, const float* z2_d,
@@ -917,13 +896,7 @@ int mn_composite_backward(mn_ctx* ctx, const float* raw_d, const float* z_d, int
     a.last_delta = last_delta_d; a.N = N; a.flip = flip;
     a.grad_rgb = grad_rgb_d; a.grad_lambda = grad_lambda_d;
     a.grad_raw = grad_raw_d; a.grad_raw2 = grad_raw2_d;
-    a.npad = S2 > 0 ? pow2_at_least(S + S2) : (S + 31) / 32 * 32;
-    if (a.npad > 4096) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_composite_backward: more than 4096 samples per ray");
-    const size_t sm = (size_t)4 * a.npad * (2 * sizeof(float) + 2 * sizeof(unsigned short));
-    MN_CUDA(ctx, cudaFuncSetAttribute(composite_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    composite_bwd_kernel<<<(unsigned)mn_cdiv(N, 4), 128, sm, (cudaStream_t)stream>>>(a);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return composite_launch(ctx, composite_bwd_kernel, a, "mn_composite_backward", (cudaStream_t)stream);
 }
 
 int mn_sh_to_rgb_backward(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d,

@@ -29,7 +29,7 @@ inline bool build_dgrad_plan(const NetDims& nd, TcPlan* p) {
     auto add = [&](int n, int k, int img, int epi) {
         TcGemm& g = P.g[ng++];
         g.n = n; g.nseg = 1; g.src[0] = SRC_H; g.k[0] = k; g.src[1] = 0; g.k[1] = 0;
-        g.w_off = woff; g.bias_off = img; g.epi = epi;
+        g.w_off = woff; g.img = img; g.epi = epi;
         woff += k * n * 2;
     };
     add(nd.L, nd.L / 2, nd.layers, EPI_D_LINEAR);                    // dF  = dZ_dira  W_dira[:, 0:L]      -> image 'final'
@@ -204,7 +204,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
 // sigma Linear (1 x L) and rgb Linear (3 x L/2) weight / bias gradients from the fp32 head gradients and the fp16 tapes.
 struct HeadsArgs {
     const unsigned char* act;
-    const float* gf32;              // per tile [4][128]: d sigma pre-activation, d rgb pre-activation (3)
+    const float* gf32;              // head-gradient blocks [n_tiles][MN_TC_G32_ROWS][128]
     int64_t act_tile_bytes;
     int L, layers;
     const int* counters;
@@ -215,7 +215,7 @@ struct HeadsArgs {
     int sigma_w, sigma_b, rgb_w, rgb_b;     // float offsets in a sub-module's gradient block (rgb_w is [3][L/2])
 };
 __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) {
-    __shared__ float G4[4][kTileM];
+    __shared__ float G4[MN_TC_G32_ROWS][kTileM];
     int sub = A.fixed_sub;
     int64_t t_lo = 0, t_hi = A.n_tiles;
     if (A.counters) {
@@ -230,20 +230,20 @@ __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) 
     float ws = 0.0f, wr0 = 0.0f, wr1 = 0.0f, wr2 = 0.0f, bs = 0.0f;
     for (int64_t t = t_begin; t < t_end; ++t) {
         __syncthreads();
-        for (int i = threadIdx.x; i < 4 * kTileM; i += 256) G4[i / kTileM][i % kTileM] = A.gf32[(size_t)t * 4 * kTileM + i];
+        for (int i = threadIdx.x; i < MN_TC_G32_ROWS * kTileM; i += 256) G4[i / kTileM][i % kTileM] = A.gf32[(size_t)t * MN_TC_G32_ROWS * kTileM + i];
         __syncthreads();
         const unsigned char* rec = A.act + (size_t)t * A.act_tile_bytes;
         if (k < L) {
-            const __half* h = reinterpret_cast<const __half*>(rec + (size_t)(A.layers - 1) * L * kTileM * 2) + (size_t)(k >> 3) * (kTileM * 8) + (k & 7);
-            for (int r = 0; r < kTileM; ++r) ws = fmaf(G4[0][r], __half2float(h[r * 8]), ws);
+            const __half* h = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers - 1, L)) + (size_t)(k >> 3) * (kTileM * 8) + (k & 7);
+            for (int r = 0; r < kTileM; ++r) ws = fmaf(G4[MN_TC_G32_SIGMA][r], __half2float(h[r * 8]), ws);
         }
         if (k < half) {
-            const __half* g = reinterpret_cast<const __half*>(rec + (size_t)(A.layers + 1) * L * kTileM * 2) + (size_t)(k >> 3) * (kTileM * 8) + (k & 7);
+            const __half* g = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers + 1, L)) + (size_t)(k >> 3) * (kTileM * 8) + (k & 7);
             for (int r = 0; r < kTileM; ++r) {
                 const float gv = __half2float(g[r * 8]);
-                wr0 = fmaf(G4[1][r], gv, wr0);
-                wr1 = fmaf(G4[2][r], gv, wr1);
-                wr2 = fmaf(G4[3][r], gv, wr2);
+                wr0 = fmaf(G4[MN_TC_G32_RGB][r], gv, wr0);
+                wr1 = fmaf(G4[MN_TC_G32_RGB + 1][r], gv, wr1);
+                wr2 = fmaf(G4[MN_TC_G32_RGB + 2][r], gv, wr2);
             }
         }
         if (k < 4) for (int r = 0; r < kTileM; ++r) bs += G4[k][r];
