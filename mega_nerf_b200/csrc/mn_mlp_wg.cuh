@@ -2,8 +2,8 @@
 
 // Tensor-core MLP kernel for Hopper (sm_90a), included inside mn_mlp_tc.cu's anonymous namespace.
 //
-//   tc_mlp_wg_kernel<kMode, kSplit, kWide>   persistent, one 128-row tile at a time, 288 threads:
-//     warp 8          one thread streams the weight K-slabs of every GEMM (cp.async.bulk into an mbarrier ring) and the
+//   tc_mlp_wg_kernel<kMode, kSplit, kWide>   persistent, one 128-row tile at a time, 384 threads:
+//     warpgroup 2     one thread streams the weight K-slabs of every GEMM (cp.async.bulk into an mbarrier ring) and the
 //                     feature-tile segments (positional encodings, direction + appearance) into their own buffer
 //     warpgroups 0-1  rows 0-63 / 64-127 of the tile: wgmma.mma_async m64nNk16 with A = the tile's fp16 activations (or the
 //                     feature segment) in shared memory and B = the ring stage, fp32 accumulators in registers; then the
@@ -134,7 +134,13 @@ __host__ __device__ __forceinline__ void wg_walk_chunk(const TcPlan& P, int gi, 
     }
 }
 
-constexpr int kWgmmaThreads = 288;   // two consumer warpgroups + one producer warp: up to 224 registers per thread
+// Three full warpgroups: two consumers and the producer warpgroup (one of its threads issues the copies).  The launch alone caps
+// every thread at 168 registers (65536 / 384, rounded down); setmaxnreg then moves registers from the producer warpgroup
+// (kWgProducerRegs) to the consumers (kWgConsumerRegs): 128 x 56 + 256 x 224 = 64512 <= 65536.  The producer's stage walk
+// spills below 56 registers; with 224 per consumer thread only the 512-wide variant still spills.
+constexpr int kWgmmaThreads = 384;
+constexpr int kWgProducerRegs = 56;
+constexpr int kWgConsumerRegs = 224;
 constexpr int kWgRingMax = 8;
 
 struct WgLayout {
@@ -196,6 +202,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
     const int wgi = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0);     // warp-uniform role
     if (wgi == 2) {
         // =========================== producer ===========================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kWgProducerRegs));
         if (threadIdx.x == 256) {
             int stage = 0;
             uint32_t phase = 0, xphase = 0;
@@ -224,6 +231,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
         }
     } else {
         // =========================== consumers: MMA + epilogue ===========================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWgConsumerRegs));
         const int wg = wgi;
         const int t = threadIdx.x & 127, w = t >> 5, lane = t & 31, q4 = lane & 3;
         // accumulator fragment of m64nNk16: this thread holds rows ra, ra + 8 and, in every 8-column group j, columns 8j + 2 q4 + {0, 1}
