@@ -298,9 +298,10 @@ int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const
  * activations to the tape; backward = data gradients on transposed fp16 weight images (ReLU masks from the tape, gradient
  * images scaled by a power of two chosen from max|grad_out|), weight gradients as wgmma contractions of the two tapes
  * over the slot axis, fp32 accumulation, fp32 atomics into param_grads_d.  Same argument meaning as the fp32 entry points
- * above; covers layer_dim 256 with a direction / appearance head and rgb_dim 3 (mn_model_train_tc_supported), everything
- * else returns MN_ERR_UNSUPPORTED - use the fp32 entry points.  Gradients agree with the fp32 path to ~1e-2 of each
- * tensor's scale (fp16 operands, like the reference under autocast); the fp32 entry points remain the parity mode. */
+ * above; covers layer_dim 256 with a direction / appearance head and either rgb_dim 3 or a raw SH head (rgb_dim <= 32), no
+ * affine appearance (mn_model_train_tc_supported), everything else returns MN_ERR_UNSUPPORTED - use the fp32 entry points.
+ * Gradients agree with the fp32 path to ~1e-2 of each tensor's scale (fp16 operands, like the reference under autocast);
+ * the fp32 entry points remain the parity mode. */
 int mn_model_train_tc_supported(const mn_model* m);
 size_t mn_model_tape_bytes_tc(const mn_model* m, int64_t B);
 int mn_model_forward_train_tc(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse,

@@ -382,7 +382,7 @@ struct TcArgs {
     unsigned char* tape_act;      // PP_TRAIN_FWD: written;  PP_DGRAD: read (ReLU masks)
     float* tape_f32;              // fp32 head blocks [MN_TC_F32_ROWS][128]     (written / read)
     unsigned char* tape_dz;       // PP_DGRAD: gradient images dZ_0 .. dZ_{layers-1}, dZ_final, dZ_dira (same layout, scaled fp16)
-    float* tape_gf32;             // PP_DGRAD: head-gradient blocks [MN_TC_G32_ROWS][128], UNscaled fp32
+    float* tape_gf32;             // PP_DGRAD: head-gradient blocks [mn_tc_g32_rows(rgb_dim)][128], UNscaled fp32
     const float* grad_out;        // PP_DGRAD: [rows][rgb_dim + 1] upstream gradient
     float* emb_sum;               // PP_DGRAD: [n_sub][app_count][L/2] per-image sums of dZ_dira rows (appearance-embedding gradient)
     const float* scale;           // PP_DGRAD: device scalar S (power of two): gradient images hold S * dZ
@@ -512,7 +512,8 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
             packd(D.g[di++], Q + m->blay.w[l], nd.L);       // [L][L]: hidden-part columns of layer l
         float* df32 = reinterpret_cast<float*>(db + D.f32_off);
         mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, df32, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
-        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, df32 + nd.L, nullptr, (long long)3 * (nd.L / 2), PK_RGBW, {nd.L / 2, 3, 0, 0, 0, 0, 0}});
+        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, df32 + nd.L, nullptr, (long long)nd.rgb_dim * (nd.L / 2), PK_RGBW,
+                                 {nd.L / 2, nd.rgb_dim, 0, 0, 0, 0, 0}});
         m->train_tc_ok = 1;
     }
     return MN_OK;
@@ -593,7 +594,8 @@ size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
 int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
     TcArgs A;
     if (!m->train_tc_ok || !tc_forward_args(m, a, n_tiles128, &A))
-        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 with a direction / appearance head and rgb_dim 3; use train precision 'fp32'");
+        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 with a direction / appearance head and rgb_dim 3 "
+                                                "or a raw SH head (rgb_dim <= 32), no affine appearance; use train precision 'fp32'");
     if (n_tiles128 <= 0) return MN_OK;
     A.ximg = reinterpret_cast<const __half*>(tape.xreg);
     A.x_plane_halves = 0;
@@ -609,12 +611,15 @@ int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n
     return rc;
 }
 
-// backward workspace: [gradient records][head gradients fp32 [n_tiles][MN_TC_G32_ROWS][128]][embedding sums][scale]
+// backward workspace: [gradient records][head gradients fp32 [n_tiles][mn_tc_g32_rows(rgb_dim)][128]][embedding sums][scale, max |grad_out|]
 static size_t train_tc_emb_floats(const mn_model* m) {
     return m->nd.app_in_dira ? (size_t)m->d.n_sub * m->nd.app_count * (m->nd.L / 2) : 0;
 }
+static size_t train_tc_head_grad_bytes(const mn_model* m, int64_t n_tiles128) {
+    return mn_align((size_t)n_tiles128 * mn_tc_g32_rows(m->nd.rgb_dim) * kTileM * sizeof(float));
+}
 size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
-    return mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m)) + mn_align((size_t)n_tiles128 * MN_TC_G32_ROWS * kTileM * sizeof(float)) +
+    return mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m)) + train_tc_head_grad_bytes(m, n_tiles128) +
            mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) + 1024;
 }
 
@@ -628,15 +633,23 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     const size_t act_tile = mn_train_tc_act_tile_bytes(m);
     char* wp = (char*)(((uintptr_t)ws + 255) / 256 * 256);
     unsigned char* dz = (unsigned char*)wp;               wp += mn_align((size_t)n_tiles128 * act_tile);
-    float* gf32 = (float*)wp;                             wp += mn_align((size_t)n_tiles128 * MN_TC_G32_ROWS * kTileM * sizeof(float));
+    float* gf32 = (float*)wp;                             wp += train_tc_head_grad_bytes(m, n_tiles128);
     float* emb_sum = (float*)wp;                          wp += mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) - 256;
     float* scale = (float*)wp;
+    unsigned* maxbits = reinterpret_cast<unsigned*>(scale + 1);     // max |grad_out| (float bits), inside the same 256 bytes
     if (train_tc_emb_floats(m)) MN_CUDA(ctx, cudaMemsetAsync(emb_sum, 0, train_tc_emb_floats(m) * sizeof(float), st));
+    MN_CUDA(ctx, cudaMemsetAsync(maxbits, 0, sizeof(unsigned), st));
 
     mn_prof_begin(ctx, st);   // bench.py --mode train: the whole backward of the MLP stage timed as one span
     // ---- gradient scale (power of two) from the upstream gradient
-    tc_grad_scale_kernel<<<1, 1024, 0, st>>>(a.grad_out, a.grad_rows * a.out_cols, scale);
-    MN_LAUNCH_CHECK(ctx);
+    {
+        const int64_t n = a.grad_rows * a.out_cols;
+        const int64_t blocks = std::min<int64_t>(std::max<int64_t>(mn_cdiv(n, (int64_t)256 * 16), 1), (int64_t)ctx->sm_count * 4);
+        tc_grad_absmax_kernel<<<(unsigned)blocks, 256, 0, st>>>(a.grad_out, n, maxbits);
+        MN_LAUNCH_CHECK(ctx);
+        tc_grad_scale_kernel<<<1, 32, 0, st>>>(maxbits, scale);
+        MN_LAUNCH_CHECK(ctx);
+    }
 
     // ---- data gradients
     A.m = MlpArgs{};
@@ -732,6 +745,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     H.act_tile_bytes = (int64_t)act_tile;
     H.L = L;
     H.layers = nd.layers;
+    H.rgb_dim = nd.rgb_dim;
     H.counters = a.counters;
     H.n_tiles = tiles_used;
     H.fixed_sub = a.fixed_sub;
@@ -739,7 +753,9 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     H.gw = a.gw;
     H.sub_stride = a.lay.total;
     H.sigma_w = a.lay.sigma_w; H.sigma_b = a.lay.sigma_b; H.rgb_w = a.lay.rgb_w; H.rgb_b = a.lay.rgb_b;
-    tc_heads_wgrad_kernel<<<dim3((unsigned)mn_cdiv(tiles_used, 16), (unsigned)n_sub), 256, 0, st>>>(H);
+    const dim3 hgrid((unsigned)mn_cdiv(tiles_used, 16), (unsigned)n_sub);
+    if (nd.rgb_dim == 3) tc_heads_wgrad_kernel<3><<<hgrid, 256, 0, st>>>(H);
+    else tc_heads_wgrad_kernel<MN_TC_RGB_MAX><<<hgrid, 256, 0, st>>>(H);
     MN_LAUNCH_CHECK(ctx);
     if (nd.app_in_dira) {
         tc_emb_grad_kernel<<<dim3((unsigned)nd.app_count, (unsigned)a.n_sub), 64, 0, st>>>(emb_sum, a.packed_bwd, a.blay.total, a.blay.dira_e, L / 2, nd.app,

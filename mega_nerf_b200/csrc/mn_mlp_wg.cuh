@@ -262,34 +262,58 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
 
             if (kMode == PP_DGRAD) {
                 // ---- head stage of the data-gradient chain (nerf.py:132-160 backwards): upstream gradient x blend weight ->
-                // sigmoid' / softplus' -> rgb Linear transposed (3 -> L/2, CUDA cores) -> ReLU mask of dir_a_encoding -> dZ_dira
-                // as the first A operand (columns 0 .. L/2-1 of the activation buffer) and on the gradient tape; per-image sums
-                // of its rows for the appearance-embedding gradient; head pre-activation gradients in fp32 for their own Linears.
+                // sigmoid' (colour head, rgb_dim 3; raw SH coefficients pass through) / softplus' -> rgb Linear transposed
+                // (rgb_dim -> L/2, CUDA cores) -> ReLU mask of dir_a_encoding -> dZ_dira as the first A operand (columns
+                // 0 .. L/2-1 of the activation buffer) and on the gradient tape; per-image sums of its rows for the
+                // appearance-embedding gradient; head pre-activation gradients in fp32 for their own Linears.
                 // Thread t of the warpgroup: row 64 wg + t % 64, column half t / 64 (the lanes of a warp are 32 consecutive rows).
                 const float S = *A.scale;
                 const int hr = 64 * wg + (t & 63), part = t >> 6;
                 const int64_t hslot = tile * kTileM + hr;
                 const int64_t hrow = A.m.row_of_slot(hslot, n_slots);
-                const float* Wr = F32 + L;                                  // [3][L/2] rgb weights (fp32 block of the data-gradient plan)
+                const int R = A.m.nd.rgb_dim;
+                const float* Wr = F32 + L;                                  // [rgb_dim][L/2] rgb weights (fp32 block of the data-gradient plan)
                 const float* tf = A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + hr;
-                float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f, g3 = 0.0f;
-                if (hrow >= 0) {
-                    const float4 gv = *reinterpret_cast<const float4*>(A.grad_out + hrow * 4);
-                    const float bw = A.m.slot_w ? A.m.slot_w[hslot] : 1.0f;
-                    g0 = gv.x * bw; g1 = gv.y * bw; g2 = gv.z * bw; g3 = gv.w * bw;
+                // d[c]: gradient of the rgb Linear's output c of this row.  Only compile-time indices (loops unrolled to
+                // MN_TC_RGB_MAX and left at c == R), so the array stays in registers.
+                float d[MN_TC_RGB_MAX], gsig = 0.0f;
+                if (R == 3) {
+                    float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f;
+                    if (hrow >= 0) {
+                        const float4 gv = *reinterpret_cast<const float4*>(A.grad_out + hrow * 4);
+                        const float bw = A.m.slot_w ? A.m.slot_w[hslot] : 1.0f;
+                        g0 = gv.x * bw; g1 = gv.y * bw; g2 = gv.z * bw; gsig = gv.w * bw;
+                    }
+                    const float c0v = tf[MN_TC_F32_RGB * kTileM], c1v = tf[(MN_TC_F32_RGB + 1) * kTileM], c2v = tf[(MN_TC_F32_RGB + 2) * kTileM];
+                    d[0] = (g0 * (1.0f - c0v)) * c0v; d[1] = (g1 * (1.0f - c1v)) * c1v; d[2] = (g2 * (1.0f - c2v)) * c2v;
+                } else {
+#pragma unroll
+                    for (int c = 0; c < MN_TC_RGB_MAX; ++c) d[c] = 0.0f;
+                    if (hrow >= 0) {
+                        const float* go = A.grad_out + hrow * A.m.out_cols;  // [rgb_dim SH coefficients][sigma]
+                        const float bw = A.m.slot_w ? A.m.slot_w[hslot] : 1.0f;
+#pragma unroll
+                        for (int c = 0; c < MN_TC_RGB_MAX; ++c) {
+                            if (c >= R) break;
+                            d[c] = go[c] * bw;
+                        }
+                        gsig = go[R] * bw;
+                    }
                 }
-                const float c0v = tf[MN_TC_F32_RGB * kTileM], c1v = tf[(MN_TC_F32_RGB + 1) * kTileM], c2v = tf[(MN_TC_F32_RGB + 2) * kTileM];
                 const float pre = tf[MN_TC_F32_SIGMA * kTileM];
-                const float d0 = (g0 * (1.0f - c0v)) * c0v, d1 = (g1 * (1.0f - c1v)) * c1v, d2 = (g2 * (1.0f - c2v)) * c2v;
                 float dsp;
                 if (A.m.nd.softplus) { const float y = pre - 1.0f; dsp = y > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-y)); }
                 else dsp = pre > 0.0f ? 1.0f : 0.0f;
-                const float ds = g3 * dsp;
+                const float ds = gsig * dsp;
                 if (part == 0) {
                     DSIG[hr] = ds * S;
-                    float* tg = A.tape_gf32 + (size_t)tile * MN_TC_G32_ROWS * kTileM + hr;
+                    float* tg = A.tape_gf32 + (size_t)tile * mn_tc_g32_rows(R) * kTileM + hr;
                     tg[MN_TC_G32_SIGMA * kTileM] = ds;
-                    tg[MN_TC_G32_RGB * kTileM] = d0; tg[(MN_TC_G32_RGB + 1) * kTileM] = d1; tg[(MN_TC_G32_RGB + 2) * kTileM] = d2;
+#pragma unroll
+                    for (int c = 0; c < MN_TC_RGB_MAX; ++c) {
+                        if (c >= R) break;
+                        tg[(MN_TC_G32_RGB + c) * kTileM] = d[c];
+                    }
                 }
                 const int id = (int)tf[MN_TC_F32_ID * kTileM];
                 const unsigned char* gimg = A.tape_act + (size_t)tile * A.act_tile_bytes + mn_tc_img_off(A.layers + 1, L);
@@ -299,15 +323,25 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                     const int k0 = part * per + kk;
                     const uint4 gm = *reinterpret_cast<const uint4*>(gimg + (size_t)(k0 >> 3) * (kTileM * 16) + (size_t)hr * 16);
                     const __half2* gh = reinterpret_cast<const __half2*>(&gm);
+                    // v[e] = sum_c W_rgb[c][k0 + e] d[c], in the order c = 0, 1, .. (a product, then one fma per further row)
                     float v[8];
+                    {
+                        const float4 wa = *reinterpret_cast<const float4*>(Wr + k0), wb = *reinterpret_cast<const float4*>(Wr + k0 + 4);
+                        v[0] = wa.x * d[0]; v[1] = wa.y * d[0]; v[2] = wa.z * d[0]; v[3] = wa.w * d[0];
+                        v[4] = wb.x * d[0]; v[5] = wb.y * d[0]; v[6] = wb.z * d[0]; v[7] = wb.w * d[0];
+                    }
+#pragma unroll
+                    for (int c = 1; c < MN_TC_RGB_MAX; ++c) {
+                        if (c >= R) break;
+                        const float4 wa = *reinterpret_cast<const float4*>(Wr + c * half + k0);
+                        const float4 wb = *reinterpret_cast<const float4*>(Wr + c * half + k0 + 4);
+                        v[0] = fmaf(wa.x, d[c], v[0]); v[1] = fmaf(wa.y, d[c], v[1]); v[2] = fmaf(wa.z, d[c], v[2]); v[3] = fmaf(wa.w, d[c], v[3]);
+                        v[4] = fmaf(wb.x, d[c], v[4]); v[5] = fmaf(wb.y, d[c], v[5]); v[6] = fmaf(wb.z, d[c], v[6]); v[7] = fmaf(wb.w, d[c], v[7]);
+                    }
 #pragma unroll
                     for (int e = 0; e < 8; ++e) {
-                        const int k = k0 + e;
-                        float acc = Wr[k] * d0;
-                        acc = fmaf(Wr[half + k], d1, acc);
-                        acc = fmaf(Wr[2 * half + k], d2, acc);
                         const float gv = (e & 1) ? __high2float(gh[e >> 1]) : __low2float(gh[e >> 1]);
-                        v[e] = gv > 0.0f ? acc : 0.0f;
+                        v[e] = gv > 0.0f ? v[e] : 0.0f;
                     }
                     // appearance-embedding gradient, step 1: per-image sums of dZ_dira rows (fp32, unscaled); the lanes of a warp
                     // are consecutive slots, i.e. mostly samples of one ray = one image id

@@ -156,9 +156,11 @@ int mn_mlp_tp_program(const NetDims& nd, unsigned int* table_out, int cap_entrie
 __host__ __device__ __forceinline__ size_t mn_tc_img_off(int img, int L) { return (size_t)img * L * MN_TILE * 2; }
 // rows of the per-tile fp32 head block [MN_TC_F32_ROWS][128]: sigma pre-activation, rgb (3), image id
 enum { MN_TC_F32_SIGMA = 0, MN_TC_F32_RGB = 1, MN_TC_F32_ID = 4, MN_TC_F32_ROWS = 5 };
-// rows of the backward pass's per-tile fp32 head-gradient block [MN_TC_G32_ROWS][128]: d sigma pre-activation, d rgb
-// pre-activation (3)
-enum { MN_TC_G32_SIGMA = 0, MN_TC_G32_RGB = 1, MN_TC_G32_ROWS = 4 };
+// rows of the backward pass's per-tile fp32 head-gradient block [mn_tc_g32_rows(rgb_dim)][128]: d sigma pre-activation, d rgb
+// pre-activation (rgb_dim rows: 3 colour channels before the sigmoid, or the raw SH coefficients).  MN_TC_RGB_MAX bounds
+// rgb_dim on the tensor-core training path (register and shared-memory arrays of the head kernels are sized by it).
+enum { MN_TC_G32_SIGMA = 0, MN_TC_G32_RGB = 1, MN_TC_RGB_MAX = 32 };
+__host__ __device__ __forceinline__ int mn_tc_g32_rows(int rgb_dim) { return 1 + rgb_dim; }
 struct TrainTcTape {
     unsigned char* xreg;      // encoder feature tiles        [n_tiles][x_tile_bytes]
     unsigned char* act;       // activation records           [n_tiles][act_tile_bytes]

@@ -5,7 +5,8 @@
 //   forward   tc_mlp_wg_kernel<PP_TRAIN_FWD>  the inference kernel + every layer's fp16 activations written to a tape in the
 //                                             tile-image layout of the activation buffer ([cols/8][128 slots][8]).
 //   dgrad     tc_mlp_wg_kernel<PP_DGRAD>      the same GEMM pipeline on transposed weight images: head stage on CUDA cores
-//                                             (sigmoid' / softplus' / rgb Linear transposed), then dH_{l-1} = dZ_l W_l with the
+//                                             (sigmoid' for a colour head, raw SH coefficients pass through / softplus' /
+//                                             rgb Linear transposed), then dH_{l-1} = dZ_l W_l with the
 //                                             ReLU mask read from the activation tape in the epilogue; dZ images (fp16, scaled by
 //                                             a power of two S) go to a gradient tape.
 //   wgrad     tc_wgrad_kernel                 dW_l = dZ_l^T X_l over all slots of a sub-module: both tapes are consumed AS THEY
@@ -14,13 +15,15 @@
 //                                             channels per CTA (64 per consumer warpgroup), N <= 256 input channels + a 16-column
 //                                             all-ones operand whose product is the bias gradient, accumulated in registers over
 //                                             a chunk of tiles and flushed with fp32 atomics.
-//   heads     tc_heads_wgrad_kernel (sigma / rgb Linears: 1 and 3 output channels - CUDA cores), tc_emb_grad_kernel
+//   heads     tc_heads_wgrad_kernel (sigma / rgb Linears: 1 and rgb_dim output channels - CUDA cores), tc_emb_grad_kernel
 //             (appearance embedding: W_e^T times the per-image sums of dZ_dira rows collected by the dgrad head stage).
 #pragma once
 
-// ---- data-gradient plan: GEMM chain of the backward pass as a TcPlan (all operands from the activation buffer)
+// ---- data-gradient plan: GEMM chain of the backward pass as a TcPlan (all operands from the activation buffer).  Heads:
+// rgb_dim 3 (sigmoid colour) or a raw SH head of up to MN_TC_RGB_MAX coefficients (rgb_dim > 3 implies pos_dir_dim == 0).
 inline bool build_dgrad_plan(const NetDims& nd, TcPlan* p) {
-    if (nd.L != 256 || !nd.has_dir_a || nd.rgb_dim != 3 || nd.affine || nd.layers < 2 || nd.layers > 10) return false;
+    if (nd.L != 256 || !nd.has_dir_a || nd.rgb_dim < 3 || nd.rgb_dim > MN_TC_RGB_MAX || nd.affine || nd.layers < 2 || nd.layers > 10)
+        return false;
     TcPlan& P = *p;
     P = TcPlan{};
     P.L = nd.L;
@@ -38,22 +41,31 @@ inline bool build_dgrad_plan(const NetDims& nd, TcPlan* p) {
     P.n_gemm = P.n_trunk = ng;
     P.plane_bytes = woff;
     P.sigma_w_off = 0;
-    P.f32_floats = nd.L + 3 * (nd.L / 2);                            // [sigma_w (L)][rgb_w [3][L/2]]
+    P.f32_floats = nd.L + nd.rgb_dim * (nd.L / 2);                   // [sigma_w (L)][rgb_w [rgb_dim][L/2]]
     P.f32_off = woff;
     P.sub_bytes = (int)mn_align((size_t)woff + (size_t)P.f32_floats * 4, 256);
     return true;
 }
 
-// S = 2^(10 - ceil(log2(max |g|)))  (1 if g == 0 or not finite): the gradient images hold S * dZ in fp16
-__global__ void tc_grad_scale_kernel(const float* __restrict__ g, int64_t n, float* __restrict__ scale) {
+// max |g| over the upstream gradient, spread over the machine (an SH head's grad_out has 28 columns per row): every block
+// folds a grid-stride share and publishes its maximum with an integer atomicMax on *maxbits (zeroed by the caller; the bit
+// patterns of non-negative floats order like the values, and fmaxf drops NaNs, so the result is max |g| exactly)
+__global__ void tc_grad_absmax_kernel(const float* __restrict__ g, int64_t n, unsigned* __restrict__ maxbits) {
     __shared__ float red[32];
     float m = 0.0f;
-    for (int64_t i = threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(g[i]));
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(g[i]));
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
     __syncthreads();
     if (threadIdx.x == 0) {
         for (int i = 1; i < (int)(blockDim.x >> 5); ++i) m = fmaxf(m, red[i]);
+        atomicMax(maxbits, __float_as_uint(m));
+    }
+}
+// S = 2^(10 - ceil(log2(max |g|)))  (1 if g == 0 or not finite): the gradient images hold S * dZ in fp16
+__global__ void tc_grad_scale_kernel(const unsigned* __restrict__ maxbits, float* __restrict__ scale) {
+    if (threadIdx.x == 0) {
+        const float m = __uint_as_float(*maxbits);
         float s = 1.0f;
         if (m > 0.0f && m < 3.0e38f) s = exp2f(10.0f - ceilf(log2f(m)));
         scale[0] = fminf(fmaxf(s, 1.0f / 1099511627776.0f), 1099511627776.0f);       // 2^-40 .. 2^40
@@ -201,21 +213,27 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
     }
 }
 
-// sigma Linear (1 x L) and rgb Linear (3 x L/2) weight / bias gradients from the fp32 head gradients and the fp16 tapes.
+// sigma Linear (1 x L) and rgb Linear (rgb_dim x L/2) weight / bias gradients from the fp32 head gradients and the fp16 tapes.
 struct HeadsArgs {
     const unsigned char* act;
-    const float* gf32;              // head-gradient blocks [n_tiles][MN_TC_G32_ROWS][128]
+    const float* gf32;              // head-gradient blocks [n_tiles][mn_tc_g32_rows(rgb_dim)][128]
     int64_t act_tile_bytes;
-    int L, layers;
+    int L, layers, rgb_dim;
     const int* counters;
     int64_t n_tiles;
     int fixed_sub, chunk_tiles;
     float* gw;
     int64_t sub_stride;
-    int sigma_w, sigma_b, rgb_w, rgb_b;     // float offsets in a sub-module's gradient block (rgb_w is [3][L/2])
+    int sigma_w, sigma_b, rgb_w, rgb_b;     // float offsets in a sub-module's gradient block (rgb_w is [rgb_dim][L/2])
 };
+// kRgb: 3 for the colour head (exactly 3 rgb rows), MN_TC_RGB_MAX for a raw SH head (rgb_dim <= kRgb rows).  The rgb weight
+// gradient is split over the block: thread k accumulates input channel k % (L/2) for the output rows [kPer * (k / (L/2)),
+// +kPer) (256 threads, L/2 = 128: two groups of kPer rows).
+template <int kRgb>
 __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) {
-    __shared__ float G4[MN_TC_G32_ROWS][kTileM];
+    constexpr int kPer = kRgb < 16 ? kRgb : 16;       // rgb accumulators per thread
+    static_assert(2 * kPer >= kRgb, "rgb rows of tc_heads_wgrad_kernel");
+    __shared__ float G[1 + kRgb][kTileM];              // this tile's head-gradient block
     int sub = A.fixed_sub;
     int64_t t_lo = 0, t_hi = A.n_tiles;
     if (A.counters) {
@@ -226,37 +244,40 @@ __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) 
     const int64_t t_begin = t_lo + (int64_t)blockIdx.x * A.chunk_tiles;
     const int64_t t_end = min(t_hi, t_begin + (int64_t)A.chunk_tiles);
     if (t_begin >= t_end) return;
-    const int k = threadIdx.x, L = A.L, half = L / 2;
-    float ws = 0.0f, wr0 = 0.0f, wr1 = 0.0f, wr2 = 0.0f, bs = 0.0f;
+    const int rgb_dim = kRgb == 3 ? 3 : A.rgb_dim;
+    const int k = threadIdx.x, L = A.L, half = L / 2, rows = mn_tc_g32_rows(rgb_dim);
+    const int kc = k % half, c0 = kPer * (k / half);       // rgb part: input channel, first output row
+    const int nc = min(kPer, rgb_dim - c0);                // output rows of this thread (<= 0: none)
+    float ws = 0.0f, bs = 0.0f, wr[kPer];
+#pragma unroll
+    for (int c = 0; c < kPer; ++c) wr[c] = 0.0f;
     for (int64_t t = t_begin; t < t_end; ++t) {
         __syncthreads();
-        for (int i = threadIdx.x; i < MN_TC_G32_ROWS * kTileM; i += 256) G4[i / kTileM][i % kTileM] = A.gf32[(size_t)t * MN_TC_G32_ROWS * kTileM + i];
+        for (int i = threadIdx.x; i < rows * kTileM; i += 256) G[i / kTileM][i % kTileM] = A.gf32[(size_t)t * rows * kTileM + i];
         __syncthreads();
         const unsigned char* rec = A.act + (size_t)t * A.act_tile_bytes;
         if (k < L) {
             const __half* h = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers - 1, L)) + (size_t)(k >> 3) * (kTileM * 8) + (k & 7);
-            for (int r = 0; r < kTileM; ++r) ws = fmaf(G4[MN_TC_G32_SIGMA][r], __half2float(h[r * 8]), ws);
+            for (int r = 0; r < kTileM; ++r) ws = fmaf(G[MN_TC_G32_SIGMA][r], __half2float(h[r * 8]), ws);
         }
-        if (k < half) {
-            const __half* g = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers + 1, L)) + (size_t)(k >> 3) * (kTileM * 8) + (k & 7);
+        if (nc > 0) {
+            const __half* g = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers + 1, L)) + (size_t)(kc >> 3) * (kTileM * 8) + (kc & 7);
             for (int r = 0; r < kTileM; ++r) {
                 const float gv = __half2float(g[r * 8]);
-                wr0 = fmaf(G4[MN_TC_G32_RGB][r], gv, wr0);
-                wr1 = fmaf(G4[MN_TC_G32_RGB + 1][r], gv, wr1);
-                wr2 = fmaf(G4[MN_TC_G32_RGB + 2][r], gv, wr2);
+#pragma unroll
+                for (int c = 0; c < kPer; ++c)
+                    if (kRgb == 3 || c < nc) wr[c] = fmaf(G[MN_TC_G32_RGB + c0 + c][r], gv, wr[c]);     // colour head: nc == 3
             }
         }
-        if (k < 4) for (int r = 0; r < kTileM; ++r) bs += G4[k][r];
+        if (k < rows) for (int r = 0; r < kTileM; ++r) bs += G[k][r];
     }
     float* W = A.gw + (size_t)sub * A.sub_stride;
     if (k < L) atomicAdd(W + A.sigma_w + k, ws);
-    if (k < half) {
-        atomicAdd(W + A.rgb_w + k, wr0);
-        atomicAdd(W + A.rgb_w + half + k, wr1);
-        atomicAdd(W + A.rgb_w + 2 * half + k, wr2);
-    }
+#pragma unroll
+    for (int c = 0; c < kPer; ++c)
+        if (c < nc) atomicAdd(W + A.rgb_w + (c0 + c) * half + kc, wr[c]);
     if (k == 0) atomicAdd(W + A.sigma_b, bs);
-    else if (k < 4) atomicAdd(W + A.rgb_b + (k - 1), bs);
+    else if (k < rows) atomicAdd(W + A.rgb_b + (k - 1), bs);
 }
 
 // embedding_a.weight[id][j] += sum_k We[k][j] * S[sub][id][k]     (We = dir_a_encoding columns of the embedding, [L/2][app])
