@@ -41,7 +41,7 @@ __global__ void __launch_bounds__(256) pack_ops_kernel(const PackOp* __restrict_
                 if (op.dst2) reinterpret_cast<__half*>(op.dst2)[i] = __float2half_rn(v - __half2float(h));
                 break;
             }
-            case PK_TC_HALF: {        // half-major image [N-half][K/8][nw][8] fp16 (512-wide kernel)
+            case PK_TC_HALF: {        // half-major image [N-half][K/8][nw][8] fp16 (512-wide kernel, layer-GEMM path); optional fp16 residual (lo)
                 const int n_src = op.p[0], k_src = op.p[1], K = op.p[3], k_real0 = op.p[4], k_pad0 = op.p[5], nw = op.p[6];
                 const int k8 = (int)(i % 8), n = (int)((i / 8) % nw);
                 const long long rest = i / (8 * (long long)nw);
@@ -52,7 +52,9 @@ __global__ void __launch_bounds__(256) pack_ops_kernel(const PackOp* __restrict_
                 else ks = k_real0 + (k - k_pad0);
                 float v = 0.0f;
                 if (ks >= 0 && ks < k_src && ng < n_src) v = src[(long long)ks * n_src + ng];
-                reinterpret_cast<__half*>(op.dst)[i] = __float2half_rn(v);
+                const __half h = __float2half_rn(v);
+                reinterpret_cast<__half*>(op.dst)[i] = h;
+                if (op.dst2) reinterpret_cast<__half*>(op.dst2)[i] = __float2half_rn(v - __half2float(h));
                 break;
             }
             case PK_TC_F32:           // copy with zero padding

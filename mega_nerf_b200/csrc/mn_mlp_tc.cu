@@ -104,6 +104,86 @@ bool build_plan(const NetDims& nd, TcPlan* p) {
     return true;
 }
 
+// ---- layer plan: networks wider than build_plan covers, one GEMM launch per Linear (mn_layer_gemm.cuh)
+enum { LB_ACT0 = 0, LB_ACT1 = 1, LB_G = 2 };     // activation buffers of a tile group: ping, pong, dir_a_encoding output
+
+struct LgGemm {
+    int n, n_blk;        // output columns; 256-column N blocks (the image and the output buffer are padded to n_blk * 256)
+    int nseg;
+    int src[2];          // SRC_H (the input buffer), SRC_XPE, SRC_XAUX
+    int k[2];            // K columns per segment (multiple of 16)
+    int w_off;           // byte offset of the weight image [n_blk][K/8][256][8] inside one precision plane
+    int bias_off;        // float offset of the bias (n_blk * 256 floats) inside the fp32 block
+    int relu;
+    int in, out;         // LB_* buffers read (SRC_H) and written
+};
+
+struct LayerPlan {
+    int n_gemm, n_trunk;
+    LgGemm g[kMaxGemm];
+    int L, kpe, kaux;
+    int plane_bytes;     // bytes of all weight images of one sub-module (one precision plane)
+    int f32_floats;      // fp32 block: biases, sigma_w [L], sigma_b (4), rgb_w [rgb_dim][rgb_in], rgb_b (32)
+    int sigma_w_off, rgb_w_off, rgb_b_off;
+    int rgb_in, h_last;  // rgb head input width; buffer of the last trunk activations
+    int rgb_src;         // buffer the rgb head reads
+    int x_tile_bytes;
+    int buf_cols[3];     // columns of each activation buffer (0: unused)
+};
+
+bool build_layer_plan(const NetDims& nd, LayerPlan* p) {
+    if (nd.L <= 512 || nd.L > 2048 || nd.L % 256 != 0 || nd.rgb_dim > MN_TC_RGB_MAX || nd.layers + 2 > kMaxGemm) return false;
+    if (nd.affine && nd.rgb_dim != 3) return false;
+    LayerPlan& P = *p;
+    P = LayerPlan{};
+    P.L = nd.L;
+    P.kpe = pad16(nd.in_xyz);
+    P.kaux = nd.aux > 0 ? pad16(nd.aux) : 0;
+    int woff = 0, foff = 0, ng = 0;
+    auto add = [&](int n, int s0, int k0, int s1, int k1, int relu, int in, int out) {
+        LgGemm& g = P.g[ng++];
+        g.n = n;
+        g.n_blk = (n + 255) / 256;
+        g.nseg = k1 > 0 ? 2 : 1;
+        g.src[0] = s0; g.k[0] = k0; g.src[1] = s1; g.k[1] = k1;
+        g.w_off = woff;
+        g.bias_off = foff;
+        g.relu = relu;
+        g.in = in;
+        g.out = out;
+        woff += (k0 + k1) * g.n_blk * 256 * 2;
+        foff += g.n_blk * 256;
+    };
+    for (int i = 0; i < nd.layers; ++i) {
+        const int in = (i + 1) & 1, out = i & 1;       // H_i -> buffer i % 2
+        if (i == 0) add(nd.L, SRC_XPE, P.kpe, 0, 0, 1, in, out);
+        else if ((nd.skip_mask >> i) & 1) add(nd.L, SRC_XPE, P.kpe, SRC_H, nd.L, 1, in, out);
+        else add(nd.L, SRC_H, nd.L, 0, 0, 1, in, out);
+    }
+    P.n_trunk = ng;
+    P.h_last = (nd.layers - 1) & 1;
+    P.buf_cols[0] = P.buf_cols[1] = nd.L;
+    if (nd.has_dir_a) {
+        // F goes to the other ping-pong buffer and G to its own, so the head still finds H_last for sigma
+        const int fb = P.h_last ^ 1;
+        add(nd.L, SRC_H, nd.L, 0, 0, 0, P.h_last, fb);
+        add(nd.L / 2, SRC_H, nd.L, SRC_XAUX, P.kaux, 1, fb, LB_G);
+        P.buf_cols[LB_G] = P.g[ng - 1].n_blk * 256;
+        P.rgb_src = LB_G;
+    } else {
+        P.rgb_src = P.h_last;
+    }
+    P.n_gemm = ng;
+    P.rgb_in = nd.rgb_in;
+    P.plane_bytes = woff;
+    P.sigma_w_off = foff;
+    P.rgb_w_off = foff + nd.L + 4;
+    P.rgb_b_off = P.rgb_w_off + nd.rgb_dim * nd.rgb_in;
+    P.f32_floats = P.rgb_b_off + MN_TC_RGB_MAX;
+    P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
+    return true;
+}
+
 // ------------------------------------------------------------------------------------------------
 // PTX wrappers
 // ------------------------------------------------------------------------------------------------
@@ -197,14 +277,14 @@ __device__ __forceinline__ void tc_emit_rgb(const MlpArgs& m, int sub, int64_t r
 // ------------------------------------------------------------------------------------------------
 // feature tiles
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int kpe, int kaux, int split,
-                                                           __half* __restrict__ ximg, int64_t plane_stride_halves) {
+// Feature tile `tile` (global index: routing, rows) stored as tile `out_tile` of ximg.
+__device__ __forceinline__ void tc_encode_tile(const MlpArgs& a, int kpe, int kaux, int split, __half* __restrict__ ximg,
+                                               int64_t plane_stride_halves, int64_t tile, int64_t out_tile) {
     extern __shared__ __align__(16) unsigned char sm_raw[];
     __half* img = reinterpret_cast<__half*>(sm_raw);                  // hi image, then lo image
     const int ktot = kpe + kaux;
     const NetDims& nd = a.nd;
     const int t = threadIdx.x;
-    const int64_t tile = blockIdx.x;
     const int64_t slot0 = tile * kTileM;
     const int64_t n_slots = a.counters ? a.counters[CNT_NSLOTS] : a.B;
     if (slot0 >= n_slots) return;
@@ -260,13 +340,24 @@ __global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int 
     __syncthreads();
     const int nvec = ktot * kTileM * 2 / 16;
     const uint4* s4 = reinterpret_cast<const uint4*>(img);
-    uint4* d4 = reinterpret_cast<uint4*>(ximg + tile * (int64_t)ktot * kTileM);
+    uint4* d4 = reinterpret_cast<uint4*>(ximg + out_tile * (int64_t)ktot * kTileM);
     for (int i = t; i < nvec; i += kTileM) d4[i] = s4[i];
     if (split) {
         const uint4* s4l = reinterpret_cast<const uint4*>(lo_img);
-        uint4* d4l = reinterpret_cast<uint4*>(ximg + plane_stride_halves + tile * (int64_t)ktot * kTileM);
+        uint4* d4l = reinterpret_cast<uint4*>(ximg + plane_stride_halves + out_tile * (int64_t)ktot * kTileM);
         for (int i = t; i < nvec; i += kTileM) d4l[i] = s4l[i];
     }
+}
+
+__global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int kpe, int kaux, int split,
+                                                           __half* __restrict__ ximg, int64_t plane_stride_halves) {
+    tc_encode_tile(a, kpe, kaux, split, ximg, plane_stride_halves, blockIdx.x, blockIdx.x);
+}
+
+// the layer-GEMM path (mn_layer_gemm.cuh): the tiles tile0 .. tile0 + gridDim.x - 1 of one tile group, stored from tile 0 of ximg
+__global__ void __launch_bounds__(kTileM) tc_layer_encode_kernel(const MlpArgs a, int kpe, int kaux, int split,
+                                                                 __half* __restrict__ ximg, int64_t plane_stride_halves, int64_t tile0) {
+    tc_encode_tile(a, kpe, kaux, split, ximg, plane_stride_halves, tile0 + blockIdx.x, blockIdx.x);
 }
 
 
@@ -406,11 +497,35 @@ int wg_launch(mn_ctx* ctx, const TcArgs& A, int64_t n_tiles128, cudaStream_t st)
 }
 
 #include "mn_train_tc.cuh"
+#include "mn_layer_gemm.cuh"
+
+// Workspace of the layer-GEMM path: per tile of a group, the feature tile and the activation buffers, each with its lo
+// plane under tc_f16x3.  Bounded by kLgGroupTiles, not by the call's rows.
+struct LgWorkspace {
+    int64_t group_tiles;
+    size_t x_bytes, buf_bytes[3], total;     // per plane
+    int planes;
+};
+LgWorkspace lg_workspace(const LayerPlan& P, int64_t n_tiles128, int precision) {
+    LgWorkspace w{};
+    w.group_tiles = n_tiles128 < kLgGroupTiles ? n_tiles128 : kLgGroupTiles;
+    w.planes = precision == MN_PREC_TC_F16X3 ? 2 : 1;
+    w.x_bytes = mn_align((size_t)w.group_tiles * P.x_tile_bytes, 1024);
+    w.total = w.x_bytes * w.planes;
+    for (int b = 0; b < 3; ++b) {
+        w.buf_bytes[b] = mn_align((size_t)w.group_tiles * P.buf_cols[b] * kTileM * 2, 1024);
+        w.total += w.buf_bytes[b] * w.planes;
+    }
+    w.total += 1024;
+    return w;
+}
 
 }  // namespace
 
 // =================================================================================================
 size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision) {
+    LayerPlan LP;
+    if (build_layer_plan(m->nd, &LP)) return lg_workspace(LP, n_tiles128, precision).total;
     TcPlan P;
     if (!build_plan(m->nd, &P)) return 0;
     const size_t planes = precision == MN_PREC_TC_F16X3 ? 2 : 1;
@@ -442,7 +557,49 @@ int mn_mlp_tp_program(const NetDims& nd, unsigned int* table_out, int cap_entrie
     return n <= cap_entries ? MN_OK : MN_ERR_WORKSPACE;
 }
 
+// Layer-GEMM networks: per sub-module [hi plane][lo plane][fp32 block], every weight image [n_blk][K/8][256][8] with its fp16
+// residual in the lo plane.  No tensor-core training images (train_tc_ok stays 0).
+static int layer_pack(mn_ctx* ctx, mn_model* m, int sub, const LayerPlan& P, cudaStream_t st) {
+    const NetDims& nd = m->nd;
+    const size_t sub_bytes = mn_align((size_t)P.plane_bytes * 2 + (size_t)P.f32_floats * 4, 256);
+    if (!m->tc_packed) {
+        MN_CUDA(ctx, cudaMalloc(&m->tc_packed, sub_bytes * m->d.n_sub));
+        MN_CUDA(ctx, cudaMemsetAsync(m->tc_packed, 0, sub_bytes * m->d.n_sub, st));
+        m->tc_sub_bytes = sub_bytes;
+    }
+    unsigned char* base = (unsigned char*)m->tc_packed + (size_t)sub * sub_bytes;
+    const float* Pk = m->packed + (size_t)sub * m->lay.total;
+    float* f32 = reinterpret_cast<float*>(base + (size_t)P.plane_bytes * 2);
+    auto pack = [&](const LgGemm& g, const float* wt, int k_src, int k_real0, int k_pad0, const float* bias) {
+        const int K = g.k[0] + (g.nseg > 1 ? g.k[1] : 0), np = g.n_blk * 256;
+        mn_pack_push(ctx, PackOp{wt, base + g.w_off, base + P.plane_bytes + g.w_off, (long long)np * K, PK_TC_HALF,
+                                 {g.n, k_src, np, K, k_real0, k_pad0, 256}});
+        mn_pack_push(ctx, PackOp{bias, f32 + g.bias_off, nullptr, (long long)np, PK_TC_F32, {g.n, 0, 0, 0, 0, 0, 0}});
+    };
+    int gi = 0;
+    for (int i = 0; i < nd.layers; ++i, ++gi) {
+        const bool has_pe = (i == 0) || ((nd.skip_mask >> i) & 1);
+        pack(P.g[gi], Pk + m->lay.w[i], m->lay.kin[i], has_pe ? nd.in_xyz : 0, has_pe ? P.kpe : 0, Pk + m->lay.b[i]);
+    }
+    if (nd.has_dir_a) {
+        pack(P.g[gi++], Pk + m->lay.final_w, nd.L, 0, 0, Pk + m->lay.final_b);
+        pack(P.g[gi++], Pk + m->lay.dira_w, nd.L + nd.aux, 0, 0, Pk + m->lay.dira_b);
+    }
+    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + P.sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
+    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + P.sigma_w_off + nd.L, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
+    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + P.rgb_w_off, nullptr, (long long)nd.rgb_dim * nd.rgb_in, PK_RGBW,
+                             {nd.rgb_in, nd.rgb_dim, 0, 0, 0, 0, 0}});
+    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + P.rgb_b_off, nullptr, MN_TC_RGB_MAX, PK_TC_F32, {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
+    m->tc_ready = 1;
+    m->train_tc_ok = 0;
+    return MN_OK;
+}
+
 int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
+    {
+        LayerPlan LP;
+        if (build_layer_plan(m->nd, &LP)) return layer_pack(ctx, m, sub, LP, st);
+    }
     TcPlan P;
     if (!build_plan(m->nd, &P)) {
         m->tc_ready = 0;
@@ -547,12 +704,107 @@ static bool tc_forward_args(const mn_model* m, const MlpArgs& a, int64_t n_tiles
     return true;
 }
 
+// Layer-GEMM path: the slot tiles in groups of kLgGroupTiles; per group one encoder launch, one GEMM launch per Linear and one
+// head launch.  The group count follows from the slot capacity, so a call is a static launch list (graph capture works).
+static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerPlan& P, int64_t n_tiles128, int precision,
+                        void* ws, size_t ws_bytes, cudaStream_t st) {
+    if (!m->tc_ready) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: weights not packed");
+    if (n_tiles128 <= 0) return MN_OK;
+    const LgWorkspace W = lg_workspace(P, n_tiles128, precision);
+    if (ws_bytes < W.total || !ws) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
+    const bool split = precision == MN_PREC_TC_F16X3;
+    unsigned char* wp = (unsigned char*)(((uintptr_t)ws + 1023) / 1024 * 1024);
+    __half* ximg = reinterpret_cast<__half*>(wp);
+    const int64_t x_lo = (int64_t)W.x_bytes;                 // lo plane of each region right after its hi plane
+    wp += W.x_bytes * W.planes;
+    unsigned char* buf[3];
+    for (int b = 0; b < 3; ++b) { buf[b] = wp; wp += W.buf_bytes[b] * W.planes; }
+
+    const size_t enc_sm = (size_t)P.x_tile_bytes * (split ? 2 : 1);
+    MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
+    const int gemm_sm = split ? LgShape<true>::smem : LgShape<false>::smem;
+    if (split) MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
+    else MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
+    const int n_gemm = a.sigma_only ? P.n_trunk : P.n_gemm;
+    const int64_t plane_halves = x_lo / 2;
+
+    mn_prof_begin(ctx, st);
+    for (int64_t t0 = 0; t0 < n_tiles128; t0 += W.group_tiles) {
+        const int64_t nt = n_tiles128 - t0 < W.group_tiles ? n_tiles128 - t0 : W.group_tiles;
+        tc_layer_encode_kernel<<<(unsigned)nt, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split ? 1 : 0, ximg, plane_halves, t0);
+        MN_LAUNCH_CHECK(ctx);
+        for (int gi = 0; gi < n_gemm; ++gi) {
+            const LgGemm& g = P.g[gi];
+            LgArgs G{};
+            G.m = a;
+            G.tile0 = t0;
+            G.n_tiles = nt;
+            G.wpack = (const unsigned char*)m->tc_packed;
+            G.sub_bytes = (int64_t)m->tc_sub_bytes;
+            G.w_lo = P.plane_bytes;
+            G.w_off = g.w_off;
+            G.k_tot = g.k[0] + (g.nseg > 1 ? g.k[1] : 0);
+            G.n_blk = g.n_blk;
+            G.n_out = g.n;
+            G.bias_off = g.bias_off;
+            G.f32_off = P.plane_bytes * 2;
+            G.relu = g.relu;
+            G.nseg = g.nseg;
+            for (int s = 0; s < g.nseg; ++s) {
+                G.ak[s] = g.k[s];
+                if (g.src[s] == SRC_H) {
+                    G.a[s] = buf[g.in];
+                    G.a_tile_bytes[s] = (int64_t)P.buf_cols[g.in] * kTileM * 2;
+                    G.a_lo[s] = (int64_t)W.buf_bytes[g.in];
+                } else {
+                    G.a[s] = (const unsigned char*)ximg + (g.src[s] == SRC_XAUX ? P.kpe * kTileM * 2 : 0);
+                    G.a_tile_bytes[s] = P.x_tile_bytes;
+                    G.a_lo[s] = x_lo;
+                }
+            }
+            G.out = buf[g.out];
+            G.out_tile_bytes = (int64_t)P.buf_cols[g.out] * kTileM * 2;
+            G.out_lo = (int64_t)W.buf_bytes[g.out];
+            const int64_t items = nt * g.n_blk;
+            const unsigned grid = (unsigned)(items < ctx->sm_count ? items : ctx->sm_count);
+            if (split) tc_layer_gemm_kernel<true><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
+            else tc_layer_gemm_kernel<false><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
+            MN_LAUNCH_CHECK(ctx);
+        }
+        LhArgs H{};
+        H.m = a;
+        H.tile0 = t0;
+        H.wpack = (const unsigned char*)m->tc_packed;
+        H.sub_bytes = (int64_t)m->tc_sub_bytes;
+        H.f32_off = P.plane_bytes * 2;
+        H.sigma_w_off = P.sigma_w_off;
+        H.rgb_w_off = P.rgb_w_off;
+        H.rgb_b_off = P.rgb_b_off;
+        H.h = buf[P.h_last];
+        H.h_tile_bytes = (int64_t)P.buf_cols[P.h_last] * kTileM * 2;
+        H.h_lo = split ? (int64_t)W.buf_bytes[P.h_last] : 0;
+        H.g = buf[P.rgb_src];
+        H.g_tile_bytes = (int64_t)P.buf_cols[P.rgb_src] * kTileM * 2;
+        H.g_lo = split ? (int64_t)W.buf_bytes[P.rgb_src] : 0;
+        H.L = P.L;
+        H.rgb_in = P.rgb_in;
+        tc_layer_head_kernel<<<(unsigned)nt, kTileM, 0, st>>>(H);
+        MN_LAUNCH_CHECK(ctx);
+    }
+    mn_prof_end(ctx, st);
+    return MN_OK;
+}
+
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws, size_t ws_bytes,
                      cudaStream_t st) {
+    {
+        LayerPlan LP;
+        if (build_layer_plan(a.nd, &LP)) return layer_launch(ctx, m, a, LP, n_tiles128, precision, ws, ws_bytes, st);
+    }
     TcArgs A;
     if (!tc_forward_args(m, a, n_tiles128, &A))
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
-                       "tensor-core MLP path covers layer_dim 64..256 (multiple of 64) or 512 and rgb_dim <= 32; "
+                       "tensor-core MLP path covers layer_dim 64..256 (multiple of 64), 512 or 768..2048 (multiple of 256) and rgb_dim <= 32; "
                        "use precision 'fp32' for this model");
     if (a.nd.L > 256 && precision == MN_PREC_TC_F16X3)
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,

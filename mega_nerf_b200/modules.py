@@ -26,7 +26,11 @@ _precision = os.environ.get('MN_B200_PRECISION', 'tc_f16')
 
 
 def set_precision(name: str) -> None:
-    """'fp32' (CUDA-core parity mode), 'tc_f16' (wgmma, 1 pass) or 'tc_f16x3' (wgmma, split)."""
+    """'fp32' (CUDA-core parity mode), 'tc_f16' (wgmma, 1 pass) or 'tc_f16x3' (wgmma, split).
+
+    Networks with layer_dim 768..2048 (a multiple of 256; the nerf, npp and mega-nerf-dense configs set 2048) run on the
+    layer-GEMM tensor-core path in 'tc_f16' and 'tc_f16x3' ('tc_f16x3' is the parity-grade mode there); 'fp32' covers
+    layer_dim <= 512 only and refuses them."""
     global _precision
     if name not in K.PRECISIONS:
         raise ValueError(f'unknown precision {name!r}; choose from {sorted(K.PRECISIONS)}')
