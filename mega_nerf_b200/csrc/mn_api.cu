@@ -677,9 +677,9 @@ int mn_model_forward_train_tc(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
                               size_t workspace_bytes, void* stream) {
     if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_train_tc: tape is NULL");
     if (!m || !m->train_tc_ok)
-        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 with a direction / appearance head, rgb_dim 3 "
-                                                "or a raw SH head (rgb_dim <= 32), no affine appearance; use the fp32 training entry "
-                                                "points for this model");
+        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 or 768..2048 (a multiple of 256) with a direction "
+                                                "/ appearance head, rgb_dim 3 or a raw SH head (rgb_dim <= 32), no affine appearance; use "
+                                                "the fp32 training entry points for this model");
     return model_forward_impl(ctx, m, rows, B, use_coarse, 0, sigma_noise_d, MN_PREC_FP32, out_d, workspace_d, workspace_bytes, tape_d,
                               tape_bytes, stream, 1);
 }

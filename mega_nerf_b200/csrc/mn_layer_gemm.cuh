@@ -20,7 +20,14 @@
 //     and the epilogue stores the fp16 residual of every activation in the output's lo plane.
 //   tc_layer_head_kernel   one thread per tile row, CUDA cores, fp32: sigma = the last trunk activations . sigma_w + bias
 //                          (+ sigma_noise) -> ReLU / shifted softplus; rgb = W_rgb G (or W_rgb H_last without dir_a_encoding)
-//                          -> tc_emit_rgb.  sigma_only stops after sigma.
+//                          -> tc_emit_rgb.  sigma_only stops after sigma.  A recording (training) call also fills the tile's
+//                          fp32 head block of the tensor-core tape.
+//
+// Training (precision tc_f16, mn_train_tc.cuh): the recording forward is the same launch list with the encoder tiles and every
+// GEMM's output written to the tape instead of the group buffers.  The backward runs the data-gradient chain through
+// tc_layer_gemm_kernel<false, true>: A = the scaled fp16 gradient image of a Linear's output, B = a transposed weight image
+// ([in/256][out/8][256][8]), and an epilogue that adds S dsigma x sigma_w (last trunk layer) and applies the ReLU mask read
+// from the activation tape at the (row, column) it stores.  tc_layer_head_dgrad_kernel is its head stage.
 //
 // A Linear has one or two K segments: the tile's encoder features (kpe or kaux columns of the feature tile image) and / or
 // the previous activations (the layer plan's input buffer).  Skip layers read [PE, H], dir_a_encoding reads [F, aux].
@@ -42,6 +49,14 @@ struct LgArgs {
     int64_t a_tile_bytes[2], a_lo[2];    // tile stride and lo-plane offset of each segment's source
     unsigned char* out;                  // output image of tile 0 of the group, [n_blk * 256 / 8][128][8]
     int64_t out_tile_bytes, out_lo;
+    // kDgrad: no bias.  mask: activation image of the output (tile 0 of the group), NULL for xyz_encoding_final (no
+    // activation).  dsig: d sigma pre-activation per slot (unscaled fp32, tile stride dsig_tile_floats), NULL except for the
+    // last trunk layer, whose sigma weights sit in the fp32 block at bias_off.  scale: the gradient scale S.
+    const unsigned char* mask;
+    int64_t mask_tile_bytes;
+    const float* dsig;
+    int64_t dsig_tile_floats;
+    const float* scale;
 };
 
 template <bool kSplit>
@@ -69,7 +84,7 @@ __device__ __forceinline__ void lg_walk(const LgArgs& A, int64_t lt, const unsig
     }
 }
 
-template <bool kSplit>
+template <bool kSplit, bool kDgrad = false>
 __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_layer_gemm_kernel(const LgArgs A) {
     extern __shared__ __align__(1024) unsigned char smem[];
     using S = LgShape<kSplit>;
@@ -167,7 +182,55 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_layer_gemm_kernel(const L
 
             // epilogue: bias, activation, fp16 [+ residual] -> output tile image in HBM
             const float* bias = reinterpret_cast<const float*>(A.wpack + (size_t)sub * A.sub_bytes + A.f32_off) + A.bias_off + nb * kLgBlock;
-            unsigned char* o = A.out + lt * A.out_tile_bytes + (size_t)nb * (kLgBlock / 8) * (kTileM * 16) + (size_t)ra * 16 + q4 * 4;
+            const size_t po = (size_t)nb * (kLgBlock / 8) * (kTileM * 16) + (size_t)ra * 16 + q4 * 4;
+            unsigned char* o = A.out + lt * A.out_tile_bytes + po;
+            if constexpr (kDgrad) {
+                // data gradient: the accumulators hold S dH; [+ S dsigma x sigma_w]; dZ = dH where the activation is > 0
+                const unsigned char* mk = A.mask ? A.mask + lt * A.mask_tile_bytes + po : nullptr;
+                float dsa = 0.0f, dsb = 0.0f;
+                if (A.dsig) {
+                    const float S = *A.scale;
+                    dsa = A.dsig[lt * A.dsig_tile_floats + ra] * S;
+                    dsb = A.dsig[lt * A.dsig_tile_floats + ra + 8] * S;
+                }
+                // the mask and sigma-weight loads of JB column groups are issued together, as the forward's bias loads
+                constexpr int JB = 8;
+#pragma unroll
+                for (int j0 = 0; j0 < 32; j0 += JB) {
+                    __half2 ma[JB], mb[JB];
+                    float2 sv[JB];
+#pragma unroll
+                    for (int jj = 0; jj < JB; ++jj) {
+                        const int j = j0 + jj;
+                        ma[jj] = mb[jj] = __float2half2_rn(1.0f);
+                        sv[jj] = make_float2(0.0f, 0.0f);
+                        if (nb * kLgBlock + 8 * j >= A.n_out) continue;
+                        if (mk) {
+                            ma[jj] = *reinterpret_cast<const __half2*>(mk + (size_t)j * (kTileM * 16));
+                            mb[jj] = *reinterpret_cast<const __half2*>(mk + (size_t)j * (kTileM * 16) + 128);
+                        }
+                        if (A.dsig) sv[jj] = __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4));
+                    }
+#pragma unroll
+                    for (int jj = 0; jj < JB; ++jj) {
+                        const int j = j0 + jj;
+                        if (nb * kLgBlock + 8 * j >= A.n_out) continue;
+                        float a0 = acc[4 * j], a1 = acc[4 * j + 1], b0 = acc[4 * j + 2], b1 = acc[4 * j + 3];
+                        if (A.dsig) {
+                            a0 = fmaf(dsa, sv[jj].x, a0); a1 = fmaf(dsa, sv[jj].y, a1);
+                            b0 = fmaf(dsb, sv[jj].x, b0); b1 = fmaf(dsb, sv[jj].y, b1);
+                        }
+                        if (!(__low2float(ma[jj]) > 0.0f)) a0 = 0.0f;
+                        if (!(__high2float(ma[jj]) > 0.0f)) a1 = 0.0f;
+                        if (!(__low2float(mb[jj]) > 0.0f)) b0 = 0.0f;
+                        if (!(__high2float(mb[jj]) > 0.0f)) b1 = 0.0f;
+                        unsigned char* p = o + (size_t)j * (kTileM * 16);
+                        *reinterpret_cast<uint32_t*>(p) = pack_h2(a0, a1);
+                        *reinterpret_cast<uint32_t*>(p + 128) = pack_h2(b0, b1);
+                    }
+                }
+                continue;
+            }
             constexpr int JB = 8;                // column groups whose bias loads are issued together
 #pragma unroll
             for (int j0 = 0; j0 < 32; j0 += JB) {
@@ -209,6 +272,7 @@ struct LhArgs {
     const unsigned char* g;                           // rgb head input: G, or the last trunk activations
     int64_t g_tile_bytes, g_lo;
     int L, rgb_in;
+    float* tape_f32;                                  // recording call: fp32 head blocks of the tape [tiles][MN_TC_F32_ROWS][128], or NULL
 };
 
 // 8 consecutive columns c0 .. c0 + 7 of row t of a tile image, as fp32 (hi + lo when the lo plane exists)
@@ -240,7 +304,15 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_kernel(const LhArgs A) {
     const int64_t n_slots = A.m.counters ? A.m.counters[CNT_NSLOTS] : A.m.B;
     const int64_t slot = tile * kTileM + t;
     const int64_t row = A.m.row_of_slot(slot, n_slots);
-    if (row < 0) return;
+    float* tf = A.tape_f32 ? A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + t : nullptr;
+    if (row < 0) {
+        if (tf) {       // padding slot: finite values for the backward's head stage (its upstream gradient is zero)
+            tf[MN_TC_F32_SIGMA * kTileM] = 0.0f;
+            for (int c = 0; c < 3; ++c) tf[(MN_TC_F32_RGB + c) * kTileM] = 0.5f;
+            tf[MN_TC_F32_ID * kTileM] = 0.0f;
+        }
+        return;
+    }
     const int sub = A.m.sub_of_tile(tile);
     const float* f32 = reinterpret_cast<const float*>(A.wpack + (size_t)sub * A.sub_bytes + A.f32_off);
     float v[8];
@@ -256,6 +328,10 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_kernel(const LhArgs A) {
     }
     s = s + sw[A.L];                                  // sigma bias is stored right after sigma_w
     if (A.m.sigma_noise) s = s + A.m.sigma_noise[row];
+    if (tf) {
+        tf[MN_TC_F32_SIGMA * kTileM] = s;                 // pre-activation (with the density noise)
+        tf[MN_TC_F32_ID * kTileM] = A.m.nd.app > 0 ? A.m.src.index(row) : 0.0f;
+    }
     const float sg = A.m.nd.softplus ? mn_softplus_shifted(s) : fmaxf(s, 0.0f);
     if (A.m.sigma_only) {
         const int64_t o = (A.m.scatter ? row : slot) * A.m.out_cols;
@@ -287,5 +363,60 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_kernel(const LhArgs A) {
     uint32_t raw[MN_TC_RGB_MAX];
 #pragma unroll
     for (int r = 0; r < MN_TC_RGB_MAX; ++r) raw[r] = __float_as_uint(acc[r]);
-    tc_emit_rgb(A.m, sub, row, slot, raw, f32 + A.rgb_b_off, sg);
+    tc_emit_rgb(A.m, sub, row, slot, raw, f32 + A.rgb_b_off, sg, tf ? tf + MN_TC_F32_RGB * kTileM : nullptr);
+}
+
+// ---- training backward: head stage of one tile group, one thread per tile row (CUDA cores, fp32).  Upstream gradient x blend
+// weight -> sigmoid' (colour head) or the raw SH coefficients / softplus' or ReLU' -> the head-gradient block (unscaled) and
+// dZ_G = mask(G > 0) (W_rgb^T d rgb) as a scaled fp16 tile image; per-image sums of dZ_G rows for the appearance embedding.
+struct LdArgs {
+    MlpArgs m;                                        // routing, blend weights, nd
+    int64_t tile0;
+    const float* grad_out;                            // [rows][rgb_dim + 1]
+    const float* tape_f32;                            // fp32 head blocks of the tape (all tiles)
+    const unsigned char* g;                           // G activation image of tile 0 of the group (tape)
+    int64_t g_tile_bytes;
+    const unsigned char* wpack;                       // forward pack: rgb weights [rgb_dim][L/2] in the fp32 block
+    int64_t sub_bytes;
+    int f32_off, rgb_w_off, half;
+    float* gf32;                                      // head-gradient blocks of the group [tiles][mn_tc_g32_rows][128]
+    unsigned char* dz;                                // dZ_G images of the group [tiles][L/2/8][128][8], S x dZ in fp16
+    float* emb_sum;                                   // [n_sub][app_count][L/2] or NULL
+    const float* scale;
+};
+
+__global__ void __launch_bounds__(kTileM) tc_layer_head_dgrad_kernel(const LdArgs A) {
+    const int t = threadIdx.x, lane = t & 31;
+    const int64_t tile = A.tile0 + blockIdx.x;
+    const int64_t n_slots = A.m.counters ? A.m.counters[CNT_NSLOTS] : A.m.B;
+    if (tile * kTileM >= n_slots) return;
+    const int64_t slot = tile * kTileM + t;
+    const int64_t row = A.m.row_of_slot(slot, n_slots);
+    const int sub = A.m.sub_of_tile(tile);
+    const int R = A.m.nd.rgb_dim, half = A.half;
+    const float S = *A.scale;
+    const float* tf = A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + t;
+    float d[MN_TC_RGB_MAX];
+    const float ds = tc_head_grad(A.m, A.grad_out, row, slot, tf, d);
+    float* tg = A.gf32 + (size_t)blockIdx.x * mn_tc_g32_rows(R) * kTileM + t;
+    tg[MN_TC_G32_SIGMA * kTileM] = ds;
+#pragma unroll
+    for (int c = 0; c < MN_TC_RGB_MAX; ++c) {
+        if (c >= R) break;
+        tg[(MN_TC_G32_RGB + c) * kTileM] = d[c];
+    }
+    const int id = (int)tf[MN_TC_F32_ID * kTileM];
+    const float* Wr = reinterpret_cast<const float*>(A.wpack + (size_t)sub * A.sub_bytes + A.f32_off) + A.rgb_w_off;
+    const unsigned char* gimg = A.g + (int64_t)blockIdx.x * A.g_tile_bytes + (size_t)t * 16;
+    unsigned char* dimg = A.dz + (int64_t)blockIdx.x * half * (kTileM * 2) + (size_t)t * 16;
+    float* sums = A.emb_sum ? A.emb_sum + (size_t)sub * A.m.nd.app_count * half : nullptr;
+    for (int k0 = 0; k0 < half; k0 += 8) {
+        float v[8];
+        tc_rgb_dgrad8(Wr, half, k0, d, R, gimg + (size_t)(k0 >> 3) * (kTileM * 16), v);
+        if (sums) tc_emb_sums8(sums + k0, half, row >= 0, id, lane, v);
+        uint32_t pk[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) pk[e] = pack_h2(v[2 * e] * S, v[2 * e + 1] * S);
+        *reinterpret_cast<uint4*>(dimg + (size_t)(k0 >> 3) * (kTileM * 16)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+    }
 }

@@ -557,8 +557,60 @@ int mn_mlp_tp_program(const NetDims& nd, unsigned int* table_out, int cap_entrie
     return n <= cap_entries ? MN_OK : MN_ERR_WORKSPACE;
 }
 
+// ---- tensor-core training of layer-GEMM networks: the shapes the backward covers, and its transposed weight images
+static bool layer_train_ok(const NetDims& nd) {
+    return nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers >= 2;
+}
+
+// Per sub-module: the data-gradient chain's B operands, each the transposed weight [in/256][out/8][256][8] fp16 (dir_a_encoding
+// restricted to its L feature columns, xyz_encoding_final, trunk layers layers-1 .. 1 restricted to their hidden columns), then
+// an fp32 block with sigma_w [L].
+struct LgDgrad {
+    int w_dira, w_final, w_layer[MN_MAX_LAYERS], f32_off;
+    size_t sub_bytes;
+};
+static LgDgrad lg_dgrad_layout(const NetDims& nd) {
+    LgDgrad D{};
+    const int L = nd.L;
+    int off = 0;
+    D.w_dira = off;  off += L * (L / 2) * 2;
+    D.w_final = off; off += L * L * 2;
+    for (int l = nd.layers - 1; l >= 1; --l) { D.w_layer[l] = off; off += L * L * 2; }
+    D.f32_off = off;
+    D.sub_bytes = mn_align((size_t)off + (size_t)L * sizeof(float), 256);
+    return D;
+}
+
+static void layer_pack_dgrad(mn_ctx* ctx, mn_model* m, int sub) {
+    const NetDims& nd = m->nd;
+    const LgDgrad D = lg_dgrad_layout(nd);
+    const int L = nd.L;
+    unsigned char* db = (unsigned char*)m->tc_dgrad + (size_t)sub * D.sub_bytes;
+    const float* Q = m->packed_bwd + (size_t)sub * m->blay.total;
+    // element (n = input column, k = output channel) = W[k][n]: the [out][in] sub-matrix is the K-major source of PK_TC_HALF
+    auto img = [&](int w_off, const float* w, int n_out) {
+        mn_pack_push(ctx, PackOp{w, db + w_off, nullptr, (long long)L * n_out, PK_TC_HALF, {L, n_out, L, n_out, 0, 0, 256}});
+    };
+    img(D.w_dira, Q + m->blay.dira_f, L / 2);
+    img(D.w_final, Q + m->blay.final_w, L);
+    for (int l = nd.layers - 1; l >= 1; --l) img(D.w_layer[l], Q + m->blay.w[l], L);
+    mn_pack_push(ctx, PackOp{m->packed + (size_t)sub * m->lay.total + m->lay.sigma_w, db + D.f32_off, nullptr, (long long)L, PK_TC_F32,
+                             {L, 0, 0, 0, 0, 0, 0}});
+}
+
+// The transposed images cost as much as the forward images again, so they are allocated and packed by the first recording call
+// (inference-only users never hold them); from then on every mn_model_set_weights repacks them with the forward images.
+static int layer_dgrad_ready(mn_ctx* ctx, mn_model* m, cudaStream_t st) {
+    if (m->tc_dgrad) return MN_OK;
+    const LgDgrad D = lg_dgrad_layout(m->nd);
+    MN_CUDA(ctx, cudaMalloc(&m->tc_dgrad, D.sub_bytes * m->d.n_sub));
+    m->tc_dgrad_sub_bytes = D.sub_bytes;
+    for (int s = 0; s < m->d.n_sub; ++s) layer_pack_dgrad(ctx, m, s);
+    return mn_pack_flush(ctx, st);
+}
+
 // Layer-GEMM networks: per sub-module [hi plane][lo plane][fp32 block], every weight image [n_blk][K/8][256][8] with its fp16
-// residual in the lo plane.  No tensor-core training images (train_tc_ok stays 0).
+// residual in the lo plane.  Training images: see layer_dgrad_ready.
 static int layer_pack(mn_ctx* ctx, mn_model* m, int sub, const LayerPlan& P, cudaStream_t st) {
     const NetDims& nd = m->nd;
     const size_t sub_bytes = mn_align((size_t)P.plane_bytes * 2 + (size_t)P.f32_floats * 4, 256);
@@ -591,7 +643,8 @@ static int layer_pack(mn_ctx* ctx, mn_model* m, int sub, const LayerPlan& P, cud
                              {nd.rgb_in, nd.rgb_dim, 0, 0, 0, 0, 0}});
     mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + P.rgb_b_off, nullptr, MN_TC_RGB_MAX, PK_TC_F32, {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
     m->tc_ready = 1;
-    m->train_tc_ok = 0;
+    m->train_tc_ok = layer_train_ok(nd) ? 1 : 0;
+    if (m->train_tc_ok && m->tc_dgrad) layer_pack_dgrad(ctx, m, sub);
     return MN_OK;
 }
 
@@ -706,12 +759,14 @@ static bool tc_forward_args(const mn_model* m, const MlpArgs& a, int64_t n_tiles
 
 // Layer-GEMM path: the slot tiles in groups of kLgGroupTiles; per group one encoder launch, one GEMM launch per Linear and one
 // head launch.  The group count follows from the slot capacity, so a call is a static launch list (graph capture works).
+// tape != NULL (recording call, tc_f16): the encoder tiles, every GEMM's output (image gi of the tile's activation record) and
+// the fp32 head blocks go to the tape instead of the workspace, which is not used.
 static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerPlan& P, int64_t n_tiles128, int precision,
-                        void* ws, size_t ws_bytes, cudaStream_t st) {
+                        void* ws, size_t ws_bytes, cudaStream_t st, const TrainTcTape* tape = nullptr) {
     if (!m->tc_ready) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: weights not packed");
     if (n_tiles128 <= 0) return MN_OK;
     const LgWorkspace W = lg_workspace(P, n_tiles128, precision);
-    if (ws_bytes < W.total || !ws) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
+    if (!tape && (ws_bytes < W.total || !ws)) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
     const bool split = precision == MN_PREC_TC_F16X3;
     unsigned char* wp = (unsigned char*)(((uintptr_t)ws + 1023) / 1024 * 1024);
     __half* ximg = reinterpret_cast<__half*>(wp);
@@ -719,6 +774,7 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
     wp += W.x_bytes * W.planes;
     unsigned char* buf[3];
     for (int b = 0; b < 3; ++b) { buf[b] = wp; wp += W.buf_bytes[b] * W.planes; }
+    const int64_t act_tile = tape ? (int64_t)mn_train_tc_act_tile_bytes(m) : 0;
 
     const size_t enc_sm = (size_t)P.x_tile_bytes * (split ? 2 : 1);
     MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
@@ -731,6 +787,8 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
     mn_prof_begin(ctx, st);
     for (int64_t t0 = 0; t0 < n_tiles128; t0 += W.group_tiles) {
         const int64_t nt = n_tiles128 - t0 < W.group_tiles ? n_tiles128 - t0 : W.group_tiles;
+        unsigned char* rec = tape ? tape->act + t0 * act_tile : nullptr;      // activation record of the group's first tile
+        if (tape) ximg = reinterpret_cast<__half*>(tape->xreg + t0 * (int64_t)P.x_tile_bytes);
         tc_layer_encode_kernel<<<(unsigned)nt, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split ? 1 : 0, ximg, plane_halves, t0);
         MN_LAUNCH_CHECK(ctx);
         for (int gi = 0; gi < n_gemm; ++gi) {
@@ -765,6 +823,13 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
             G.out = buf[g.out];
             G.out_tile_bytes = (int64_t)P.buf_cols[g.out] * kTileM * 2;
             G.out_lo = (int64_t)W.buf_bytes[g.out];
+            if (tape) {                 // GEMM gi reads image gi - 1 (SRC_H) and writes image gi of the activation record
+                for (int s = 0; s < g.nseg; ++s)
+                    if (g.src[s] == SRC_H) { G.a[s] = rec + mn_tc_img_off(gi - 1, P.L); G.a_tile_bytes[s] = act_tile; G.a_lo[s] = 0; }
+                G.out = rec + mn_tc_img_off(gi, P.L);
+                G.out_tile_bytes = act_tile;
+                G.out_lo = 0;
+            }
             const int64_t items = nt * g.n_blk;
             const unsigned grid = (unsigned)(items < ctx->sm_count ? items : ctx->sm_count);
             if (split) tc_layer_gemm_kernel<true><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
@@ -788,6 +853,12 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
         H.g_lo = split ? (int64_t)W.buf_bytes[P.rgb_src] : 0;
         H.L = P.L;
         H.rgb_in = P.rgb_in;
+        if (tape) {
+            H.h = rec + mn_tc_img_off(a.nd.layers - 1, P.L);
+            H.g = rec + mn_tc_img_off(a.nd.layers + 1, P.L);
+            H.h_tile_bytes = H.g_tile_bytes = act_tile;
+            H.tape_f32 = tape->f32;
+        }
         tc_layer_head_kernel<<<(unsigned)nt, kTileM, 0, st>>>(H);
         MN_LAUNCH_CHECK(ctx);
     }
@@ -834,6 +905,8 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
 // tensor-core training path: host side (kernels in mn_train_tc.cuh)
 // =================================================================================================
 size_t mn_train_tc_x_tile_bytes(const mn_model* m) {
+    LayerPlan LP;
+    if (build_layer_plan(m->nd, &LP)) return (size_t)LP.x_tile_bytes;
     TcPlan P;
     return build_plan(m->nd, &P) ? (size_t)P.x_tile_bytes : 0;
 }
@@ -845,10 +918,18 @@ size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
 // recording forward: encoder tiles and every layer's activations land in the caller's tape
 int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
     TcArgs A;
-    if (!m->train_tc_ok || !tc_forward_args(m, a, n_tiles128, &A))
-        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 with a direction / appearance head and rgb_dim 3 "
-                                                "or a raw SH head (rgb_dim <= 32), no affine appearance; use train precision 'fp32'");
+    LayerPlan LP;
+    const bool layer = build_layer_plan(a.nd, &LP);
+    if (!m->train_tc_ok || (!layer && !tc_forward_args(m, a, n_tiles128, &A)))
+        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 or 768..2048 (a multiple of 256) with a direction / "
+                                                "appearance head and rgb_dim 3 or a raw SH head (rgb_dim <= 32), no affine appearance; "
+                                                "use train precision 'fp32'");
     if (n_tiles128 <= 0) return MN_OK;
+    if (layer) {
+        const int rc = layer_dgrad_ready(ctx, m, st);
+        if (rc) return rc;
+        return layer_launch(ctx, m, a, LP, n_tiles128, MN_PREC_TC_F16, nullptr, 0, st, &tape);
+    }
     A.ximg = reinterpret_cast<const __half*>(tape.xreg);
     A.x_plane_halves = 0;
     A.tape_act = tape.act;
@@ -870,18 +951,224 @@ static size_t train_tc_emb_floats(const mn_model* m) {
 static size_t train_tc_head_grad_bytes(const mn_model* m, int64_t n_tiles128) {
     return mn_align((size_t)n_tiles128 * mn_tc_g32_rows(m->nd.rgb_dim) * kTileM * sizeof(float));
 }
+// Layer-GEMM networks: gradient images of one tile group only (dZ_G and two ping-pong L-column buffers), so the workspace is
+// bounded by kLgGroupTiles, not by the row count.
+static int64_t lg_train_group_tiles(int64_t n_tiles128) { return n_tiles128 < kLgGroupTiles ? n_tiles128 : kLgGroupTiles; }
+static size_t lg_train_dz_bytes(const mn_model* m, int64_t n_tiles128) {
+    return mn_align((size_t)lg_train_group_tiles(n_tiles128) * (m->nd.L / 2) * kTileM * 2) +
+           2 * mn_align((size_t)lg_train_group_tiles(n_tiles128) * m->nd.L * kTileM * 2);
+}
 size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
+    LayerPlan LP;
+    if (build_layer_plan(m->nd, &LP))
+        return lg_train_dz_bytes(m, n_tiles128) + train_tc_head_grad_bytes(m, lg_train_group_tiles(n_tiles128)) +
+               mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) + 1024;
     return mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m)) + train_tc_head_grad_bytes(m, n_tiles128) +
            mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) + 1024;
+}
+
+// ---- backward of a layer-GEMM network, one tile group at a time: head stage -> per Linear (output side first) the weight
+// gradient from its dZ image, then the data-gradient GEMM that produces the next dZ in the other ping-pong buffer; then the
+// sigma / rgb head weight gradients.  dZ of Linear l is consumed by its weight gradient before the buffer is overwritten.
+static int layer_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, const LayerPlan& P, int64_t n_tiles128, const TrainTcTape& tape,
+                          void* ws, cudaStream_t st) {
+    const NetDims& nd = a.nd;
+    const int L = nd.L, half = L / 2, rows = mn_tc_g32_rows(nd.rgb_dim);
+    const int64_t gt = lg_train_group_tiles(n_tiles128);
+    const int64_t act_tile = (int64_t)mn_train_tc_act_tile_bytes(m);
+    const LgDgrad D = lg_dgrad_layout(nd);
+    char* wp = (char*)(((uintptr_t)ws + 255) / 256 * 256);
+    unsigned char* dzg = (unsigned char*)wp;              wp += mn_align((size_t)gt * half * kTileM * 2);
+    unsigned char* pp[2];
+    for (int b = 0; b < 2; ++b) { pp[b] = (unsigned char*)wp; wp += mn_align((size_t)gt * L * kTileM * 2); }
+    float* gf32 = (float*)wp;                             wp += train_tc_head_grad_bytes(m, gt);
+    float* emb_sum = (float*)wp;                          wp += mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) - 256;
+    float* scale = (float*)wp;
+    unsigned* maxbits = reinterpret_cast<unsigned*>(scale + 1);
+    if (train_tc_emb_floats(m)) MN_CUDA(ctx, cudaMemsetAsync(emb_sum, 0, train_tc_emb_floats(m) * sizeof(float), st));
+    MN_CUDA(ctx, cudaMemsetAsync(maxbits, 0, sizeof(unsigned), st));
+
+    mn_prof_begin(ctx, st);
+    {
+        const int64_t n = a.grad_rows * a.out_cols;
+        const int64_t blocks = std::min<int64_t>(std::max<int64_t>(mn_cdiv(n, (int64_t)256 * 16), 1), (int64_t)ctx->sm_count * 4);
+        tc_grad_absmax_kernel<<<(unsigned)blocks, 256, 0, st>>>(a.grad_out, n, maxbits);
+        MN_LAUNCH_CHECK(ctx);
+        tc_grad_scale_kernel<<<1, 32, 0, st>>>(maxbits, scale);
+        MN_LAUNCH_CHECK(ctx);
+    }
+    MlpArgs mm{};
+    mm.nd = nd;
+    mm.slot_row = a.slot_row;
+    mm.slot_w = a.slot_w;
+    mm.counters = a.counters;
+    mm.n_sub = a.n_sub;
+    mm.fixed_sub = a.fixed_sub;
+    mm.B = a.B;
+    mm.out_cols = a.out_cols;
+    const int n_sub = a.counters ? a.n_sub : 1;
+    const int64_t tiles_used = a.counters ? n_tiles128 : mn_cdiv(a.B, (int64_t)kTileM);
+    constexpr int gemm_sm = LgShape<false>::smem;
+    MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
+    const int wg_smem = 2 * kWgStageBytes + 6144 + 256;
+    MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
+
+    for (int64_t t0 = 0; t0 < tiles_used; t0 += gt) {
+        const int64_t nt = tiles_used - t0 < gt ? tiles_used - t0 : gt;
+        const unsigned char* rec = tape.act + t0 * act_tile;
+        // ---- head stage
+        {
+            LdArgs H{};
+            H.m = mm;
+            H.tile0 = t0;
+            H.grad_out = a.grad_out;
+            H.tape_f32 = tape.f32;
+            H.g = rec + mn_tc_img_off(nd.layers + 1, L);
+            H.g_tile_bytes = act_tile;
+            H.wpack = (const unsigned char*)m->tc_packed;
+            H.sub_bytes = (int64_t)m->tc_sub_bytes;
+            H.f32_off = P.plane_bytes * 2;
+            H.rgb_w_off = P.rgb_w_off;
+            H.half = half;
+            H.gf32 = gf32;
+            H.dz = dzg;
+            H.emb_sum = nd.app_in_dira ? emb_sum : nullptr;
+            H.scale = scale;
+            tc_layer_head_dgrad_kernel<<<(unsigned)nt, kTileM, 0, st>>>(H);
+            MN_LAUNCH_CHECK(ctx);
+        }
+        // ---- weight gradient of one Linear: dz = its output gradient images (n_out columns), segments (x_region, x_off, columns,
+        // weight columns, first weight column); the first segment owns the bias
+        struct Seg { int x_region, x_off, n, n_real, in0; };
+        auto wgrad = [&](const unsigned char* dz, int n_out, int w, int k_in, int b, Seg s0, Seg s1, int nseg) {
+            WgArgs W{};
+            const Seg seg[2] = {s0, s1};
+            for (int s = 0; s < nseg; ++s) {
+                WgItem& it = W.item[s];
+                it.dz_off = 0;
+                it.x_region = seg[s].x_region;
+                it.x_off = seg[s].x_off;
+                it.n = seg[s].n;
+                it.n_real = seg[s].n_real;
+                it.w_off = w + seg[s].in0;
+                it.k_in = k_in;
+                it.b_off = s == 0 ? b : -1;
+                W.n_chunks[s] = (seg[s].n + 255) / 256;
+            }
+            const int items = (n_out / 128) * (W.n_chunks[0] + W.n_chunks[1]);
+            W.n_items = items;
+            W.act = tape.act;
+            W.dz = dz;
+            W.xreg = tape.xreg;
+            W.act_tile_bytes = act_tile;
+            W.x_tile_bytes = P.x_tile_bytes;
+            W.dz_tile_bytes = (int64_t)n_out * kTileM * 2;
+            W.t_min = t0;
+            W.t_max = t0 + nt;
+            W.counters = a.counters;
+            W.n_tiles = tiles_used;
+            W.fixed_sub = a.fixed_sub;
+            W.gw = a.gw;
+            W.sub_stride = a.lay.total;
+            W.scale = scale;
+            // about one CTA per SM: every CTA flushes its 128 x 256 accumulators with fp32 atomics once
+            const int64_t chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count, (int64_t)items));
+            W.chunk_tiles = (int)mn_cdiv(nt, chunks);
+            tc_wgrad_kernel<true><<<dim3((unsigned)chunks, (unsigned)items, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
+            MN_LAUNCH_CHECK(ctx);
+        };
+        // ---- data gradient: dz_out = [mask](dz_in W^T) [+ S dsigma x sigma_w]
+        auto dgrad = [&](const unsigned char* dz_in, int k, int w_off, unsigned char* dz_out, int mask_img, bool sigma) {
+            LgArgs G{};
+            G.m = mm;
+            G.tile0 = t0;
+            G.n_tiles = nt;
+            G.wpack = (const unsigned char*)m->tc_dgrad;
+            G.sub_bytes = (int64_t)D.sub_bytes;
+            G.w_off = w_off;
+            G.k_tot = k;
+            G.n_blk = L / kLgBlock;
+            G.n_out = L;
+            G.bias_off = 0;
+            G.f32_off = D.f32_off;
+            G.nseg = 1;
+            G.a[0] = dz_in;
+            G.ak[0] = k;
+            G.a_tile_bytes[0] = (int64_t)k * kTileM * 2;
+            G.out = dz_out;
+            G.out_tile_bytes = (int64_t)L * kTileM * 2;
+            G.mask = mask_img >= 0 ? rec + mn_tc_img_off(mask_img, L) : nullptr;
+            G.mask_tile_bytes = act_tile;
+            G.dsig = sigma ? gf32 + MN_TC_G32_SIGMA * kTileM : nullptr;
+            G.dsig_tile_floats = (int64_t)rows * kTileM;
+            G.scale = scale;
+            const int64_t items = nt * G.n_blk;
+            const unsigned grid = (unsigned)(items < ctx->sm_count ? items : ctx->sm_count);
+            tc_layer_gemm_kernel<false, true><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
+            MN_LAUNCH_CHECK(ctx);
+        };
+        const Seg none{0, 0, 0, 0, 0};
+        const int xaux = (P.kpe / 8) * (kTileM * 16);
+        auto hseg = [&](int img, int in0) { return Seg{0, (int)mn_tc_img_off(img, L), L, L, in0}; };
+        // dir_a_encoding: input [F, dir PE + embedding]
+        wgrad(dzg, half, a.lay.dira_w, L + nd.aux, a.lay.dira_b, hseg(nd.layers, 0), Seg{1, xaux, P.kaux, nd.aux, L}, 2);
+        dgrad(dzg, half, D.w_dira, pp[0], -1, false);                                      // dF (xyz_encoding_final has no activation)
+        wgrad(pp[0], L, a.lay.final_w, L, a.lay.final_b, hseg(nd.layers - 1, 0), none, 1);
+        dgrad(pp[0], L, D.w_final, pp[1], nd.layers - 1, true);                            // dZ of the last trunk layer
+        int cur = 1;
+        for (int l = nd.layers - 1; l >= 0; --l) {
+            const Seg pe{1, 0, P.kpe, nd.in_xyz, 0};
+            const int k_in = a.lay.kin[l];
+            if (l == 0) wgrad(pp[cur], L, a.lay.w[l], k_in, a.lay.b[l], pe, none, 1);
+            else if ((nd.skip_mask >> l) & 1) wgrad(pp[cur], L, a.lay.w[l], k_in, a.lay.b[l], pe, hseg(l - 1, nd.in_xyz), 2);
+            else wgrad(pp[cur], L, a.lay.w[l], k_in, a.lay.b[l], hseg(l - 1, 0), none, 1);
+            if (l >= 1) {
+                dgrad(pp[cur], L, D.w_layer[l], pp[cur ^ 1], l - 1, false);               // dZ_{l-1} = mask(dZ_l W_l[:, hidden])
+                cur ^= 1;
+            }
+        }
+        // ---- sigma / rgb heads
+        HeadsArgs H{};
+        H.act = tape.act;
+        H.gf32 = gf32;
+        H.act_tile_bytes = act_tile;
+        H.L = L;
+        H.layers = nd.layers;
+        H.rgb_dim = nd.rgb_dim;
+        H.counters = a.counters;
+        H.n_tiles = tiles_used;
+        H.t_min = t0;
+        H.t_max = t0 + nt;
+        H.fixed_sub = a.fixed_sub;
+        H.chunk_tiles = 16;
+        H.gw = a.gw;
+        H.sub_stride = a.lay.total;
+        H.sigma_w = a.lay.sigma_w; H.sigma_b = a.lay.sigma_b; H.rgb_w = a.lay.rgb_w; H.rgb_b = a.lay.rgb_b;
+        const dim3 hgrid((unsigned)mn_cdiv(nt, (int64_t)16), (unsigned)n_sub, (unsigned)(L / 256));
+        if (nd.rgb_dim == 3) tc_heads_wgrad_kernel<3><<<hgrid, 256, 0, st>>>(H);
+        else tc_heads_wgrad_kernel<MN_TC_RGB_MAX><<<hgrid, 256, 0, st>>>(H);
+        MN_LAUNCH_CHECK(ctx);
+    }
+    if (nd.app_in_dira) {
+        tc_emb_grad_kernel<<<dim3((unsigned)nd.app_count, (unsigned)a.n_sub), 64, 0, st>>>(emb_sum, a.packed_bwd, a.blay.total, a.blay.dira_e, half, nd.app,
+                                                                                          nd.app_count, a.gw, a.lay.total, a.lay.emb);
+        MN_LAUNCH_CHECK(ctx);
+    }
+    mn_prof_end(ctx, st);
+    return MN_OK;
 }
 
 int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_tiles128, const TrainTcTape& tape, void* ws, size_t ws_bytes,
                          cudaStream_t st) {
     TcArgs A{};
     const NetDims& nd = a.nd;
-    if (!m->train_tc_ok || !build_dgrad_plan(nd, &A.plan)) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: unsupported network shape");
+    LayerPlan LP;
+    const bool layer = build_layer_plan(nd, &LP);
+    if (!m->train_tc_ok || (layer ? !m->tc_dgrad : !build_dgrad_plan(nd, &A.plan)))
+        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: unsupported network shape");
     if (n_tiles128 <= 0) return MN_OK;
     if (!ws || ws_bytes < mn_train_tc_backward_workspace(m, n_tiles128)) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_train_tc_backward: workspace too small");
+    if (layer) return layer_backward(ctx, m, a, LP, n_tiles128, tape, ws, st);
     const size_t act_tile = mn_train_tc_act_tile_bytes(m);
     char* wp = (char*)(((uintptr_t)ws + 255) / 256 * 256);
     unsigned char* dz = (unsigned char*)wp;               wp += mn_align((size_t)n_tiles128 * act_tile);
@@ -986,8 +1273,8 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     W.chunk_tiles = (int)chunk_tiles;
     const unsigned gx = (unsigned)mn_cdiv(tiles_used, chunk_tiles);
     const int wg_smem = 2 * kWgStageBytes + 6144 + 256;
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
-    tc_wgrad_kernel<<<dim3(gx, (unsigned)ni, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
+    MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
+    tc_wgrad_kernel<false><<<dim3(gx, (unsigned)ni, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
     MN_LAUNCH_CHECK(ctx);
 
     // ---- sigma / rgb heads and the appearance embedding
@@ -1000,6 +1287,8 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     H.rgb_dim = nd.rgb_dim;
     H.counters = a.counters;
     H.n_tiles = tiles_used;
+    H.t_min = 0;
+    H.t_max = tiles_used;
     H.fixed_sub = a.fixed_sub;
     H.chunk_tiles = 16;
     H.gw = a.gw;

@@ -169,6 +169,91 @@ __host__ __device__ inline WgLayout wg_layout(const TcPlan& p, bool split) {
     return s;
 }
 
+// ---- head stage of the data-gradient chain (nerf.py:132-160 backwards), per row; shared by tc_mlp_wg_kernel<PP_DGRAD> and the
+// layer-GEMM path's tc_layer_head_dgrad_kernel.
+// d[c] = gradient of the rgb Linear's output c: upstream gradient x blend weight, then sigmoid' (colour head, rgb_dim 3) or the
+// raw SH coefficients as they are.  Returns the gradient of the sigma pre-activation (softplus' or ReLU').  tf: the row's entry
+// of the tape's fp32 head block.  Only compile-time indices into d (loops unrolled to MN_TC_RGB_MAX and left at c == R), so
+// the array stays in registers.
+__device__ __forceinline__ float tc_head_grad(const MlpArgs& m, const float* grad_out, int64_t row, int64_t slot, const float* tf,
+                                              float* d) {
+    const int R = m.nd.rgb_dim;
+    float gsig = 0.0f;
+    if (R == 3) {
+        float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f;
+        if (row >= 0) {
+            const float4 gv = *reinterpret_cast<const float4*>(grad_out + row * 4);
+            const float bw = m.slot_w ? m.slot_w[slot] : 1.0f;
+            g0 = gv.x * bw; g1 = gv.y * bw; g2 = gv.z * bw; gsig = gv.w * bw;
+        }
+        const float c0v = tf[MN_TC_F32_RGB * kTileM], c1v = tf[(MN_TC_F32_RGB + 1) * kTileM], c2v = tf[(MN_TC_F32_RGB + 2) * kTileM];
+        d[0] = (g0 * (1.0f - c0v)) * c0v; d[1] = (g1 * (1.0f - c1v)) * c1v; d[2] = (g2 * (1.0f - c2v)) * c2v;
+    } else {
+#pragma unroll
+        for (int c = 0; c < MN_TC_RGB_MAX; ++c) d[c] = 0.0f;
+        if (row >= 0) {
+            const float* go = grad_out + row * m.out_cols;          // [rgb_dim SH coefficients][sigma]
+            const float bw = m.slot_w ? m.slot_w[slot] : 1.0f;
+#pragma unroll
+            for (int c = 0; c < MN_TC_RGB_MAX; ++c) {
+                if (c >= R) break;
+                d[c] = go[c] * bw;
+            }
+            gsig = go[R] * bw;
+        }
+    }
+    const float pre = tf[MN_TC_F32_SIGMA * kTileM];
+    float dsp;
+    if (m.nd.softplus) { const float y = pre - 1.0f; dsp = y > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-y)); }
+    else dsp = pre > 0.0f ? 1.0f : 0.0f;
+    return gsig * dsp;
+}
+
+// v[e] = mask(G > 0) (sum_c W_rgb[c][k0 + e] d[c]) for the 8 columns k0 .. k0 + 7 of one row; Wr = [rgb_dim][half] fp32, g = the
+// row's 8 fp16 values of G in the tile image.  Order c = 0, 1, .. (a product, then one fma per further row).
+__device__ __forceinline__ void tc_rgb_dgrad8(const float* Wr, int half, int k0, const float* d, int R, const unsigned char* g, float* v) {
+    const uint4 gm = *reinterpret_cast<const uint4*>(g);
+    const __half2* gh = reinterpret_cast<const __half2*>(&gm);
+    {
+        const float4 wa = *reinterpret_cast<const float4*>(Wr + k0), wb = *reinterpret_cast<const float4*>(Wr + k0 + 4);
+        v[0] = wa.x * d[0]; v[1] = wa.y * d[0]; v[2] = wa.z * d[0]; v[3] = wa.w * d[0];
+        v[4] = wb.x * d[0]; v[5] = wb.y * d[0]; v[6] = wb.z * d[0]; v[7] = wb.w * d[0];
+    }
+#pragma unroll
+    for (int c = 1; c < MN_TC_RGB_MAX; ++c) {
+        if (c >= R) break;
+        const float4 wa = *reinterpret_cast<const float4*>(Wr + c * half + k0);
+        const float4 wb = *reinterpret_cast<const float4*>(Wr + c * half + k0 + 4);
+        v[0] = fmaf(wa.x, d[c], v[0]); v[1] = fmaf(wa.y, d[c], v[1]); v[2] = fmaf(wa.z, d[c], v[2]); v[3] = fmaf(wa.w, d[c], v[3]);
+        v[4] = fmaf(wb.x, d[c], v[4]); v[5] = fmaf(wb.y, d[c], v[5]); v[6] = fmaf(wb.z, d[c], v[6]); v[7] = fmaf(wb.w, d[c], v[7]);
+    }
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+        const float gv = (e & 1) ? __high2float(gh[e >> 1]) : __low2float(gh[e >> 1]);
+        v[e] = gv > 0.0f ? v[e] : 0.0f;
+    }
+}
+
+// Appearance-embedding gradient, step 1: per-image sums of dZ_dira rows (fp32, unscaled).  Called by a whole warp; the lanes
+// are consecutive slots, i.e. mostly samples of one ray = one image id.  sums = column k0 of image 0 of the sub-module's
+// [app_count][half] block.
+__device__ __forceinline__ void tc_emb_sums8(float* sums, int half, bool valid, int id, int lane, const float* v) {
+    unsigned todo = __ballot_sync(0xffffffffu, valid);
+    while (todo) {
+        const int leader = __ffs(todo) - 1;
+        const int cur = __shfl_sync(0xffffffffu, id, leader);
+        const bool mine = valid && id == cur;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) {
+            float s = mine ? v[e] : 0.0f;
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            if (lane == leader) atomicAdd(sums + (size_t)cur * half + e, s);
+        }
+        todo &= ~__ballot_sync(0xffffffffu, mine);
+    }
+}
+
 template <int kMode, bool kSplit, bool kWide>
 __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArgs A) {
     extern __shared__ __align__(1024) unsigned char smem[];
@@ -274,37 +359,8 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                 const int R = A.m.nd.rgb_dim;
                 const float* Wr = F32 + L;                                  // [rgb_dim][L/2] rgb weights (fp32 block of the data-gradient plan)
                 const float* tf = A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + hr;
-                // d[c]: gradient of the rgb Linear's output c of this row.  Only compile-time indices (loops unrolled to
-                // MN_TC_RGB_MAX and left at c == R), so the array stays in registers.
-                float d[MN_TC_RGB_MAX], gsig = 0.0f;
-                if (R == 3) {
-                    float g0 = 0.0f, g1 = 0.0f, g2 = 0.0f;
-                    if (hrow >= 0) {
-                        const float4 gv = *reinterpret_cast<const float4*>(A.grad_out + hrow * 4);
-                        const float bw = A.m.slot_w ? A.m.slot_w[hslot] : 1.0f;
-                        g0 = gv.x * bw; g1 = gv.y * bw; g2 = gv.z * bw; gsig = gv.w * bw;
-                    }
-                    const float c0v = tf[MN_TC_F32_RGB * kTileM], c1v = tf[(MN_TC_F32_RGB + 1) * kTileM], c2v = tf[(MN_TC_F32_RGB + 2) * kTileM];
-                    d[0] = (g0 * (1.0f - c0v)) * c0v; d[1] = (g1 * (1.0f - c1v)) * c1v; d[2] = (g2 * (1.0f - c2v)) * c2v;
-                } else {
-#pragma unroll
-                    for (int c = 0; c < MN_TC_RGB_MAX; ++c) d[c] = 0.0f;
-                    if (hrow >= 0) {
-                        const float* go = A.grad_out + hrow * A.m.out_cols;  // [rgb_dim SH coefficients][sigma]
-                        const float bw = A.m.slot_w ? A.m.slot_w[hslot] : 1.0f;
-#pragma unroll
-                        for (int c = 0; c < MN_TC_RGB_MAX; ++c) {
-                            if (c >= R) break;
-                            d[c] = go[c] * bw;
-                        }
-                        gsig = go[R] * bw;
-                    }
-                }
-                const float pre = tf[MN_TC_F32_SIGMA * kTileM];
-                float dsp;
-                if (A.m.nd.softplus) { const float y = pre - 1.0f; dsp = y > 20.0f ? 1.0f : 1.0f / (1.0f + expf(-y)); }
-                else dsp = pre > 0.0f ? 1.0f : 0.0f;
-                const float ds = gsig * dsp;
+                float d[MN_TC_RGB_MAX];
+                const float ds = tc_head_grad(A.m, A.grad_out, hrow, hslot, tf, d);
                 if (part == 0) {
                     DSIG[hr] = ds * S;
                     float* tg = A.tape_gf32 + (size_t)tile * mn_tc_g32_rows(R) * kTileM + hr;
@@ -321,46 +377,9 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                 const int half = L / 2, per = half / 2;
                 for (int kk = 0; kk < per; kk += 8) {
                     const int k0 = part * per + kk;
-                    const uint4 gm = *reinterpret_cast<const uint4*>(gimg + (size_t)(k0 >> 3) * (kTileM * 16) + (size_t)hr * 16);
-                    const __half2* gh = reinterpret_cast<const __half2*>(&gm);
-                    // v[e] = sum_c W_rgb[c][k0 + e] d[c], in the order c = 0, 1, .. (a product, then one fma per further row)
                     float v[8];
-                    {
-                        const float4 wa = *reinterpret_cast<const float4*>(Wr + k0), wb = *reinterpret_cast<const float4*>(Wr + k0 + 4);
-                        v[0] = wa.x * d[0]; v[1] = wa.y * d[0]; v[2] = wa.z * d[0]; v[3] = wa.w * d[0];
-                        v[4] = wb.x * d[0]; v[5] = wb.y * d[0]; v[6] = wb.z * d[0]; v[7] = wb.w * d[0];
-                    }
-#pragma unroll
-                    for (int c = 1; c < MN_TC_RGB_MAX; ++c) {
-                        if (c >= R) break;
-                        const float4 wa = *reinterpret_cast<const float4*>(Wr + c * half + k0);
-                        const float4 wb = *reinterpret_cast<const float4*>(Wr + c * half + k0 + 4);
-                        v[0] = fmaf(wa.x, d[c], v[0]); v[1] = fmaf(wa.y, d[c], v[1]); v[2] = fmaf(wa.z, d[c], v[2]); v[3] = fmaf(wa.w, d[c], v[3]);
-                        v[4] = fmaf(wb.x, d[c], v[4]); v[5] = fmaf(wb.y, d[c], v[5]); v[6] = fmaf(wb.z, d[c], v[6]); v[7] = fmaf(wb.w, d[c], v[7]);
-                    }
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const float gv = (e & 1) ? __high2float(gh[e >> 1]) : __low2float(gh[e >> 1]);
-                        v[e] = gv > 0.0f ? v[e] : 0.0f;
-                    }
-                    // appearance-embedding gradient, step 1: per-image sums of dZ_dira rows (fp32, unscaled); the lanes of a warp
-                    // are consecutive slots, i.e. mostly samples of one ray = one image id
-                    if (A.emb_sum) {
-                        unsigned todo = __ballot_sync(0xffffffffu, hrow >= 0);
-                        while (todo) {
-                            const int leader = __ffs(todo) - 1;
-                            const int cur = __shfl_sync(0xffffffffu, id, leader);
-                            const bool mine = hrow >= 0 && id == cur;
-#pragma unroll
-                            for (int e = 0; e < 8; ++e) {
-                                float s = mine ? v[e] : 0.0f;
-#pragma unroll
-                                for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-                                if (lane == leader) atomicAdd(A.emb_sum + ((size_t)sub * A.m.nd.app_count + cur) * half + k0 + e, s);
-                            }
-                            todo &= ~__ballot_sync(0xffffffffu, mine);
-                        }
-                    }
+                    tc_rgb_dgrad8(Wr, half, k0, d, R, gimg + (size_t)(k0 >> 3) * (kTileM * 16) + (size_t)hr * 16, v);
+                    if (A.emb_sum) tc_emb_sums8(A.emb_sum + (size_t)sub * A.m.nd.app_count * half + k0, half, hrow >= 0, id, lane, v);
                     uint32_t pk[4];
 #pragma unroll
                     for (int e = 0; e < 4; ++e) pk[e] = pack_h2(v[2 * e] * S, v[2 * e + 1] * S);

@@ -87,12 +87,16 @@ struct WgItem {
 };
 constexpr int kWgMaxItems = 48;
 struct WgArgs {
-    WgItem item[kWgMaxItems];
+    WgItem item[kWgMaxItems];       // kLinear: item[s] = input segment s of one Linear for its first output half and X chunk
     int n_items;
     const unsigned char* act;       // activation records
-    const unsigned char* dz;        // gradient records (same layout)
+    const unsigned char* dz;        // gradient records (same layout); kLinear: gradient images of tile t_min onwards
     const unsigned char* xreg;      // encoder tiles
     int64_t act_tile_bytes, x_tile_bytes;
+    // kLinear (layer-GEMM path, one tile group and one Linear per launch): item y = (output half, X chunk of <= 256 columns)
+    int n_chunks[2];                // X chunks of each input segment
+    int64_t dz_tile_bytes;          // tile stride of the gradient images
+    int64_t t_min, t_max;           // tiles of the group
     const int* counters;            // routing counters saved by the forward pass, or NULL
     int64_t n_tiles;                // counters == NULL: all tiles belong to fixed_sub
     int fixed_sub;
@@ -104,6 +108,24 @@ struct WgArgs {
 constexpr int kWgStageBytes = 96 * 1024;
 constexpr int kWgThreads = 384;     // warpgroup 0: producer thread; warpgroups 1-2: output channels 0-63 / 64-127 of the item
 
+// Work item y of a kLinear launch: output channels [128 mh, +128) x input columns [256 c, +256) of segment s.
+__device__ __forceinline__ WgItem wg_linear_item(const WgArgs& A, int y) {
+    const int per = A.n_chunks[0] + A.n_chunks[1];
+    const int mh = y / per;
+    int c = y - mh * per;
+    const int s = c < A.n_chunks[0] ? 0 : 1;
+    if (s) c -= A.n_chunks[0];
+    WgItem it = A.item[s];
+    it.dz_off += mh * 16 * (kTileM * 16);
+    it.x_off += c * 32 * (kTileM * 16);
+    it.n = min(256, it.n - 256 * c);
+    it.n_real = min(256, it.n_real - 256 * c);
+    it.w_off += mh * 128 * it.k_in + 256 * c;
+    it.b_off = (it.b_off >= 0 && c == 0) ? it.b_off + mh * 128 : -1;
+    return it;
+}
+
+template <bool kLinear>
 __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A) {
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char* ring = smem;                                   // 2 x 96 KiB: [dZ half 32 KiB][X <= 64 KiB]
@@ -111,13 +133,17 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
     uint64_t* bars = reinterpret_cast<uint64_t*>(ones + 6144);
     uint64_t* full = bars;        // [2]
     uint64_t* empty = bars + 2;   // [2], one arrival per consumer warpgroup
-    const WgItem it = A.item[blockIdx.y];
+    const WgItem it = kLinear ? wg_linear_item(A, blockIdx.y) : A.item[blockIdx.y];
     int sub = A.fixed_sub;
     int64_t t_lo = 0, t_hi = A.n_tiles;
     if (A.counters) {
         sub = (int)blockIdx.z;
         t_lo = A.counters[CNT_START + sub] / kTileM;
         t_hi = A.counters[CNT_START + sub + 1] / kTileM;
+    }
+    if (kLinear) {
+        t_lo = max(t_lo, A.t_min);
+        t_hi = min(t_hi, A.t_max);
     }
     const int64_t t_begin = t_lo + (int64_t)blockIdx.x * A.chunk_tiles;
     const int64_t t_end = min(t_hi, t_begin + (int64_t)A.chunk_tiles);
@@ -141,7 +167,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
             for (int64_t t = t_begin; t < t_end; ++t) {
                 mbar_wait(&empty[st], ph ^ 1);
                 mbar_expect_tx(&full[st], 32768u + xbytes);
-                bulk_g2s(ring + (size_t)st * kWgStageBytes, A.dz + (size_t)t * A.act_tile_bytes + it.dz_off, 32768u, &full[st]);
+                const unsigned char* dzt = kLinear ? A.dz + (size_t)(t - A.t_min) * A.dz_tile_bytes : A.dz + (size_t)t * A.act_tile_bytes;
+                bulk_g2s(ring + (size_t)st * kWgStageBytes, dzt + it.dz_off, 32768u, &full[st]);
                 bulk_g2s(ring + (size_t)st * kWgStageBytes + 32768, xbase + (size_t)t * xstride + it.x_off, xbytes, &full[st]);
                 if (++st == 2) { st = 0; ph ^= 1; }
             }
@@ -216,36 +243,38 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
 // sigma Linear (1 x L) and rgb Linear (rgb_dim x L/2) weight / bias gradients from the fp32 head gradients and the fp16 tapes.
 struct HeadsArgs {
     const unsigned char* act;
-    const float* gf32;              // head-gradient blocks [n_tiles][mn_tc_g32_rows(rgb_dim)][128]
+    const float* gf32;              // head-gradient blocks [n_tiles][mn_tc_g32_rows(rgb_dim)][128], of tile t_min onwards
     int64_t act_tile_bytes;
     int L, layers, rgb_dim;
     const int* counters;
     int64_t n_tiles;
+    int64_t t_min, t_max;           // tiles covered by gf32 (the layer-GEMM path's tile group; 0 .. n_tiles otherwise)
     int fixed_sub, chunk_tiles;
     float* gw;
     int64_t sub_stride;
     int sigma_w, sigma_b, rgb_w, rgb_b;     // float offsets in a sub-module's gradient block (rgb_w is [rgb_dim][L/2])
 };
 // kRgb: 3 for the colour head (exactly 3 rgb rows), MN_TC_RGB_MAX for a raw SH head (rgb_dim <= kRgb rows).  The rgb weight
-// gradient is split over the block: thread k accumulates input channel k % (L/2) for the output rows [kPer * (k / (L/2)),
-// +kPer) (256 threads, L/2 = 128: two groups of kPer rows).
+// gradient is split over the channel index k: k accumulates input channel k % (L/2) for the output rows [kPer * (k / (L/2)),
+// +kPer) (two groups of kPer rows over k < L).  Block z of the grid takes the 256 channels k = 256 z + threadIdx.x, so wider
+// networks run L / 256 channel blocks.
 template <int kRgb>
 __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) {
     constexpr int kPer = kRgb < 16 ? kRgb : 16;       // rgb accumulators per thread
     static_assert(2 * kPer >= kRgb, "rgb rows of tc_heads_wgrad_kernel");
     __shared__ float G[1 + kRgb][kTileM];              // this tile's head-gradient block
     int sub = A.fixed_sub;
-    int64_t t_lo = 0, t_hi = A.n_tiles;
+    int64_t t_lo = A.t_min, t_hi = min(A.n_tiles, A.t_max);
     if (A.counters) {
         sub = (int)blockIdx.y;
-        t_lo = A.counters[CNT_START + sub] / kTileM;
-        t_hi = A.counters[CNT_START + sub + 1] / kTileM;
+        t_lo = max(t_lo, (int64_t)(A.counters[CNT_START + sub] / kTileM));
+        t_hi = min(A.t_max, (int64_t)(A.counters[CNT_START + sub + 1] / kTileM));
     }
     const int64_t t_begin = t_lo + (int64_t)blockIdx.x * A.chunk_tiles;
     const int64_t t_end = min(t_hi, t_begin + (int64_t)A.chunk_tiles);
     if (t_begin >= t_end) return;
     const int rgb_dim = kRgb == 3 ? 3 : A.rgb_dim;
-    const int k = threadIdx.x, L = A.L, half = L / 2, rows = mn_tc_g32_rows(rgb_dim);
+    const int k = threadIdx.x + 256 * (int)blockIdx.z, L = A.L, half = L / 2, rows = mn_tc_g32_rows(rgb_dim);
     const int kc = k % half, c0 = kPer * (k / half);       // rgb part: input channel, first output row
     const int nc = min(kPer, rgb_dim - c0);                // output rows of this thread (<= 0: none)
     float ws = 0.0f, bs = 0.0f, wr[kPer];
@@ -253,7 +282,7 @@ __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) 
     for (int c = 0; c < kPer; ++c) wr[c] = 0.0f;
     for (int64_t t = t_begin; t < t_end; ++t) {
         __syncthreads();
-        for (int i = threadIdx.x; i < rows * kTileM; i += 256) G[i / kTileM][i % kTileM] = A.gf32[(size_t)t * rows * kTileM + i];
+        for (int i = threadIdx.x; i < rows * kTileM; i += 256) G[i / kTileM][i % kTileM] = A.gf32[(size_t)(t - A.t_min) * rows * kTileM + i];
         __syncthreads();
         const unsigned char* rec = A.act + (size_t)t * A.act_tile_bytes;
         if (k < L) {
