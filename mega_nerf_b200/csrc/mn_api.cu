@@ -27,21 +27,10 @@ __global__ void __launch_bounds__(256) pack_ops_kernel(const PackOp* __restrict_
                 reinterpret_cast<float*>(op.dst)[i] = src[(long long)n * K + koff + k];
                 break;
             }
-            case PK_TC_IMAGE: {       // K-major Wt[k][n_src] fp32 -> image [K/8][N][8] fp16 (hi) and the fp16 residual (lo)
-                const int n_src = op.p[0], k_src = op.p[1], N = op.p[2], k_real0 = op.p[4], k_pad0 = op.p[5];
-                const int k8 = (int)(i % 8), n = (int)((i / 8) % N), kc = (int)(i / (8 * (long long)N));
-                const int k = kc * 8 + k8;
-                int ks;
-                if (k < k_pad0) ks = k < k_real0 ? k : -1;
-                else ks = k_real0 + (k - k_pad0);
-                float v = 0.0f;
-                if (ks >= 0 && ks < k_src && n < n_src) v = src[(long long)ks * n_src + n];
-                const __half h = __float2half_rn(v);
-                reinterpret_cast<__half*>(op.dst)[i] = h;
-                if (op.dst2) reinterpret_cast<__half*>(op.dst2)[i] = __float2half_rn(v - __half2float(h));
-                break;
-            }
-            case PK_TC_HALF: {        // half-major image [N-half][K/8][nw][8] fp16 (512-wide kernel, layer-GEMM path); optional fp16 residual (lo)
+            // K-major Wt[k][n_src] fp32 -> the tensor-core image [N/nw][K/8][nw][8] fp16, optional fp16 residual (lo).  Source
+            // column ks of image column k: the first k_pad0 image columns hold k_real0 source columns and zero padding, the rest
+            // follow contiguously; columns and rows past the source are zero.
+            case PK_TC_HALF: {
                 const int n_src = op.p[0], k_src = op.p[1], K = op.p[3], k_real0 = op.p[4], k_pad0 = op.p[5], nw = op.p[6];
                 const int k8 = (int)(i % 8), n = (int)((i / 8) % nw);
                 const long long rest = i / (8 * (long long)nw);
@@ -60,12 +49,6 @@ __global__ void __launch_bounds__(256) pack_ops_kernel(const PackOp* __restrict_
             case PK_TC_F32:           // copy with zero padding
                 reinterpret_cast<float*>(op.dst)[i] = i < op.p[0] ? src[i] : 0.0f;
                 break;
-            case PK_DGRAD: {          // image (n, k) = Wd[k * ld + n]: transposed fp16 image of the data-gradient chain
-                const int ld = op.p[0], N = op.p[1];
-                const int k8 = (int)(i % 8), n = (int)((i / 8) % N), kc = (int)(i / (8 * (long long)N));
-                reinterpret_cast<__half*>(op.dst)[i] = __float2half_rn(src[(long long)(kc * 8 + k8) * ld + n]);
-                break;
-            }
             case PK_RGBW: {           // K-major Wt[k][c] -> [c][k]
                 const int K = op.p[0], Cc = op.p[1];
                 reinterpret_cast<float*>(op.dst)[(i % Cc) * K + i / Cc] = src[i];
@@ -198,7 +181,7 @@ int mn_debug_tp_program(const mn_model_desc* desc, unsigned int* table_out, int 
     mn_model m;
     m.d = *desc;
     build_layout(&m);
-    return mn_mlp_tp_program(m.nd, table_out, cap_entries, info8);
+    return mn_mlp_tp_program(m, table_out, cap_entries, info8);
 }
 
 int mn_create(mn_ctx** out, int device) {
@@ -676,10 +659,7 @@ int mn_model_forward_train_tc(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
                               const float* sigma_noise_d, float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d,
                               size_t workspace_bytes, void* stream) {
     if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_train_tc: tape is NULL");
-    if (!m || !m->train_tc_ok)
-        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 or 768..2048 (a multiple of 256) with a direction "
-                                                "/ appearance head, rgb_dim 3 or a raw SH head (rgb_dim <= 32), no affine appearance; use "
-                                                "the fp32 training entry points for this model");
+    if (!m || !m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
     return model_forward_impl(ctx, m, rows, B, use_coarse, 0, sigma_noise_d, MN_PREC_FP32, out_d, workspace_d, workspace_bytes, tape_d,
                               tape_bytes, stream, 1);
 }

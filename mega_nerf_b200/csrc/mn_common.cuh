@@ -21,7 +21,7 @@
 // One element-wise re-layout of a weight tensor (fp32 transposes / sub-matrices / copies, fp16 tensor-core images).  The ~75 of
 // them a sub-module needs are queued by mn_model_set_weights and run as TWO launches (fp32 layouts first, the fp16 images that read
 // them second) instead of one tiny launch each: a training step re-packs every sub-module after the optimiser step.
-enum { PK_COPY = 0, PK_TRANSPOSE, PK_SUBMATRIX, PK_TC_IMAGE, PK_TC_HALF, PK_TC_F32, PK_DGRAD, PK_RGBW };
+enum { PK_COPY = 0, PK_TRANSPOSE, PK_SUBMATRIX, PK_TC_HALF, PK_TC_F32, PK_RGBW };
 struct PackOp {
     const float* src;
     void* dst;

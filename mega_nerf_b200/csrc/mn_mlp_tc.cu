@@ -2,7 +2,7 @@
 //
 //   tc_encode_kernel   sample rows -> fp16 feature tiles (positional encodings of xyz / dir, appearance
 //                      embedding) written in the exact shared-memory operand image, one 128-row tile
-//                      per CTA, coalesced 16-byte stores.
+//                      per CTA, coalesced 16-byte stores (tc_encode_fast_kernel: the common shape).
 //   tc_mlp_wg_kernel   persistent, warp-specialised (mn_mlp_wg.cuh): one producer thread (cp.async.bulk of
 //                      weight K-slabs through an mbarrier ring and of the feature tiles), two consumer
 //                      warpgroups issuing wgmma.mma_async (accumulators in registers) and running the
@@ -14,6 +14,12 @@
 // i.e. [K/8][R][8] fp16.  wgmma descriptor: LBO = R*16 (next 8-column chunk), SBO = 128 (next 8-row group).
 // The epilogue's per-row 16-byte stores and the packer's images are contiguous in this layout, any K that
 // is a multiple of 16 works, and no TMA tensor map is needed (plain 1-D bulk copies).
+//
+// Networks wider than 512 run on the layer-GEMM engine instead (mn_layer_gemm.cuh).  Host side: tc_linears lists the
+// network's Linears once; tc_net picks the engine (build_layer_plan or build_plan) and the training coverage
+// (build_dgrad_plan) from that table, and every entry point below calls it once.  mn_mlp_tc_pack writes the forward images of
+// either engine, tc_dgrad_ready / tc_pack_dgrad the transposed images of the backward, and mn_train_tc_backward runs
+// the backward of either engine between one shared workspace carve, gradient scale and head / embedding epilogue.
 #include <cuda_fp16.h>
 
 #include <type_traits>
@@ -60,51 +66,95 @@ struct TcPlan {
 
 int pad16(int x) { return (x + 15) / 16 * 16; }
 
-bool build_plan(const NetDims& nd, TcPlan* p) {
+// ---- the network's Linears in forward order (nerf.py:115-160): trunk layers 0 .. layers-1, xyz_encoding_final,
+// dir_a_encoding, rgb.  The plans of both engines, the weight packs and the weight-gradient items of the backward all walk
+// this one table.  Linear j's SRC_H segment reads the output of Linear j - 1 (image j - 1 of a tile's activation record).
+struct TcSeg {
+    int src;             // SRC_XPE / SRC_XAUX (a segment of the feature tile) or SRC_H (the previous Linear's output)
+    int k, k_real;       // padded K columns (multiple of 16); columns that exist in the nn.Linear weight
+    int in0;             // first input column of the segment in the nn.Linear weight
+};
+struct TcLinear {
+    int n;               // output features
+    int nseg;
+    TcSeg seg[2];
+    int kin;             // in_features
+    int w, b;            // PackedLayout float offsets of the weight and the bias (also their offsets in the gradient block)
+    int bwd;             // BwdLayout float offset of the [n][L] sub-matrix the data-gradient chain streams; -1: none
+    int epi;             // EPI_RELU, EPI_RELU_SIGMA (last trunk layer), EPI_LINEAR (xyz_encoding_final) or EPI_RGB
+};
+struct TcLinears {
+    int n, n_trunk;
+    int kpe, kaux;       // padded feature-tile widths
+    TcLinear l[MN_MAX_LAYERS + 3];
+};
+
+TcLinears tc_linears(const mn_model& m) {
+    const NetDims& nd = m.nd;
+    TcLinears T{};
+    T.kpe = pad16(nd.in_xyz);
+    T.kaux = nd.aux > 0 ? pad16(nd.aux) : 0;
+    const TcSeg pe{SRC_XPE, T.kpe, nd.in_xyz, 0};
+    auto h = [](int k, int in0) { return TcSeg{SRC_H, k, k, in0}; };
+    auto add = [&](int n, TcSeg s0, int kin, int w, int b, int bwd, int epi) -> TcLinear& {
+        TcLinear& l = T.l[T.n++];
+        l = TcLinear{n, 1, {s0, {}}, kin, w, b, bwd, epi};
+        return l;
+    };
+    for (int i = 0; i < nd.layers; ++i) {
+        TcLinear& l = add(nd.L, i == 0 ? pe : h(nd.L, 0), m.lay.kin[i], m.lay.w[i], m.lay.b[i], i > 0 ? m.blay.w[i] : -1,
+                          i == nd.layers - 1 ? EPI_RELU_SIGMA : EPI_RELU);
+        if (i > 0 && ((nd.skip_mask >> i) & 1)) {      // cat[PE, h]: PE columns first
+            l.nseg = 2;
+            l.seg[0] = pe;
+            l.seg[1] = h(nd.L, nd.in_xyz);
+        }
+    }
+    T.n_trunk = T.n;
+    if (nd.has_dir_a) {                                // has_dir_a implies aux > 0: dir_a_encoding reads [F, dir PE + embedding]
+        add(nd.L, h(nd.L, 0), nd.L, m.lay.final_w, m.lay.final_b, m.blay.final_w, EPI_LINEAR);
+        TcLinear& d = add(nd.L / 2, h(nd.L, 0), nd.L + nd.aux, m.lay.dira_w, m.lay.dira_b, m.blay.dira_f, EPI_RELU);
+        d.nseg = 2;
+        d.seg[1] = TcSeg{SRC_XAUX, T.kaux, nd.aux, nd.L};
+    }
+    add(nd.rgb_dim, h(nd.rgb_in, 0), nd.rgb_in, m.lay.rgb_w, m.lay.rgb_b, -1, EPI_RGB);
+    return T;
+}
+
+// ---- fused plan: every Linear (the rgb head as an N = 32 GEMM) in one tc_mlp_wg_kernel launch
+bool build_plan(const NetDims& nd, const TcLinears& T, TcPlan* p) {
     if (nd.L % 64 != 0 || (nd.L > 256 && nd.L != 512) || nd.L < 64 || nd.rgb_dim > 32 || nd.layers > 12) return false;
     if (nd.affine && nd.rgb_dim != 3) return false;
     TcPlan& P = *p;
     P = TcPlan{};
     P.L = nd.L;
     P.bstride = nd.L > 256 ? 512 : 256;
-    P.kpe = pad16(nd.in_xyz);
-    P.kaux = nd.aux > 0 ? pad16(nd.aux) : 0;
-    int woff = 0, ng = 0;
-    auto add = [&](int n, int s0, int k0, int s1, int k1, int epi) {
-        TcGemm& g = P.g[ng];
-        g.n = n;
-        g.nseg = k1 > 0 ? 2 : 1;
-        g.src[0] = s0; g.k[0] = k0; g.src[1] = s1; g.k[1] = k1;
+    P.kpe = T.kpe;
+    P.kaux = T.kaux;
+    int woff = 0;
+    for (int gi = 0; gi < T.n; ++gi) {
+        const TcLinear& l = T.l[gi];
+        TcGemm& g = P.g[gi];
+        g.n = l.epi == EPI_RGB ? 32 : l.n;
+        g.nseg = l.nseg;
+        for (int s = 0; s < l.nseg; ++s) { g.src[s] = l.seg[s].src; g.k[s] = l.seg[s].k; }
         g.w_off = woff;
-        g.bias_off = ng * P.bstride;
-        g.epi = epi;
-        woff += (k0 + k1) * n * 2;
-        ++ng;
-    };
-    for (int i = 0; i < nd.layers; ++i) {
-        const int epi = (i == nd.layers - 1) ? EPI_RELU_SIGMA : EPI_RELU;
-        if (i == 0) add(nd.L, SRC_XPE, P.kpe, 0, 0, epi);
-        else if ((nd.skip_mask >> i) & 1) add(nd.L, SRC_XPE, P.kpe, SRC_H, nd.L, epi);
-        else add(nd.L, SRC_H, nd.L, 0, 0, epi);
+        g.bias_off = gi * P.bstride;
+        g.epi = l.epi;
+        woff += (g.k[0] + g.k[1]) * g.n * 2;
     }
-    P.n_trunk = ng;
-    if (nd.has_dir_a) {
-        add(nd.L, SRC_H, nd.L, 0, 0, EPI_LINEAR);
-        add(nd.L / 2, SRC_H, nd.L, SRC_XAUX, P.kaux, EPI_RELU);
-        add(32, SRC_H, nd.L / 2, 0, 0, EPI_RGB);
-    } else {
-        add(32, SRC_H, nd.L, 0, 0, EPI_RGB);
-    }
-    P.n_gemm = ng;
+    P.n_trunk = T.n_trunk;
+    P.n_gemm = T.n;
     P.plane_bytes = woff;
-    P.sigma_w_off = ng * P.bstride;
-    P.f32_floats = ng * P.bstride + nd.L + 4;
+    P.sigma_w_off = T.n * P.bstride;
+    P.f32_floats = T.n * P.bstride + nd.L + 4;
     P.f32_off = woff * 2;
     P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
     return true;
 }
 
-// ---- layer plan: networks wider than build_plan covers, one GEMM launch per Linear (mn_layer_gemm.cuh)
+// ---- layer plan: networks wider than build_plan covers, one GEMM launch per Linear (mn_layer_gemm.cuh); the rgb head runs
+// in tc_layer_head_kernel from the fp32 block
 enum { LB_ACT0 = 0, LB_ACT1 = 1, LB_G = 2 };     // activation buffers of a tile group: ping, pong, dir_a_encoding output
 
 struct LgGemm {
@@ -131,43 +181,37 @@ struct LayerPlan {
     int buf_cols[3];     // columns of each activation buffer (0: unused)
 };
 
-bool build_layer_plan(const NetDims& nd, LayerPlan* p) {
+bool build_layer_plan(const NetDims& nd, const TcLinears& T, LayerPlan* p) {
     if (nd.L <= 512 || nd.L > 2048 || nd.L % 256 != 0 || nd.rgb_dim > MN_TC_RGB_MAX || nd.layers + 2 > kMaxGemm) return false;
     if (nd.affine && nd.rgb_dim != 3) return false;
     LayerPlan& P = *p;
     P = LayerPlan{};
     P.L = nd.L;
-    P.kpe = pad16(nd.in_xyz);
-    P.kaux = nd.aux > 0 ? pad16(nd.aux) : 0;
-    int woff = 0, foff = 0, ng = 0;
-    auto add = [&](int n, int s0, int k0, int s1, int k1, int relu, int in, int out) {
-        LgGemm& g = P.g[ng++];
-        g.n = n;
-        g.n_blk = (n + 255) / 256;
-        g.nseg = k1 > 0 ? 2 : 1;
-        g.src[0] = s0; g.k[0] = k0; g.src[1] = s1; g.k[1] = k1;
+    P.kpe = T.kpe;
+    P.kaux = T.kaux;
+    const int ng = T.n - 1;
+    int woff = 0, foff = 0;
+    for (int gi = 0; gi < ng; ++gi) {
+        const TcLinear& l = T.l[gi];
+        LgGemm& g = P.g[gi];
+        g.n = l.n;
+        g.n_blk = (l.n + 255) / 256;
+        g.nseg = l.nseg;
+        for (int s = 0; s < l.nseg; ++s) { g.src[s] = l.seg[s].src; g.k[s] = l.seg[s].k; }
         g.w_off = woff;
         g.bias_off = foff;
-        g.relu = relu;
-        g.in = in;
-        g.out = out;
-        woff += (k0 + k1) * g.n_blk * 256 * 2;
+        g.relu = l.epi != EPI_LINEAR;
+        // Linear gi writes buffer gi % 2 and reads the other one.  dir_a_encoding writes G to its own buffer: F went to the other
+        // ping-pong buffer, so the head still finds H_last for sigma.
+        g.in = (gi + 1) & 1;
+        g.out = nd.has_dir_a && gi == ng - 1 ? LB_G : gi & 1;
+        woff += (g.k[0] + g.k[1]) * g.n_blk * 256 * 2;
         foff += g.n_blk * 256;
-    };
-    for (int i = 0; i < nd.layers; ++i) {
-        const int in = (i + 1) & 1, out = i & 1;       // H_i -> buffer i % 2
-        if (i == 0) add(nd.L, SRC_XPE, P.kpe, 0, 0, 1, in, out);
-        else if ((nd.skip_mask >> i) & 1) add(nd.L, SRC_XPE, P.kpe, SRC_H, nd.L, 1, in, out);
-        else add(nd.L, SRC_H, nd.L, 0, 0, 1, in, out);
     }
-    P.n_trunk = ng;
+    P.n_trunk = T.n_trunk;
     P.h_last = (nd.layers - 1) & 1;
     P.buf_cols[0] = P.buf_cols[1] = nd.L;
     if (nd.has_dir_a) {
-        // F goes to the other ping-pong buffer and G to its own, so the head still finds H_last for sigma
-        const int fb = P.h_last ^ 1;
-        add(nd.L, SRC_H, nd.L, 0, 0, 0, P.h_last, fb);
-        add(nd.L / 2, SRC_H, nd.L, SRC_XAUX, P.kaux, 1, fb, LB_G);
         P.buf_cols[LB_G] = P.g[ng - 1].n_blk * 256;
         P.rgb_src = LB_G;
     } else {
@@ -182,6 +226,60 @@ bool build_layer_plan(const NetDims& nd, LayerPlan* p) {
     P.f32_floats = P.rgb_b_off + MN_TC_RGB_MAX;
     P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
     return true;
+}
+
+// ---- data-gradient chain of the backward (training, needs dir_a_encoding): dX of every Linear from dir_a_encoding down to trunk
+// layer 1, restricted to its L hidden input columns, each a GEMM on the Linear's transposed weight image [L/256][out/8][256][8]
+// fp16 (at L = 256 the [K/8][N][8] image of the fused kernel).  The images follow each other in that order, then the fp32
+// block [sigma_w (L)][rgb_w [rgb_dim][L/2]].  The fused engine runs the plan in tc_mlp_wg_kernel<PP_DGRAD>; the layer
+// engine reads the images' offsets from it (one tc_layer_gemm_kernel<false, true> launch each) and ignores rgb_w.
+void build_dgrad_plan(const NetDims& nd, const TcLinears& T, TcPlan* p) {
+    TcPlan& P = *p;
+    P = TcPlan{};
+    P.L = nd.L;
+    P.bstride = 256;
+    int woff = 0, ng = 0;
+    for (int j = T.n - 2; j >= 1; --j) {     // T.l[T.n - 1] is the rgb Linear: its input gradient comes from the head stage
+        const int epi = T.l[j - 1].epi;      // of the Linear whose output gradient this GEMM produces (tape image j - 1)
+        TcGemm& g = P.g[ng++];
+        g.n = nd.L;
+        g.nseg = 1;
+        g.src[0] = SRC_H;
+        g.k[0] = T.l[j].n;
+        g.w_off = woff;
+        g.img = j - 1;
+        g.epi = epi == EPI_LINEAR ? EPI_D_LINEAR : epi == EPI_RELU_SIGMA ? EPI_D_MASK_SIGMA : EPI_D_MASK;
+        woff += g.k[0] * g.n * 2;
+    }
+    P.n_gemm = P.n_trunk = ng;
+    P.plane_bytes = woff;
+    P.sigma_w_off = 0;
+    P.f32_floats = nd.L + nd.rgb_dim * (nd.L / 2);
+    P.f32_off = woff;
+    P.sub_bytes = (int)mn_align((size_t)woff + (size_t)P.f32_floats * 4, 256);
+}
+
+// ---- which engine serves a network, and whether tensor-core training covers it
+enum { TC_NONE = 0, TC_FUSED = 1, TC_LAYER = 2 };
+struct TcNet {
+    int engine;
+    bool train;          // tensor-core training covers the shape (mn_model_train_tc_supported once the weights are packed)
+    TcLinears lin;
+    TcPlan F;            // TC_FUSED
+    LayerPlan P;         // TC_LAYER
+    TcPlan D;            // train: the data-gradient chain and the layout of the transposed weight images (tc_dgrad)
+};
+
+TcNet tc_net(const mn_model& m) {
+    const NetDims& nd = m.nd;
+    TcNet t{};
+    t.lin = tc_linears(m);
+    if (build_layer_plan(nd, t.lin, &t.P)) t.engine = TC_LAYER;
+    else if (build_plan(nd, t.lin, &t.F)) t.engine = TC_FUSED;
+    t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers >= 2 &&
+              (t.engine == TC_LAYER || (t.engine == TC_FUSED && nd.L == 256 && nd.layers <= 10));
+    if (t.train) build_dgrad_plan(nd, t.lin, &t.D);
+    return t;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -277,9 +375,11 @@ __device__ __forceinline__ void tc_emit_rgb(const MlpArgs& m, int sub, int64_t r
 // ------------------------------------------------------------------------------------------------
 // feature tiles
 // ------------------------------------------------------------------------------------------------
-// Feature tile `tile` (global index: routing, rows) stored as tile `out_tile` of ximg.
-__device__ __forceinline__ void tc_encode_tile(const MlpArgs& a, int kpe, int kaux, int split, __half* __restrict__ ximg,
-                                               int64_t plane_stride_halves, int64_t tile, int64_t out_tile) {
+// Feature tiles tile0 .. tile0 + gridDim.x - 1 (global index: routing, rows), stored from tile 0 of ximg: the fused engine
+// encodes every tile in one launch (tile0 = 0), the layer-GEMM engine one tile group per launch.
+__global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int kpe, int kaux, int split, __half* __restrict__ ximg,
+                                                           int64_t plane_stride_halves, int64_t tile0) {
+    const int64_t tile = tile0 + blockIdx.x, out_tile = blockIdx.x;
     extern __shared__ __align__(16) unsigned char sm_raw[];
     __half* img = reinterpret_cast<__half*>(sm_raw);                  // hi image, then lo image
     const int ktot = kpe + kaux;
@@ -347,17 +447,6 @@ __device__ __forceinline__ void tc_encode_tile(const MlpArgs& a, int kpe, int ka
         uint4* d4l = reinterpret_cast<uint4*>(ximg + plane_stride_halves + out_tile * (int64_t)ktot * kTileM);
         for (int i = t; i < nvec; i += kTileM) d4l[i] = s4l[i];
     }
-}
-
-__global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int kpe, int kaux, int split,
-                                                           __half* __restrict__ ximg, int64_t plane_stride_halves) {
-    tc_encode_tile(a, kpe, kaux, split, ximg, plane_stride_halves, blockIdx.x, blockIdx.x);
-}
-
-// the layer-GEMM path (mn_layer_gemm.cuh): the tiles tile0 .. tile0 + gridDim.x - 1 of one tile group, stored from tile 0 of ximg
-__global__ void __launch_bounds__(kTileM) tc_layer_encode_kernel(const MlpArgs a, int kpe, int kaux, int split,
-                                                                 __half* __restrict__ ximg, int64_t plane_stride_halves, int64_t tile0) {
-    tc_encode_tile(a, kpe, kaux, split, ximg, plane_stride_halves, tile0 + blockIdx.x, blockIdx.x);
 }
 
 
@@ -523,19 +612,23 @@ LgWorkspace lg_workspace(const LayerPlan& P, int64_t n_tiles128, int precision) 
 }  // namespace
 
 // =================================================================================================
-size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision) {
-    LayerPlan LP;
-    if (build_layer_plan(m->nd, &LP)) return lg_workspace(LP, n_tiles128, precision).total;
-    TcPlan P;
-    if (!build_plan(m->nd, &P)) return 0;
+static size_t fused_workspace(const TcPlan& F, int64_t n_tiles128, int precision) {
     const size_t planes = precision == MN_PREC_TC_F16X3 ? 2 : 1;
-    return mn_align((size_t)n_tiles128 * P.x_tile_bytes * planes, 1024) + 1024;
+    return mn_align((size_t)n_tiles128 * F.x_tile_bytes * planes, 1024) + 1024;
+}
+
+size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision) {
+    const TcNet net = tc_net(*m);
+    if (net.engine == TC_LAYER) return lg_workspace(net.P, n_tiles128, precision).total;
+    if (net.engine == TC_FUSED) return fused_workspace(net.F, n_tiles128, precision);
+    return 0;
 }
 
 
-int mn_mlp_tp_program(const NetDims& nd, unsigned int* table_out, int cap_entries, int* info8) {
-    TcPlan P;
-    if (!build_plan(nd, &P)) return MN_ERR_UNSUPPORTED;
+int mn_mlp_tp_program(const mn_model& m, unsigned int* table_out, int cap_entries, int* info8) {
+    const TcNet net = tc_net(m);
+    if (net.engine != TC_FUSED) return MN_ERR_UNSUPPORTED;
+    const TcPlan& P = net.F;
     const WgLayout L = wg_layout(P, false);
     int n = 0, n_trunk = 0;
     for (int gi = 0; gi < P.n_gemm; ++gi) {
@@ -557,112 +650,54 @@ int mn_mlp_tp_program(const NetDims& nd, unsigned int* table_out, int cap_entrie
     return n <= cap_entries ? MN_OK : MN_ERR_WORKSPACE;
 }
 
-// ---- tensor-core training of layer-GEMM networks: the shapes the backward covers, and its transposed weight images
-static bool layer_train_ok(const NetDims& nd) {
-    return nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers >= 2;
-}
-
-// Per sub-module: the data-gradient chain's B operands, each the transposed weight [in/256][out/8][256][8] fp16 (dir_a_encoding
-// restricted to its L feature columns, xyz_encoding_final, trunk layers layers-1 .. 1 restricted to their hidden columns), then
-// an fp32 block with sigma_w [L].
-struct LgDgrad {
-    int w_dira, w_final, w_layer[MN_MAX_LAYERS], f32_off;
-    size_t sub_bytes;
-};
-static LgDgrad lg_dgrad_layout(const NetDims& nd) {
-    LgDgrad D{};
-    const int L = nd.L;
-    int off = 0;
-    D.w_dira = off;  off += L * (L / 2) * 2;
-    D.w_final = off; off += L * L * 2;
-    for (int l = nd.layers - 1; l >= 1; --l) { D.w_layer[l] = off; off += L * L * 2; }
-    D.f32_off = off;
-    D.sub_bytes = mn_align((size_t)off + (size_t)L * sizeof(float), 256);
-    return D;
-}
-
-static void layer_pack_dgrad(mn_ctx* ctx, mn_model* m, int sub) {
+// ---- transposed weight images of the data-gradient chain (build_dgrad_plan), one fp16 plane + the fp32 block per sub-module.
+// Element (n = input column, k = output channel) = W[k][n]: the [out][L] BwdLayout sub-matrix is the K-major source.
+static void tc_pack_dgrad(mn_ctx* ctx, mn_model* m, int sub, const TcNet& net) {
     const NetDims& nd = m->nd;
-    const LgDgrad D = lg_dgrad_layout(nd);
-    const int L = nd.L;
+    const TcPlan& D = net.D;
     unsigned char* db = (unsigned char*)m->tc_dgrad + (size_t)sub * D.sub_bytes;
     const float* Q = m->packed_bwd + (size_t)sub * m->blay.total;
-    // element (n = input column, k = output channel) = W[k][n]: the [out][in] sub-matrix is the K-major source of PK_TC_HALF
-    auto img = [&](int w_off, const float* w, int n_out) {
-        mn_pack_push(ctx, PackOp{w, db + w_off, nullptr, (long long)L * n_out, PK_TC_HALF, {L, n_out, L, n_out, 0, 0, 256}});
-    };
-    img(D.w_dira, Q + m->blay.dira_f, L / 2);
-    img(D.w_final, Q + m->blay.final_w, L);
-    for (int l = nd.layers - 1; l >= 1; --l) img(D.w_layer[l], Q + m->blay.w[l], L);
-    mn_pack_push(ctx, PackOp{m->packed + (size_t)sub * m->lay.total + m->lay.sigma_w, db + D.f32_off, nullptr, (long long)L, PK_TC_F32,
-                             {L, 0, 0, 0, 0, 0, 0}});
+    const float* Pk = m->packed + (size_t)sub * m->lay.total;
+    for (int gi = 0; gi < D.n_gemm; ++gi) {
+        const TcGemm& g = D.g[gi];
+        const int k = g.k[0];
+        mn_pack_push(ctx, PackOp{Q + net.lin.l[g.img + 1].bwd, db + g.w_off, nullptr, (long long)g.n * k, PK_TC_HALF,
+                                 {nd.L, k, g.n, k, 0, 0, 256}});
+    }
+    float* f32 = reinterpret_cast<float*>(db + D.f32_off);
+    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
+    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + nd.L, nullptr, (long long)nd.rgb_dim * (nd.L / 2), PK_RGBW,
+                             {nd.L / 2, nd.rgb_dim, 0, 0, 0, 0, 0}});
 }
 
 // The transposed images cost as much as the forward images again, so they are allocated and packed by the first recording call
 // (inference-only users never hold them); from then on every mn_model_set_weights repacks them with the forward images.
-static int layer_dgrad_ready(mn_ctx* ctx, mn_model* m, cudaStream_t st) {
+static int tc_dgrad_ready(mn_ctx* ctx, mn_model* m, const TcNet& net, cudaStream_t st) {
     if (m->tc_dgrad) return MN_OK;
-    const LgDgrad D = lg_dgrad_layout(m->nd);
-    MN_CUDA(ctx, cudaMalloc(&m->tc_dgrad, D.sub_bytes * m->d.n_sub));
-    m->tc_dgrad_sub_bytes = D.sub_bytes;
-    for (int s = 0; s < m->d.n_sub; ++s) layer_pack_dgrad(ctx, m, s);
+    const size_t bytes = (size_t)net.D.sub_bytes * m->d.n_sub;
+    MN_CUDA(ctx, cudaMalloc(&m->tc_dgrad, bytes));
+    MN_CUDA(ctx, cudaMemsetAsync(m->tc_dgrad, 0, bytes, st));
+    m->tc_dgrad_sub_bytes = (size_t)net.D.sub_bytes;
+    for (int s = 0; s < m->d.n_sub; ++s) tc_pack_dgrad(ctx, m, s, net);
     return mn_pack_flush(ctx, st);
 }
 
-// Layer-GEMM networks: per sub-module [hi plane][lo plane][fp32 block], every weight image [n_blk][K/8][256][8] with its fp16
-// residual in the lo plane.  Training images: see layer_dgrad_ready.
-static int layer_pack(mn_ctx* ctx, mn_model* m, int sub, const LayerPlan& P, cudaStream_t st) {
-    const NetDims& nd = m->nd;
-    const size_t sub_bytes = mn_align((size_t)P.plane_bytes * 2 + (size_t)P.f32_floats * 4, 256);
-    if (!m->tc_packed) {
-        MN_CUDA(ctx, cudaMalloc(&m->tc_packed, sub_bytes * m->d.n_sub));
-        MN_CUDA(ctx, cudaMemsetAsync(m->tc_packed, 0, sub_bytes * m->d.n_sub, st));
-        m->tc_sub_bytes = sub_bytes;
-    }
-    unsigned char* base = (unsigned char*)m->tc_packed + (size_t)sub * sub_bytes;
-    const float* Pk = m->packed + (size_t)sub * m->lay.total;
-    float* f32 = reinterpret_cast<float*>(base + (size_t)P.plane_bytes * 2);
-    auto pack = [&](const LgGemm& g, const float* wt, int k_src, int k_real0, int k_pad0, const float* bias) {
-        const int K = g.k[0] + (g.nseg > 1 ? g.k[1] : 0), np = g.n_blk * 256;
-        mn_pack_push(ctx, PackOp{wt, base + g.w_off, base + P.plane_bytes + g.w_off, (long long)np * K, PK_TC_HALF,
-                                 {g.n, k_src, np, K, k_real0, k_pad0, 256}});
-        mn_pack_push(ctx, PackOp{bias, f32 + g.bias_off, nullptr, (long long)np, PK_TC_F32, {g.n, 0, 0, 0, 0, 0, 0}});
-    };
-    int gi = 0;
-    for (int i = 0; i < nd.layers; ++i, ++gi) {
-        const bool has_pe = (i == 0) || ((nd.skip_mask >> i) & 1);
-        pack(P.g[gi], Pk + m->lay.w[i], m->lay.kin[i], has_pe ? nd.in_xyz : 0, has_pe ? P.kpe : 0, Pk + m->lay.b[i]);
-    }
-    if (nd.has_dir_a) {
-        pack(P.g[gi++], Pk + m->lay.final_w, nd.L, 0, 0, Pk + m->lay.final_b);
-        pack(P.g[gi++], Pk + m->lay.dira_w, nd.L + nd.aux, 0, 0, Pk + m->lay.dira_b);
-    }
-    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + P.sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
-    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + P.sigma_w_off + nd.L, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
-    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + P.rgb_w_off, nullptr, (long long)nd.rgb_dim * nd.rgb_in, PK_RGBW,
-                             {nd.rgb_in, nd.rgb_dim, 0, 0, 0, 0, 0}});
-    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + P.rgb_b_off, nullptr, MN_TC_RGB_MAX, PK_TC_F32, {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
-    m->tc_ready = 1;
-    m->train_tc_ok = layer_train_ok(nd) ? 1 : 0;
-    if (m->train_tc_ok && m->tc_dgrad) layer_pack_dgrad(ctx, m, sub);
-    return MN_OK;
-}
-
+// Forward weight images.  Per sub-module: [hi plane][lo plane][fp32 block], every weight image [N/nw][K/8][nw][8] fp16 with its
+// fp16 residual in the lo plane: nw = N <= 256 for the fused engine (two N = 256 halves for the 512-wide network), 256 for the
+// layer engine (its N is padded to 256-column blocks).  The fp32 block holds the biases, sigma_w and sigma_b, and for the layer
+// engine the rgb head.  Queued: all images of the sub-module are written by ONE launch (mn_pack_flush in mn_model_set_weights).
 int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
-    {
-        LayerPlan LP;
-        if (build_layer_plan(m->nd, &LP)) return layer_pack(ctx, m, sub, LP, st);
-    }
-    TcPlan P;
-    if (!build_plan(m->nd, &P)) {
+    const TcNet net = tc_net(*m);
+    if (net.engine == TC_NONE) {
         m->tc_ready = 0;
         return MN_OK;  // configuration only served by the fp32 kernel
     }
     const NetDims& nd = m->nd;
-    // per sub-module: [hi plane][lo plane][fp32 block, 256-aligned]
-    // 512-wide network (tc_f16 only): its one image per GEMM ([N half of 256][K/8][256][8]) lives in the hi plane
-    const bool wide = nd.L > 256;
-    const size_t sub_bytes = mn_align((size_t)P.plane_bytes * 2 + (size_t)(((P.f32_floats * 4 + 255) / 256) * 256), 256);
+    const bool fused = net.engine == TC_FUSED;
+    const TcPlan& F = net.F;
+    const LayerPlan& P = net.P;
+    const int plane = fused ? F.plane_bytes : P.plane_bytes, n_gemm = fused ? F.n_gemm : P.n_gemm;
+    const size_t sub_bytes = mn_align((size_t)plane * 2 + (size_t)(fused ? F.f32_floats : P.f32_floats) * 4, 256);
     if (!m->tc_packed) {
         MN_CUDA(ctx, cudaMalloc(&m->tc_packed, sub_bytes * m->d.n_sub));
         MN_CUDA(ctx, cudaMemsetAsync(m->tc_packed, 0, sub_bytes * m->d.n_sub, st));
@@ -670,62 +705,31 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
     }
     unsigned char* base = (unsigned char*)m->tc_packed + (size_t)sub * sub_bytes;
     const float* Pk = m->packed + (size_t)sub * m->lay.total;
-    float* f32 = reinterpret_cast<float*>(base + (size_t)P.plane_bytes * 2);
-    auto pack = [&](const TcGemm& g, const float* wt, int n_src, int k_src, int k_real0, int k_pad0, const float* bias,
-                    int n_bias) {
-        const int K = g.k[0] + (g.nseg > 1 ? g.k[1] : 0);
-        const int64_t n = (int64_t)g.n * K;
-        __half* hi = reinterpret_cast<__half*>(base + g.w_off);
-        __half* lo = reinterpret_cast<__half*>(base + P.plane_bytes + g.w_off);
-        // queued: all images of the sub-module are written by ONE launch (mn_pack_flush in mn_model_set_weights)
-        if (wide) {
-            mn_pack_push(ctx, PackOp{wt, hi, nullptr, (long long)n, PK_TC_HALF, {n_src, k_src, g.n, K, k_real0, k_pad0, g.n < 256 ? g.n : 256}});
-            mn_pack_push(ctx, PackOp{bias, f32 + g.bias_off, nullptr, (long long)P.bstride, PK_TC_F32, {n_bias, 0, 0, 0, 0, 0, 0}});
-            return;
-        }
-        mn_pack_push(ctx, PackOp{wt, hi, lo, (long long)n, PK_TC_IMAGE, {n_src, k_src, g.n, K, k_real0, k_pad0, 0}});
-        mn_pack_push(ctx, PackOp{bias, f32 + g.bias_off, nullptr, 256, PK_TC_F32, {n_bias, 0, 0, 0, 0, 0, 0}});
-    };
-    int gi = 0;
-    for (int i = 0; i < nd.layers; ++i, ++gi) {
-        const bool has_pe = (i == 0) || ((nd.skip_mask >> i) & 1);
-        pack(P.g[gi], Pk + m->lay.w[i], nd.L, m->lay.kin[i], has_pe ? nd.in_xyz : 0, has_pe ? P.kpe : 0, Pk + m->lay.b[i], nd.L);
+    float* f32 = reinterpret_cast<float*>(base + (size_t)plane * 2);
+    for (int gi = 0; gi < n_gemm; ++gi) {
+        const TcLinear& l = net.lin.l[gi];
+        // image N (the fused rgb GEMM has N = 32) and the floats reserved for the bias: the fused plan's bias stride, or the
+        // layer plan's N blocks
+        const int n_img = fused ? F.g[gi].n : P.g[gi].n_blk * 256, w_off = fused ? F.g[gi].w_off : P.g[gi].w_off;
+        const int b_off = fused ? F.g[gi].bias_off : P.g[gi].bias_off, b_n = fused ? F.bstride : n_img;
+        const int K = l.seg[0].k + (l.nseg > 1 ? l.seg[1].k : 0);
+        // a leading PE segment holds its real columns, then zeros up to its padded width; the other columns follow contiguously
+        const bool pe = l.seg[0].src == SRC_XPE;
+        mn_pack_push(ctx, PackOp{Pk + l.w, base + w_off, base + plane + w_off, (long long)n_img * K, PK_TC_HALF,
+                                 {l.n, l.kin, n_img, K, pe ? l.seg[0].k_real : 0, pe ? l.seg[0].k : 0, n_img < 256 ? n_img : 256}});
+        mn_pack_push(ctx, PackOp{Pk + l.b, f32 + b_off, nullptr, (long long)b_n, PK_TC_F32, {l.n, 0, 0, 0, 0, 0, 0}});
     }
-    if (nd.has_dir_a) {
-        pack(P.g[gi++], Pk + m->lay.final_w, nd.L, nd.L, 0, 0, Pk + m->lay.final_b, nd.L);
-        pack(P.g[gi++], Pk + m->lay.dira_w, nd.L / 2, nd.L + nd.aux, 0, 0, Pk + m->lay.dira_b, nd.L / 2);
+    const int sigma_w_off = fused ? F.sigma_w_off : P.sigma_w_off;
+    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
+    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + sigma_w_off + nd.L, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
+    if (!fused) {      // tc_layer_head_kernel computes the rgb head on the CUDA cores
+        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + P.rgb_w_off, nullptr, (long long)nd.rgb_dim * nd.rgb_in, PK_RGBW,
+                                 {nd.rgb_in, nd.rgb_dim, 0, 0, 0, 0, 0}});
+        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + P.rgb_b_off, nullptr, MN_TC_RGB_MAX, PK_TC_F32, {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
     }
-    pack(P.g[gi++], Pk + m->lay.rgb_w, nd.rgb_dim, nd.rgb_in, 0, 0, Pk + m->lay.rgb_b, nd.rgb_dim);
-    // sigma_w [L] + sigma_b
-    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + P.sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
-    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + P.sigma_w_off + nd.L, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
     m->tc_ready = 1;
-
-    // ---- data-gradient images of the tensor-core training path (transposed weights, single fp16 plane + fp32 block)
-    TcPlan D;
-    m->train_tc_ok = 0;
-    if (!wide && build_dgrad_plan(nd, &D)) {
-        if (!m->tc_dgrad) {
-            MN_CUDA(ctx, cudaMalloc(&m->tc_dgrad, (size_t)D.sub_bytes * m->d.n_sub));
-            MN_CUDA(ctx, cudaMemsetAsync(m->tc_dgrad, 0, (size_t)D.sub_bytes * m->d.n_sub, st));
-            m->tc_dgrad_sub_bytes = (size_t)D.sub_bytes;
-        }
-        unsigned char* db = (unsigned char*)m->tc_dgrad + (size_t)sub * D.sub_bytes;
-        const float* Q = m->packed_bwd + (size_t)sub * m->blay.total;
-        auto packd = [&](const TcGemm& g, const float* wd, int ld) {
-            mn_pack_push(ctx, PackOp{wd, db + g.w_off, nullptr, (long long)g.n * g.k[0], PK_DGRAD, {ld, g.n, g.k[0], 0, 0, 0, 0}});
-        };
-        int di = 0;
-        packd(D.g[di++], Q + m->blay.dira_f, nd.L);         // [L/2][L]
-        packd(D.g[di++], Q + m->blay.final_w, nd.L);        // [L][L]
-        for (int l = nd.layers - 1; l >= 1; --l)
-            packd(D.g[di++], Q + m->blay.w[l], nd.L);       // [L][L]: hidden-part columns of layer l
-        float* df32 = reinterpret_cast<float*>(db + D.f32_off);
-        mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, df32, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
-        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, df32 + nd.L, nullptr, (long long)nd.rgb_dim * (nd.L / 2), PK_RGBW,
-                                 {nd.L / 2, nd.rgb_dim, 0, 0, 0, 0, 0}});
-        m->train_tc_ok = 1;
-    }
+    m->train_tc_ok = net.train ? 1 : 0;
+    if (net.train && m->tc_dgrad) tc_pack_dgrad(ctx, m, sub, net);
     return MN_OK;
 }
 
@@ -740,21 +744,20 @@ static int tc_encode(mn_ctx* ctx, const mn_model* m, const MlpArgs& a, const TcP
     if (fast_shape)
         tc_encode_fast_kernel<3, 12, 4, 48><<<(unsigned)n_tiles128, kTileM, 0, st>>>(a, ximg);
     else
-        tc_encode_kernel<<<(unsigned)n_tiles128, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split, ximg, plane_halves);
+        tc_encode_kernel<<<(unsigned)n_tiles128, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split, ximg, plane_halves, 0);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }
 
-// TcArgs fields common to the inference and the recording forward: the plan and the model's packed weights.  False when the
-// network shape has no tensor-core plan or the weights are not packed.
-static bool tc_forward_args(const mn_model* m, const MlpArgs& a, int64_t n_tiles128, TcArgs* A) {
-    *A = TcArgs{};
-    if (!build_plan(a.nd, &A->plan) || !m->tc_ready) return false;
-    A->plan.sub_bytes = (int)m->tc_sub_bytes;
-    A->m = a;
-    A->wpack = (const unsigned char*)m->tc_packed;
-    A->n_tiles_cap = n_tiles128;
-    return true;
+// TcArgs fields common to the inference and the recording forward of the fused engine: the plan and the model's packed weights.
+static TcArgs tc_forward_args(const mn_model* m, const TcPlan& F, const MlpArgs& a, int64_t n_tiles128) {
+    TcArgs A{};
+    A.plan = F;
+    A.plan.sub_bytes = (int)m->tc_sub_bytes;
+    A.m = a;
+    A.wpack = (const unsigned char*)m->tc_packed;
+    A.n_tiles_cap = n_tiles128;
+    return A;
 }
 
 // Layer-GEMM path: the slot tiles in groups of kLgGroupTiles; per group one encoder launch, one GEMM launch per Linear and one
@@ -777,7 +780,7 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
     const int64_t act_tile = tape ? (int64_t)mn_train_tc_act_tile_bytes(m) : 0;
 
     const size_t enc_sm = (size_t)P.x_tile_bytes * (split ? 2 : 1);
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
+    MN_CUDA(ctx, cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
     const int gemm_sm = split ? LgShape<true>::smem : LgShape<false>::smem;
     if (split) MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
     else MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
@@ -789,7 +792,7 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
         const int64_t nt = n_tiles128 - t0 < W.group_tiles ? n_tiles128 - t0 : W.group_tiles;
         unsigned char* rec = tape ? tape->act + t0 * act_tile : nullptr;      // activation record of the group's first tile
         if (tape) ximg = reinterpret_cast<__half*>(tape->xreg + t0 * (int64_t)P.x_tile_bytes);
-        tc_layer_encode_kernel<<<(unsigned)nt, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split ? 1 : 0, ximg, plane_halves, t0);
+        tc_encode_kernel<<<(unsigned)nt, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split ? 1 : 0, ximg, plane_halves, t0);
         MN_LAUNCH_CHECK(ctx);
         for (int gi = 0; gi < n_gemm; ++gi) {
             const LgGemm& g = P.g[gi];
@@ -868,12 +871,9 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
 
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws, size_t ws_bytes,
                      cudaStream_t st) {
-    {
-        LayerPlan LP;
-        if (build_layer_plan(a.nd, &LP)) return layer_launch(ctx, m, a, LP, n_tiles128, precision, ws, ws_bytes, st);
-    }
-    TcArgs A;
-    if (!tc_forward_args(m, a, n_tiles128, &A))
+    const TcNet net = tc_net(*m);
+    if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net.P, n_tiles128, precision, ws, ws_bytes, st);
+    if (net.engine != TC_FUSED || !m->tc_ready)
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "tensor-core MLP path covers layer_dim 64..256 (multiple of 64), 512 or 768..2048 (multiple of 256) and rgb_dim <= 32; "
                        "use precision 'fp32' for this model");
@@ -881,11 +881,11 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "precision 'tc_f16x3' covers layer_dim <= 256; use 'tc_f16' or 'fp32' for the 512-wide network");
     if (n_tiles128 <= 0) return MN_OK;
+    TcArgs A = tc_forward_args(m, net.F, a, n_tiles128);
     const TcPlan& P = A.plan;
     const int split = precision == MN_PREC_TC_F16X3 ? 1 : 0;
     A.split = split;
-    const size_t need = mn_mlp_tc_workspace(m, n_tiles128, precision);
-    if (ws_bytes < need || !ws) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
+    if (ws_bytes < fused_workspace(P, n_tiles128, precision) || !ws) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
     uintptr_t wp = ((uintptr_t)ws + 1023) / 1024 * 1024;
     __half* ximg = reinterpret_cast<__half*>(wp);
     A.ximg = ximg;
@@ -905,10 +905,9 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
 // tensor-core training path: host side (kernels in mn_train_tc.cuh)
 // =================================================================================================
 size_t mn_train_tc_x_tile_bytes(const mn_model* m) {
-    LayerPlan LP;
-    if (build_layer_plan(m->nd, &LP)) return (size_t)LP.x_tile_bytes;
-    TcPlan P;
-    return build_plan(m->nd, &P) ? (size_t)P.x_tile_bytes : 0;
+    const TcNet net = tc_net(*m);
+    if (net.engine == TC_LAYER) return (size_t)net.P.x_tile_bytes;
+    return net.engine == TC_FUSED ? (size_t)net.F.x_tile_bytes : 0;
 }
 size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
     const NetDims& nd = m->nd;
@@ -917,26 +916,20 @@ size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
 
 // recording forward: encoder tiles and every layer's activations land in the caller's tape
 int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
-    TcArgs A;
-    LayerPlan LP;
-    const bool layer = build_layer_plan(a.nd, &LP);
-    if (!m->train_tc_ok || (!layer && !tc_forward_args(m, a, n_tiles128, &A)))
-        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core training covers layer_dim 256 or 768..2048 (a multiple of 256) with a direction / "
-                                                "appearance head and rgb_dim 3 or a raw SH head (rgb_dim <= 32), no affine appearance; "
-                                                "use train precision 'fp32'");
+    if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
     if (n_tiles128 <= 0) return MN_OK;
-    if (layer) {
-        const int rc = layer_dgrad_ready(ctx, m, st);
-        if (rc) return rc;
-        return layer_launch(ctx, m, a, LP, n_tiles128, MN_PREC_TC_F16, nullptr, 0, st, &tape);
-    }
+    const TcNet net = tc_net(*m);
+    int rc = tc_dgrad_ready(ctx, m, net, st);
+    if (rc) return rc;
+    if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net.P, n_tiles128, MN_PREC_TC_F16, nullptr, 0, st, &tape);
+    TcArgs A = tc_forward_args(m, net.F, a, n_tiles128);
     A.ximg = reinterpret_cast<const __half*>(tape.xreg);
     A.x_plane_halves = 0;
     A.tape_act = tape.act;
     A.tape_f32 = tape.f32;
     A.act_tile_bytes = (int64_t)mn_train_tc_act_tile_bytes(m);
     A.layers = a.nd.layers;
-    int rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st);
+    rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st);
     if (rc) return rc;
     mn_prof_begin(ctx, st);
     rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
@@ -944,51 +937,70 @@ int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n
     return rc;
 }
 
-// backward workspace: [gradient records][head gradients fp32 [n_tiles][mn_tc_g32_rows(rgb_dim)][128]][embedding sums][scale, max |grad_out|]
-static size_t train_tc_emb_floats(const mn_model* m) {
-    return m->nd.app_in_dira ? (size_t)m->d.n_sub * m->nd.app_count * (m->nd.L / 2) : 0;
-}
-static size_t train_tc_head_grad_bytes(const mn_model* m, int64_t n_tiles128) {
-    return mn_align((size_t)n_tiles128 * mn_tc_g32_rows(m->nd.rgb_dim) * kTileM * sizeof(float));
-}
-// Layer-GEMM networks: gradient images of one tile group only (dZ_G and two ping-pong L-column buffers), so the workspace is
-// bounded by kLgGroupTiles, not by the row count.
-static int64_t lg_train_group_tiles(int64_t n_tiles128) { return n_tiles128 < kLgGroupTiles ? n_tiles128 : kLgGroupTiles; }
-static size_t lg_train_dz_bytes(const mn_model* m, int64_t n_tiles128) {
-    return mn_align((size_t)lg_train_group_tiles(n_tiles128) * (m->nd.L / 2) * kTileM * 2) +
-           2 * mn_align((size_t)lg_train_group_tiles(n_tiles128) * m->nd.L * kTileM * 2);
+// backward workspace: [gradient images][head gradients fp32 [head_tiles][mn_tc_g32_rows(rgb_dim)][128]][embedding sums][scale,
+// max |grad_out|].  Fused engine: the gradient records of every tile.  Layer engine: the gradient images of one tile group only
+// (dZ_G and two ping-pong L-column buffers), so its workspace is bounded by kLgGroupTiles, not by the row count.
+struct TcBwdWorkspace {
+    int64_t head_tiles;
+    size_t dz_bytes, head_bytes, emb_floats, total;
+};
+static TcBwdWorkspace tc_bwd_workspace(const mn_model* m, const TcNet& net, int64_t n_tiles128) {
+    const NetDims& nd = m->nd;
+    TcBwdWorkspace w{};
+    if (net.engine == TC_LAYER) {
+        w.head_tiles = n_tiles128 < kLgGroupTiles ? n_tiles128 : kLgGroupTiles;
+        w.dz_bytes = mn_align((size_t)w.head_tiles * (nd.L / 2) * kTileM * 2) + 2 * mn_align((size_t)w.head_tiles * nd.L * kTileM * 2);
+    } else {
+        w.head_tiles = n_tiles128;
+        w.dz_bytes = mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m));
+    }
+    w.head_bytes = mn_align((size_t)w.head_tiles * mn_tc_g32_rows(nd.rgb_dim) * kTileM * sizeof(float));
+    w.emb_floats = nd.app_in_dira ? (size_t)m->d.n_sub * nd.app_count * (nd.L / 2) : 0;
+    w.total = w.dz_bytes + w.head_bytes + mn_align(w.emb_floats * sizeof(float) + 256) + 1024;
+    return w;
 }
 size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
-    LayerPlan LP;
-    if (build_layer_plan(m->nd, &LP))
-        return lg_train_dz_bytes(m, n_tiles128) + train_tc_head_grad_bytes(m, lg_train_group_tiles(n_tiles128)) +
-               mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) + 1024;
-    return mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m)) + train_tc_head_grad_bytes(m, n_tiles128) +
-           mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) + 1024;
+    return tc_bwd_workspace(m, tc_net(*m), n_tiles128).total;
 }
 
-// ---- backward of a layer-GEMM network, one tile group at a time: head stage -> per Linear (output side first) the weight
-// gradient from its dZ image, then the data-gradient GEMM that produces the next dZ in the other ping-pong buffer; then the
-// sigma / rgb head weight gradients.  dZ of Linear l is consumed by its weight gradient before the buffer is overwritten.
-static int layer_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, const LayerPlan& P, int64_t n_tiles128, const TrainTcTape& tape,
-                          void* ws, cudaStream_t st) {
+// Weight-gradient item of input segment s of Linear j for its output channels 0..127 and the segment's first columns: X is
+// image j - 1 of the activation record (SRC_H) or a segment of the feature tile.
+static WgItem wg_item(const TcLinears& T, int j, int s, int L) {
+    const TcLinear& l = T.l[j];
+    const TcSeg& g = l.seg[s];
+    WgItem it{};
+    it.x_region = g.src == SRC_H ? 0 : 1;
+    it.x_off = g.src == SRC_H ? (int)mn_tc_img_off(j - 1, L) : g.src == SRC_XAUX ? (T.kpe / 8) * (kTileM * 16) : 0;
+    it.n = g.k;
+    it.n_real = g.k_real;
+    it.w_off = l.w + g.in0;
+    it.k_in = l.kin;
+    it.b_off = s == 0 ? l.b : -1;      // the first segment owns the bias
+    return it;
+}
+
+int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_tiles128, const TrainTcTape& tape, void* ws, size_t ws_bytes,
+                         cudaStream_t st) {
+    if (!m->train_tc_ok || !m->tc_dgrad) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: unsupported network shape");
+    if (n_tiles128 <= 0) return MN_OK;
+    const TcNet net = tc_net(*m);
+    const TcBwdWorkspace WS = tc_bwd_workspace(m, net, n_tiles128);
+    if (!ws || ws_bytes < WS.total) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_train_tc_backward: workspace too small");
     const NetDims& nd = a.nd;
-    const int L = nd.L, half = L / 2, rows = mn_tc_g32_rows(nd.rgb_dim);
-    const int64_t gt = lg_train_group_tiles(n_tiles128);
+    const TcLinears& lin = net.lin;
+    const int L = nd.L, half = L / 2;
     const int64_t act_tile = (int64_t)mn_train_tc_act_tile_bytes(m);
-    const LgDgrad D = lg_dgrad_layout(nd);
     char* wp = (char*)(((uintptr_t)ws + 255) / 256 * 256);
-    unsigned char* dzg = (unsigned char*)wp;              wp += mn_align((size_t)gt * half * kTileM * 2);
-    unsigned char* pp[2];
-    for (int b = 0; b < 2; ++b) { pp[b] = (unsigned char*)wp; wp += mn_align((size_t)gt * L * kTileM * 2); }
-    float* gf32 = (float*)wp;                             wp += train_tc_head_grad_bytes(m, gt);
-    float* emb_sum = (float*)wp;                          wp += mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) - 256;
+    unsigned char* dz = (unsigned char*)wp;               wp += WS.dz_bytes;
+    float* gf32 = (float*)wp;                             wp += WS.head_bytes;
+    float* emb_sum = (float*)wp;                          wp += mn_align(WS.emb_floats * sizeof(float) + 256) - 256;
     float* scale = (float*)wp;
-    unsigned* maxbits = reinterpret_cast<unsigned*>(scale + 1);
-    if (train_tc_emb_floats(m)) MN_CUDA(ctx, cudaMemsetAsync(emb_sum, 0, train_tc_emb_floats(m) * sizeof(float), st));
+    unsigned* maxbits = reinterpret_cast<unsigned*>(scale + 1);     // max |grad_out| (float bits), inside the same 256 bytes
+    if (WS.emb_floats) MN_CUDA(ctx, cudaMemsetAsync(emb_sum, 0, WS.emb_floats * sizeof(float), st));
     MN_CUDA(ctx, cudaMemsetAsync(maxbits, 0, sizeof(unsigned), st));
 
-    mn_prof_begin(ctx, st);
+    mn_prof_begin(ctx, st);   // bench.py --mode train: the whole backward of the MLP stage timed as one span
+    // ---- gradient scale (power of two) from the upstream gradient
     {
         const int64_t n = a.grad_rows * a.out_cols;
         const int64_t blocks = std::min<int64_t>(std::max<int64_t>(mn_cdiv(n, (int64_t)256 * 16), 1), (int64_t)ctx->sm_count * 4);
@@ -1007,127 +1019,11 @@ static int layer_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, const Laye
     mm.B = a.B;
     mm.out_cols = a.out_cols;
     const int n_sub = a.counters ? a.n_sub : 1;
+    // tiles the forward pass really wrote: all bucketed tiles when routed, ceil(rows / 128) otherwise
     const int64_t tiles_used = a.counters ? n_tiles128 : mn_cdiv(a.B, (int64_t)kTileM);
-    constexpr int gemm_sm = LgShape<false>::smem;
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
     const int wg_smem = 2 * kWgStageBytes + 6144 + 256;
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
-
-    for (int64_t t0 = 0; t0 < tiles_used; t0 += gt) {
-        const int64_t nt = tiles_used - t0 < gt ? tiles_used - t0 : gt;
-        const unsigned char* rec = tape.act + t0 * act_tile;
-        // ---- head stage
-        {
-            LdArgs H{};
-            H.m = mm;
-            H.tile0 = t0;
-            H.grad_out = a.grad_out;
-            H.tape_f32 = tape.f32;
-            H.g = rec + mn_tc_img_off(nd.layers + 1, L);
-            H.g_tile_bytes = act_tile;
-            H.wpack = (const unsigned char*)m->tc_packed;
-            H.sub_bytes = (int64_t)m->tc_sub_bytes;
-            H.f32_off = P.plane_bytes * 2;
-            H.rgb_w_off = P.rgb_w_off;
-            H.half = half;
-            H.gf32 = gf32;
-            H.dz = dzg;
-            H.emb_sum = nd.app_in_dira ? emb_sum : nullptr;
-            H.scale = scale;
-            tc_layer_head_dgrad_kernel<<<(unsigned)nt, kTileM, 0, st>>>(H);
-            MN_LAUNCH_CHECK(ctx);
-        }
-        // ---- weight gradient of one Linear: dz = its output gradient images (n_out columns), segments (x_region, x_off, columns,
-        // weight columns, first weight column); the first segment owns the bias
-        struct Seg { int x_region, x_off, n, n_real, in0; };
-        auto wgrad = [&](const unsigned char* dz, int n_out, int w, int k_in, int b, Seg s0, Seg s1, int nseg) {
-            WgArgs W{};
-            const Seg seg[2] = {s0, s1};
-            for (int s = 0; s < nseg; ++s) {
-                WgItem& it = W.item[s];
-                it.dz_off = 0;
-                it.x_region = seg[s].x_region;
-                it.x_off = seg[s].x_off;
-                it.n = seg[s].n;
-                it.n_real = seg[s].n_real;
-                it.w_off = w + seg[s].in0;
-                it.k_in = k_in;
-                it.b_off = s == 0 ? b : -1;
-                W.n_chunks[s] = (seg[s].n + 255) / 256;
-            }
-            const int items = (n_out / 128) * (W.n_chunks[0] + W.n_chunks[1]);
-            W.n_items = items;
-            W.act = tape.act;
-            W.dz = dz;
-            W.xreg = tape.xreg;
-            W.act_tile_bytes = act_tile;
-            W.x_tile_bytes = P.x_tile_bytes;
-            W.dz_tile_bytes = (int64_t)n_out * kTileM * 2;
-            W.t_min = t0;
-            W.t_max = t0 + nt;
-            W.counters = a.counters;
-            W.n_tiles = tiles_used;
-            W.fixed_sub = a.fixed_sub;
-            W.gw = a.gw;
-            W.sub_stride = a.lay.total;
-            W.scale = scale;
-            // about one CTA per SM: every CTA flushes its 128 x 256 accumulators with fp32 atomics once
-            const int64_t chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count, (int64_t)items));
-            W.chunk_tiles = (int)mn_cdiv(nt, chunks);
-            tc_wgrad_kernel<true><<<dim3((unsigned)chunks, (unsigned)items, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
-            MN_LAUNCH_CHECK(ctx);
-        };
-        // ---- data gradient: dz_out = [mask](dz_in W^T) [+ S dsigma x sigma_w]
-        auto dgrad = [&](const unsigned char* dz_in, int k, int w_off, unsigned char* dz_out, int mask_img, bool sigma) {
-            LgArgs G{};
-            G.m = mm;
-            G.tile0 = t0;
-            G.n_tiles = nt;
-            G.wpack = (const unsigned char*)m->tc_dgrad;
-            G.sub_bytes = (int64_t)D.sub_bytes;
-            G.w_off = w_off;
-            G.k_tot = k;
-            G.n_blk = L / kLgBlock;
-            G.n_out = L;
-            G.bias_off = 0;
-            G.f32_off = D.f32_off;
-            G.nseg = 1;
-            G.a[0] = dz_in;
-            G.ak[0] = k;
-            G.a_tile_bytes[0] = (int64_t)k * kTileM * 2;
-            G.out = dz_out;
-            G.out_tile_bytes = (int64_t)L * kTileM * 2;
-            G.mask = mask_img >= 0 ? rec + mn_tc_img_off(mask_img, L) : nullptr;
-            G.mask_tile_bytes = act_tile;
-            G.dsig = sigma ? gf32 + MN_TC_G32_SIGMA * kTileM : nullptr;
-            G.dsig_tile_floats = (int64_t)rows * kTileM;
-            G.scale = scale;
-            const int64_t items = nt * G.n_blk;
-            const unsigned grid = (unsigned)(items < ctx->sm_count ? items : ctx->sm_count);
-            tc_layer_gemm_kernel<false, true><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
-            MN_LAUNCH_CHECK(ctx);
-        };
-        const Seg none{0, 0, 0, 0, 0};
-        const int xaux = (P.kpe / 8) * (kTileM * 16);
-        auto hseg = [&](int img, int in0) { return Seg{0, (int)mn_tc_img_off(img, L), L, L, in0}; };
-        // dir_a_encoding: input [F, dir PE + embedding]
-        wgrad(dzg, half, a.lay.dira_w, L + nd.aux, a.lay.dira_b, hseg(nd.layers, 0), Seg{1, xaux, P.kaux, nd.aux, L}, 2);
-        dgrad(dzg, half, D.w_dira, pp[0], -1, false);                                      // dF (xyz_encoding_final has no activation)
-        wgrad(pp[0], L, a.lay.final_w, L, a.lay.final_b, hseg(nd.layers - 1, 0), none, 1);
-        dgrad(pp[0], L, D.w_final, pp[1], nd.layers - 1, true);                            // dZ of the last trunk layer
-        int cur = 1;
-        for (int l = nd.layers - 1; l >= 0; --l) {
-            const Seg pe{1, 0, P.kpe, nd.in_xyz, 0};
-            const int k_in = a.lay.kin[l];
-            if (l == 0) wgrad(pp[cur], L, a.lay.w[l], k_in, a.lay.b[l], pe, none, 1);
-            else if ((nd.skip_mask >> l) & 1) wgrad(pp[cur], L, a.lay.w[l], k_in, a.lay.b[l], pe, hseg(l - 1, nd.in_xyz), 2);
-            else wgrad(pp[cur], L, a.lay.w[l], k_in, a.lay.b[l], hseg(l - 1, 0), none, 1);
-            if (l >= 1) {
-                dgrad(pp[cur], L, D.w_layer[l], pp[cur ^ 1], l - 1, false);               // dZ_{l-1} = mask(dZ_l W_l[:, hidden])
-                cur ^= 1;
-            }
-        }
-        // ---- sigma / rgb heads
+    // ---- sigma / rgb head weight gradients of the tiles t0 .. t0 + nt - 1, whose head-gradient blocks gf32 holds
+    auto heads = [&](int64_t t0, int64_t nt) -> int {
         HeadsArgs H{};
         H.act = tape.act;
         H.gf32 = gf32;
@@ -1148,158 +1044,180 @@ static int layer_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, const Laye
         if (nd.rgb_dim == 3) tc_heads_wgrad_kernel<3><<<hgrid, 256, 0, st>>>(H);
         else tc_heads_wgrad_kernel<MN_TC_RGB_MAX><<<hgrid, 256, 0, st>>>(H);
         MN_LAUNCH_CHECK(ctx);
-    }
-    if (nd.app_in_dira) {
-        tc_emb_grad_kernel<<<dim3((unsigned)nd.app_count, (unsigned)a.n_sub), 64, 0, st>>>(emb_sum, a.packed_bwd, a.blay.total, a.blay.dira_e, half, nd.app,
-                                                                                          nd.app_count, a.gw, a.lay.total, a.lay.emb);
-        MN_LAUNCH_CHECK(ctx);
-    }
-    mn_prof_end(ctx, st);
-    return MN_OK;
-}
-
-int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_tiles128, const TrainTcTape& tape, void* ws, size_t ws_bytes,
-                         cudaStream_t st) {
-    TcArgs A{};
-    const NetDims& nd = a.nd;
-    LayerPlan LP;
-    const bool layer = build_layer_plan(nd, &LP);
-    if (!m->train_tc_ok || (layer ? !m->tc_dgrad : !build_dgrad_plan(nd, &A.plan)))
-        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: unsupported network shape");
-    if (n_tiles128 <= 0) return MN_OK;
-    if (!ws || ws_bytes < mn_train_tc_backward_workspace(m, n_tiles128)) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_train_tc_backward: workspace too small");
-    if (layer) return layer_backward(ctx, m, a, LP, n_tiles128, tape, ws, st);
-    const size_t act_tile = mn_train_tc_act_tile_bytes(m);
-    char* wp = (char*)(((uintptr_t)ws + 255) / 256 * 256);
-    unsigned char* dz = (unsigned char*)wp;               wp += mn_align((size_t)n_tiles128 * act_tile);
-    float* gf32 = (float*)wp;                             wp += train_tc_head_grad_bytes(m, n_tiles128);
-    float* emb_sum = (float*)wp;                          wp += mn_align(train_tc_emb_floats(m) * sizeof(float) + 256) - 256;
-    float* scale = (float*)wp;
-    unsigned* maxbits = reinterpret_cast<unsigned*>(scale + 1);     // max |grad_out| (float bits), inside the same 256 bytes
-    if (train_tc_emb_floats(m)) MN_CUDA(ctx, cudaMemsetAsync(emb_sum, 0, train_tc_emb_floats(m) * sizeof(float), st));
-    MN_CUDA(ctx, cudaMemsetAsync(maxbits, 0, sizeof(unsigned), st));
-
-    mn_prof_begin(ctx, st);   // bench.py --mode train: the whole backward of the MLP stage timed as one span
-    // ---- gradient scale (power of two) from the upstream gradient
-    {
-        const int64_t n = a.grad_rows * a.out_cols;
-        const int64_t blocks = std::min<int64_t>(std::max<int64_t>(mn_cdiv(n, (int64_t)256 * 16), 1), (int64_t)ctx->sm_count * 4);
-        tc_grad_absmax_kernel<<<(unsigned)blocks, 256, 0, st>>>(a.grad_out, n, maxbits);
-        MN_LAUNCH_CHECK(ctx);
-        tc_grad_scale_kernel<<<1, 32, 0, st>>>(maxbits, scale);
-        MN_LAUNCH_CHECK(ctx);
-    }
-
-    // ---- data gradients
-    A.m = MlpArgs{};
-    A.m.nd = nd;
-    A.m.slot_row = a.slot_row;
-    A.m.slot_w = a.slot_w;
-    A.m.counters = a.counters;
-    A.m.n_sub = a.n_sub;
-    A.m.fixed_sub = a.fixed_sub;
-    A.m.B = a.B;
-    A.m.out_cols = a.out_cols;
-    A.wpack = (const unsigned char*)m->tc_dgrad;
-    A.n_tiles_cap = n_tiles128;
-    A.tape_act = tape.act;
-    A.tape_f32 = tape.f32;
-    A.tape_dz = dz;
-    A.tape_gf32 = gf32;
-    A.grad_out = a.grad_out;
-    A.emb_sum = nd.app_in_dira ? emb_sum : nullptr;
-    A.scale = scale;
-    A.act_tile_bytes = (int64_t)act_tile;
-    A.layers = nd.layers;
-    {
-        const int rc = wg_launch<PP_DGRAD, false, false>(ctx, A, n_tiles128, st);
-        if (rc != MN_OK) return rc;
-    }
-
-    // ---- weight gradients: one item per (Linear input segment, 128-channel output half)
-    WgArgs W{};
-    const int L = nd.L;
-    auto img = [&](int i) { return (int)mn_tc_img_off(i, L); };
-    TcPlan F;
-    build_plan(nd, &F);
-    int ni = 0;
-    auto item = [&](int dz_img, int half, int x_region, int x_off, int n, int n_real, int w_off, int k_in, int in0, int b_off) {
-        WgItem& it = W.item[ni++];
-        it.dz_off = img(dz_img) + half * 16 * (kTileM * 16);
-        it.x_region = x_region;
-        it.x_off = x_off;
-        it.n = n;
-        it.n_real = n_real;
-        it.w_off = w_off + half * 128 * k_in + in0;
-        it.k_in = k_in;
-        it.b_off = b_off >= 0 ? b_off + half * 128 : -1;
+        return MN_OK;
     };
-    for (int i = 0; i < nd.layers; ++i) {
-        const bool skip = i > 0 && ((nd.skip_mask >> i) & 1);
-        const int k_in = a.lay.kin[i];
-        for (int h = 0; h < L / 128; ++h) {
-            if (i == 0) item(i, h, 1, 0, F.kpe, nd.in_xyz, a.lay.w[i], k_in, 0, a.lay.b[i]);
-            else if (skip) {
-                item(i, h, 1, 0, F.kpe, nd.in_xyz, a.lay.w[i], k_in, 0, a.lay.b[i]);                       // cat[PE, h]: PE columns first
-                item(i, h, 0, img(i - 1), L, L, a.lay.w[i], k_in, nd.in_xyz, -1);
-            } else item(i, h, 0, img(i - 1), L, L, a.lay.w[i], k_in, 0, a.lay.b[i]);
+    int rc;
+
+    if (net.engine == TC_FUSED) {
+        // ---- data gradients: one launch of the fused kernel over the transposed images
+        TcArgs A{};
+        A.m = mm;
+        A.plan = net.D;
+        A.wpack = (const unsigned char*)m->tc_dgrad;
+        A.n_tiles_cap = n_tiles128;
+        A.tape_act = tape.act;
+        A.tape_f32 = tape.f32;
+        A.tape_dz = dz;
+        A.tape_gf32 = gf32;
+        A.grad_out = a.grad_out;
+        A.emb_sum = nd.app_in_dira ? emb_sum : nullptr;
+        A.scale = scale;
+        A.act_tile_bytes = act_tile;
+        A.layers = nd.layers;
+        if ((rc = wg_launch<PP_DGRAD, false, false>(ctx, A, n_tiles128, st))) return rc;
+
+        // ---- weight gradients: one item per (input segment, 128-channel output half) of every Linear but rgb
+        WgArgs W{};
+        int ni = 0;
+        for (int j = 0; j < lin.n - 1; ++j)
+            for (int h = 0; h < lin.l[j].n / 128; ++h)
+                for (int s = 0; s < lin.l[j].nseg; ++s) {
+                    if (ni == kWgMaxItems) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: too many weight-gradient items");
+                    WgItem& it = W.item[ni++];
+                    it = wg_item(lin, j, s, L);
+                    it.dz_off = (int)mn_tc_img_off(j, L) + h * 16 * (kTileM * 16);
+                    it.w_off += h * 128 * it.k_in;
+                    if (it.b_off >= 0) it.b_off += h * 128;
+                }
+        W.n_items = ni;
+        W.act = tape.act;
+        W.dz = dz;
+        W.xreg = tape.xreg;
+        W.act_tile_bytes = act_tile;
+        W.x_tile_bytes = (int64_t)net.F.x_tile_bytes;
+        W.counters = a.counters;
+        W.n_tiles = tiles_used;
+        W.fixed_sub = a.fixed_sub;
+        W.gw = a.gw;
+        W.sub_stride = a.lay.total;
+        W.scale = scale;
+        // chunks: enough CTAs to fill the machine about three times over (each streams its tiles once; results are fp32 atomics)
+        int64_t chunks = mn_cdiv((int64_t)ctx->sm_count * 3, (int64_t)ni * n_sub);
+        if (chunks < 1) chunks = 1;
+        int64_t chunk_tiles = mn_cdiv(mn_cdiv(tiles_used, n_sub), chunks);
+        if (chunk_tiles < 8) chunk_tiles = 8;
+        W.chunk_tiles = (int)chunk_tiles;
+        const unsigned gx = (unsigned)mn_cdiv(tiles_used, chunk_tiles);
+        MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
+        tc_wgrad_kernel<false><<<dim3(gx, (unsigned)ni, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
+        MN_LAUNCH_CHECK(ctx);
+        if ((rc = heads(0, tiles_used))) return rc;
+    } else {
+        // ---- layer engine, one tile group at a time: head stage -> per Linear (output side first) the weight gradient from its dZ
+        // image, then the data-gradient GEMM that produces the next dZ in the other ping-pong buffer; then the sigma / rgb head
+        // weight gradients.  dZ of Linear j is consumed by its weight gradient before the buffer is overwritten.
+        const LayerPlan& P = net.P;
+        const TcPlan& D = net.D;
+        const int rows = mn_tc_g32_rows(nd.rgb_dim);
+        const int64_t gt = WS.head_tiles;
+        unsigned char* dzg = dz;                              // dZ of dir_a_encoding (L/2 columns)
+        unsigned char* pp[2];
+        pp[0] = dzg + mn_align((size_t)gt * half * kTileM * 2);
+        pp[1] = pp[0] + mn_align((size_t)gt * L * kTileM * 2);
+        constexpr int gemm_sm = LgShape<false>::smem;
+        MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
+        MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
+
+        for (int64_t t0 = 0; t0 < tiles_used; t0 += gt) {
+            const int64_t nt = tiles_used - t0 < gt ? tiles_used - t0 : gt;
+            const unsigned char* rec = tape.act + t0 * act_tile;
+            // ---- head stage
+            {
+                LdArgs H{};
+                H.m = mm;
+                H.tile0 = t0;
+                H.grad_out = a.grad_out;
+                H.tape_f32 = tape.f32;
+                H.g = rec + mn_tc_img_off(nd.layers + 1, L);
+                H.g_tile_bytes = act_tile;
+                H.wpack = (const unsigned char*)m->tc_packed;
+                H.sub_bytes = (int64_t)m->tc_sub_bytes;
+                H.f32_off = P.plane_bytes * 2;
+                H.rgb_w_off = P.rgb_w_off;
+                H.half = half;
+                H.gf32 = gf32;
+                H.dz = dzg;
+                H.emb_sum = nd.app_in_dira ? emb_sum : nullptr;
+                H.scale = scale;
+                tc_layer_head_dgrad_kernel<<<(unsigned)nt, kTileM, 0, st>>>(H);
+                MN_LAUNCH_CHECK(ctx);
+            }
+            // ---- weight gradient of Linear j from its output gradient images dzj
+            auto wgrad = [&](const unsigned char* dzj, int j) -> int {
+                const TcLinear& l = lin.l[j];
+                WgArgs W{};
+                for (int s = 0; s < l.nseg; ++s) {
+                    W.item[s] = wg_item(lin, j, s, L);
+                    W.n_chunks[s] = (l.seg[s].k + 255) / 256;
+                }
+                const int items = (l.n / 128) * (W.n_chunks[0] + W.n_chunks[1]);
+                W.n_items = items;
+                W.act = tape.act;
+                W.dz = dzj;
+                W.xreg = tape.xreg;
+                W.act_tile_bytes = act_tile;
+                W.x_tile_bytes = P.x_tile_bytes;
+                W.dz_tile_bytes = (int64_t)l.n * kTileM * 2;
+                W.t_min = t0;
+                W.t_max = t0 + nt;
+                W.counters = a.counters;
+                W.n_tiles = tiles_used;
+                W.fixed_sub = a.fixed_sub;
+                W.gw = a.gw;
+                W.sub_stride = a.lay.total;
+                W.scale = scale;
+                // about one CTA per SM: every CTA flushes its 128 x 256 accumulators with fp32 atomics once
+                const int64_t chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count, (int64_t)items));
+                W.chunk_tiles = (int)mn_cdiv(nt, chunks);
+                tc_wgrad_kernel<true><<<dim3((unsigned)chunks, (unsigned)items, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
+                MN_LAUNCH_CHECK(ctx);
+                return MN_OK;
+            };
+            // ---- data-gradient GEMM g: dz_out = [mask](dz_in W^T) [+ S dsigma x sigma_w]
+            auto dgrad = [&](const unsigned char* dz_in, const TcGemm& g, unsigned char* dz_out) -> int {
+                LgArgs G{};
+                G.m = mm;
+                G.tile0 = t0;
+                G.n_tiles = nt;
+                G.wpack = (const unsigned char*)m->tc_dgrad;
+                G.sub_bytes = (int64_t)D.sub_bytes;
+                G.w_off = g.w_off;
+                G.k_tot = g.k[0];
+                G.n_blk = L / kLgBlock;
+                G.n_out = L;
+                G.bias_off = 0;
+                G.f32_off = D.f32_off;
+                G.nseg = 1;
+                G.a[0] = dz_in;
+                G.ak[0] = g.k[0];
+                G.a_tile_bytes[0] = (int64_t)g.k[0] * kTileM * 2;
+                G.out = dz_out;
+                G.out_tile_bytes = (int64_t)L * kTileM * 2;
+                G.mask = g.epi != EPI_D_LINEAR ? rec + mn_tc_img_off(g.img, L) : nullptr;     // xyz_encoding_final has no activation
+                G.mask_tile_bytes = act_tile;
+                G.dsig = g.epi == EPI_D_MASK_SIGMA ? gf32 + MN_TC_G32_SIGMA * kTileM : nullptr;
+                G.dsig_tile_floats = (int64_t)rows * kTileM;
+                G.scale = scale;
+                const int64_t items = nt * G.n_blk;
+                const unsigned grid = (unsigned)(items < ctx->sm_count ? items : ctx->sm_count);
+                tc_layer_gemm_kernel<false, true><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
+                MN_LAUNCH_CHECK(ctx);
+                return MN_OK;
+            };
+            // Linear j (dir_a_encoding down to trunk layer 0): weight gradient, then data-gradient GEMM lin.n - 2 - j gives dZ of j - 1
+            const unsigned char* dzj = dzg;
+            for (int j = lin.n - 2, nxt = 0; j >= 0; --j, nxt ^= 1) {
+                if ((rc = wgrad(dzj, j))) return rc;
+                if (j == 0) break;
+                if ((rc = dgrad(dzj, D.g[lin.n - 2 - j], pp[nxt]))) return rc;
+                dzj = pp[nxt];
+            }
+            if ((rc = heads(t0, nt))) return rc;
         }
     }
-    for (int h = 0; h < L / 128; ++h) item(nd.layers, h, 0, img(nd.layers - 1), L, L, a.lay.final_w, L, 0, a.lay.final_b);
-    // dir_a_encoding: L/2 = 128 output channels (one half); input = cat[final (L), dir PE + embedding (aux)]
-    item(nd.layers + 1, 0, 0, img(nd.layers), L, L, a.lay.dira_w, L + nd.aux, 0, a.lay.dira_b);
-    item(nd.layers + 1, 0, 1, (F.kpe / 8) * (kTileM * 16), F.kaux, nd.aux, a.lay.dira_w, L + nd.aux, L, -1);
-    if (ni > kWgMaxItems) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: too many weight-gradient items");
-    W.n_items = ni;
-    W.act = tape.act;
-    W.dz = dz;
-    W.xreg = tape.xreg;
-    W.act_tile_bytes = (int64_t)act_tile;
-    W.x_tile_bytes = (int64_t)F.x_tile_bytes;
-    // tiles the forward pass really wrote: all bucketed tiles when routed, ceil(rows / 128) otherwise
-    const int64_t tiles_used = a.counters ? n_tiles128 : mn_cdiv(a.B, (int64_t)kTileM);
-    W.counters = a.counters;
-    W.n_tiles = tiles_used;
-    W.fixed_sub = a.fixed_sub;
-    W.gw = a.gw;
-    W.sub_stride = a.lay.total;
-    W.scale = scale;
-    // chunks: enough CTAs to fill the machine about three times over (each streams its tiles once; results are fp32 atomics)
-    const int n_sub = a.counters ? a.n_sub : 1;
-    int64_t chunks = mn_cdiv((int64_t)ctx->sm_count * 3, (int64_t)ni * n_sub);
-    if (chunks < 1) chunks = 1;
-    int64_t chunk_tiles = mn_cdiv(mn_cdiv(tiles_used, n_sub), chunks);
-    if (chunk_tiles < 8) chunk_tiles = 8;
-    W.chunk_tiles = (int)chunk_tiles;
-    const unsigned gx = (unsigned)mn_cdiv(tiles_used, chunk_tiles);
-    const int wg_smem = 2 * kWgStageBytes + 6144 + 256;
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
-    tc_wgrad_kernel<false><<<dim3(gx, (unsigned)ni, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
-    MN_LAUNCH_CHECK(ctx);
-
-    // ---- sigma / rgb heads and the appearance embedding
-    HeadsArgs H{};
-    H.act = tape.act;
-    H.gf32 = gf32;
-    H.act_tile_bytes = (int64_t)act_tile;
-    H.L = L;
-    H.layers = nd.layers;
-    H.rgb_dim = nd.rgb_dim;
-    H.counters = a.counters;
-    H.n_tiles = tiles_used;
-    H.t_min = 0;
-    H.t_max = tiles_used;
-    H.fixed_sub = a.fixed_sub;
-    H.chunk_tiles = 16;
-    H.gw = a.gw;
-    H.sub_stride = a.lay.total;
-    H.sigma_w = a.lay.sigma_w; H.sigma_b = a.lay.sigma_b; H.rgb_w = a.lay.rgb_w; H.rgb_b = a.lay.rgb_b;
-    const dim3 hgrid((unsigned)mn_cdiv(tiles_used, 16), (unsigned)n_sub);
-    if (nd.rgb_dim == 3) tc_heads_wgrad_kernel<3><<<hgrid, 256, 0, st>>>(H);
-    else tc_heads_wgrad_kernel<MN_TC_RGB_MAX><<<hgrid, 256, 0, st>>>(H);
-    MN_LAUNCH_CHECK(ctx);
+    // ---- appearance embedding
     if (nd.app_in_dira) {
-        tc_emb_grad_kernel<<<dim3((unsigned)nd.app_count, (unsigned)a.n_sub), 64, 0, st>>>(emb_sum, a.packed_bwd, a.blay.total, a.blay.dira_e, L / 2, nd.app,
+        tc_emb_grad_kernel<<<dim3((unsigned)nd.app_count, (unsigned)a.n_sub), 64, 0, st>>>(emb_sum, a.packed_bwd, a.blay.total, a.blay.dira_e, half, nd.app,
                                                                                           nd.app_count, a.gw, a.lay.total, a.lay.emb);
         MN_LAUNCH_CHECK(ctx);
     }

@@ -17,35 +17,10 @@
 //                                             a chunk of tiles and flushed with fp32 atomics.
 //   heads     tc_heads_wgrad_kernel (sigma / rgb Linears: 1 and rgb_dim output channels - CUDA cores), tc_emb_grad_kernel
 //             (appearance embedding: W_e^T times the per-image sums of dZ_dira rows collected by the dgrad head stage).
+//
+// Host side (mn_mlp_tc.cu): build_dgrad_plan (the data-gradient chain and the layout of the transposed images,
+// packed by tc_dgrad_ready / tc_pack_dgrad), mn_mlp_tc_launch_train and mn_train_tc_backward, shared with the layer-GEMM engine.
 #pragma once
-
-// ---- data-gradient plan: GEMM chain of the backward pass as a TcPlan (all operands from the activation buffer).  Heads:
-// rgb_dim 3 (sigmoid colour) or a raw SH head of up to MN_TC_RGB_MAX coefficients (rgb_dim > 3 implies pos_dir_dim == 0).
-inline bool build_dgrad_plan(const NetDims& nd, TcPlan* p) {
-    if (nd.L != 256 || !nd.has_dir_a || nd.rgb_dim < 3 || nd.rgb_dim > MN_TC_RGB_MAX || nd.affine || nd.layers < 2 || nd.layers > 10)
-        return false;
-    TcPlan& P = *p;
-    P = TcPlan{};
-    P.L = nd.L;
-    P.bstride = 256;
-    int woff = 0, ng = 0;
-    auto add = [&](int n, int k, int img, int epi) {
-        TcGemm& g = P.g[ng++];
-        g.n = n; g.nseg = 1; g.src[0] = SRC_H; g.k[0] = k; g.src[1] = 0; g.k[1] = 0;
-        g.w_off = woff; g.img = img; g.epi = epi;
-        woff += k * n * 2;
-    };
-    add(nd.L, nd.L / 2, nd.layers, EPI_D_LINEAR);                    // dF  = dZ_dira  W_dira[:, 0:L]      -> image 'final'
-    add(nd.L, nd.L, nd.layers - 1, EPI_D_MASK_SIGMA);                // dH  = dF W_final + dsigma w_sigma  -> dZ of the last trunk layer
-    for (int l = nd.layers - 1; l >= 1; --l) add(nd.L, nd.L, l - 1, EPI_D_MASK);   // dZ_{l-1} = mask(dZ_l W_l[:, hidden part])
-    P.n_gemm = P.n_trunk = ng;
-    P.plane_bytes = woff;
-    P.sigma_w_off = 0;
-    P.f32_floats = nd.L + nd.rgb_dim * (nd.L / 2);                   // [sigma_w (L)][rgb_w [rgb_dim][L/2]]
-    P.f32_off = woff;
-    P.sub_bytes = (int)mn_align((size_t)woff + (size_t)P.f32_floats * 4, 256);
-    return true;
-}
 
 // max |g| over the upstream gradient, spread over the machine (an SH head's grad_out has 28 columns per row): every block
 // folds a grid-stride share and publishes its maximum with an integer atomicMax on *maxbits (zeroed by the caller; the bit

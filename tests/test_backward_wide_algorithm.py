@@ -1,5 +1,5 @@
 """CPU-only: the tensor-core training arithmetic of the layer-GEMM path (layer_dim 768..2048; csrc/mn_layer_gemm.cuh,
-csrc/mn_mlp_tc.cu::layer_backward) restated with plain tensor algebra at L = 768 (and 2048 for one net) and checked against the oracle's autograd.
+csrc/mn_mlp_tc.cu::mn_train_tc_backward) restated with plain tensor algebra at L = 768 (and 2048 for one net) and checked against the oracle's autograd.
 
 The restatement follows the kernels step by step: fp16 operands with fp32 accumulation in every GEMM, fp16 activations on
 the tape, the head stage in fp32, gradient images S x dZ rounded to fp16 with S = 2^(10 - ceil(log2 max|grad_out|)), the

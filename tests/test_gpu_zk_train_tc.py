@@ -119,7 +119,9 @@ def test_unsupported_shapes_fall_back_to_fp32():
 
 def test_render_rays_training_step_on_tensor_cores():
     """render_rays in train() mode (jitter, density noise, random resampling) with MSE loss: the tc_f16 step's loss equals the
-    fp32 step's to fp16 accuracy, gradients agree to the 16-bit bounds, and 30 Adam steps reduce the loss."""
+    fp32 step's to fp16 accuracy, gradients agree to the 16-bit bounds, and 30 Adam steps reduce the loss.  One more step's
+    gradients then match the fp32 step's at the updated weights, which holds only if the transposed weight images of the
+    data-gradient chain (packed by the first recording call) were repacked after every opt.step()."""
     m = M()
     net, _, rays, idx, opts, _, _ = C.render_case('c2_mega8_blend')
     hp = Namespace(**vars(opts))
@@ -152,5 +154,10 @@ def test_render_rays_training_step_on_tensor_cores():
             opt.step()
             losses.append(float(loss.detach()))
         assert losses[-1] < 0.9 * losses[0], losses
+        l_tc, g_tc = step(pn, 'tc_f16', 12)
+        l_32, g_32 = step(pn, 'fp32', 12)
+        assert abs(l_tc - l_32) <= 2e-3 * abs(l_32), (l_tc, l_32)
+        l2, worst = compare(g_tc, g_32, 'render_rays train step after 30 Adam steps')
+        print(f'after Adam: loss tc {l_tc:.6f} fp32 {l_32:.6f}; grads rel L2 {l2:.2e}, worst {worst}')
     finally:
         m.set_train_precision('fp32')
