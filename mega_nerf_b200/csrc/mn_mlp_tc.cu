@@ -277,7 +277,7 @@ TcNet tc_net(const mn_model& m) {
     if (build_layer_plan(nd, t.lin, &t.P)) t.engine = TC_LAYER;
     else if (build_plan(nd, t.lin, &t.F)) t.engine = TC_FUSED;
     t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers >= 2 &&
-              (t.engine == TC_LAYER || (t.engine == TC_FUSED && nd.L == 256 && nd.layers <= 10));
+              (t.engine == TC_LAYER || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 10));
     if (t.train) build_dgrad_plan(nd, t.lin, &t.D);
     return t;
 }
@@ -932,7 +932,8 @@ int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n
     rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st);
     if (rc) return rc;
     mn_prof_begin(ctx, st);
-    rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
+    if (A.plan.L > 256) rc = wg_launch<PP_TRAIN_FWD, false, true>(ctx, A, n_tiles128, st);
+    else rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
     mn_prof_end(ctx, st);
     return rc;
 }
@@ -1046,10 +1047,50 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         MN_LAUNCH_CHECK(ctx);
         return MN_OK;
     };
+    // ---- weight gradient of Linear j over the tiles t0 .. t0 + nt - 1 from its output gradient images (dzj: those of tile t0,
+    // dz_tile_bytes apart), one tc_wgrad_kernel<true> launch: item = (128-channel output half, X chunk of <= 256 columns)
+    auto wgrad = [&](const unsigned char* dzj, int64_t dz_tile_bytes, int j, int64_t t0, int64_t nt) -> int {
+        const TcLinear& l = lin.l[j];
+        WgArgs W{};
+        for (int s = 0; s < l.nseg; ++s) {
+            W.item[s] = wg_item(lin, j, s, L);
+            W.n_chunks[s] = (l.seg[s].k + 255) / 256;
+        }
+        const int items = (l.n / 128) * (W.n_chunks[0] + W.n_chunks[1]);
+        W.n_items = items;
+        W.act = tape.act;
+        W.dz = dzj;
+        W.xreg = tape.xreg;
+        W.act_tile_bytes = act_tile;
+        W.x_tile_bytes = net.engine == TC_LAYER ? net.P.x_tile_bytes : net.F.x_tile_bytes;
+        W.dz_tile_bytes = dz_tile_bytes;
+        W.t_min = t0;
+        W.t_max = t0 + nt;
+        W.counters = a.counters;
+        W.n_tiles = tiles_used;
+        W.fixed_sub = a.fixed_sub;
+        W.gw = a.gw;
+        W.sub_stride = a.lay.total;
+        W.scale = scale;
+        int64_t chunks;
+        if (net.engine == TC_LAYER) {
+            // about one CTA per SM: every CTA flushes its 128 x 256 accumulators with fp32 atomics once
+            chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count, (int64_t)items));
+            W.chunk_tiles = (int)mn_cdiv(nt, chunks);
+        } else {
+            // every tile of the call, shared by n_sub sub-modules: about three CTAs per SM, as the fused engine's per-segment items
+            chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count * 3, (int64_t)items * n_sub));
+            W.chunk_tiles = (int)std::max<int64_t>(8, mn_cdiv(mn_cdiv(nt, (int64_t)n_sub), chunks));
+            chunks = mn_cdiv(nt, (int64_t)W.chunk_tiles);
+        }
+        tc_wgrad_kernel<true><<<dim3((unsigned)chunks, (unsigned)items, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
+        MN_LAUNCH_CHECK(ctx);
+        return MN_OK;
+    };
     int rc;
 
     if (net.engine == TC_FUSED) {
-        // ---- data gradients: one launch of the fused kernel over the transposed images
+        // ---- data gradients: one launch of the fused kernel over the transposed images (512 wide: every GEMM in two N = 256 chunks)
         TcArgs A{};
         A.m = mm;
         A.plan = net.D;
@@ -1064,43 +1105,52 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         A.scale = scale;
         A.act_tile_bytes = act_tile;
         A.layers = nd.layers;
-        if ((rc = wg_launch<PP_DGRAD, false, false>(ctx, A, n_tiles128, st))) return rc;
+        if (L > 256) {
+            if ((rc = wg_launch<PP_DGRAD, false, true>(ctx, A, n_tiles128, st))) return rc;
+            // ---- weight gradients, 512 wide: one per-Linear launch each, straight from the gradient records.  The per-segment
+            // items below would come to ~80 (each trunk segment is 512 columns wide), more than kWgMaxItems.
+            MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
+            for (int j = lin.n - 2; j >= 0; --j)
+                if ((rc = wgrad(dz + mn_tc_img_off(j, L), act_tile, j, 0, tiles_used))) return rc;
+        } else {
+            if ((rc = wg_launch<PP_DGRAD, false, false>(ctx, A, n_tiles128, st))) return rc;
 
-        // ---- weight gradients: one item per (input segment, 128-channel output half) of every Linear but rgb
-        WgArgs W{};
-        int ni = 0;
-        for (int j = 0; j < lin.n - 1; ++j)
-            for (int h = 0; h < lin.l[j].n / 128; ++h)
-                for (int s = 0; s < lin.l[j].nseg; ++s) {
-                    if (ni == kWgMaxItems) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: too many weight-gradient items");
-                    WgItem& it = W.item[ni++];
-                    it = wg_item(lin, j, s, L);
-                    it.dz_off = (int)mn_tc_img_off(j, L) + h * 16 * (kTileM * 16);
-                    it.w_off += h * 128 * it.k_in;
-                    if (it.b_off >= 0) it.b_off += h * 128;
-                }
-        W.n_items = ni;
-        W.act = tape.act;
-        W.dz = dz;
-        W.xreg = tape.xreg;
-        W.act_tile_bytes = act_tile;
-        W.x_tile_bytes = (int64_t)net.F.x_tile_bytes;
-        W.counters = a.counters;
-        W.n_tiles = tiles_used;
-        W.fixed_sub = a.fixed_sub;
-        W.gw = a.gw;
-        W.sub_stride = a.lay.total;
-        W.scale = scale;
-        // chunks: enough CTAs to fill the machine about three times over (each streams its tiles once; results are fp32 atomics)
-        int64_t chunks = mn_cdiv((int64_t)ctx->sm_count * 3, (int64_t)ni * n_sub);
-        if (chunks < 1) chunks = 1;
-        int64_t chunk_tiles = mn_cdiv(mn_cdiv(tiles_used, n_sub), chunks);
-        if (chunk_tiles < 8) chunk_tiles = 8;
-        W.chunk_tiles = (int)chunk_tiles;
-        const unsigned gx = (unsigned)mn_cdiv(tiles_used, chunk_tiles);
-        MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
-        tc_wgrad_kernel<false><<<dim3(gx, (unsigned)ni, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
-        MN_LAUNCH_CHECK(ctx);
+            // ---- weight gradients: one item per (input segment, 128-channel output half) of every Linear but rgb
+            WgArgs W{};
+            int ni = 0;
+            for (int j = 0; j < lin.n - 1; ++j)
+                for (int h = 0; h < lin.l[j].n / 128; ++h)
+                    for (int s = 0; s < lin.l[j].nseg; ++s) {
+                        if (ni == kWgMaxItems) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: too many weight-gradient items");
+                        WgItem& it = W.item[ni++];
+                        it = wg_item(lin, j, s, L);
+                        it.dz_off = (int)mn_tc_img_off(j, L) + h * 16 * (kTileM * 16);
+                        it.w_off += h * 128 * it.k_in;
+                        if (it.b_off >= 0) it.b_off += h * 128;
+                    }
+            W.n_items = ni;
+            W.act = tape.act;
+            W.dz = dz;
+            W.xreg = tape.xreg;
+            W.act_tile_bytes = act_tile;
+            W.x_tile_bytes = (int64_t)net.F.x_tile_bytes;
+            W.counters = a.counters;
+            W.n_tiles = tiles_used;
+            W.fixed_sub = a.fixed_sub;
+            W.gw = a.gw;
+            W.sub_stride = a.lay.total;
+            W.scale = scale;
+            // chunks: enough CTAs to fill the machine about three times over (each streams its tiles once; results are fp32 atomics)
+            int64_t chunks = mn_cdiv((int64_t)ctx->sm_count * 3, (int64_t)ni * n_sub);
+            if (chunks < 1) chunks = 1;
+            int64_t chunk_tiles = mn_cdiv(mn_cdiv(tiles_used, n_sub), chunks);
+            if (chunk_tiles < 8) chunk_tiles = 8;
+            W.chunk_tiles = (int)chunk_tiles;
+            const unsigned gx = (unsigned)mn_cdiv(tiles_used, chunk_tiles);
+            MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
+            tc_wgrad_kernel<false><<<dim3(gx, (unsigned)ni, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
+            MN_LAUNCH_CHECK(ctx);
+        }
         if ((rc = heads(0, tiles_used))) return rc;
     } else {
         // ---- layer engine, one tile group at a time: head stage -> per Linear (output side first) the weight gradient from its dZ
@@ -1142,37 +1192,6 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
                 tc_layer_head_dgrad_kernel<<<(unsigned)nt, kTileM, 0, st>>>(H);
                 MN_LAUNCH_CHECK(ctx);
             }
-            // ---- weight gradient of Linear j from its output gradient images dzj
-            auto wgrad = [&](const unsigned char* dzj, int j) -> int {
-                const TcLinear& l = lin.l[j];
-                WgArgs W{};
-                for (int s = 0; s < l.nseg; ++s) {
-                    W.item[s] = wg_item(lin, j, s, L);
-                    W.n_chunks[s] = (l.seg[s].k + 255) / 256;
-                }
-                const int items = (l.n / 128) * (W.n_chunks[0] + W.n_chunks[1]);
-                W.n_items = items;
-                W.act = tape.act;
-                W.dz = dzj;
-                W.xreg = tape.xreg;
-                W.act_tile_bytes = act_tile;
-                W.x_tile_bytes = P.x_tile_bytes;
-                W.dz_tile_bytes = (int64_t)l.n * kTileM * 2;
-                W.t_min = t0;
-                W.t_max = t0 + nt;
-                W.counters = a.counters;
-                W.n_tiles = tiles_used;
-                W.fixed_sub = a.fixed_sub;
-                W.gw = a.gw;
-                W.sub_stride = a.lay.total;
-                W.scale = scale;
-                // about one CTA per SM: every CTA flushes its 128 x 256 accumulators with fp32 atomics once
-                const int64_t chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count, (int64_t)items));
-                W.chunk_tiles = (int)mn_cdiv(nt, chunks);
-                tc_wgrad_kernel<true><<<dim3((unsigned)chunks, (unsigned)items, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
-                MN_LAUNCH_CHECK(ctx);
-                return MN_OK;
-            };
             // ---- data-gradient GEMM g: dz_out = [mask](dz_in W^T) [+ S dsigma x sigma_w]
             auto dgrad = [&](const unsigned char* dz_in, const TcGemm& g, unsigned char* dz_out) -> int {
                 LgArgs G{};
@@ -1207,7 +1226,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
             // Linear j (dir_a_encoding down to trunk layer 0): weight gradient, then data-gradient GEMM lin.n - 2 - j gives dZ of j - 1
             const unsigned char* dzj = dzg;
             for (int j = lin.n - 2, nxt = 0; j >= 0; --j, nxt ^= 1) {
-                if ((rc = wgrad(dzj, j))) return rc;
+                if ((rc = wgrad(dzj, (int64_t)lin.l[j].n * kTileM * 2, j, t0, nt))) return rc;
                 if (j == 0) break;
                 if ((rc = dgrad(dzj, D.g[lin.n - 2 - j], pp[nxt]))) return rc;
                 dzj = pp[nxt];

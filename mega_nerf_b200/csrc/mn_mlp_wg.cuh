@@ -446,20 +446,24 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                         if (kMode == PP_DGRAD) {
                             // dH = accumulator (scaled by S) [+ S dsigma x w_sigma] -> ReLU mask from the activation tape -> fp16 ->
                             // next A operand + gradient tape.  The mask image and the target image coincide: dZ_l = dH_l where H_l > 0.
+                            // N = 512 (kWide): chunk 0 (columns 0..255) goes to the gradient tape at once, but its fp16 pairs wait in
+                            // `held` until chunk 1's MMAs have read the old dZ from Hs.
                             const size_t ioff = (size_t)tile * A.act_tile_bytes + mn_tc_img_off(gm.img, L);
                             const unsigned char* mimg = A.tape_act + ioff;
                             unsigned char* dimg = A.tape_dz + ioff;
                             const float dsa = DSIG[ra], dsb = DSIG[rb];
+                            const int c0 = kWide ? cb : 0;
+                            const bool dhold = kWide && nch == 2 && ch == 0;
                             constexpr int JB = NM / 8 < 8 ? NM / 8 : 8;        // column groups whose loads are issued together
 #pragma unroll
                             for (int j0 = 0; j0 < NM / 8; j0 += JB) {
                             __half2 mka[JB], mkb[JB];
 #pragma unroll
                             for (int jj = 0; jj < JB; ++jj) {
-                                const int c = 8 * (j0 + jj) + 2 * q4;
+                                const int c = c0 + 8 * (j0 + jj) + 2 * q4;
                                 const size_t po = (size_t)(c >> 3) * (kTileM * 16) + (size_t)ra * 16 + (size_t)(c & 7) * 2;
                                 mka[jj] = mkb[jj] = __float2half2_rn(1.0f);
-                                if (gm.epi != EPI_D_LINEAR && 8 * (j0 + jj) < gm.n) {
+                                if (gm.epi != EPI_D_LINEAR && c0 + 8 * (j0 + jj) < gm.n) {
                                     mka[jj] = *reinterpret_cast<const __half2*>(mimg + po);
                                     mkb[jj] = *reinterpret_cast<const __half2*>(mimg + po + 128);
                                 }
@@ -467,8 +471,8 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
 #pragma unroll
                             for (int jj = 0; jj < JB; ++jj) {
                                 const int j = j0 + jj;
-                                const int c = 8 * j + 2 * q4;
-                                if (8 * j >= gm.n) continue;
+                                const int c = c0 + 8 * j + 2 * q4;
+                                if (c0 + 8 * j >= gm.n) continue;
                                 float a0 = acc[4 * j], a1 = acc[4 * j + 1], b0 = acc[4 * j + 2], b1 = acc[4 * j + 3];
                                 if (gm.epi == EPI_D_MASK_SIGMA) {                                      // F32[0..L) = sigma weights
                                     const float2 s = *reinterpret_cast<const float2*>(F32 + c);
@@ -484,11 +488,25 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                                     if (!(__high2float(mb) > 0.0f)) b1 = 0.0f;
                                 }
                                 const uint32_t ha = pack_h2(a0, a1), hb = pack_h2(b0, b1);
-                                st_shared_u32(Hs + po, ha);
-                                st_shared_u32(Hs + po + 128, hb);
+                                if (dhold) {
+                                    held[(2 * j) % (NM / 4)] = ha;
+                                    held[(2 * j + 1) % (NM / 4)] = hb;
+                                } else {
+                                    st_shared_u32(Hs + po, ha);
+                                    st_shared_u32(Hs + po + 128, hb);
+                                }
                                 *reinterpret_cast<uint32_t*>(dimg + po) = ha;
                                 *reinterpret_cast<uint32_t*>(dimg + po + 128) = hb;
                             }
+                            }
+                            if (kWide && nch == 2 && ch == 1) {
+#pragma unroll
+                                for (int j = 0; j < NM / 8; ++j) {
+                                    const int c = 8 * j + 2 * q4;
+                                    const size_t po = (size_t)(c >> 3) * (kTileM * 16) + (size_t)ra * 16 + (size_t)(c & 7) * 2;
+                                    st_shared_u32(Hs + po, held[(2 * j) % (NM / 4)]);
+                                    st_shared_u32(Hs + po + 128, held[(2 * j + 1) % (NM / 4)]);
+                                }
                             }
                             fence_proxy_async();
                             wg_sync();

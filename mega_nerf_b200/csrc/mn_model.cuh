@@ -168,7 +168,7 @@ struct TrainTcTape {
 };
 // the shapes whose recording calls run on the tensor cores (tc_net in mn_mlp_tc.cu; mn_model_train_tc_supported)
 #define MN_TC_TRAIN_COVERAGE                                                                                                    \
-    "tensor-core training covers layer_dim 256 or 768..2048 (a multiple of 256) with a direction / appearance head, rgb_dim 3 " \
+    "tensor-core training covers layer_dim 256, 512 or 768..2048 (a multiple of 256) with a direction / appearance head, rgb_dim 3 " \
     "or a raw SH head (rgb_dim <= 32), no affine appearance; use train precision 'fp32'"
 size_t mn_train_tc_x_tile_bytes(const mn_model* m);
 size_t mn_train_tc_act_tile_bytes(const mn_model* m);

@@ -49,7 +49,8 @@ def set_train_precision(name: str) -> None:
     'fp32'   CUDA-core kernels - the parity mode (gradients equal the reference's fp32 autograd to its own noise level);
     'tc_f16' tensor cores: fp16 operands, fp32 accumulation, gradient images scaled by a power of two - what the reference
              does on a GPU under autocast + GradScaler (runner.py:243-274).  The tensor-core training kernels cover
-             layer_dim 256 and 768..2048 (a multiple of 256: the nerf, npp and mega-nerf-dense configs' 2048) with a
+             layer_dim 256, 512 (up to 10 trunk layers) and 768..2048 (a multiple of 256: the nerf, npp and
+             mega-nerf-dense configs' 2048) with a
              direction / appearance head and either an rgb head (rgb_dim 3) or a raw SH head (rgb_dim <= 32, e.g.
              sh_deg 2); other networks (other widths, affine appearance, heads without dir_a_encoding) silently use the
              fp32 kernels, which refuse layer_dim > 512 - NativeModel.train_on_tensor_cores() tells which."""
