@@ -149,6 +149,7 @@ bool build_plan(const NetDims& nd, const TcLinears& T, TcPlan* p) {
     P.sigma_w_off = T.n * P.bstride;
     P.f32_floats = T.n * P.bstride + nd.L + 4;
     P.f32_off = woff * 2;
+    P.sub_bytes = (int)mn_align((size_t)woff * 2 + (size_t)P.f32_floats * 4, 256);
     P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
     return true;
 }
@@ -174,6 +175,7 @@ struct LayerPlan {
     int L, kpe, kaux;
     int plane_bytes;     // bytes of all weight images of one sub-module (one precision plane)
     int f32_floats;      // fp32 block: biases, sigma_w [L], sigma_b (4), rgb_w [rgb_dim][rgb_in], rgb_b (32)
+    int sub_bytes;       // total bytes per sub-module: planes (hi, lo) + fp32 block
     int sigma_w_off, rgb_w_off, rgb_b_off;
     int rgb_in, h_last;  // rgb head input width; buffer of the last trunk activations
     int rgb_src;         // buffer the rgb head reads
@@ -224,6 +226,7 @@ bool build_layer_plan(const NetDims& nd, const TcLinears& T, LayerPlan* p) {
     P.rgb_w_off = foff + nd.L + 4;
     P.rgb_b_off = P.rgb_w_off + nd.rgb_dim * nd.rgb_in;
     P.f32_floats = P.rgb_b_off + MN_TC_RGB_MAX;
+    P.sub_bytes = (int)mn_align((size_t)woff * 2 + (size_t)P.f32_floats * 4, 256);
     P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
     return true;
 }
@@ -677,7 +680,6 @@ static int tc_dgrad_ready(mn_ctx* ctx, mn_model* m, const TcNet& net, cudaStream
     const size_t bytes = (size_t)net.D.sub_bytes * m->d.n_sub;
     MN_CUDA(ctx, cudaMalloc(&m->tc_dgrad, bytes));
     MN_CUDA(ctx, cudaMemsetAsync(m->tc_dgrad, 0, bytes, st));
-    m->tc_dgrad_sub_bytes = (size_t)net.D.sub_bytes;
     for (int s = 0; s < m->d.n_sub; ++s) tc_pack_dgrad(ctx, m, s, net);
     return mn_pack_flush(ctx, st);
 }
@@ -697,11 +699,10 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
     const TcPlan& F = net.F;
     const LayerPlan& P = net.P;
     const int plane = fused ? F.plane_bytes : P.plane_bytes, n_gemm = fused ? F.n_gemm : P.n_gemm;
-    const size_t sub_bytes = mn_align((size_t)plane * 2 + (size_t)(fused ? F.f32_floats : P.f32_floats) * 4, 256);
+    const size_t sub_bytes = (size_t)(fused ? F.sub_bytes : P.sub_bytes);
     if (!m->tc_packed) {
         MN_CUDA(ctx, cudaMalloc(&m->tc_packed, sub_bytes * m->d.n_sub));
         MN_CUDA(ctx, cudaMemsetAsync(m->tc_packed, 0, sub_bytes * m->d.n_sub, st));
-        m->tc_sub_bytes = sub_bytes;
     }
     unsigned char* base = (unsigned char*)m->tc_packed + (size_t)sub * sub_bytes;
     const float* Pk = m->packed + (size_t)sub * m->lay.total;
@@ -753,7 +754,6 @@ static int tc_encode(mn_ctx* ctx, const mn_model* m, const MlpArgs& a, const TcP
 static TcArgs tc_forward_args(const mn_model* m, const TcPlan& F, const MlpArgs& a, int64_t n_tiles128) {
     TcArgs A{};
     A.plan = F;
-    A.plan.sub_bytes = (int)m->tc_sub_bytes;
     A.m = a;
     A.wpack = (const unsigned char*)m->tc_packed;
     A.n_tiles_cap = n_tiles128;
@@ -801,7 +801,7 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
             G.tile0 = t0;
             G.n_tiles = nt;
             G.wpack = (const unsigned char*)m->tc_packed;
-            G.sub_bytes = (int64_t)m->tc_sub_bytes;
+            G.sub_bytes = P.sub_bytes;
             G.w_lo = P.plane_bytes;
             G.w_off = g.w_off;
             G.k_tot = g.k[0] + (g.nseg > 1 ? g.k[1] : 0);
@@ -843,7 +843,7 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
         H.m = a;
         H.tile0 = t0;
         H.wpack = (const unsigned char*)m->tc_packed;
-        H.sub_bytes = (int64_t)m->tc_sub_bytes;
+        H.sub_bytes = P.sub_bytes;
         H.f32_off = P.plane_bytes * 2;
         H.sigma_w_off = P.sigma_w_off;
         H.rgb_w_off = P.rgb_w_off;
@@ -964,20 +964,26 @@ size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
     return tc_bwd_workspace(m, tc_net(*m), n_tiles128).total;
 }
 
-// Weight-gradient item of input segment s of Linear j for its output channels 0..127 and the segment's first columns: X is
-// image j - 1 of the activation record (SRC_H) or a segment of the feature tile.
-static WgItem wg_item(const TcLinears& T, int j, int s, int L) {
+// Weight-gradient entry of Linear j: per input segment, the item of output channels 0..127 and the segment's first X chunk.  X is
+// image j - 1 of the activation record (SRC_H) or a segment of the feature tile; dZ lies at dz_off inside a tile's gradient images.
+static WgLinear wg_linear(const TcLinears& T, int j, int L, int dz_off) {
     const TcLinear& l = T.l[j];
-    const TcSeg& g = l.seg[s];
-    WgItem it{};
-    it.x_region = g.src == SRC_H ? 0 : 1;
-    it.x_off = g.src == SRC_H ? (int)mn_tc_img_off(j - 1, L) : g.src == SRC_XAUX ? (T.kpe / 8) * (kTileM * 16) : 0;
-    it.n = g.k;
-    it.n_real = g.k_real;
-    it.w_off = l.w + g.in0;
-    it.k_in = l.kin;
-    it.b_off = s == 0 ? l.b : -1;      // the first segment owns the bias
-    return it;
+    WgLinear w{};
+    for (int s = 0; s < l.nseg; ++s) {
+        const TcSeg& g = l.seg[s];
+        WgItem& it = w.seg[s];
+        it.dz_off = dz_off;
+        it.x_region = g.src == SRC_H ? 0 : 1;
+        it.x_off = g.src == SRC_H ? (int)mn_tc_img_off(j - 1, L) : g.src == SRC_XAUX ? (T.kpe / 8) * (kTileM * 16) : 0;
+        it.n = g.k;
+        it.n_real = g.k_real;
+        it.w_off = l.w + g.in0;
+        it.k_in = l.kin;
+        it.b_off = s == 0 ? l.b : -1;      // the first segment owns the bias
+        w.n_chunks[s] = (g.k + 255) / 256;
+    }
+    w.n_items = (l.n / 128) * (w.n_chunks[0] + w.n_chunks[1]);
+    return w;
 }
 
 int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_tiles128, const TrainTcTape& tape, void* ws, size_t ws_bytes,
@@ -1023,6 +1029,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     // tiles the forward pass really wrote: all bucketed tiles when routed, ceil(rows / 128) otherwise
     const int64_t tiles_used = a.counters ? n_tiles128 : mn_cdiv(a.B, (int64_t)kTileM);
     const int wg_smem = 2 * kWgStageBytes + 6144 + 256;
+    MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
     // ---- sigma / rgb head weight gradients of the tiles t0 .. t0 + nt - 1, whose head-gradient blocks gf32 holds
     auto heads = [&](int64_t t0, int64_t nt) -> int {
         HeadsArgs H{};
@@ -1047,43 +1054,43 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         MN_LAUNCH_CHECK(ctx);
         return MN_OK;
     };
-    // ---- weight gradient of Linear j over the tiles t0 .. t0 + nt - 1 from its output gradient images (dzj: those of tile t0,
-    // dz_tile_bytes apart), one tc_wgrad_kernel<true> launch: item = (128-channel output half, X chunk of <= 256 columns)
-    auto wgrad = [&](const unsigned char* dzj, int64_t dz_tile_bytes, int j, int64_t t0, int64_t nt) -> int {
-        const TcLinear& l = lin.l[j];
+    // ---- weight gradients of Linears j0 .. j1 - 1 over the tiles t0 .. t0 + nt - 1, one tc_wgrad_kernel launch.  dzt: the gradient
+    // images of tile t0, dz_tile_bytes apart: the fused engine's gradient records (Linear j's image at mn_tc_img_off(j)) or the
+    // layer engine's group buffer of its one Linear.
+    auto wgrad = [&](int j0, int j1, const unsigned char* dzt, int64_t dz_tile_bytes, int64_t t0, int64_t nt) -> int {
+        const bool fused = net.engine == TC_FUSED;
         WgArgs W{};
-        for (int s = 0; s < l.nseg; ++s) {
-            W.item[s] = wg_item(lin, j, s, L);
-            W.n_chunks[s] = (l.seg[s].k + 255) / 256;
+        int64_t items = 0;
+        for (int j = j0; j < j1; ++j) {
+            W.lin[j - j0] = wg_linear(lin, j, L, fused ? (int)mn_tc_img_off(j, L) : 0);
+            items += W.lin[j - j0].n_items;
         }
-        const int items = (l.n / 128) * (W.n_chunks[0] + W.n_chunks[1]);
-        W.n_items = items;
         W.act = tape.act;
-        W.dz = dzj;
+        W.dz = dzt;
         W.xreg = tape.xreg;
         W.act_tile_bytes = act_tile;
-        W.x_tile_bytes = net.engine == TC_LAYER ? net.P.x_tile_bytes : net.F.x_tile_bytes;
+        W.x_tile_bytes = fused ? net.F.x_tile_bytes : net.P.x_tile_bytes;
         W.dz_tile_bytes = dz_tile_bytes;
         W.t_min = t0;
         W.t_max = t0 + nt;
         W.counters = a.counters;
-        W.n_tiles = tiles_used;
         W.fixed_sub = a.fixed_sub;
         W.gw = a.gw;
         W.sub_stride = a.lay.total;
         W.scale = scale;
         int64_t chunks;
-        if (net.engine == TC_LAYER) {
-            // about one CTA per SM: every CTA flushes its 128 x 256 accumulators with fp32 atomics once
-            chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count, (int64_t)items));
-            W.chunk_tiles = (int)mn_cdiv(nt, chunks);
-        } else {
-            // every tile of the call, shared by n_sub sub-modules: about three CTAs per SM, as the fused engine's per-segment items
-            chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count * 3, (int64_t)items * n_sub));
+        if (fused) {
+            // every tile of the call, shared by n_sub sub-modules: enough CTAs to fill the machine about three times over (each
+            // streams its tiles once; results are fp32 atomics)
+            chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count * 3, items * n_sub));
             W.chunk_tiles = (int)std::max<int64_t>(8, mn_cdiv(mn_cdiv(nt, (int64_t)n_sub), chunks));
             chunks = mn_cdiv(nt, (int64_t)W.chunk_tiles);
+        } else {
+            // about one CTA per SM: every CTA flushes its 128 x 256 accumulators with fp32 atomics once
+            chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count, items));
+            W.chunk_tiles = (int)mn_cdiv(nt, chunks);
         }
-        tc_wgrad_kernel<true><<<dim3((unsigned)chunks, (unsigned)items, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
+        tc_wgrad_kernel<<<dim3((unsigned)chunks, (unsigned)items, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
         MN_LAUNCH_CHECK(ctx);
         return MN_OK;
     };
@@ -1105,52 +1112,15 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         A.scale = scale;
         A.act_tile_bytes = act_tile;
         A.layers = nd.layers;
+        rc = L > 256 ? wg_launch<PP_DGRAD, false, true>(ctx, A, n_tiles128, st) : wg_launch<PP_DGRAD, false, false>(ctx, A, n_tiles128, st);
+        if (rc) return rc;
+        // ---- weight gradients of every Linear but rgb, straight from the gradient records.  512 wide: one launch per Linear.  A
+        // single launch would be faster, but over ~80 items the chunk policy gives each CTA more tiles to sum in its accumulators,
+        // which moves the gradients by more than fp32 atomic order does (DESIGN §8).
         if (L > 256) {
-            if ((rc = wg_launch<PP_DGRAD, false, true>(ctx, A, n_tiles128, st))) return rc;
-            // ---- weight gradients, 512 wide: one per-Linear launch each, straight from the gradient records.  The per-segment
-            // items below would come to ~80 (each trunk segment is 512 columns wide), more than kWgMaxItems.
-            MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
             for (int j = lin.n - 2; j >= 0; --j)
-                if ((rc = wgrad(dz + mn_tc_img_off(j, L), act_tile, j, 0, tiles_used))) return rc;
-        } else {
-            if ((rc = wg_launch<PP_DGRAD, false, false>(ctx, A, n_tiles128, st))) return rc;
-
-            // ---- weight gradients: one item per (input segment, 128-channel output half) of every Linear but rgb
-            WgArgs W{};
-            int ni = 0;
-            for (int j = 0; j < lin.n - 1; ++j)
-                for (int h = 0; h < lin.l[j].n / 128; ++h)
-                    for (int s = 0; s < lin.l[j].nseg; ++s) {
-                        if (ni == kWgMaxItems) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: too many weight-gradient items");
-                        WgItem& it = W.item[ni++];
-                        it = wg_item(lin, j, s, L);
-                        it.dz_off = (int)mn_tc_img_off(j, L) + h * 16 * (kTileM * 16);
-                        it.w_off += h * 128 * it.k_in;
-                        if (it.b_off >= 0) it.b_off += h * 128;
-                    }
-            W.n_items = ni;
-            W.act = tape.act;
-            W.dz = dz;
-            W.xreg = tape.xreg;
-            W.act_tile_bytes = act_tile;
-            W.x_tile_bytes = (int64_t)net.F.x_tile_bytes;
-            W.counters = a.counters;
-            W.n_tiles = tiles_used;
-            W.fixed_sub = a.fixed_sub;
-            W.gw = a.gw;
-            W.sub_stride = a.lay.total;
-            W.scale = scale;
-            // chunks: enough CTAs to fill the machine about three times over (each streams its tiles once; results are fp32 atomics)
-            int64_t chunks = mn_cdiv((int64_t)ctx->sm_count * 3, (int64_t)ni * n_sub);
-            if (chunks < 1) chunks = 1;
-            int64_t chunk_tiles = mn_cdiv(mn_cdiv(tiles_used, n_sub), chunks);
-            if (chunk_tiles < 8) chunk_tiles = 8;
-            W.chunk_tiles = (int)chunk_tiles;
-            const unsigned gx = (unsigned)mn_cdiv(tiles_used, chunk_tiles);
-            MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
-            tc_wgrad_kernel<false><<<dim3(gx, (unsigned)ni, (unsigned)n_sub), kWgThreads, wg_smem, st>>>(W);
-            MN_LAUNCH_CHECK(ctx);
-        }
+                if ((rc = wgrad(j, j + 1, dz, act_tile, 0, tiles_used))) return rc;
+        } else if ((rc = wgrad(0, lin.n - 1, dz, act_tile, 0, tiles_used))) return rc;
         if ((rc = heads(0, tiles_used))) return rc;
     } else {
         // ---- layer engine, one tile group at a time: head stage -> per Linear (output side first) the weight gradient from its dZ
@@ -1166,7 +1136,6 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         pp[1] = pp[0] + mn_align((size_t)gt * L * kTileM * 2);
         constexpr int gemm_sm = LgShape<false>::smem;
         MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
-        MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
 
         for (int64_t t0 = 0; t0 < tiles_used; t0 += gt) {
             const int64_t nt = tiles_used - t0 < gt ? tiles_used - t0 : gt;
@@ -1181,7 +1150,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
                 H.g = rec + mn_tc_img_off(nd.layers + 1, L);
                 H.g_tile_bytes = act_tile;
                 H.wpack = (const unsigned char*)m->tc_packed;
-                H.sub_bytes = (int64_t)m->tc_sub_bytes;
+                H.sub_bytes = P.sub_bytes;
                 H.f32_off = P.plane_bytes * 2;
                 H.rgb_w_off = P.rgb_w_off;
                 H.half = half;
@@ -1226,7 +1195,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
             // Linear j (dir_a_encoding down to trunk layer 0): weight gradient, then data-gradient GEMM lin.n - 2 - j gives dZ of j - 1
             const unsigned char* dzj = dzg;
             for (int j = lin.n - 2, nxt = 0; j >= 0; --j, nxt ^= 1) {
-                if ((rc = wgrad(dzj, (int64_t)lin.l[j].n * kTileM * 2, j, t0, nt))) return rc;
+                if ((rc = wgrad(j, j + 1, dzj, (int64_t)lin.l[j].n * kTileM * 2, t0, nt))) return rc;
                 if (j == 0) break;
                 if ((rc = dgrad(dzj, D.g[lin.n - 2 - j], pp[nxt]))) return rc;
                 dzj = pp[nxt];

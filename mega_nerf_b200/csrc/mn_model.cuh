@@ -60,11 +60,9 @@ struct mn_model {
     int max_multiplicity = 0;         // slot capacity per row for blended routing
     // tensor-core packed weights (fp16 hi / lo images), see mn_mlp_tc.cu
     void* tc_packed = nullptr;
-    size_t tc_sub_bytes = 0;
     int tc_ready = 0;
     // transposed fp16 weight images of the tensor-core data-gradient chain (mn_train_tc.cuh); NULL if the shape is not covered
     void* tc_dgrad = nullptr;
-    size_t tc_dgrad_sub_bytes = 0;
     int train_tc_ok = 0;
 };
 

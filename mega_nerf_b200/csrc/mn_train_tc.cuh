@@ -14,7 +14,10 @@
 //                                             between 8-slot groups, SBO = 2048 B between 8-column groups), M = 128 output
 //                                             channels per CTA (64 per consumer warpgroup), N <= 256 input channels + a 16-column
 //                                             all-ones operand whose product is the bias gradient, accumulated in registers over
-//                                             a chunk of tiles and flushed with fp32 atomics.
+//                                             a chunk of tiles and flushed with fp32 atomics.  A launch takes a list of Linears
+//                                             (WgLinear) and decodes its work item (Linear, output half, X chunk) from blockIdx.y:
+//                                             at 256 the fused engine covers every Linear but rgb in one launch; at 512 it makes
+//                                             one launch per Linear, and the layer engine one per Linear and tile group.
 //   heads     tc_heads_wgrad_kernel (sigma / rgb Linears: 1 and rgb_dim output channels - CUDA cores), tc_emb_grad_kernel
 //             (appearance embedding: W_e^T times the per-image sums of dZ_dira rows collected by the dgrad head stage).
 //
@@ -51,7 +54,7 @@ __global__ void tc_grad_scale_kernel(const unsigned* __restrict__ maxbits, float
 // weight gradients
 // ------------------------------------------------------------------------------------------------
 struct WgItem {
-    int dz_off;       // byte offset of the 128-column dZ half inside a tile's gradient record
+    int dz_off;       // byte offset of the 128-column dZ half inside a tile's gradient images
     int x_region;     // 0: activation record, 1: encoder (feature) tile
     int x_off;        // byte offset of the first X column group inside that record
     int n;            // MMA N = X columns (multiple of 16, <= 256)
@@ -60,20 +63,20 @@ struct WgItem {
     int k_in;         // row stride (in_features) of that weight matrix
     int b_off;        // float offset of bias[out0], or -1 when another item of the same layer owns the bias
 };
-constexpr int kWgMaxItems = 48;
+// One Linear of a launch: its work items are (128-channel output half, X chunk of <= 256 columns of an input segment)
+struct WgLinear {
+    WgItem seg[2];                  // input segment s for output channels 0..127 and the segment's first X chunk
+    int n_chunks[2];                // X chunks of each input segment (0: no second segment)
+    int n_items;                    // (out / 128) * (n_chunks[0] + n_chunks[1])
+};
 struct WgArgs {
-    WgItem item[kWgMaxItems];       // kLinear: item[s] = input segment s of one Linear for its first output half and X chunk
-    int n_items;
+    WgLinear lin[MN_MAX_LAYERS + 2];  // Linears of the launch (trunk, xyz_encoding_final, dir_a_encoding; never rgb), in order
     const unsigned char* act;       // activation records
-    const unsigned char* dz;        // gradient records (same layout); kLinear: gradient images of tile t_min onwards
+    const unsigned char* dz;        // gradient images of tile t_min onwards, dz_tile_bytes apart
     const unsigned char* xreg;      // encoder tiles
-    int64_t act_tile_bytes, x_tile_bytes;
-    // kLinear (layer-GEMM path, one tile group and one Linear per launch): item y = (output half, X chunk of <= 256 columns)
-    int n_chunks[2];                // X chunks of each input segment
-    int64_t dz_tile_bytes;          // tile stride of the gradient images
-    int64_t t_min, t_max;           // tiles of the group
-    const int* counters;            // routing counters saved by the forward pass, or NULL
-    int64_t n_tiles;                // counters == NULL: all tiles belong to fixed_sub
+    int64_t act_tile_bytes, x_tile_bytes, dz_tile_bytes;
+    int64_t t_min, t_max;           // tiles covered by the launch
+    const int* counters;            // routing counters saved by the forward pass, or NULL (all tiles belong to fixed_sub)
     int fixed_sub;
     int chunk_tiles;
     float* gw;                      // [n_sub][sub_stride] fp32
@@ -83,14 +86,18 @@ struct WgArgs {
 constexpr int kWgStageBytes = 96 * 1024;
 constexpr int kWgThreads = 384;     // warpgroup 0: producer thread; warpgroups 1-2: output channels 0-63 / 64-127 of the item
 
-// Work item y of a kLinear launch: output channels [128 mh, +128) x input columns [256 c, +256) of segment s.
-__device__ __forceinline__ WgItem wg_linear_item(const WgArgs& A, int y) {
-    const int per = A.n_chunks[0] + A.n_chunks[1];
+// Work item y of a launch: the Linear whose items span y, then output channels [128 mh, +128) x input columns [256 c, +256)
+// of its segment s.
+__device__ __forceinline__ WgItem wg_work_item(const WgArgs& A, int y) {
+    int li = 0;
+    while (y >= A.lin[li].n_items) y -= A.lin[li++].n_items;
+    const WgLinear& l = A.lin[li];
+    const int per = l.n_chunks[0] + l.n_chunks[1];
     const int mh = y / per;
     int c = y - mh * per;
-    const int s = c < A.n_chunks[0] ? 0 : 1;
-    if (s) c -= A.n_chunks[0];
-    WgItem it = A.item[s];
+    const int s = c < l.n_chunks[0] ? 0 : 1;
+    if (s) c -= l.n_chunks[0];
+    WgItem it = l.seg[s];
     it.dz_off += mh * 16 * (kTileM * 16);
     it.x_off += c * 32 * (kTileM * 16);
     it.n = min(256, it.n - 256 * c);
@@ -100,7 +107,6 @@ __device__ __forceinline__ WgItem wg_linear_item(const WgArgs& A, int y) {
     return it;
 }
 
-template <bool kLinear>
 __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A) {
     extern __shared__ __align__(1024) unsigned char smem[];
     unsigned char* ring = smem;                                   // 2 x 96 KiB: [dZ half 32 KiB][X <= 64 KiB]
@@ -108,17 +114,13 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
     uint64_t* bars = reinterpret_cast<uint64_t*>(ones + 6144);
     uint64_t* full = bars;        // [2]
     uint64_t* empty = bars + 2;   // [2], one arrival per consumer warpgroup
-    const WgItem it = kLinear ? wg_linear_item(A, blockIdx.y) : A.item[blockIdx.y];
+    const WgItem it = wg_work_item(A, blockIdx.y);
     int sub = A.fixed_sub;
-    int64_t t_lo = 0, t_hi = A.n_tiles;
+    int64_t t_lo = A.t_min, t_hi = A.t_max;
     if (A.counters) {
         sub = (int)blockIdx.z;
-        t_lo = A.counters[CNT_START + sub] / kTileM;
-        t_hi = A.counters[CNT_START + sub + 1] / kTileM;
-    }
-    if (kLinear) {
-        t_lo = max(t_lo, A.t_min);
-        t_hi = min(t_hi, A.t_max);
+        t_lo = max(t_lo, (int64_t)(A.counters[CNT_START + sub] / kTileM));
+        t_hi = min(t_hi, (int64_t)(A.counters[CNT_START + sub + 1] / kTileM));
     }
     const int64_t t_begin = t_lo + (int64_t)blockIdx.x * A.chunk_tiles;
     const int64_t t_end = min(t_hi, t_begin + (int64_t)A.chunk_tiles);
@@ -142,8 +144,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
             for (int64_t t = t_begin; t < t_end; ++t) {
                 mbar_wait(&empty[st], ph ^ 1);
                 mbar_expect_tx(&full[st], 32768u + xbytes);
-                const unsigned char* dzt = kLinear ? A.dz + (size_t)(t - A.t_min) * A.dz_tile_bytes : A.dz + (size_t)t * A.act_tile_bytes;
-                bulk_g2s(ring + (size_t)st * kWgStageBytes, dzt + it.dz_off, 32768u, &full[st]);
+                bulk_g2s(ring + (size_t)st * kWgStageBytes, A.dz + (size_t)(t - A.t_min) * A.dz_tile_bytes + it.dz_off, 32768u, &full[st]);
                 bulk_g2s(ring + (size_t)st * kWgStageBytes + 32768, xbase + (size_t)t * xstride + it.x_off, xbytes, &full[st]);
                 if (++st == 2) { st = 0; ph ^= 1; }
             }

@@ -22,7 +22,7 @@ import mega_nerf_b200 as M  # noqa: E402
 from mega_nerf_b200.synthetic import build_net  # noqa: E402
 
 DEV = torch.device('cuda:0')
-KERNELS = (r'tc_mlp_wg_kernel<\d, \w+, \w+>', r'tc_wgrad_kernel<\w+>', r'tc_heads_wgrad_kernel<\d+>', r'\btc_\w+_kernel',
+KERNELS = (r'tc_mlp_wg_kernel<\d, \w+, \w+>', r'\btc_wgrad_kernel\b', r'tc_heads_wgrad_kernel<\d+>', r'\btc_\w+_kernel',
            r'\bmn_\w+_kernel', r'\w+_kernel')
 
 
@@ -93,7 +93,7 @@ def main():
                total_kernel_ms=round(sum(per.values()), 3))
     mlp = 0.0
     for tag, key in (('train_fwd', 'tc_mlp_wg_kernel<1, false, true>'), ('dgrad', 'tc_mlp_wg_kernel<2, false, true>'),
-                     ('wgrad', 'tc_wgrad_kernel<true>')):
+                     ('wgrad', 'tc_wgrad_kernel')):
         ms = per.get(key)
         if ms:
             mlp += ms

@@ -169,7 +169,7 @@ def profile_step(out, n_rays, samples):
         if e.device_type != torch.autograd.DeviceType.CUDA:
             continue
         name = e.name
-        m = re.search(r'(tc_layer_gemm_kernel<\w+, \w+>|tc_wgrad_kernel<\w+>|tc_heads_wgrad_kernel<\d+>|\btc_\w+_kernel)', name)
+        m = re.search(r'(tc_layer_gemm_kernel<\w+, \w+>|tc_wgrad_kernel\b|tc_heads_wgrad_kernel<\d+>|\btc_\w+_kernel)', name)
         key = m.group(1) if m else name[:60]
         per[key] = per.get(key, 0.0) + e.time_range.elapsed_us() / 1e3
     rows = n_rays * (samples[0] + samples[0] + samples[1])          # coarse pass + fine pass (coarse and fine samples)
@@ -178,7 +178,7 @@ def profile_step(out, n_rays, samples):
                total_kernel_ms=round(sum(per.values()), 2))
     for tag, key, fl in (('forward_layer_gemm', 'tc_layer_gemm_kernel<false, false>', f_fwd),
                          ('dgrad_layer_gemm', 'tc_layer_gemm_kernel<false, true>', f_dgrad),
-                         ('wgrad', 'tc_wgrad_kernel<true>', f_wgrad)):
+                         ('wgrad', 'tc_wgrad_kernel', f_wgrad)):
         if key in per:
             res[f'{tag}_ms'] = round(per[key], 3)
             res[f'{tag}_tflops'] = round(rows * fl / (per[key] * 1e-3) / 1e12, 1)

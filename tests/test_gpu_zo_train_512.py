@@ -1,5 +1,5 @@
 """GPU: tensor-core training (`set_train_precision('tc_f16')`) of the 512-wide networks - BASELINE configs[3]'s 25 x 512
-sub-modules - on the fused engine (tc_mlp_wg_kernel<PP_TRAIN_FWD / PP_DGRAD, false, true>, per-Linear tc_wgrad_kernel<true>).
+sub-modules - on the fused engine (tc_mlp_wg_kernel<PP_TRAIN_FWD / PP_DGRAD, false, true>, tc_wgrad_kernel, one launch per Linear).
 
 As in tests/test_gpu_zk_train_tc.py the reference is the fp32 CUDA-core training path of the same library (which accepts 512
 and which tests/test_gpu_zc_backward.py pins to the reference's gradients), with the same 16-bit bounds: TC_L2 on the whole
