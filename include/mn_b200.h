@@ -228,6 +228,45 @@ int mn_render_rays(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* i
                    int sh_deg, int precision, float* rgb_out_d, float* depth_out_d, float* depth_var_out_d,
                    float* rgb_coarse_out_d, void* workspace_d, size_t workspace_bytes, void* stream);
 
+/* ---- the same with a background (NeRF++) network ------------------------ mega_nerf/rendering.py:15-173 ----
+ * render_rays(nerf, bg_nerf, ...) in eval mode: the sphere split of every ray (fg_far = max(exit of the ellipsoid
+ * sphere_center3 / sphere_radius3, near); a ray reaches the background iff far > fg_far), the background pass over those rays
+ * (compacted on the device in ascending ray order; half the coarse samples, fine_samples / 2 draws, points inside the
+ * inverted sphere, flipped two-pass render), the foreground pass (far clipped to fg_far, last delta fg_far) and the blend
+ * val + bg_val * bg_lambda.  No host sync: the background ray count stays on the device, every background kernel skips the
+ * rays past it, so the launch sequence depends on N only (CUDA-graph capturable) and the background work on the count.
+ * A camera outside the ellipsoid sets the status word: MN_ERR_SPHERE is returned by the next mn_check_status, the results
+ * of this call are then undefined.
+ *   fg / bg: models of the same kind (use_cascade) and head (sh_deg); image_indices_d required iff either has an appearance
+ *   embedding; sphere_radius3_d NULL = the unit sphere at the origin;
+ *   include_xyz_real / cluster_2d as for mn_points_outside (render.py:304-305);
+ *   z_steps_bg_d = torch.linspace(0,1,coarse_samples/2), u_fine_bg_d = torch.linspace(0,1,fine_samples/2), passed in like
+ *   z_steps_d / u_fine_d (SURVEY §8c: these values are not a subset of the longer vectors).
+ * mn_render_outputs: nullable device pointers named after the result keys of the final type (fine, coarse when
+ * fine_samples == 0) and of the coarse type under use_cascade with fine_samples > 0; rgb is required.  fg_* / bg_* are the
+ * two terms of the blend (get_bg_fg_rgb); bg_lambda* are computed either way. */
+typedef struct mn_render_outputs {
+    float* rgb;               /* [N,3] rgb_<final>                                   */
+    float* depth;             /* [N]   depth_<final>                                 */
+    float* depth_var;         /* [N]   depth_variance_<final> (foreground only)      */
+    float* bg_lambda;         /* [N]   bg_lambda_<final>                             */
+    float* fg_rgb;            /* [N,3] fg_rgb_<final>                                */
+    float* bg_rgb;            /* [N,3] bg_rgb_<final>                                */
+    float* fg_depth;          /* [N]   fg_depth_<final>                              */
+    float* bg_depth;          /* [N]   bg_depth_<final>                              */
+    float* rgb_coarse;        /* [N,3] rgb_coarse (use_cascade, fine_samples > 0)    */
+    float* bg_lambda_coarse;  /* [N]   bg_lambda_coarse                              */
+    float* fg_rgb_coarse;     /* [N,3] fg_rgb_coarse                                 */
+    float* bg_rgb_coarse;     /* [N,3] bg_rgb_coarse                                 */
+} mn_render_outputs;
+size_t mn_render_rays_bg_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                         int use_cascade, int sh_deg, int precision);
+int mn_render_rays_bg(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays_d, const float* image_indices_d, int64_t N,
+                      const float* sphere_center3_d, const float* sphere_radius3_d, int include_xyz_real, int cluster_2d,
+                      const float* z_steps_d, const float* z_steps_bg_d, int coarse_samples, const float* u_fine_d,
+                      const float* u_fine_bg_d, int fine_samples, int use_cascade, int sh_deg, int precision,
+                      const mn_render_outputs* out, void* workspace_d, size_t workspace_bytes, void* stream);
+
 /* Fused per-ray all-gather over peer memory (SURVEY.md §8e): stores this rank's (rgb, depth) rows [row0, row0+n) into
  * every buffer of peer_bufs[0..n_peers) - HOST array of device pointers to [n_total, 4] fp32 buffers, one per rank,
  * peer-mapped into this process (e.g. torch symmetric memory) - with 16-byte P2P stores.  Cross-rank ordering (nobody

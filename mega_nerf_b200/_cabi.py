@@ -44,6 +44,12 @@ class Rows(C.Structure):
                 ('dir_stride', C.c_int64), ('idx_d', C.c_void_p), ('samples_per_ray', C.c_int)]
 
 
+class RenderOutputs(C.Structure):
+    """mn_render_outputs: device pointers (or None) named after render_rays' result keys."""
+    _fields_ = [(k, C.c_void_p) for k in ('rgb', 'depth', 'depth_var', 'bg_lambda', 'fg_rgb', 'bg_rgb', 'fg_depth', 'bg_depth',
+                                          'rgb_coarse', 'bg_lambda_coarse', 'fg_rgb_coarse', 'bg_rgb_coarse')]
+
+
 # name -> (restype, argtypes); every symbol of include/mn_b200.h
 _P, _I, _L, _F, _Z = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_size_t
 SIGNATURES = {
@@ -80,6 +86,9 @@ SIGNATURES = {
     'mn_model_last_stats': (_I, [_P, _P, C.POINTER(_L), C.POINTER(_L), _P]),
     'mn_render_rays_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
     'mn_render_rays': (_I, [_P, _P, _P, _P, _L, _P, _I, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _Z, _P]),
+    'mn_render_rays_bg_workspace_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_bg': (_I, [_P, _P, _P, _P, _P, _L, _P, _P, _I, _I, _P, _P, _I, _P, _P, _I, _I, _I, _I,
+                               C.POINTER(RenderOutputs), _P, _Z, _P]),
     'mn_peer_gather_store': (_I, [_P, _P, _P, _L, _L, C.POINTER(C.c_void_p), _I, _P]),
     'mn_cluster_min_dist_ratios': (_I, [_P, _P, _L, _P, _I, _P, _I, _I, _F, _P, _P, _P]),
     # training (SURVEY.md §8f-1)

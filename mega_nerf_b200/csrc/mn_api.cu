@@ -437,10 +437,12 @@ static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, Ta
     return off;
 }
 
-// train_tc != 0: recording forward on the tensor cores (precision tc_f16) into the tensor-core tape regions
+// train_tc != 0: recording forward on the tensor cores (precision tc_f16) into the tensor-core tape regions.
+// live: the rows that hold data when their count lives on the device (inference only), see LiveRows.
 static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, int sigma_only,
                               const float* sigma_noise_d, int precision, float* out_d, void* workspace_d,
-                              size_t workspace_bytes, void* tape_d, size_t tape_bytes, void* stream, int train_tc = 0) {
+                              size_t workspace_bytes, void* tape_d, size_t tape_bytes, void* stream, int train_tc = 0,
+                              LiveRows live = LiveRows{}) {
     if (!ctx || !m || !rows || B < 0) return MN_ERR_INVALID;
     const mn_model_desc& d = m->d;
     const NetDims& nd = m->nd;
@@ -503,6 +505,7 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
     a.sigma_noise = sigma_noise_d;
     a.out = out_d;
     a.out_cols = sigma_only ? 1 : nd.rgb_dim + 1;
+    a.live = live;
 
     const int64_t cap = slot_capacity(m, B);
     const size_t need = mn_model_workspace_bytes(m, B, precision);
@@ -532,7 +535,7 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
             slot_row = T.slot_row;
             slot_w = T.slot_w;
         }
-        if ((rc = mn_route_build(ctx, m, src, B, cap, slot_row, slot_w, row_slots, route_scratch, st))) return rc;
+        if ((rc = mn_route_build(ctx, m, src, B, live, cap, slot_row, slot_w, row_slots, route_scratch, st))) return rc;
         if (tape_d)
             MN_CUDA(ctx, cudaMemcpyAsync(T.counters, m->counters_d, CNT_TOTAL * sizeof(int), cudaMemcpyDeviceToDevice, st));
         a.slot_row = slot_row;
@@ -549,7 +552,7 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
     const int64_t n_tiles = cap / MN_TILE;
     if (tape_d && train_tc) {
         if ((rc = mn_mlp_tc_launch_train(ctx, m, a, n_tiles, T.tc, st))) return rc;
-        if (row_slots) return mn_route_combine(ctx, m, B, row_slots, slot_out, a.out_cols, out_d, st);
+        if (row_slots) return mn_route_combine(ctx, m, B, live, row_slots, slot_out, a.out_cols, out_d, st);
         return MN_OK;
     }
     if (tape_d) {
@@ -561,7 +564,7 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
     else
         rc = mn_mlp_tc_launch(ctx, m, a, n_tiles, precision, ws, workspace_bytes - (size_t)(ws - (char*)workspace_d), st);
     if (rc) return rc;
-    if (row_slots) return mn_route_combine(ctx, m, B, row_slots, slot_out, a.out_cols, out_d, st);
+    if (row_slots) return mn_route_combine(ctx, m, B, live, row_slots, slot_out, a.out_cols, out_d, st);
     return MN_OK;
 }
 
@@ -571,6 +574,16 @@ int mn_model_forward(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, i
     return model_forward_impl(ctx, m, rows, B, use_coarse, sigma_only, sigma_noise_d, precision, out_d, workspace_d,
                               workspace_bytes, nullptr, 0, stream);
 }
+
+}  // extern "C"
+
+int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,
+                          float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+    return model_forward_impl(ctx, m, rows, B, use_coarse, 0, nullptr, precision, out_d, workspace_d, workspace_bytes, nullptr, 0, st,
+                              0, live);
+}
+
+extern "C" {
 
 // ---- training (SURVEY.md §8f-1) --------------------------------------------------------------------
 size_t mn_model_tape_bytes(const mn_model* m, int64_t B) { return m ? tape_regions(m, B, false, nullptr) : 0; }

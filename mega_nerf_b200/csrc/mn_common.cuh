@@ -118,6 +118,14 @@ struct RowSrc {
     __device__ __forceinline__ float index(int64_t row) const { return idx[(row / div) * idx_stride]; }
 };
 
+// Rows of a call whose count lives on the device (the background pass of mn_render_rays_bg): `rays` points at a device count of
+// live rays, each `mul` rows; rows at or past mul * *rays are not read or written.  rays == NULL: every one of the call's rows.
+struct LiveRows {
+    const int* rays;
+    int mul;
+    __device__ __forceinline__ int64_t rows(int64_t all) const { return rays ? (int64_t)*rays * mul : all; }
+};
+
 // ------------------------------------------------------------------------------------------------
 // device helpers
 // ------------------------------------------------------------------------------------------------
@@ -136,3 +144,25 @@ __device__ __forceinline__ float mn_softplus_shifted(float x) {
 }
 
 __device__ __forceinline__ float mn_sigmoid(float x) { return 1.0f / (1.0f + expf(-x)); }
+
+__device__ __forceinline__ float mn_dot3(const float* a, const float* b) { return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2]; }
+
+// Depth at which ray [8] leaves the ellipsoid (center3, radius3; NULL radius = unit sphere at the origin), rendering.py:396-414.
+// *outside: the closest point of the ray's line lies on or outside the surface (the camera is not bounded by it).
+__device__ __forceinline__ float mn_sphere_far(const float* __restrict__ ray, const float* __restrict__ center,
+                                               const float* __restrict__ radius, bool* outside) {
+    float o[3], d[3];
+    for (int j = 0; j < 3; ++j) {
+        o[j] = ray[j];
+        d[j] = ray[3 + j];
+        if (radius) { o[j] = (o[j] - center[j]) / radius[j]; d[j] = d[j] / radius[j]; }
+    }
+    const float dd = mn_dot3(d, d);
+    const float d1 = -mn_dot3(d, o) / dd;
+    float p[3];
+    for (int j = 0; j < 3; ++j) p[j] = o[j] + d1 * d[j];
+    const float cosv = 1.0f / sqrtf(dd);
+    const float pn2 = mn_dot3(p, p);
+    *outside = pn2 >= 1.0f;
+    return d1 + sqrtf(1.0f - pn2) * cosv;
+}

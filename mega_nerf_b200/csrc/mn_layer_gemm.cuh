@@ -93,7 +93,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_layer_gemm_kernel(const L
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + kLgStages * S::stage_bytes);
     uint64_t* empty = full + kLgStages;          // one arrival per consumer warpgroup
 
-    const int64_t n_slots = A.m.counters ? A.m.counters[CNT_NSLOTS] : A.m.B;
+    const int64_t n_slots = A.m.n_slots();
     int64_t n_tiles = (n_slots + kTileM - 1) / kTileM - A.tile0;     // tiles at or past n_slots exit early
     if (n_tiles > A.n_tiles) n_tiles = A.n_tiles;
     const int64_t n_items = n_tiles > 0 ? n_tiles * A.n_blk : 0;
@@ -303,7 +303,7 @@ __device__ __forceinline__ void lg_load8(const unsigned char* img, int64_t lo, i
 __global__ void __launch_bounds__(kTileM) tc_layer_head_kernel(const LhArgs A) {
     const int t = threadIdx.x;
     const int64_t tile = A.tile0 + blockIdx.x;
-    const int64_t n_slots = A.m.counters ? A.m.counters[CNT_NSLOTS] : A.m.B;
+    const int64_t n_slots = A.m.n_slots();
     const int64_t slot = tile * kTileM + t;
     const int64_t row = A.m.row_of_slot(slot, n_slots);
     float* tf = A.tape_f32 ? A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + t : nullptr;
@@ -390,7 +390,7 @@ struct LdArgs {
 __global__ void __launch_bounds__(kTileM) tc_layer_head_dgrad_kernel(const LdArgs A) {
     const int t = threadIdx.x, lane = t & 31;
     const int64_t tile = A.tile0 + blockIdx.x;
-    const int64_t n_slots = A.m.counters ? A.m.counters[CNT_NSLOTS] : A.m.B;
+    const int64_t n_slots = A.m.n_slots();
     if (tile * kTileM >= n_slots) return;
     const int64_t slot = tile * kTileM + t;
     const int64_t row = A.m.row_of_slot(slot, n_slots);

@@ -80,7 +80,7 @@ __global__ void __launch_bounds__(256, 1) mlp_simt_kernel(const MlpArgs a) {
     const int tid = threadIdx.x;
 
     const int64_t slot0 = (int64_t)blockIdx.x * TM;
-    const int64_t n_slots = a.counters ? a.counters[CNT_NSLOTS] : a.B;
+    const int64_t n_slots = a.n_slots();
     if (slot0 >= n_slots) return;
     int sub = a.fixed_sub;
     if (a.counters) {

@@ -389,7 +389,7 @@ __global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int 
     const NetDims& nd = a.nd;
     const int t = threadIdx.x;
     const int64_t slot0 = tile * kTileM;
-    const int64_t n_slots = a.counters ? a.counters[CNT_NSLOTS] : a.B;
+    const int64_t n_slots = a.n_slots();
     if (slot0 >= n_slots) return;
     const int64_t row = a.row_of_slot(slot0 + t, n_slots);
     __half* lo_img = img + (size_t)ktot * kTileM;
@@ -479,7 +479,7 @@ __global__ void __launch_bounds__(kTileM) tc_encode_fast_kernel(const MlpArgs a,
     const int t = threadIdx.x;
     const int64_t tile = blockIdx.x;
     const int64_t slot0 = tile * kTileM;
-    const int64_t n_slots = a.counters ? a.counters[CNT_NSLOTS] : a.B;
+    const int64_t n_slots = a.n_slots();
     if (slot0 >= n_slots) return;
     const int64_t row = a.row_of_slot(slot0 + t, n_slots);
     uint4* out = reinterpret_cast<uint4*>(ximg + tile * (int64_t)(KPE + KAUX) * kTileM) + t;   // + chunk * kTileM

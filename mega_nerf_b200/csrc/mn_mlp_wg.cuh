@@ -271,7 +271,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
     uint64_t* xa_full = bars + 2 * kWgRingMax;
     uint64_t* xa_empty = xa_full + 1;
 
-    const int64_t n_slots = A.m.counters ? A.m.counters[CNT_NSLOTS] : A.m.B;
+    const int64_t n_slots = A.m.n_slots();
     const int64_t n_tiles = (n_slots + kTileM - 1) / kTileM;
     const int n_gemm = A.m.sigma_only ? P.n_trunk : P.n_gemm;
     constexpr int npass = kSplit ? 3 : 1;

@@ -94,7 +94,10 @@ struct MlpArgs {
     int scatter;              // 1: out index = row, 0: out index = slot
     float* tape;              // activation tape (training forward) or NULL
     TapeLayout tl;
+    LiveRows live;            // unrouted calls: rows that hold data (routed calls: the router skips the others)
 
+    // slots that hold rows: the routed slot count, else the live rows
+    __device__ __forceinline__ int64_t n_slots() const { return counters ? (int64_t)counters[CNT_NSLOTS] : live.rows(B); }
     // sub-module that owns the 128-slot tile `tile` (routed: the bucket it lies in)
     __device__ __forceinline__ int sub_of_tile(int64_t tile) const {
         int sub = fixed_sub;
@@ -135,11 +138,35 @@ struct BwdArgs {
     float* gw;                 // parameter gradients, [n_sub * lay.total], matrices stored [out][in] (nn.Linear layout)
 };
 
-int mn_route_build(mn_ctx* ctx, mn_model* m, const RowSrc& src, int64_t B, int64_t cap, int* slot_row, float* slot_w,
+int mn_route_build(mn_ctx* ctx, mn_model* m, const RowSrc& src, int64_t B, LiveRows live, int64_t cap, int* slot_row, float* slot_w,
                    int* row_slots, void* scratch, cudaStream_t st);
 size_t mn_route_scratch_bytes(const mn_model* m, int64_t B);   // per-row active-set masks (+ blend weights [K][B])
-int mn_route_combine(mn_ctx* ctx, mn_model* m, int64_t B, const int* row_slots, const float* slot_out, int out_cols,
+int mn_route_combine(mn_ctx* ctx, mn_model* m, int64_t B, LiveRows live, const int* row_slots, const float* slot_out, int out_cols,
                      float* out, cudaStream_t st);
+// mn_model_forward (inference) over the first live.rows(B) of B rows: the router, the encoders and the MLP tiles see only those,
+// the launch sequence is the one for B rows (csrc/mn_api.cu)
+int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,
+                          float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st);
+// ---- the one launch of each stage kernel (csrc/mn_sample.cu).  The public stage entry points validate their arguments and call
+// these; the background pass of mn_render_rays_bg calls them with its device ray count (`live`: rays at or past it are skipped,
+// grids stay sized for N) and the sample orders it needs: flip = reversed stratify output, flip_pts = points in reversed sample
+// order (depth_real in sample order), out_flip_d = a second, reversed copy of sort_cat's output.
+int mn_stage_stratify(mn_ctx* ctx, const float* z_d, int64_t z_row_stride, const float* rand_d, float perturb, int64_t N, int S, int flip,
+                      LiveRows live, float* z_out_d, cudaStream_t st);
+int mn_stage_points_outside(mn_ctx* ctx, const float* rays_d, const int64_t* ray_ids_d, const float* depth_d, const float* center3_d,
+                            const float* radius3_d, int64_t n, int S, int include_xyz_real, int cluster_2d, int flip_pts, LiveRows live,
+                            float* pts_out_d, float* depth_real_out_d, cudaStream_t st);
+int mn_stage_sample_pdf(mn_ctx* ctx, const float* z_coarse_d, const float* weights_d, int64_t w_stride, const float* cdf_d, const float* u_d,
+                        int64_t u_row_stride, int64_t N, int S, int F, LiveRows live, float* z_out_d, int64_t* inds_out_d,
+                        float* cdf_out_d, cudaStream_t st);
+int mn_stage_sort_cat(mn_ctx* ctx, const float* a_d, int na, const float* b_d, int nb, int64_t N, int descending, LiveRows live,
+                      float* out_d, float* out_flip_d, cudaStream_t st);
+int mn_stage_composite(mn_ctx* ctx, const float* raw_d, const float* z_d, const float* depth_real_d, int S, const float* raw2_d,
+                       const float* z2_d, const float* depth_real2_d, int S2, const float* last_delta_d, int64_t N, int flip,
+                       LiveRows live, float* weights_out_d, float* rgb_out_d, float* depth_out_d, float* depth_var_out_d,
+                       float* bg_lambda_out_d, cudaStream_t st);
+int mn_stage_sh_to_rgb(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
+                       int dir_div, int64_t B, int apply_sigmoid, LiveRows live, float* out_d, cudaStream_t st);
 int mn_mlp_simt_launch(mn_ctx* ctx, const MlpArgs& a, int64_t n_tiles128, cudaStream_t st);
 int mn_mlp_bwd_launch(mn_ctx* ctx, const BwdArgs& a, int64_t n_tiles128, cudaStream_t st);
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws,

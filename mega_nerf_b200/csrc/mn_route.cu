@@ -89,18 +89,21 @@ __device__ __forceinline__ uint64_t route_row(const float* d, int K, float margi
 
 // The routing decision (distances, threshold, normalised weights: ~2000 instructions per row with IEEE sqrt / div) is
 // made ONCE, here; the scatter pass re-reads the active-set mask [B] and the blend weights [K][B] (active entries only).
+// Rows at or past live.rows(B) (a call whose row count lives on the device) are not routed; cdist's direct path follows that
+// count, as it follows the batch size in the reference.
 template <int KMAX>
-__global__ void route_count_kernel(RowSrc src, int64_t B, const float* __restrict__ cent, int K, int s, float margin,
-                                   int direct, int* counters, unsigned long long* __restrict__ mask_out,
-                                   float* __restrict__ w_out) {
+__global__ void route_count_kernel(RowSrc src, int64_t B, LiveRows live, const float* __restrict__ cent, int K, int s, float margin,
+                                   int* counters, unsigned long long* __restrict__ mask_out, float* __restrict__ w_out) {
     __shared__ int hist[MN_MAX_SUB];
     __shared__ float sc[MN_MAX_SUB * 3];
     for (int i = threadIdx.x; i < K * 3; i += blockDim.x) sc[i] = cent[i];
     for (int i = threadIdx.x; i < K; i += blockDim.x) hist[i] = 0;
     __syncthreads();
     const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t n = live.rows(B);
+    const bool direct = n <= 25 && K <= 25;
     uint64_t mask = 0;
-    if (row < B) {
+    if (row < n) {
         float d[KMAX], w[KMAX];
         distances<KMAX>(src, row, sc, K, s, direct, d, margin > 1.0f ? margin * margin : 1.0f);
         mask = route_row<KMAX>(d, K, margin, w);
@@ -143,12 +146,13 @@ __global__ void route_count_kernel(RowSrc src, int64_t B, const float* __restric
 }
 
 template <int KMAX>
-__global__ void route_scatter_kernel(int64_t B, int K, int* counters, int64_t cap, const unsigned long long* __restrict__ mask_in,
-                                     const float* __restrict__ w_in, int* slot_row, float* slot_w, int* row_slots,
-                                     unsigned int* status) {
+__global__ void route_scatter_kernel(int64_t B, LiveRows live, int K, int* counters, int64_t cap,
+                                     const unsigned long long* __restrict__ mask_in, const float* __restrict__ w_in, int* slot_row,
+                                     float* slot_w, int* row_slots, unsigned int* status) {
     const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int lane = threadIdx.x & 31;
-    const uint64_t mask = row < B ? mask_in[row] : 0ull;
+    const int64_t n = live.rows(B);
+    const uint64_t mask = row < n ? mask_in[row] : 0ull;
     // one global atomic per (block, sub-module): warp ballots -> shared per-warp counts -> block prefix
     __shared__ int wcnt[8][KMAX];     // blockDim.x == 256
     const int warp = threadIdx.x >> 5;
@@ -192,14 +196,14 @@ __global__ void route_scatter_kernel(int64_t B, int K, int* counters, int64_t ca
                 if (slot_w) slot_w[slot] = w_in[(int64_t)k * B + row];
             }
         }
-        if (row < B && row_slots) row_slots[row * K + k] = slot;
+        if (row < n && row_slots) row_slots[row * K + k] = slot;
     }
 }
 
-__global__ void combine_kernel(int64_t B, int K, const int* __restrict__ row_slots, const float* __restrict__ slot_out,
+__global__ void combine_kernel(int64_t B, LiveRows live, int K, const int* __restrict__ row_slots, const float* __restrict__ slot_out,
                                int out_cols, float* __restrict__ out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= B * out_cols) return;
+    if (i >= live.rows(B) * out_cols) return;
     const int64_t row = i / out_cols;
     const int c = (int)(i % out_cols);
     float acc = 0.0f;
@@ -307,14 +311,13 @@ size_t mn_route_scratch_bytes(const mn_model* m, int64_t B) {
     return n;
 }
 
-int mn_route_build(mn_ctx* ctx, mn_model* m, const RowSrc& src, int64_t B, int64_t cap, int* slot_row, float* slot_w,
+int mn_route_build(mn_ctx* ctx, mn_model* m, const RowSrc& src, int64_t B, LiveRows live, int64_t cap, int* slot_row, float* slot_w,
                    int* row_slots, void* scratch, cudaStream_t st) {
     unsigned long long* mask_buf = reinterpret_cast<unsigned long long*>(scratch);
     float* w_buf = m->d.boundary_margin > 1.0f
                        ? reinterpret_cast<float*>(reinterpret_cast<char*>(scratch) + mn_align((size_t)B * sizeof(unsigned long long)))
                        : nullptr;
     const int K = m->d.n_sub;
-    const int direct = (B <= 25 && K <= 25) ? 1 : 0;
     MN_CUDA(ctx, cudaMemsetAsync(m->counters_d, 0, CNT_TOTAL * sizeof(int), st));
     MN_CUDA(ctx, cudaMemsetAsync(slot_row, 0xFF, (size_t)cap * sizeof(int), st));
     const unsigned blocks = (unsigned)mn_cdiv(B, 256);
@@ -324,19 +327,19 @@ int mn_route_build(mn_ctx* ctx, mn_model* m, const RowSrc& src, int64_t B, int64
         else if (K <= 32) KERNEL<32><<<GRID, BLOCK, 0, st>>>(__VA_ARGS__);            \
         else KERNEL<MN_MAX_SUB><<<GRID, BLOCK, 0, st>>>(__VA_ARGS__);                 \
     } while (0)
-    MN_ROUTE_DISPATCH(route_count_kernel, blocks, 256, src, B, m->centroids_d, K, m->d.cluster_dim_start, m->d.boundary_margin,
-                      direct, m->counters_d, mask_buf, w_buf);
+    MN_ROUTE_DISPATCH(route_count_kernel, blocks, 256, src, B, live, m->centroids_d, K, m->d.cluster_dim_start, m->d.boundary_margin,
+                      m->counters_d, mask_buf, w_buf);
     MN_LAUNCH_CHECK(ctx);
-    MN_ROUTE_DISPATCH(route_scatter_kernel, blocks, 256, B, K, m->counters_d, cap, mask_buf, w_buf, slot_row, slot_w, row_slots,
+    MN_ROUTE_DISPATCH(route_scatter_kernel, blocks, 256, B, live, K, m->counters_d, cap, mask_buf, w_buf, slot_row, slot_w, row_slots,
                       ctx->status_d);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }
 
-int mn_route_combine(mn_ctx* ctx, mn_model* m, int64_t B, const int* row_slots, const float* slot_out, int out_cols,
+int mn_route_combine(mn_ctx* ctx, mn_model* m, int64_t B, LiveRows live, const int* row_slots, const float* slot_out, int out_cols,
                      float* out, cudaStream_t st) {
     const int64_t n = B * out_cols;
-    combine_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, st>>>(B, m->d.n_sub, row_slots, slot_out, out_cols, out);
+    combine_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, st>>>(B, live, m->d.n_sub, row_slots, slot_out, out_cols, out);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }

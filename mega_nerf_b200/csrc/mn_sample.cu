@@ -115,14 +115,15 @@ __global__ void sample_coarse_kernel(const float* __restrict__ rays, const float
     }
 }
 
+// flip (perturb == 0 only): row written in reverse order, torch.flip(z, [-1])
 __global__ void stratify_kernel(const float* __restrict__ zin, int64_t stride, const float* __restrict__ rnd, float perturb,
-                                int64_t N, int S, float* __restrict__ z_out) {
+                                int64_t N, int S, float* __restrict__ z_out, LiveRows live, int flip) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= N * S) return;
+    if (t >= live.rows(N) * S) return;
     const int64_t ray = t / S;
     const int s = (int)(t % S);
     const float* zr = zin + ray * stride;
-    float z = zr[s];
+    float z = zr[flip ? S - 1 - s : s];
     if (perturb > 0.0f) {
         const float lower = s > 0 ? 0.5f * (zr[s - 1] + z) : z;
         const float upper = s < S - 1 ? 0.5f * (z + zr[s + 1]) : z;
@@ -318,13 +319,14 @@ struct CompositeArgs {
     int flip;
     float *weights, *rgb, *depth, *var, *lambda;
     int npad;              // shared-memory elements per warp
+    LiveRows live;         // rays at or past live.rows(N) are skipped
 };
 
 __global__ void __launch_bounds__(128) composite_kernel(const CompositeArgs a) {
     extern __shared__ unsigned char sm_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t ray = (int64_t)blockIdx.x * 4 + warp;
-    if (ray >= a.N) return;
+    if (ray >= a.live.rows(a.N)) return;
     const int n = a.S + a.S2;
     const CompositeSmem sm = composite_smem(sm_raw, warp, a.npad);
     const float* zs = sm.zs;
@@ -399,11 +401,11 @@ __global__ void __launch_bounds__(128) sample_pdf_kernel(const float* __restrict
                                                          int64_t w_stride, const float* __restrict__ cdf_in,
                                                          const float* __restrict__ u, int64_t u_stride, int64_t N, int S,
                                                          int F, float* __restrict__ z_out, int64_t* __restrict__ inds_out,
-                                                         float* __restrict__ cdf_out) {
+                                                         float* __restrict__ cdf_out, LiveRows live) {
     extern __shared__ unsigned char sm_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t ray = (int64_t)blockIdx.x * 4 + warp;
-    if (ray >= N) return;
+    if (ray >= live.rows(N)) return;
     const int nb = S - 2;          // pdf / cdf entries
     const int nc = S - 1;          // padded cdf entries == number of bin edges
     float* cs = reinterpret_cast<float*>(sm_raw) + (size_t)warp * 2 * S;
@@ -448,13 +450,14 @@ __global__ void __launch_bounds__(128) sample_pdf_kernel(const float* __restrict
     }
 }
 
+// out_flip (optional): the same rows in reverse order, torch.flip(out, [-1])
 __global__ void __launch_bounds__(128) sort_cat_kernel(const float* __restrict__ a, int na, const float* __restrict__ b,
                                                        int nb, int64_t N, int descending, int npad,
-                                                       float* __restrict__ out) {
+                                                       float* __restrict__ out, float* __restrict__ out_flip, LiveRows live) {
     extern __shared__ unsigned char sm_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t ray = (int64_t)blockIdx.x * 4 + warp;
-    if (ray >= N) return;
+    if (ray >= live.rows(N)) return;
     float* key = reinterpret_cast<float*>(sm_raw) + (size_t)warp * npad;
     unsigned short* id = reinterpret_cast<unsigned short*>(reinterpret_cast<float*>(sm_raw) + (size_t)4 * npad) +
                          (size_t)warp * npad;
@@ -466,40 +469,32 @@ __global__ void __launch_bounds__(128) sort_cat_kernel(const float* __restrict__
     __syncwarp();
     warp_bitonic(key, id, npad, descending != 0, lane);
     for (int i = lane; i < n; i += 32) out[ray * n + i] = key[i];
+    if (out_flip)
+        for (int i = lane; i < n; i += 32) out_flip[ray * n + (n - 1 - i)] = key[i];
 }
 
 // ------------------------------------------------------------------------------------------------
 // background geometry                                                  (rendering.py:396-469)
 // ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float dot3(const float* a, const float* b) { return (a[0] * b[0] + a[1] * b[1]) + a[2] * b[2]; }
+__device__ __forceinline__ float dot3(const float* a, const float* b) { return mn_dot3(a, b); }
 
 __global__ void intersect_sphere_kernel(const float* __restrict__ rays, const float* __restrict__ center,
                                         const float* __restrict__ radius, int64_t N, float* __restrict__ fg_far,
                                         unsigned int* status) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
-    float o[3], d[3];
-    for (int j = 0; j < 3; ++j) {
-        o[j] = rays[i * 8 + j];
-        d[j] = rays[i * 8 + 3 + j];
-        if (radius) { o[j] = (o[j] - center[j]) / radius[j]; d[j] = d[j] / radius[j]; }
-    }
-    const float dd = dot3(d, d);
-    const float d1 = -dot3(d, o) / dd;
-    float p[3];
-    for (int j = 0; j < 3; ++j) p[j] = o[j] + d1 * d[j];
-    const float cosv = 1.0f / sqrtf(dd);
-    const float pn2 = dot3(p, p);
-    if (pn2 >= 1.0f) atomicOr(status, MN_STATUS_SPHERE);
-    fg_far[i] = d1 + sqrtf(1.0f - pn2) * cosv;
+    bool outside;
+    fg_far[i] = mn_sphere_far(rays + i * 8, center, radius, &outside);
+    if (outside) atomicOr(status, MN_STATUS_SPHERE);
 }
 
+// flip_pts: the points of each ray are written in reverse sample order (torch.flip(pts, [-2])), depth_real in sample order
 __global__ void points_outside_kernel(const float* __restrict__ rays, const int64_t* __restrict__ ids,
                                       const float* __restrict__ depth, const float* __restrict__ center,
                                       const float* __restrict__ radius, int64_t n, int S, int real, int c2d,
-                                      float* __restrict__ pts, float* __restrict__ depth_real) {
+                                      float* __restrict__ pts, float* __restrict__ depth_real, LiveRows live, int flip_pts) {
     const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n * S) return;
+    if (t >= live.rows(n) * S) return;
     const int64_t r = t / S;
     const int64_t ray = ids ? ids[r] : r;
     float o0[3], d0[3], o[3], d[3];
@@ -535,7 +530,7 @@ __global__ void points_outside_kernel(const float* __restrict__ rays, const int6
     const float dr = (1.0f / (dep + 1e-8f)) * cosf(theta) + d1;
     depth_real[t] = dr;
     const int C = real ? 7 : 4;
-    float* q = pts + t * C;
+    float* q = pts + (flip_pts ? r * S + (S - 1 - (t - r * S)) : t) * C;
     if (real) {
         const float s = c2d ? dr : (d1 + d2);
         for (int j = 0; j < 3; ++j) q[j] = o0[j] + d0[j] * s;
@@ -573,9 +568,9 @@ __device__ __forceinline__ float sh_eval(int deg, const float* s, float x, float
 }
 
 __global__ void sh_to_rgb_kernel(int deg, const float* __restrict__ coef, int64_t cstride, const float* __restrict__ dirs,
-                                 int64_t dstride, int ddiv, int64_t B, int sig, float* __restrict__ out) {
+                                 int64_t dstride, int ddiv, int64_t B, int sig, float* __restrict__ out, LiveRows live) {
     const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
+    if (b >= live.rows(B)) return;
     const int nc = (deg + 1) * (deg + 1);
     const float* c = coef + b * cstride;
     const float* d = dirs + (b / ddiv) * dstride;
@@ -826,9 +821,7 @@ int mn_stratify(mn_ctx* ctx, const float* z_d, int64_t z_row_stride, const float
     if (!ctx || !z_d || !z_out_d || S < 1) return MN_ERR_INVALID;
     if (perturb > 0 && !rand_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_stratify: perturb > 0 needs rand_d");
     if (N == 0) return MN_OK;
-    stratify_kernel<<<(unsigned)mn_cdiv(N * S, 256), 256, 0, (cudaStream_t)stream>>>(z_d, z_row_stride, rand_d, perturb, N, S, z_out_d);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return mn_stage_stratify(ctx, z_d, z_row_stride, rand_d, perturb, N, S, 0, LiveRows{}, z_out_d, (cudaStream_t)stream);
 }
 
 int mn_points_from_z(mn_ctx* ctx, const float* rays_d, const float* z_d, int64_t N, int S, float* xyz_out_d, void* stream) {
@@ -846,26 +839,15 @@ int mn_sample_pdf(mn_ctx* ctx, const float* z_coarse_d, const float* weights_d, 
     if ((weights_d == nullptr) == (cdf_d == nullptr))
         return mn_fail(ctx, MN_ERR_INVALID, "mn_sample_pdf: exactly one of weights_d / cdf_d");
     if (N == 0) return MN_OK;
-    const size_t sm = (size_t)4 * 2 * S * sizeof(float);
-    if (sm > 200 * 1024) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_sample_pdf: too many coarse samples");
-    MN_CUDA(ctx, cudaFuncSetAttribute(sample_pdf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    sample_pdf_kernel<<<(unsigned)mn_cdiv(N, 4), 128, sm, (cudaStream_t)stream>>>(z_coarse_d, weights_d, w_stride, cdf_d, u_d,
-                                                                                 u_row_stride, N, S, F, z_out_d, inds_out_d, cdf_out_d);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return mn_stage_sample_pdf(ctx, z_coarse_d, weights_d, w_stride, cdf_d, u_d, u_row_stride, N, S, F, LiveRows{}, z_out_d, inds_out_d,
+                               cdf_out_d, (cudaStream_t)stream);
 }
 
 int mn_sort_cat(mn_ctx* ctx, const float* a_d, int na, const float* b_d, int nb, int64_t N, int descending, float* out_d,
                 void* stream) {
     if (!ctx || !a_d || (nb > 0 && !b_d) || !out_d) return MN_ERR_INVALID;
     if (N == 0) return MN_OK;
-    const int npad = pow2_at_least(na + nb);
-    if (npad > 4096) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_sort_cat: more than 4096 samples per ray");
-    const size_t sm = (size_t)4 * npad * (sizeof(float) + sizeof(unsigned short));
-    MN_CUDA(ctx, cudaFuncSetAttribute(sort_cat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
-    sort_cat_kernel<<<(unsigned)mn_cdiv(N, 4), 128, sm, (cudaStream_t)stream>>>(a_d, na, b_d, nb, N, descending, npad, out_d);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return mn_stage_sort_cat(ctx, a_d, na, b_d, nb, N, descending, LiveRows{}, out_d, nullptr, (cudaStream_t)stream);
 }
 
 int mn_composite(mn_ctx* ctx, const float* raw_d, const float* z_d, const float* depth_real_d, int S, const float* raw2_d,
@@ -876,12 +858,8 @@ int mn_composite(mn_ctx* ctx, const float* raw_d, const float* z_d, const float*
     if (S2 > 0 && (!raw2_d || !z2_d)) return MN_ERR_INVALID;
     if (depth_real_d && S2 > 0 && !depth_real2_d) return MN_ERR_INVALID;
     if (N == 0) return MN_OK;
-    CompositeArgs a{};
-    a.raw = raw_d; a.z = z_d; a.dreal = depth_real_d; a.S = S;
-    a.raw2 = raw2_d; a.z2 = z2_d; a.dreal2 = depth_real2_d; a.S2 = S2;
-    a.last_delta = last_delta_d; a.N = N; a.flip = flip;
-    a.weights = weights_out_d; a.rgb = rgb_out_d; a.depth = depth_out_d; a.var = depth_var_out_d; a.lambda = bg_lambda_out_d;
-    return composite_launch(ctx, composite_kernel, a, "mn_composite", (cudaStream_t)stream);
+    return mn_stage_composite(ctx, raw_d, z_d, depth_real_d, S, raw2_d, z2_d, depth_real2_d, S2, last_delta_d, N, flip, LiveRows{},
+                              weights_out_d, rgb_out_d, depth_out_d, depth_var_out_d, bg_lambda_out_d, (cudaStream_t)stream);
 }
 
 int mn_composite_backward(mn_ctx* ctx, const float* raw_d, const float* z_d, int S, const float* raw2_d, const float* z2_d,
@@ -926,20 +904,16 @@ int mn_points_outside(mn_ctx* ctx, const float* rays_d, const int64_t* ray_ids_d
                       float* depth_real_out_d, void* stream) {
     if (!ctx || !rays_d || !depth_d || !pts_out_d || !depth_real_out_d) return MN_ERR_INVALID;
     if (n == 0) return MN_OK;
-    points_outside_kernel<<<(unsigned)mn_cdiv(n * S, 256), 256, 0, (cudaStream_t)stream>>>(
-        rays_d, ray_ids_d, depth_d, center3_d, radius3_d, n, S, include_xyz_real, cluster_2d, pts_out_d, depth_real_out_d);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return mn_stage_points_outside(ctx, rays_d, ray_ids_d, depth_d, center3_d, radius3_d, n, S, include_xyz_real, cluster_2d, 0,
+                                   LiveRows{}, pts_out_d, depth_real_out_d, (cudaStream_t)stream);
 }
 
 int mn_sh_to_rgb(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
                  int dir_div, int64_t B, int apply_sigmoid, float* out_d, void* stream) {
     if (!ctx || !coef_d || !dirs_d || !out_d || deg < 0 || deg > 4 || dir_div < 1) return MN_ERR_INVALID;
     if (B == 0) return MN_OK;
-    sh_to_rgb_kernel<<<(unsigned)mn_cdiv(B, 256), 256, 0, (cudaStream_t)stream>>>(deg, coef_d, coef_stride, dirs_d, dir_stride,
-                                                                                  dir_div, B, apply_sigmoid, out_d);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return mn_stage_sh_to_rgb(ctx, deg, coef_d, coef_stride, dirs_d, dir_stride, dir_div, B, apply_sigmoid, LiveRows{}, out_d,
+                              (cudaStream_t)stream);
 }
 
 int mn_embed(mn_ctx* ctx, const float* x_d, int64_t B, int dim, int n_freqs, float* out_d, void* stream) {
@@ -952,3 +926,67 @@ int mn_embed(mn_ctx* ctx, const float* x_d, int64_t B, int dim, int n_freqs, flo
 }
 
 }  // extern "C"
+
+// ---- the one launch of each stage kernel (mn_model.cuh): the public entry points above validate and call these; the background
+// pass of mn_render_rays_bg calls them with its device ray count and sample-order options ----
+int mn_stage_stratify(mn_ctx* ctx, const float* z_d, int64_t z_row_stride, const float* rand_d, float perturb, int64_t N, int S, int flip,
+                      LiveRows live, float* z_out_d, cudaStream_t st) {
+    stratify_kernel<<<(unsigned)mn_cdiv(N * S, 256), 256, 0, st>>>(z_d, z_row_stride, rand_d, perturb, N, S, z_out_d, live, flip);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+int mn_stage_points_outside(mn_ctx* ctx, const float* rays_d, const int64_t* ray_ids_d, const float* depth_d, const float* center3_d,
+                            const float* radius3_d, int64_t n, int S, int include_xyz_real, int cluster_2d, int flip_pts, LiveRows live,
+                            float* pts_out_d, float* depth_real_out_d, cudaStream_t st) {
+    points_outside_kernel<<<(unsigned)mn_cdiv(n * S, 256), 256, 0, st>>>(rays_d, ray_ids_d, depth_d, center3_d, radius3_d, n, S,
+                                                                         include_xyz_real, cluster_2d, pts_out_d, depth_real_out_d,
+                                                                         live, flip_pts);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+int mn_stage_sample_pdf(mn_ctx* ctx, const float* z_coarse_d, const float* weights_d, int64_t w_stride, const float* cdf_d, const float* u_d,
+                        int64_t u_row_stride, int64_t N, int S, int F, LiveRows live, float* z_out_d, int64_t* inds_out_d,
+                        float* cdf_out_d, cudaStream_t st) {
+    if (S < 3 || F < 1) return mn_fail(ctx, MN_ERR_INVALID, "mn_sample_pdf: resampling needs >= 3 coarse samples and >= 1 draw");
+    const size_t sm = (size_t)4 * 2 * S * sizeof(float);
+    if (sm > 200 * 1024) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_sample_pdf: too many coarse samples");
+    MN_CUDA(ctx, cudaFuncSetAttribute(sample_pdf_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    sample_pdf_kernel<<<(unsigned)mn_cdiv(N, 4), 128, sm, st>>>(z_coarse_d, weights_d, w_stride, cdf_d, u_d, u_row_stride, N, S, F, z_out_d,
+                                                                 inds_out_d, cdf_out_d, live);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+int mn_stage_sort_cat(mn_ctx* ctx, const float* a_d, int na, const float* b_d, int nb, int64_t N, int descending, LiveRows live,
+                      float* out_d, float* out_flip_d, cudaStream_t st) {
+    const int npad = pow2_at_least(na + nb);
+    if (npad > 4096) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_sort_cat: more than 4096 samples per ray");
+    const size_t sm = (size_t)4 * npad * (sizeof(float) + sizeof(unsigned short));
+    MN_CUDA(ctx, cudaFuncSetAttribute(sort_cat_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm));
+    sort_cat_kernel<<<(unsigned)mn_cdiv(N, 4), 128, sm, st>>>(a_d, na, b_d, nb, N, descending, npad, out_d, out_flip_d, live);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+int mn_stage_composite(mn_ctx* ctx, const float* raw_d, const float* z_d, const float* depth_real_d, int S, const float* raw2_d,
+                       const float* z2_d, const float* depth_real2_d, int S2, const float* last_delta_d, int64_t N, int flip,
+                       LiveRows live, float* weights_out_d, float* rgb_out_d, float* depth_out_d, float* depth_var_out_d,
+                       float* bg_lambda_out_d, cudaStream_t st) {
+    CompositeArgs a{};
+    a.raw = raw_d; a.z = z_d; a.dreal = depth_real_d; a.S = S;
+    a.raw2 = raw2_d; a.z2 = z2_d; a.dreal2 = depth_real2_d; a.S2 = S2;
+    a.last_delta = last_delta_d; a.N = N; a.flip = flip;
+    a.weights = weights_out_d; a.rgb = rgb_out_d; a.depth = depth_out_d; a.var = depth_var_out_d; a.lambda = bg_lambda_out_d;
+    a.live = live;
+    return composite_launch(ctx, composite_kernel, a, "mn_composite", st);
+}
+
+int mn_stage_sh_to_rgb(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
+                       int dir_div, int64_t B, int apply_sigmoid, LiveRows live, float* out_d, cudaStream_t st) {
+    sh_to_rgb_kernel<<<(unsigned)mn_cdiv(B, 256), 256, 0, st>>>(deg, coef_d, coef_stride, dirs_d, dir_stride, dir_div, B, apply_sigmoid,
+                                                                out_d, live);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}

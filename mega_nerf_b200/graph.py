@@ -9,8 +9,12 @@ replay it with no host work besides the copy of the inputs.
     g = GraphedRenderRays(nerf, hparams, n_rays=4096, device=dev)
     results = g(rays, image_indices)        # same dict as render_rays(...)[0]; tensors are reused by the next call
 
-The background (NeRF++) path is not captured: the reference synchronises with the host there (the bounds check that
-raises `Exception`, rendering.py:37,42,412-414) and so does ours; use `render_rays` for it.
+With a background (NeRF++) network the graph captures `render_rays_fused`, whose background split runs on the device:
+the number of rays that reach the background lives there too, so one graph serves every chunk of that ray count whatever
+its split.  The reference's sphere bound check (rendering.py:412-414) becomes a status word read after each replay, which
+raises the same `Exception`.
+
+    g = GraphedRenderRays(nerf, hparams, 4096, dev, bg_nerf=bg, sphere_center=c, sphere_radius=r, get_bg_fg_rgb=True)
 """
 from argparse import Namespace
 from typing import Dict, Optional
@@ -18,19 +22,27 @@ from typing import Dict, Optional
 import torch
 from torch import nn
 
-from .render import render_rays
+from . import _cabi as K
+from .render import render_rays, render_rays_fused
 
 
 class GraphedRenderRays:
     def __init__(self, nerf: nn.Module, hparams: Namespace, n_rays: int, device: torch.device, with_indices: bool = True,
-                 get_depth: bool = True, get_depth_variance: bool = False, warmup: int = 2, post=None):
+                 get_depth: bool = True, get_depth_variance: bool = False, warmup: int = 2, post=None,
+                 bg_nerf: Optional[nn.Module] = None, sphere_center: Optional[torch.Tensor] = None,
+                 sphere_radius: Optional[torch.Tensor] = None, get_bg_fg_rgb: bool = False):
         """`post(results)`, if given, runs right after render_rays INSIDE the captured region - e.g. the per-chunk
         exchange of a multi-GPU render (`torch.distributed.all_gather_into_tensor` on NCCL is capturable), so that a
-        step stays one graph launch; whatever it returns is kept in `self.post_result`."""
-        if nerf.training:
+        step stays one graph launch; whatever it returns is kept in `self.post_result`.
+        bg_nerf / sphere_center / sphere_radius / get_bg_fg_rgb: as for render_rays (the background path)."""
+        if nerf.training or (bg_nerf is not None and bg_nerf.training):
             raise ValueError('GraphedRenderRays replays the inference path; call nerf.eval() first')
         self.nerf, self.hparams = nerf, hparams
         self.flags = (get_depth, get_depth_variance, False)
+        self.bg_nerf = bg_nerf
+        self.get_bg_fg_rgb = get_bg_fg_rgb
+        self.center = sphere_center.to(device).float().contiguous() if sphere_center is not None else None
+        self.radius = sphere_radius.to(device).float().contiguous() if sphere_radius is not None else None
         self.post = post
         self.post_result = None
         self.rays = torch.zeros(n_rays, 8, device=device, dtype=torch.float32)
@@ -38,9 +50,9 @@ class GraphedRenderRays:
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.results: Optional[Dict[str, torch.Tensor]] = None
         self.warmup = warmup
-        net = nerf.module if hasattr(nerf, 'module') and not hasattr(nerf, '_native') else nerf
-        self._native = net._native()
-        self._params = [p for sub in self._native.subs for p in sub.parameters()]
+        unwrap = lambda m: m.module if hasattr(m, 'module') and not hasattr(m, '_native') else m
+        self._natives = [unwrap(m)._native() for m in (nerf, bg_nerf) if m is not None]
+        self._params = [p for nat in self._natives for sub in nat.subs for p in sub.parameters()]
         self._versions = -1
 
     def _weights_version(self) -> int:
@@ -51,15 +63,28 @@ class GraphedRenderRays:
         changed since the last pack - e.g. an optimiser step between two validation renders.  Called by every replay."""
         v = self._weights_version()
         if v != self._versions:
-            self._native.sync(self.rays.device)
+            for nat in self._natives:
+                nat.sync(self.rays.device)
             self._versions = v
 
     def _run(self) -> Dict[str, torch.Tensor]:
         with torch.no_grad():      # inference path only (a recording call would switch to the fp32 training kernels)
-            res, _ = render_rays(self.nerf, None, self.rays, self.indices, self.hparams, None, None, *self.flags)
+            if self.bg_nerf is None:
+                res, _ = render_rays(self.nerf, None, self.rays, self.indices, self.hparams, None, None, *self.flags)
+            else:
+                # no sync inside the captured region: the status word is checked after each replay (_check)
+                res = render_rays_fused(self.nerf, self.rays, self.indices, self.hparams, self.flags[0], self.flags[1],
+                                        bg_nerf=self.bg_nerf, sphere_center=self.center, sphere_radius=self.radius,
+                                        get_bg_fg_rgb=self.get_bg_fg_rgb, check_status=False)
             if self.post is not None:
                 self.post_result = self.post(res)
         return res
+
+    def _check(self) -> None:
+        """With a background network: raise the reference's sphere-bound `Exception` if a replayed camera was outside."""
+        if self.bg_nerf is not None:
+            h = K.ctx(self.rays.device)
+            K.check(K.lib().mn_check_status(h, K.stream_of(self.rays.device)), h)
 
     def _load(self, rays: torch.Tensor, image_indices: Optional[torch.Tensor]) -> None:
         if rays.shape != self.rays.shape:
@@ -79,6 +104,7 @@ class GraphedRenderRays:
                 self._run()
         cur.wait_stream(side)
         torch.cuda.synchronize(self.rays.device)
+        self._check()
         self.graph = torch.cuda.CUDAGraph()
         # thread_local: other threads of the process (e.g. the NCCL watchdog polling its events) must not invalidate the capture
         with torch.cuda.graph(self.graph, capture_error_mode='thread_local'):
@@ -91,4 +117,5 @@ class GraphedRenderRays:
         self.refresh_weights()
         self._load(rays, image_indices)
         self.graph.replay()
+        self._check()
         return self.results

@@ -366,14 +366,21 @@ def _render(net, bg, rays, image_indices, hparams, sphere_center, sphere_radius,
 
 
 def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Optional[torch.Tensor], hparams: Namespace,
-                      get_depth: bool, get_depth_variance: bool) -> Dict[str, torch.Tensor]:
-    """The foreground inference path of `render_rays(nerf, None, ...)` as ONE library call (`mn_render_rays`): the same
-    kernels in the same order, sequenced in C on the current stream instead of from Python.  Eval mode, no background
-    network; returns the same keys and values as `render_rays(...)[0]` for that case."""
+                      get_depth: bool, get_depth_variance: bool, bg_nerf: Optional[nn.Module] = None,
+                      sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None,
+                      get_bg_fg_rgb: bool = False, check_status: bool = True) -> Dict[str, torch.Tensor]:
+    """The inference path of `render_rays(nerf, bg_nerf, ...)` as ONE library call (`mn_render_rays`, or `mn_render_rays_bg`
+    with a background network): the same kernels in the same order, sequenced in C on the current stream instead of from
+    Python.  Eval mode; returns the same keys and values as `render_rays(...)[0]` for the same flags.
+
+    With a background network the split of the rays happens on the device (no host sync per chunk); the one sync is the
+    status check at the end, where the reference checks its sphere bound too: a camera outside the ellipsoid raises its
+    `Exception`.  `check_status=False` leaves that check to the caller (CUDA-graph capture, where no sync may happen)."""
     net = _unwrap(nerf)
-    if not isinstance(net, (NeRF, MegaNeRF, Cascade)):
+    bg = _unwrap(bg_nerf)
+    if not isinstance(net, (NeRF, MegaNeRF, Cascade)) or (bg is not None and not isinstance(bg, (NeRF, MegaNeRF, Cascade))):
         raise TypeError('mega_nerf_b200.render_rays_fused needs mega_nerf_b200 modules (use get_nerf / install())')
-    if net.training:
+    if net.training or (bg is not None and bg.training):
         raise ValueError('render_rays_fused is the inference path; call nerf.eval() first')
     if bool(hparams.use_cascade) != isinstance(net, Cascade):
         raise ValueError('hparams.use_cascade does not match the network')
@@ -386,25 +393,71 @@ def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
     N = rays.shape[0]
     idx = K.f32c(image_indices.to(dev)).view(-1) if image_indices is not None else None
     Sc, Sf = hparams.coarse_samples, hparams.fine_samples
+    cascade = bool(hparams.use_cascade)
     sh_deg = hparams.sh_deg if (hparams.pos_dir_dim == 0 and hparams.sh_deg is not None) else -1
     prec = K.PRECISIONS[get_precision()]
     steps = torch.linspace(0, 1, Sc, device=dev)
     u = torch.linspace(0, 1, Sf, device=dev) if Sf > 0 else None
     typ = 'fine' if Sf > 0 else 'coarse'
-    rgb = torch.empty(N, 3, device=dev, dtype=torch.float32)
-    depth = torch.empty(N, device=dev, dtype=torch.float32) if get_depth else None
-    var = torch.empty(N, device=dev, dtype=torch.float32) if get_depth_variance else None
-    rgb_c = torch.empty(N, 3, device=dev, dtype=torch.float32) if (hparams.use_cascade and Sf > 0) else None
-    nbytes = int(L.mn_render_rays_workspace_bytes(native.handle, N, Sc, Sf, int(hparams.use_cascade), sh_deg, prec))
-    ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
-    K.check(L.mn_render_rays(h, native.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(steps), Sc, K.ptr(u), Sf, int(hparams.use_cascade),
-                             sh_deg, prec, K.ptr(rgb), K.ptr(depth), K.ptr(var), K.ptr(rgb_c), K.ptr(ws), ws.numel(),
-                             K.stream_of(dev)), h)
+    new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
+    rgb = new(N, 3)
+    depth = new(N) if get_depth else None
+    var = new(N) if get_depth_variance else None
+    rgb_c = new(N, 3) if (cascade and Sf > 0) else None
+    if bg is None:
+        nbytes = int(L.mn_render_rays_workspace_bytes(native.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
+        ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
+        K.check(L.mn_render_rays(h, native.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(steps), Sc, K.ptr(u), Sf, int(cascade),
+                                 sh_deg, prec, K.ptr(rgb), K.ptr(depth), K.ptr(var), K.ptr(rgb_c), K.ptr(ws), ws.numel(),
+                                 K.stream_of(dev)), h)
+        res = {f'rgb_{typ}': rgb}
+        if depth is not None:
+            res[f'depth_{typ}'] = depth
+        if var is not None:
+            res[f'depth_variance_{typ}'] = var
+        if rgb_c is not None:
+            res['rgb_coarse'] = rgb_c
+        return res
+
+    bnative = bg._native()
+    bnative.sync(dev)
+    center = K.f32c(sphere_center.to(dev)) if sphere_center is not None else None
+    radius = K.f32c(sphere_radius.to(dev)) if sphere_radius is not None else None
+    real = getattr(hparams, 'container_path', None) is not None or getattr(hparams, 'train_mega_nerf', None) is not None
+    c2d = real and getattr(net, 'cluster_dim_start', 0) == 1                          # render.py:304-305
+    steps_bg = torch.linspace(0, 1, Sc // 2, device=dev)
+    u_bg = torch.linspace(0, 1, Sf // 2, device=dev) if Sf > 0 else None
     res = {f'rgb_{typ}': rgb}
     if depth is not None:
         res[f'depth_{typ}'] = depth
     if var is not None:
         res[f'depth_variance_{typ}'] = var
+    res[f'bg_lambda_{typ}'] = new(N)
     if rgb_c is not None:
         res['rgb_coarse'] = rgb_c
+        res['bg_lambda_coarse'] = new(N)
+    if get_bg_fg_rgb:
+        for key, cols in (('rgb', 3), ('depth', 1)):
+            for t in ([typ, 'coarse'] if rgb_c is not None else [typ]):
+                if f'{key}_{t}' in res:
+                    res[f'fg_{key}_{t}'] = new(N, 3) if cols == 3 else new(N)
+                    res[f'bg_{key}_{t}'] = new(N, 3) if cols == 3 else new(N)
+    out = K.RenderOutputs()
+    for field, key in (('rgb', f'rgb_{typ}'), ('depth', f'depth_{typ}'), ('depth_var', f'depth_variance_{typ}'),
+                       ('bg_lambda', f'bg_lambda_{typ}'), ('fg_rgb', f'fg_rgb_{typ}'), ('bg_rgb', f'bg_rgb_{typ}'),
+                       ('fg_depth', f'fg_depth_{typ}'), ('bg_depth', f'bg_depth_{typ}'), ('rgb_coarse', 'rgb_coarse'),
+                       ('bg_lambda_coarse', 'bg_lambda_coarse'), ('fg_rgb_coarse', 'fg_rgb_coarse'),
+                       ('bg_rgb_coarse', 'bg_rgb_coarse')):
+        if typ == 'coarse' and field.endswith('_coarse'):
+            continue                                       # coarse-only render: the final type is the coarse one
+        setattr(out, field, K.ptr(res.get(key)))
+    nbytes = int(L.mn_render_rays_bg_workspace_bytes(native.handle, bnative.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
+    ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
+    st = K.stream_of(dev)
+    K.check(L.mn_render_rays_bg(h, native.handle, bnative.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(center), K.ptr(radius),
+                                int(real), int(c2d), K.ptr(steps), K.ptr(steps_bg), Sc, K.ptr(u), K.ptr(u_bg), Sf, int(cascade),
+                                sh_deg, prec, C.byref(out), K.ptr(ws), ws.numel(), st), h)
+    if check_status:
+        # the reference raises from a host-side `.any()` over the sphere check (rendering.py:412-414)
+        K.check(L.mn_check_status(h, st), h)
     return res
