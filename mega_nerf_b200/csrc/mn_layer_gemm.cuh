@@ -30,9 +30,10 @@
 // from the activation tape at the (row, column) it stores.  tc_layer_head_dgrad_kernel is its head stage.
 //
 // A Linear has one or two K segments: the tile's encoder features (kpe or kaux columns of the feature tile image) and / or
-// the previous activations (the layer plan's input buffer).  Skip layers read [PE, H], dir_a_encoding reads [F, aux].
-// The host side is in mn_mlp_tc.cu: build_layer_plan maps the Linear table (tc_linears) to the launches, layer_launch issues
-// the forward, mn_train_tc_backward the backward, whose data-gradient GEMMs read their images from build_dgrad_plan's layout.
+// the previous activations (an activation buffer of the group).  Skip layers read [PE, H], dir_a_encoding reads [F, aux].
+// The host side is in mn_mlp_tc.cu: build_plan maps the Linear table (tc_linears) to the forward GEMMs of either engine,
+// lg_net derives this engine's activation buffers and rgb head from that plan, and lg_gemm launches one GEMM of the forward
+// (layer_launch) or of the backward's data-gradient chain (mn_train_tc_backward, images in build_dgrad_plan's layout).
 
 constexpr int kLgGroupTiles = 384;       // tiles per group: bounds the activation workspace (see mn_mlp_tc_workspace)
 constexpr int kLgStages = 4;             // ring stages of 48 KiB

@@ -16,10 +16,11 @@
 // is a multiple of 16 works, and no TMA tensor map is needed (plain 1-D bulk copies).
 //
 // Networks wider than 512 run on the layer-GEMM engine instead (mn_layer_gemm.cuh).  Host side: tc_linears lists the
-// network's Linears once; tc_net picks the engine (build_layer_plan or build_plan) and the training coverage
-// (build_dgrad_plan) from that table, and every entry point below calls it once.  mn_mlp_tc_pack writes the forward images of
-// either engine, tc_dgrad_ready / tc_pack_dgrad the transposed images of the backward, and mn_train_tc_backward runs
-// the backward of either engine between one shared workspace carve, gradient scale and head / embedding epilogue.
+// network's Linears once; tc_net picks the engine and the training coverage from that table, and builds the forward plan of
+// either engine (build_plan) and the data-gradient plan (build_dgrad_plan); every entry point below calls it once.
+// mn_mlp_tc_pack writes the forward images of either engine, tc_dgrad_ready / tc_pack_dgrad the transposed images of the
+// backward, and mn_train_tc_backward runs the backward of either engine between one shared workspace carve, gradient scale
+// and head / embedding epilogue.
 #include <cuda_fp16.h>
 
 #include <type_traits>
@@ -40,7 +41,7 @@ enum { EPI_RELU = 0, EPI_RELU_SIGMA = 1, EPI_LINEAR = 2, EPI_RGB = 3,
 enum { PP_INFER = 0, PP_TRAIN_FWD = 1, PP_DGRAD = 2 };
 
 struct TcGemm {
-    int n;           // MMA N
+    int n;           // MMA N = columns of the weight image (layer engine: the output columns padded to 256-column blocks)
     int nseg;
     int src[2];
     int k[2];        // padded K columns per segment (multiple of 16)
@@ -55,20 +56,20 @@ struct TcPlan {
     TcGemm g[kMaxGemm];
     int kpe, kaux;         // padded feature-tile widths
     int plane_bytes;       // bytes of all weight images of one sub-module (one precision plane)
-    int f32_floats;        // fp32 block: biases per GEMM (256 each) + sigma_w[L] + sigma_b
+    int f32_floats;        // fp32 block: the biases, sigma_w [L], sigma_b (4) [, the layer engine's rgb head]
     int sigma_w_off;       // float offset of sigma_w in the fp32 block
     int sub_bytes;         // total bytes per sub-module: planes (hi[,lo]) + fp32 block
     int x_tile_bytes;      // bytes of one feature tile image (one plane)
     int L;
-    int bstride;           // floats reserved per GEMM bias in the fp32 block (256; 512 for the 512-wide network)
+    int bstride;           // fused engine: floats reserved per GEMM bias in the fp32 block (256; 512 for the 512-wide network)
     int f32_off;           // byte offset of the fp32 block inside one sub-module's pack (after the hi and lo planes)
 };
 
 int pad16(int x) { return (x + 15) / 16 * 16; }
 
 // ---- the network's Linears in forward order (nerf.py:115-160): trunk layers 0 .. layers-1, xyz_encoding_final,
-// dir_a_encoding, rgb.  The plans of both engines, the weight packs and the weight-gradient items of the backward all walk
-// this one table.  Linear j's SRC_H segment reads the output of Linear j - 1 (image j - 1 of a tile's activation record).
+// dir_a_encoding, rgb.  The forward and data-gradient plans, the weight packs and the weight-gradient items of the backward all
+// walk this one table.  Linear j's SRC_H segment reads the output of Linear j - 1 (image j - 1 of a tile's activation record).
 struct TcSeg {
     int src;             // SRC_XPE / SRC_XAUX (a segment of the feature tile) or SRC_H (the previous Linear's output)
     int k, k_real;       // padded K columns (multiple of 16); columns that exist in the nn.Linear weight
@@ -121,114 +122,39 @@ TcLinears tc_linears(const mn_model& m) {
     return T;
 }
 
-// ---- fused plan: every Linear (the rgb head as an N = 32 GEMM) in one tc_mlp_wg_kernel launch
-bool build_plan(const NetDims& nd, const TcLinears& T, TcPlan* p) {
-    if (nd.L % 64 != 0 || (nd.L > 256 && nd.L != 512) || nd.L < 64 || nd.rgb_dim > 32 || nd.layers > 12) return false;
-    if (nd.affine && nd.rgb_dim != 3) return false;
+// ---- forward plan of either engine: one GEMM per Linear, the weight images back to back in a precision plane, the fp32 block
+// [biases][sigma_w (L)][sigma_b (4)].  The fused engine (tc_mlp_wg_kernel) runs every GEMM in one launch, the rgb head as an
+// N = 32 GEMM, and reserves bstride floats per bias.  The layer engine (mn_layer_gemm.cuh) launches one GEMM per Linear with
+// N padded to 256-column blocks, in the image and in the bias; its rgb head is not a GEMM: tc_layer_head_kernel reads
+// [rgb_w [rgb_dim][rgb_in]][rgb_b (32)] from the end of the fp32 block (lg_net).
+void build_plan(const NetDims& nd, const TcLinears& T, bool layer, TcPlan* p) {
     TcPlan& P = *p;
     P = TcPlan{};
     P.L = nd.L;
-    P.bstride = nd.L > 256 ? 512 : 256;
+    P.bstride = layer ? 0 : nd.L > 256 ? 512 : 256;
     P.kpe = T.kpe;
     P.kaux = T.kaux;
-    int woff = 0;
-    for (int gi = 0; gi < T.n; ++gi) {
+    P.n_trunk = T.n_trunk;
+    P.n_gemm = layer ? T.n - 1 : T.n;
+    int woff = 0, foff = 0;
+    for (int gi = 0; gi < P.n_gemm; ++gi) {
         const TcLinear& l = T.l[gi];
         TcGemm& g = P.g[gi];
-        g.n = l.epi == EPI_RGB ? 32 : l.n;
-        g.nseg = l.nseg;
-        for (int s = 0; s < l.nseg; ++s) { g.src[s] = l.seg[s].src; g.k[s] = l.seg[s].k; }
-        g.w_off = woff;
-        g.bias_off = gi * P.bstride;
-        g.epi = l.epi;
-        woff += (g.k[0] + g.k[1]) * g.n * 2;
-    }
-    P.n_trunk = T.n_trunk;
-    P.n_gemm = T.n;
-    P.plane_bytes = woff;
-    P.sigma_w_off = T.n * P.bstride;
-    P.f32_floats = T.n * P.bstride + nd.L + 4;
-    P.f32_off = woff * 2;
-    P.sub_bytes = (int)mn_align((size_t)woff * 2 + (size_t)P.f32_floats * 4, 256);
-    P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
-    return true;
-}
-
-// ---- layer plan: networks wider than build_plan covers, one GEMM launch per Linear (mn_layer_gemm.cuh); the rgb head runs
-// in tc_layer_head_kernel from the fp32 block
-enum { LB_ACT0 = 0, LB_ACT1 = 1, LB_G = 2 };     // activation buffers of a tile group: ping, pong, dir_a_encoding output
-
-struct LgGemm {
-    int n, n_blk;        // output columns; 256-column N blocks (the image and the output buffer are padded to n_blk * 256)
-    int nseg;
-    int src[2];          // SRC_H (the input buffer), SRC_XPE, SRC_XAUX
-    int k[2];            // K columns per segment (multiple of 16)
-    int w_off;           // byte offset of the weight image [n_blk][K/8][256][8] inside one precision plane
-    int bias_off;        // float offset of the bias (n_blk * 256 floats) inside the fp32 block
-    int relu;
-    int in, out;         // LB_* buffers read (SRC_H) and written
-};
-
-struct LayerPlan {
-    int n_gemm, n_trunk;
-    LgGemm g[kMaxGemm];
-    int L, kpe, kaux;
-    int plane_bytes;     // bytes of all weight images of one sub-module (one precision plane)
-    int f32_floats;      // fp32 block: biases, sigma_w [L], sigma_b (4), rgb_w [rgb_dim][rgb_in], rgb_b (32)
-    int sub_bytes;       // total bytes per sub-module: planes (hi, lo) + fp32 block
-    int sigma_w_off, rgb_w_off, rgb_b_off;
-    int rgb_in, h_last;  // rgb head input width; buffer of the last trunk activations
-    int rgb_src;         // buffer the rgb head reads
-    int x_tile_bytes;
-    int buf_cols[3];     // columns of each activation buffer (0: unused)
-};
-
-bool build_layer_plan(const NetDims& nd, const TcLinears& T, LayerPlan* p) {
-    if (nd.L <= 512 || nd.L > 2048 || nd.L % 256 != 0 || nd.rgb_dim > MN_TC_RGB_MAX || nd.layers + 2 > kMaxGemm) return false;
-    if (nd.affine && nd.rgb_dim != 3) return false;
-    LayerPlan& P = *p;
-    P = LayerPlan{};
-    P.L = nd.L;
-    P.kpe = T.kpe;
-    P.kaux = T.kaux;
-    const int ng = T.n - 1;
-    int woff = 0, foff = 0;
-    for (int gi = 0; gi < ng; ++gi) {
-        const TcLinear& l = T.l[gi];
-        LgGemm& g = P.g[gi];
-        g.n = l.n;
-        g.n_blk = (l.n + 255) / 256;
+        g.n = layer ? (l.n + 255) / 256 * 256 : l.epi == EPI_RGB ? 32 : l.n;
         g.nseg = l.nseg;
         for (int s = 0; s < l.nseg; ++s) { g.src[s] = l.seg[s].src; g.k[s] = l.seg[s].k; }
         g.w_off = woff;
         g.bias_off = foff;
-        g.relu = l.epi != EPI_LINEAR;
-        // Linear gi writes buffer gi % 2 and reads the other one.  dir_a_encoding writes G to its own buffer: F went to the other
-        // ping-pong buffer, so the head still finds H_last for sigma.
-        g.in = (gi + 1) & 1;
-        g.out = nd.has_dir_a && gi == ng - 1 ? LB_G : gi & 1;
-        woff += (g.k[0] + g.k[1]) * g.n_blk * 256 * 2;
-        foff += g.n_blk * 256;
+        g.epi = l.epi;
+        woff += (g.k[0] + g.k[1]) * g.n * 2;
+        foff += layer ? g.n : P.bstride;
     }
-    P.n_trunk = T.n_trunk;
-    P.h_last = (nd.layers - 1) & 1;
-    P.buf_cols[0] = P.buf_cols[1] = nd.L;
-    if (nd.has_dir_a) {
-        P.buf_cols[LB_G] = P.g[ng - 1].n_blk * 256;
-        P.rgb_src = LB_G;
-    } else {
-        P.rgb_src = P.h_last;
-    }
-    P.n_gemm = ng;
-    P.rgb_in = nd.rgb_in;
     P.plane_bytes = woff;
     P.sigma_w_off = foff;
-    P.rgb_w_off = foff + nd.L + 4;
-    P.rgb_b_off = P.rgb_w_off + nd.rgb_dim * nd.rgb_in;
-    P.f32_floats = P.rgb_b_off + MN_TC_RGB_MAX;
+    P.f32_floats = foff + nd.L + 4 + (layer ? nd.rgb_dim * nd.rgb_in + MN_TC_RGB_MAX : 0);
+    P.f32_off = woff * 2;
     P.sub_bytes = (int)mn_align((size_t)woff * 2 + (size_t)P.f32_floats * 4, 256);
     P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
-    return true;
 }
 
 // ---- data-gradient chain of the backward (training, needs dir_a_encoding): dX of every Linear from dir_a_encoding down to trunk
@@ -268,8 +194,7 @@ struct TcNet {
     int engine;
     bool train;          // tensor-core training covers the shape (mn_model_train_tc_supported once the weights are packed)
     TcLinears lin;
-    TcPlan F;            // TC_FUSED
-    LayerPlan P;         // TC_LAYER
+    TcPlan P;            // engine != TC_NONE: the forward GEMMs and the layout of the forward weight images (tc_packed)
     TcPlan D;            // train: the data-gradient chain and the layout of the transposed weight images (tc_dgrad)
 };
 
@@ -277,8 +202,12 @@ TcNet tc_net(const mn_model& m) {
     const NetDims& nd = m.nd;
     TcNet t{};
     t.lin = tc_linears(m);
-    if (build_layer_plan(nd, t.lin, &t.P)) t.engine = TC_LAYER;
-    else if (build_plan(nd, t.lin, &t.F)) t.engine = TC_FUSED;
+    if (nd.affine && nd.rgb_dim != 3) t.engine = TC_NONE;
+    else if (nd.L > 512 && nd.L <= 2048 && nd.L % 256 == 0 && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers + 2 <= kMaxGemm)
+        t.engine = TC_LAYER;
+    else if (nd.L % 64 == 0 && (nd.L <= 256 || nd.L == 512) && nd.L >= 64 && nd.rgb_dim <= 32 && nd.layers <= 12)
+        t.engine = TC_FUSED;
+    if (t.engine != TC_NONE) build_plan(nd, t.lin, t.engine == TC_LAYER, &t.P);
     t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers >= 2 &&
               (t.engine == TC_LAYER || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 10));
     if (t.train) build_dgrad_plan(nd, t.lin, &t.D);
@@ -591,47 +520,113 @@ int wg_launch(mn_ctx* ctx, const TcArgs& A, int64_t n_tiles128, cudaStream_t st)
 #include "mn_train_tc.cuh"
 #include "mn_layer_gemm.cuh"
 
-// Workspace of the layer-GEMM path: per tile of a group, the feature tile and the activation buffers, each with its lo
-// plane under tc_f16x3.  Bounded by kLgGroupTiles, not by the call's rows.
-struct LgWorkspace {
+// The layer engine's activation buffers and rgb head, from the forward plan.  GEMM gi writes ping-pong buffer gi % 2 and reads
+// the other one; dir_a_encoding writes G to its own buffer: F went to the other ping-pong buffer, so the head still finds
+// H_last for sigma.  rgb_w and rgb_b follow sigma_w and sigma_b in the fp32 block.
+enum { LB_ACT0 = 0, LB_ACT1 = 1, LB_G = 2 };
+struct LgNet {
+    int g_gemm;          // the GEMM that writes LB_G (dir_a_encoding), or -1
+    int buf_cols[3];     // columns of each activation buffer (0: unused)
+    int h_last;          // buffer of the last trunk activations
+    int rgb_src;         // buffer the rgb head reads
+    int rgb_w_off, rgb_b_off;
+    int in(int gi) const { return (gi + 1) & 1; }
+    int out(int gi) const { return gi == g_gemm ? LB_G : gi & 1; }
+};
+LgNet lg_net(const TcPlan& P, const NetDims& nd) {
+    LgNet b{};
+    b.g_gemm = nd.has_dir_a ? P.n_gemm - 1 : -1;
+    b.buf_cols[LB_ACT0] = b.buf_cols[LB_ACT1] = nd.L;
+    if (nd.has_dir_a) b.buf_cols[LB_G] = P.g[b.g_gemm].n;
+    b.h_last = (nd.layers - 1) & 1;
+    b.rgb_src = nd.has_dir_a ? LB_G : b.h_last;
+    b.rgb_w_off = P.sigma_w_off + nd.L + 4;
+    b.rgb_b_off = b.rgb_w_off + nd.rgb_dim * nd.rgb_in;
+    return b;
+}
+
+// Workspace of a forward call: per tile of a group, the feature tile and the layer engine's activation buffers, each with its lo
+// plane under tc_f16x3.  The fused engine's one group covers every tile and has no activation buffers; the layer engine's
+// groups are bounded by kLgGroupTiles, not by the call's rows.
+struct TcWorkspace {
     int64_t group_tiles;
     size_t x_bytes, buf_bytes[3], total;     // per plane
     int planes;
 };
-LgWorkspace lg_workspace(const LayerPlan& P, int64_t n_tiles128, int precision) {
-    LgWorkspace w{};
-    w.group_tiles = n_tiles128 < kLgGroupTiles ? n_tiles128 : kLgGroupTiles;
+TcWorkspace tc_workspace(const TcNet& net, const NetDims& nd, int64_t n_tiles128, int precision) {
+    const bool layer = net.engine == TC_LAYER;
+    const LgNet B = layer ? lg_net(net.P, nd) : LgNet{};
+    TcWorkspace w{};
+    w.group_tiles = layer && n_tiles128 > kLgGroupTiles ? kLgGroupTiles : n_tiles128;
     w.planes = precision == MN_PREC_TC_F16X3 ? 2 : 1;
-    w.x_bytes = mn_align((size_t)w.group_tiles * P.x_tile_bytes, 1024);
+    w.x_bytes = mn_align((size_t)w.group_tiles * net.P.x_tile_bytes, 1024);
     w.total = w.x_bytes * w.planes;
     for (int b = 0; b < 3; ++b) {
-        w.buf_bytes[b] = mn_align((size_t)w.group_tiles * P.buf_cols[b] * kTileM * 2, 1024);
+        w.buf_bytes[b] = mn_align((size_t)w.group_tiles * B.buf_cols[b] * kTileM * 2, 1024);
         w.total += w.buf_bytes[b] * w.planes;
     }
     w.total += 1024;
     return w;
 }
 
+// A tile image that a layer GEMM reads or writes: tile 0 of the group, the tile stride, the lo plane's offset (0: none).
+struct LgImg {
+    unsigned char* p;
+    int64_t tile_bytes, lo;
+};
+
+// One tc_layer_gemm_kernel launch of GEMM g of plan P (weights at wpack) over the tiles t0 .. t0 + nt - 1 of a group, storing its
+// first n_out columns to out.  A segment reads x (SRC_XPE / SRC_XAUX: the feature tile) or h (SRC_H).  G carries what the forward
+// and the data-gradient GEMMs do not share: bias and ReLU, or mask, dsig and scale.
+int lg_gemm(mn_ctx* ctx, LgArgs G, const MlpArgs& a, const TcPlan& P, const TcGemm& g, const void* wpack, int n_out, int64_t t0,
+            int64_t nt, LgImg x, LgImg h, LgImg out, bool split, bool dgrad, cudaStream_t st) {
+    G.m = a;
+    G.tile0 = t0;
+    G.n_tiles = nt;
+    G.wpack = (const unsigned char*)wpack;
+    G.sub_bytes = P.sub_bytes;
+    G.w_off = g.w_off;
+    G.k_tot = g.k[0] + (g.nseg > 1 ? g.k[1] : 0);
+    G.n_blk = g.n / kLgBlock;
+    G.n_out = n_out;
+    G.f32_off = P.f32_off;
+    G.nseg = g.nseg;
+    for (int s = 0; s < g.nseg; ++s) {
+        const LgImg& in = g.src[s] == SRC_H ? h : x;
+        G.a[s] = in.p + (g.src[s] == SRC_XAUX ? P.kpe * kTileM * 2 : 0);
+        G.ak[s] = g.k[s];
+        G.a_tile_bytes[s] = in.tile_bytes;
+        G.a_lo[s] = in.lo;
+    }
+    G.out = out.p;
+    G.out_tile_bytes = out.tile_bytes;
+    G.out_lo = out.lo;
+    const int64_t items = nt * G.n_blk;
+    const unsigned grid = (unsigned)(items < ctx->sm_count ? items : ctx->sm_count);
+    auto launch = [&](auto kernel, int smem) -> int {
+        MN_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+        kernel<<<grid, kWgmmaThreads, smem, st>>>(G);
+        MN_LAUNCH_CHECK(ctx);
+        return MN_OK;
+    };
+    if (dgrad) return launch(tc_layer_gemm_kernel<false, true>, LgShape<false>::smem);
+    if (split) return launch(tc_layer_gemm_kernel<true>, LgShape<true>::smem);
+    return launch(tc_layer_gemm_kernel<false>, LgShape<false>::smem);
+}
+
 }  // namespace
 
 // =================================================================================================
-static size_t fused_workspace(const TcPlan& F, int64_t n_tiles128, int precision) {
-    const size_t planes = precision == MN_PREC_TC_F16X3 ? 2 : 1;
-    return mn_align((size_t)n_tiles128 * F.x_tile_bytes * planes, 1024) + 1024;
-}
-
 size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision) {
     const TcNet net = tc_net(*m);
-    if (net.engine == TC_LAYER) return lg_workspace(net.P, n_tiles128, precision).total;
-    if (net.engine == TC_FUSED) return fused_workspace(net.F, n_tiles128, precision);
-    return 0;
+    return net.engine == TC_NONE ? 0 : tc_workspace(net, m->nd, n_tiles128, precision).total;
 }
 
 
 int mn_mlp_tp_program(const mn_model& m, unsigned int* table_out, int cap_entries, int* info8) {
     const TcNet net = tc_net(m);
     if (net.engine != TC_FUSED) return MN_ERR_UNSUPPORTED;
-    const TcPlan& P = net.F;
+    const TcPlan& P = net.P;
     const WgLayout L = wg_layout(P, false);
     int n = 0, n_trunk = 0;
     for (int gi = 0; gi < P.n_gemm; ++gi) {
@@ -695,38 +690,34 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
         return MN_OK;  // configuration only served by the fp32 kernel
     }
     const NetDims& nd = m->nd;
-    const bool fused = net.engine == TC_FUSED;
-    const TcPlan& F = net.F;
-    const LayerPlan& P = net.P;
-    const int plane = fused ? F.plane_bytes : P.plane_bytes, n_gemm = fused ? F.n_gemm : P.n_gemm;
-    const size_t sub_bytes = (size_t)(fused ? F.sub_bytes : P.sub_bytes);
+    const TcPlan& P = net.P;
+    const size_t sub_bytes = (size_t)P.sub_bytes;
     if (!m->tc_packed) {
         MN_CUDA(ctx, cudaMalloc(&m->tc_packed, sub_bytes * m->d.n_sub));
         MN_CUDA(ctx, cudaMemsetAsync(m->tc_packed, 0, sub_bytes * m->d.n_sub, st));
     }
     unsigned char* base = (unsigned char*)m->tc_packed + (size_t)sub * sub_bytes;
     const float* Pk = m->packed + (size_t)sub * m->lay.total;
-    float* f32 = reinterpret_cast<float*>(base + (size_t)plane * 2);
-    for (int gi = 0; gi < n_gemm; ++gi) {
+    float* f32 = reinterpret_cast<float*>(base + P.f32_off);
+    for (int gi = 0; gi < P.n_gemm; ++gi) {
         const TcLinear& l = net.lin.l[gi];
-        // image N (the fused rgb GEMM has N = 32) and the floats reserved for the bias: the fused plan's bias stride, or the
-        // layer plan's N blocks
-        const int n_img = fused ? F.g[gi].n : P.g[gi].n_blk * 256, w_off = fused ? F.g[gi].w_off : P.g[gi].w_off;
-        const int b_off = fused ? F.g[gi].bias_off : P.g[gi].bias_off, b_n = fused ? F.bstride : n_img;
-        const int K = l.seg[0].k + (l.nseg > 1 ? l.seg[1].k : 0);
+        const TcGemm& g = P.g[gi];
+        const int K = g.k[0] + g.k[1];
         // a leading PE segment holds its real columns, then zeros up to its padded width; the other columns follow contiguously
         const bool pe = l.seg[0].src == SRC_XPE;
-        mn_pack_push(ctx, PackOp{Pk + l.w, base + w_off, base + plane + w_off, (long long)n_img * K, PK_TC_HALF,
-                                 {l.n, l.kin, n_img, K, pe ? l.seg[0].k_real : 0, pe ? l.seg[0].k : 0, n_img < 256 ? n_img : 256}});
-        mn_pack_push(ctx, PackOp{Pk + l.b, f32 + b_off, nullptr, (long long)b_n, PK_TC_F32, {l.n, 0, 0, 0, 0, 0, 0}});
+        mn_pack_push(ctx, PackOp{Pk + l.w, base + g.w_off, base + P.plane_bytes + g.w_off, (long long)g.n * K, PK_TC_HALF,
+                                 {l.n, l.kin, g.n, K, pe ? l.seg[0].k_real : 0, pe ? l.seg[0].k : 0, g.n < 256 ? g.n : 256}});
+        // the bias fills the floats the plan reserved for it, up to the next bias (sigma_w after the last one)
+        const int b_end = gi + 1 < P.n_gemm ? P.g[gi + 1].bias_off : P.sigma_w_off;
+        mn_pack_push(ctx, PackOp{Pk + l.b, f32 + g.bias_off, nullptr, (long long)(b_end - g.bias_off), PK_TC_F32, {l.n, 0, 0, 0, 0, 0, 0}});
     }
-    const int sigma_w_off = fused ? F.sigma_w_off : P.sigma_w_off;
-    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
-    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + sigma_w_off + nd.L, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
-    if (!fused) {      // tc_layer_head_kernel computes the rgb head on the CUDA cores
-        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + P.rgb_w_off, nullptr, (long long)nd.rgb_dim * nd.rgb_in, PK_RGBW,
+    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + P.sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
+    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + P.sigma_w_off + nd.L, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
+    if (net.engine == TC_LAYER) {      // tc_layer_head_kernel computes the rgb head on the CUDA cores
+        const LgNet B = lg_net(P, nd);
+        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + B.rgb_w_off, nullptr, (long long)nd.rgb_dim * nd.rgb_in, PK_RGBW,
                                  {nd.rgb_in, nd.rgb_dim, 0, 0, 0, 0, 0}});
-        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + P.rgb_b_off, nullptr, MN_TC_RGB_MAX, PK_TC_F32, {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
+        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + B.rgb_b_off, nullptr, MN_TC_RGB_MAX, PK_TC_F32, {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
     }
     m->tc_ready = 1;
     m->train_tc_ok = net.train ? 1 : 0;
@@ -764,26 +755,28 @@ static TcArgs tc_forward_args(const mn_model* m, const TcPlan& F, const MlpArgs&
 // head launch.  The group count follows from the slot capacity, so a call is a static launch list (graph capture works).
 // tape != NULL (recording call, tc_f16): the encoder tiles, every GEMM's output (image gi of the tile's activation record) and
 // the fp32 head blocks go to the tape instead of the workspace, which is not used.
-static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerPlan& P, int64_t n_tiles128, int precision,
+static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet& net, int64_t n_tiles128, int precision,
                         void* ws, size_t ws_bytes, cudaStream_t st, const TrainTcTape* tape = nullptr) {
     if (!m->tc_ready) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: weights not packed");
     if (n_tiles128 <= 0) return MN_OK;
-    const LgWorkspace W = lg_workspace(P, n_tiles128, precision);
+    const TcPlan& P = net.P;
+    const LgNet B = lg_net(P, m->nd);
+    const TcWorkspace W = tc_workspace(net, m->nd, n_tiles128, precision);
     if (!tape && (ws_bytes < W.total || !ws)) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
     const bool split = precision == MN_PREC_TC_F16X3;
     unsigned char* wp = (unsigned char*)(((uintptr_t)ws + 1023) / 1024 * 1024);
     __half* ximg = reinterpret_cast<__half*>(wp);
     const int64_t x_lo = (int64_t)W.x_bytes;                 // lo plane of each region right after its hi plane
     wp += W.x_bytes * W.planes;
-    unsigned char* buf[3];
-    for (int b = 0; b < 3; ++b) { buf[b] = wp; wp += W.buf_bytes[b] * W.planes; }
+    LgImg buf[3];
+    for (int b = 0; b < 3; ++b) {
+        buf[b] = LgImg{wp, (int64_t)B.buf_cols[b] * kTileM * 2, (int64_t)W.buf_bytes[b]};
+        wp += W.buf_bytes[b] * W.planes;
+    }
     const int64_t act_tile = tape ? (int64_t)mn_train_tc_act_tile_bytes(m) : 0;
 
     const size_t enc_sm = (size_t)P.x_tile_bytes * (split ? 2 : 1);
     MN_CUDA(ctx, cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
-    const int gemm_sm = split ? LgShape<true>::smem : LgShape<false>::smem;
-    if (split) MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
-    else MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
     const int n_gemm = a.sigma_only ? P.n_trunk : P.n_gemm;
     const int64_t plane_halves = x_lo / 2;
 
@@ -794,68 +787,38 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
         if (tape) ximg = reinterpret_cast<__half*>(tape->xreg + t0 * (int64_t)P.x_tile_bytes);
         tc_encode_kernel<<<(unsigned)nt, kTileM, enc_sm, st>>>(a, P.kpe, P.kaux, split ? 1 : 0, ximg, plane_halves, t0);
         MN_LAUNCH_CHECK(ctx);
+        const LgImg x{reinterpret_cast<unsigned char*>(ximg), P.x_tile_bytes, x_lo};
         for (int gi = 0; gi < n_gemm; ++gi) {
-            const LgGemm& g = P.g[gi];
+            const TcGemm& g = P.g[gi];
             LgArgs G{};
-            G.m = a;
-            G.tile0 = t0;
-            G.n_tiles = nt;
-            G.wpack = (const unsigned char*)m->tc_packed;
-            G.sub_bytes = P.sub_bytes;
             G.w_lo = P.plane_bytes;
-            G.w_off = g.w_off;
-            G.k_tot = g.k[0] + (g.nseg > 1 ? g.k[1] : 0);
-            G.n_blk = g.n_blk;
-            G.n_out = g.n;
             G.bias_off = g.bias_off;
-            G.f32_off = P.plane_bytes * 2;
-            G.relu = g.relu;
-            G.nseg = g.nseg;
-            for (int s = 0; s < g.nseg; ++s) {
-                G.ak[s] = g.k[s];
-                if (g.src[s] == SRC_H) {
-                    G.a[s] = buf[g.in];
-                    G.a_tile_bytes[s] = (int64_t)P.buf_cols[g.in] * kTileM * 2;
-                    G.a_lo[s] = (int64_t)W.buf_bytes[g.in];
-                } else {
-                    G.a[s] = (const unsigned char*)ximg + (g.src[s] == SRC_XAUX ? P.kpe * kTileM * 2 : 0);
-                    G.a_tile_bytes[s] = P.x_tile_bytes;
-                    G.a_lo[s] = x_lo;
-                }
+            G.relu = g.epi != EPI_LINEAR;
+            LgImg h = buf[B.in(gi)], out = buf[B.out(gi)];
+            if (tape) {       // GEMM gi reads image gi - 1 (SRC_H; trunk layer 0 has none) and writes image gi of the activation record
+                h = gi > 0 ? LgImg{rec + mn_tc_img_off(gi - 1, P.L), act_tile, 0} : LgImg{};
+                out = LgImg{rec + mn_tc_img_off(gi, P.L), act_tile, 0};
             }
-            G.out = buf[g.out];
-            G.out_tile_bytes = (int64_t)P.buf_cols[g.out] * kTileM * 2;
-            G.out_lo = (int64_t)W.buf_bytes[g.out];
-            if (tape) {                 // GEMM gi reads image gi - 1 (SRC_H) and writes image gi of the activation record
-                for (int s = 0; s < g.nseg; ++s)
-                    if (g.src[s] == SRC_H) { G.a[s] = rec + mn_tc_img_off(gi - 1, P.L); G.a_tile_bytes[s] = act_tile; G.a_lo[s] = 0; }
-                G.out = rec + mn_tc_img_off(gi, P.L);
-                G.out_tile_bytes = act_tile;
-                G.out_lo = 0;
-            }
-            const int64_t items = nt * g.n_blk;
-            const unsigned grid = (unsigned)(items < ctx->sm_count ? items : ctx->sm_count);
-            if (split) tc_layer_gemm_kernel<true><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
-            else tc_layer_gemm_kernel<false><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
-            MN_LAUNCH_CHECK(ctx);
+            const int rc = lg_gemm(ctx, G, a, P, g, m->tc_packed, net.lin.l[gi].n, t0, nt, x, h, out, split, false, st);
+            if (rc) return rc;
         }
         LhArgs H{};
         H.m = a;
         H.tile0 = t0;
         H.wpack = (const unsigned char*)m->tc_packed;
         H.sub_bytes = P.sub_bytes;
-        H.f32_off = P.plane_bytes * 2;
+        H.f32_off = P.f32_off;
         H.sigma_w_off = P.sigma_w_off;
-        H.rgb_w_off = P.rgb_w_off;
-        H.rgb_b_off = P.rgb_b_off;
-        H.h = buf[P.h_last];
-        H.h_tile_bytes = (int64_t)P.buf_cols[P.h_last] * kTileM * 2;
-        H.h_lo = split ? (int64_t)W.buf_bytes[P.h_last] : 0;
-        H.g = buf[P.rgb_src];
-        H.g_tile_bytes = (int64_t)P.buf_cols[P.rgb_src] * kTileM * 2;
-        H.g_lo = split ? (int64_t)W.buf_bytes[P.rgb_src] : 0;
+        H.rgb_w_off = B.rgb_w_off;
+        H.rgb_b_off = B.rgb_b_off;
+        H.h = buf[B.h_last].p;
+        H.h_tile_bytes = buf[B.h_last].tile_bytes;
+        H.h_lo = split ? buf[B.h_last].lo : 0;
+        H.g = buf[B.rgb_src].p;
+        H.g_tile_bytes = buf[B.rgb_src].tile_bytes;
+        H.g_lo = split ? buf[B.rgb_src].lo : 0;
         H.L = P.L;
-        H.rgb_in = P.rgb_in;
+        H.rgb_in = m->nd.rgb_in;
         if (tape) {
             H.h = rec + mn_tc_img_off(a.nd.layers - 1, P.L);
             H.g = rec + mn_tc_img_off(a.nd.layers + 1, P.L);
@@ -872,7 +835,7 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const LayerP
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws, size_t ws_bytes,
                      cudaStream_t st) {
     const TcNet net = tc_net(*m);
-    if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net.P, n_tiles128, precision, ws, ws_bytes, st);
+    if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net, n_tiles128, precision, ws, ws_bytes, st);
     if (net.engine != TC_FUSED || !m->tc_ready)
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "tensor-core MLP path covers layer_dim 64..256 (multiple of 64), 512 or 768..2048 (multiple of 256) and rgb_dim <= 32; "
@@ -881,15 +844,16 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "precision 'tc_f16x3' covers layer_dim <= 256; use 'tc_f16' or 'fp32' for the 512-wide network");
     if (n_tiles128 <= 0) return MN_OK;
-    TcArgs A = tc_forward_args(m, net.F, a, n_tiles128);
+    TcArgs A = tc_forward_args(m, net.P, a, n_tiles128);
     const TcPlan& P = A.plan;
     const int split = precision == MN_PREC_TC_F16X3 ? 1 : 0;
     A.split = split;
-    if (ws_bytes < fused_workspace(P, n_tiles128, precision) || !ws) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
+    const TcWorkspace W = tc_workspace(net, m->nd, n_tiles128, precision);
+    if (ws_bytes < W.total || !ws) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
     uintptr_t wp = ((uintptr_t)ws + 1023) / 1024 * 1024;
     __half* ximg = reinterpret_cast<__half*>(wp);
     A.ximg = ximg;
-    A.x_plane_halves = (int64_t)n_tiles128 * (P.kpe + P.kaux) * kTileM;
+    A.x_plane_halves = (int64_t)W.x_bytes / 2;
     int rc = tc_encode(ctx, m, a, P, n_tiles128, split, ximg, A.x_plane_halves, st);
     if (rc) return rc;
 
@@ -906,8 +870,7 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
 // =================================================================================================
 size_t mn_train_tc_x_tile_bytes(const mn_model* m) {
     const TcNet net = tc_net(*m);
-    if (net.engine == TC_LAYER) return (size_t)net.P.x_tile_bytes;
-    return net.engine == TC_FUSED ? (size_t)net.F.x_tile_bytes : 0;
+    return net.engine == TC_NONE ? 0 : (size_t)net.P.x_tile_bytes;
 }
 size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
     const NetDims& nd = m->nd;
@@ -921,8 +884,8 @@ int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n
     const TcNet net = tc_net(*m);
     int rc = tc_dgrad_ready(ctx, m, net, st);
     if (rc) return rc;
-    if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net.P, n_tiles128, MN_PREC_TC_F16, nullptr, 0, st, &tape);
-    TcArgs A = tc_forward_args(m, net.F, a, n_tiles128);
+    if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net, n_tiles128, MN_PREC_TC_F16, nullptr, 0, st, &tape);
+    TcArgs A = tc_forward_args(m, net.P, a, n_tiles128);
     A.ximg = reinterpret_cast<const __half*>(tape.xreg);
     A.x_plane_halves = 0;
     A.tape_act = tape.act;
@@ -1054,22 +1017,21 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         MN_LAUNCH_CHECK(ctx);
         return MN_OK;
     };
-    // ---- weight gradients of Linears j0 .. j1 - 1 over the tiles t0 .. t0 + nt - 1, one tc_wgrad_kernel launch.  dzt: the gradient
-    // images of tile t0, dz_tile_bytes apart: the fused engine's gradient records (Linear j's image at mn_tc_img_off(j)) or the
-    // layer engine's group buffer of its one Linear.
+    // ---- weight gradients of Linears j0 .. j1 - 1 over the tiles t0 .. t0 + nt - 1, one tc_wgrad_kernel launch.  dzt: the dZ image
+    // of Linear j0 in tile t0, the tiles dz_tile_bytes apart, and the images of the later Linears after it as in a gradient record:
+    // the fused engine's gradient records, or the layer engine's group buffer of its one Linear.
     auto wgrad = [&](int j0, int j1, const unsigned char* dzt, int64_t dz_tile_bytes, int64_t t0, int64_t nt) -> int {
-        const bool fused = net.engine == TC_FUSED;
         WgArgs W{};
         int64_t items = 0;
         for (int j = j0; j < j1; ++j) {
-            W.lin[j - j0] = wg_linear(lin, j, L, fused ? (int)mn_tc_img_off(j, L) : 0);
+            W.lin[j - j0] = wg_linear(lin, j, L, (int)mn_tc_img_off(j - j0, L));
             items += W.lin[j - j0].n_items;
         }
         W.act = tape.act;
         W.dz = dzt;
         W.xreg = tape.xreg;
         W.act_tile_bytes = act_tile;
-        W.x_tile_bytes = fused ? net.F.x_tile_bytes : net.P.x_tile_bytes;
+        W.x_tile_bytes = net.P.x_tile_bytes;
         W.dz_tile_bytes = dz_tile_bytes;
         W.t_min = t0;
         W.t_max = t0 + nt;
@@ -1079,7 +1041,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         W.sub_stride = a.lay.total;
         W.scale = scale;
         int64_t chunks;
-        if (fused) {
+        if (net.engine == TC_FUSED) {
             // every tile of the call, shared by n_sub sub-modules: enough CTAs to fill the machine about three times over (each
             // streams its tiles once; results are fp32 atomics)
             chunks = std::max<int64_t>(1, mn_cdiv((int64_t)ctx->sm_count * 3, items * n_sub));
@@ -1119,14 +1081,14 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         // which moves the gradients by more than fp32 atomic order does (DESIGN §8).
         if (L > 256) {
             for (int j = lin.n - 2; j >= 0; --j)
-                if ((rc = wgrad(j, j + 1, dz, act_tile, 0, tiles_used))) return rc;
+                if ((rc = wgrad(j, j + 1, dz + mn_tc_img_off(j, L), act_tile, 0, tiles_used))) return rc;
         } else if ((rc = wgrad(0, lin.n - 1, dz, act_tile, 0, tiles_used))) return rc;
         if ((rc = heads(0, tiles_used))) return rc;
     } else {
         // ---- layer engine, one tile group at a time: head stage -> per Linear (output side first) the weight gradient from its dZ
         // image, then the data-gradient GEMM that produces the next dZ in the other ping-pong buffer; then the sigma / rgb head
         // weight gradients.  dZ of Linear j is consumed by its weight gradient before the buffer is overwritten.
-        const LayerPlan& P = net.P;
+        const TcPlan& P = net.P;
         const TcPlan& D = net.D;
         const int rows = mn_tc_g32_rows(nd.rgb_dim);
         const int64_t gt = WS.head_tiles;
@@ -1134,8 +1096,6 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         unsigned char* pp[2];
         pp[0] = dzg + mn_align((size_t)gt * half * kTileM * 2);
         pp[1] = pp[0] + mn_align((size_t)gt * L * kTileM * 2);
-        constexpr int gemm_sm = LgShape<false>::smem;
-        MN_CUDA(ctx, cudaFuncSetAttribute(tc_layer_gemm_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, gemm_sm));
 
         for (int64_t t0 = 0; t0 < tiles_used; t0 += gt) {
             const int64_t nt = tiles_used - t0 < gt ? tiles_used - t0 : gt;
@@ -1151,8 +1111,8 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
                 H.g_tile_bytes = act_tile;
                 H.wpack = (const unsigned char*)m->tc_packed;
                 H.sub_bytes = P.sub_bytes;
-                H.f32_off = P.plane_bytes * 2;
-                H.rgb_w_off = P.rgb_w_off;
+                H.f32_off = P.f32_off;
+                H.rgb_w_off = lg_net(P, nd).rgb_w_off;
                 H.half = half;
                 H.gf32 = gf32;
                 H.dz = dzg;
@@ -1162,38 +1122,18 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
                 MN_LAUNCH_CHECK(ctx);
             }
             // ---- data-gradient GEMM g: dz_out = [mask](dz_in W^T) [+ S dsigma x sigma_w]
-            auto dgrad = [&](const unsigned char* dz_in, const TcGemm& g, unsigned char* dz_out) -> int {
+            auto dgrad = [&](unsigned char* dz_in, const TcGemm& g, unsigned char* dz_out) -> int {
                 LgArgs G{};
-                G.m = mm;
-                G.tile0 = t0;
-                G.n_tiles = nt;
-                G.wpack = (const unsigned char*)m->tc_dgrad;
-                G.sub_bytes = (int64_t)D.sub_bytes;
-                G.w_off = g.w_off;
-                G.k_tot = g.k[0];
-                G.n_blk = L / kLgBlock;
-                G.n_out = L;
-                G.bias_off = 0;
-                G.f32_off = D.f32_off;
-                G.nseg = 1;
-                G.a[0] = dz_in;
-                G.ak[0] = g.k[0];
-                G.a_tile_bytes[0] = (int64_t)g.k[0] * kTileM * 2;
-                G.out = dz_out;
-                G.out_tile_bytes = (int64_t)L * kTileM * 2;
                 G.mask = g.epi != EPI_D_LINEAR ? rec + mn_tc_img_off(g.img, L) : nullptr;     // xyz_encoding_final has no activation
                 G.mask_tile_bytes = act_tile;
                 G.dsig = g.epi == EPI_D_MASK_SIGMA ? gf32 + MN_TC_G32_SIGMA * kTileM : nullptr;
                 G.dsig_tile_floats = (int64_t)rows * kTileM;
                 G.scale = scale;
-                const int64_t items = nt * G.n_blk;
-                const unsigned grid = (unsigned)(items < ctx->sm_count ? items : ctx->sm_count);
-                tc_layer_gemm_kernel<false, true><<<grid, kWgmmaThreads, gemm_sm, st>>>(G);
-                MN_LAUNCH_CHECK(ctx);
-                return MN_OK;
+                return lg_gemm(ctx, G, mm, D, g, m->tc_dgrad, L, t0, nt, LgImg{}, LgImg{dz_in, (int64_t)g.k[0] * kTileM * 2, 0},
+                               LgImg{dz_out, (int64_t)L * kTileM * 2, 0}, false, true, st);
             };
             // Linear j (dir_a_encoding down to trunk layer 0): weight gradient, then data-gradient GEMM lin.n - 2 - j gives dZ of j - 1
-            const unsigned char* dzj = dzg;
+            unsigned char* dzj = dzg;
             for (int j = lin.n - 2, nxt = 0; j >= 0; --j, nxt ^= 1) {
                 if ((rc = wgrad(j, j + 1, dzj, (int64_t)lin.l[j].n * kTileM * 2, t0, nt))) return rc;
                 if (j == 0) break;
