@@ -148,9 +148,9 @@ int mn_route_combine(mn_ctx* ctx, mn_model* m, int64_t B, LiveRows live, const i
 int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,
                           float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st);
 // ---- the one launch of each stage kernel (csrc/mn_sample.cu).  The public stage entry points validate their arguments and call
-// these; the background pass of mn_render_rays_bg calls them with its device ray count (`live`: rays at or past it are skipped,
-// grids stay sized for N) and the sample orders it needs: flip = reversed stratify output, flip_pts = points in reversed sample
-// order (depth_real in sample order), out_flip_d = a second, reversed copy of sort_cat's output.
+// these; the render passes of mn_render_rays(_bg) call them directly, the background pass with its device ray count (`live`: rays
+// at or past it are skipped, grids stay sized for N) and the sample orders it needs: flip = reversed stratify output, flip_pts =
+// points in reversed sample order (depth_real in sample order), out_flip_d = a second, reversed copy of sort_cat's output.
 int mn_stage_stratify(mn_ctx* ctx, const float* z_d, int64_t z_row_stride, const float* rand_d, float perturb, int64_t N, int S, int flip,
                       LiveRows live, float* z_out_d, cudaStream_t st);
 int mn_stage_points_outside(mn_ctx* ctx, const float* rays_d, const int64_t* ray_ids_d, const float* depth_d, const float* center3_d,

@@ -1,9 +1,11 @@
-// mn_render_rays / mn_render_rays_bg: the inference path of render_rays (rendering.py:15-248, eval mode) as ONE C call - coarse
-// depths -> model query -> weights -> inverse-CDF resampling -> fine query -> merge + volume rendering, and with a background
-// (NeRF++) network its pass too (rendering.py:34-62, 143-173): sphere split, inverted-sphere points, flipped two-pass render and
-// the lambda blend.  It only sequences the stage kernels of this library on the caller's stream, from a caller-provided
-// workspace: no allocation, no host sync, ~20 (foreground) / ~40 (with background) launches issued back to back without
-// returning to the host language in between (the Python mirror spends 1.6-2.0 ms of interpreter time on the foreground alone).
+// mn_render_rays / mn_render_rays_bg: the inference path of render_rays (rendering.py:15-248, eval mode) as ONE C call.  Each
+// network is rendered by one two-pass routine, as the reference's _get_results (rendering.py:176-248): coarse query ->
+// composite -> inverse-CDF resampling -> fine query -> merge + volume rendering.  The foreground pass runs it on all rays; with
+// a background (NeRF++) network (rendering.py:34-62, 143-173) a sphere split comes first, the background pass runs it flipped
+// on the inverted-sphere points of the compacted background rays, and a lambda blend comes last.  The call only sequences the
+// stage kernels of this library on the caller's stream, from a caller-provided workspace: no allocation, no host sync, ~20
+// (foreground) / ~40 (with background) launches issued back to back without returning to the host language in between (the
+// Python mirror spends 1.6-2.0 ms of interpreter time on the foreground alone).
 //
 // The background rays are compacted on the device (stable: ascending ray order) and their count stays there: every kernel of
 // the background pass - stages, router, encoders, MLP tiles - skips rays / rows past it, while grids are sized for all N rays.
@@ -105,45 +107,66 @@ __global__ void bg_blend_kernel(float* __restrict__ val, const float* __restrict
     val[i] = __fadd_rn(v, add);
 }
 
+// Workspace offsets: each buffer aligned on its own.
+struct Carve {
+    size_t off = 0;
+    size_t operator()(size_t bytes) { const size_t o = off; off += mn_align(bytes); return o; }
+};
+
+constexpr size_t kNone = ~(size_t)0;   // offset of a buffer the pass does not use
+
+// The buffers of one two-pass render over N rays: S coarse samples, F fine draws, Sq samples of the fine query (F, or S + F
+// under cascade).  z_c / z_q hold the coarse / fine-query depths in sample order, from which the fine draws are resampled and
+// the points made.  z_c_comp / z_q_comp hold them as the composite reads them: the same buffers, or with flip (the background
+// pass) reversed copies of the coarse depths and, under cascade, of the fine-query depths.  With flip, dreal_c / dreal_f are
+// the real depths of the points outside the sphere.
+struct PassBufs {
+    int S, F, Sq, flip;
+    size_t z_c, z_c_comp, xyz_c, dreal_c, mlp_c, raw_c, w_c, z_f, z_q, z_q_comp, xyz_f, dreal_f, mlp_f, raw_f;
+    size_t model_ws_bytes;     // model workspace of the larger of the pass's two queries
+};
+
+// pt_cols: columns of the pass's points (3 for the foreground, up to 7 for the background).
+PassBufs carve_pass(Carve& take, const mn_model* net, int64_t N, int S, int F, int use_cascade, bool sh, int pt_cols, bool flip,
+                    int precision) {
+    PassBufs b{};
+    b.S = S; b.F = F; b.flip = flip;
+    b.Sq = F > 0 ? (use_cascade ? S + F : F) : 0;
+    const int Sc = S > 0 ? S : 1, Sq = b.Sq > 0 ? b.Sq : 1, out_cols = net->nd.rgb_dim + 1;
+    b.z_c = take((size_t)N * Sc * 4);
+    b.z_c_comp = flip ? take((size_t)N * Sc * 4) : b.z_c;
+    b.xyz_c = take((size_t)N * Sc * pt_cols * 4);
+    b.dreal_c = flip ? take((size_t)N * Sc * 4) : kNone;
+    b.mlp_c = sh ? take((size_t)N * Sc * out_cols * 4) : kNone;      // raw SH coefficients before the head
+    b.raw_c = take((size_t)N * Sc * 16);
+    b.w_c = take((size_t)N * Sc * 4);
+    b.z_f = take((size_t)N * (F > 0 ? F : 1) * 4);
+    b.z_q = use_cascade && F > 0 ? take((size_t)N * Sq * 4) : b.z_f;
+    b.z_q_comp = flip && use_cascade && F > 0 ? take((size_t)N * Sq * 4) : b.z_q;
+    b.xyz_f = take((size_t)N * Sq * pt_cols * 4);
+    b.dreal_f = flip ? take((size_t)N * Sq * 4) : kNone;
+    b.mlp_f = sh ? take((size_t)N * Sq * out_cols * 4) : kNone;
+    b.raw_f = take((size_t)N * Sq * 16);
+    const size_t a = mn_model_workspace_bytes(net, N * Sc, precision);
+    const size_t c = b.Sq > 0 ? mn_model_workspace_bytes(net, N * b.Sq, precision) : 0;
+    b.model_ws_bytes = a > c ? a : c;
+    return b;
+}
+
 struct RenderPlan {
-    int64_t N;
-    int Sc, Sf, Sq;            // coarse samples, fine draws, samples of the fine query (Sf, or Sc + Sf under cascade)
-    int out_cols;              // columns of the raw model output (rgb_dim + 1)
-    size_t z_c, xyz_c, mlp_c, raw_c, w_c, z_f, z_q, xyz_f, mlp_f, raw_f, last_delta, model_ws, total;
-    size_t model_ws_bytes;
-    // background pass: Sb coarse samples (Sc / 2), Fb fine draws (Sf / 2), Sqb samples of its fine query; every per-ray buffer
-    // holds N rays (the compacted background rays first)
-    int Sb, Fb, Sqb;
-    size_t far_ov, pos, blk, count, ids, dirs, idx, zb, zb_flip, xyz_b, dreal_b, mlp_b, raw_b, w_b, zf_b, zq_b, zq_b_flip, xyz_fb,
-        dreal_fb, mlp_fb, raw_fb, ld_b, rgb_b, depth_b, rgb_cb, lam, lam_c;
+    PassBufs fg, bg;
+    size_t last_delta, model_ws, model_ws_bytes, total;
+    // background split and blend; every per-ray buffer holds N rays (the compacted background rays first)
+    size_t far_ov, pos, blk, count, ids, dirs, idx, ld_b, rgb_b, depth_b, rgb_cb, lam, lam_c;
 };
 
 RenderPlan make_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, int sh, int precision) {
     RenderPlan p{};
-    p.N = N; p.Sc = Sc; p.Sf = Sf;
-    p.Sq = Sf > 0 ? (use_cascade ? Sc + Sf : Sf) : 0;
-    p.out_cols = m->nd.rgb_dim + 1;
-    size_t off = 0;
-    auto take = [&](size_t bytes) { size_t o = off; off += mn_align(bytes); return o; };
-    p.z_c = take((size_t)N * Sc * 4);
-    p.xyz_c = take((size_t)N * Sc * 12);
-    p.mlp_c = sh ? take((size_t)N * Sc * p.out_cols * 4) : 0;      // raw SH coefficients before the head
-    p.raw_c = take((size_t)N * Sc * 16);
-    p.w_c = take((size_t)N * Sc * 4);
-    p.z_f = take((size_t)N * (Sf > 0 ? Sf : 1) * 4);
-    p.z_q = use_cascade && Sf > 0 ? take((size_t)N * p.Sq * 4) : p.z_f;
-    p.xyz_f = take((size_t)N * (p.Sq > 0 ? p.Sq : 1) * 12);
-    p.mlp_f = sh ? take((size_t)N * (p.Sq > 0 ? p.Sq : 1) * p.out_cols * 4) : 0;
-    p.raw_f = take((size_t)N * (p.Sq > 0 ? p.Sq : 1) * 16);
+    Carve take;
+    p.fg = carve_pass(take, m, N, Sc, Sf, use_cascade, sh, 3, false, precision);
     p.last_delta = take((size_t)N * 4);
-    const size_t a = mn_model_workspace_bytes(m, N * Sc, precision);
-    const size_t b = p.Sq > 0 ? mn_model_workspace_bytes(m, N * p.Sq, precision) : 0;
-    p.model_ws_bytes = a > b ? a : b;
+    p.model_ws_bytes = p.fg.model_ws_bytes;
     if (bg) {
-        p.Sb = Sc / 2;
-        p.Fb = Sf / 2;
-        p.Sqb = p.Fb > 0 ? (use_cascade ? p.Sb + p.Fb : p.Fb) : 0;
-        const int Sb = p.Sb > 0 ? p.Sb : 1, Sqb = p.Sqb > 0 ? p.Sqb : 1, bcols = bg->nd.rgb_dim + 1;
         p.far_ov = take((size_t)N * 4);
         p.pos = take((size_t)N * 4);
         p.blk = take((size_t)mn_cdiv(N, kSplitBlock) * 4);
@@ -151,33 +174,18 @@ RenderPlan make_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, i
         p.ids = take((size_t)N * 8);
         p.dirs = take((size_t)N * 12);
         p.idx = take((size_t)N * 4);
-        p.zb = take((size_t)N * Sb * 4);
-        p.zb_flip = take((size_t)N * Sb * 4);
-        p.xyz_b = take((size_t)N * Sb * 28);                            // 7 columns with the real-xyz prefix, else 4
-        p.dreal_b = take((size_t)N * Sb * 4);
-        p.mlp_b = sh ? take((size_t)N * Sb * bcols * 4) : 0;
-        p.raw_b = take((size_t)N * Sb * 16);
-        p.w_b = take((size_t)N * Sb * 4);
-        p.zf_b = take((size_t)N * (p.Fb > 0 ? p.Fb : 1) * 4);
-        p.zq_b = use_cascade && p.Fb > 0 ? take((size_t)N * Sqb * 4) : p.zf_b;
-        p.zq_b_flip = use_cascade && p.Fb > 0 ? take((size_t)N * Sqb * 4) : 0;
-        p.xyz_fb = take((size_t)N * Sqb * 28);
-        p.dreal_fb = take((size_t)N * Sqb * 4);
-        p.mlp_fb = sh ? take((size_t)N * Sqb * bcols * 4) : 0;
-        p.raw_fb = take((size_t)N * Sqb * 16);
+        // half the samples (rendering.py:47-48); 7 point columns with the real-xyz prefix, else 4
+        p.bg = carve_pass(take, bg, N, Sc / 2, Sf / 2, use_cascade, sh, 7, true, precision);
         p.ld_b = take((size_t)N * 4);
         p.rgb_b = take((size_t)N * 12);
         p.depth_b = take((size_t)N * 4);
         p.rgb_cb = take((size_t)N * 12);
         p.lam = take((size_t)N * 4);
         p.lam_c = take((size_t)N * 4);
-        const size_t c = mn_model_workspace_bytes(bg, N * Sb, precision);
-        const size_t d = p.Sqb > 0 ? mn_model_workspace_bytes(bg, N * p.Sqb, precision) : 0;
-        if (c > p.model_ws_bytes) p.model_ws_bytes = c;
-        if (d > p.model_ws_bytes) p.model_ws_bytes = d;
+        if (p.bg.model_ws_bytes > p.model_ws_bytes) p.model_ws_bytes = p.bg.model_ws_bytes;
     }
     p.model_ws = take(p.model_ws_bytes);
-    p.total = off + 256;
+    p.total = take.off + 256;
     return p;
 }
 
@@ -219,19 +227,12 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
     const RenderPlan p = make_plan(m, bg, N, coarse_samples, fine_samples, use_cascade, sh, precision);
     if (!workspace_d || workspace_bytes < p.total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     char* W = (char*)workspace_d;
-    auto F = [&](size_t off) { return reinterpret_cast<float*>(W + off); };
+    auto F = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
     auto I = [&](size_t off) { return reinterpret_cast<int*>(W + off); };
     cudaStream_t st = (cudaStream_t)stream;
-    const int Sc = p.Sc, Sf = p.Sf, Sq = p.Sq;
-    const bool fine = Sf > 0;
-    const bool want_depth = o.depth || o.depth_var;
-    float* rgb_out_d = o.rgb;
-    float* depth_out_d = o.depth;
-    float* depth_var_out_d = o.depth_var;
-    float* rgb_coarse_out_d = o.rgb_coarse;
+    const bool fine = fine_samples > 0;
 
-    // one model query on [n, S, cols] points -> raw [n, S, 4]   (rendering.py:275-334).  dirs / idx: per ray; live: the rays
-    // that hold data (background pass) or all n.
+    // one model query on [N, S, cols] points -> raw [N, S, 4]   (rendering.py:275-334).  dirs / idx: per ray.
     auto query = [&](mn_model* net, const float* xyz, int cols, int S, int coarse, float* mlp_out, float* raw_out, const float* dirs,
                      int64_t dstride, const float* idx, const int* live) -> int {
         mn_rows rows{};
@@ -244,11 +245,42 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
         rows.samples_per_ray = S;
         float* out = sh ? mlp_out : raw_out;
         const LiveRows lr{live, S};
-        int r = live ? mn_model_forward_live(ctx, net, &rows, N * S, lr, coarse, precision, out, W + p.model_ws, p.model_ws_bytes, st)
-                     : mn_model_forward(ctx, net, &rows, N * S, coarse, 0, nullptr, precision, out, W + p.model_ws, p.model_ws_bytes, stream);
+        int r = mn_model_forward_live(ctx, net, &rows, N * S, lr, coarse, precision, out, W + p.model_ws, p.model_ws_bytes, st);
         if (r) return r;
         if (sh) return mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, net->nd.rgb_dim + 1, dirs, dstride, S, N * S, 1, lr, raw_out, st);
         return MN_OK;
+    };
+
+    // The two-pass render of one network (rendering.py:176-248, render.py `_two_pass`) from the coarse depths and points the
+    // caller wrote into b.z_c, b.z_c_comp, b.xyz_c and b.dreal_c.  live: the device count of the rays that hold data (background
+    // pass), or null for all N.  cols: point columns.  fine_points(z, S, flip_pts, xyz, dreal) makes the fine points from the
+    // fine-query depths (rendering.py `xyz_fine_fn`).  r: rgb, depth, depth_var and bg_lambda of the final type, rgb_coarse and
+    // bg_lambda_coarse of the cascade's coarse type (null: not wanted).
+    auto two_pass = [&](mn_model* net, const PassBufs& b, const int* live, int cols, const float* last_delta, const float* u_fine,
+                        const float* dirs, int64_t dstride, const float* idx, const mn_render_outputs& r, auto&& fine_points) -> int {
+        const LiveRows lr{live, 1};
+        // depth scratch when only the variance is wanted: the coarse weights are dead by the time it is written
+        float* depth = r.depth ? r.depth : (r.depth_var ? F(b.w_c) : nullptr);
+        int e;
+        if ((e = query(net, F(b.xyz_c), cols, b.S, 1, F(b.mlp_c), F(b.raw_c), dirs, dstride, idx, live))) return e;
+        if ((e = mn_stage_composite(ctx, F(b.raw_c), F(b.z_c_comp), F(b.dreal_c), b.S, nullptr, nullptr, nullptr, 0, last_delta, N,
+                                    b.flip, lr, fine ? F(b.w_c) : nullptr, use_cascade ? (fine ? r.rgb_coarse : r.rgb) : nullptr,
+                                    fine ? nullptr : depth, fine ? nullptr : r.depth_var,
+                                    use_cascade ? (fine ? r.bg_lambda_coarse : r.bg_lambda) : nullptr, st)))
+            return e;
+        if (!fine) return MN_OK;
+        // resampling from the bins of the depths in sample order, with the weights as composited (quirk Q7)
+        if ((e = mn_stage_sample_pdf(ctx, F(b.z_c), F(b.w_c), b.S, nullptr, u_fine, 0, N, b.S, b.F, lr, F(b.z_f), nullptr, nullptr, st)))
+            return e;
+        if (use_cascade)
+            if ((e = mn_stage_sort_cat(ctx, F(b.z_c), b.S, F(b.z_f), b.F, N, 0, lr, F(b.z_q), b.flip ? F(b.z_q_comp) : nullptr, st))) return e;
+        if ((e = fine_points(F(b.z_q), b.Sq, b.flip && use_cascade, F(b.xyz_f), F(b.dreal_f)))) return e;
+        if ((e = query(net, F(b.xyz_f), cols, b.Sq, 0, F(b.mlp_f), F(b.raw_f), dirs, dstride, idx, live))) return e;
+        if (use_cascade)
+            return mn_stage_composite(ctx, F(b.raw_f), F(b.z_q_comp), F(b.dreal_f), b.Sq, nullptr, nullptr, nullptr, 0, last_delta, N,
+                                      b.flip, lr, nullptr, r.rgb, depth, r.depth_var, r.bg_lambda, st);
+        return mn_stage_composite(ctx, F(b.raw_f), F(b.z_q_comp), F(b.dreal_f), b.Sq, F(b.raw_c), F(b.z_c_comp), F(b.dreal_c), b.S,
+                                  last_delta, N, b.flip, lr, nullptr, r.rgb, depth, r.depth_var, r.bg_lambda, st);
     };
 
     if (!bg) {
@@ -267,73 +299,36 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
         fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(F(p.ld_b), N, 1e10f);            // no bg_lambda in this pass
         MN_LAUNCH_CHECK(ctx);
 
-        // ---- background pass over the compacted rays (render.py:300-312 -> _two_pass with flip):  coarse depths from
-        // z_steps_bg; query and composite see them flipped, with the unflipped real depths (quirk of the reference)
+        // ---- background pass over the compacted rays (render.py:300-312): coarse depths from z_steps_bg, in sample order and
+        // reversed, and the points outside the sphere in reversed order
         const int* cnt = I(p.count);
         const LiveRows lr{cnt, 1};
         const int64_t* ids = reinterpret_cast<const int64_t*>(W + p.ids);
-        const int Sb = p.Sb, Fb = p.Fb, Sqb = p.Sqb, cols = include_xyz_real ? 7 : 4;
-        const bool bfine = Fb > 0;
-        if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, nullptr, 0.0f, N, Sb, 0, lr, F(p.zb), st))) return rc;
-        if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, nullptr, 0.0f, N, Sb, 1, lr, F(p.zb_flip), st))) return rc;
-        if ((rc = mn_stage_points_outside(ctx, rays_d, ids, F(p.zb), center_d, radius_d, N, Sb, include_xyz_real, cluster_2d, 1, lr,
-                                          F(p.xyz_b), F(p.dreal_b), st)))
-            return rc;
-        if ((rc = query(bg, F(p.xyz_b), cols, Sb, 1, F(p.mlp_b), F(p.raw_b), F(p.dirs), 3, bidx, cnt))) return rc;
-        if ((rc = mn_stage_composite(ctx, F(p.raw_b), F(p.zb_flip), F(p.dreal_b), Sb, nullptr, nullptr, nullptr, 0, F(p.ld_b), N, 1, lr,
-                                     bfine ? F(p.w_b) : nullptr, use_cascade ? (bfine ? F(p.rgb_cb) : F(p.rgb_b)) : nullptr,
-                                     (!bfine && depth_out_d) ? F(p.depth_b) : nullptr, nullptr, nullptr, st)))
-            return rc;
-        if (bfine) {
-            // resampling from the unflipped bins with the weights in flipped order (quirk Q7), then points outside the sphere
-            if ((rc = mn_stage_sample_pdf(ctx, F(p.zb), F(p.w_b), Sb, nullptr, u_fine_bg_d, 0, N, Sb, Fb, lr, F(p.zf_b), nullptr, nullptr, st))) return rc;
-            if (use_cascade)
-                if ((rc = mn_stage_sort_cat(ctx, F(p.zb), Sb, F(p.zf_b), Fb, N, 0, lr, F(p.zq_b), F(p.zq_b_flip), st))) return rc;
-            if ((rc = mn_stage_points_outside(ctx, rays_d, ids, F(p.zq_b), center_d, radius_d, N, Sqb, include_xyz_real, cluster_2d,
-                                              use_cascade ? 1 : 0, lr, F(p.xyz_fb), F(p.dreal_fb), st)))
-                return rc;
-            if ((rc = query(bg, F(p.xyz_fb), cols, Sqb, 0, F(p.mlp_fb), F(p.raw_fb), F(p.dirs), 3, bidx, cnt))) return rc;
-            float* bdepth = depth_out_d ? F(p.depth_b) : nullptr;
-            if (use_cascade)
-                rc = mn_stage_composite(ctx, F(p.raw_fb), F(p.zq_b_flip), F(p.dreal_fb), Sqb, nullptr, nullptr, nullptr, 0, F(p.ld_b), N,
-                                        1, lr, nullptr, F(p.rgb_b), bdepth, nullptr, nullptr, st);
-            else
-                rc = mn_stage_composite(ctx, F(p.raw_fb), F(p.zf_b), F(p.dreal_fb), Fb, F(p.raw_b), F(p.zb_flip), F(p.dreal_b), Sb,
-                                        F(p.ld_b), N, 1, lr, nullptr, F(p.rgb_b), bdepth, nullptr, nullptr, st);
-            if (rc) return rc;
-        }
+        const PassBufs& b = p.bg;
+        auto outside = [&](const float* z, int S, int flip_pts, float* xyz, float* dreal) {
+            return mn_stage_points_outside(ctx, rays_d, ids, z, center_d, radius_d, N, S, include_xyz_real, cluster_2d, flip_pts, lr,
+                                           xyz, dreal, st);
+        };
+        if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, nullptr, 0.0f, N, b.S, 0, lr, F(b.z_c), st))) return rc;
+        if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, nullptr, 0.0f, N, b.S, 1, lr, F(b.z_c_comp), st))) return rc;
+        if ((rc = outside(F(b.z_c), b.S, 1, F(b.xyz_c), F(b.dreal_c)))) return rc;
+        mn_render_outputs bo{};
+        bo.rgb = F(p.rgb_b);
+        bo.depth = o.depth ? F(p.depth_b) : nullptr;
+        bo.rgb_coarse = F(p.rgb_cb);
+        if ((rc = two_pass(bg, b, cnt, include_xyz_real ? 7 : 4, F(p.ld_b), u_fine_bg_d, F(p.dirs), 3, bidx, bo, outside))) return rc;
     }
-    const float* far_ov = bg ? F(p.far_ov) : nullptr;
-    // bg_lambda of the final type and of the cascade's coarse type (render.py:317: requested iff there is a background)
-    float* lam = bg ? (o.bg_lambda ? o.bg_lambda : F(p.lam)) : nullptr;
-    float* lam_c = (bg && use_cascade && fine) ? (o.bg_lambda_coarse ? o.bg_lambda_coarse : F(p.lam_c)) : nullptr;
 
-    // ---- coarse pass (rendering.py:82-87, 190-205)
-    if ((rc = mn_sample_coarse(ctx, rays_d, far_ov, z_steps_d, nullptr, 0.0f, N, Sc, F(p.z_c), F(p.xyz_c), stream))) return rc;
-    if ((rc = query(m, F(p.xyz_c), 3, Sc, 1, F(p.mlp_c), F(p.raw_c), rays_d + 3, 8, image_indices_d, nullptr))) return rc;
-    if ((rc = mn_composite(ctx, F(p.raw_c), F(p.z_c), nullptr, Sc, nullptr, nullptr, nullptr, 0, F(p.last_delta), N, 0,
-                           fine ? F(p.w_c) : nullptr, use_cascade ? (fine ? rgb_coarse_out_d : rgb_out_d) : nullptr,
-                           (!fine && want_depth) ? (depth_out_d ? depth_out_d : F(p.w_c)) : nullptr,
-                           !fine ? depth_var_out_d : nullptr, use_cascade ? (fine ? lam_c : lam) : nullptr, stream)))
+    // ---- foreground pass (rendering.py:82-87, 176-248); bg_lambda of the final type and of the cascade's coarse type
+    // (render.py:317: requested iff there is a background)
+    mn_render_outputs fo = o;
+    fo.bg_lambda = bg ? (o.bg_lambda ? o.bg_lambda : F(p.lam)) : nullptr;
+    fo.bg_lambda_coarse = (bg && use_cascade && fine) ? (o.bg_lambda_coarse ? o.bg_lambda_coarse : F(p.lam_c)) : nullptr;
+    if ((rc = mn_sample_coarse(ctx, rays_d, bg ? F(p.far_ov) : nullptr, z_steps_d, nullptr, 0.0f, N, p.fg.S, F(p.fg.z_c),
+                               F(p.fg.xyz_c), stream)))
         return rc;
-
-    if (fine) {
-        // ---- resample (rendering.py:207-223) and fine pass (:224-243)
-        if ((rc = mn_sample_pdf(ctx, F(p.z_c), F(p.w_c), Sc, nullptr, u_fine_d, 0, N, Sc, Sf, F(p.z_f), nullptr, nullptr, stream))) return rc;
-        if (use_cascade)
-            if ((rc = mn_sort_cat(ctx, F(p.z_c), Sc, F(p.z_f), Sf, N, 0, F(p.z_q), stream))) return rc;
-        if ((rc = mn_points_from_z(ctx, rays_d, F(p.z_q), N, Sq, F(p.xyz_f), stream))) return rc;
-        if ((rc = query(m, F(p.xyz_f), 3, Sq, 0, F(p.mlp_f), F(p.raw_f), rays_d + 3, 8, image_indices_d, nullptr))) return rc;
-        // depth scratch when only the variance is wanted: the coarse weights are dead by now
-        float* depth_dst = want_depth ? (depth_out_d ? depth_out_d : F(p.w_c)) : nullptr;
-        if (use_cascade)
-            rc = mn_composite(ctx, F(p.raw_f), F(p.z_q), nullptr, Sq, nullptr, nullptr, nullptr, 0, F(p.last_delta), N, 0, nullptr,
-                              rgb_out_d, depth_dst, depth_var_out_d, lam, stream);
-        else
-            rc = mn_composite(ctx, F(p.raw_f), F(p.z_f), nullptr, Sf, F(p.raw_c), F(p.z_c), nullptr, Sc, F(p.last_delta), N, 0, nullptr,
-                              rgb_out_d, depth_dst, depth_var_out_d, lam, stream);
-        if (rc) return rc;
-    }
+    auto from_z = [&](const float* z, int S, int, float* xyz, float*) { return mn_points_from_z(ctx, rays_d, z, N, S, xyz, stream); };
+    if ((rc = two_pass(m, p.fg, nullptr, 3, F(p.last_delta), u_fine_d, rays_d + 3, 8, image_indices_d, fo, from_z))) return rc;
     if (!bg) return MN_OK;
 
     // ---- blend (render.py:320-340): the final type's rgb / depth, and rgb_coarse under cascade with fine samples
@@ -342,11 +337,11 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
         MN_LAUNCH_CHECK(ctx);
         return MN_OK;
     };
-    if ((rc = blend(rgb_out_d, F(p.rgb_b), lam, 3, o.fg_rgb, o.bg_rgb))) return rc;
-    if (depth_out_d)
-        if ((rc = blend(depth_out_d, F(p.depth_b), lam, 1, o.fg_depth, o.bg_depth))) return rc;
-    if (use_cascade && fine && rgb_coarse_out_d)
-        if ((rc = blend(rgb_coarse_out_d, F(p.rgb_cb), lam_c, 3, o.fg_rgb_coarse, o.bg_rgb_coarse))) return rc;
+    if ((rc = blend(o.rgb, F(p.rgb_b), fo.bg_lambda, 3, o.fg_rgb, o.bg_rgb))) return rc;
+    if (o.depth)
+        if ((rc = blend(o.depth, F(p.depth_b), fo.bg_lambda, 1, o.fg_depth, o.bg_depth))) return rc;
+    if (use_cascade && fine && o.rgb_coarse)
+        if ((rc = blend(o.rgb_coarse, F(p.rgb_cb), fo.bg_lambda_coarse, 3, o.fg_rgb_coarse, o.bg_rgb_coarse))) return rc;
     return MN_OK;
 }
 

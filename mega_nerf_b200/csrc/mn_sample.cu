@@ -927,8 +927,8 @@ int mn_embed(mn_ctx* ctx, const float* x_d, int64_t B, int dim, int n_freqs, flo
 
 }  // extern "C"
 
-// ---- the one launch of each stage kernel (mn_model.cuh): the public entry points above validate and call these; the background
-// pass of mn_render_rays_bg calls them with its device ray count and sample-order options ----
+// ---- the one launch of each stage kernel (mn_model.cuh): the public entry points above validate and call these; the render
+// passes of mn_render_rays(_bg) call them directly, the background pass with its device ray count and sample-order options ----
 int mn_stage_stratify(mn_ctx* ctx, const float* z_d, int64_t z_row_stride, const float* rand_d, float perturb, int64_t N, int S, int flip,
                       LiveRows live, float* z_out_d, cudaStream_t st) {
     stratify_kernel<<<(unsigned)mn_cdiv(N * S, 256), 256, 0, st>>>(z_d, z_row_stride, rand_d, perturb, N, S, z_out_d, live, flip);

@@ -23,7 +23,7 @@ import torch
 from torch import nn
 
 from . import _cabi as K
-from .render import render_rays, render_rays_fused
+from .render import _unwrap, render_rays, render_rays_fused
 
 
 class GraphedRenderRays:
@@ -50,8 +50,7 @@ class GraphedRenderRays:
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.results: Optional[Dict[str, torch.Tensor]] = None
         self.warmup = warmup
-        unwrap = lambda m: m.module if hasattr(m, 'module') and not hasattr(m, '_native') else m
-        self._natives = [unwrap(m)._native() for m in (nerf, bg_nerf) if m is not None]
+        self._natives = [_unwrap(m)._native() for m in (nerf, bg_nerf) if m is not None]
         self._params = [p for nat in self._natives for sub in nat.subs for p in sub.parameters()]
         self._versions = -1
 

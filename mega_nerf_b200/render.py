@@ -30,6 +30,14 @@ def _unwrap(m: Optional[nn.Module]):
     return m.module if hasattr(m, 'module') and not isinstance(m, (NeRF, MegaNeRF, Cascade)) else m
 
 
+def _nets(nerf: nn.Module, bg_nerf: Optional[nn.Module], fn: str):
+    """The library modules inside `nerf` / `bg_nerf` (e.g. under DistributedDataParallel); fn names the caller."""
+    net, bg = _unwrap(nerf), _unwrap(bg_nerf)
+    if not isinstance(net, (NeRF, MegaNeRF, Cascade)) or (bg is not None and not isinstance(bg, (NeRF, MegaNeRF, Cascade))):
+        raise TypeError(f'mega_nerf_b200.{fn} needs mega_nerf_b200 modules (use get_nerf / install())')
+    return net, bg
+
+
 class _Stage:
     """Thin typed wrappers over the stage entry points, bound to one device/stream."""
 
@@ -256,10 +264,7 @@ def render_rays(nerf: nn.Module,
                 get_depth: bool,
                 get_depth_variance: bool,
                 get_bg_fg_rgb: bool) -> Tuple[Dict[str, torch.Tensor], bool]:
-    net = _unwrap(nerf)
-    bg = _unwrap(bg_nerf)
-    if not isinstance(net, (NeRF, MegaNeRF, Cascade)) or (bg is not None and not isinstance(bg, (NeRF, MegaNeRF, Cascade))):
-        raise TypeError('mega_nerf_b200.render_rays needs mega_nerf_b200 modules (use get_nerf / install())')
+    net, bg = _nets(nerf, bg_nerf, 'render_rays')
     recording = net._native().needs_grad() or (bg is not None and bg._native().needs_grad())
     if recording:
         # training step (runner.py:346-358): queries and compositing are recorded, see mega_nerf_b200/autograd.py
@@ -289,27 +294,29 @@ def _render(net, bg, rays, image_indices, hparams, sphere_center, sphere_radius,
     center = K.f32c(sphere_center.to(dev)) if sphere_center is not None else None
     radius = K.f32c(sphere_radius.to(dev)) if sphere_radius is not None else None
 
+    def bg_pass(ids, last, real):
+        """The background network's render of the rays `ids` (rendering.py:44-72): half the coarse samples, the points outside
+        the sphere, flipped two-pass render.  last: the last delta of every ray; real: whether the points carry the real-xyz
+        prefix."""
+        n, half = ids.shape[0], S // 2
+        bz1 = torch.linspace(0, 1, half, device=dev)
+        rnd = torch.rand(n, half, device=dev) if perturb > 0 else None
+        bz = sg.stratify(bz1, rnd, perturb, n, half)
+        c2d = real and net.cluster_dim_start == 1
+        mk = lambda zz: sg.points_outside(rays, ids, zz, center, radius, real, c2d)
+        bpts, breal = mk(bz)
+        return _two_pass(sg, bg, hparams, rays[ids][:, 3:6], idx[ids].contiguous() if idx is not None else None, bpts, bz,
+                         torch.full((n,), last, device=dev, dtype=torch.float32), get_depth, get_depth_variance,
+                         False, True, breal, mk, call_bg)
+
     if bg is not None:
         fg_far = sg.intersect_sphere(rays, center, radius)
         fg_far = torch.maximum(fg_far, rays[:, 6])
         with_bg = torch.arange(N, device=dev)[rays[:, 7] > fg_far]          # host sync, as in the reference (:37)
-        nb = with_bg.shape[0]
-        if nb > 0:
+        if with_bg.shape[0] > 0:
             last_delta[with_bg] = fg_far[with_bg]
             far_override = torch.minimum(rays[:, 7], fg_far)
-            half = S // 2
-            bz1 = torch.linspace(0, 1, half, device=dev)
-            rnd = torch.rand(nb, half, device=dev) if perturb > 0 else None
-            bz = sg.stratify(bz1, rnd, perturb, nb, half)
-            real = hparams.container_path is not None or hparams.train_mega_nerf is not None
-            c2d = real and net.cluster_dim_start == 1
-            mk = lambda zz: sg.points_outside(rays, with_bg, zz, center, radius, real, c2d)
-            bpts, breal = mk(bz)
-            bg_dirs = rays[with_bg][:, 3:6]
-            bg_idx = idx[with_bg].contiguous() if idx is not None else None
-            bg_res = _two_pass(sg, bg, hparams, bg_dirs, bg_idx, bpts, bz,
-                               torch.full((nb,), 1e10, device=dev, dtype=torch.float32), get_depth,
-                               get_depth_variance, False, True, breal, mk, call_bg)
+            bg_res = bg_pass(with_bg, 1e10, hparams.container_path is not None or hparams.train_mega_nerf is not None)
 
     steps = torch.linspace(0, 1, S, device=dev)
     rnd = torch.rand(N, S, device=dev) if perturb > 0 else None
@@ -344,19 +351,9 @@ def _render(net, bg, rays, image_indices, hparams, sphere_center, sphere_radius,
         # dummy background ray through bg_nerf - i.e. through its DistributedDataParallel wrapper, whose forward is
         # what arms the gradient reducer for this iteration - and adds 0 x its colour, so that this rank joins the
         # bg all-reduce with all-zero gradients and the optimiser steps on every rank.  Same here, through `call_bg`;
-        # the random draws (jitter, density noise, resampling) are consumed in the reference's order.
-        half = S // 2
-        bz1 = torch.linspace(0, 1, half, device=dev)
-        rnd = torch.rand(1, half, device=dev) if perturb > 0 else None
-        bz = sg.stratify(bz1, rnd, perturb, 1, half)
-        real = hparams.train_mega_nerf is not None                       # rendering.py:147 (no container_path here)
-        c2d = real and net.cluster_dim_start == 1
-        first = torch.zeros(1, device=dev, dtype=with_bg.dtype)
-        mk = lambda zz: sg.points_outside(rays, first, zz, center, radius, real, c2d)
-        bpts, breal = mk(bz)
-        dummy = _two_pass(sg, bg, hparams, rays[:1, 3:6], idx[:1].contiguous() if idx is not None else None, bpts, bz,
-                          torch.ones(1, device=dev, dtype=torch.float32), get_depth, get_depth_variance, False, True,
-                          breal, mk, call_bg)
+        # the random draws (jitter, density noise, resampling) are consumed in the reference's order.  Its points carry the
+        # real-xyz prefix by train_mega_nerf alone (rendering.py:147: no container_path here).
+        dummy = bg_pass(with_bg.new_zeros(1), 1.0, hparams.train_mega_nerf is not None)
         key = f'rgb_{"fine" if hparams.fine_samples > 0 else "coarse"}'
         # `results[key][:0] += 0 * grad_results[key]`: an EMPTY slice - the values never mix (a non-finite dummy colour
         # cannot poison the batch), only the graph edge to the bg parameters is added
@@ -376,10 +373,7 @@ def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
     With a background network the split of the rays happens on the device (no host sync per chunk); the one sync is the
     status check at the end, where the reference checks its sphere bound too: a camera outside the ellipsoid raises its
     `Exception`.  `check_status=False` leaves that check to the caller (CUDA-graph capture, where no sync may happen)."""
-    net = _unwrap(nerf)
-    bg = _unwrap(bg_nerf)
-    if not isinstance(net, (NeRF, MegaNeRF, Cascade)) or (bg is not None and not isinstance(bg, (NeRF, MegaNeRF, Cascade))):
-        raise TypeError('mega_nerf_b200.render_rays_fused needs mega_nerf_b200 modules (use get_nerf / install())')
+    net, bg = _nets(nerf, bg_nerf, 'render_rays_fused')
     if net.training or (bg is not None and bg.training):
         raise ValueError('render_rays_fused is the inference path; call nerf.eval() first')
     if bool(hparams.use_cascade) != isinstance(net, Cascade):
@@ -399,24 +393,38 @@ def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
     steps = torch.linspace(0, 1, Sc, device=dev)
     u = torch.linspace(0, 1, Sf, device=dev) if Sf > 0 else None
     typ = 'fine' if Sf > 0 else 'coarse'
+    coarse = cascade and Sf > 0                               # the cascade's coarse results too
     new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
-    rgb = new(N, 3)
-    depth = new(N) if get_depth else None
-    var = new(N) if get_depth_variance else None
-    rgb_c = new(N, 3) if (cascade and Sf > 0) else None
+    res = {f'rgb_{typ}': new(N, 3)}
+    if get_depth:
+        res[f'depth_{typ}'] = new(N)
+    if get_depth_variance:
+        res[f'depth_variance_{typ}'] = new(N)
+    if bg is not None:
+        res[f'bg_lambda_{typ}'] = new(N)
+    if coarse:
+        res['rgb_coarse'] = new(N, 3)
+        if bg is not None:
+            res['bg_lambda_coarse'] = new(N)
+    if bg is not None and get_bg_fg_rgb:
+        for name in [f'{key}_{t}' for key in TO_COMPOSITE for t in ((typ, 'coarse') if coarse else (typ,))]:
+            if name in res:
+                res[f'fg_{name}'], res[f'bg_{name}'] = torch.empty_like(res[name]), torch.empty_like(res[name])
+    out = K.RenderOutputs()
+    for field, key in (('rgb', f'rgb_{typ}'), ('depth', f'depth_{typ}'), ('depth_var', f'depth_variance_{typ}'),
+                       ('bg_lambda', f'bg_lambda_{typ}'), ('fg_rgb', f'fg_rgb_{typ}'), ('bg_rgb', f'bg_rgb_{typ}'),
+                       ('fg_depth', f'fg_depth_{typ}'), ('bg_depth', f'bg_depth_{typ}'), ('rgb_coarse', 'rgb_coarse'),
+                       ('bg_lambda_coarse', 'bg_lambda_coarse'), ('fg_rgb_coarse', 'fg_rgb_coarse'),
+                       ('bg_rgb_coarse', 'bg_rgb_coarse')):
+        if typ == 'coarse' and field.endswith('_coarse'):
+            continue                                       # coarse-only render: the final type is the coarse one
+        setattr(out, field, K.ptr(res.get(key)))
+    st = K.stream_of(dev)
     if bg is None:
         nbytes = int(L.mn_render_rays_workspace_bytes(native.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
         ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
         K.check(L.mn_render_rays(h, native.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(steps), Sc, K.ptr(u), Sf, int(cascade),
-                                 sh_deg, prec, K.ptr(rgb), K.ptr(depth), K.ptr(var), K.ptr(rgb_c), K.ptr(ws), ws.numel(),
-                                 K.stream_of(dev)), h)
-        res = {f'rgb_{typ}': rgb}
-        if depth is not None:
-            res[f'depth_{typ}'] = depth
-        if var is not None:
-            res[f'depth_variance_{typ}'] = var
-        if rgb_c is not None:
-            res['rgb_coarse'] = rgb_c
+                                 sh_deg, prec, out.rgb, out.depth, out.depth_var, out.rgb_coarse, K.ptr(ws), ws.numel(), st), h)
         return res
 
     bnative = bg._native()
@@ -427,33 +435,8 @@ def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
     c2d = real and getattr(net, 'cluster_dim_start', 0) == 1                          # render.py:304-305
     steps_bg = torch.linspace(0, 1, Sc // 2, device=dev)
     u_bg = torch.linspace(0, 1, Sf // 2, device=dev) if Sf > 0 else None
-    res = {f'rgb_{typ}': rgb}
-    if depth is not None:
-        res[f'depth_{typ}'] = depth
-    if var is not None:
-        res[f'depth_variance_{typ}'] = var
-    res[f'bg_lambda_{typ}'] = new(N)
-    if rgb_c is not None:
-        res['rgb_coarse'] = rgb_c
-        res['bg_lambda_coarse'] = new(N)
-    if get_bg_fg_rgb:
-        for key, cols in (('rgb', 3), ('depth', 1)):
-            for t in ([typ, 'coarse'] if rgb_c is not None else [typ]):
-                if f'{key}_{t}' in res:
-                    res[f'fg_{key}_{t}'] = new(N, 3) if cols == 3 else new(N)
-                    res[f'bg_{key}_{t}'] = new(N, 3) if cols == 3 else new(N)
-    out = K.RenderOutputs()
-    for field, key in (('rgb', f'rgb_{typ}'), ('depth', f'depth_{typ}'), ('depth_var', f'depth_variance_{typ}'),
-                       ('bg_lambda', f'bg_lambda_{typ}'), ('fg_rgb', f'fg_rgb_{typ}'), ('bg_rgb', f'bg_rgb_{typ}'),
-                       ('fg_depth', f'fg_depth_{typ}'), ('bg_depth', f'bg_depth_{typ}'), ('rgb_coarse', 'rgb_coarse'),
-                       ('bg_lambda_coarse', 'bg_lambda_coarse'), ('fg_rgb_coarse', 'fg_rgb_coarse'),
-                       ('bg_rgb_coarse', 'bg_rgb_coarse')):
-        if typ == 'coarse' and field.endswith('_coarse'):
-            continue                                       # coarse-only render: the final type is the coarse one
-        setattr(out, field, K.ptr(res.get(key)))
     nbytes = int(L.mn_render_rays_bg_workspace_bytes(native.handle, bnative.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
     ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
-    st = K.stream_of(dev)
     K.check(L.mn_render_rays_bg(h, native.handle, bnative.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(center), K.ptr(radius),
                                 int(real), int(c2d), K.ptr(steps), K.ptr(steps_bg), Sc, K.ptr(u), K.ptr(u_bg), Sf, int(cascade),
                                 sh_deg, prec, C.byref(out), K.ptr(ws), ws.numel(), st), h)
