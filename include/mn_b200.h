@@ -207,6 +207,20 @@ int mn_model_forward(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, i
  * weights_out_d [B,n_sub] (margin>1). */
 int mn_model_route(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int32_t* assign_out_d,
                    float* weights_out_d, void* stream);
+/* Density grid of octree extraction (scripts/create_octree.py:61-105 _auto_scale, :139-162 _step1): sigma_out_d[r - row0] is
+ * nerf(x_r, sigma_only=True) (Cascade: nerf(use_coarse, x_r, ...)) for every lattice row r in [row0, row0 + n_rows) of the
+ * reso^3 lattice torch.stack(torch.meshgrid(xx, yy, zz)).reshape(3, -1).T, i.e. r = (i * reso + j) * reso + k (x slowest) and
+ * x_r = (((i, j, k) + 0.5) / reso - offset) / scale per axis in fp32, bit-identical to torch's CPU lattice.  The range runs
+ * through slabs of a fixed row count - lattice points into the workspace, then the mn_model_forward kernels (sigma_only,
+ * `precision`) - on `stream`, with no allocation and no host sync; the workspace size does not depend on reso or n_rows.
+ * Routing slots are sized for every sub-module per row (a dense box reaches past the centroid hull), for this call only.
+ * As with any model call, a tail slab of <= 25 rows routes through cdist's direct path (mn_model_route).
+ *   reso 1 .. 2097151; scale > 0 on every axis; the range inside reso^3 (else MN_ERR_INVALID); models whose rows are not plain
+ *   xyz (xyz_dim != 3, or a real-xyz routing prefix) return MN_ERR_UNSUPPORTED. */
+size_t mn_model_density_grid_workspace_bytes(const mn_model* m, int precision);
+int mn_model_density_grid(mn_ctx* ctx, mn_model* m, int use_coarse, const float offset[3], const float scale[3], int reso,
+                          int64_t row0, int64_t n_rows, int precision, float* sigma_out_d, void* workspace_d,
+                          size_t workspace_bytes, void* stream);
 /* Counters of the last mn_model_forward on this model, read back lazily (synchronises `stream`):
  * slots = routed (row, sub-module) pairs, tiles = 128-row MLP tiles. */
 int mn_model_last_stats(mn_ctx* ctx, mn_model* m, int64_t* slots, int64_t* tiles, void* stream);

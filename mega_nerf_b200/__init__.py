@@ -11,4 +11,5 @@ from .raygen import get_ray_directions, get_rays, get_rays_batch  # noqa: F401
 from .sh import eval_sh  # noqa: F401
 from .install import install  # noqa: F401
 from . import cluster_masks  # noqa: F401
+from . import octree  # noqa: F401
 from . import expert_parallel  # noqa: F401

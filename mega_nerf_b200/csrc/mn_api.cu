@@ -373,14 +373,14 @@ int mn_model_set_weights(mn_model* m, int sub, const mn_nerf_weights* w, void* s
     return mn_pack_flush(ctx, st);
 }
 
-static int64_t slot_capacity(const mn_model* m, int64_t B) {
+// mult: sub-modules per row the slots are sized for; 0 = the model's max_multiplicity
+static int64_t slot_capacity(const mn_model* m, int64_t B, int mult = 0) {
     if (m->d.kind != 2) return mn_cdiv(B, MN_BUCKET) * MN_BUCKET;
-    return mn_cdiv(B * m->max_multiplicity, MN_BUCKET) * MN_BUCKET + (int64_t)m->d.n_sub * MN_BUCKET;
+    return mn_cdiv(B * (mult > 0 ? mult : m->max_multiplicity), MN_BUCKET) * MN_BUCKET + (int64_t)m->d.n_sub * MN_BUCKET;
 }
 
-size_t mn_model_workspace_bytes(const mn_model* m, int64_t B, int precision) {
-    if (!m) return 0;
-    const int64_t cap = slot_capacity(m, B);
+static size_t forward_workspace_bytes(const mn_model* m, int64_t B, int precision, int mult) {
+    const int64_t cap = slot_capacity(m, B, mult);
     size_t bytes = 256;
     if (m->d.kind == 2) {
         bytes += mn_align((size_t)cap * sizeof(int));                                       // slot_row
@@ -393,6 +393,10 @@ size_t mn_model_workspace_bytes(const mn_model* m, int64_t B, int precision) {
     }
     if (precision != MN_PREC_FP32) bytes += mn_mlp_tc_workspace(m, cap / MN_TILE, precision);
     return bytes;
+}
+
+size_t mn_model_workspace_bytes(const mn_model* m, int64_t B, int precision) {
+    return m ? forward_workspace_bytes(m, B, precision, 0) : 0;
 }
 
 // Tape header: the routing counters of THIS forward call (the model's own counters are overwritten by the next call).
@@ -439,10 +443,11 @@ static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, Ta
 
 // train_tc != 0: recording forward on the tensor cores (precision tc_f16) into the tensor-core tape regions.
 // live: the rows that hold data when their count lives on the device (inference only), see LiveRows.
+// mult: sub-modules per row the routing slots of this call are sized for (inference only; 0 = the model's max_multiplicity).
 static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, int sigma_only,
                               const float* sigma_noise_d, int precision, float* out_d, void* workspace_d,
                               size_t workspace_bytes, void* tape_d, size_t tape_bytes, void* stream, int train_tc = 0,
-                              LiveRows live = LiveRows{}) {
+                              LiveRows live = LiveRows{}, int mult = 0) {
     if (!ctx || !m || !rows || B < 0) return MN_ERR_INVALID;
     const mn_model_desc& d = m->d;
     const NetDims& nd = m->nd;
@@ -507,8 +512,8 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
     a.out_cols = sigma_only ? 1 : nd.rgb_dim + 1;
     a.live = live;
 
-    const int64_t cap = slot_capacity(m, B);
-    const size_t need = mn_model_workspace_bytes(m, B, precision);
+    const int64_t cap = slot_capacity(m, B, mult);
+    const size_t need = forward_workspace_bytes(m, B, precision, mult);
     if (need > 256 && (!workspace_d || workspace_bytes < need))
         return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward: workspace too small");
     char* ws = (char*)workspace_d;
@@ -583,7 +588,79 @@ int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t
                               0, live);
 }
 
+// ---- density grid (scripts/create_octree.py:61-105, 139-162) -------------------------------------------------------
+// Rows per slab: a multiple of the reference's 32768-row model_chunk_size, large enough that each slab fills the GPU.
+#define MN_GRID_SLAB (1 << 18)
+// Largest lattice edge: reso^3 rows fit int64_t and every lattice index converts to fp32 exactly.
+#define MN_GRID_MAX_RESO 2097151
+
+namespace {
+
+// xyz [n, 3] of lattice rows r0 .. r0 + n - 1: row r = (i * reso + j) * reso + k, point a = ((idx_a + 0.5) / reso - offset_a) / scale_a,
+// each operation one IEEE fp32 rounding, as torch evaluates arange / meshgrid on the CPU (create_octree.py:71-76).
+__global__ void __launch_bounds__(256) lattice_kernel(int64_t r0, int64_t n, int reso, float ox, float oy, float oz, float sx,
+                                                      float sy, float sz, float* __restrict__ xyz) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const int64_t r = r0 + t;
+    const int64_t rr = reso;
+    const float fr = (float)reso;
+    const int i = (int)(r / (rr * rr)), j = (int)((r / rr) % rr), k = (int)(r % rr);
+    xyz[t * 3 + 0] = (((float)i + 0.5f) / fr - ox) / sx;
+    xyz[t * 3 + 1] = (((float)j + 0.5f) / fr - oy) / sy;
+    xyz[t * 3 + 2] = (((float)k + 0.5f) / fr - oz) / sz;
+}
+
+}  // namespace
+
 extern "C" {
+
+size_t mn_model_density_grid_workspace_bytes(const mn_model* m, int precision) {
+    if (!m) return 0;
+    return mn_align((size_t)MN_GRID_SLAB * 3 * sizeof(float)) + forward_workspace_bytes(m, MN_GRID_SLAB, precision, m->d.n_sub);
+}
+
+int mn_model_density_grid(mn_ctx* ctx, mn_model* m, int use_coarse, const float offset[3], const float scale[3], int reso,
+                          int64_t row0, int64_t n_rows, int precision, float* sigma_out_d, void* workspace_d,
+                          size_t workspace_bytes, void* stream) {
+    if (!ctx || !m || !offset || !scale) return MN_ERR_INVALID;
+    if (reso < 1 || reso > MN_GRID_MAX_RESO)
+        return mn_fail(ctx, MN_ERR_INVALID, "mn_model_density_grid: reso " + std::to_string(reso) + " outside 1.." +
+                                                std::to_string(MN_GRID_MAX_RESO));
+    for (int a = 0; a < 3; ++a)
+        if (!(scale[a] > 0.0f && scale[a] < INFINITY))
+            return mn_fail(ctx, MN_ERR_INVALID, "mn_model_density_grid: scale must be positive and finite on every axis");
+    const int64_t total = (int64_t)reso * reso * reso;
+    if (row0 < 0 || n_rows < 0 || row0 > total || n_rows > total - row0)
+        return mn_fail(ctx, MN_ERR_INVALID, "mn_model_density_grid: rows [" + std::to_string(row0) + ", " + std::to_string(row0) + " + " +
+                                                std::to_string(n_rows) + ") outside the " + std::to_string(total) + "-row lattice");
+    if (m->d.xyz_dim != 3 || (m->d.kind == 2 && m->d.xyz_real))
+        return mn_fail(ctx, MN_ERR_UNSUPPORTED,
+                       "mn_model_density_grid: the model's rows are not plain xyz (xyz_dim != 3 or a real-xyz routing prefix)");
+    if (n_rows == 0) return MN_OK;
+    if (!sigma_out_d) return MN_ERR_INVALID;
+    if (!workspace_d || workspace_bytes < mn_model_density_grid_workspace_bytes(m, precision))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_density_grid: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    float* pts = (float*)workspace_d;
+    const size_t pts_bytes = mn_align((size_t)MN_GRID_SLAB * 3 * sizeof(float));
+    mn_rows rows{};
+    rows.mode = 0;
+    rows.x_d = pts;
+    rows.cols = 3;
+    for (int64_t s = 0; s < n_rows; s += MN_GRID_SLAB) {
+        const int64_t n = n_rows - s < MN_GRID_SLAB ? n_rows - s : MN_GRID_SLAB;
+        lattice_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, st>>>(row0 + s, n, reso, offset[0], offset[1], offset[2], scale[0], scale[1],
+                                                                   scale[2], pts);
+        MN_LAUNCH_CHECK(ctx);
+        // a dense box reaches past the centroid hull, where more sub-modules blend than max_multiplicity assumes: size this call's
+        // slots for all of them
+        const int rc = model_forward_impl(ctx, m, &rows, n, use_coarse, 1, nullptr, precision, sigma_out_d + s, (char*)workspace_d + pts_bytes,
+                                          workspace_bytes - pts_bytes, nullptr, 0, stream, 0, LiveRows{}, m->d.n_sub);
+        if (rc) return rc;
+    }
+    return MN_OK;
+}
 
 // ---- training (SURVEY.md §8f-1) --------------------------------------------------------------------
 size_t mn_model_tape_bytes(const mn_model* m, int64_t B) { return m ? tape_regions(m, B, false, nullptr) : 0; }

@@ -93,7 +93,7 @@ __device__ __forceinline__ uint64_t route_row(const float* d, int K, float margi
 // count, as it follows the batch size in the reference.
 template <int KMAX>
 __global__ void route_count_kernel(RowSrc src, int64_t B, LiveRows live, const float* __restrict__ cent, int K, int s, float margin,
-                                   int* counters, unsigned long long* __restrict__ mask_out, float* __restrict__ w_out) {
+                                   int64_t cap, int* counters, unsigned long long* __restrict__ mask_out, float* __restrict__ w_out) {
     __shared__ int hist[MN_MAX_SUB];
     __shared__ float sc[MN_MAX_SUB * 3];
     for (int i = threadIdx.x; i < K * 3; i += blockDim.x) sc[i] = cent[i];
@@ -140,7 +140,9 @@ __global__ void route_count_kernel(RowSrc src, int64_t B, LiveRows live, const f
             counters[CNT_CURSOR + k] = 0;
         }
         counters[CNT_START + K] = off;
-        counters[CNT_NSLOTS] = off;
+        // the MLP kernels walk the tiles below CNT_NSLOTS: past the slot capacity (an overflow, whose pairs the scatter pass drops)
+        // there is no slot, image or output to read or write
+        counters[CNT_NSLOTS] = off < cap ? off : (int)cap;
         counters[CNT_NPAIRS] = pairs;
     }
 }
@@ -328,7 +330,7 @@ int mn_route_build(mn_ctx* ctx, mn_model* m, const RowSrc& src, int64_t B, LiveR
         else KERNEL<MN_MAX_SUB><<<GRID, BLOCK, 0, st>>>(__VA_ARGS__);                 \
     } while (0)
     MN_ROUTE_DISPATCH(route_count_kernel, blocks, 256, src, B, live, m->centroids_d, K, m->d.cluster_dim_start, m->d.boundary_margin,
-                      m->counters_d, mask_buf, w_buf);
+                      cap, m->counters_d, mask_buf, w_buf);
     MN_LAUNCH_CHECK(ctx);
     MN_ROUTE_DISPATCH(route_scatter_kernel, blocks, 256, B, live, K, m->counters_d, cap, mask_buf, w_buf, slot_row, slot_w, row_slots,
                       ctx->status_d);
