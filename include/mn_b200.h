@@ -352,8 +352,8 @@ int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const
  * images scaled by a power of two chosen from max|grad_out|), weight gradients as wgmma contractions of the two tapes
  * over the slot axis, fp32 accumulation, fp32 atomics into param_grads_d.  Same argument meaning as the fp32 entry points
  * above; covers layer_dim 256, 512 (up to 10 trunk layers) and 768..2048 (a multiple of 256; the layer-GEMM path, backward
- * one tile group at a time) with a direction / appearance head and either rgb_dim 3 or a raw SH head (rgb_dim <= 32), no
- * affine appearance (mn_model_train_tc_supported), everything else returns MN_ERR_UNSUPPORTED - use the fp32 entry points.
+ * one tile group at a time) with a direction / appearance head and either rgb_dim 3 or a raw SH head (rgb_dim <= 80, i.e.
+ * sh_deg <= 4; rgb_dim 48 and 75 run on the layer-GEMM path at 256 and 512 wide too), no affine appearance (mn_model_train_tc_supported), everything else returns MN_ERR_UNSUPPORTED - use the fp32 entry points.
  * The first recording call allocates the transposed weight images of the backward (about 4.25 MiB per 512-wide and 71 MB
  * per 2048-wide sub-module).
  * Gradients agree with the fp32 path to ~1e-2 of each tensor's scale (fp16 operands, like the reference under autocast);

@@ -1,6 +1,9 @@
 #pragma once
 
-// Layer-GEMM path for networks wider than the fused kernel covers (512 < layer_dim <= 2048, a multiple of 256), included
+// Layer-GEMM path for networks wider than the fused kernel covers (512 < layer_dim <= 2048, a multiple of 256), and for the
+// spherical-harmonics heads of degree 3 and 4 (32 < rgb_dim <= MN_TC_LG_RGB_MAX) at every width the fused kernel covers
+// (64..256, a multiple of 64, and 512): its rgb head is not a GEMM, so a wider head needs no new tiling, and N is padded to
+// 256-column blocks anyway (zero weights and biases in the padding; the next GEMM reads only the first L columns).  Included
 // inside mn_mlp_tc.cu's anonymous namespace after mn_mlp_wg.cuh (whose wgmma wrappers it uses).
 //
 // One 128-row tile of 2048-wide fp16 activations is 512 KiB and one 2048 x 2048 layer 8 MiB of fp16 weights, so neither
@@ -21,7 +24,8 @@
 //   tc_layer_head_kernel   one thread per tile row, CUDA cores, fp32: sigma = the last trunk activations . sigma_w + bias
 //                          (+ sigma_noise) -> ReLU / shifted softplus; rgb = W_rgb G (or W_rgb H_last without dir_a_encoding)
 //                          -> tc_emit_rgb.  sigma_only stops after sigma.  A recording (training) call also fills the tile's
-//                          fp32 head block of the tensor-core tape.
+//                          fp32 head block of the tensor-core tape.  <32> for rgb_dim <= 32, <MN_TC_LG_RGB_MAX> above: the
+//                          rgb accumulators of a row stay in registers either way.
 //
 // Training (precision tc_f16, mn_train_tc.cuh): the recording forward is the same launch list with the encoder tiles and every
 // GEMM's output written to the tape instead of the group buffers.  The backward runs the data-gradient chain through
@@ -301,6 +305,8 @@ __device__ __forceinline__ void lg_load8(const unsigned char* img, int64_t lo, i
     }
 }
 
+// kR bounds rgb_dim (mn_tc_lg_rgb_bound): 32, or MN_TC_LG_RGB_MAX for the SH heads of degree 3 and 4.
+template <int kR>
 __global__ void __launch_bounds__(kTileM) tc_layer_head_kernel(const LhArgs A) {
     const int t = threadIdx.x;
     const int64_t tile = A.tile0 + blockIdx.x;
@@ -343,17 +349,17 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_kernel(const LhArgs A) {
     }
 
     // rgb Linear over the head input, rgb_dim rows of [rgb_dim][rgb_in] fp32 weights.  Only compile-time indices into acc
-    // (loops unrolled to MN_TC_RGB_MAX and left at r == R), so the array stays in registers.
+    // (loops unrolled to kR and left at r == R), so the array stays in registers.
     const int R = A.m.nd.rgb_dim;
     const float* wr = f32 + A.rgb_w_off;
     const unsigned char* g = A.g + (int64_t)blockIdx.x * A.g_tile_bytes;
-    float acc[MN_TC_RGB_MAX];
+    float acc[kR];
 #pragma unroll
-    for (int r = 0; r < MN_TC_RGB_MAX; ++r) acc[r] = 0.0f;
+    for (int r = 0; r < kR; ++r) acc[r] = 0.0f;
     for (int c = 0; c < A.rgb_in; c += 8) {
         lg_load8(g, A.g_lo, c, t, v);
 #pragma unroll
-        for (int r = 0; r < MN_TC_RGB_MAX; ++r) {
+        for (int r = 0; r < kR; ++r) {
             if (r >= R) break;
             const float4 wa = __ldg(reinterpret_cast<const float4*>(wr + (size_t)r * A.rgb_in + c));
             const float4 wb = __ldg(reinterpret_cast<const float4*>(wr + (size_t)r * A.rgb_in + c + 4));
@@ -363,10 +369,10 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_kernel(const LhArgs A) {
             acc[r] = x;
         }
     }
-    uint32_t raw[MN_TC_RGB_MAX];
+    uint32_t raw[kR];
 #pragma unroll
-    for (int r = 0; r < MN_TC_RGB_MAX; ++r) raw[r] = __float_as_uint(acc[r]);
-    tc_emit_rgb(A.m, sub, row, slot, raw, f32 + A.rgb_b_off, sg, tf ? tf + MN_TC_F32_RGB * kTileM : nullptr);
+    for (int r = 0; r < kR; ++r) raw[r] = __float_as_uint(acc[r]);
+    tc_emit_rgb<kR>(A.m, sub, row, slot, raw, f32 + A.rgb_b_off, sg, tf ? tf + MN_TC_F32_RGB * kTileM : nullptr);
 }
 
 // ---- training backward: head stage of one tile group, one thread per tile row (CUDA cores, fp32).  Upstream gradient x blend
@@ -388,6 +394,7 @@ struct LdArgs {
     const float* scale;
 };
 
+template <int kR>
 __global__ void __launch_bounds__(kTileM) tc_layer_head_dgrad_kernel(const LdArgs A) {
     const int t = threadIdx.x, lane = t & 31;
     const int64_t tile = A.tile0 + blockIdx.x;
@@ -399,12 +406,12 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_dgrad_kernel(const LdArg
     const int R = A.m.nd.rgb_dim, half = A.half;
     const float S = *A.scale;
     const float* tf = A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + t;
-    float d[MN_TC_RGB_MAX];
-    const float ds = tc_head_grad(A.m, A.grad_out, row, slot, tf, d);
+    float d[kR];
+    const float ds = tc_head_grad<kR>(A.m, A.grad_out, row, slot, tf, d);
     float* tg = A.gf32 + (size_t)blockIdx.x * mn_tc_g32_rows(R) * kTileM + t;
     tg[MN_TC_G32_SIGMA * kTileM] = ds;
 #pragma unroll
-    for (int c = 0; c < MN_TC_RGB_MAX; ++c) {
+    for (int c = 0; c < kR; ++c) {
         if (c >= R) break;
         tg[(MN_TC_G32_RGB + c) * kTileM] = d[c];
     }
@@ -415,7 +422,7 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_dgrad_kernel(const LdArg
     float* sums = A.emb_sum ? A.emb_sum + (size_t)sub * A.m.nd.app_count * half : nullptr;
     for (int k0 = 0; k0 < half; k0 += 8) {
         float v[8];
-        tc_rgb_dgrad8(Wr, half, k0, d, R, gimg + (size_t)(k0 >> 3) * (kTileM * 16), v);
+        tc_rgb_dgrad8<kR>(Wr, half, k0, d, R, gimg + (size_t)(k0 >> 3) * (kTileM * 16), v);
         if (sums) tc_emb_sums8(sums + k0, half, row >= 0, id, lane, v);
         uint32_t pk[4];
 #pragma unroll

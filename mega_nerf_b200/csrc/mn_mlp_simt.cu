@@ -62,6 +62,10 @@ __device__ __forceinline__ void gemm_layer(const float* __restrict__ Wt, const f
     }
 }
 
+// Rows of the PE block: the xyz encoding, and later the rgb head's outputs, which can outnumber it (an SH head of degree 4 has
+// 75 coefficients, the xyz encoding of pos_xyz_dim 10 has 63 channels).
+__host__ __device__ __forceinline__ int simt_pe_rows(const NetDims& nd) { return nd.in_xyz > nd.rgb_dim ? nd.in_xyz : nd.rgb_dim; }
+
 // SAVE = training forward: every value the backward pass needs is also written to the activation tape
 // (TapeLayout, mn_model.cuh); the arithmetic is the same instruction stream either way.
 template <int TM, bool SAVE>
@@ -70,8 +74,8 @@ __global__ void __launch_bounds__(256, 1) mlp_simt_kernel(const MlpArgs a) {
     const NetDims& nd = a.nd;
     const int L = nd.L;
     float* const T = SAVE ? a.tape + (size_t)blockIdx.x * a.tl.a_total * TM : nullptr;
-    float* PE = smem;                    // [in_xyz][TM]
-    float* AUX = PE + nd.in_xyz * TM;    // [aux][TM]  = dir encoding | appearance embedding
+    float* PE = smem;                    // [in_xyz][TM]; [simt_pe_rows(nd)] reserved: the rgb head's outputs reuse it
+    float* AUX = PE + simt_pe_rows(nd) * TM;    // [aux][TM]  = dir encoding | appearance embedding
     float* H0 = AUX + nd.aux * TM;       // [L][TM]
     float* H1 = H0 + L * TM;             // [L][TM]
     float* SIG = H1 + L * TM;            // [TM]
@@ -218,7 +222,7 @@ __global__ void __launch_bounds__(256, 1) mlp_simt_kernel(const MlpArgs a) {
         rgb_src = cur;
     }
     // rgb head (nerf.py:152-154)
-    float* OUTS = PE;  // [rgb_dim][TM], PE is dead by now
+    float* OUTS = PE;  // [rgb_dim][TM] (simt_pe_rows), PE is dead by now
     {
         const float* wr = P + a.lay.rgb_w;
         const float* br = P + a.lay.rgb_b;
@@ -276,7 +280,7 @@ __global__ void __launch_bounds__(256, 1) mlp_simt_kernel(const MlpArgs a) {
 
 template <int TM>
 size_t simt_smem_bytes(const NetDims& nd) {
-    return (size_t)(nd.in_xyz + nd.aux + 2 * nd.L + 1) * TM * 4 + (size_t)TM * 4 + (size_t)TM * 8 * 4;
+    return (size_t)(simt_pe_rows(nd) + nd.aux + 2 * nd.L + 1) * TM * 4 + (size_t)TM * 4 + (size_t)TM * 8 * 4;
 }
 
 }  // namespace

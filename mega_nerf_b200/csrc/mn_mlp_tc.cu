@@ -15,7 +15,8 @@
 // The epilogue's per-row 16-byte stores and the packer's images are contiguous in this layout, any K that
 // is a multiple of 16 works, and no TMA tensor map is needed (plain 1-D bulk copies).
 //
-// Networks wider than 512 run on the layer-GEMM engine instead (mn_layer_gemm.cuh).  Host side: tc_linears lists the
+// Networks wider than 512, and the spherical-harmonics heads of degree 3 and 4 (rgb_dim 48, 75) at any width, run on the
+// layer-GEMM engine instead (mn_layer_gemm.cuh).  Host side: tc_linears lists the
 // network's Linears once; tc_net picks the engine and the training coverage from that table, and builds the forward plan of
 // either engine (build_plan) and the data-gradient plan (build_dgrad_plan); every entry point below calls it once.
 // mn_mlp_tc_pack writes the forward images of either engine, tc_dgrad_ready / tc_pack_dgrad the transposed images of the
@@ -126,7 +127,7 @@ TcLinears tc_linears(const mn_model& m) {
 // [biases][sigma_w (L)][sigma_b (4)].  The fused engine (tc_mlp_wg_kernel) runs every GEMM in one launch, the rgb head as an
 // N = 32 GEMM, and reserves bstride floats per bias.  The layer engine (mn_layer_gemm.cuh) launches one GEMM per Linear with
 // N padded to 256-column blocks, in the image and in the bias; its rgb head is not a GEMM: tc_layer_head_kernel reads
-// [rgb_w [rgb_dim][rgb_in]][rgb_b (32)] from the end of the fp32 block (lg_net).
+// [rgb_w [rgb_dim][rgb_in]][rgb_b (mn_tc_lg_rgb_bound(rgb_dim))] from the end of the fp32 block (lg_net).
 void build_plan(const NetDims& nd, const TcLinears& T, bool layer, TcPlan* p) {
     TcPlan& P = *p;
     P = TcPlan{};
@@ -151,7 +152,7 @@ void build_plan(const NetDims& nd, const TcLinears& T, bool layer, TcPlan* p) {
     }
     P.plane_bytes = woff;
     P.sigma_w_off = foff;
-    P.f32_floats = foff + nd.L + 4 + (layer ? nd.rgb_dim * nd.rgb_in + MN_TC_RGB_MAX : 0);
+    P.f32_floats = foff + nd.L + 4 + (layer ? nd.rgb_dim * nd.rgb_in + mn_tc_lg_rgb_bound(nd.rgb_dim) : 0);
     P.f32_off = woff * 2;
     P.sub_bytes = (int)mn_align((size_t)woff * 2 + (size_t)P.f32_floats * 4, 256);
     P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
@@ -188,7 +189,10 @@ void build_dgrad_plan(const NetDims& nd, const TcLinears& T, TcPlan* p) {
     P.sub_bytes = (int)mn_align((size_t)woff + (size_t)P.f32_floats * 4, 256);
 }
 
-// ---- which engine serves a network, and whether tensor-core training covers it
+// ---- which engine serves a network, and whether tensor-core training covers it.  The fused engine takes rgb_dim <= 32 (its
+// N = 32 rgb GEMM) at 64..256 and 512 wide; the layer engine everything wider, and the SH heads of degree 3 and 4 (rgb_dim
+// <= MN_TC_LG_RGB_MAX) at the fused engine's widths too.  Training runs on either engine at 256 and 512 wide, on the layer
+// engine above; it needs dir_a_encoding (its data-gradient chain ends there) and no affine appearance.
 enum { TC_NONE = 0, TC_FUSED = 1, TC_LAYER = 2 };
 struct TcNet {
     int engine;
@@ -202,14 +206,16 @@ TcNet tc_net(const mn_model& m) {
     const NetDims& nd = m.nd;
     TcNet t{};
     t.lin = tc_linears(m);
+    const bool fused_width = nd.L % 64 == 0 && (nd.L <= 256 || nd.L == 512) && nd.L >= 64;
+    const bool wide = nd.L > 512 && nd.L <= 2048 && nd.L % 256 == 0;
     if (nd.affine && nd.rgb_dim != 3) t.engine = TC_NONE;
-    else if (nd.L > 512 && nd.L <= 2048 && nd.L % 256 == 0 && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers + 2 <= kMaxGemm)
-        t.engine = TC_LAYER;
-    else if (nd.L % 64 == 0 && (nd.L <= 256 || nd.L == 512) && nd.L >= 64 && nd.rgb_dim <= 32 && nd.layers <= 12)
+    else if (fused_width && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers <= 12)
         t.engine = TC_FUSED;
+    else if ((wide || (fused_width && nd.rgb_dim > MN_TC_RGB_MAX)) && nd.rgb_dim <= MN_TC_LG_RGB_MAX && nd.layers + 2 <= kMaxGemm)
+        t.engine = TC_LAYER;
     if (t.engine != TC_NONE) build_plan(nd, t.lin, t.engine == TC_LAYER, &t.P);
-    t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers >= 2 &&
-              (t.engine == TC_LAYER || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 10));
+    t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.layers >= 2 &&
+              ((t.engine == TC_LAYER && nd.L >= 256) || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 10));
     if (t.train) build_dgrad_plan(nd, t.lin, &t.D);
     return t;
 }
@@ -264,7 +270,8 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 
 // rgb head epilogue shared by the tensor-core kernels (nerf.py:152-160): bias, optional per-image affine appearance
 // transform (3x4 matrix = affine(embedding_a[idx]), nerf.py:156-158), sigmoid when rgb_dim == 3, blend weight.
-// v = the row's raw fp32 accumulators of the rgb GEMM.
+// v = the row's raw fp32 accumulators of the rgb GEMM, kR >= rgb_dim of them.
+template <int kR = MN_TC_RGB_MAX>
 __device__ __forceinline__ void tc_emit_rgb(const MlpArgs& m, int sub, int64_t row, int64_t slot, const uint32_t* v,
                                             const float* bias, float sigma, float* tape_rgb = nullptr) {
     const NetDims& nd = m.nd;
@@ -292,7 +299,7 @@ __device__ __forceinline__ void tc_emit_rgb(const MlpArgs& m, int sub, int64_t r
         }
     } else {
 #pragma unroll
-        for (int c = 0; c < 32; ++c) {
+        for (int c = 0; c < kR; ++c) {
             if (c < nd.rgb_dim) {
                 float x = __uint_as_float(v[c]) + bias[c];
                 if (nd.rgb_dim == 3) x = mn_sigmoid(x);
@@ -717,7 +724,8 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
         const LgNet B = lg_net(P, nd);
         mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + B.rgb_w_off, nullptr, (long long)nd.rgb_dim * nd.rgb_in, PK_RGBW,
                                  {nd.rgb_in, nd.rgb_dim, 0, 0, 0, 0, 0}});
-        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + B.rgb_b_off, nullptr, MN_TC_RGB_MAX, PK_TC_F32, {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
+        mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + B.rgb_b_off, nullptr, mn_tc_lg_rgb_bound(nd.rgb_dim), PK_TC_F32,
+                                 {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
     }
     m->tc_ready = 1;
     m->train_tc_ok = net.train ? 1 : 0;
@@ -825,7 +833,8 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet&
             H.h_tile_bytes = H.g_tile_bytes = act_tile;
             H.tape_f32 = tape->f32;
         }
-        tc_layer_head_kernel<<<(unsigned)nt, kTileM, 0, st>>>(H);
+        if (m->nd.rgb_dim <= MN_TC_RGB_MAX) tc_layer_head_kernel<MN_TC_RGB_MAX><<<(unsigned)nt, kTileM, 0, st>>>(H);
+        else tc_layer_head_kernel<MN_TC_LG_RGB_MAX><<<(unsigned)nt, kTileM, 0, st>>>(H);
         MN_LAUNCH_CHECK(ctx);
     }
     mn_prof_end(ctx, st);
@@ -838,8 +847,8 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
     if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net, n_tiles128, precision, ws, ws_bytes, st);
     if (net.engine != TC_FUSED || !m->tc_ready)
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
-                       "tensor-core MLP path covers layer_dim 64..256 (multiple of 64), 512 or 768..2048 (multiple of 256) and rgb_dim <= 32; "
-                       "use precision 'fp32' for this model");
+                       "tensor-core MLP path covers layer_dim 64..256 (multiple of 64), 512 or 768..2048 (multiple of 256) and rgb_dim <= 80 "
+                       "(sh_deg <= 4), without affine appearance for rgb_dim > 3; use precision 'fp32' for this model");
     if (a.nd.L > 256 && precision == MN_PREC_TC_F16X3)
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "precision 'tc_f16x3' covers layer_dim <= 256; use 'tc_f16' or 'fp32' for the 512-wide network");
@@ -1011,9 +1020,12 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         H.gw = a.gw;
         H.sub_stride = a.lay.total;
         H.sigma_w = a.lay.sigma_w; H.sigma_b = a.lay.sigma_b; H.rgb_w = a.lay.rgb_w; H.rgb_b = a.lay.rgb_b;
-        const dim3 hgrid((unsigned)mn_cdiv(nt, (int64_t)16), (unsigned)n_sub, (unsigned)(L / 256));
+        // channel blocks: L for the sigma row; the rgb rows in groups of 16 over L/2 channels each (2 groups up to 32 rows)
+        const int rgb_groups = nd.rgb_dim == 3 ? 1 : (nd.rgb_dim + 15) / 16;
+        const dim3 hgrid((unsigned)mn_cdiv(nt, (int64_t)16), (unsigned)n_sub, (unsigned)mn_cdiv(std::max(L, rgb_groups * half), 256));
         if (nd.rgb_dim == 3) tc_heads_wgrad_kernel<3><<<hgrid, 256, 0, st>>>(H);
-        else tc_heads_wgrad_kernel<MN_TC_RGB_MAX><<<hgrid, 256, 0, st>>>(H);
+        else if (nd.rgb_dim <= MN_TC_RGB_MAX) tc_heads_wgrad_kernel<MN_TC_RGB_MAX><<<hgrid, 256, 0, st>>>(H);
+        else tc_heads_wgrad_kernel<MN_TC_LG_RGB_MAX><<<hgrid, 256, 0, st>>>(H);
         MN_LAUNCH_CHECK(ctx);
         return MN_OK;
     };
@@ -1118,7 +1130,8 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
                 H.dz = dzg;
                 H.emb_sum = nd.app_in_dira ? emb_sum : nullptr;
                 H.scale = scale;
-                tc_layer_head_dgrad_kernel<<<(unsigned)nt, kTileM, 0, st>>>(H);
+                if (nd.rgb_dim <= MN_TC_RGB_MAX) tc_layer_head_dgrad_kernel<MN_TC_RGB_MAX><<<(unsigned)nt, kTileM, 0, st>>>(H);
+                else tc_layer_head_dgrad_kernel<MN_TC_LG_RGB_MAX><<<(unsigned)nt, kTileM, 0, st>>>(H);
                 MN_LAUNCH_CHECK(ctx);
             }
             // ---- data-gradient GEMM g: dz_out = [mask](dz_in W^T) [+ S dsigma x sigma_w]

@@ -173,8 +173,9 @@ __host__ __device__ inline WgLayout wg_layout(const TcPlan& p, bool split) {
 // layer-GEMM path's tc_layer_head_dgrad_kernel.
 // d[c] = gradient of the rgb Linear's output c: upstream gradient x blend weight, then sigmoid' (colour head, rgb_dim 3) or the
 // raw SH coefficients as they are.  Returns the gradient of the sigma pre-activation (softplus' or ReLU').  tf: the row's entry
-// of the tape's fp32 head block.  Only compile-time indices into d (loops unrolled to MN_TC_RGB_MAX and left at c == R), so
-// the array stays in registers.
+// of the tape's fp32 head block.  kR bounds rgb_dim (d holds kR floats).  Only compile-time indices into d (loops unrolled to
+// kR and left at c == R), so the array stays in registers.
+template <int kR>
 __device__ __forceinline__ float tc_head_grad(const MlpArgs& m, const float* grad_out, int64_t row, int64_t slot, const float* tf,
                                               float* d) {
     const int R = m.nd.rgb_dim;
@@ -190,12 +191,12 @@ __device__ __forceinline__ float tc_head_grad(const MlpArgs& m, const float* gra
         d[0] = (g0 * (1.0f - c0v)) * c0v; d[1] = (g1 * (1.0f - c1v)) * c1v; d[2] = (g2 * (1.0f - c2v)) * c2v;
     } else {
 #pragma unroll
-        for (int c = 0; c < MN_TC_RGB_MAX; ++c) d[c] = 0.0f;
+        for (int c = 0; c < kR; ++c) d[c] = 0.0f;
         if (row >= 0) {
             const float* go = grad_out + row * m.out_cols;          // [rgb_dim SH coefficients][sigma]
             const float bw = m.slot_w ? m.slot_w[slot] : 1.0f;
 #pragma unroll
-            for (int c = 0; c < MN_TC_RGB_MAX; ++c) {
+            for (int c = 0; c < kR; ++c) {
                 if (c >= R) break;
                 d[c] = go[c] * bw;
             }
@@ -210,7 +211,9 @@ __device__ __forceinline__ float tc_head_grad(const MlpArgs& m, const float* gra
 }
 
 // v[e] = mask(G > 0) (sum_c W_rgb[c][k0 + e] d[c]) for the 8 columns k0 .. k0 + 7 of one row; Wr = [rgb_dim][half] fp32, g = the
-// row's 8 fp16 values of G in the tile image.  Order c = 0, 1, .. (a product, then one fma per further row).
+// row's 8 fp16 values of G in the tile image, d = kR floats (tc_head_grad).  Order c = 0, 1, .. (a product, then one fma per
+// further row).
+template <int kR>
 __device__ __forceinline__ void tc_rgb_dgrad8(const float* Wr, int half, int k0, const float* d, int R, const unsigned char* g, float* v) {
     const uint4 gm = *reinterpret_cast<const uint4*>(g);
     const __half2* gh = reinterpret_cast<const __half2*>(&gm);
@@ -220,7 +223,7 @@ __device__ __forceinline__ void tc_rgb_dgrad8(const float* Wr, int half, int k0,
         v[4] = wb.x * d[0]; v[5] = wb.y * d[0]; v[6] = wb.z * d[0]; v[7] = wb.w * d[0];
     }
 #pragma unroll
-    for (int c = 1; c < MN_TC_RGB_MAX; ++c) {
+    for (int c = 1; c < kR; ++c) {
         if (c >= R) break;
         const float4 wa = *reinterpret_cast<const float4*>(Wr + c * half + k0);
         const float4 wb = *reinterpret_cast<const float4*>(Wr + c * half + k0 + 4);
@@ -360,7 +363,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                 const float* Wr = F32 + L;                                  // [rgb_dim][L/2] rgb weights (fp32 block of the data-gradient plan)
                 const float* tf = A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + hr;
                 float d[MN_TC_RGB_MAX];
-                const float ds = tc_head_grad(A.m, A.grad_out, hrow, hslot, tf, d);
+                const float ds = tc_head_grad<MN_TC_RGB_MAX>(A.m, A.grad_out, hrow, hslot, tf, d);
                 if (part == 0) {
                     DSIG[hr] = ds * S;
                     float* tg = A.tape_gf32 + (size_t)tile * mn_tc_g32_rows(R) * kTileM + hr;
@@ -378,7 +381,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                 for (int kk = 0; kk < per; kk += 8) {
                     const int k0 = part * per + kk;
                     float v[8];
-                    tc_rgb_dgrad8(Wr, half, k0, d, R, gimg + (size_t)(k0 >> 3) * (kTileM * 16) + (size_t)hr * 16, v);
+                    tc_rgb_dgrad8<MN_TC_RGB_MAX>(Wr, half, k0, d, R, gimg + (size_t)(k0 >> 3) * (kTileM * 16) + (size_t)hr * 16, v);
                     if (A.emb_sum) tc_emb_sums8(A.emb_sum + (size_t)sub * A.m.nd.app_count * half + k0, half, hrow >= 0, id, lane, v);
                     uint32_t pk[4];
 #pragma unroll

@@ -182,10 +182,13 @@ __host__ __device__ __forceinline__ size_t mn_tc_img_off(int img, int L) { retur
 // rows of the per-tile fp32 head block [MN_TC_F32_ROWS][128]: sigma pre-activation, rgb (3), image id
 enum { MN_TC_F32_SIGMA = 0, MN_TC_F32_RGB = 1, MN_TC_F32_ID = 4, MN_TC_F32_ROWS = 5 };
 // rows of the backward pass's per-tile fp32 head-gradient block [mn_tc_g32_rows(rgb_dim)][128]: d sigma pre-activation, d rgb
-// pre-activation (rgb_dim rows: 3 colour channels before the sigmoid, or the raw SH coefficients).  MN_TC_RGB_MAX bounds
-// rgb_dim on the tensor-core training path (register and shared-memory arrays of the head kernels are sized by it).
-enum { MN_TC_G32_SIGMA = 0, MN_TC_G32_RGB = 1, MN_TC_RGB_MAX = 32 };
+// pre-activation (rgb_dim rows: 3 colour channels before the sigmoid, or the raw SH coefficients).
+// Bounds of rgb_dim (register and shared-memory arrays of the head kernels are sized by them): MN_TC_RGB_MAX for the fused
+// engine (its rgb head is an N = 32 GEMM), MN_TC_LG_RGB_MAX for the layer-GEMM engine's CUDA-core head (SH degree 4: 75
+// coefficients).  The layer engine's head kernels come in both sizes; mn_tc_lg_rgb_bound picks the one a network runs.
+enum { MN_TC_G32_SIGMA = 0, MN_TC_G32_RGB = 1, MN_TC_RGB_MAX = 32, MN_TC_LG_RGB_MAX = 80 };
 __host__ __device__ __forceinline__ int mn_tc_g32_rows(int rgb_dim) { return 1 + rgb_dim; }
+__host__ __device__ __forceinline__ int mn_tc_lg_rgb_bound(int rgb_dim) { return rgb_dim <= MN_TC_RGB_MAX ? MN_TC_RGB_MAX : MN_TC_LG_RGB_MAX; }
 struct TrainTcTape {
     unsigned char* xreg;      // encoder feature tiles        [n_tiles][x_tile_bytes]
     unsigned char* act;       // activation records           [n_tiles][act_tile_bytes]
@@ -194,7 +197,7 @@ struct TrainTcTape {
 // the shapes whose recording calls run on the tensor cores (tc_net in mn_mlp_tc.cu; mn_model_train_tc_supported)
 #define MN_TC_TRAIN_COVERAGE                                                                                                    \
     "tensor-core training covers layer_dim 256, 512 or 768..2048 (a multiple of 256) with a direction / appearance head, rgb_dim 3 " \
-    "or a raw SH head (rgb_dim <= 32), no affine appearance; use train precision 'fp32'"
+    "or a raw SH head (rgb_dim <= 80: sh_deg <= 4), no affine appearance; use train precision 'fp32'"
 size_t mn_train_tc_x_tile_bytes(const mn_model* m);
 size_t mn_train_tc_act_tile_bytes(const mn_model* m);
 int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st);

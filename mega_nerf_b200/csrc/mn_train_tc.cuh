@@ -230,14 +230,14 @@ struct HeadsArgs {
     int64_t sub_stride;
     int sigma_w, sigma_b, rgb_w, rgb_b;     // float offsets in a sub-module's gradient block (rgb_w is [rgb_dim][L/2])
 };
-// kRgb: 3 for the colour head (exactly 3 rgb rows), MN_TC_RGB_MAX for a raw SH head (rgb_dim <= kRgb rows).  The rgb weight
-// gradient is split over the channel index k: k accumulates input channel k % (L/2) for the output rows [kPer * (k / (L/2)),
-// +kPer) (two groups of kPer rows over k < L).  Block z of the grid takes the 256 channels k = 256 z + threadIdx.x, so wider
-// networks run L / 256 channel blocks.
+// kRgb: 3 for the colour head (exactly 3 rgb rows), MN_TC_RGB_MAX or MN_TC_LG_RGB_MAX for a raw SH head (rgb_dim <= kRgb
+// rows).  The rgb weight gradient is split over the channel index k: k accumulates input channel k % (L/2) for the output rows
+// [kPer * (k / (L/2)), +kPer) (up to 32 rows: two groups of kPer rows over k < L; up to 80: five groups over k < 5 L/2).  Block z
+// of the grid takes the 256 channels k = 256 z + threadIdx.x, so the grid runs max(L, groups x L/2) / 256 channel blocks.
 template <int kRgb>
 __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) {
     constexpr int kPer = kRgb < 16 ? kRgb : 16;       // rgb accumulators per thread
-    static_assert(2 * kPer >= kRgb, "rgb rows of tc_heads_wgrad_kernel");
+    static_assert(kRgb <= MN_TC_LG_RGB_MAX, "rgb rows of tc_heads_wgrad_kernel (the shared block below, the bias rows k < 1 + kRgb)");
     __shared__ float G[1 + kRgb][kTileM];              // this tile's head-gradient block
     int sub = A.fixed_sub;
     int64_t t_lo = A.t_min, t_hi = min(A.n_tiles, A.t_max);

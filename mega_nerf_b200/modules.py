@@ -30,7 +30,9 @@ def set_precision(name: str) -> None:
 
     Networks with layer_dim 768..2048 (a multiple of 256; the nerf, npp and mega-nerf-dense configs set 2048) run on the
     layer-GEMM tensor-core path in 'tc_f16' and 'tc_f16x3' ('tc_f16x3' is the parity-grade mode there); 'fp32' covers
-    layer_dim <= 512 only and refuses them."""
+    layer_dim <= 512 only and refuses them.  So do raw SH heads of degree 3 and 4 (rgb_dim 48, 75) at every width, 64..512
+    included: 'tc_f16x3' serves them at 512 wide too, while it refuses the 512-wide networks of rgb_dim <= 32 (those run on
+    the fused kernel, which covers 'tc_f16' only at that width)."""
     global _precision
     if name not in K.PRECISIONS:
         raise ValueError(f'unknown precision {name!r}; choose from {sorted(K.PRECISIONS)}')
@@ -51,8 +53,8 @@ def set_train_precision(name: str) -> None:
              does on a GPU under autocast + GradScaler (runner.py:243-274).  The tensor-core training kernels cover
              layer_dim 256, 512 (up to 10 trunk layers) and 768..2048 (a multiple of 256: the nerf, npp and
              mega-nerf-dense configs' 2048) with a
-             direction / appearance head and either an rgb head (rgb_dim 3) or a raw SH head (rgb_dim <= 32, e.g.
-             sh_deg 2); other networks (other widths, affine appearance, heads without dir_a_encoding) silently use the
+             direction / appearance head and either an rgb head (rgb_dim 3) or a raw SH head (rgb_dim <= 80: sh_deg
+             0..4; degrees 3 and 4 on the layer-GEMM path at every one of these widths); other networks (other widths, affine appearance, heads without dir_a_encoding) silently use the
              fp32 kernels, which refuse layer_dim > 512 - NativeModel.train_on_tensor_cores() tells which."""
     global _train_precision
     if name not in ('fp32', 'tc_f16'):
