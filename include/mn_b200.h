@@ -86,6 +86,17 @@ int mn_rays_pairs(mn_ctx* ctx, const float* dirs_d, int64_t P, const float* c2w_
                   const int32_t* pix_idx_d, int64_t M, float near, float far, int has_altitude, float alt_max, float alt_min,
                   float* out_d, void* stream);
 
+/* ---- training batches -------------------- DataLoader(FilesystemDataset / MemoryDataset), runner.py:228-238 */
+/* One training batch from a device-resident chunk (mega_nerf_b200/batches.py): dst_k[b] = src_k[idx_d[b]] for up to three
+ * row-major columns of 4-byte elements (rgbs [n,3] fp32, rays [n,8] fp32, img_indices [n] int32), what the reference's
+ * DataLoader assembles row by row with `__getitem__` + `default_collate`.
+ *   idx_d int64 [B] (a slice of the permutation, already on the device); n_rows = rows of the chunk; src_k_d [n_rows, w_k],
+ *   dst_k_d [B, w_k]; a column with src_k_d == NULL is skipped.  Rows move in 16-byte units where w_k % 4 == 0 and both
+ *   pointers are 16-byte aligned.  One launch on `stream`, no host sync.  An index outside [0, n_rows) is never read: its
+ *   output row is all one bits and MN_ERR_INVALID is raised at the next mn_check_status. */
+int mn_gather_batch(mn_ctx* ctx, const int64_t* idx_d, int64_t B, int64_t n_rows, const void* src0_d, int w0, void* dst0_d,
+                    const void* src1_d, int w1, void* dst1_d, const void* src2_d, int w2, void* dst2_d, void* stream);
+
 /* ---- sampling --------------------------------------------------------- mega_nerf/rendering.py */
 /* Coarse depths + optional stratified jitter + points (rendering.py:82-87, 472-483).
  *   rays_d [N,8]; z_steps_d [S] (torch.linspace(0,1,S) — passed in, never restated, SURVEY §8c);

@@ -226,7 +226,7 @@ int mn_check_status(mn_ctx* ctx, void* stream) {
                        "Not all your cameras are bounded by the unit sphere; please make sure the cameras are "
                        "normalized properly!");
     if (h & MN_STATUS_INDEX)
-        return mn_fail(ctx, MN_ERR_INVALID, "index out of range (image / pixel index of a ray pair)");
+        return mn_fail(ctx, MN_ERR_INVALID, "index out of range (image / pixel index of a ray pair, or row index of a gathered batch)");
     if (h & MN_STATUS_OVERFLOW)
         return mn_fail(ctx, MN_ERR_WORKSPACE, "routing slot capacity exceeded (raise max multiplicity)");
     return MN_OK;

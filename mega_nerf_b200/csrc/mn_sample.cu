@@ -88,6 +88,51 @@ __global__ void rays_pairs_kernel(const float* __restrict__ dirs, int64_t P, con
 }
 
 // ------------------------------------------------------------------------------------------------
+// training batch assembly                      (DataLoader over FilesystemDataset / MemoryDataset)
+// ------------------------------------------------------------------------------------------------
+// Up to three row-major columns of 4-byte elements gathered at the rows of an index slice: out[b] = src[idx[b]].  A column is
+// moved in 16-byte units where its row width is a multiple of 4 elements and both pointers are 16-byte aligned, else element
+// by element.  One thread per (batch row, unit); the units of the three columns are laid end to end.
+struct GatherArgs {
+    const unsigned int* src[3];
+    unsigned int* dst[3];
+    int w[3];        // row width in 4-byte elements (0: no column)
+    int vec[3];      // 1: 16-byte units
+    int units[3];    // units per row
+    int row_units;   // units[0] + units[1] + units[2]
+};
+
+// v[c] with c in 0..2 by selects, so that the kernel parameters are not copied to local memory for a dynamic index
+template <class T>
+__device__ __forceinline__ T pick3(const T (&v)[3], int c) { return c == 0 ? v[0] : (c == 1 ? v[1] : v[2]); }
+
+__global__ void gather_batch_kernel(const int64_t* __restrict__ idx, int64_t B, int64_t n_rows, const GatherArgs a,
+                                    unsigned int* status) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= B * a.row_units) return;
+    const int64_t b = t / a.row_units;
+    const int first = (int)(t % a.row_units);
+    int u = first, c = 0;
+    if (u >= a.units[0]) {
+        u -= a.units[0];
+        c = 1;
+        if (u >= a.units[1]) { u -= a.units[1]; c = 2; }
+    }
+    const unsigned int* src = pick3(a.src, c);
+    unsigned int* dst = pick3(a.dst, c);
+    const int w = pick3(a.w, c);
+    const int64_t row = idx[b];
+    const bool ok = row >= 0 && row < n_rows;
+    if (!ok && first == 0) atomicOr(status, MN_STATUS_INDEX);    // the reference's tensor indexing raises IndexError
+    if (pick3(a.vec, c)) {
+        uint4* d = reinterpret_cast<uint4*>(dst + b * w) + u;
+        *d = ok ? __ldg(reinterpret_cast<const uint4*>(src + row * w) + u) : make_uint4(~0u, ~0u, ~0u, ~0u);
+    } else {
+        dst[b * w + u] = ok ? __ldg(src + row * w + u) : ~0u;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
 // depth sampling                                               (rendering.py:82-87, 472-483)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ float lerp_depth(float near, float far, float t) { return near * (1.0f - t) + far * t; }
@@ -790,6 +835,29 @@ int mn_rays_pairs(mn_ctx* ctx, const float* dirs_d, int64_t P, const float* c2w_
     if (M == 0) return MN_OK;
     rays_pairs_kernel<<<(unsigned)mn_cdiv(M, 256), 256, 0, (cudaStream_t)stream>>>(dirs_d, P, c2w_d, n_poses, img_idx_d, pix_idx_d, M, near,
                                                                                    far, has_altitude, alt_max, alt_min, out_d, ctx->status_d);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+int mn_gather_batch(mn_ctx* ctx, const int64_t* idx_d, int64_t B, int64_t n_rows, const void* src0_d, int w0, void* dst0_d,
+                    const void* src1_d, int w1, void* dst1_d, const void* src2_d, int w2, void* dst2_d, void* stream) {
+    if (!ctx || !idx_d || B < 0 || n_rows < 0) return MN_ERR_INVALID;
+    GatherArgs a{};
+    const void* src[3] = {src0_d, src1_d, src2_d};
+    void* dst[3] = {dst0_d, dst1_d, dst2_d};
+    const int w[3] = {w0, w1, w2};
+    for (int c = 0; c < 3; ++c) {
+        if (!src[c]) continue;
+        if (!dst[c] || w[c] < 1) return mn_fail(ctx, MN_ERR_INVALID, "mn_gather_batch: a column needs a destination and a width >= 1");
+        a.src[c] = static_cast<const unsigned int*>(src[c]);
+        a.dst[c] = static_cast<unsigned int*>(dst[c]);
+        a.w[c] = w[c];
+        a.vec[c] = w[c] % 4 == 0 && ((uintptr_t)src[c] | (uintptr_t)dst[c]) % 16 == 0;
+        a.units[c] = a.vec[c] ? w[c] / 4 : w[c];
+        a.row_units += a.units[c];
+    }
+    if (B == 0 || a.row_units == 0) return MN_OK;
+    gather_batch_kernel<<<(unsigned)mn_cdiv(B * a.row_units, 256), 256, 0, (cudaStream_t)stream>>>(idx_d, B, n_rows, a, ctx->status_d);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }

@@ -7,7 +7,8 @@ train.py / eval.py / Runner import this package's path unchanged:
 Replaced names (runner.py:33-35, filesystem_dataset.py:18):
     mega_nerf.rendering.render_rays, mega_nerf.models.model_utils.get_nerf / get_bg_nerf,
     mega_nerf.ray_utils.get_rays / get_ray_directions / get_rays_batch, the model classes, and
-    FilesystemDataset._load_chunk_inner (the chunk loader's ray generation, filesystem_dataset.py:95-131).
+    FilesystemDataset._load_chunk_inner (the chunk loader's ray generation, filesystem_dataset.py:95-131), and
+    mega_nerf.runner.DataLoader (training batches gathered on the device, runner.py:23, 228-236).
 """
 from __future__ import annotations
 
@@ -70,6 +71,21 @@ def install(patch_loaded: bool = True) -> None:
                     if hasattr(m, k):
                         setattr(m, k, v)
     patch_loader()
+    patch_data_loader()
+
+
+def patch_data_loader() -> bool:
+    """Bind the device batches (mega_nerf_b200/batches.py) over the `DataLoader` name `Runner.train()` builds its loaders with
+    (runner.py:23, 228-236) if `mega_nerf.runner` is - or can be - imported.  torch's own DataLoader is not touched."""
+    from . import batches
+    m = sys.modules.get('mega_nerf.runner')
+    if m is None:
+        try:
+            m = importlib.import_module('mega_nerf.runner')
+        except Exception:       # no reference on the path, or its imports (cv2, lpips, ...) unavailable
+            return False
+    m.DataLoader = batches.data_loader
+    return True
 
 
 def patch_loader() -> bool:
