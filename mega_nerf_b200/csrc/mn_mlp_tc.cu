@@ -6,7 +6,8 @@
 //   tc_mlp_wg_kernel   persistent, warp-specialised (mn_mlp_wg.cuh): one producer thread (cp.async.bulk of
 //                      weight K-slabs through an mbarrier ring and of the feature tiles), two consumer
 //                      warpgroups issuing wgmma.mma_async (accumulators in registers) and running the
-//                      epilogue (bias/ReLU -> fp16 -> next layer's A operand in shared memory; heads -> HBM).
+//                      epilogue (bias/ReLU -> fp16 -> next layer's A operand, in registers for tc_f16 inference up to
+//                      256 wide and in shared memory otherwise; heads -> HBM).
 //                      Activations never leave the SM between layers.
 //
 // Operand layout (both A tiles and packed weights): K-major, no swizzle, "interleaved" core matrices:
@@ -515,7 +516,7 @@ constexpr int kSmemMax = 227 * 1024;
 
 template <int kMode, bool kSplit, bool kWide>
 int wg_launch(mn_ctx* ctx, const TcArgs& A, int64_t n_tiles128, cudaStream_t st) {
-    const WgLayout WL = wg_layout(A.plan, kSplit);
+    const WgLayout WL = wg_layout(A.plan, kSplit, wg_reg_act(kMode, kSplit, kWide));
     if (WL.total > kSmemMax || WL.stages < 2) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: shared-memory budget exceeded");
     MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_wg_kernel<kMode, kSplit, kWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, WL.total));
     const unsigned grid = (unsigned)(n_tiles128 < ctx->sm_count ? n_tiles128 : ctx->sm_count);
@@ -634,7 +635,7 @@ int mn_mlp_tp_program(const mn_model& m, unsigned int* table_out, int cap_entrie
     const TcNet net = tc_net(m);
     if (net.engine != TC_FUSED) return MN_ERR_UNSUPPORTED;
     const TcPlan& P = net.P;
-    const WgLayout L = wg_layout(P, false);
+    const WgLayout L = wg_layout(P, false, wg_reg_act(PP_INFER, false, P.L > 256));     // the tc_f16 inference launch's layout
     int n = 0, n_trunk = 0;
     for (int gi = 0; gi < P.n_gemm; ++gi) {
         const int nch = (P.g[gi].n + 255) >> 8;

@@ -9,6 +9,8 @@
 //                     feature segment) in shared memory and B = the ring stage, fp32 accumulators in registers; then the
 //                     epilogue straight from the registers: bias / ReLU -> fp16 -> the next layer's A operand, written IN
 //                     PLACE (every MMA that read the old activations has completed), sigma and rgb heads -> HBM.
+//   kMode == PP_INFER up to 256 wide without kSplit (wg_reg_act): each warpgroup keeps its activations in registers instead,
+//   the A operand of the register form of wgmma, and the epilogue packs the accumulators straight into them.
 //   The two consumer warpgroups share the weight stream (a ring stage is released when both have read it) and never touch
 //   each other's rows.  GEMMs wider than 256 (the 512-wide network, kWide) run as two N = 256 halves; the first half's
 //   fp16 result waits in registers until the second half has read the old activations.
@@ -70,6 +72,45 @@ __device__ __forceinline__ void wg_mma(float* d, uint64_t da, uint64_t db, uint3
     else if constexpr (N == 64) wg_mma_n64<TA, TB>(d, da, db, accumulate);
     else if constexpr (N == 128) wg_mma_n128<TA, TB>(d, da, db, accumulate);
     else wg_mma_n256<TA, TB>(d, da, db, accumulate);
+}
+
+// The same MMA with A from registers (the m64k16 fp16 fragment: a[0] / a[1] = rows ra / rb at columns 2 q4 + {0, 1}, a[2] /
+// a[3] the same rows at columns 8 + 2 q4 + {0, 1}) and a K-major B from a shared-memory descriptor.
+__device__ __forceinline__ void wg_mma_rs_n32(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wg_mma_rs_n64(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wg_mma_rs_n128(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wg_mma_rs_n256(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %133, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, {%128, %129, %130, %131}, %132, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+template <int N>
+__device__ __forceinline__ void wg_mma_rs(float* d, const uint32_t* a, uint64_t db, uint32_t accumulate) {
+    static_assert(N == 32 || N == 64 || N == 128 || N == 256, "wgmma N");
+    if constexpr (N == 32) wg_mma_rs_n32(d, a, db, accumulate);
+    else if constexpr (N == 64) wg_mma_rs_n64(d, a, db, accumulate);
+    else if constexpr (N == 128) wg_mma_rs_n128(d, a, db, accumulate);
+    else wg_mma_rs_n256(d, a, db, accumulate);
 }
 
 __device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -147,21 +188,28 @@ struct WgLayout {
     int ring, h, xa, f32, f32_vec4, dsig, bars, total, stages, slab, stage_bytes;
 };
 
-// ring first: an MMA of a narrow GEMM rounded up to the next supported N reads (and ignores) up to 512 bytes past its stage
-__host__ __device__ inline WgLayout wg_layout(const TcPlan& p, bool split) {
+// Whether a variant keeps each consumer warpgroup's activations in registers, as the A operand of the register form of wgmma,
+// instead of in the shared tile image Hs: the tc_f16 inference kernel up to 256 wide.  The training variants write every
+// layer's image to the tapes from Hs, tc_f16x3 needs hi and lo planes, and the 512-wide activations do not fit in registers.
+__host__ __device__ constexpr bool wg_reg_act(int mode, bool split, bool wide) { return mode == PP_INFER && !split && !wide; }
+
+// ring first: an MMA of a narrow GEMM rounded up to the next supported N reads (and ignores) up to 512 bytes past its stage.
+// reg_act (wg_reg_act): no Hs region, the ring takes its place.
+__host__ __device__ inline WgLayout wg_layout(const TcPlan& p, bool split, bool reg_act) {
     WgLayout s;
     const int kx = p.kpe > p.kaux ? p.kpe : p.kaux;
     const int nw = p.L > 256 ? 256 : p.L;                   // widest B slab (no GEMM is wider than layer_dim)
+    const int h_bytes = reg_act ? 0 : p.L * kTileM * 2 * (split ? 2 : 1);
     s.slab = (split || p.L > 256) ? 32 : 64;
     s.stage_bytes = s.slab * nw * 2;
     s.f32_vec4 = (p.f32_floats + 3) / 4;
-    const int fixed = p.L * kTileM * 2 * (split ? 2 : 1) + kx * kTileM * 2 + s.f32_vec4 * 16 + kTileM * 4 + 256;
+    const int fixed = h_bytes + kx * kTileM * 2 + s.f32_vec4 * 16 + kTileM * 4 + 256;
     int st = (kSmemMax - fixed) / s.stage_bytes;
     if (st > kWgRingMax) st = kWgRingMax;
     s.stages = st;
     s.ring = 0;
     s.h = st * s.stage_bytes;
-    s.xa = s.h + p.L * kTileM * 2 * (split ? 2 : 1);
+    s.xa = s.h + h_bytes;
     s.f32 = s.xa + kx * kTileM * 2;
     s.dsig = s.f32 + s.f32_vec4 * 16;
     s.bars = s.dsig + kTileM * 4;
@@ -260,8 +308,9 @@ __device__ __forceinline__ void tc_emb_sums8(float* sums, int half, bool valid, 
 template <int kMode, bool kSplit, bool kWide>
 __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArgs A) {
     extern __shared__ __align__(1024) unsigned char smem[];
+    constexpr bool kRegAct = wg_reg_act(kMode, kSplit, kWide);
     const TcPlan& P = A.plan;
-    const WgLayout SL = wg_layout(P, kSplit);
+    const WgLayout SL = wg_layout(P, kSplit, kRegAct);
     const int stages = SL.stages, slab = SL.slab, stage_bytes = SL.stage_bytes;
     unsigned char* ring = smem + SL.ring;
     unsigned char* Hs = smem + SL.h;
@@ -332,6 +381,9 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
         auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(bar_id) : "memory"); };
         int stage = 0, cur_sub = -1;
         uint32_t phase = 0, xphase = 0;
+        // kRegAct: this warpgroup's rows of the previous GEMM's fp16 output, 4 registers per 16 K-columns (the m64k16 A fragment,
+        // which has the accumulator fragment's row / column map: hreg[2 j] / hreg[2 j + 1] = rows ra / rb, column group j)
+        uint32_t hreg[kRegAct ? 64 : 1];
 
         for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             const int sub = A.m.sub_of_tile(tile);
@@ -420,11 +472,30 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                             mbar_wait(&full[stage], phase);
                             const uint32_t b_base = ring_s + (uint32_t)(stage * stage_bytes);
                             wg_fence();
-                            for (int kk = 0; kk < st.kc; kk += 16) {
-                                const uint64_t ad = wg_desc(a_base + (uint32_t)((st.a_col + kk) >> 3) * (kTileM * 16), kTileM * 16, 128);
-                                const uint64_t bd = wg_desc(b_base + (uint32_t)((kk >> 3) * st.nw * 16), (uint32_t)st.nw * 16, 128);
-                                wg_mma<NM>(acc, ad, bd, accum);
-                                accum = 1;
+                            auto mma_smem_a = [&]() {
+                                for (int kk = 0; kk < st.kc; kk += 16) {
+                                    const uint64_t ad = wg_desc(a_base + (uint32_t)((st.a_col + kk) >> 3) * (kTileM * 16), kTileM * 16, 128);
+                                    const uint64_t bd = wg_desc(b_base + (uint32_t)((kk >> 3) * st.nw * 16), (uint32_t)st.nw * 16, 128);
+                                    wg_mma<NM>(acc, ad, bd, accum);
+                                    accum = 1;
+                                }
+                            };
+                            if constexpr (kRegAct) {
+                                if (from_x) mma_smem_a();
+                                else {
+                                    // K-steps a_col / 16 .. (a_col + kc) / 16 - 1 of the activations: one branch per K-step keeps
+                                    // every register index a compile-time constant
+                                    const int k0 = st.a_col >> 4, k1 = (st.a_col + st.kc) >> 4;
+#pragma unroll
+                                    for (int k = 0; k < 16; ++k) {
+                                        if (k < k0 || k >= k1) continue;
+                                        const uint64_t bd = wg_desc(b_base + (uint32_t)(2 * (k - k0) * st.nw * 16), (uint32_t)st.nw * 16, 128);
+                                        wg_mma_rs<NM>(acc, hreg + 4 * k, bd, accum);
+                                        accum = 1;
+                                    }
+                                }
+                            } else {
+                                mma_smem_a();
                             }
                             wg_commit();
                             // the MMAs of the previous stage have completed: release it (one arrival per warpgroup)
@@ -443,7 +514,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                         wg_wait<0>();
                         wg_fence_operand<NM / 2>(acc);
                         if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
-                        wg_sync();      // every warp's MMAs have read the old activations: the epilogue may overwrite them
+                        if (!kRegAct) wg_sync();     // every warp's MMAs have read the old activations: the epilogue may overwrite them
 
                         const int cb = ch * 256;
                         if (kMode == PP_DGRAD) {
@@ -538,7 +609,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                         unsigned char* timg = kMode == PP_TRAIN_FWD ? A.tape_act + (size_t)tile * A.act_tile_bytes + mn_tc_img_off(gi, L) : nullptr;
                         const float* bias = F32 + gm.bias_off + cb;
                         const bool relu = gm.epi != EPI_LINEAR;
-                        const bool hold = kWide && nch == 2 && ch == 0;
+                        [[maybe_unused]] const bool hold = kWide && nch == 2 && ch == 0;
                         auto put = [&](int cc, uint32_t ha, uint32_t hb, float a0, float a1, float b0, float b1) {
                             const size_t po = (size_t)(cc >> 3) * (kTileM * 16) + (size_t)ra * 16 + (size_t)(cc & 7) * 2;
                             st_shared_u32(Hs + po, ha);
@@ -567,19 +638,22 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
 #pragma unroll
                         for (int jj = 0; jj < JB; ++jj) {
                             const int j = j0 + jj;
-                            const int c = 8 * j + 2 * q4;
-                            if (cb + 8 * j >= gm.n) continue;
+                            // kRegAct: every column group is written, so no register keeps its old value across the
+                            // epilogue; groups past gm.n hold values that no MMA reads (the next K is at most gm.n)
+                            const bool in_n = cb + 8 * j < gm.n;
+                            if (!kRegAct && !in_n) continue;
                             const float2 bv = bvs[jj];
                             float a0 = acc[4 * j] + bv.x, a1 = acc[4 * j + 1] + bv.y, b0 = acc[4 * j + 2] + bv.x, b1 = acc[4 * j + 3] + bv.y;
                             if (relu) { a0 = fmaxf(a0, 0.0f); a1 = fmaxf(a1, 0.0f); b0 = fmaxf(b0, 0.0f); b1 = fmaxf(b1, 0.0f); }
-                            if (want_sigma) {
+                            if (want_sigma && in_n) {
                                 const float2 s = svs[jj];
                                 sacc_a = fmaf(a1, s.y, fmaf(a0, s.x, sacc_a));
                                 sacc_b = fmaf(b1, s.y, fmaf(b0, s.x, sacc_b));
                             }
                             const uint32_t ha = pack_h2(a0, a1), hb = pack_h2(b0, b1);
-                            if (hold) { held[(2 * j) % (NM / 4)] = ha; held[(2 * j + 1) % (NM / 4)] = hb; }
-                            else if (publish) put(cb + c, ha, hb, a0, a1, b0, b1);
+                            if constexpr (kRegAct) { hreg[2 * j] = ha; hreg[2 * j + 1] = hb; }
+                            else if (hold) { held[(2 * j) % (NM / 4)] = ha; held[(2 * j + 1) % (NM / 4)] = hb; }
+                            else if (publish) put(cb + 8 * j + 2 * q4, ha, hb, a0, a1, b0, b1);
                         }
                         }
                         if (kWide && nch == 2 && ch == 1 && publish) {
@@ -589,7 +663,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                         }
                     }
                     if (kMode == PP_DGRAD || rgb) return;
-                    if (publish) fence_proxy_async();    // generic-proxy stores to H -> visible to the tensor core
+                    if (!kRegAct && publish) fence_proxy_async();    // generic-proxy stores to H -> visible to the tensor core
                     if (want_sigma) {
                         sacc_a += __shfl_xor_sync(0xffffffffu, sacc_a, 1);
                         sacc_a += __shfl_xor_sync(0xffffffffu, sacc_a, 2);
@@ -618,7 +692,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                             }
                         }
                     }
-                    wg_sync();          // this layer's activations are complete before the next GEMM's MMAs read them
+                    if (!kRegAct) wg_sync();          // this layer's activations are complete before the next GEMM's MMAs read them
                 };
                 const int n = gm.n;
                 if (n > 128) gemm(std::integral_constant<int, 256>{});
