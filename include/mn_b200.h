@@ -232,6 +232,45 @@ size_t mn_model_density_grid_workspace_bytes(const mn_model* m, int precision);
 int mn_model_density_grid(mn_ctx* ctx, mn_model* m, int use_coarse, const float offset[3], const float scale[3], int reso,
                           int64_t row0, int64_t n_rows, int precision, float* sigma_out_d, void* workspace_d,
                           size_t workspace_bytes, void* stream);
+/* ---- expert-parallel ("one centroid per GPU") query --------------------------- models/mega_nerf.py:19-61 ----
+ * MegaNeRF.forward with sub-module k evaluated on rank k mod world only (mega_nerf_b200/expert_parallel.py).  Three device
+ * steps around two equal-split all-to-alls, none of which synchronises the host or takes a size from the device:
+ *   home:  mn_model_route -> mn_model_ep_dispatch -> [send segments, counts]
+ *   owner: mn_model_forward_assigned on the received segments -> [results]
+ *   home:  mn_model_ep_combine on the returned segments.
+ * Every rank must query the same row count B: the segments are sized from it.
+ *
+ * Rows of one segment: B x max_multiplicity (mn_model_set_max_multiplicity; 1 under hard routing), the router's own slot
+ * bound, so the pairs of one query fit any one segment.  A row within the margin of more sub-modules than max_multiplicity
+ * can push a segment past it; its result is then NaN and MN_ERR_WORKSPACE follows at the next mn_check_status. */
+int64_t mn_model_ep_segment_rows(const mn_model* m, int64_t B);
+/* Dispatch (mega_nerf.py:19-61, the `cluster_mask` selection of every sub-module): the (row, sub-module) pairs of
+ * x_d [B, cols] (the model's rows; the first 3 columns are routing-only with xyz_real) from the router's output - assign_d
+ * int32 [B] (boundary_margin == 1) or weights_d [B, n_sub] (> 1, pairs where the weight is > 0) - ordered by destination
+ * rank (k mod world), sub-module, row.  Pair p for destination d occupies row d * S + p (S = mn_model_ep_segment_rows) of:
+ *   send_d [world * S, c + 1 (+1)]: the child's input (cols - 3 with xyz_real, else cols columns), the sub-module id as a
+ *     float and, if sigma_noise_d [B] is given, the row's density noise; rows past a segment's pairs carry id -1;
+ *   pair_row_d int32 [world * S] (home row, -1 past the pairs) and pair_w_d [world * S] (blend weight; margin > 1 only).
+ * counts_d int32 [world, n_sub]: pairs per (destination, sub-module).  row_slots_d int32: [B] the slot of each row's pair
+ * (hard routing) or [B, n_sub] the slot per sub-module, -1 where none (margin > 1) - what mn_model_ep_combine reads. */
+size_t mn_model_ep_dispatch_workspace_bytes(const mn_model* m, int64_t B, int world);
+int mn_model_ep_dispatch(mn_ctx* ctx, mn_model* m, const float* x_d, int64_t B, int cols, const int32_t* assign_d,
+                         const float* weights_d, const float* sigma_noise_d, int world, float* send_d, int32_t* counts_d,
+                         int32_t* pair_row_d, float* pair_w_d, int32_t* row_slots_d, void* workspace_d, size_t workspace_bytes,
+                         void* stream);
+/* Owner call (mega_nerf.py:19-61, `sub_module(x[cluster_mask])` of the sub-modules this rank owns): rows_d [n, cols + 1 (+1)]
+ * in the layout mn_model_ep_dispatch sends - the child's input (cols columns), the sub-module id, the density noise iff
+ * has_noise - each row through its own sub-module, all in one call; rows with id -1 are skipped (their out_d rows are not
+ * written).  out_d [n, rgb_dim + 1].  Only the weights of the sub-modules that occur need to be set. */
+size_t mn_model_forward_assigned_workspace_bytes(const mn_model* m, int64_t n, int precision);
+int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, int precision,
+                              float* out_d, void* workspace_d, size_t workspace_bytes, void* stream);
+/* Combine (mega_nerf.py:34,46-49): out_d [B, rgb_dim + 1] from back_d [world * S, rgb_dim + 1] (the owners' results in
+ * the dispatch's slots): every row starts from 0 and adds back x w over its pairs in ascending sub-module order, multiply
+ * and add rounded separately as `results[mask] += sub_result * weights[mask, i]`; hard routing copies the row's result.
+ * row_slots_d / pair_w_d as written by mn_model_ep_dispatch. */
+int mn_model_ep_combine(mn_ctx* ctx, mn_model* m, int64_t B, const int32_t* row_slots_d, const float* pair_w_d, const float* back_d,
+                        float* out_d, void* stream);
 /* Counters of the last mn_model_forward on this model, read back lazily (synchronises `stream`):
  * slots = routed (row, sub-module) pairs, tiles = 128-row MLP tiles. */
 int mn_model_last_stats(mn_ctx* ctx, mn_model* m, int64_t* slots, int64_t* tiles, void* stream);

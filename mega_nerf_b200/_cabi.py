@@ -85,6 +85,12 @@ SIGNATURES = {
     'mn_model_forward': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _I, _P, _I, _P, _P, _Z, _P]),
     'mn_model_route': (_I, [_P, _P, C.POINTER(Rows), _L, _P, _P, _P]),
     'mn_model_last_stats': (_I, [_P, _P, C.POINTER(_L), C.POINTER(_L), _P]),
+    'mn_model_ep_segment_rows': (_L, [_P, _L]),
+    'mn_model_ep_dispatch_workspace_bytes': (_Z, [_P, _L, _I]),
+    'mn_model_ep_dispatch': (_I, [_P, _P, _P, _L, _I, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    'mn_model_forward_assigned_workspace_bytes': (_Z, [_P, _L, _I]),
+    'mn_model_forward_assigned': (_I, [_P, _P, _P, _L, _I, _I, _I, _P, _P, _Z, _P]),
+    'mn_model_ep_combine': (_I, [_P, _P, _L, _P, _P, _P, _P, _P]),
     'mn_model_density_grid_workspace_bytes': (_Z, [_P, _I]),
     'mn_model_density_grid': (_I, [_P, _P, _I, C.POINTER(_F), C.POINTER(_F), _I, _L, _L, _I, _P, _P, _Z, _P]),
     'mn_render_rays_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),

@@ -580,6 +580,73 @@ int mn_model_forward(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, i
                               workspace_bytes, nullptr, 0, stream);
 }
 
+// ---- owner side of an expert-parallel query (mega_nerf_b200/expert_parallel.py) ------------------------------------
+// Rows arrive with their sub-module id, so the router's bucket count / scan / scatter run on the ids (no distances) and every
+// sub-module runs on its bucket in one MLP launch sequence, results scattered back to the rows' own indices.
+size_t mn_model_forward_assigned_workspace_bytes(const mn_model* m, int64_t n, int precision) {
+    if (!m || n < 0) return 0;
+    const int64_t cap = slot_capacity(m, n, 1);
+    size_t bytes = 256 + mn_align((size_t)cap * sizeof(int)) + mn_align(mn_route_assigned_scratch_bytes(n));
+    if (precision != MN_PREC_FP32) bytes += mn_mlp_tc_workspace(m, cap / MN_TILE, precision);
+    return bytes;
+}
+
+int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, int precision,
+                              float* out_d, void* workspace_d, size_t workspace_bytes, void* stream) {
+    if (!ctx || !m || n < 0 || cols < 1) return MN_ERR_INVALID;
+    if (m->d.kind != 2) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_assigned: not a MegaNeRF model");
+    const mn_model_desc& d = m->d;
+    const int expected = d.xyz_dim + 3 * (d.pos_dir_dim > 0 ? 1 : 0) + (d.appearance_dim > 0 ? 1 : 0);
+    if (cols != expected) {
+        char buf[256];
+        snprintf(buf, sizeof(buf), "Unexpected input shape: torch.Size([%lld, %d]) (expected: %d, xyz_dim: %d)", (long long)n, cols, expected,
+                 d.xyz_dim);
+        return mn_fail(ctx, MN_ERR_SHAPE, buf);
+    }
+    if (n == 0) return MN_OK;
+    if (!rows_d || !out_d) return MN_ERR_INVALID;
+    if (!workspace_d || workspace_bytes < mn_model_forward_assigned_workspace_bytes(m, n, precision))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward_assigned: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int stride = cols + 1 + (has_noise ? 1 : 0);
+    // mode-0 rows of `cols` columns inside the wider payload row: directions x[:, -4:-1], image index x[:, -1] (nerf.py:146,149)
+    RowSrc src{};
+    src.xyz_dim = d.xyz_dim;
+    src.x = rows_d;
+    src.cols = stride;
+    src.div = 1;
+    src.dirs = rows_d + cols - 4;
+    src.dir_stride = stride;
+    src.idx = rows_d + cols - 1;
+    src.idx_stride = stride;
+
+    const int64_t cap = slot_capacity(m, n, 1);
+    char* ws = (char*)workspace_d;
+    auto carve = [&](size_t b) { char* p = ws; ws += mn_align(b); return p; };
+    int* slot_row = (int*)carve((size_t)cap * sizeof(int));
+    void* scratch = carve(mn_route_assigned_scratch_bytes(n));
+    const float* noise = nullptr;
+    int rc;
+    if ((rc = mn_route_build_assigned(ctx, m, rows_d, n, stride, cols, has_noise, cap, slot_row, scratch, &noise, st))) return rc;
+
+    MlpArgs a{};
+    a.nd = m->nd;
+    a.lay = m->lay;
+    a.packed = m->packed;
+    a.src = src;
+    a.n_sub = d.n_sub;
+    a.B = cap;
+    a.sigma_noise = noise;
+    a.out = out_d;
+    a.out_cols = m->nd.rgb_dim + 1;
+    a.slot_row = slot_row;
+    a.counters = m->counters_d;
+    a.scatter = 1;
+    const int64_t n_tiles = cap / MN_TILE;
+    if (precision == MN_PREC_FP32) return mn_mlp_simt_launch(ctx, a, n_tiles, st);
+    return mn_mlp_tc_launch(ctx, m, a, n_tiles, precision, ws, workspace_bytes - (size_t)(ws - (char*)workspace_d), st);
+}
+
 }  // extern "C"
 
 int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,

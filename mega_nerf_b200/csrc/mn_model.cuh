@@ -143,6 +143,11 @@ int mn_route_build(mn_ctx* ctx, mn_model* m, const RowSrc& src, int64_t B, LiveR
 size_t mn_route_scratch_bytes(const mn_model* m, int64_t B);   // per-row active-set masks (+ blend weights [K][B])
 int mn_route_combine(mn_ctx* ctx, mn_model* m, int64_t B, LiveRows live, const int* row_slots, const float* slot_out, int out_cols,
                      float* out, cudaStream_t st);
+// Buckets of an owner call (mn_model_forward_assigned): n rows of `stride` floats whose column id_col holds the sub-module
+// (-1 = empty slot) and, if has_noise, column id_col + 1 the density noise, copied to *noise_out (inside `scratch`).
+size_t mn_route_assigned_scratch_bytes(int64_t n);
+int mn_route_build_assigned(mn_ctx* ctx, mn_model* m, const float* rows, int64_t n, int stride, int id_col, int has_noise, int64_t cap,
+                            int* slot_row, void* scratch, const float** noise_out, cudaStream_t st);
 // mn_model_forward (inference) over the first live.rows(B) of B rows: the router, the encoders and the MLP tiles see only those,
 // the launch sequence is the one for B rows (csrc/mn_api.cu)
 int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,

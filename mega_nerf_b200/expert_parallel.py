@@ -10,74 +10,32 @@ all-gather alone cannot express this partitioning (SURVEY.md §8e).
 
 Payload per routed pair: the child's input row (xyz, dir, image index: 28 B) + sub-module id (+ density noise) out,
 16 B back.  The exchange is `torch.distributed.all_to_all_single` (NCCL over NVLink on GPUs, gloo in the CPU tests of
-this host logic); the split sizes are exchanged first, which costs one host sync per query - the reference itself syncs
-once per sub-module (`x[cluster_mask]`).  Inference only; every rank must issue the same sequence of queries (true for
-`render_rays` on the foreground network with the same sampling configuration on every rank).
+this host logic).  Inference only; every rank must issue the same sequence of queries (true for `render_rays` on the
+foreground network with the same sampling configuration on every rank).
 
-The two device-side steps are injectable (`route_fn`, `sub_fn`) so that the dispatch / return / accumulation logic is
-testable without a GPU; the defaults call libmn_b200.so (`mn_model_route`, and `NeRF.forward` of the owned sub-module).
+CUDA tensors take the device path: `mn_model_route`, then `mn_model_ep_dispatch` writes the pairs straight into `world`
+segments of a fixed capacity (B x max_multiplicity rows, the router's own slot bound), one all-to-all with equal splits
+moves the segments and one the per-(rank, sub-module) counts, `mn_model_forward_assigned` runs every owned sub-module over
+what arrived in one library call, a third all-to-all returns the results and `mn_model_ep_combine` blends them.  No step
+synchronises the host, so a query can be captured in a CUDA graph (`GraphedRenderRays`); the price is that the segments
+travel padded, and that every rank must query the same row count B.
+
+The torch path - split sizes exchanged and read back (`counts.tolist()`, one host sync per query; the reference itself
+syncs once per sub-module, `x[cluster_mask]`), one `NeRF.forward` per owned sub-module, a Python loop for the blend - serves
+CPU tensors and injected device steps (`route_fn`, `sub_fn`), so that the dispatch / return / accumulation logic is
+testable without a GPU; `plan_dispatch` is the order the device dispatch reproduces.
 """
 from __future__ import annotations
 
 import ctypes as C
+from dataclasses import dataclass
 from typing import Callable, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
 
 from . import _cabi as K
-
-
-class _RouteOnly:
-    """A native MegaNeRF model used for routing only: centroids are set, no weights are packed."""
-
-    def __init__(self, mega):
-        self.mega = mega
-        self.handle = None
-        self.device = None
-        self.stamp = None
-
-    def __del__(self):
-        try:
-            if self.handle is not None:
-                K.lib().mn_model_destroy(self.handle)
-        except Exception:
-            pass
-
-    def sync(self, device: torch.device):
-        from .modules import model_desc
-        L = K.lib()
-        h = K.ctx(device)
-        m = self.mega
-        if self.handle is None or self.device != device:
-            if self.handle is not None:
-                L.mn_model_destroy(self.handle)
-            d = model_desc(m.sub_modules[0], 2, len(m.sub_modules), m.boundary_margin, m.xyz_real, m.cluster_dim_start)
-            out = C.c_void_p()
-            K.check(L.mn_model_create(h, C.byref(d), C.byref(out)), h)
-            self.handle, self.device, self.stamp = out.value, device, None
-        stamp = (m.centroids.data_ptr(), m.centroids._version)
-        if stamp != self.stamp:
-            c = K.f32c(m.centroids.to(device))
-            K.check(L.mn_model_set_centroids(self.handle, K.ptr(c), K.stream_of(device)), h)
-            self.keep, self.stamp = c, stamp
-        return h
-
-    def route(self, x: torch.Tensor) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
-        """-> (assign int64 [B] or None, weights [B,K] or None), like models/mega_nerf.py:21-30."""
-        dev = x.device
-        h = self.sync(dev)
-        xin = K.f32c(x)
-        rows = K.Rows()
-        rows.mode, rows.x_d, rows.cols = 0, xin.data_ptr(), xin.shape[1]
-        B, Kn = xin.shape[0], len(self.mega.sub_modules)
-        if self.mega.boundary_margin > 1:
-            w = torch.empty(B, Kn, device=dev, dtype=torch.float32)
-            K.check(K.lib().mn_model_route(h, self.handle, C.byref(rows), B, None, K.ptr(w), K.stream_of(dev)), h)
-            return None, w
-        a = torch.empty(B, device=dev, dtype=torch.int32)
-        K.check(K.lib().mn_model_route(h, self.handle, C.byref(rows), B, K.ptr(a), None, K.stream_of(dev)), h)
-        return a.long(), None
+from .modules import _Native, get_precision
 
 
 def owner_of(k: int, world: int) -> int:
@@ -110,17 +68,57 @@ class ExpertParallel:
         self.mega = mega
         self.group = group
         self.n_sub = len(mega.sub_modules)
-        self._router = None
+        self._native = None
+        self._torch_path = route_fn is not None or sub_fn is not None
         self.route_fn = route_fn or self._route_native
         self.sub_fn = sub_fn or self._sub_native
-        self.last_pairs = 0          # routed pairs of the last query that originated on this rank
-        self.last_owned = 0          # pairs this rank computed for everybody
+        self._last = (0, 0)
+
+    # routed pairs of the last query that originated on this rank, and pairs this rank computed for everybody; after a
+    # device query these read the device counts back (a host sync) when accessed
+    @property
+    def last_pairs(self) -> int:
+        return int(self._last[0])
+
+    @property
+    def last_owned(self) -> int:
+        return int(self._last[1])
 
     # ---- device-side defaults
+    def native(self, device: torch.device) -> _Native:
+        """The native MegaNeRF of this rank: the centroids (routing) and the weights of the owned sub-modules only, packed
+        on `device`; sub-modules owned elsewhere are never read."""
+        m = self.mega
+        if self._native is None:
+            self._native = _Native(m, 2, list(m.sub_modules), m.centroids, m.boundary_margin, m.xyz_real, m.cluster_dim_start)
+            self._native.packed_subs = set(self.owned())
+            self._native.max_multiplicity = m._native().max_multiplicity
+        self._native.centroids = m.centroids
+        return self._native
+
+    def sync(self, device: torch.device) -> None:
+        """Re-pack the native weights if a parameter changed (in place: a captured graph keeps reading them)."""
+        self.native(device).sync(device)
+
+    def _route_device(self, x: torch.Tensor) -> Tuple[Optional[torch.Tensor], Optional[torch.Tensor]]:
+        """-> (assign int32 [B] or None, weights [B,K] or None), like models/mega_nerf.py:21-30."""
+        dev = x.device
+        nat = self.native(dev)
+        h = nat.sync(dev)
+        rows = K.Rows()
+        rows.mode, rows.x_d, rows.cols = 0, x.data_ptr(), x.shape[1]
+        B = x.shape[0]
+        if self.mega.boundary_margin > 1:
+            w = torch.empty(B, self.n_sub, device=dev, dtype=torch.float32)
+            K.check(K.lib().mn_model_route(h, nat.handle, C.byref(rows), B, None, K.ptr(w), K.stream_of(dev)), h)
+            return None, w
+        a = torch.empty(B, device=dev, dtype=torch.int32)
+        K.check(K.lib().mn_model_route(h, nat.handle, C.byref(rows), B, K.ptr(a), None, K.stream_of(dev)), h)
+        return a, None
+
     def _route_native(self, x):
-        if self._router is None:
-            self._router = _RouteOnly(self.mega)
-        return self._router.route(x)
+        assign, w = self._route_device(K.f32c(x))
+        return (assign.long() if assign is not None else None), w
 
     def _sub_native(self, k: int, rows: torch.Tensor, sigma_noise: Optional[torch.Tensor]) -> torch.Tensor:
         return self.mega.sub_modules[k](rows, sigma_noise=sigma_noise)
@@ -133,6 +131,74 @@ class ExpertParallel:
     def forward(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.mega.parameters()):
             raise RuntimeError('expert-parallel execution is inference-only (wrap the call in torch.no_grad())')
+        if x.is_cuda and not self._torch_path:
+            return self._forward_device(x, sigma_noise)
+        return self._forward_torch(x, sigma_noise)
+
+    # ---- device path: the three steps, each callable on its own (a test can play several ranks on one device)
+    def dispatch(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor], world: int) -> 'Dispatch':
+        """Route x [B, cols] and write its pairs into `world` segments (mn_model_ep_dispatch)."""
+        dev = x.device
+        x = K.f32c(x)
+        assign, weights = self._route_device(x)
+        nat = self.native(dev)
+        L, h = K.lib(), K.ctx(dev)
+        B, cols = x.shape
+        c_in = cols - (3 if self.mega.xyz_real else 0)
+        noise = K.f32c(sigma_noise).view(-1) if sigma_noise is not None else None
+        cap = int(L.mn_model_ep_segment_rows(nat.handle, B))
+        i32 = dict(device=dev, dtype=torch.int32)
+        d = Dispatch(world=world, cap=cap, c_in=c_in, has_noise=noise is not None, assign=assign, weights=weights,
+                     send=torch.empty(world * cap, c_in + 1 + (noise is not None), device=dev, dtype=torch.float32),
+                     counts=torch.empty(world, self.n_sub, **i32), pair_row=torch.empty(world * cap, **i32),
+                     pair_w=torch.empty(world * cap, device=dev, dtype=torch.float32) if weights is not None else None,
+                     row_slots=torch.empty(B * (self.n_sub if weights is not None else 1), **i32))
+        ws = torch.empty(max(int(L.mn_model_ep_dispatch_workspace_bytes(nat.handle, B, world)), 256), device=dev, dtype=torch.uint8)
+        K.check(L.mn_model_ep_dispatch(h, nat.handle, K.ptr(x), B, cols, K.ptr(assign), K.ptr(weights), K.ptr(noise), world,
+                                       K.ptr(d.send), K.ptr(d.counts), K.ptr(d.pair_row), K.ptr(d.pair_w), K.ptr(d.row_slots),
+                                       K.ptr(ws), ws.numel(), K.stream_of(dev)), h)
+        return d
+
+    def compute(self, recv: torch.Tensor, c_in: int, has_noise: bool) -> torch.Tensor:
+        """The owner's share: every received row through its own sub-module (mn_model_forward_assigned) -> [n, rgb_dim + 1];
+        rows with sub-module id -1 are left unwritten."""
+        dev = recv.device
+        nat = self.native(dev)
+        L, h = K.lib(), nat.sync(dev)
+        n = recv.shape[0]
+        prec = K.PRECISIONS[get_precision()]
+        res = torch.empty(n, self.mega.sub_modules[0].rgb_dim + 1, device=dev, dtype=torch.float32)
+        ws = torch.empty(max(int(L.mn_model_forward_assigned_workspace_bytes(nat.handle, n, prec)), 256), device=dev,
+                         dtype=torch.uint8)
+        K.check(L.mn_model_forward_assigned(h, nat.handle, K.ptr(recv), n, c_in, int(has_noise), prec, K.ptr(res), K.ptr(ws),
+                                            ws.numel(), K.stream_of(dev)), h)
+        return res
+
+    def combine(self, d: 'Dispatch', back: torch.Tensor) -> torch.Tensor:
+        """Blend the returned results of a dispatch's pairs at home (mn_model_ep_combine) -> [B, rgb_dim + 1]."""
+        dev = back.device
+        nat = self.native(dev)
+        B = d.row_slots.shape[0] // (self.n_sub if d.pair_w is not None else 1)
+        out = torch.empty(B, back.shape[1], device=dev, dtype=torch.float32)
+        h = K.ctx(dev)
+        K.check(K.lib().mn_model_ep_combine(h, nat.handle, B, K.ptr(d.row_slots), K.ptr(d.pair_w), K.ptr(back), K.ptr(out),
+                                            K.stream_of(dev)), h)
+        return out
+
+    def _forward_device(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor]) -> torch.Tensor:
+        world = dist.get_world_size(self.group)
+        d = self.dispatch(x, sigma_noise, world)
+        recv, recv_counts = torch.empty_like(d.send), torch.empty_like(d.counts)
+        dist.all_to_all_single(recv, d.send, group=self.group)
+        dist.all_to_all_single(recv_counts, d.counts, group=self.group)
+        res = self.compute(recv, d.c_in, d.has_noise)
+        back = torch.empty_like(res)
+        dist.all_to_all_single(back, res, group=self.group)
+        self._last = (_LazySum(d.counts), _LazySum(recv_counts))
+        return self.combine(d, back)
+
+    # ---- torch path
+    def _forward_torch(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         world, rank = dist.get_world_size(self.group), dist.get_rank(self.group)
         B = x.shape[0]
         assign, weights = self.route_fn(x)
@@ -163,7 +229,7 @@ class ExpertParallel:
                 continue
             nz = recv[m, c_in + 1] if sigma_noise is not None else None
             res[m] = self.sub_fn(k, recv[m, :c_in].contiguous(), nz.unsqueeze(1) if nz is not None else None).to(res.dtype)
-        self.last_pairs, self.last_owned = int(rows.shape[0]), int(recv.shape[0])
+        self._last = (int(rows.shape[0]), int(recv.shape[0]))
 
         # results travel back along the same routes
         back = res.new_empty(rows.shape[0], out_cols)
@@ -179,6 +245,32 @@ class ExpertParallel:
                 if bool(m.any()):
                     out[rows[m]] += back[m] * w[m].unsqueeze(-1)
         return out
+
+
+class _LazySum:
+    """Sum of a device tensor, read back when converted to int."""
+
+    def __init__(self, t: torch.Tensor):
+        self.t = t
+
+    def __int__(self) -> int:
+        return int(self.t.sum())
+
+
+@dataclass
+class Dispatch:
+    """One query's dispatch (mn_model_ep_dispatch): `world` segments of `cap` rows each."""
+    world: int
+    cap: int
+    c_in: int                          # child input columns of a payload row (then the sub-module id, then the noise)
+    has_noise: bool
+    assign: Optional[torch.Tensor]     # the router's output: int32 [B] (hard routing) ...
+    weights: Optional[torch.Tensor]    # ... or blend weights [B, K]
+    send: torch.Tensor                 # [world * cap, c_in + 1 (+1)] payload rows
+    counts: torch.Tensor               # int32 [world, K] pairs per (destination, sub-module)
+    pair_row: torch.Tensor             # int32 [world * cap] home row of each slot, -1 past the pairs
+    pair_w: Optional[torch.Tensor]     # [world * cap] blend weight of each slot (blending only)
+    row_slots: torch.Tensor            # int32 [B] or [B, K]: the slots of each row, for the combine
 
 
 def enable(mega, group=None, **kw) -> ExpertParallel:

@@ -52,6 +52,11 @@ class GraphedRenderRays:
         self.warmup = warmup
         self._natives = [_unwrap(m)._native() for m in (nerf, bg_nerf) if m is not None]
         self._params = [p for nat in self._natives for sub in nat.subs for p in sub.parameters()]
+        # a foreground network under expert parallelism (mega_nerf_b200/expert_parallel.py) is queried through the rank's own
+        # native model, which holds the owned sub-modules only
+        ep = getattr(_unwrap(nerf), '_ep', None)
+        if ep is not None:
+            self._natives[0] = ep
         self._versions = -1
 
     def _weights_version(self) -> int:

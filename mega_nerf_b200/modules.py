@@ -138,6 +138,7 @@ class _Native:
         self.stamp = None
         self.keep = []
         self.max_multiplicity = None      # None: the library's geometric default (mn_model_create)
+        self.packed_subs = None           # indices of the sub-modules whose weights are packed; None: all
 
     def invalidate(self):
         """Force a re-pack of the native weights at the next call.  Needed only after updates that bypass autograd's
@@ -167,9 +168,12 @@ class _Native:
     def _sd(sub: nn.Module):
         return {k: v for k, v in sub.state_dict().items()}
 
+    def _packed(self):
+        return [(i, sub) for i, sub in enumerate(self.subs) if self.packed_subs is None or i in self.packed_subs]
+
     def _stamp(self):
         s = []
-        for sub in self.subs:
+        for _, sub in self._packed():
             for p in sub.parameters():
                 s.append((p.data_ptr(), p._version))
         if self.centroids is not None:
@@ -201,7 +205,7 @@ class _Native:
                 c = K.f32c(self.centroids.to(device))
                 keep.append(c)
                 K.check(L.mn_model_set_centroids(self.handle, K.ptr(c), st), h)
-            for i, sub in enumerate(self.subs):
+            for i, sub in self._packed():
                 sd = self._sd(sub)
                 w = K.NerfWeights()
 
