@@ -49,9 +49,9 @@ __global__ void __launch_bounds__(256) pack_ops_kernel(const PackOp* __restrict_
             case PK_TC_F32:           // copy with zero padding
                 reinterpret_cast<float*>(op.dst)[i] = i < op.p[0] ? src[i] : 0.0f;
                 break;
-            case PK_RGBW: {           // K-major Wt[k][c] -> [c][k]
-                const int K = op.p[0], Cc = op.p[1];
-                reinterpret_cast<float*>(op.dst)[(i % Cc) * K + i / Cc] = src[i];
+            case PK_RGBW: {           // K-major Wt[k][c] -> [c][k], rows p[2] floats apart (0: K)
+                const int K = op.p[0], Cc = op.p[1], ld = op.p[2] > 0 ? op.p[2] : K;
+                reinterpret_cast<float*>(op.dst)[(i % Cc) * ld + i / Cc] = src[i];
                 break;
             }
         }

@@ -1,10 +1,11 @@
 #pragma once
 
-// Layer-GEMM path for networks wider than the fused kernel covers (512 < layer_dim <= 2048, a multiple of 256), and for the
-// spherical-harmonics heads of degree 3 and 4 (32 < rgb_dim <= MN_TC_LG_RGB_MAX) at every width the fused kernel covers
-// (64..256, a multiple of 64, and 512): its rgb head is not a GEMM, so a wider head needs no new tiling, and N is padded to
-// 256-column blocks anyway (zero weights and biases in the padding; the next GEMM reads only the first L columns).  Included
-// inside mn_mlp_tc.cu's anonymous namespace after mn_mlp_wg.cuh (whose wgmma wrappers it uses).
+// Layer-GEMM path for every network the fused kernel does not take: layer_dim 64..4096 of any value, 1..MN_MAX_LAYERS trunk
+// layers, and the spherical-harmonics heads of degree 3 and 4 (32 < rgb_dim <= MN_TC_LG_RGB_MAX) at every width.  Its rgb head
+// is not a GEMM, so a wider head needs no new tiling.  N is padded to 256-column blocks and every activation image to a multiple
+// of 128 columns (lg_cols in mn_mlp_tc.cu), with zero weights and biases in the padding: the padded columns are exactly 0, and
+// each GEMM reads its input images' padded width as K, so no kernel here has an N or K tail.  Included inside mn_mlp_tc.cu's
+// anonymous namespace after mn_mlp_wg.cuh (whose wgmma wrappers it uses).
 //
 // One 128-row tile of 2048-wide fp16 activations is 512 KiB and one 2048 x 2048 layer 8 MiB of fp16 weights, so neither
 // fits in shared memory.  Each Linear of the network is one launch of tc_layer_gemm_kernel, Y = act(X W^T + b), with the
@@ -278,8 +279,8 @@ struct LhArgs {
     int64_t h_tile_bytes, h_lo;                       // lo-plane offset (tc_f16x3) or 0
     const unsigned char* g;                           // rgb head input: G, or the last trunk activations
     int64_t g_tile_bytes, g_lo;
-    int L, rgb_in;
-    float* tape_f32;                                  // recording call: fp32 head blocks of the tape [tiles][MN_TC_F32_ROWS][128], or NULL
+    int L, rgb_in;                                    // columns the sigma / rgb loops read: L, rgb_in rounded up to 8 (zero weights)
+    float* tape_f32;                                 // recording call: fp32 head blocks of the tape [tiles][MN_TC_F32_ROWS][128], or NULL
 };
 
 // 8 consecutive columns c0 .. c0 + 7 of row t of a tile image, as fp32 (hi + lo when the lo plane exists)
@@ -385,12 +386,14 @@ struct LdArgs {
     const float* tape_f32;                            // fp32 head blocks of the tape (all tiles)
     const unsigned char* g;                           // G activation image of tile 0 of the group (tape)
     int64_t g_tile_bytes;
-    const unsigned char* wpack;                       // forward pack: rgb weights [rgb_dim][L/2] in the fp32 block
+    const unsigned char* wpack;                       // forward pack: rgb weights [rgb_dim][rgb_k] in the fp32 block
     int64_t sub_bytes;
-    int f32_off, rgb_w_off, half;
+    int f32_off, rgb_w_off;
+    int rgb_k;                                        // L/2 rounded up to 8: the weight rows' stride, zero past L/2
+    int cols;                                         // columns of a dZ_G image (L/2 padded; zeros from rgb_k on)
     float* gf32;                                      // head-gradient blocks of the group [tiles][mn_tc_g32_rows][128]
-    unsigned char* dz;                                // dZ_G images of the group [tiles][L/2/8][128][8], S x dZ in fp16
-    float* emb_sum;                                   // [n_sub][app_count][L/2] or NULL
+    unsigned char* dz;                                // dZ_G images of the group [tiles][cols/8][128][8], S x dZ in fp16
+    float* emb_sum;                                   // [n_sub][app_count][rgb_k] or NULL
     const float* scale;
 };
 
@@ -403,7 +406,7 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_dgrad_kernel(const LdArg
     const int64_t slot = tile * kTileM + t;
     const int64_t row = A.m.row_of_slot(slot, n_slots);
     const int sub = A.m.sub_of_tile(tile);
-    const int R = A.m.nd.rgb_dim, half = A.half;
+    const int R = A.m.nd.rgb_dim, rk = A.rgb_k;
     const float S = *A.scale;
     const float* tf = A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + t;
     float d[kR];
@@ -418,15 +421,17 @@ __global__ void __launch_bounds__(kTileM) tc_layer_head_dgrad_kernel(const LdArg
     const int id = (int)tf[MN_TC_F32_ID * kTileM];
     const float* Wr = reinterpret_cast<const float*>(A.wpack + (size_t)sub * A.sub_bytes + A.f32_off) + A.rgb_w_off;
     const unsigned char* gimg = A.g + (int64_t)blockIdx.x * A.g_tile_bytes + (size_t)t * 16;
-    unsigned char* dimg = A.dz + (int64_t)blockIdx.x * half * (kTileM * 2) + (size_t)t * 16;
-    float* sums = A.emb_sum ? A.emb_sum + (size_t)sub * A.m.nd.app_count * half : nullptr;
-    for (int k0 = 0; k0 < half; k0 += 8) {
+    unsigned char* dimg = A.dz + (int64_t)blockIdx.x * A.cols * (kTileM * 2) + (size_t)t * 16;
+    float* sums = A.emb_sum ? A.emb_sum + (size_t)sub * A.m.nd.app_count * rk : nullptr;
+    for (int k0 = 0; k0 < rk; k0 += 8) {
         float v[8];
-        tc_rgb_dgrad8<kR>(Wr, half, k0, d, R, gimg + (size_t)(k0 >> 3) * (kTileM * 16), v);
-        if (sums) tc_emb_sums8(sums + k0, half, row >= 0, id, lane, v);
+        tc_rgb_dgrad8<kR>(Wr, rk, k0, d, R, gimg + (size_t)(k0 >> 3) * (kTileM * 16), v);
+        if (sums) tc_emb_sums8(sums + k0, rk, row >= 0, id, lane, v);
         uint32_t pk[4];
 #pragma unroll
         for (int e = 0; e < 4; ++e) pk[e] = pack_h2(v[2 * e] * S, v[2 * e + 1] * S);
         *reinterpret_cast<uint4*>(dimg + (size_t)(k0 >> 3) * (kTileM * 16)) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
     }
+    // the image's padding columns: zero gradients for the data-gradient GEMM and the weight gradient of dir_a_encoding
+    for (int k0 = rk; k0 < A.cols; k0 += 8) *reinterpret_cast<uint4*>(dimg + (size_t)(k0 >> 3) * (kTileM * 16)) = make_uint4(0, 0, 0, 0);
 }

@@ -16,8 +16,8 @@
 // The epilogue's per-row 16-byte stores and the packer's images are contiguous in this layout, any K that
 // is a multiple of 16 works, and no TMA tensor map is needed (plain 1-D bulk copies).
 //
-// Networks wider than 512, and the spherical-harmonics heads of degree 3 and 4 (rgb_dim 48, 75) at any width, run on the
-// layer-GEMM engine instead (mn_layer_gemm.cuh).  Host side: tc_linears lists the
+// Every other network of 64..4096 wide and 1..16 trunk layers, and the spherical-harmonics heads of degree 3 and 4 (rgb_dim 48,
+// 75) at any width, run on the layer-GEMM engine instead (mn_layer_gemm.cuh).  Host side: tc_linears lists the
 // network's Linears once; tc_net picks the engine and the training coverage from that table, and builds the forward plan of
 // either engine (build_plan) and the data-gradient plan (build_dgrad_plan); every entry point below calls it once.
 // mn_mlp_tc_pack writes the forward images of either engine, tc_dgrad_ready / tc_pack_dgrad the transposed images of the
@@ -33,7 +33,7 @@
 namespace {
 
 constexpr int kTileM = MN_TILE;
-constexpr int kMaxGemm = 16;
+constexpr int kMaxGemm = MN_MAX_LAYERS + 2;     // layer engine: every trunk layer, xyz_encoding_final and dir_a_encoding
 
 enum { SRC_H = 0, SRC_XPE = 1, SRC_XAUX = 2 };
 enum { EPI_RELU = 0, EPI_RELU_SIGMA = 1, EPI_LINEAR = 2, EPI_RGB = 3,
@@ -68,6 +68,13 @@ struct TcPlan {
 };
 
 int pad16(int x) { return (x + 15) / 16 * 16; }
+int pad8(int x) { return (x + 7) / 8 * 8; }
+
+// Layer engine: every activation image (and so every hidden K segment) is padded to a multiple of kLgCols columns, the
+// 128-channel output block of the weight-gradient kernel.  The padded columns hold exactly 0: zero weights and zero bias,
+// then ReLU (or none), so every GEMM reads whole K slabs and no kernel has a column tail.
+constexpr int kLgCols = 128;
+int lg_cols(int x) { return (x + kLgCols - 1) / kLgCols * kLgCols; }
 
 // ---- the network's Linears in forward order (nerf.py:115-160): trunk layers 0 .. layers-1, xyz_encoding_final,
 // dir_a_encoding, rgb.  The forward and data-gradient plans, the weight packs and the weight-gradient items of the backward all
@@ -79,6 +86,7 @@ struct TcSeg {
 };
 struct TcLinear {
     int n;               // output features
+    int cols;            // columns of the output's activation image (n, or lg_cols(n) on the layer engine)
     int nseg;
     TcSeg seg[2];
     int kin;             // in_features
@@ -89,46 +97,52 @@ struct TcLinear {
 struct TcLinears {
     int n, n_trunk;
     int kpe, kaux;       // padded feature-tile widths
+    int hc, gc;          // columns of the H / F images and of the G image (L and L/2 unless padded for the layer engine)
     TcLinear l[MN_MAX_LAYERS + 3];
 };
 
-TcLinears tc_linears(const mn_model& m) {
+// layer: the table of the layer engine, whose activation images are padded to lg_cols; the fused engine's are not.
+TcLinears tc_linears(const mn_model& m, bool layer) {
     const NetDims& nd = m.nd;
     TcLinears T{};
     T.kpe = pad16(nd.in_xyz);
     T.kaux = nd.aux > 0 ? pad16(nd.aux) : 0;
+    T.hc = layer ? lg_cols(nd.L) : nd.L;
+    T.gc = layer ? lg_cols(nd.L / 2) : nd.L / 2;
     const TcSeg pe{SRC_XPE, T.kpe, nd.in_xyz, 0};
-    auto h = [](int k, int in0) { return TcSeg{SRC_H, k, k, in0}; };
-    auto add = [&](int n, TcSeg s0, int kin, int w, int b, int bwd, int epi) -> TcLinear& {
+    const TcSeg hs{SRC_H, T.hc, nd.L, 0};              // the previous Linear's H or F image
+    auto add = [&](int n, int cols, TcSeg s0, int kin, int w, int b, int bwd, int epi) -> TcLinear& {
         TcLinear& l = T.l[T.n++];
-        l = TcLinear{n, 1, {s0, {}}, kin, w, b, bwd, epi};
+        l = TcLinear{n, cols, 1, {s0, {}}, kin, w, b, bwd, epi};
         return l;
     };
     for (int i = 0; i < nd.layers; ++i) {
-        TcLinear& l = add(nd.L, i == 0 ? pe : h(nd.L, 0), m.lay.kin[i], m.lay.w[i], m.lay.b[i], i > 0 ? m.blay.w[i] : -1,
+        TcLinear& l = add(nd.L, T.hc, i == 0 ? pe : hs, m.lay.kin[i], m.lay.w[i], m.lay.b[i], i > 0 ? m.blay.w[i] : -1,
                           i == nd.layers - 1 ? EPI_RELU_SIGMA : EPI_RELU);
         if (i > 0 && ((nd.skip_mask >> i) & 1)) {      // cat[PE, h]: PE columns first
             l.nseg = 2;
             l.seg[0] = pe;
-            l.seg[1] = h(nd.L, nd.in_xyz);
+            l.seg[1] = TcSeg{SRC_H, T.hc, nd.L, nd.in_xyz};
         }
     }
     T.n_trunk = T.n;
     if (nd.has_dir_a) {                                // has_dir_a implies aux > 0: dir_a_encoding reads [F, dir PE + embedding]
-        add(nd.L, h(nd.L, 0), nd.L, m.lay.final_w, m.lay.final_b, m.blay.final_w, EPI_LINEAR);
-        TcLinear& d = add(nd.L / 2, h(nd.L, 0), nd.L + nd.aux, m.lay.dira_w, m.lay.dira_b, m.blay.dira_f, EPI_RELU);
+        add(nd.L, T.hc, hs, nd.L, m.lay.final_w, m.lay.final_b, m.blay.final_w, EPI_LINEAR);
+        TcLinear& d = add(nd.L / 2, T.gc, hs, nd.L + nd.aux, m.lay.dira_w, m.lay.dira_b, m.blay.dira_f, EPI_RELU);
         d.nseg = 2;
         d.seg[1] = TcSeg{SRC_XAUX, T.kaux, nd.aux, nd.L};
     }
-    add(nd.rgb_dim, h(nd.rgb_in, 0), nd.rgb_in, m.lay.rgb_w, m.lay.rgb_b, -1, EPI_RGB);
+    add(nd.rgb_dim, nd.rgb_dim, TcSeg{SRC_H, nd.rgb_in, nd.rgb_in, 0}, nd.rgb_in, m.lay.rgb_w, m.lay.rgb_b, -1, EPI_RGB);
     return T;
 }
 
 // ---- forward plan of either engine: one GEMM per Linear, the weight images back to back in a precision plane, the fp32 block
 // [biases][sigma_w (L)][sigma_b (4)].  The fused engine (tc_mlp_wg_kernel) runs every GEMM in one launch, the rgb head as an
 // N = 32 GEMM, and reserves bstride floats per bias.  The layer engine (mn_layer_gemm.cuh) launches one GEMM per Linear with
-// N padded to 256-column blocks, in the image and in the bias; its rgb head is not a GEMM: tc_layer_head_kernel reads
-// [rgb_w [rgb_dim][rgb_in]][rgb_b (mn_tc_lg_rgb_bound(rgb_dim))] from the end of the fp32 block (lg_net).
+// N padded to 256-column blocks, in the image and in the bias, and K padded as its input images are (TcLinears::hc); its rgb
+// head is not a GEMM: tc_layer_head_kernel reads [rgb_w [rgb_dim][pad8(rgb_in)]][rgb_b (mn_tc_lg_rgb_bound(rgb_dim))] from
+// the end of the fp32 block (lg_net), and sigma_w takes pad8(L) floats there.  The fp32 padding is zero (the pack is zeroed
+// once at allocation and repacks write only the real entries), so the head loops run over whole groups of 8 columns.
 void build_plan(const NetDims& nd, const TcLinears& T, bool layer, TcPlan* p) {
     TcPlan& P = *p;
     P = TcPlan{};
@@ -153,18 +167,21 @@ void build_plan(const NetDims& nd, const TcLinears& T, bool layer, TcPlan* p) {
     }
     P.plane_bytes = woff;
     P.sigma_w_off = foff;
-    P.f32_floats = foff + nd.L + 4 + (layer ? nd.rgb_dim * nd.rgb_in + mn_tc_lg_rgb_bound(nd.rgb_dim) : 0);
+    P.f32_floats = layer ? foff + pad8(nd.L) + 4 + nd.rgb_dim * pad8(nd.rgb_in) + mn_tc_lg_rgb_bound(nd.rgb_dim) : foff + nd.L + 4;
     P.f32_off = woff * 2;
     P.sub_bytes = (int)mn_align((size_t)woff * 2 + (size_t)P.f32_floats * 4, 256);
     P.x_tile_bytes = (P.kpe + P.kaux) * kTileM * 2;
 }
 
 // ---- data-gradient chain of the backward (training, needs dir_a_encoding): dX of every Linear from dir_a_encoding down to trunk
-// layer 1, restricted to its L hidden input columns, each a GEMM on the Linear's transposed weight image [L/256][out/8][256][8]
-// fp16 (at L = 256 the [K/8][N][8] image of the fused kernel).  The images follow each other in that order, then the fp32
-// block [sigma_w (L)][rgb_w [rgb_dim][L/2]].  The fused engine runs the plan in tc_mlp_wg_kernel<PP_DGRAD>; the layer
-// engine reads the images' offsets from it (one tc_layer_gemm_kernel<false, true> launch each) and ignores rgb_w.
-void build_dgrad_plan(const NetDims& nd, const TcLinears& T, TcPlan* p) {
+// layer 1, restricted to its L hidden input columns, each a GEMM on the Linear's transposed weight image [N/256][K/8][256][8]
+// fp16 (at L = 256 the [K/8][N][8] image of the fused kernel), N = the hidden input columns, K = the Linear's output columns.
+// On the layer engine K is the width of the output's gradient image (TcLinear::cols) and N is padded to 256-column blocks,
+// both with zero weights.  The images follow each other in that order, then the fp32 block [sigma_w (hc)][rgb_w [rgb_dim][L/2]]
+// (sigma_w zero-padded to the H image's columns, which the layer engine's dsigma epilogue reads).  The fused engine runs the plan
+// in tc_mlp_wg_kernel<PP_DGRAD>; the layer engine reads the images' offsets from it (one tc_layer_gemm_kernel<false, true>
+// launch each) and ignores rgb_w.
+void build_dgrad_plan(const NetDims& nd, const TcLinears& T, bool layer, TcPlan* p) {
     TcPlan& P = *p;
     P = TcPlan{};
     P.L = nd.L;
@@ -173,10 +190,10 @@ void build_dgrad_plan(const NetDims& nd, const TcLinears& T, TcPlan* p) {
     for (int j = T.n - 2; j >= 1; --j) {     // T.l[T.n - 1] is the rgb Linear: its input gradient comes from the head stage
         const int epi = T.l[j - 1].epi;      // of the Linear whose output gradient this GEMM produces (tape image j - 1)
         TcGemm& g = P.g[ng++];
-        g.n = nd.L;
+        g.n = layer ? (nd.L + 255) / 256 * 256 : nd.L;
         g.nseg = 1;
         g.src[0] = SRC_H;
-        g.k[0] = T.l[j].n;
+        g.k[0] = T.l[j].cols;
         g.w_off = woff;
         g.img = j - 1;
         g.epi = epi == EPI_LINEAR ? EPI_D_LINEAR : epi == EPI_RELU_SIGMA ? EPI_D_MASK_SIGMA : EPI_D_MASK;
@@ -185,16 +202,18 @@ void build_dgrad_plan(const NetDims& nd, const TcLinears& T, TcPlan* p) {
     P.n_gemm = P.n_trunk = ng;
     P.plane_bytes = woff;
     P.sigma_w_off = 0;
-    P.f32_floats = nd.L + nd.rgb_dim * (nd.L / 2);
+    P.f32_floats = T.hc + nd.rgb_dim * (nd.L / 2);
     P.f32_off = woff;
     P.sub_bytes = (int)mn_align((size_t)woff + (size_t)P.f32_floats * 4, 256);
 }
 
 // ---- which engine serves a network, and whether tensor-core training covers it.  The fused engine takes rgb_dim <= 32 (its
-// N = 32 rgb GEMM) at 64..256 and 512 wide; the layer engine everything wider, and the SH heads of degree 3 and 4 (rgb_dim
-// <= MN_TC_LG_RGB_MAX) at the fused engine's widths too.  Training runs on either engine at 256 and 512 wide, on the layer
-// engine above; it needs dir_a_encoding (its data-gradient chain ends there) and no affine appearance.
+// N = 32 rgb GEMM) at 64..256 (a multiple of 64) and 512 wide, up to 12 trunk layers; the layer engine every other width of
+// 64..kLgMaxL and depth (up to MN_MAX_LAYERS), and the SH heads of degree 3 and 4 (rgb_dim <= MN_TC_LG_RGB_MAX).  Training
+// runs on the fused engine at 256 and 512 wide (up to 10 trunk layers) and on the layer engine from 256 wide; it needs
+// dir_a_encoding (its data-gradient chain ends there) and no affine appearance.
 enum { TC_NONE = 0, TC_FUSED = 1, TC_LAYER = 2 };
+constexpr int kLgMaxL = 4096;
 struct TcNet {
     int engine;
     bool train;          // tensor-core training covers the shape (mn_model_train_tc_supported once the weights are packed)
@@ -206,18 +225,18 @@ struct TcNet {
 TcNet tc_net(const mn_model& m) {
     const NetDims& nd = m.nd;
     TcNet t{};
-    t.lin = tc_linears(m);
     const bool fused_width = nd.L % 64 == 0 && (nd.L <= 256 || nd.L == 512) && nd.L >= 64;
-    const bool wide = nd.L > 512 && nd.L <= 2048 && nd.L % 256 == 0;
     if (nd.affine && nd.rgb_dim != 3) t.engine = TC_NONE;
     else if (fused_width && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers <= 12)
         t.engine = TC_FUSED;
-    else if ((wide || (fused_width && nd.rgb_dim > MN_TC_RGB_MAX)) && nd.rgb_dim <= MN_TC_LG_RGB_MAX && nd.layers + 2 <= kMaxGemm)
+    else if (nd.L >= 64 && nd.L <= kLgMaxL && nd.rgb_dim <= MN_TC_LG_RGB_MAX && nd.layers + 2 <= kMaxGemm)
         t.engine = TC_LAYER;
-    if (t.engine != TC_NONE) build_plan(nd, t.lin, t.engine == TC_LAYER, &t.P);
+    const bool layer = t.engine == TC_LAYER;
+    t.lin = tc_linears(m, layer);
+    if (t.engine != TC_NONE) build_plan(nd, t.lin, layer, &t.P);
     t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.layers >= 2 &&
-              ((t.engine == TC_LAYER && nd.L >= 256) || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 10));
-    if (t.train) build_dgrad_plan(nd, t.lin, &t.D);
+              ((layer && nd.L >= 256) || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 10));
+    if (t.train) build_dgrad_plan(nd, t.lin, layer, &t.D);
     return t;
 }
 
@@ -530,26 +549,31 @@ int wg_launch(mn_ctx* ctx, const TcArgs& A, int64_t n_tiles128, cudaStream_t st)
 
 // The layer engine's activation buffers and rgb head, from the forward plan.  GEMM gi writes ping-pong buffer gi % 2 and reads
 // the other one; dir_a_encoding writes G to its own buffer: F went to the other ping-pong buffer, so the head still finds
-// H_last for sigma.  rgb_w and rgb_b follow sigma_w and sigma_b in the fp32 block.
+// H_last for sigma.  The buffers have the padded widths of the activation images (TcLinears::hc, gc).  rgb_w ([rgb_dim][rgb_k])
+// and rgb_b follow sigma_w (sigma_k floats) and sigma_b in the fp32 block (build_plan).
 enum { LB_ACT0 = 0, LB_ACT1 = 1, LB_G = 2 };
 struct LgNet {
     int g_gemm;          // the GEMM that writes LB_G (dir_a_encoding), or -1
     int buf_cols[3];     // columns of each activation buffer (0: unused)
     int h_last;          // buffer of the last trunk activations
     int rgb_src;         // buffer the rgb head reads
+    int sigma_k, rgb_k;  // columns the fp32 heads read: L and rgb_in rounded up to 8 (the padding weights are zero)
     int rgb_w_off, rgb_b_off;
     int in(int gi) const { return (gi + 1) & 1; }
     int out(int gi) const { return gi == g_gemm ? LB_G : gi & 1; }
 };
-LgNet lg_net(const TcPlan& P, const NetDims& nd) {
+LgNet lg_net(const TcNet& net, const NetDims& nd) {
+    const TcPlan& P = net.P;
     LgNet b{};
     b.g_gemm = nd.has_dir_a ? P.n_gemm - 1 : -1;
-    b.buf_cols[LB_ACT0] = b.buf_cols[LB_ACT1] = nd.L;
-    if (nd.has_dir_a) b.buf_cols[LB_G] = P.g[b.g_gemm].n;
+    b.buf_cols[LB_ACT0] = b.buf_cols[LB_ACT1] = net.lin.hc;
+    if (nd.has_dir_a) b.buf_cols[LB_G] = net.lin.gc;
     b.h_last = (nd.layers - 1) & 1;
     b.rgb_src = nd.has_dir_a ? LB_G : b.h_last;
-    b.rgb_w_off = P.sigma_w_off + nd.L + 4;
-    b.rgb_b_off = b.rgb_w_off + nd.rgb_dim * nd.rgb_in;
+    b.sigma_k = pad8(nd.L);
+    b.rgb_k = pad8(nd.rgb_in);
+    b.rgb_w_off = P.sigma_w_off + b.sigma_k + 4;
+    b.rgb_b_off = b.rgb_w_off + nd.rgb_dim * b.rgb_k;
     return b;
 }
 
@@ -563,7 +587,7 @@ struct TcWorkspace {
 };
 TcWorkspace tc_workspace(const TcNet& net, const NetDims& nd, int64_t n_tiles128, int precision) {
     const bool layer = net.engine == TC_LAYER;
-    const LgNet B = layer ? lg_net(net.P, nd) : LgNet{};
+    const LgNet B = layer ? lg_net(net, nd) : LgNet{};
     TcWorkspace w{};
     w.group_tiles = layer && n_tiles128 > kLgGroupTiles ? kLgGroupTiles : n_tiles128;
     w.planes = precision == MN_PREC_TC_F16X3 ? 2 : 1;
@@ -666,13 +690,13 @@ static void tc_pack_dgrad(mn_ctx* ctx, mn_model* m, int sub, const TcNet& net) {
     const float* Pk = m->packed + (size_t)sub * m->lay.total;
     for (int gi = 0; gi < D.n_gemm; ++gi) {
         const TcGemm& g = D.g[gi];
-        const int k = g.k[0];
-        mn_pack_push(ctx, PackOp{Q + net.lin.l[g.img + 1].bwd, db + g.w_off, nullptr, (long long)g.n * k, PK_TC_HALF,
-                                 {nd.L, k, g.n, k, 0, 0, 256}});
+        const TcLinear& l = net.lin.l[g.img + 1];
+        const int k = g.k[0];          // l.cols: the output channels past l.n are zero rows of the image
+        mn_pack_push(ctx, PackOp{Q + l.bwd, db + g.w_off, nullptr, (long long)g.n * k, PK_TC_HALF, {nd.L, l.n, g.n, k, 0, 0, 256}});
     }
     float* f32 = reinterpret_cast<float*>(db + D.f32_off);
     mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
-    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + nd.L, nullptr, (long long)nd.rgb_dim * (nd.L / 2), PK_RGBW,
+    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + net.lin.hc, nullptr, (long long)nd.rgb_dim * (nd.L / 2), PK_RGBW,
                              {nd.L / 2, nd.rgb_dim, 0, 0, 0, 0, 0}});
 }
 
@@ -711,20 +735,22 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
         const TcLinear& l = net.lin.l[gi];
         const TcGemm& g = P.g[gi];
         const int K = g.k[0] + g.k[1];
-        // a leading PE segment holds its real columns, then zeros up to its padded width; the other columns follow contiguously
-        const bool pe = l.seg[0].src == SRC_XPE;
+        // the leading segment holds its real columns, then zeros up to its padded width; the second segment's columns follow
+        // contiguously, and columns past in_features (the padding of a second H segment) are zero
         mn_pack_push(ctx, PackOp{Pk + l.w, base + g.w_off, base + P.plane_bytes + g.w_off, (long long)g.n * K, PK_TC_HALF,
-                                 {l.n, l.kin, g.n, K, pe ? l.seg[0].k_real : 0, pe ? l.seg[0].k : 0, g.n < 256 ? g.n : 256}});
+                                 {l.n, l.kin, g.n, K, l.seg[0].k_real, l.seg[0].k, g.n < 256 ? g.n : 256}});
         // the bias fills the floats the plan reserved for it, up to the next bias (sigma_w after the last one)
         const int b_end = gi + 1 < P.n_gemm ? P.g[gi + 1].bias_off : P.sigma_w_off;
         mn_pack_push(ctx, PackOp{Pk + l.b, f32 + g.bias_off, nullptr, (long long)(b_end - g.bias_off), PK_TC_F32, {l.n, 0, 0, 0, 0, 0, 0}});
     }
+    const bool layer = net.engine == TC_LAYER;
+    const LgNet B = layer ? lg_net(net, nd) : LgNet{};
+    const int sigma_k = layer ? B.sigma_k : nd.L;
     mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + P.sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
-    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + P.sigma_w_off + nd.L, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
-    if (net.engine == TC_LAYER) {      // tc_layer_head_kernel computes the rgb head on the CUDA cores
-        const LgNet B = lg_net(P, nd);
+    mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + P.sigma_w_off + sigma_k, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
+    if (layer) {      // tc_layer_head_kernel computes the rgb head on the CUDA cores
         mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + B.rgb_w_off, nullptr, (long long)nd.rgb_dim * nd.rgb_in, PK_RGBW,
-                                 {nd.rgb_in, nd.rgb_dim, 0, 0, 0, 0, 0}});
+                                 {nd.rgb_in, nd.rgb_dim, B.rgb_k, 0, 0, 0, 0}});
         mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + B.rgb_b_off, nullptr, mn_tc_lg_rgb_bound(nd.rgb_dim), PK_TC_F32,
                                  {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
     }
@@ -769,7 +795,8 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet&
     if (!m->tc_ready) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: weights not packed");
     if (n_tiles128 <= 0) return MN_OK;
     const TcPlan& P = net.P;
-    const LgNet B = lg_net(P, m->nd);
+    const LgNet B = lg_net(net, m->nd);
+    const int hc = net.lin.hc;
     const TcWorkspace W = tc_workspace(net, m->nd, n_tiles128, precision);
     if (!tape && (ws_bytes < W.total || !ws)) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
     const bool split = precision == MN_PREC_TC_F16X3;
@@ -805,10 +832,11 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet&
             G.relu = g.epi != EPI_LINEAR;
             LgImg h = buf[B.in(gi)], out = buf[B.out(gi)];
             if (tape) {       // GEMM gi reads image gi - 1 (SRC_H; trunk layer 0 has none) and writes image gi of the activation record
-                h = gi > 0 ? LgImg{rec + mn_tc_img_off(gi - 1, P.L), act_tile, 0} : LgImg{};
-                out = LgImg{rec + mn_tc_img_off(gi, P.L), act_tile, 0};
+                h = gi > 0 ? LgImg{rec + mn_tc_img_off(gi - 1, hc), act_tile, 0} : LgImg{};
+                out = LgImg{rec + mn_tc_img_off(gi, hc), act_tile, 0};
             }
-            const int rc = lg_gemm(ctx, G, a, P, g, m->tc_packed, net.lin.l[gi].n, t0, nt, x, h, out, split, false, st);
+            // every column of the output image, its zero padding included
+            const int rc = lg_gemm(ctx, G, a, P, g, m->tc_packed, net.lin.l[gi].cols, t0, nt, x, h, out, split, false, st);
             if (rc) return rc;
         }
         LhArgs H{};
@@ -826,11 +854,11 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet&
         H.g = buf[B.rgb_src].p;
         H.g_tile_bytes = buf[B.rgb_src].tile_bytes;
         H.g_lo = split ? buf[B.rgb_src].lo : 0;
-        H.L = P.L;
-        H.rgb_in = m->nd.rgb_in;
+        H.L = B.sigma_k;
+        H.rgb_in = B.rgb_k;
         if (tape) {
-            H.h = rec + mn_tc_img_off(a.nd.layers - 1, P.L);
-            H.g = rec + mn_tc_img_off(a.nd.layers + 1, P.L);
+            H.h = rec + mn_tc_img_off(a.nd.layers - 1, hc);
+            H.g = rec + mn_tc_img_off(a.nd.layers + 1, hc);
             H.h_tile_bytes = H.g_tile_bytes = act_tile;
             H.tape_f32 = tape->f32;
         }
@@ -848,8 +876,8 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
     if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net, n_tiles128, precision, ws, ws_bytes, st);
     if (net.engine != TC_FUSED || !m->tc_ready)
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
-                       "tensor-core MLP path covers layer_dim 64..256 (multiple of 64), 512 or 768..2048 (multiple of 256) and rgb_dim <= 80 "
-                       "(sh_deg <= 4), without affine appearance for rgb_dim > 3; use precision 'fp32' for this model");
+                       "tensor-core MLP path covers layer_dim 64..4096 with up to 16 layers and rgb_dim <= 80 (sh_deg <= 4), without "
+                       "affine appearance for rgb_dim > 3; use precision 'fp32' for this model");
     if (a.nd.L > 256 && precision == MN_PREC_TC_F16X3)
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "precision 'tc_f16x3' covers layer_dim <= 256; use 'tc_f16' or 'fp32' for the 512-wide network");
@@ -883,8 +911,8 @@ size_t mn_train_tc_x_tile_bytes(const mn_model* m) {
     return net.engine == TC_NONE ? 0 : (size_t)net.P.x_tile_bytes;
 }
 size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
-    const NetDims& nd = m->nd;
-    return mn_tc_img_off(nd.layers + 1, nd.L) + mn_tc_img_off(1, nd.L / 2);     // ends with G (L/2 columns)
+    const TcNet net = tc_net(*m);
+    return mn_tc_img_off(m->nd.layers + 1, net.lin.hc) + mn_tc_img_off(1, net.lin.gc);     // ends with G (L/2 columns, padded)
 }
 
 // recording forward: encoder tiles and every layer's activations land in the caller's tape
@@ -913,23 +941,28 @@ int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n
 
 // backward workspace: [gradient images][head gradients fp32 [head_tiles][mn_tc_g32_rows(rgb_dim)][128]][embedding sums][scale,
 // max |grad_out|].  Fused engine: the gradient records of every tile.  Layer engine: the gradient images of one tile group only
-// (dZ_G and two ping-pong L-column buffers), so its workspace is bounded by kLgGroupTiles, not by the row count.
+// (dZ_G and two ping-pong H-image-wide buffers), so its workspace is bounded by kLgGroupTiles, not by the row count.  The
+// embedding sums are [n_sub][app_count][emb_k] (emb_k: L/2, rounded up to 8 on the layer engine, whose head stage writes whole
+// groups of 8 columns).
 struct TcBwdWorkspace {
     int64_t head_tiles;
+    int emb_k;
     size_t dz_bytes, head_bytes, emb_floats, total;
 };
 static TcBwdWorkspace tc_bwd_workspace(const mn_model* m, const TcNet& net, int64_t n_tiles128) {
     const NetDims& nd = m->nd;
     TcBwdWorkspace w{};
+    w.emb_k = nd.L / 2;
     if (net.engine == TC_LAYER) {
         w.head_tiles = n_tiles128 < kLgGroupTiles ? n_tiles128 : kLgGroupTiles;
-        w.dz_bytes = mn_align((size_t)w.head_tiles * (nd.L / 2) * kTileM * 2) + 2 * mn_align((size_t)w.head_tiles * nd.L * kTileM * 2);
+        w.dz_bytes = mn_align((size_t)w.head_tiles * net.lin.gc * kTileM * 2) + 2 * mn_align((size_t)w.head_tiles * net.lin.hc * kTileM * 2);
+        w.emb_k = pad8(nd.L / 2);
     } else {
         w.head_tiles = n_tiles128;
         w.dz_bytes = mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m));
     }
     w.head_bytes = mn_align((size_t)w.head_tiles * mn_tc_g32_rows(nd.rgb_dim) * kTileM * sizeof(float));
-    w.emb_floats = nd.app_in_dira ? (size_t)m->d.n_sub * nd.app_count * (nd.L / 2) : 0;
+    w.emb_floats = nd.app_in_dira ? (size_t)m->d.n_sub * nd.app_count * w.emb_k : 0;
     w.total = w.dz_bytes + w.head_bytes + mn_align(w.emb_floats * sizeof(float) + 256) + 1024;
     return w;
 }
@@ -939,7 +972,9 @@ size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
 
 // Weight-gradient entry of Linear j: per input segment, the item of output channels 0..127 and the segment's first X chunk.  X is
 // image j - 1 of the activation record (SRC_H) or a segment of the feature tile; dZ lies at dz_off inside a tile's gradient images.
-static WgLinear wg_linear(const TcLinears& T, int j, int L, int dz_off) {
+// The output channels run in blocks of 128; a last partial block (layer engine: l.n < l.cols) reads the zero padding of the
+// gradient image and stores only the channels below l.n.
+static WgLinear wg_linear(const TcLinears& T, int j, int dz_off) {
     const TcLinear& l = T.l[j];
     WgLinear w{};
     for (int s = 0; s < l.nseg; ++s) {
@@ -947,15 +982,16 @@ static WgLinear wg_linear(const TcLinears& T, int j, int L, int dz_off) {
         WgItem& it = w.seg[s];
         it.dz_off = dz_off;
         it.x_region = g.src == SRC_H ? 0 : 1;
-        it.x_off = g.src == SRC_H ? (int)mn_tc_img_off(j - 1, L) : g.src == SRC_XAUX ? (T.kpe / 8) * (kTileM * 16) : 0;
+        it.x_off = g.src == SRC_H ? (int)mn_tc_img_off(j - 1, T.hc) : g.src == SRC_XAUX ? (T.kpe / 8) * (kTileM * 16) : 0;
         it.n = g.k;
         it.n_real = g.k_real;
+        it.m_real = l.n;
         it.w_off = l.w + g.in0;
         it.k_in = l.kin;
         it.b_off = s == 0 ? l.b : -1;      // the first segment owns the bias
         w.n_chunks[s] = (g.k + 255) / 256;
     }
-    w.n_items = (l.n / 128) * (w.n_chunks[0] + w.n_chunks[1]);
+    w.n_items = ((l.n + 127) / 128) * (w.n_chunks[0] + w.n_chunks[1]);
     return w;
 }
 
@@ -968,7 +1004,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     if (!ws || ws_bytes < WS.total) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_train_tc_backward: workspace too small");
     const NetDims& nd = a.nd;
     const TcLinears& lin = net.lin;
-    const int L = nd.L, half = L / 2;
+    const int L = nd.L, half = L / 2, hc = lin.hc;
     const int64_t act_tile = (int64_t)mn_train_tc_act_tile_bytes(m);
     char* wp = (char*)(((uintptr_t)ws + 255) / 256 * 256);
     unsigned char* dz = (unsigned char*)wp;               wp += WS.dz_bytes;
@@ -1010,6 +1046,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         H.gf32 = gf32;
         H.act_tile_bytes = act_tile;
         H.L = L;
+        H.cols = hc;
         H.layers = nd.layers;
         H.rgb_dim = nd.rgb_dim;
         H.counters = a.counters;
@@ -1037,7 +1074,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         WgArgs W{};
         int64_t items = 0;
         for (int j = j0; j < j1; ++j) {
-            W.lin[j - j0] = wg_linear(lin, j, L, (int)mn_tc_img_off(j - j0, L));
+            W.lin[j - j0] = wg_linear(lin, j, (int)mn_tc_img_off(j - j0, hc));
             items += W.lin[j - j0].n_items;
         }
         W.act = tape.act;
@@ -1103,12 +1140,13 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         // weight gradients.  dZ of Linear j is consumed by its weight gradient before the buffer is overwritten.
         const TcPlan& P = net.P;
         const TcPlan& D = net.D;
+        const LgNet B = lg_net(net, nd);
         const int rows = mn_tc_g32_rows(nd.rgb_dim);
         const int64_t gt = WS.head_tiles;
-        unsigned char* dzg = dz;                              // dZ of dir_a_encoding (L/2 columns)
+        unsigned char* dzg = dz;                              // dZ of dir_a_encoding (gc columns)
         unsigned char* pp[2];
-        pp[0] = dzg + mn_align((size_t)gt * half * kTileM * 2);
-        pp[1] = pp[0] + mn_align((size_t)gt * L * kTileM * 2);
+        pp[0] = dzg + mn_align((size_t)gt * lin.gc * kTileM * 2);
+        pp[1] = pp[0] + mn_align((size_t)gt * hc * kTileM * 2);
 
         for (int64_t t0 = 0; t0 < tiles_used; t0 += gt) {
             const int64_t nt = tiles_used - t0 < gt ? tiles_used - t0 : gt;
@@ -1120,13 +1158,14 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
                 H.tile0 = t0;
                 H.grad_out = a.grad_out;
                 H.tape_f32 = tape.f32;
-                H.g = rec + mn_tc_img_off(nd.layers + 1, L);
+                H.g = rec + mn_tc_img_off(nd.layers + 1, hc);
                 H.g_tile_bytes = act_tile;
                 H.wpack = (const unsigned char*)m->tc_packed;
                 H.sub_bytes = P.sub_bytes;
                 H.f32_off = P.f32_off;
-                H.rgb_w_off = lg_net(P, nd).rgb_w_off;
-                H.half = half;
+                H.rgb_w_off = B.rgb_w_off;
+                H.rgb_k = B.rgb_k;
+                H.cols = lin.gc;
                 H.gf32 = gf32;
                 H.dz = dzg;
                 H.emb_sum = nd.app_in_dira ? emb_sum : nullptr;
@@ -1138,18 +1177,20 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
             // ---- data-gradient GEMM g: dz_out = [mask](dz_in W^T) [+ S dsigma x sigma_w]
             auto dgrad = [&](unsigned char* dz_in, const TcGemm& g, unsigned char* dz_out) -> int {
                 LgArgs G{};
-                G.mask = g.epi != EPI_D_LINEAR ? rec + mn_tc_img_off(g.img, L) : nullptr;     // xyz_encoding_final has no activation
+                G.mask = g.epi != EPI_D_LINEAR ? rec + mn_tc_img_off(g.img, hc) : nullptr;     // xyz_encoding_final has no activation
                 G.mask_tile_bytes = act_tile;
                 G.dsig = g.epi == EPI_D_MASK_SIGMA ? gf32 + MN_TC_G32_SIGMA * kTileM : nullptr;
                 G.dsig_tile_floats = (int64_t)rows * kTileM;
                 G.scale = scale;
-                return lg_gemm(ctx, G, mm, D, g, m->tc_dgrad, L, t0, nt, LgImg{}, LgImg{dz_in, (int64_t)g.k[0] * kTileM * 2, 0},
-                               LgImg{dz_out, (int64_t)L * kTileM * 2, 0}, false, true, st);
+                // every column of the H-wide gradient image: the padding comes out 0 (zero weights, then the mask of a zero
+                // activation), so the next GEMM and the weight gradient read whole blocks
+                return lg_gemm(ctx, G, mm, D, g, m->tc_dgrad, hc, t0, nt, LgImg{}, LgImg{dz_in, (int64_t)g.k[0] * kTileM * 2, 0},
+                               LgImg{dz_out, (int64_t)hc * kTileM * 2, 0}, false, true, st);
             };
             // Linear j (dir_a_encoding down to trunk layer 0): weight gradient, then data-gradient GEMM lin.n - 2 - j gives dZ of j - 1
             unsigned char* dzj = dzg;
             for (int j = lin.n - 2, nxt = 0; j >= 0; --j, nxt ^= 1) {
-                if ((rc = wgrad(j, j + 1, dzj, (int64_t)lin.l[j].n * kTileM * 2, t0, nt))) return rc;
+                if ((rc = wgrad(j, j + 1, dzj, (int64_t)lin.l[j].cols * kTileM * 2, t0, nt))) return rc;
                 if (j == 0) break;
                 if ((rc = dgrad(dzj, D.g[lin.n - 2 - j], pp[nxt]))) return rc;
                 dzj = pp[nxt];
@@ -1159,8 +1200,9 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     }
     // ---- appearance embedding
     if (nd.app_in_dira) {
-        tc_emb_grad_kernel<<<dim3((unsigned)nd.app_count, (unsigned)a.n_sub), 64, 0, st>>>(emb_sum, a.packed_bwd, a.blay.total, a.blay.dira_e, half, nd.app,
-                                                                                          nd.app_count, a.gw, a.lay.total, a.lay.emb);
+        tc_emb_grad_kernel<<<dim3((unsigned)nd.app_count, (unsigned)a.n_sub), 64, 0, st>>>(emb_sum, WS.emb_k, a.packed_bwd, a.blay.total,
+                                                                                          a.blay.dira_e, half, nd.app, nd.app_count, a.gw,
+                                                                                          a.lay.total, a.lay.emb);
         MN_LAUNCH_CHECK(ctx);
     }
     mn_prof_end(ctx, st);

@@ -181,9 +181,11 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st);
 int mn_mlp_tp_program(const mn_model& m, unsigned int* table_out, int cap_entries, int* info8);   // host only (test hook)
 // ---- tensor-core training path (csrc/mn_train_tc.cuh): per-tile tape records and the two passes
 // An activation record (and the backward pass's gradient record, same layout) holds fp16 images in the layout of the MLP
-// kernel's activation buffer, [cols/8][128 slots][8], one every L * 128 * 2 bytes: H_0 .. H_{layers-1}, then F
-// (xyz_encoding_final) at image `layers`, then G (dir_a_encoding, L/2 columns) at image `layers + 1`.
-__host__ __device__ __forceinline__ size_t mn_tc_img_off(int img, int L) { return (size_t)img * L * MN_TILE * 2; }
+// kernel's activation buffer, [cols/8][128 slots][8], one every cols * 128 * 2 bytes: H_0 .. H_{layers-1}, then F
+// (xyz_encoding_final) at image `layers`, then G (dir_a_encoding, L/2 columns) at image `layers + 1`.  cols = L on the fused
+// engine; the layer engine pads L and L/2 to a multiple of 128 columns (zeros), so a 4096-wide, 8-layer record holds about
+// 78 KB per sample.
+__host__ __device__ __forceinline__ size_t mn_tc_img_off(int img, int cols) { return (size_t)img * cols * MN_TILE * 2; }
 // rows of the per-tile fp32 head block [MN_TC_F32_ROWS][128]: sigma pre-activation, rgb (3), image id
 enum { MN_TC_F32_SIGMA = 0, MN_TC_F32_RGB = 1, MN_TC_F32_ID = 4, MN_TC_F32_ROWS = 5 };
 // rows of the backward pass's per-tile fp32 head-gradient block [mn_tc_g32_rows(rgb_dim)][128]: d sigma pre-activation, d rgb
@@ -200,9 +202,9 @@ struct TrainTcTape {
     float* f32;               // fp32 head blocks             [n_tiles][MN_TC_F32_ROWS][128]
 };
 // the shapes whose recording calls run on the tensor cores (tc_net in mn_mlp_tc.cu; mn_model_train_tc_supported)
-#define MN_TC_TRAIN_COVERAGE                                                                                                    \
-    "tensor-core training covers layer_dim 256, 512 or 768..2048 (a multiple of 256) with a direction / appearance head, rgb_dim 3 " \
-    "or a raw SH head (rgb_dim <= 80: sh_deg <= 4), no affine appearance; use train precision 'fp32'"
+#define MN_TC_TRAIN_COVERAGE                                                                                                     \
+    "tensor-core training covers layer_dim 256..4096 (at 256 and 512: up to 10 or 13..16 layers) with a direction / appearance head, " \
+    "rgb_dim 3 or a raw SH head (rgb_dim <= 80: sh_deg <= 4), no affine appearance; use train precision 'fp32'"
 size_t mn_train_tc_x_tile_bytes(const mn_model* m);
 size_t mn_train_tc_act_tile_bytes(const mn_model* m);
 int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st);

@@ -59,6 +59,7 @@ struct WgItem {
     int x_off;        // byte offset of the first X column group inside that record
     int n;            // MMA N = X columns (multiple of 16, <= 256)
     int n_real;       // columns that exist in the weight matrix
+    int m_real;       // output channels that exist from out0 on (fewer than 128 in a padded last block)
     int w_off;        // float offset of W[out0][in0] inside one sub-module's gradient block
     int k_in;         // row stride (in_features) of that weight matrix
     int b_off;        // float offset of bias[out0], or -1 when another item of the same layer owns the bias
@@ -102,6 +103,7 @@ __device__ __forceinline__ WgItem wg_work_item(const WgArgs& A, int y) {
     it.x_off += c * 32 * (kTileM * 16);
     it.n = min(256, it.n - 256 * c);
     it.n_real = min(256, it.n_real - 256 * c);
+    it.m_real -= mh * 128;
     it.w_off += mh * 128 * it.k_in + 256 * c;
     it.b_off = (it.b_off >= 0 && c == 0) ? it.b_off + mh * 128 : -1;
     return it;
@@ -193,20 +195,21 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
             // ---- flush: unscale and accumulate into the fp32 gradient block ([out][in] rows of the nn.Linear weight)
             const float inv = 1.0f / *A.scale;
             float* W = A.gw + (size_t)sub * A.sub_stride;
+            const bool va = ca < it.m_real, vb = cb < it.m_real;
 #pragma unroll
             for (int j = 0; j < NM / 8; ++j) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int c = 8 * j + 2 * q4 + e;
                     if (c < it.n_real) {
-                        atomicAdd(W + it.w_off + (size_t)ca * it.k_in + c, acc[4 * j + e] * inv);
-                        atomicAdd(W + it.w_off + (size_t)cb * it.k_in + c, acc[4 * j + 2 + e] * inv);
+                        if (va) atomicAdd(W + it.w_off + (size_t)ca * it.k_in + c, acc[4 * j + e] * inv);
+                        if (vb) atomicAdd(W + it.w_off + (size_t)cb * it.k_in + c, acc[4 * j + 2 + e] * inv);
                     }
                 }
             }
             if (it.b_off >= 0 && q4 == 0) {
-                atomicAdd(W + it.b_off + ca, accb[0] * inv);
-                atomicAdd(W + it.b_off + cb, accb[2] * inv);
+                if (va) atomicAdd(W + it.b_off + ca, accb[0] * inv);
+                if (vb) atomicAdd(W + it.b_off + cb, accb[2] * inv);
             }
         };
         if (it.n > 128) run(std::integral_constant<int, 256>{});
@@ -222,6 +225,7 @@ struct HeadsArgs {
     const float* gf32;              // head-gradient blocks [n_tiles][mn_tc_g32_rows(rgb_dim)][128], of tile t_min onwards
     int64_t act_tile_bytes;
     int L, layers, rgb_dim;
+    int cols;                       // columns of an H image in the activation record (L, or padded on the layer engine)
     const int* counters;
     int64_t n_tiles;
     int64_t t_min, t_max;           // tiles covered by gf32 (the layer-GEMM path's tile group; 0 .. n_tiles otherwise)
@@ -262,11 +266,11 @@ __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) 
         __syncthreads();
         const unsigned char* rec = A.act + (size_t)t * A.act_tile_bytes;
         if (k < L) {
-            const __half* h = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers - 1, L)) + (size_t)(k >> 3) * (kTileM * 8) + (k & 7);
+            const __half* h = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers - 1, A.cols)) + (size_t)(k >> 3) * (kTileM * 8) + (k & 7);
             for (int r = 0; r < kTileM; ++r) ws = fmaf(G[MN_TC_G32_SIGMA][r], __half2float(h[r * 8]), ws);
         }
         if (nc > 0) {
-            const __half* g = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers + 1, L)) + (size_t)(kc >> 3) * (kTileM * 8) + (kc & 7);
+            const __half* g = reinterpret_cast<const __half*>(rec + mn_tc_img_off(A.layers + 1, A.cols)) + (size_t)(kc >> 3) * (kTileM * 8) + (kc & 7);
             for (int r = 0; r < kTileM; ++r) {
                 const float gv = __half2float(g[r * 8]);
 #pragma unroll
@@ -285,12 +289,13 @@ __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) 
     else if (k < rows) atomicAdd(W + A.rgb_b + (k - 1), bs);
 }
 
-// embedding_a.weight[id][j] += sum_k We[k][j] * S[sub][id][k]     (We = dir_a_encoding columns of the embedding, [L/2][app])
-__global__ void tc_emb_grad_kernel(const float* __restrict__ emb_sum, const float* __restrict__ packed_bwd, int64_t bwd_stride, int dira_e,
-                                   int half, int app, int app_count, float* gw, int64_t sub_stride, int emb_off) {
+// embedding_a.weight[id][j] += sum_k We[k][j] * S[sub][id][k]     (We = dir_a_encoding columns of the embedding, [L/2][app];
+// S rows emb_k >= L/2 floats apart)
+__global__ void tc_emb_grad_kernel(const float* __restrict__ emb_sum, int emb_k, const float* __restrict__ packed_bwd, int64_t bwd_stride,
+                                   int dira_e, int half, int app, int app_count, float* gw, int64_t sub_stride, int emb_off) {
     const int id = blockIdx.x, sub = blockIdx.y, j = threadIdx.x;
     if (j >= app) return;
-    const float* S = emb_sum + ((size_t)sub * app_count + id) * half;
+    const float* S = emb_sum + ((size_t)sub * app_count + id) * emb_k;
     const float* We = packed_bwd + (size_t)sub * bwd_stride + dira_e;
     float acc = 0.0f;
     bool any = false;

@@ -28,11 +28,12 @@ _precision = os.environ.get('MN_B200_PRECISION', 'tc_f16')
 def set_precision(name: str) -> None:
     """'fp32' (CUDA-core parity mode), 'tc_f16' (wgmma, 1 pass) or 'tc_f16x3' (wgmma, split).
 
-    Networks with layer_dim 768..2048 (a multiple of 256; the nerf, npp and mega-nerf-dense configs set 2048) run on the
-    layer-GEMM tensor-core path in 'tc_f16' and 'tc_f16x3' ('tc_f16x3' is the parity-grade mode there); 'fp32' covers
-    layer_dim <= 512 only and refuses them.  So do raw SH heads of degree 3 and 4 (rgb_dim 48, 75) at every width, 64..512
-    included: 'tc_f16x3' serves them at 512 wide too, while it refuses the 512-wide networks of rgb_dim <= 32 (those run on
-    the fused kernel, which covers 'tc_f16' only at that width)."""
+    The tensor-core modes serve every layer_dim of 64..4096 and every depth of 1..16 trunk layers.  64..256 (a multiple of 64)
+    and 512 wide with up to 12 layers and rgb_dim <= 32 run on the fused kernel; every other network - the nerf, npp and
+    mega-nerf-dense configs' 2048, widths such as 96, 640, 1000 or 3072 (padded with zero weights), 13..16 layers, raw SH heads
+    of degree 3 and 4 (rgb_dim 48, 75) - runs on the layer-GEMM tensor-core path in 'tc_f16' and 'tc_f16x3' ('tc_f16x3' is the
+    parity-grade mode there).  'fp32' covers layer_dim <= 512 in multiples of 64 only and refuses the others.  'tc_f16x3'
+    refuses the fused kernel's 512-wide networks (that kernel covers 'tc_f16' only at that width)."""
     global _precision
     if name not in K.PRECISIONS:
         raise ValueError(f'unknown precision {name!r}; choose from {sorted(K.PRECISIONS)}')
@@ -51,11 +52,13 @@ def set_train_precision(name: str) -> None:
     'fp32'   CUDA-core kernels - the parity mode (gradients equal the reference's fp32 autograd to its own noise level);
     'tc_f16' tensor cores: fp16 operands, fp32 accumulation, gradient images scaled by a power of two - what the reference
              does on a GPU under autocast + GradScaler (runner.py:243-274).  The tensor-core training kernels cover
-             layer_dim 256, 512 (up to 10 trunk layers) and 768..2048 (a multiple of 256: the nerf, npp and
-             mega-nerf-dense configs' 2048) with a
+             layer_dim 256..4096 (any width, e.g. the nerf, npp and mega-nerf-dense configs' 2048; at 256 and 512 with up
+             to 10 or with 13..16 trunk layers) with a
              direction / appearance head and either an rgb head (rgb_dim 3) or a raw SH head (rgb_dim <= 80: sh_deg
-             0..4; degrees 3 and 4 on the layer-GEMM path at every one of these widths); other networks (other widths, affine appearance, heads without dir_a_encoding) silently use the
-             fp32 kernels, which refuse layer_dim > 512 - NativeModel.train_on_tensor_cores() tells which."""
+             0..4; degrees 3 and 4 on the layer-GEMM path at every one of these widths); other networks (narrower ones,
+             256 and 512 wide with 11 or 12 layers, affine appearance, heads without dir_a_encoding) silently use the
+             fp32 kernels, which refuse layer_dim > 512 and widths that are not a multiple of 64 -
+             NativeModel.train_on_tensor_cores() tells which."""
     global _train_precision
     if name not in ('fp32', 'tc_f16'):
         raise ValueError(f"unknown train precision {name!r}; choose 'fp32' or 'tc_f16'")
