@@ -271,6 +271,32 @@ int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int
  * row_slots_d / pair_w_d as written by mn_model_ep_dispatch. */
 int mn_model_ep_combine(mn_ctx* ctx, mn_model* m, int64_t B, const int32_t* row_slots_d, const float* pair_w_d, const float* back_d,
                         float* out_d, void* stream);
+/* Training under expert parallelism: the same three steps recording, then their backward in reverse, around the same
+ * equal-split all-to-alls (the result gradients travel home -> owner like the rows).
+ *   home:  mn_model_ep_combine_backward: dback_d [n_slots, rgb_dim + 1] (n_slots = world * S) from dout_d [B, rgb_dim + 1],
+ *          the gradient of mn_model_ep_combine's output: slot s gets w[s] x dout[pair_row[s]] (one fp32 multiply; hard routing
+ *          copies dout[pair_row[s]]), 0 where pair_row[s] is -1.  pair_row_d / pair_w_d as written by mn_model_ep_dispatch.
+ *   owner: mn_model_forward_assigned_train, then mn_model_backward_assigned on the returned result gradients.
+ * The owner's tape is sized by max_pairs, the pairs that actually arrived (the sum of the received counts: one host read per
+ * query), not by the n = world * S padded rows: mn_model_assigned_tape_bytes(m, max_pairs, precision).  The rows stay where
+ * they arrived.  More pairs than max_pairs cannot write past the tape: the extra pairs are dropped, their out_d rows are NaN
+ * and MN_ERR_WORKSPACE follows at the next mn_check_status.
+ * mn_model_forward_assigned_train: mn_model_forward_assigned that also writes the tape; precision MN_PREC_FP32 (the fp32 kernels
+ * of mn_model_forward_train) or MN_PREC_TC_F16 (those of mn_model_forward_train_tc, same coverage); out_d rows with id -1 are NaN.
+ * mn_model_backward_assigned: grad_out_d [n, rgb_dim + 1] is dL/d(out) of the matching recording call (same n, max_pairs,
+ * precision, tape); parameter gradients are ACCUMULATED into param_grads_d as by mn_model_backward (only the sub-modules that
+ * occur in the rows get non-zero entries). */
+int mn_model_ep_combine_backward(mn_ctx* ctx, mn_model* m, int64_t n_slots, const int32_t* pair_row_d, const float* pair_w_d,
+                                 const float* dout_d, float* dback_d, void* stream);
+size_t mn_model_assigned_tape_bytes(const mn_model* m, int64_t max_pairs, int precision);
+size_t mn_model_forward_assigned_train_workspace_bytes(const mn_model* m, int64_t n);
+int mn_model_forward_assigned_train(mn_ctx* ctx, mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, int64_t max_pairs,
+                                    int precision, float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes,
+                                    void* stream);
+size_t mn_model_backward_assigned_workspace_bytes(const mn_model* m, int64_t max_pairs, int precision);
+int mn_model_backward_assigned(mn_ctx* ctx, mn_model* m, int64_t n, int64_t max_pairs, int precision, const float* grad_out_d,
+                               const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes,
+                               void* stream);
 /* Counters of the last mn_model_forward on this model, read back lazily (synchronises `stream`):
  * slots = routed (row, sub-module) pairs, tiles = 128-row MLP tiles. */
 int mn_model_last_stats(mn_ctx* ctx, mn_model* m, int64_t* slots, int64_t* tiles, void* stream);

@@ -91,6 +91,12 @@ SIGNATURES = {
     'mn_model_forward_assigned_workspace_bytes': (_Z, [_P, _L, _I]),
     'mn_model_forward_assigned': (_I, [_P, _P, _P, _L, _I, _I, _I, _P, _P, _Z, _P]),
     'mn_model_ep_combine': (_I, [_P, _P, _L, _P, _P, _P, _P, _P]),
+    'mn_model_ep_combine_backward': (_I, [_P, _P, _L, _P, _P, _P, _P, _P]),
+    'mn_model_assigned_tape_bytes': (_Z, [_P, _L, _I]),
+    'mn_model_forward_assigned_train_workspace_bytes': (_Z, [_P, _L]),
+    'mn_model_forward_assigned_train': (_I, [_P, _P, _P, _L, _I, _I, _L, _I, _P, _P, _Z, _P, _Z, _P]),
+    'mn_model_backward_assigned_workspace_bytes': (_Z, [_P, _L, _I]),
+    'mn_model_backward_assigned': (_I, [_P, _P, _L, _L, _I, _P, _P, _Z, _P, _P, _Z, _P]),
     'mn_model_density_grid_workspace_bytes': (_Z, [_P, _I]),
     'mn_model_density_grid': (_I, [_P, _P, _I, C.POINTER(_F), C.POINTER(_F), _I, _L, _L, _I, _P, _P, _Z, _P]),
     'mn_render_rays_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),

@@ -413,9 +413,9 @@ struct TapeRegions {
     TrainTcTape tc;      // tensor-core tape
 };
 
-// Carves the regions of a tape at `base` into *r (base may be null when only the size is wanted) and returns the tape's size.
-static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, TapeRegions* r = nullptr) {
-    const int64_t cap = slot_capacity(m, B);
+// Carves the regions of a tape of `cap` slots at `base` into *r (base may be null when only the size is wanted) and returns the
+// tape's size; with_w: routed models keep a slot_w region.
+static size_t tape_regions_cap(const mn_model* m, int64_t cap, bool with_w, bool tc, void* base, TapeRegions* r) {
     TapeRegions t{};
     size_t off = 0;
     auto take = [&](size_t n) -> void* {
@@ -426,7 +426,7 @@ static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, Ta
     t.counters = (int*)take(MN_TAPE_HEADER);
     if (m->d.kind == 2) {
         t.slot_row = (int*)take((size_t)cap * sizeof(int));
-        if (m->d.boundary_margin > 1.0f) t.slot_w = (float*)take((size_t)cap * sizeof(float));
+        if (with_w) t.slot_w = (float*)take((size_t)cap * sizeof(float));
     }
     if (tc) {
         const int64_t n_tiles = cap / MN_TILE;
@@ -439,6 +439,11 @@ static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, Ta
     }
     if (r) *r = t;
     return off;
+}
+
+// The tape of a model call over B rows.
+static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, TapeRegions* r = nullptr) {
+    return tape_regions_cap(m, slot_capacity(m, B), m->d.boundary_margin > 1.0f, tc, base, r);
 }
 
 // train_tc != 0: recording forward on the tensor cores (precision tc_f16) into the tensor-core tape regions.
@@ -591,10 +596,11 @@ size_t mn_model_forward_assigned_workspace_bytes(const mn_model* m, int64_t n, i
     return bytes;
 }
 
-int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, int precision,
-                              float* out_d, void* workspace_d, size_t workspace_bytes, void* stream) {
-    if (!ctx || !m || n < 0 || cols < 1) return MN_ERR_INVALID;
-    if (m->d.kind != 2) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_assigned: not a MegaNeRF model");
+// The payload rows of an owner call as the MLP kernels read them: checks the column count (the child's MN_ERR_SHAPE) and fills
+// the mode-0 RowSrc of `cols` columns inside the wider payload row - directions x[:, -4:-1], image index x[:, -1] (nerf.py:146,149).
+static int assigned_rows(mn_ctx* ctx, const mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, const char* who,
+                         RowSrc* src) {
+    if (m->d.kind != 2) return mn_fail(ctx, MN_ERR_INVALID, std::string(who) + ": not a MegaNeRF model");
     const mn_model_desc& d = m->d;
     const int expected = d.xyz_dim + 3 * (d.pos_dir_dim > 0 ? 1 : 0) + (d.appearance_dim > 0 ? 1 : 0);
     if (cols != expected) {
@@ -603,38 +609,27 @@ int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int
                  d.xyz_dim);
         return mn_fail(ctx, MN_ERR_SHAPE, buf);
     }
-    if (n == 0) return MN_OK;
-    if (!rows_d || !out_d) return MN_ERR_INVALID;
-    if (!workspace_d || workspace_bytes < mn_model_forward_assigned_workspace_bytes(m, n, precision))
-        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward_assigned: workspace too small");
-    cudaStream_t st = (cudaStream_t)stream;
     const int stride = cols + 1 + (has_noise ? 1 : 0);
-    // mode-0 rows of `cols` columns inside the wider payload row: directions x[:, -4:-1], image index x[:, -1] (nerf.py:146,149)
-    RowSrc src{};
-    src.xyz_dim = d.xyz_dim;
-    src.x = rows_d;
-    src.cols = stride;
-    src.div = 1;
-    src.dirs = rows_d + cols - 4;
-    src.dir_stride = stride;
-    src.idx = rows_d + cols - 1;
-    src.idx_stride = stride;
+    *src = RowSrc{};
+    src->xyz_dim = d.xyz_dim;
+    src->x = rows_d;
+    src->cols = stride;
+    src->div = 1;
+    src->dirs = rows_d + cols - 4;
+    src->dir_stride = stride;
+    src->idx = rows_d + cols - 1;
+    src->idx_stride = stride;
+    return MN_OK;
+}
 
-    const int64_t cap = slot_capacity(m, n, 1);
-    char* ws = (char*)workspace_d;
-    auto carve = [&](size_t b) { char* p = ws; ws += mn_align(b); return p; };
-    int* slot_row = (int*)carve((size_t)cap * sizeof(int));
-    void* scratch = carve(mn_route_assigned_scratch_bytes(n));
-    const float* noise = nullptr;
-    int rc;
-    if ((rc = mn_route_build_assigned(ctx, m, rows_d, n, stride, cols, has_noise, cap, slot_row, scratch, &noise, st))) return rc;
-
+// MlpArgs of an owner call: every bucketed slot through its own sub-module, results scattered to the rows' own indices.
+static MlpArgs assigned_args(const mn_model* m, const RowSrc& src, int64_t cap, const int* slot_row, const float* noise, float* out_d) {
     MlpArgs a{};
     a.nd = m->nd;
     a.lay = m->lay;
     a.packed = m->packed;
     a.src = src;
-    a.n_sub = d.n_sub;
+    a.n_sub = m->d.n_sub;
     a.B = cap;
     a.sigma_noise = noise;
     a.out = out_d;
@@ -642,6 +637,29 @@ int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int
     a.slot_row = slot_row;
     a.counters = m->counters_d;
     a.scatter = 1;
+    return a;
+}
+
+int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, int precision,
+                              float* out_d, void* workspace_d, size_t workspace_bytes, void* stream) {
+    if (!ctx || !m || n < 0 || cols < 1) return MN_ERR_INVALID;
+    RowSrc src;
+    int rc;
+    if ((rc = assigned_rows(ctx, m, rows_d, n, cols, has_noise, "mn_model_forward_assigned", &src))) return rc;
+    if (n == 0) return MN_OK;
+    if (!rows_d || !out_d) return MN_ERR_INVALID;
+    if (!workspace_d || workspace_bytes < mn_model_forward_assigned_workspace_bytes(m, n, precision))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward_assigned: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int64_t cap = slot_capacity(m, n, 1);
+    char* ws = (char*)workspace_d;
+    auto carve = [&](size_t b) { char* p = ws; ws += mn_align(b); return p; };
+    int* slot_row = (int*)carve((size_t)cap * sizeof(int));
+    void* scratch = carve(mn_route_assigned_scratch_bytes(n));
+    const float* noise = nullptr;
+    if ((rc = mn_route_build_assigned(ctx, m, rows_d, n, src.cols, cols, has_noise, cap, slot_row, scratch, &noise, st))) return rc;
+
+    const MlpArgs a = assigned_args(m, src, cap, slot_row, noise, out_d);
     const int64_t n_tiles = cap / MN_TILE;
     if (precision == MN_PREC_FP32) return mn_mlp_simt_launch(ctx, a, n_tiles, st);
     return mn_mlp_tc_launch(ctx, m, a, n_tiles, precision, ws, workspace_bytes - (size_t)(ws - (char*)workspace_d), st);
@@ -837,6 +855,93 @@ int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, co
     BwdArgs a = bwd_args(m, B, use_coarse, grad_out_d, param_grads_d, T);
     a.grad_rows = B;
     return mn_train_tc_backward(ctx, m, a, slot_capacity(m, B) / MN_TILE, T.tc, workspace_d, workspace_bytes, (cudaStream_t)stream);
+}
+
+// ---- training on the owner side of an expert-parallel query ------------------------------------------------------------
+// The tape of a recording owner call holds max_pairs pairs, bucketed like mn_model_forward_assigned: slot_capacity(m, max_pairs, 1)
+// slots and no slot_w (the blend weights are applied at home).  The rows stay where they arrived; slot_row points into them.
+static int assigned_train_prec(mn_ctx* ctx, const mn_model* m, int precision, const char* who) {
+    if (precision == MN_PREC_FP32) return MN_OK;
+    if (precision != MN_PREC_TC_F16) return mn_fail(ctx, MN_ERR_INVALID, std::string(who) + ": training precision is fp32 or tc_f16");
+    if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
+    return MN_OK;
+}
+
+size_t mn_model_assigned_tape_bytes(const mn_model* m, int64_t max_pairs, int precision) {
+    if (!m || max_pairs < 0) return 0;
+    return tape_regions_cap(m, slot_capacity(m, max_pairs, 1), false, precision != MN_PREC_FP32, nullptr, nullptr);
+}
+
+size_t mn_model_forward_assigned_train_workspace_bytes(const mn_model* m, int64_t n) {
+    if (!m || n < 0) return 0;
+    return 256 + mn_align(mn_route_assigned_scratch_bytes(n));
+}
+
+int mn_model_forward_assigned_train(mn_ctx* ctx, mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, int64_t max_pairs,
+                                    int precision, float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes,
+                                    void* stream) {
+    if (!ctx || !m || n < 0 || cols < 1 || max_pairs < 0) return MN_ERR_INVALID;
+    const char* who = "mn_model_forward_assigned_train";
+    RowSrc src;
+    int rc;
+    if ((rc = assigned_rows(ctx, m, rows_d, n, cols, has_noise, who, &src))) return rc;
+    if ((rc = assigned_train_prec(ctx, m, precision, who))) return rc;
+    if (n == 0) return MN_OK;
+    if (!rows_d || !out_d || !tape_d) return mn_fail(ctx, MN_ERR_INVALID, std::string(who) + ": missing buffer");
+    const bool tc = precision == MN_PREC_TC_F16;
+    const int64_t cap = slot_capacity(m, max_pairs, 1);
+    TapeRegions T;
+    if (tape_bytes < tape_regions_cap(m, cap, false, tc, tape_d, &T)) return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": tape too small");
+    if (!workspace_d || workspace_bytes < mn_model_forward_assigned_train_workspace_bytes(m, n))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    // rows whose pair finds no slot (more pairs than max_pairs: the scatter pass drops them and sets MN_STATUS_OVERFLOW) keep this
+    // NaN, as do the empty rows (id -1); every other row is written by the MLP
+    MN_CUDA(ctx, cudaMemsetAsync(out_d, 0xFF, (size_t)n * (m->nd.rgb_dim + 1) * sizeof(float), st));
+    const float* noise = nullptr;
+    if ((rc = mn_route_build_assigned(ctx, m, rows_d, n, src.cols, cols, has_noise, cap, T.slot_row, (char*)workspace_d + 256, &noise, st)))
+        return rc;
+    MN_CUDA(ctx, cudaMemcpyAsync(T.counters, m->counters_d, CNT_TOTAL * sizeof(int), cudaMemcpyDeviceToDevice, st));
+    MlpArgs a = assigned_args(m, src, cap, T.slot_row, noise, out_d);
+    const int64_t n_tiles = cap / MN_TILE;
+    if (tc) return mn_mlp_tc_launch_train(ctx, m, a, n_tiles, T.tc, st);
+    a.tape = T.act;
+    a.tl = m->tape;
+    return mn_mlp_simt_launch(ctx, a, n_tiles, st);
+}
+
+size_t mn_model_backward_assigned_workspace_bytes(const mn_model* m, int64_t max_pairs, int precision) {
+    if (!m || max_pairs < 0) return 0;
+    const int64_t cap = slot_capacity(m, max_pairs, 1);
+    if (precision != MN_PREC_FP32) return 256 + mn_train_tc_backward_workspace(m, cap / MN_TILE);
+    const int TM = mn_tape_tm(m->nd.L);
+    return 256 + mn_align((size_t)(cap / TM) * m->tape.g_total * TM * sizeof(float));
+}
+
+int mn_model_backward_assigned(mn_ctx* ctx, mn_model* m, int64_t n, int64_t max_pairs, int precision, const float* grad_out_d,
+                               const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes,
+                               void* stream) {
+    if (!ctx || !m || n < 0 || max_pairs < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;
+    const char* who = "mn_model_backward_assigned";
+    if (m->d.kind != 2) return mn_fail(ctx, MN_ERR_INVALID, std::string(who) + ": not a MegaNeRF model");
+    int rc;
+    if ((rc = assigned_train_prec(ctx, m, precision, who))) return rc;
+    if (n == 0) return MN_OK;
+    const bool tc = precision == MN_PREC_TC_F16;
+    const int64_t cap = slot_capacity(m, max_pairs, 1);
+    TapeRegions T;
+    if (tape_bytes < tape_regions_cap(m, cap, false, tc, const_cast<void*>(tape_d), &T))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": tape too small");
+    if (!workspace_d || workspace_bytes < mn_model_backward_assigned_workspace_bytes(m, max_pairs, precision))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": workspace too small");
+    BwdArgs a = bwd_args(m, n, 0, grad_out_d, param_grads_d, T);
+    a.B = cap;
+    a.grad_rows = n;
+    if (tc) return mn_train_tc_backward(ctx, m, a, cap / MN_TILE, T.tc, workspace_d, workspace_bytes, (cudaStream_t)stream);
+    a.tl = m->tape;
+    a.act = T.act;
+    a.grad = (float*)workspace_d;
+    return mn_mlp_bwd_launch(ctx, a, cap / MN_TILE, (cudaStream_t)stream);
 }
 
 int mn_model_last_stats(mn_ctx* ctx, mn_model* m, int64_t* slots, int64_t* tiles, void* stream) {

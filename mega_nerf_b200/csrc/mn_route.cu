@@ -403,6 +403,23 @@ __global__ void ep_combine_kernel(int64_t B, int K, const int* __restrict__ row_
     out[i] = acc;
 }
 
+// Backward of ep_combine_kernel: the gradient of every slot's result is its home row's gradient times the slot's blend weight
+// (the gradient of `back[m] * w[m]`, one fp32 multiply), the row's gradient itself under hard routing, 0 past the pairs.
+__global__ void ep_combine_backward_kernel(int64_t n_slots, const int* __restrict__ pair_row, const float* __restrict__ pair_w,
+                                           const float* __restrict__ dout, int out_cols, float* __restrict__ dback) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_slots * out_cols) return;
+    const int64_t slot = i / out_cols;
+    const int c = (int)(i % out_cols);
+    const int row = pair_row[slot];
+    float g = 0.0f;
+    if (row >= 0) {
+        g = dout[(int64_t)row * out_cols + c];
+        if (pair_w) g = __fmul_rn(g, pair_w[slot]);
+    }
+    dback[i] = g;
+}
+
 // Bucket counts of an owner call: the sub-module of each received row is given (payload column `id_col`, -1 = empty slot);
 // the density noise column, if any, is copied to a contiguous [n] for the MLP kernels.
 template <int KMAX>
@@ -647,6 +664,22 @@ int mn_model_ep_combine(mn_ctx* ctx, mn_model* m, int64_t B, const int32_t* row_
     const int64_t n = B * out_cols;
     ep_combine_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(B, m->d.n_sub, row_slots_d, blend ? pair_w_d : nullptr,
                                                                                  back_d, out_cols, out_d);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+int mn_model_ep_combine_backward(mn_ctx* ctx, mn_model* m, int64_t n_slots, const int32_t* pair_row_d, const float* pair_w_d,
+                                 const float* dout_d, float* dback_d, void* stream) {
+    if (!ctx || !m || n_slots < 0) return MN_ERR_INVALID;
+    if (m->d.kind != 2) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_ep_combine_backward: not a MegaNeRF model");
+    const bool blend = m->d.boundary_margin > 1.0f;
+    if (n_slots == 0) return MN_OK;
+    if (!pair_row_d || !dout_d || !dback_d || (blend && !pair_w_d))
+        return mn_fail(ctx, MN_ERR_INVALID, "mn_model_ep_combine_backward: missing buffer");
+    const int out_cols = m->nd.rgb_dim + 1;
+    const int64_t n = n_slots * out_cols;
+    ep_combine_backward_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(n_slots, pair_row_d, blend ? pair_w_d : nullptr,
+                                                                                          dout_d, out_cols, dback_d);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }

@@ -10,8 +10,17 @@ all-gather alone cannot express this partitioning (SURVEY.md §8e).
 
 Payload per routed pair: the child's input row (xyz, dir, image index: 28 B) + sub-module id (+ density noise) out,
 16 B back.  The exchange is `torch.distributed.all_to_all_single` (NCCL over NVLink on GPUs, gloo in the CPU tests of
-this host logic).  Inference only; every rank must issue the same sequence of queries (true for `render_rays` on the
-foreground network with the same sampling configuration on every rank).
+this host logic).  Every rank must issue the same sequence of queries (true for `render_rays` on the foreground network
+with the same sampling configuration on every rank).
+
+Training (CUDA tensors, device path): when autograd records, the owner call records a tape (mn_model_forward_assigned_train,
+sized by the pairs that arrived: the query reads that count back once) and the result exchange is differentiable, so
+`loss.backward()` runs mn_model_ep_combine_backward at home, the reverse all-to-all of the result gradients and
+mn_model_backward_assigned at the owner.  Owned parameters receive the MEAN over ranks of what each rank's loss gives them
+(divided by world in `_owner_backward`, nowhere else) - what DDP over a replicated MegaNeRF leaves in `.grad`; sub-modules
+owned elsewhere get no `.grad` at all.  Conditions: every rank calls backward on the same sequence of queries (the coarse
+and the fine query both feed the reference's loss), every rank queries the same row count, and the foreground network is
+NOT wrapped in DistributedDataParallel (the owners already hold the reduced gradient).  The torch path is inference-only.
 
 CUDA tensors take the device path: `mn_model_route`, then `mn_model_ep_dispatch` writes the pairs straight into `world`
 segments of a fixed capacity (B x max_multiplicity rows, the router's own slot bound), one all-to-all with equal splits
@@ -129,13 +138,18 @@ class ExpertParallel:
 
     # ---- nn.Module.__call__ of MegaNeRF on rows, distributed
     def forward(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.mega.parameters()):
-            raise RuntimeError('expert-parallel execution is inference-only (wrap the call in torch.no_grad())')
         if x.is_cuda and not self._torch_path:
             return self._forward_device(x, sigma_noise)
+        if self._recording():
+            raise RuntimeError('expert-parallel execution is inference-only (wrap the call in torch.no_grad())')
         return self._forward_torch(x, sigma_noise)
 
-    # ---- device path: the three steps, each callable on its own (a test can play several ranks on one device)
+    def _recording(self) -> bool:
+        return torch.is_grad_enabled() and any(p.requires_grad for p in self.mega.parameters())
+
+    # ---- device path: the three steps, each callable on its own (a test can play several ranks on one device).  When
+    # autograd records (a parameter requires grad), `compute` and `combine` return differentiable results: the backward of
+    # `combine` is mn_model_ep_combine_backward, that of `compute` mn_model_backward_assigned over the owner's tape.
     def dispatch(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor], world: int) -> 'Dispatch':
         """Route x [B, cols] and write its pairs into `world` segments (mn_model_ep_dispatch)."""
         dev = x.device
@@ -159,9 +173,22 @@ class ExpertParallel:
                                        K.ptr(ws), ws.numel(), K.stream_of(dev)), h)
         return d
 
-    def compute(self, recv: torch.Tensor, c_in: int, has_noise: bool) -> torch.Tensor:
+    def compute(self, recv: torch.Tensor, c_in: int, has_noise: bool, max_pairs: Optional[int] = None, rank: Optional[int] = None,
+                world: Optional[int] = None) -> torch.Tensor:
         """The owner's share: every received row through its own sub-module (mn_model_forward_assigned) -> [n, rgb_dim + 1];
-        rows with sub-module id -1 are left unwritten."""
+        rows with sub-module id -1 are left unwritten.
+
+        Recording (autograd on, a parameter requires grad): mn_model_forward_assigned_train, whose tape holds `max_pairs` pairs
+        (default: the rows with an id, read back once); rows with id -1 are NaN, and more pairs than max_pairs raise here
+        (a status check, which synchronises the host).  Its backward gives the parameters of the sub-modules owned by `rank`
+        out of `world` (default: this rank of the group) their gradient divided by `world`; the others get none."""
+        if self._recording():
+            if rank is None or world is None:
+                rank, world = dist.get_rank(self.group), dist.get_world_size(self.group)
+            if max_pairs is None:
+                max_pairs = int((recv[:, c_in] >= 0).sum())
+            plist = self.native(recv.device).param_list()
+            return _OwnerFn.apply(self, recv, c_in, has_noise, int(max_pairs), rank, world, *[p for _, _, p in plist])
         dev = recv.device
         nat = self.native(dev)
         L, h = K.lib(), nat.sync(dev)
@@ -176,6 +203,8 @@ class ExpertParallel:
 
     def combine(self, d: 'Dispatch', back: torch.Tensor) -> torch.Tensor:
         """Blend the returned results of a dispatch's pairs at home (mn_model_ep_combine) -> [B, rgb_dim + 1]."""
+        if back.requires_grad and torch.is_grad_enabled():
+            return _CombineFn.apply(self, d, back)
         dev = back.device
         nat = self.native(dev)
         B = d.row_slots.shape[0] // (self.n_sub if d.pair_w is not None else 1)
@@ -185,17 +214,95 @@ class ExpertParallel:
                                             K.stream_of(dev)), h)
         return out
 
+    def combine_backward(self, d: 'Dispatch', dout: torch.Tensor) -> torch.Tensor:
+        """Gradient of `combine`'s output [B, rgb_dim + 1] -> gradient of the returned results [world * cap, rgb_dim + 1]
+        (mn_model_ep_combine_backward): w x dout[home row] per slot, 0 past the pairs."""
+        dev = dout.device
+        nat = self.native(dev)
+        n_slots = d.pair_row.shape[0]
+        dback = torch.empty(n_slots, dout.shape[1], device=dev, dtype=torch.float32)
+        h = K.ctx(dev)
+        K.check(K.lib().mn_model_ep_combine_backward(h, nat.handle, n_slots, K.ptr(d.pair_row), K.ptr(d.pair_w), K.ptr(K.f32c(dout)),
+                                                     K.ptr(dback), K.stream_of(dev)), h)
+        return dback
+
     def _forward_device(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor]) -> torch.Tensor:
         world = dist.get_world_size(self.group)
         d = self.dispatch(x, sigma_noise, world)
         recv, recv_counts = torch.empty_like(d.send), torch.empty_like(d.counts)
         dist.all_to_all_single(recv, d.send, group=self.group)
         dist.all_to_all_single(recv_counts, d.counts, group=self.group)
+        self._last = (_LazySum(d.counts), _LazySum(recv_counts))
+        if self._recording():
+            # training: the owner's tape is sized by the pairs that arrived (one host read), and the result exchange is
+            # differentiable - its backward carries the result gradients from home back to the owners
+            res = self.compute(recv, d.c_in, d.has_noise, int(recv_counts.sum()))
+            return self.combine(d, _AllToAll.apply(res, self.group))
         res = self.compute(recv, d.c_in, d.has_noise)
         back = torch.empty_like(res)
         dist.all_to_all_single(back, res, group=self.group)
-        self._last = (_LazySum(d.counts), _LazySum(recv_counts))
         return self.combine(d, back)
+
+    def _record(self, recv: torch.Tensor, c_in: int, has_noise: bool, max_pairs: int) -> Tuple[torch.Tensor, 'OwnerTape']:
+        """The recording owner call (mn_model_forward_assigned_train) in the training arithmetic of `set_train_precision`."""
+        dev = recv.device
+        nat = self.native(dev)
+        L, h, st = K.lib(), nat.sync(dev), K.stream_of(dev)
+        n = recv.shape[0]
+        prec = K.PREC_TC_F16 if nat.train_on_tensor_cores() else K.PREC_FP32
+        res = torch.empty(n, self.mega.sub_modules[0].rgb_dim + 1, device=dev, dtype=torch.float32)
+        tape = torch.empty(max(int(L.mn_model_assigned_tape_bytes(nat.handle, max_pairs, prec)), 256), device=dev, dtype=torch.uint8)
+        ws = torch.empty(max(int(L.mn_model_forward_assigned_train_workspace_bytes(nat.handle, n)), 256), device=dev, dtype=torch.uint8)
+        K.check(L.mn_model_forward_assigned_train(h, nat.handle, K.ptr(recv), n, c_in, int(has_noise), max_pairs, prec, K.ptr(res),
+                                                  K.ptr(tape), tape.numel(), K.ptr(ws), ws.numel(), st), h)
+        K.check(L.mn_check_status(h, st), h)           # more pairs than max_pairs: raise before anything reads the tape
+        return res, OwnerTape(tape=tape, n=n, max_pairs=max_pairs, precision=prec)
+
+    def _owner_backward(self, t: 'OwnerTape', grad_res: torch.Tensor, rank: int, world: int) -> List[Optional[torch.Tensor]]:
+        """Parameter gradients of a recording owner call (mn_model_backward_assigned), in param_list() order: the sub-modules
+        owned by `rank` get the gradient divided by `world` - the one place the mean over ranks is taken, so that an owned
+        parameter holds what DDP over a replicated MegaNeRF would leave in it - the others None."""
+        dev = grad_res.device
+        nat = self.native(dev)
+        L, h = K.lib(), K.ctx(dev)
+        gbuf = torch.zeros(int(L.mn_model_grad_floats(nat.handle)), device=dev, dtype=torch.float32)
+        ws = torch.empty(max(int(L.mn_model_backward_assigned_workspace_bytes(nat.handle, t.max_pairs, t.precision)), 256), device=dev,
+                         dtype=torch.uint8)
+        g = K.f32c(grad_res)
+        K.check(L.mn_model_backward_assigned(h, nat.handle, t.n, t.max_pairs, t.precision, K.ptr(g), K.ptr(t.tape), t.tape.numel(),
+                                             K.ptr(gbuf), K.ptr(ws), ws.numel(), K.stream_of(dev)), h)
+        gbuf.div_(world)
+        off = nat._offsets()
+        stride = off['stride']
+        grads = []
+        for k, key, p in nat.param_list():
+            if owner_of(k, world) != rank:
+                grads.append(None)
+                continue
+            a = k * stride + off[key]
+            grads.append(gbuf[a:a + p.numel()].view(p.shape))
+        return grads
+
+    # ---- checkpoints
+    def full_state_dict(self) -> dict:
+        """The whole MegaNeRF's state dict under the reference's key names (`sub_modules.<k>.<name>`, `centroids`), every
+        sub-module's tensors broadcast from their owner (rank k mod world), so that rank 0 can save it as `model_state_dict`
+        and the reference loads it unchanged.  A collective: every rank calls it and gets the same tensors, each on the
+        device of its own copy of that entry."""
+        world = dist.get_world_size(self.group)
+        comm = torch.device('cuda', torch.cuda.current_device()) if dist.get_backend(self.group) == 'nccl' else torch.device('cpu')
+        out = {}
+        for key, t in self.mega.state_dict().items():
+            parts = key.split('.')
+            if parts[0] != 'sub_modules':
+                out[key] = t
+                continue
+            owner = owner_of(int(parts[1]), world)
+            src = owner if self.group is None else dist.get_global_rank(self.group, owner)
+            buf = t.detach().to(comm, copy=True).contiguous()
+            dist.broadcast(buf, src=src, group=self.group)
+            out[key] = buf.to(t.device)
+        return out
 
     # ---- torch path
     def _forward_torch(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -245,6 +352,62 @@ class ExpertParallel:
                 if bool(m.any()):
                     out[rows[m]] += back[m] * w[m].unsqueeze(-1)
         return out
+
+
+@dataclass
+class OwnerTape:
+    """What the backward of a recording owner call needs (mn_model_backward_assigned)."""
+    tape: torch.Tensor
+    n: int                  # received rows
+    max_pairs: int          # pairs the tape holds
+    precision: int          # K.PREC_FP32 or K.PREC_TC_F16
+
+
+class _OwnerFn(torch.autograd.Function):
+    """`ExpertParallel.compute` under autograd: the parameters are inputs so that their gradients land like _ModelFn's."""
+
+    @staticmethod
+    def forward(ctx, ep, recv, c_in, has_noise, max_pairs, rank, world, *params):
+        res, tape = ep._record(recv, c_in, has_noise, max_pairs)
+        ctx.ep, ctx.tape, ctx.rank, ctx.world = ep, tape, rank, world
+        return res
+
+    @staticmethod
+    def backward(ctx, grad_res):
+        grads = ctx.ep._owner_backward(ctx.tape, grad_res, ctx.rank, ctx.world)
+        ctx.tape = None
+        need = ctx.needs_input_grad[7:]
+        return (None,) * 7 + tuple(g if n else None for g, n in zip(grads, need))
+
+
+class _CombineFn(torch.autograd.Function):
+    """`ExpertParallel.combine` under autograd; no gradient reaches the blend weights (the routing is not differentiated)."""
+
+    @staticmethod
+    def forward(ctx, ep, d, back):
+        ctx.ep, ctx.d = ep, d
+        return ep.combine(d, back)          # autograd is off inside forward: the plain combine
+
+    @staticmethod
+    def backward(ctx, dout):
+        return None, None, ctx.ep.combine_backward(ctx.d, dout)
+
+
+class _AllToAll(torch.autograd.Function):
+    """Equal-split all_to_all_single; its backward is the same exchange of the gradients, in the other direction."""
+
+    @staticmethod
+    def forward(ctx, x, group):
+        ctx.group = group
+        out = torch.empty_like(x)
+        dist.all_to_all_single(out, x.contiguous(), group=group)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        out = torch.empty_like(g)
+        dist.all_to_all_single(out, g.contiguous(), group=ctx.group)
+        return out, None
 
 
 class _LazySum:
