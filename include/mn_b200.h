@@ -238,23 +238,30 @@ int mn_model_density_grid(mn_ctx* ctx, mn_model* m, int use_coarse, const float 
  *   home:  mn_model_route -> mn_model_ep_dispatch -> [send segments, counts]
  *   owner: mn_model_forward_assigned on the received segments -> [results]
  *   home:  mn_model_ep_combine on the returned segments.
- * Every rank must query the same row count B: the segments are sized from it.
+ * Every rank must pass the same capacity row count B_cap >= B: the segments are sized from it.  B_cap == B on every rank is
+ * the plain case; a query whose row count differs from rank to rank (the rays that reach a background network) passes the
+ * maximum over the ranks.
  *
- * Rows of one segment: B x max_multiplicity (mn_model_set_max_multiplicity; 1 under hard routing), the router's own slot
+ * Rows of one segment: B_cap x max_multiplicity (mn_model_set_max_multiplicity; 1 under hard routing), the router's own slot
  * bound, so the pairs of one query fit any one segment.  A row within the margin of more sub-modules than max_multiplicity
  * can push a segment past it; its result is then NaN and MN_ERR_WORKSPACE follows at the next mn_check_status. */
 int64_t mn_model_ep_segment_rows(const mn_model* m, int64_t B);
 /* Dispatch (mega_nerf.py:19-61, the `cluster_mask` selection of every sub-module): the (row, sub-module) pairs of
  * x_d [B, cols] (the model's rows; the first 3 columns are routing-only with xyz_real) from the router's output - assign_d
  * int32 [B] (boundary_margin == 1) or weights_d [B, n_sub] (> 1, pairs where the weight is > 0) - ordered by destination
- * rank (k mod world), sub-module, row.  Pair p for destination d occupies row d * S + p (S = mn_model_ep_segment_rows) of:
+ * rank (k mod world), sub-module, row.  Pair p for destination d occupies row d * S + p (S = mn_model_ep_segment_rows(m, B_cap))
+ * of:
  *   send_d [world * S, c + 1 (+1)]: the child's input (cols - 3 with xyz_real, else cols columns), the sub-module id as a
  *     float and, if sigma_noise_d [B] is given, the row's density noise; rows past a segment's pairs carry id -1;
  *   pair_row_d int32 [world * S] (home row, -1 past the pairs) and pair_w_d [world * S] (blend weight; margin > 1 only).
  * counts_d int32 [world, n_sub]: pairs per (destination, sub-module).  row_slots_d int32: [B] the slot of each row's pair
- * (hard routing) or [B, n_sub] the slot per sub-module, -1 where none (margin > 1) - what mn_model_ep_combine reads. */
+ * (hard routing) or [B, n_sub] the slot per sub-module, -1 where none (margin > 1) - what mn_model_ep_combine reads.
+ * B is this rank's own row count: the rows routed, counted and scattered (routing still follows B, cdist's direct path for
+ * B <= 25 included).  B == 0 with B_cap > 0 still writes the segments: id -1 in every payload row, pair_row -1, pair_w 0 and
+ * counts 0; x_d, assign_d / weights_d and row_slots_d may then be NULL, but sigma_noise_d must be non-NULL iff the payload
+ * rows carry the noise column (it sets the row width; nothing is read from it). */
 size_t mn_model_ep_dispatch_workspace_bytes(const mn_model* m, int64_t B, int world);
-int mn_model_ep_dispatch(mn_ctx* ctx, mn_model* m, const float* x_d, int64_t B, int cols, const int32_t* assign_d,
+int mn_model_ep_dispatch(mn_ctx* ctx, mn_model* m, const float* x_d, int64_t B, int64_t B_cap, int cols, const int32_t* assign_d,
                          const float* weights_d, const float* sigma_noise_d, int world, float* send_d, int32_t* counts_d,
                          int32_t* pair_row_d, float* pair_w_d, int32_t* row_slots_d, void* workspace_d, size_t workspace_bytes,
                          void* stream);

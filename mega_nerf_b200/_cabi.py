@@ -87,7 +87,7 @@ SIGNATURES = {
     'mn_model_last_stats': (_I, [_P, _P, C.POINTER(_L), C.POINTER(_L), _P]),
     'mn_model_ep_segment_rows': (_L, [_P, _L]),
     'mn_model_ep_dispatch_workspace_bytes': (_Z, [_P, _L, _I]),
-    'mn_model_ep_dispatch': (_I, [_P, _P, _P, _L, _I, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
+    'mn_model_ep_dispatch': (_I, [_P, _P, _P, _L, _L, _I, _P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _Z, _P]),
     'mn_model_forward_assigned_workspace_bytes': (_Z, [_P, _L, _I]),
     'mn_model_forward_assigned': (_I, [_P, _P, _P, _L, _I, _I, _I, _P, _P, _Z, _P]),
     'mn_model_ep_combine': (_I, [_P, _P, _L, _P, _P, _P, _P, _P]),

@@ -73,6 +73,8 @@ class _CompositeFn(torch.autograd.Function):
             g_rgb = torch.zeros(N, 3, device=z.device, dtype=torch.float32)
         g_rgb = K.f32c(g_rgb)
         g_lam = K.f32c(g_lam) if g_lam is not None else None
+        if N == 0:          # a pass over no rays (render.py: background expert parallelism): nothing to launch
+            return None, g_raw, None, None, g_raw2, None, None, None, None, None, None, None
         K.check(sg.L.mn_composite_backward(sg.h, K.ptr(raw), K.ptr(z), S, K.ptr(raw2), K.ptr(z2), S2, K.ptr(last_delta), N,
                                            int(ctx.flip), K.ptr(g_rgb), K.ptr(g_lam), K.ptr(g_raw), K.ptr(g_raw2), sg.st), sg.h)
         return None, g_raw, None, None, g_raw2, None, None, None, None, None, None, None
@@ -101,6 +103,8 @@ class _ShFn(torch.autograd.Function):
         B = coef.shape[0]
         g = K.f32c(g_out)
         g_coef = torch.zeros_like(coef)
+        if B == 0:
+            return None, None, g_coef, None, None
         K.check(sg.L.mn_sh_to_rgb_backward(sg.h, ctx.deg, K.ptr(coef), coef.shape[1], K.ptr(dirs), dirs.stride(0), ctx.S, B, 1,
                                            K.ptr(g), K.ptr(g_coef), sg.st), sg.h)
         return None, None, g_coef, None, None

@@ -380,6 +380,17 @@ __global__ void __launch_bounds__(EP_ROWS) ep_scatter_kernel(const float* __rest
     }
 }
 
+// The segments of a dispatch of no rows (B == 0, B_cap > 0): every slot lies past the pairs, filled as the tail of
+// ep_scatter_kernel, so that the owners skip what this rank sends.
+__global__ void ep_empty_kernel(int64_t n_slots, int width, int id_col, float* __restrict__ send, int* __restrict__ pair_row,
+                                float* __restrict__ pair_w) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_slots) return;
+    send[t * width + id_col] = -1.0f;
+    pair_row[t] = -1;
+    if (pair_w) pair_w[t] = 0.0f;
+}
+
 // out[row] = sum over the row's pairs in ascending sub-module order of back x w, from 0, multiply and add rounded separately
 // (`out[rows[m]] += back[m] * w[m]`, mega_nerf.py:46-49); hard routing copies the row's one result.
 __global__ void ep_combine_kernel(int64_t B, int K, const int* __restrict__ row_slots, const float* __restrict__ pair_w,
@@ -620,16 +631,18 @@ size_t mn_model_ep_dispatch_workspace_bytes(const mn_model* m, int64_t B, int wo
     return ep_scan_bytes(B, m->d.n_sub, world, nullptr, nullptr);
 }
 
-int mn_model_ep_dispatch(mn_ctx* ctx, mn_model* m, const float* x_d, int64_t B, int cols, const int32_t* assign_d,
+int mn_model_ep_dispatch(mn_ctx* ctx, mn_model* m, const float* x_d, int64_t B, int64_t B_cap, int cols, const int32_t* assign_d,
                          const float* weights_d, const float* sigma_noise_d, int world, float* send_d, int32_t* counts_d,
                          int32_t* pair_row_d, float* pair_w_d, int32_t* row_slots_d, void* workspace_d, size_t workspace_bytes,
                          void* stream) {
-    if (!ctx || !m || B < 0 || world < 1) return MN_ERR_INVALID;
+    if (!ctx || !m || B < 0 || B_cap < B || world < 1) return MN_ERR_INVALID;
     if (m->d.kind != 2) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_ep_dispatch: not a MegaNeRF model");
     const bool blend = m->d.boundary_margin > 1.0f;
     const int xoff = m->d.xyz_real ? 3 : 0;
     if (cols <= xoff) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_ep_dispatch: rows have no child columns");
-    if (!counts_d || (B > 0 && (!x_d || !send_d || !pair_row_d || !row_slots_d || (blend ? (!weights_d || !pair_w_d) : !assign_d))))
+    const int64_t cap = mn_model_ep_segment_rows(m, B_cap);
+    if (!counts_d || (cap > 0 && (!send_d || !pair_row_d || (blend && !pair_w_d))) ||
+        (B > 0 && (!x_d || !row_slots_d || (blend ? !weights_d : !assign_d))))
         return mn_fail(ctx, MN_ERR_INVALID, "mn_model_ep_dispatch: missing buffer (weights / pair_w with boundary_margin > 1, else assign)");
     const int K = m->d.n_sub;
     cudaStream_t st = (cudaStream_t)stream;
@@ -638,9 +651,14 @@ int mn_model_ep_dispatch(mn_ctx* ctx, mn_model* m, const float* x_d, int64_t B, 
         return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_ep_dispatch: workspace too small");
     if (B == 0) {
         MN_CUDA(ctx, cudaMemsetAsync(counts_d, 0, (size_t)world * K * sizeof(int), st));
+        if (cap == 0) return MN_OK;
+        const int64_t n_slots = (int64_t)world * cap;
+        const int c_in = cols - xoff;
+        ep_empty_kernel<<<(unsigned)mn_cdiv(n_slots, 256), 256, 0, st>>>(n_slots, c_in + 1 + (sigma_noise_d ? 1 : 0), c_in, send_d,
+                                                                        pair_row_d, blend ? pair_w_d : nullptr);
+        MN_LAUNCH_CHECK(ctx);
         return MN_OK;
     }
-    const int64_t cap = mn_model_ep_segment_rows(m, B);
     const float* w = blend ? weights_d : nullptr;
     const int* a = blend ? nullptr : assign_d;
     MN_CUDA(ctx, cudaMemsetAsync(s.ticket, 0, sizeof(int), st));

@@ -22,6 +22,10 @@ owned elsewhere get no `.grad` at all.  Conditions: every rank calls backward on
 and the fine query both feed the reference's loss), every rank queries the same row count, and the foreground network is
 NOT wrapped in DistributedDataParallel (the owners already hold the reduced gradient).  The torch path is inference-only.
 
+A query whose row count differs from rank to rank - `render_rays` queries a background network for the rays that reach the
+background only - passes `rows_cap`, the largest count over the ranks (`max_over_ranks`), so that every rank sizes its
+segments alike; a rank with no rows still takes part, sending empty segments.
+
 CUDA tensors take the device path: `mn_model_route`, then `mn_model_ep_dispatch` writes the pairs straight into `world`
 segments of a fixed capacity (B x max_multiplicity rows, the router's own slot bound), one all-to-all with equal splits
 moves the segments and one the per-(rank, sub-module) counts, `mn_model_forward_assigned` runs every owned sub-module over
@@ -137,9 +141,11 @@ class ExpertParallel:
         return [k for k in range(self.n_sub) if owner_of(k, world) == rank]
 
     # ---- nn.Module.__call__ of MegaNeRF on rows, distributed
-    def forward(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def forward(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor] = None, rows_cap: Optional[int] = None) -> torch.Tensor:
+        """rows_cap: the capacity row count of the device path's segments, the same on every rank and >= x.shape[0] (default:
+        x.shape[0], which every rank must then share).  The torch path exchanges its split sizes and ignores it."""
         if x.is_cuda and not self._torch_path:
-            return self._forward_device(x, sigma_noise)
+            return self._forward_device(x, sigma_noise, rows_cap)
         if self._recording():
             raise RuntimeError('expert-parallel execution is inference-only (wrap the call in torch.no_grad())')
         return self._forward_torch(x, sigma_noise)
@@ -147,20 +153,33 @@ class ExpertParallel:
     def _recording(self) -> bool:
         return torch.is_grad_enabled() and any(p.requires_grad for p in self.mega.parameters())
 
+    def max_over_ranks(self, n: int, device: torch.device) -> int:
+        """The largest of every rank's `n` over the group (one all-reduce, read back): the capacity that lets ranks with
+        different row counts run the same query."""
+        t = torch.tensor([n], device=device, dtype=torch.int64)
+        dist.all_reduce(t, op=dist.ReduceOp.MAX, group=self.group)
+        return int(t.item())
+
     # ---- device path: the three steps, each callable on its own (a test can play several ranks on one device).  When
     # autograd records (a parameter requires grad), `compute` and `combine` return differentiable results: the backward of
     # `combine` is mn_model_ep_combine_backward, that of `compute` mn_model_backward_assigned over the owner's tape.
-    def dispatch(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor], world: int) -> 'Dispatch':
-        """Route x [B, cols] and write its pairs into `world` segments (mn_model_ep_dispatch)."""
+    def dispatch(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor], world: int, rows_cap: Optional[int] = None) -> 'Dispatch':
+        """Route x [B, cols] and write its pairs into `world` segments (mn_model_ep_dispatch) sized for `rows_cap` rows
+        (default B; the same on every rank).  With B == 0 every slot is empty (id -1)."""
         dev = x.device
         x = K.f32c(x)
         assign, weights = self._route_device(x)
         nat = self.native(dev)
         L, h = K.lib(), K.ctx(dev)
         B, cols = x.shape
+        B_cap = B if rows_cap is None else int(rows_cap)
+        if B_cap < B:
+            raise ValueError(f'rows_cap {B_cap} is below the row count {B}')
         c_in = cols - (3 if self.mega.xyz_real else 0)
         noise = K.f32c(sigma_noise).view(-1) if sigma_noise is not None else None
-        cap = int(L.mn_model_ep_segment_rows(nat.handle, B))
+        if noise is not None and B == 0:
+            noise = torch.empty(1, device=dev)        # the pointer sets the payload width; with no rows nothing is read
+        cap = int(L.mn_model_ep_segment_rows(nat.handle, B_cap))
         i32 = dict(device=dev, dtype=torch.int32)
         d = Dispatch(world=world, cap=cap, c_in=c_in, has_noise=noise is not None, assign=assign, weights=weights,
                      send=torch.empty(world * cap, c_in + 1 + (noise is not None), device=dev, dtype=torch.float32),
@@ -168,7 +187,7 @@ class ExpertParallel:
                      pair_w=torch.empty(world * cap, device=dev, dtype=torch.float32) if weights is not None else None,
                      row_slots=torch.empty(B * (self.n_sub if weights is not None else 1), **i32))
         ws = torch.empty(max(int(L.mn_model_ep_dispatch_workspace_bytes(nat.handle, B, world)), 256), device=dev, dtype=torch.uint8)
-        K.check(L.mn_model_ep_dispatch(h, nat.handle, K.ptr(x), B, cols, K.ptr(assign), K.ptr(weights), K.ptr(noise), world,
+        K.check(L.mn_model_ep_dispatch(h, nat.handle, K.ptr(x), B, B_cap, cols, K.ptr(assign), K.ptr(weights), K.ptr(noise), world,
                                        K.ptr(d.send), K.ptr(d.counts), K.ptr(d.pair_row), K.ptr(d.pair_w), K.ptr(d.row_slots),
                                        K.ptr(ws), ws.numel(), K.stream_of(dev)), h)
         return d
@@ -220,15 +239,17 @@ class ExpertParallel:
         dev = dout.device
         nat = self.native(dev)
         n_slots = d.pair_row.shape[0]
+        if dout.shape[0] == 0:
+            return torch.zeros(n_slots, dout.shape[1], device=dev, dtype=torch.float32)      # no pairs: every slot is past them
         dback = torch.empty(n_slots, dout.shape[1], device=dev, dtype=torch.float32)
         h = K.ctx(dev)
         K.check(K.lib().mn_model_ep_combine_backward(h, nat.handle, n_slots, K.ptr(d.pair_row), K.ptr(d.pair_w), K.ptr(K.f32c(dout)),
                                                      K.ptr(dback), K.stream_of(dev)), h)
         return dback
 
-    def _forward_device(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor]) -> torch.Tensor:
+    def _forward_device(self, x: torch.Tensor, sigma_noise: Optional[torch.Tensor], rows_cap: Optional[int] = None) -> torch.Tensor:
         world = dist.get_world_size(self.group)
-        d = self.dispatch(x, sigma_noise, world)
+        d = self.dispatch(x, sigma_noise, world, rows_cap)
         recv, recv_counts = torch.empty_like(d.send), torch.empty_like(d.counts)
         dist.all_to_all_single(recv, d.send, group=self.group)
         dist.all_to_all_single(recv_counts, d.counts, group=self.group)

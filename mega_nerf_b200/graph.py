@@ -23,7 +23,7 @@ import torch
 from torch import nn
 
 from . import _cabi as K
-from .render import _unwrap, render_rays, render_rays_fused
+from .render import _refuse_bg_ep, _unwrap, render_rays, render_rays_fused
 
 
 class GraphedRenderRays:
@@ -37,6 +37,7 @@ class GraphedRenderRays:
         bg_nerf / sphere_center / sphere_radius / get_bg_fg_rgb: as for render_rays (the background path)."""
         if nerf.training or (bg_nerf is not None and bg_nerf.training):
             raise ValueError('GraphedRenderRays replays the inference path; call nerf.eval() first')
+        _refuse_bg_ep(bg_nerf, 'GraphedRenderRays')
         self.nerf, self.hparams = nerf, hparams
         self.flags = (get_depth, get_depth_variance, False)
         self.bg_nerf = bg_nerf

@@ -59,9 +59,12 @@ class _Stage:
                                         K.ptr(z), K.ptr(xyz), self.st), self.h)
         return z, xyz
 
+    # A pass over no rays (a background pass under expert parallelism on a rank with no background ray) calls no entry point:
+    # an empty tensor has no data pointer.
     def stratify(self, z1d, rand, perturb, N, S):
         out = self.new(N, S)
-        K.check(self.L.mn_stratify(self.h, K.ptr(z1d), 0, K.ptr(rand), float(perturb), N, S, K.ptr(out), self.st), self.h)
+        if N > 0:
+            K.check(self.L.mn_stratify(self.h, K.ptr(z1d), 0, K.ptr(rand), float(perturb), N, S, K.ptr(out), self.st), self.h)
         return out
 
     def points_from_z(self, rays, z):
@@ -74,15 +77,17 @@ class _Stage:
         N, S = z_coarse.shape
         out = self.new(N, F)
         ustride = 0 if u.dim() == 1 else F
-        K.check(self.L.mn_sample_pdf(self.h, K.ptr(z_coarse), K.ptr(weights), weights.shape[1], None, K.ptr(u), ustride,
-                                     N, S, F, K.ptr(out), None, None, self.st), self.h)
+        if N > 0:
+            K.check(self.L.mn_sample_pdf(self.h, K.ptr(z_coarse), K.ptr(weights), weights.shape[1], None, K.ptr(u), ustride,
+                                         N, S, F, K.ptr(out), None, None, self.st), self.h)
         return out
 
     def sort_cat(self, a, b, descending=False):
         N = a.shape[0]
         out = self.new(N, a.shape[1] + b.shape[1])
-        K.check(self.L.mn_sort_cat(self.h, K.ptr(a), a.shape[1], K.ptr(b), b.shape[1], N, int(descending), K.ptr(out),
-                                   self.st), self.h)
+        if N > 0:
+            K.check(self.L.mn_sort_cat(self.h, K.ptr(a), a.shape[1], K.ptr(b), b.shape[1], N, int(descending), K.ptr(out),
+                                       self.st), self.h)
         return out
 
     def composite(self, raw, z, dreal, raw2, z2, dreal2, last_delta, flip, want_w, want_rgb, want_depth, want_var,
@@ -94,9 +99,10 @@ class _Stage:
         depth = self.new(N) if want_depth else None
         var = self.new(N) if want_var else None
         lam = self.new(N) if want_lambda else None
-        K.check(self.L.mn_composite(self.h, K.ptr(raw), K.ptr(z), K.ptr(dreal), S, K.ptr(raw2), K.ptr(z2), K.ptr(dreal2), S2,
-                                    K.ptr(last_delta), N, int(flip), K.ptr(w), K.ptr(rgb), K.ptr(depth), K.ptr(var),
-                                    K.ptr(lam), self.st), self.h)
+        if N > 0:
+            K.check(self.L.mn_composite(self.h, K.ptr(raw), K.ptr(z), K.ptr(dreal), S, K.ptr(raw2), K.ptr(z2), K.ptr(dreal2),
+                                        S2, K.ptr(last_delta), N, int(flip), K.ptr(w), K.ptr(rgb), K.ptr(depth), K.ptr(var),
+                                        K.ptr(lam), self.st), self.h)
         return w, rgb, depth, var, lam
 
     def intersect_sphere(self, rays, center, radius):
@@ -111,22 +117,25 @@ class _Stage:
         n, S = depth.shape
         pts = self.new(n, S, 7 if real else 4)
         dreal = self.new(n, S)
-        K.check(self.L.mn_points_outside(self.h, K.ptr(rays), K.ptr(ids), K.ptr(depth), K.ptr(center), K.ptr(radius), n, S,
-                                         int(real), int(c2d), K.ptr(pts), K.ptr(dreal), self.st), self.h)
+        if n > 0:
+            K.check(self.L.mn_points_outside(self.h, K.ptr(rays), K.ptr(ids), K.ptr(depth), K.ptr(center), K.ptr(radius), n, S,
+                                             int(real), int(c2d), K.ptr(pts), K.ptr(dreal), self.st), self.h)
         return pts, dreal
 
     def sh_to_rgb(self, deg, coef, dirs, S):
         B = coef.shape[0]
         out = self.new(B, 4)
-        K.check(self.L.mn_sh_to_rgb(self.h, deg, K.ptr(coef), coef.shape[1], K.ptr(dirs), dirs.stride(0), S, B, 1,
-                                    K.ptr(out), self.st), self.h)
+        if B > 0:
+            K.check(self.L.mn_sh_to_rgb(self.h, deg, K.ptr(coef), coef.shape[1], K.ptr(dirs), dirs.stride(0), S, B, 1,
+                                        K.ptr(out), self.st), self.h)
         return out
 
 
 def _query(sg: _Stage, net: nn.Module, hparams: Namespace, typ: str, xyz: torch.Tensor, dirs: torch.Tensor,
-           idx: Optional[torch.Tensor], call: Optional[nn.Module] = None) -> torch.Tensor:
+           idx: Optional[torch.Tensor], call: Optional[nn.Module] = None, rays_cap: Optional[int] = None) -> torch.Tensor:
     """Model query for [n,S,C] points -> raw [n,S,4] = (rgb, sigma).  rendering.py:275-334.
-    `call` is the module as the caller handed it in (e.g. DistributedDataParallel around `net`)."""
+    `call` is the module as the caller handed it in (e.g. DistributedDataParallel around `net`).  rays_cap: under expert
+    parallelism, the ray count the exchange is sized for, the same on every rank (default n)."""
     n, S, Cc = xyz.shape
     B = n * S
     native = net._native()
@@ -136,7 +145,8 @@ def _query(sg: _Stage, net: nn.Module, hparams: Namespace, typ: str, xyz: torch.
     if net.training:
         # same draw order / shapes as the reference's per-chunk torch.rand (rendering.py:294,321)
         ch = hparams.model_chunk_size
-        noise = torch.cat([torch.rand(min(ch, B - a), 1, device=xyz.device) for a in range(0, B, ch)], 0)
+        noise = torch.cat([torch.rand(min(ch, B - a), 1, device=xyz.device) for a in range(0, B, ch)], 0) if B > 0 \
+            else xyz.new_empty(0, 1)
     rr = RayRows(xyz, S, dirs if use_dirs else None, idx)
     target = call if call is not None else net
     ep = getattr(net, '_ep', None)
@@ -148,7 +158,7 @@ def _query(sg: _Stage, net: nn.Module, hparams: Namespace, typ: str, xyz: torch.
             cols.append(dirs.unsqueeze(1).expand(n, S, 3).reshape(B, 3))
         if idx is not None:
             cols.append(idx.view(n, 1, 1).expand(n, S, 1).reshape(B, 1))
-        out = ep.forward(torch.cat(cols, 1) if len(cols) > 1 else cols[0], noise)
+        out = ep.forward(torch.cat(cols, 1) if len(cols) > 1 else cols[0], noise, None if rays_cap is None else rays_cap * S)
     elif native.needs_grad():
         # through the wrapper's __call__, like `nerf(x)` in the reference (rendering.py:296-299)
         out = target(typ == 'coarse', rr, sigma_noise=noise) if isinstance(net, Cascade) else target(rr, sigma_noise=noise)
@@ -163,8 +173,8 @@ def _query(sg: _Stage, net: nn.Module, hparams: Namespace, typ: str, xyz: torch.
 def _two_pass(sg: _Stage, net: nn.Module, hparams: Namespace, dirs: torch.Tensor, idx: Optional[torch.Tensor],
               xyz_coarse: torch.Tensor, z: torch.Tensor, last_delta: torch.Tensor, get_depth: bool,
               get_depth_variance: bool, get_bg_lambda: bool, flip: bool, depth_real: Optional[torch.Tensor],
-              xyz_fine_fn: Callable, call: Optional[nn.Module] = None) -> Dict[str, torch.Tensor]:
-    """coarse -> resample -> fine  (rendering.py:176-248 with _inference :251-393 inlined)."""
+              xyz_fine_fn: Callable, call: Optional[nn.Module] = None, rays_cap: Optional[int] = None) -> Dict[str, torch.Tensor]:
+    """coarse -> resample -> fine  (rendering.py:176-248 with _inference :251-393 inlined).  rays_cap: as for _query."""
     res: Dict[str, torch.Tensor] = {}
     fine = hparams.fine_samples > 0
     cascade = hparams.use_cascade
@@ -175,7 +185,7 @@ def _two_pass(sg: _Stage, net: nn.Module, hparams: Namespace, dirs: torch.Tensor
     if flip:
         xyz_c = torch.flip(xyz_coarse, dims=[-2]).contiguous()
         z_c = torch.flip(z, dims=[-1]).contiguous()
-    raw_c = _query(sg, net, hparams, 'coarse', xyz_c, dirs, idx, call)
+    raw_c = _query(sg, net, hparams, 'coarse', xyz_c, dirs, idx, call, rays_cap)
     grad = raw_c.requires_grad
 
     def composite(raw, zz, dreal, raw2, z2, dreal2, want_depth, want_var, want_lambda):
@@ -237,11 +247,11 @@ def _two_pass(sg: _Stage, net: nn.Module, hparams: Namespace, dirs: torch.Tensor
         if flip:
             xyz_f = torch.flip(xyz_f, dims=[-2]).contiguous()
             z_f = torch.flip(z_f, dims=[-1]).contiguous()
-        raw_f = _query(sg, net, hparams, 'fine', xyz_f, dirs, idx, call)
+        raw_f = _query(sg, net, hparams, 'fine', xyz_f, dirs, idx, call, rays_cap)
         rgb, depth, var, lam = composite(raw_f, z_f, dreal_f, None, None, None, get_depth or get_depth_variance,
                                          get_depth_variance, get_bg_lambda)
     else:
-        raw_f = _query(sg, net, hparams, 'fine', xyz_f, dirs, idx, call)
+        raw_f = _query(sg, net, hparams, 'fine', xyz_f, dirs, idx, call, rays_cap)
         rgb, depth, var, lam = composite(raw_f, z_f, dreal_f, raw_c, z_c, depth_real if dreal_f is not None else None,
                                          get_depth or get_depth_variance, get_depth_variance, get_bg_lambda)
     res['rgb_fine'] = rgb
@@ -294,10 +304,10 @@ def _render(net, bg, rays, image_indices, hparams, sphere_center, sphere_radius,
     center = K.f32c(sphere_center.to(dev)) if sphere_center is not None else None
     radius = K.f32c(sphere_radius.to(dev)) if sphere_radius is not None else None
 
-    def bg_pass(ids, last, real):
+    def bg_pass(ids, last, real, rays_cap=None):
         """The background network's render of the rays `ids` (rendering.py:44-72): half the coarse samples, the points outside
         the sphere, flipped two-pass render.  last: the last delta of every ray; real: whether the points carry the real-xyz
-        prefix."""
+        prefix; rays_cap: under expert parallelism, the ray count the exchanges are sized for."""
         n, half = ids.shape[0], S // 2
         bz1 = torch.linspace(0, 1, half, device=dev)
         rnd = torch.rand(n, half, device=dev) if perturb > 0 else None
@@ -307,16 +317,25 @@ def _render(net, bg, rays, image_indices, hparams, sphere_center, sphere_radius,
         bpts, breal = mk(bz)
         return _two_pass(sg, bg, hparams, rays[ids][:, 3:6], idx[ids].contiguous() if idx is not None else None, bpts, bz,
                          torch.full((n,), last, device=dev, dtype=torch.float32), get_depth, get_depth_variance,
-                         False, True, breal, mk, call_bg)
+                         False, True, breal, mk, call_bg, rays_cap)
 
+    bg_ep = getattr(bg, '_ep', None) if bg is not None else None
     if bg is not None:
         fg_far = sg.intersect_sphere(rays, center, radius)
         fg_far = torch.maximum(fg_far, rays[:, 6])
         with_bg = torch.arange(N, device=dev)[rays[:, 7] > fg_far]          # host sync, as in the reference (:37)
-        if with_bg.shape[0] > 0:
+        n_bg = with_bg.shape[0]
+        # A background network under expert parallelism is queried through its group's collectives, so every rank runs the
+        # background pass whenever any rank has a background ray - a rank with none included - with the exchanges sized for
+        # the largest count.  It runs here, before the foreground pass, on every rank: ranks that issued the two networks'
+        # exchanges in different orders would deadlock.
+        n_max = bg_ep.max_over_ranks(n_bg, dev) if bg_ep is not None else n_bg
+        if n_bg > 0:
             last_delta[with_bg] = fg_far[with_bg]
             far_override = torch.minimum(rays[:, 7], fg_far)
-            bg_res = bg_pass(with_bg, 1e10, hparams.container_path is not None or hparams.train_mega_nerf is not None)
+        if n_max > 0:
+            bg_res = bg_pass(with_bg, 1e10, hparams.container_path is not None or hparams.train_mega_nerf is not None,
+                             n_max if bg_ep is not None else None)
 
     steps = torch.linspace(0, 1, S, device=dev)
     rnd = torch.rand(N, S, device=dev) if perturb > 0 else None
@@ -342,11 +361,20 @@ def _render(net, bg, rays, image_indices, hparams, sphere_center, sphere_radius,
                         res[f'fg_{name}'] = val
                         res[f'bg_{name}'] = add
                     res[name] = val + add
-                elif get_bg_fg_rgb:
-                    res[f'fg_{name}'] = val
-                    res[f'bg_{name}'] = torch.zeros_like(val)
+                else:
+                    if get_bg_fg_rgb:
+                        res[f'fg_{name}'] = val
+                        res[f'bg_{name}'] = torch.zeros_like(val)
+                    if bg_res is not None:
+                        # a background pass over no rays (expert parallelism): bg_res[name] has no rows, so the values stay and
+                        # only the graph edge is added - the backward then runs the background's exchanges on this rank too, in
+                        # the order of every other rank
+                        res[name] = torch.cat([val, bg_res[name]], 0)
     present = bool(bg is not None and with_bg.shape[0] > 0)
-    if bg is not None and not present and 'RANK' in os.environ and net.training:
+    # Under background expert parallelism there is no dummy ray: the owners need no DDP hook, and its draws and exchanges would
+    # come after the foreground pass.  A training rank with no background ray therefore draws less from the random stream
+    # than a DDP run of the reference does in the same step.
+    if bg is not None and bg_ep is None and not present and 'RANK' in os.environ and net.training:
         # Distributed training with no background ray in this batch (rendering.py:143-171): the reference renders ONE
         # dummy background ray through bg_nerf - i.e. through its DistributedDataParallel wrapper, whose forward is
         # what arms the gradient reducer for this iteration - and adds 0 x its colour, so that this rank joins the
@@ -362,6 +390,12 @@ def _render(net, bg, rays, image_indices, hparams, sphere_center, sphere_radius,
     return res, present
 
 
+def _refuse_bg_ep(bg: Optional[nn.Module], fn: str) -> None:
+    """The one-call path sequences a background pass in C, where the NCCL exchanges of expert parallelism cannot run."""
+    if bg is not None and getattr(_unwrap(bg), '_ep', None) is not None:
+        raise ValueError(f'{fn} cannot render a background network under expert parallelism: use render_rays')
+
+
 def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Optional[torch.Tensor], hparams: Namespace,
                       get_depth: bool, get_depth_variance: bool, bg_nerf: Optional[nn.Module] = None,
                       sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None,
@@ -374,6 +408,7 @@ def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
     status check at the end, where the reference checks its sphere bound too: a camera outside the ellipsoid raises its
     `Exception`.  `check_status=False` leaves that check to the caller (CUDA-graph capture, where no sync may happen)."""
     net, bg = _nets(nerf, bg_nerf, 'render_rays_fused')
+    _refuse_bg_ep(bg, 'render_rays_fused')
     if net.training or (bg is not None and bg.training):
         raise ValueError('render_rays_fused is the inference path; call nerf.eval() first')
     if bool(hparams.use_cascade) != isinstance(net, Cascade):
