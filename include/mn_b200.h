@@ -434,8 +434,8 @@ int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const
  * activations to the tape; backward = data gradients on transposed fp16 weight images (ReLU masks from the tape, gradient
  * images scaled by a power of two chosen from max|grad_out|), weight gradients as wgmma contractions of the two tapes
  * over the slot axis, fp32 accumulation, fp32 atomics into param_grads_d.  Same argument meaning as the fp32 entry points
- * above; covers layer_dim 256, 512 (up to 10 trunk layers) and 768..2048 (a multiple of 256; the layer-GEMM path, backward
- * one tile group at a time) with a direction / appearance head and either rgb_dim 3 or a raw SH head (rgb_dim <= 80, i.e.
+ * above; covers layer_dim 256..4096 with 2..16 trunk layers (256 and 512 wide up to 12 layers on the fused kernel; every other
+ * width and depth on the layer-GEMM path, backward one tile group at a time) with a direction / appearance head and either rgb_dim 3 or a raw SH head (rgb_dim <= 80, i.e.
  * sh_deg <= 4; rgb_dim 48 and 75 run on the layer-GEMM path at 256 and 512 wide too), no affine appearance (mn_model_train_tc_supported), everything else returns MN_ERR_UNSUPPORTED - use the fp32 entry points.
  * The first recording call allocates the transposed weight images of the backward (about 4.25 MiB per 512-wide and 71 MB
  * per 2048-wide sub-module).
@@ -461,6 +461,15 @@ int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, co
  * feature-tile bytes, ring-stage bytes, K columns per stage}.  Returns MN_ERR_UNSUPPORTED for shapes only the fp32 kernels
  * run, MN_ERR_WORKSPACE when cap_entries is too small.  Used by tests/test_tp_program.py and tests/tp_protocol_sim.py. */
 int mn_debug_tp_program(const mn_model_desc* desc, unsigned int* table_out, int cap_entries, int* info8);
+/* The same for one launch of the kernel: MN_TP_INFER is mn_debug_tp_program; MN_TP_TRAIN_FWD the recording forward of tc_f16
+ * training (the forward program in the training variant's shared-memory layout); MN_TP_DGRAD the data-gradient chain of its
+ * backward (one GEMM per Linear from dir_a_encoding down to trunk layer 1 on the transposed weight images, no feature segments;
+ * info[1] == info[0], as no sigma_only form exists).  The training modes return MN_ERR_UNSUPPORTED unless the fused kernel
+ * trains the shape (mn_model_train_tc_supported, and not the layer-GEMM engine).  Used by tests/test_tp_deep_train_program.py. */
+#define MN_TP_INFER 0
+#define MN_TP_TRAIN_FWD 1
+#define MN_TP_DGRAD 2
+int mn_debug_tp_program_mode(const mn_model_desc* desc, int mode, unsigned int* table_out, int cap_entries, int* info8);
 
 #ifdef __cplusplus
 }

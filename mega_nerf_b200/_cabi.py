@@ -66,6 +66,7 @@ SIGNATURES = {
     'mn_rays_pairs': (_I, [_P, _P, _L, _P, _I, _P, _P, _L, _F, _F, _I, _F, _F, _P, _P]),
     'mn_gather_batch': (_I, [_P, _P, _L, _L, _P, _I, _P, _P, _I, _P, _P, _I, _P, _P]),
     'mn_debug_tp_program': (_I, [_P, _P, _I, _P]),
+    'mn_debug_tp_program_mode': (_I, [_P, _I, _P, _I, _P]),
     'mn_sample_coarse': (_I, [_P, _P, _P, _P, _P, _F, _L, _I, _P, _P, _P]),
     'mn_stratify': (_I, [_P, _P, _L, _P, _F, _L, _I, _P, _P]),
     'mn_points_from_z': (_I, [_P, _P, _P, _L, _I, _P, _P]),

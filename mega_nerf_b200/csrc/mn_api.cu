@@ -174,14 +174,18 @@ extern "C" {
 
 int mn_abi_version(void) { return MN_ABI_VERSION; }
 
-int mn_debug_tp_program(const mn_model_desc* desc, unsigned int* table_out, int cap_entries, int* info8) {
-    if (!desc || !table_out || !info8) return MN_ERR_INVALID;
+int mn_debug_tp_program_mode(const mn_model_desc* desc, int mode, unsigned int* table_out, int cap_entries, int* info8) {
+    if (!desc || !table_out || !info8 || mode < MN_TP_INFER || mode > MN_TP_DGRAD) return MN_ERR_INVALID;
     if (desc->layers < 1 || desc->layers > MN_MAX_LAYERS || desc->xyz_dim < 3 || desc->xyz_dim > 4 || desc->n_skip < 0 || desc->n_skip > 8)
         return MN_ERR_INVALID;
     mn_model m;
     m.d = *desc;
     build_layout(&m);
-    return mn_mlp_tp_program(m, table_out, cap_entries, info8);
+    return mn_mlp_tp_program(m, mode, table_out, cap_entries, info8);
+}
+
+int mn_debug_tp_program(const mn_model_desc* desc, unsigned int* table_out, int cap_entries, int* info8) {
+    return mn_debug_tp_program_mode(desc, MN_TP_INFER, table_out, cap_entries, info8);
 }
 
 int mn_create(mn_ctx** out, int device) {

@@ -39,8 +39,9 @@ enum { SRC_H = 0, SRC_XPE = 1, SRC_XAUX = 2 };
 enum { EPI_RELU = 0, EPI_RELU_SIGMA = 1, EPI_LINEAR = 2, EPI_RGB = 3,
        // data-gradient chain (training, mn_train_tc.cuh): plain copy, ReLU mask from the activation tape, mask + sigma-head term
        EPI_D_LINEAR = 4, EPI_D_MASK = 5, EPI_D_MASK_SIGMA = 6 };
-// kernel modes of tc_mlp_wg_kernel
+// kernel modes of tc_mlp_wg_kernel (the test hook mn_debug_tp_program_mode names them MN_TP_*)
 enum { PP_INFER = 0, PP_TRAIN_FWD = 1, PP_DGRAD = 2 };
+static_assert(PP_INFER == MN_TP_INFER && PP_TRAIN_FWD == MN_TP_TRAIN_FWD && PP_DGRAD == MN_TP_DGRAD, "mn_debug_tp_program_mode modes");
 
 struct TcGemm {
     int n;           // MMA N = columns of the weight image (layer engine: the output columns padded to 256-column blocks)
@@ -210,8 +211,9 @@ void build_dgrad_plan(const NetDims& nd, const TcLinears& T, bool layer, TcPlan*
 // ---- which engine serves a network, and whether tensor-core training covers it.  The fused engine takes rgb_dim <= 32 (its
 // N = 32 rgb GEMM) at 64..256 (a multiple of 64) and 512 wide, up to 12 trunk layers; the layer engine every other width of
 // 64..kLgMaxL and depth (up to MN_MAX_LAYERS), and the SH heads of degree 3 and 4 (rgb_dim <= MN_TC_LG_RGB_MAX).  Training
-// runs on the fused engine at 256 and 512 wide (up to 10 trunk layers) and on the layer engine from 256 wide; it needs
-// dir_a_encoding (its data-gradient chain ends there) and no affine appearance.
+// runs on the fused engine at 256 and 512 wide (every depth it takes, 2..12 trunk layers) and on the layer engine from 256
+// wide; it needs dir_a_encoding (its data-gradient chain ends there) and no affine appearance.  A network is trained on the
+// engine that runs its inference, so the recording forward writes the tape that engine's backward reads.
 enum { TC_NONE = 0, TC_FUSED = 1, TC_LAYER = 2 };
 constexpr int kLgMaxL = 4096;
 struct TcNet {
@@ -235,7 +237,7 @@ TcNet tc_net(const mn_model& m) {
     t.lin = tc_linears(m, layer);
     if (t.engine != TC_NONE) build_plan(nd, t.lin, layer, &t.P);
     t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.layers >= 2 &&
-              ((layer && nd.L >= 256) || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 10));
+              ((layer && nd.L >= 256) || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 12));
     if (t.train) build_dgrad_plan(nd, t.lin, layer, &t.D);
     return t;
 }
@@ -655,11 +657,14 @@ size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision)
 }
 
 
-int mn_mlp_tp_program(const mn_model& m, unsigned int* table_out, int cap_entries, int* info8) {
+// mode: PP_INFER (the tc_f16 inference launch), PP_TRAIN_FWD (the recording forward: the forward plan in the training variant's
+// layout) or PP_DGRAD (the data-gradient chain of the backward on the transposed images); the training modes only for shapes
+// whose training runs on the fused engine.
+int mn_mlp_tp_program(const mn_model& m, int mode, unsigned int* table_out, int cap_entries, int* info8) {
     const TcNet net = tc_net(m);
-    if (net.engine != TC_FUSED) return MN_ERR_UNSUPPORTED;
-    const TcPlan& P = net.P;
-    const WgLayout L = wg_layout(P, false, wg_reg_act(PP_INFER, false, P.L > 256));     // the tc_f16 inference launch's layout
+    if (net.engine != TC_FUSED || (mode != PP_INFER && !net.train)) return MN_ERR_UNSUPPORTED;
+    const TcPlan& P = mode == PP_DGRAD ? net.D : net.P;
+    const WgLayout L = wg_layout(P, false, wg_reg_act(mode, false, P.L > 256));     // the tc_f16 launch's layout
     int n = 0, n_trunk = 0;
     for (int gi = 0; gi < P.n_gemm; ++gi) {
         const int nch = (P.g[gi].n + 255) >> 8;

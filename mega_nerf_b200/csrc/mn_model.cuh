@@ -178,7 +178,8 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
                      size_t ws_bytes, cudaStream_t st);
 size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision);
 int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st);
-int mn_mlp_tp_program(const mn_model& m, unsigned int* table_out, int cap_entries, int* info8);   // host only (test hook)
+// host only (test hook): mode 0 inference, 1 recording forward, 2 data-gradient chain (MN_TP_* in mn_b200.h)
+int mn_mlp_tp_program(const mn_model& m, int mode, unsigned int* table_out, int cap_entries, int* info8);
 // ---- tensor-core training path (csrc/mn_train_tc.cuh): per-tile tape records and the two passes
 // An activation record (and the backward pass's gradient record, same layout) holds fp16 images in the layout of the MLP
 // kernel's activation buffer, [cols/8][128 slots][8], one every cols * 128 * 2 bytes: H_0 .. H_{layers-1}, then F
@@ -203,7 +204,7 @@ struct TrainTcTape {
 };
 // the shapes whose recording calls run on the tensor cores (tc_net in mn_mlp_tc.cu; mn_model_train_tc_supported)
 #define MN_TC_TRAIN_COVERAGE                                                                                                     \
-    "tensor-core training covers layer_dim 256..4096 (at 256 and 512: up to 10 or 13..16 layers) with a direction / appearance head, " \
+    "tensor-core training covers layer_dim 256..4096 with 2..16 layers and a direction / appearance head, "                       \
     "rgb_dim 3 or a raw SH head (rgb_dim <= 80: sh_deg <= 4), no affine appearance; use train precision 'fp32'"
 size_t mn_train_tc_x_tile_bytes(const mn_model* m);
 size_t mn_train_tc_act_tile_bytes(const mn_model* m);

@@ -52,11 +52,11 @@ def set_train_precision(name: str) -> None:
     'fp32'   CUDA-core kernels - the parity mode (gradients equal the reference's fp32 autograd to its own noise level);
     'tc_f16' tensor cores: fp16 operands, fp32 accumulation, gradient images scaled by a power of two - what the reference
              does on a GPU under autocast + GradScaler (runner.py:243-274).  The tensor-core training kernels cover
-             layer_dim 256..4096 (any width, e.g. the nerf, npp and mega-nerf-dense configs' 2048; at 256 and 512 with up
-             to 10 or with 13..16 trunk layers) with a
+             layer_dim 256..4096 (any width, e.g. the nerf, npp and mega-nerf-dense configs' 2048) with 2..16 trunk
+             layers and a
              direction / appearance head and either an rgb head (rgb_dim 3) or a raw SH head (rgb_dim <= 80: sh_deg
              0..4; degrees 3 and 4 on the layer-GEMM path at every one of these widths); other networks (narrower ones,
-             256 and 512 wide with 11 or 12 layers, affine appearance, heads without dir_a_encoding) silently use the
+             one-layer ones, affine appearance, heads without dir_a_encoding) silently use the
              fp32 kernels, which refuse layer_dim > 512 and widths that are not a multiple of 64 -
              NativeModel.train_on_tensor_cores() tells which."""
     global _train_precision
