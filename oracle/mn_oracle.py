@@ -226,13 +226,22 @@ class Net:
         return 1 if self.cluster_2d else 0
 
 
-def net_to(net: Optional[Net], device) -> Optional[Net]:
-    """The same network with its tensors on `device` (bench.py: the restatement under torch-CUDA as the GPU incumbent)."""
+def net_to(net: Optional[Net], device, dtype: Optional[torch.dtype] = None) -> Optional[Net]:
+    """The same network with its tensors on `device` (bench.py: the restatement under torch-CUDA as the GPU incumbent) and,
+    given a dtype, converted to it: weights and centroids."""
     if net is None:
         return None
     import dataclasses
-    return dataclasses.replace(net, weights=[{k: v.to(device) for k, v in w.items()} for w in net.weights],
-                               centroids=net.centroids.to(device) if net.centroids is not None else None)
+    return dataclasses.replace(net, weights=[{k: v.to(device=device, dtype=dtype) for k, v in w.items()} for w in net.weights],
+                               centroids=net.centroids.to(device=device, dtype=dtype) if net.centroids is not None else None)
+
+
+def net_double(net: Optional[Net]) -> Optional[Net]:
+    """The same network in float64 on the same device.  render_rays on float64 rays (and float64 sphere centre / radius) then
+    runs end to end in float64: the high-precision reference of the sampling, resampling and compositing arithmetic."""
+    if net is None:
+        return None
+    return net_to(net, next(iter(net.weights[0].values())).device, torch.float64)
 
 
 def route(net: Net, x: torch.Tensor):
@@ -350,7 +359,7 @@ def sample_cdf(bins: torch.Tensor, cdf: torch.Tensor, n_fine: int, det: bool,
     n_rays, n_bins = cdf.shape
     cdf = torch.cat([torch.zeros_like(cdf[:, :1]), cdf], -1)
     if u is None:
-        u = (torch.linspace(0, 1, n_fine, device=cdf.device).expand(n_rays, n_fine) if det
+        u = (torch.linspace(0, 1, n_fine, device=cdf.device, dtype=cdf.dtype).expand(n_rays, n_fine) if det
              else torch.rand(n_rays, n_fine, device=cdf.device))
     u = u.contiguous()
     inds = torch.searchsorted(cdf, u, right=True)
@@ -564,7 +573,7 @@ def render_rays(net: Net, bg_net: Optional[Net], rays: torch.Tensor, image_indic
         image_indices = image_indices.unsqueeze(-1).unsqueeze(-1)
     perturb = opts.perturb if net.training else 0
     dev = rays.device
-    last_delta = 1e10 * torch.ones(n, 1, device=dev)
+    last_delta = 1e10 * torch.ones(n, 1, device=dev, dtype=rays.dtype)
     with_bg = None
     if bg_net is not None:
         fg_far = intersect_sphere(o, d, sphere_center, sphere_radius)
@@ -576,16 +585,16 @@ def render_rays(net: Net, bg_net: Optional[Net], rays: torch.Tensor, image_indic
         last_delta[with_bg, 0] = fg_far[with_bg]
         far = torch.minimum(far.squeeze(), fg_far).unsqueeze(-1)
         half = opts.coarse_samples // 2
-        bz = stratify(torch.linspace(0, 1, half, device=dev), half, perturb, with_bg.shape[0])
+        bz = stratify(torch.linspace(0, 1, half, device=dev, dtype=rays.dtype), half, perturb, with_bg.shape[0])
         xyz_real = opts.container_path is not None or opts.train_mega_nerf is not None
         c2d = xyz_real and net.cluster_dim_start == 1
         mk = lambda zz: points_outside(o[with_bg], d[with_bg], zz, sphere_center, sphere_radius, xyz_real, c2d)
         bpts, breal = mk(bz)
         bg_res = _two_pass(bg_net, opts, d[with_bg],
                            image_indices[with_bg] if image_indices is not None else None,
-                           bpts, bz, 1e10 * torch.ones(with_bg.shape[0], 1, device=dev), get_depth, get_depth_variance,
-                           False, True, breal, mk)
-    t = torch.linspace(0, 1, opts.coarse_samples, device=dev)
+                           bpts, bz, 1e10 * torch.ones(with_bg.shape[0], 1, device=dev, dtype=rays.dtype), get_depth,
+                           get_depth_variance, False, True, breal, mk)
+    t = torch.linspace(0, 1, opts.coarse_samples, device=dev, dtype=rays.dtype)
     z = stratify(near * (1 - t) + far * t, opts.coarse_samples, perturb, n)
     xyz = o + d * z.unsqueeze(-1)
     res = _two_pass(net, opts, d, image_indices, xyz, z, last_delta, get_depth, get_depth_variance,
