@@ -471,6 +471,55 @@ int mn_debug_tp_program(const mn_model_desc* desc, unsigned int* table_out, int 
 #define MN_TP_DGRAD 2
 int mn_debug_tp_program_mode(const mn_model_desc* desc, int mode, unsigned int* table_out, int cap_entries, int* info8);
 
+/* ---- test hook (host only, no CUDA call): where the tensor-core training passes keep their intermediates -----------------
+ * For a call of mn_model_forward_train_tc / mn_model_backward_tc over B rows of model m, out[] receives (indices MN_TCL_*):
+ * the engine (0 not trained on the tensor cores, 1 the fused kernel, 2 the layer-GEMM engine); the tile count and byte size of
+ * the tape and the byte offsets of its regions (routing counters, slot_row and slot_w or -1, encoder tiles, activation
+ * records, fp32 head blocks); the bytes of one encoder tile and of one activation record; the padded widths of the encoder
+ * segments and of the H / G images; the rows of the fp32 head block (sigma pre-activation, rgb, image id) and of the
+ * head-gradient block; the backward workspace's size and the byte offsets, from workspace_d rounded up to 256 bytes, of the
+ * gradient images (fused engine: one record per tile, laid out as the activation records), the head-gradient blocks, the
+ * per-image embedding sums ([n_sub][app_count][emb_k] floats) and the scale S, then emb_k and the tiles the head-gradient
+ * blocks cover; on the layer engine the offsets of the dZ_G image and of the two ping-pong gradient images of the last tile
+ * group (-1 on the fused engine); then the number of images of a record and, per image (trunk layers, F, G), its byte offset
+ * in the record and its columns.  Every tile image is [cols/8][128 rows][8] fp16.  Returns the entries written, or
+ * MN_ERR_WORKSPACE when cap is too small.  Used by tests/test_gpu_zzc_train_tc_stages.py. */
+#define MN_TCL_ENGINE 0
+#define MN_TCL_N_TILES 1
+#define MN_TCL_TAPE_BYTES 2
+#define MN_TCL_TAPE_COUNTERS 3
+#define MN_TCL_TAPE_SLOT_ROW 4
+#define MN_TCL_TAPE_SLOT_W 5
+#define MN_TCL_TAPE_XREG 6
+#define MN_TCL_TAPE_ACT 7
+#define MN_TCL_TAPE_F32 8
+#define MN_TCL_X_TILE 9
+#define MN_TCL_ACT_TILE 10
+#define MN_TCL_KPE 11
+#define MN_TCL_KAUX 12
+#define MN_TCL_HC 13
+#define MN_TCL_GC 14
+#define MN_TCL_F32_SIGMA 15
+#define MN_TCL_F32_RGB 16
+#define MN_TCL_F32_ID 17
+#define MN_TCL_F32_ROWS 18
+#define MN_TCL_G32_SIGMA 19
+#define MN_TCL_G32_RGB 20
+#define MN_TCL_G32_ROWS 21
+#define MN_TCL_BWD_BYTES 22
+#define MN_TCL_BWD_DZ 23
+#define MN_TCL_BWD_GF32 24
+#define MN_TCL_BWD_EMB 25
+#define MN_TCL_BWD_SCALE 26
+#define MN_TCL_BWD_EMB_K 27
+#define MN_TCL_BWD_HEAD_TILES 28
+#define MN_TCL_BWD_DZG 29
+#define MN_TCL_BWD_PP0 30
+#define MN_TCL_BWD_PP1 31
+#define MN_TCL_N_IMG 32
+#define MN_TCL_IMG 33
+int mn_debug_tc_train_layout(const mn_model* m, int64_t B, int64_t* out, int cap);
+
 #ifdef __cplusplus
 }
 #endif

@@ -848,6 +848,26 @@ size_t mn_model_backward_workspace_bytes_tc(const mn_model* m, int64_t B) {
     return 256 + mn_train_tc_backward_workspace(m, slot_capacity(m, B) / MN_TILE);
 }
 
+int mn_debug_tc_train_layout(const mn_model* m, int64_t B, int64_t* out, int cap) {
+    if (!m || !out || B < 0) return MN_ERR_INVALID;
+    const int64_t n_tiles = slot_capacity(m, B) / MN_TILE;
+    const int rc = mn_train_tc_layout(m, n_tiles, out, cap);
+    if (rc) return rc;
+    char* const base = (char*)(uintptr_t)4096;      // any non-null base: tape_regions_cap returns pointers base + offset
+    TapeRegions T{};
+    out[MN_TCL_N_TILES] = n_tiles;
+    out[MN_TCL_TAPE_BYTES] = (int64_t)tape_regions(m, B, true, base, &T);
+    auto off = [&](const void* p) -> int64_t { return p ? (int64_t)((const char*)p - base) : -1; };
+    out[MN_TCL_TAPE_COUNTERS] = off(T.counters);
+    out[MN_TCL_TAPE_SLOT_ROW] = off(T.slot_row);
+    out[MN_TCL_TAPE_SLOT_W] = off(T.slot_w);
+    out[MN_TCL_TAPE_XREG] = off(T.tc.xreg);
+    out[MN_TCL_TAPE_ACT] = off(T.tc.act);
+    out[MN_TCL_TAPE_F32] = off(T.tc.f32);
+    out[MN_TCL_BWD_BYTES] = (int64_t)mn_model_backward_workspace_bytes_tc(m, B);
+    return MN_TCL_IMG + 2 * (int)out[MN_TCL_N_IMG];
+}
+
 int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const float* grad_out_d, const void* tape_d,
                          size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream) {
     if (!ctx || !m || B < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;

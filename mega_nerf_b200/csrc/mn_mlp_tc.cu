@@ -412,9 +412,10 @@ __global__ void __launch_bounds__(kTileM) tc_encode_kernel(const MlpArgs a, int 
 
 
 // sin / cos of 2^k x for consecutive k (nerf.py:19-25): every fourth band is evaluated with the accurate sincosf, the
-// three bands after it by the double-angle identities.  Each doubling at most doubles the absolute error, so the
-// result stays within ~8 fp32 ulps (5e-7) of the directly evaluated value - three orders of magnitude below the fp16
-// rounding (2.4e-4) these features undergo on their way into the tensor-core operand tile.  (s, c) carry band k-1 in.
+// three bands after it by the double-angle identities.  A doubling can multiply the absolute error by up to 6 (the sine's
+// error feeds the cosine's and back), so the result is not a few ulps away: tests/test_tc_train_ref.py measures up to 1.4e-6
+// (about 24 fp32 ulps at 1) from the directly evaluated value - still two orders of magnitude below the fp16 rounding
+// (2.4e-4) these features undergo on their way into the tensor-core operand tile.  (s, c) carry band k-1 in.
 __device__ __forceinline__ void pe_band(float x, int k, float* s, float* c) {
     if ((k & 3) == 0) {
         mn_pe_sincos(x, k, s, c);
@@ -973,6 +974,49 @@ static TcBwdWorkspace tc_bwd_workspace(const mn_model* m, const TcNet& net, int6
 }
 size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
     return tc_bwd_workspace(m, tc_net(*m), n_tiles128).total;
+}
+
+// Test hook (mn_debug_tc_train_layout): entries MN_TCL_ENGINE .. of the layout the two training passes share, from the same
+// tc_net / tc_bwd_workspace the passes call.  Backward-workspace offsets are relative to the 256-byte aligned base that
+// mn_train_tc_backward carves.
+int mn_train_tc_layout(const mn_model* m, int64_t n_tiles128, int64_t* out, int cap) {
+    const TcNet net = tc_net(*m);
+    const NetDims& nd = m->nd;
+    const int n_img = nd.layers + 2;
+    if (cap < MN_TCL_IMG + 2 * n_img) return MN_ERR_WORKSPACE;
+    out[MN_TCL_ENGINE] = net.train ? net.engine : TC_NONE;
+    out[MN_TCL_X_TILE] = net.P.x_tile_bytes;
+    out[MN_TCL_ACT_TILE] = (int64_t)mn_train_tc_act_tile_bytes(m);
+    out[MN_TCL_KPE] = net.lin.kpe;
+    out[MN_TCL_KAUX] = net.lin.kaux;
+    out[MN_TCL_HC] = net.lin.hc;
+    out[MN_TCL_GC] = net.lin.gc;
+    out[MN_TCL_F32_SIGMA] = MN_TC_F32_SIGMA;
+    out[MN_TCL_F32_RGB] = MN_TC_F32_RGB;
+    out[MN_TCL_F32_ID] = MN_TC_F32_ID;
+    out[MN_TCL_F32_ROWS] = MN_TC_F32_ROWS;
+    out[MN_TCL_G32_SIGMA] = MN_TC_G32_SIGMA;
+    out[MN_TCL_G32_RGB] = MN_TC_G32_RGB;
+    out[MN_TCL_G32_ROWS] = mn_tc_g32_rows(nd.rgb_dim);
+    const TcBwdWorkspace WS = tc_bwd_workspace(m, net, n_tiles128);
+    out[MN_TCL_BWD_DZ] = 0;
+    out[MN_TCL_BWD_GF32] = (int64_t)WS.dz_bytes;
+    out[MN_TCL_BWD_EMB] = (int64_t)(WS.dz_bytes + WS.head_bytes);
+    out[MN_TCL_BWD_SCALE] = (int64_t)(WS.dz_bytes + WS.head_bytes + mn_align(WS.emb_floats * sizeof(float) + 256) - 256);
+    out[MN_TCL_BWD_EMB_K] = WS.emb_k;
+    out[MN_TCL_BWD_HEAD_TILES] = WS.head_tiles;
+    const bool layer = net.engine == TC_LAYER;
+    const size_t pp0 = layer ? mn_align((size_t)WS.head_tiles * net.lin.gc * kTileM * 2) : 0;
+    out[MN_TCL_BWD_DZG] = layer ? 0 : -1;
+    out[MN_TCL_BWD_PP0] = layer ? (int64_t)pp0 : -1;
+    out[MN_TCL_BWD_PP1] = layer ? (int64_t)(pp0 + mn_align((size_t)WS.head_tiles * net.lin.hc * kTileM * 2)) : -1;
+    out[MN_TCL_N_IMG] = n_img;
+    // image j of a record: trunk layer j (j < layers), F (layers), G (layers + 1); offset in the record and columns
+    for (int j = 0; j < n_img; ++j) {
+        out[MN_TCL_IMG + 2 * j] = (int64_t)mn_tc_img_off(j, net.lin.hc);
+        out[MN_TCL_IMG + 2 * j + 1] = j == nd.layers + 1 ? net.lin.gc : net.lin.hc;
+    }
+    return MN_OK;
 }
 
 // Weight-gradient entry of Linear j: per input segment, the item of output channels 0..127 and the segment's first X chunk.  X is

@@ -11,7 +11,8 @@ import torch
 
 import cases as C
 from oracle import mn_oracle as O
-from test_backward_wide_algorithm import TC_L2, TC_TENSOR, errors, h16, wide_tc_chain
+from tc_train_ref import errors, h16, wide_tc_chain
+from test_backward_wide_algorithm import TC_L2, TC_TENSOR
 
 L = 512
 

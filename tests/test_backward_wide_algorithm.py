@@ -9,111 +9,13 @@ it must equal autograd (the algebra); run with fp16 rounding its error figures p
 tests/test_gpu_zn_train_wide.py (TC_L2 = 3e-2 on the whole gradient vector, TC_TENSOR = 3.5e-1 per tensor)."""
 import pytest
 import torch
-import torch.nn.functional as F
 
 import cases as C
 from oracle import mn_oracle as O
+from tc_train_ref import errors, grad_scale, h16, wide_tc_chain
 
 L = 768
 TC_L2, TC_TENSOR = 3e-2, 3.5e-1          # tests/test_gpu_zk_train_tc.py
-
-
-def h16(t):
-    return t.half().float()
-
-
-def grad_scale(cot):
-    m = float(cot.abs().max())
-    return 2.0 ** (10 - torch.tensor(m).log2().ceil().item()) if 0 < m < 3e38 else 1.0
-
-
-def wide_tc_chain(spec: O.NerfSpec, w, x, cot, noise, rnd, stats=None):
-    """-> gradient dict in state-dict layout.  rnd: fp16 rounding of every tensor-core operand and tape image, or identity."""
-    L, layers, in_xyz = spec.layer_dim, spec.layers, spec.in_xyz
-    R = lambda t: rnd(t)                                                              # noqa: E731
-    mm = lambda a, b: a @ b                                                           # fp32 accumulation
-    # ---- recording forward (layer_launch with a tape)
-    pe = R(O.embed(x[:, :spec.xyz_dim], spec.pos_xyz_dim))
-    aux = []
-    if spec.pos_dir_dim > 0:
-        aux.append(O.embed(x[:, -4:-1], spec.pos_dir_dim))
-    ids = x[:, -1].long() if spec.appearance_dim > 0 else None
-    if spec.appearance_dim > 0:
-        aux.append(w['embedding_a.weight'][ids])
-    aux = R(torch.cat(aux, -1))
-    h, xin = [], []
-    cur = pe
-    for i in range(layers):
-        inp = torch.cat([pe, cur], -1) if i in spec.skip_layers else cur
-        xin.append(inp)
-        cur = R(torch.relu(mm(inp, R(w[f'xyz_encodings.{i}.0.weight']).t()) + w[f'xyz_encodings.{i}.0.bias']))
-        h.append(cur)
-    sig_pre = mm(h[-1], w['sigma.weight'].t())[:, 0] + w['sigma.bias'] + noise.view(-1)      # fp32, CUDA cores
-    f = R(mm(h[-1], R(w['xyz_encoding_final.weight']).t()) + w['xyz_encoding_final.bias'])
-    fx = torch.cat([f, aux], -1)
-    g = R(torch.relu(mm(fx, R(w['dir_a_encoding.0.weight']).t()) + w['dir_a_encoding.0.bias']))
-    lin = mm(g, w['rgb.weight'].t()) + w['rgb.bias']
-    s = torch.sigmoid(lin) if spec.rgb_dim == 3 else lin
-
-    # ---- head stage (tc_layer_head_dgrad_kernel), fp32
-    S = grad_scale(cot)
-    go_rgb, go_sig = cot[:, :spec.rgb_dim], cot[:, spec.rgb_dim]
-    if spec.shifted_softplus:
-        y = sig_pre - 1
-        dsp = torch.where(y > 20, torch.ones_like(y), 1 / (1 + torch.exp(-y)))
-    else:
-        dsp = (sig_pre > 0).float()
-    ds = go_sig * dsp
-    d = go_rgb * (1 - s) * s if spec.rgb_dim == 3 else go_rgb
-    dzg = mm(d, w['rgb.weight']) * (g > 0)                                           # fp32, unscaled
-    dzg_img = R(dzg * S)
-
-    G = {k: torch.zeros_like(v) for k, v in w.items()}
-
-    def wop(name, dz_img, xx):                                                        # tc_wgrad_kernel: dZ^T X / S
-        G[name + '.weight'] += mm(dz_img.t(), xx) / S
-        G[name + '.bias'] += dz_img.sum(0) / S
-
-    # ---- heads (tc_heads_wgrad_kernel) and the embedding (per-image sums x W_e, tc_emb_grad_kernel)
-    G['sigma.weight'] += mm(ds.unsqueeze(0), h[-1])
-    G['sigma.bias'] += ds.sum().view(1)
-    G['rgb.weight'] += mm(d.t(), g)
-    G['rgb.bias'] += d.sum(0)
-    if spec.appearance_dim > 0:
-        sums = torch.zeros(spec.appearance_count, L // 2).index_add_(0, ids, dzg)
-        G['embedding_a.weight'] += mm(sums, w['dir_a_encoding.0.weight'][:, L + spec.in_dir:])
-    # ---- data-gradient chain (tc_layer_gemm_kernel<false, true>) interleaved with the weight gradients
-    Wd = w['dir_a_encoding.0.weight']
-    wop('dir_a_encoding.0', dzg_img, fx)
-    df = R(mm(dzg_img, R(Wd[:, :L])))                                                 # no mask: F has no activation
-    wop('xyz_encoding_final', df, h[-1])
-    dz = R((mm(df, R(w['xyz_encoding_final.weight'])) + (ds * S).unsqueeze(-1) * w['sigma.weight']) * (h[-1] > 0))
-    if stats is not None:
-        stats.append(('S', S))
-    for i in range(layers - 1, -1, -1):
-        if stats is not None:
-            stats.append((f'max |S dZ_{i}|', float(dz.abs().max())))
-        wop(f'xyz_encodings.{i}.0', dz, xin[i])
-        if i == 0:
-            break
-        Wi = w[f'xyz_encodings.{i}.0.weight']
-        Wh = Wi[:, in_xyz:] if i in spec.skip_layers else Wi                          # hidden columns only
-        dz = R(mm(dz, R(Wh)) * (h[i - 1] > 0))
-    return G
-
-
-def errors(got, want):
-    num = den = 0.0
-    worst = ('', 0.0)
-    for k, v in want.items():
-        num += float((got[k].double() - v.double()).square().sum())
-        den += float(v.double().square().sum())
-        scale = float(v.abs().max())
-        if scale > 0:
-            e = float((got[k] - v).abs().max()) / scale
-            if e > worst[1]:
-                worst = (k, e)
-    return (num / den) ** 0.5, worst
 
 
 SPECS = {
