@@ -473,7 +473,7 @@ int mn_debug_tp_program_mode(const mn_model_desc* desc, int mode, unsigned int* 
 
 /* ---- test hook (host only, no CUDA call): where the tensor-core training passes keep their intermediates -----------------
  * For a call of mn_model_forward_train_tc / mn_model_backward_tc over B rows of model m, out[] receives (indices MN_TCL_*):
- * the engine (0 not trained on the tensor cores, 1 the fused kernel, 2 the layer-GEMM engine); the tile count and byte size of
+ * the engine that runs the network's tensor-core forward (0 none, 1 the fused kernel, 2 the layer-GEMM engine); the tile count and byte size of
  * the tape and the byte offsets of its regions (routing counters, slot_row and slot_w or -1, encoder tiles, activation
  * records, fp32 head blocks); the bytes of one encoder tile and of one activation record; the padded widths of the encoder
  * segments and of the H / G images; the rows of the fp32 head block (sigma pre-activation, rgb, image id) and of the
@@ -481,9 +481,11 @@ int mn_debug_tp_program_mode(const mn_model_desc* desc, int mode, unsigned int* 
  * gradient images (fused engine: one record per tile, laid out as the activation records), the head-gradient blocks, the
  * per-image embedding sums ([n_sub][app_count][emb_k] floats) and the scale S, then emb_k and the tiles the head-gradient
  * blocks cover; on the layer engine the offsets of the dZ_G image and of the two ping-pong gradient images of the last tile
- * group (-1 on the fused engine); then the number of images of a record and, per image (trunk layers, F, G), its byte offset
- * in the record and its columns.  Every tile image is [cols/8][128 rows][8] fp16.  Returns the entries written, or
- * MN_ERR_WORKSPACE when cap is too small.  Used by tests/test_gpu_zzc_train_tc_stages.py. */
+ * group (-1 on the fused engine); the number of images of a record (layers + 2, or the trunk layers alone without
+ * dir_a_encoding); whether tensor-core training covers the network (mn_model_train_tc_supported once packed); then per image
+ * (trunk layers, F, G), its byte offset in the record and its columns.  Every tile image is [cols/8][128 rows][8] fp16.  Returns the entries written, or
+ * MN_ERR_WORKSPACE when cap is too small.  The backward entries only mean something for networks trained on the tensor cores.
+ * Used by tests/test_gpu_zzc_train_tc_stages.py and tests/test_gpu_zzd_infer_tc.py. */
 #define MN_TCL_ENGINE 0
 #define MN_TCL_N_TILES 1
 #define MN_TCL_TAPE_BYTES 2
@@ -517,8 +519,19 @@ int mn_debug_tp_program_mode(const mn_model_desc* desc, int mode, unsigned int* 
 #define MN_TCL_BWD_PP0 30
 #define MN_TCL_BWD_PP1 31
 #define MN_TCL_N_IMG 32
-#define MN_TCL_IMG 33
+#define MN_TCL_TRAIN 33
+#define MN_TCL_IMG 34
 int mn_debug_tc_train_layout(const mn_model* m, int64_t B, int64_t* out, int cap);
+
+/* ---- test hook: the recording forward of any network the tensor cores run --------------------------------------------
+ * mn_model_forward_train_tc's forward (arguments and tape as there, laid out as mn_debug_tc_train_layout reports) for every
+ * network whose tc_f16 inference runs on the tensor cores, including the shapes tensor-core training does not cover (64..192
+ * wide, affine appearance, no direction / appearance head).  Same plan, packed weights, encoder, GEMM order and epilogue
+ * arithmetic as the tc_f16 inference call, so out_d equals that call's output; the tape holds what the forward computed on the
+ * way.  Allocates no backward images.  MN_ERR_UNSUPPORTED for networks only the fp32 kernels run.  Used by
+ * tests/test_gpu_zzd_infer_tc.py. */
+int mn_debug_tc_forward_record(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, const float* sigma_noise_d,
+                               float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

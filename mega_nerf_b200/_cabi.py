@@ -122,6 +122,7 @@ SIGNATURES = {
     'mn_model_backward_workspace_bytes_tc': (_Z, [_P, _L]),
     'mn_model_backward_tc': (_I, [_P, _P, _L, _I, _P, _P, _Z, _P, _P, _Z, _P]),
     'mn_debug_tc_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),
+    'mn_debug_tc_forward_record': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _P, _P, _P, _Z, _P, _Z, _P]),
 }
 MN_PARAM_OFFSETS = 44
 # entries of mn_debug_tc_train_layout (MN_TCL_* in include/mn_b200.h), then 2 per record image from TCL['IMG'] on
@@ -129,7 +130,7 @@ TCL = {k: i for i, k in enumerate((
     'ENGINE', 'N_TILES', 'TAPE_BYTES', 'TAPE_COUNTERS', 'TAPE_SLOT_ROW', 'TAPE_SLOT_W', 'TAPE_XREG', 'TAPE_ACT', 'TAPE_F32',
     'X_TILE', 'ACT_TILE', 'KPE', 'KAUX', 'HC', 'GC', 'F32_SIGMA', 'F32_RGB', 'F32_ID', 'F32_ROWS', 'G32_SIGMA', 'G32_RGB',
     'G32_ROWS', 'BWD_BYTES', 'BWD_DZ', 'BWD_GF32', 'BWD_EMB', 'BWD_SCALE', 'BWD_EMB_K', 'BWD_HEAD_TILES', 'BWD_DZG',
-    'BWD_PP0', 'BWD_PP1', 'N_IMG', 'IMG'))}
+    'BWD_PP0', 'BWD_PP1', 'N_IMG', 'TRAIN', 'IMG'))}
 
 _lib = None
 _lock = threading.Lock()

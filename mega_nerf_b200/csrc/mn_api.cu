@@ -450,7 +450,8 @@ static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, Ta
     return tape_regions_cap(m, slot_capacity(m, B), m->d.boundary_margin > 1.0f, tc, base, r);
 }
 
-// train_tc != 0: recording forward on the tensor cores (precision tc_f16) into the tensor-core tape regions.
+// train_tc != 0: recording forward on the tensor cores (precision tc_f16) into the tensor-core tape regions; 2: the test hook's
+// recording forward (mn_debug_tc_forward_record), which also runs networks that tensor-core training does not cover.
 // live: the rows that hold data when their count lives on the device (inference only), see LiveRows.
 // mult: sub-modules per row the routing slots of this call are sized for (inference only; 0 = the model's max_multiplicity).
 static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, int sigma_only,
@@ -565,7 +566,8 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
 
     const int64_t n_tiles = cap / MN_TILE;
     if (tape_d && train_tc) {
-        if ((rc = mn_mlp_tc_launch_train(ctx, m, a, n_tiles, T.tc, st))) return rc;
+        rc = train_tc == 2 ? mn_mlp_tc_launch_record(ctx, m, a, n_tiles, T.tc, st) : mn_mlp_tc_launch_train(ctx, m, a, n_tiles, T.tc, st);
+        if (rc) return rc;
         if (row_slots) return mn_route_combine(ctx, m, B, live, row_slots, slot_out, a.out_cols, out_d, st);
         return MN_OK;
     }
@@ -841,6 +843,13 @@ int mn_model_forward_train_tc(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
     if (!m || !m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
     return model_forward_impl(ctx, m, rows, B, use_coarse, 0, sigma_noise_d, MN_PREC_FP32, out_d, workspace_d, workspace_bytes, tape_d,
                               tape_bytes, stream, 1);
+}
+
+int mn_debug_tc_forward_record(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, const float* sigma_noise_d,
+                               float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes, void* stream) {
+    if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_debug_tc_forward_record: tape is NULL");
+    return model_forward_impl(ctx, m, rows, B, use_coarse, 0, sigma_noise_d, MN_PREC_FP32, out_d, workspace_d, workspace_bytes, tape_d,
+                              tape_bytes, stream, 2);
 }
 
 size_t mn_model_backward_workspace_bytes_tc(const mn_model* m, int64_t B) {

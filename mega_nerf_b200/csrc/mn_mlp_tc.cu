@@ -862,9 +862,9 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet&
         H.g_lo = split ? buf[B.rgb_src].lo : 0;
         H.L = B.sigma_k;
         H.rgb_in = B.rgb_k;
-        if (tape) {
+        if (tape) {      // without dir_a_encoding the rgb head reads the last trunk image, as it reads B.rgb_src above
             H.h = rec + mn_tc_img_off(a.nd.layers - 1, hc);
-            H.g = rec + mn_tc_img_off(a.nd.layers + 1, hc);
+            H.g = rec + mn_tc_img_off(a.nd.has_dir_a ? a.nd.layers + 1 : a.nd.layers - 1, hc);
             H.h_tile_bytes = H.g_tile_bytes = act_tile;
             H.tape_f32 = tape->f32;
         }
@@ -921,13 +921,9 @@ size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
     return mn_tc_img_off(m->nd.layers + 1, net.lin.hc) + mn_tc_img_off(1, net.lin.gc);     // ends with G (L/2 columns, padded)
 }
 
-// recording forward: encoder tiles and every layer's activations land in the caller's tape
-int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
-    if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
-    if (n_tiles128 <= 0) return MN_OK;
-    const TcNet net = tc_net(*m);
-    int rc = tc_dgrad_ready(ctx, m, net, st);
-    if (rc) return rc;
+// recording forward of either engine: encoder tiles and every layer's activations land in the caller's tape
+static int tc_record_forward(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet& net, int64_t n_tiles128, const TrainTcTape& tape,
+                             cudaStream_t st) {
     if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net, n_tiles128, MN_PREC_TC_F16, nullptr, 0, st, &tape);
     TcArgs A = tc_forward_args(m, net.P, a, n_tiles128);
     A.ximg = reinterpret_cast<const __half*>(tape.xreg);
@@ -936,13 +932,31 @@ int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n
     A.tape_f32 = tape.f32;
     A.act_tile_bytes = (int64_t)mn_train_tc_act_tile_bytes(m);
     A.layers = a.nd.layers;
-    rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st);
+    int rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st);
     if (rc) return rc;
     mn_prof_begin(ctx, st);
     if (A.plan.L > 256) rc = wg_launch<PP_TRAIN_FWD, false, true>(ctx, A, n_tiles128, st);
     else rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
     mn_prof_end(ctx, st);
     return rc;
+}
+
+int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
+    if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
+    if (n_tiles128 <= 0) return MN_OK;
+    const TcNet net = tc_net(*m);
+    const int rc = tc_dgrad_ready(ctx, m, net, st);
+    if (rc) return rc;
+    return tc_record_forward(ctx, m, a, net, n_tiles128, tape, st);
+}
+
+// Test hook (mn_debug_tc_forward_record): the same recording forward for every network the tensor cores serve, trained there or
+// not.  It needs no transposed images, so none are allocated.
+int mn_mlp_tc_launch_record(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
+    const TcNet net = tc_net(*m);
+    if (net.engine == TC_NONE || !m->tc_ready) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_debug_tc_forward_record: the network has no tensor-core forward");
+    if (n_tiles128 <= 0) return MN_OK;
+    return tc_record_forward(ctx, m, a, net, n_tiles128, tape, st);
 }
 
 // backward workspace: [gradient images][head gradients fp32 [head_tiles][mn_tc_g32_rows(rgb_dim)][128]][embedding sums][scale,
@@ -982,9 +996,10 @@ size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
 int mn_train_tc_layout(const mn_model* m, int64_t n_tiles128, int64_t* out, int cap) {
     const TcNet net = tc_net(*m);
     const NetDims& nd = m->nd;
-    const int n_img = nd.layers + 2;
+    const int n_img = nd.has_dir_a ? nd.layers + 2 : nd.layers;      // without dir_a_encoding the record holds the trunk only
     if (cap < MN_TCL_IMG + 2 * n_img) return MN_ERR_WORKSPACE;
-    out[MN_TCL_ENGINE] = net.train ? net.engine : TC_NONE;
+    out[MN_TCL_ENGINE] = net.engine;
+    out[MN_TCL_TRAIN] = net.train ? 1 : 0;
     out[MN_TCL_X_TILE] = net.P.x_tile_bytes;
     out[MN_TCL_ACT_TILE] = (int64_t)mn_train_tc_act_tile_bytes(m);
     out[MN_TCL_KPE] = net.lin.kpe;

@@ -7,6 +7,11 @@ Two users:
                      blocks, head-gradient blocks, dZ images, embedding sums), so no bound propagates through depth: each
                      stage is one rounding step away from its inputs.  tests/test_gpu_zzc_train_tc_stages.py feeds it what the
                      GPU wrote; tests/test_tc_train_ref.py an fp32 emulation, with and without injected bugs.
+  check_forward      its forward half alone (check_backward the rest), for every network with a tensor-core forward: also
+                     the 64..192-wide fused plans, the affine colour head and the rgb head that reads the trunk directly.
+  check_output       output assembly: `out` from the head block and the head input image (slot_outputs), through the blend
+                     weight and combine_kernel's sum.  tests/test_gpu_zzd_infer_tc.py feeds both the recording forward of a
+                     tc_f16 inference call (mn_debug_tc_forward_record), whose `out` equals that call's bit for bit.
 
 Rounding points, as the kernels implement them:
   encoder     tc_encode_kernel / tc_encode_fast_kernel (mn_mlp_tc.cu): x, sin(2^k x), cos(2^k x) in fp32 (sincosf, or the
@@ -18,8 +23,11 @@ Rounding points, as the kernels implement them:
               rounded (mn_mlp_wg.cuh, sacc_a / sacc_b); those values are not on the tape, so beta adds sum |w_sigma| half-ulp16(h).
               Layer engine: tc_layer_head_kernel sums the fp16 tape image times fp32 sigma_w (mn_layer_gemm.cuh).  Then
               + sigma_b + noise, stored as the fp32 pre-activation.
-  rgb         fused engine: an MMA, fp16 G times fp16 W_rgb; layer engine: fp16 G times fp32 W_rgb on CUDA cores.  Colour
-              heads store sigmoid(pre) in the fp32 head block.
+  rgb         fused engine: an MMA, fp16 G times fp16 W_rgb; layer engine: fp16 G times fp32 W_rgb on CUDA cores (the last
+              trunk image instead of G without dir_a_encoding).  Colour heads store sigmoid(pre) in the fp32 head block; the
+              affine head (tc_emit_rgb) transforms pre by affine(embedding_a[id]) first and stores only to `out`.
+  out         tc_emit_rgb / the sigma epilogue: x (rgb) and sigma_activation(pre) (mn_softplus_shifted or fmaxf), times the
+              slot's blend weight when blending; combine_kernel sums a row's slots in fp32, ascending sub-module order.
   backward    S = 2^(10 - ceil(log2 max|grad_out|)) (tc_grad_scale_kernel).  Head stage in fp32 (tc_head_grad): d = (g w (1 -
               c)) c for colour, g w for SH; dsigma = g_sigma w ReLU'(pre) or softplus'(pre - 1).  dZ_G = mask(G > 0)
               (sum_c W_rgb[c] d[c]) in fp32 (tc_rgb_dgrad8), times S, fp16.  Data-gradient GEMMs: fp16 dZ times fp16 W, fp32
@@ -325,10 +333,29 @@ def check_stages(spec: O.NerfSpec, w, cap, fused: bool, rep: Report, tag=''):
       sig [n], rgb [n, 3], id [n], S, gf32 [n, 1 + rgb_dim], dz {j: [n, cols]} (dZ images present), emb_sum
       [app_count, emb_k] or None, grads {state-dict key: tensor}, and optional `seed_grads` {key: (v, tol)} for tensors whose
       dZ is not resident (compared at a per-tensor tolerance instead)."""
+    check_forward(spec, w, cap, fused, rep, tag)
+    check_backward(spec, w, cap, fused, rep, tag)
+
+
+def app_in_dira(spec: O.NerfSpec) -> bool:
+    """The appearance embedding is an input of dir_a_encoding (not the affine colour transform)."""
+    return spec.appearance_dim > 0 and not spec.affine_appearance
+
+
+def head_input(spec: O.NerfSpec, img):
+    """The fp16 image the rgb head reads: G, or the last trunk image without dir_a_encoding (nerf.py:154)."""
+    L, layers = spec.layer_dim, spec.layers
+    return img[layers + 1][:, :L // 2] if spec.has_dir_a else img[layers - 1][:, :L]
+
+
+def check_forward(spec: O.NerfSpec, w, cap, fused: bool, rep: Report, tag=''):
+    """The recording forward of one sub-module's slots: encoder tiles, every activation image from the kernel's previous one, and
+    the fp32 head block (sigma pre-activation; the colour / first 3 SH channels unless the rgb goes through the affine transform,
+    which only `out` holds: check_output).  cap holds the forward entries of check_stages; without dir_a_encoding img has the
+    trunk images only."""
     L, layers, in_xyz, R = spec.layer_dim, spec.layers, spec.in_xyz, spec.rgb_dim
     half = L // 2
     val = cap['valid']
-    S = cap['S']
     img = cap['img']
     p = f'{tag}' if tag else ''
     # ---- encoder tiles
@@ -342,45 +369,66 @@ def check_stages(spec: O.NerfSpec, w, cap, fused: bool, rep: Report, tag=''):
         v, b = pe_features(x[:, -4:-1], spec.pos_dir_dim)
         rep.img(p + 'encoder dir PE', cap['xaux'][val][:, :spec.in_dir], v, b)
         col = spec.in_dir
-    ids = None
-    if spec.appearance_dim > 0:
-        ids = x[:, -1].long()
+    ids = x[:, -1].long() if spec.appearance_dim > 0 else None
+    n_aux = col
+    if app_in_dira(spec):
         e = w['embedding_a.weight'][ids].double()
         rep.img(p + 'encoder embedding', cap['xaux'][val][:, col:col + spec.appearance_dim], e, torch.zeros_like(e))
+        n_aux += spec.appearance_dim
+    if cap['xaux'].shape[1] > n_aux:
+        rep.exact(p + 'encoder aux padding', cap['xaux'][:, n_aux:], torch.zeros_like(cap['xaux'][:, n_aux:]))
     rep.exact(p + 'encoder padding rows', cap['xpe'][~val], torch.zeros_like(cap['xpe'][~val]))
 
     # ---- forward images, each from the kernel's previous image
     pe16 = cap['xpe'][:, :in_xyz]
-    xin = []
     for i in range(layers):
         prev = pe16 if i == 0 else img[i - 1][:, :L]
         X = torch.cat([pe16, prev], -1) if (i in spec.skip_layers and i > 0) else prev
-        xin.append(X)
         v, b = linear_fwd(X, w[f'xyz_encodings.{i}.0.weight'], w[f'xyz_encodings.{i}.0.bias'])
         rep.img(p + f'fwd H{i}', img[i][:, :L], v, b, relu)
     H = img[layers - 1][:, :L]
-    v, b = linear_fwd(H, w['xyz_encoding_final.weight'], w['xyz_encoding_final.bias'])
-    rep.img(p + 'fwd F', img[layers][:, :L], v, b)
-    aux16 = cap['xaux'][:, :spec.in_dir + spec.appearance_dim]
-    FX = torch.cat([img[layers][:, :L], aux16], -1)
-    v, b = linear_fwd(FX, w['dir_a_encoding.0.weight'], w['dir_a_encoding.0.bias'])
-    rep.img(p + 'fwd G', img[layers + 1][:, :half], v, b, relu)
-    for j in range(layers + 2):                    # the layer engine's padding columns hold exactly 0
+    if spec.has_dir_a:
+        v, b = linear_fwd(H, w['xyz_encoding_final.weight'], w['xyz_encoding_final.bias'])
+        rep.img(p + 'fwd F', img[layers][:, :L], v, b)
+        aux16 = cap['xaux'][:, :n_aux]
+        FX = torch.cat([img[layers][:, :L], aux16], -1)
+        v, b = linear_fwd(FX, w['dir_a_encoding.0.weight'], w['dir_a_encoding.0.bias'])
+        rep.img(p + 'fwd G', img[layers + 1][:, :half], v, b, relu)
+    for j in range(len(img)):                      # the layer engine's padding columns hold exactly 0
         if img[j].shape[1] > (half if j == layers + 1 else L):
             pad = img[j][:, half if j == layers + 1 else L:]
             rep.exact(p + f'fwd image {j} padding', pad, torch.zeros_like(pad))
-    G16 = img[layers + 1][:, :half]
     noise = cap['noise'].double()
     v, b = sigma_pre(H[val], w['sigma.weight'], w['sigma.bias'], noise[val], fused)
     rep.f32(p + 'head sigma pre-activation', cap['sig'][val], v, b)
-    v, b = rgb_head(G16[val], w['rgb.weight'], w['rgb.bias'], fused)
-    if R == 3:
-        c = torch.sigmoid(v)
-        rep.f32(p + 'head rgb', cap['rgb'][val], c, 0.25 * b + 4 * U32)
-    else:
-        rep.f32(p + 'head rgb', cap['rgb'][val], v[:, :3], b[:, :3])
+    if not spec.affine_appearance:
+        v, b = rgb_head(head_input(spec, img)[val], w['rgb.weight'], w['rgb.bias'], fused)
+        if R == 3:
+            c = torch.sigmoid(v)
+            rep.f32(p + 'head rgb', cap['rgb'][val], c, 0.25 * b + 4 * U32)
+        else:
+            rep.f32(p + 'head rgb', cap['rgb'][val], v[:, :3], b[:, :3])
     if ids is not None:
         rep.exact(p + 'head image id', cap['id'][val], x[:, -1].double())
+
+
+def check_backward(spec: O.NerfSpec, w, cap, fused: bool, rep: Report, tag=''):
+    """The backward of one sub-module's slots (check_stages), seeded from the kernels' forward tape and head-gradient blocks."""
+    L, layers, in_xyz, R = spec.layer_dim, spec.layers, spec.in_xyz, spec.rgb_dim
+    half = L // 2
+    val = cap['valid']
+    S = cap['S']
+    img = cap['img']
+    p = f'{tag}' if tag else ''
+    x = cap['x'][val]
+    ids = x[:, -1].long() if spec.appearance_dim > 0 else None
+    H = img[layers - 1][:, :L]
+    G16 = img[layers + 1][:, :half]
+    aux16 = cap['xaux'][:, :spec.in_dir + spec.appearance_dim]
+    FX = torch.cat([img[layers][:, :L], aux16], -1)
+    pe16 = cap['xpe'][:, :in_xyz]
+    xin = [torch.cat([pe16, img[i - 1][:, :L]], -1) if (i in spec.skip_layers and i > 0) else (pe16 if i == 0 else img[i - 1][:, :L])
+           for i in range(layers)]
 
     # ---- backward head stage
     d, bd, ds, bds = head_grads(spec, cap['go'], cap['bw'], cap['rgb'], cap['sig'])
@@ -458,6 +506,89 @@ def check_stages(spec: O.NerfSpec, w, cap, fused: bool, rep: Report, tag=''):
         unused[idv[val]] = False
         rep.exact(p + 'grad embedding_a.weight unused ids', grads['embedding_a.weight'][unused],
                   torch.zeros_like(grads['embedding_a.weight'][unused]))
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# output assembly: what a call writes to `out` (tc_emit_rgb and the sigma epilogue of either engine, then combine_kernel)
+# ------------------------------------------------------------------------------------------------------------------------
+def sigma_act(spec: O.NerfSpec, pre):
+    """sigma_activation of the kernel's fp32 pre-activation, (v, beta).  ReLU (fmaxf) is exact.  mn_softplus_shifted rounds
+    y = pre - 1 (U32 |y|), then log1pf(expf(y)): expf within 2 ulps (4 U32 of e^y, which moves softplus by 4 U32 sigmoid(y))
+    and log1pf within 1 ulp (2 U32 softplus(y)); beta is twice their sum.  Above y = 20 it returns y, 2e-9 from softplus(y)."""
+    pre = pre.double()
+    if not spec.shifted_softplus:
+        return pre.clamp(min=0), torch.zeros_like(pre)
+    y = pre - 1
+    v = torch.logaddexp(y, torch.zeros_like(y))
+    sg = torch.sigmoid(y)
+    return v, 2 * (sg * (U32 * y.abs() + 4 * U32) + 2 * U32 * v)
+
+
+def rgb_out(spec: O.NerfSpec, w, src16, ids, fused: bool):
+    """The rgb columns of one slot's output from the head's input image, (v [n, rgb_dim], beta): the rgb Linear (rgb_head), then
+    tc_emit_rgb - the affine transform T = affine(embedding_a[id]) (fp32 fmaf chains over the embedding), y_c = sum_k T[c][k]
+    r_k + T[c][3] (three roundings), and the sigmoid of a colour head (1 / (1 + expf(-y)): 2 ulps of expf, one add and one
+    divide, 8 U32 of the value; the slope of the sigmoid is at most 1/4)."""
+    v, b = rgb_head(src16, w['rgb.weight'], w['rgb.bias'], fused)
+    if spec.affine_appearance and spec.appearance_dim > 0:
+        e = w['embedding_a.weight'].double()[ids]
+        A, ab = w['affine.weight'].double(), w['affine.bias'].double()
+        T = (e @ A.t() + ab).view(-1, 3, 4)
+        bT = dot_beta(e, A.t(), e.shape[1], ab.abs()).view(-1, 3, 4)
+        prod = T[:, :, :3] * v.unsqueeze(1)
+        y = prod.sum(-1) + T[:, :, 3]
+        by = ((T[:, :, :3].abs() + bT[:, :, :3]) * b.unsqueeze(1) + v.abs().unsqueeze(1) * bT[:, :, :3]).sum(-1) + bT[:, :, 3] \
+            + 4 * U32 * (prod.abs().sum(-1) + T[:, :, 3].abs())
+        v, b = y, by
+    if spec.rgb_dim == 3:
+        c = torch.sigmoid(v)
+        return c, 0.25 * b + 8 * U32 * c
+    return v, b
+
+
+def slot_outputs(spec: O.NerfSpec, w, cap, fused: bool):
+    """Per valid slot of one sub-module, before the blend weight: v / beta [n, rgb_dim + 1] restated from the kernel's head input
+    image and fp32 sigma pre-activation, and `exact` the colour (or first 3 SH channels) of the fp32 head block, which the
+    kernel stores to `out` unchanged (None for the affine head, which the head block does not hold)."""
+    val = cap['valid']
+    ids = cap['x'][val][:, -1].long() if spec.appearance_dim > 0 else None
+    vr, br = rgb_out(spec, w, head_input(spec, cap['img'])[val], ids, fused)
+    vs, bs = sigma_act(spec, cap['sig'][val])
+    exact = None if spec.affine_appearance else cap['rgb'][val][:, :min(spec.rgb_dim, 3)]
+    return dict(v=torch.cat([vr, vs.view(-1, 1)], 1), beta=torch.cat([br, bs.view(-1, 1)], 1), exact=exact)
+
+
+def check_output(spec: O.NerfSpec, out, pieces, rep: Report, tag=''):
+    """out [n, rgb_dim + 1]: the call's output for n rows.  pieces: per sub-module in ascending order, (rows [k] indices into out,
+    bw [k] fp32 blend weights or None, slot_outputs of those slots).  A blended call stores x * w per slot (one fp32 rounding)
+    and combine_kernel sums a row's slots from 0 in ascending sub-module order; an unblended one stores x.  The head block's
+    colour then gives `out` bit for bit (float32 arithmetic here in the kernel's order); every column is within the sum of the
+    slots' betas, their products' and the sum's roundings (k U32 sum |x w| for k slots) of the float64 restatement."""
+    p = f'{tag}' if tag else ''
+    n, C = out.shape
+    m = min(spec.rgb_dim, 3)
+    v = torch.zeros(n, C, dtype=torch.float64)
+    b = torch.zeros_like(v)
+    mag = torch.zeros_like(v)
+    cnt = torch.zeros(n, 1, dtype=torch.float64)
+    acc = torch.zeros(n, m, dtype=torch.float32)
+    exact = all(so['exact'] is not None for _, _, so in pieces)
+    for rows, bw, so in pieces:
+        wv = torch.ones(len(rows), 1, dtype=torch.float64) if bw is None else bw.double().view(-1, 1)
+        val = so['v'] * wv
+        v.index_add_(0, rows, val)
+        b.index_add_(0, rows, so['beta'] * wv + (0.0 if bw is None else U32 * val.abs()))
+        mag.index_add_(0, rows, val.abs())
+        cnt.index_add_(0, rows, torch.ones(len(rows), 1, dtype=torch.float64))
+        if exact:
+            x32 = so['exact'].float()
+            acc[rows] = acc[rows] + (x32 if bw is None else x32 * bw.float().view(-1, 1))
+    b = b + cnt * U32 * mag
+    out = out.double()
+    rep.f32(p + 'out rgb', out[:, :C - 1], v[:, :C - 1], b[:, :C - 1])
+    rep.f32(p + 'out sigma', out[:, C - 1], v[:, C - 1], b[:, C - 1])
+    if exact:
+        rep.exact(p + 'out rgb = head block (bitwise)', out[:, :m], acc.double())
 
 
 def seeded_chain(spec: O.NerfSpec, w, cap, S):

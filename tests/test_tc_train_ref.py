@@ -2,7 +2,9 @@
 
 An fp32 emulation of the kernels (fp16 operands and images, fp32 accumulation in torch's summation order, which differs from
 the float64 reference's) must pass every stage check at the shapes tests/test_gpu_zzc_train_tc_stages.py uses; each injected
-bug must fail at least one stage; and without rounding the restatement is float64 autograd of the oracle's forward."""
+bug must fail at least one stage; and without rounding the restatement is float64 autograd of the oracle's forward.  The same for
+the forward stages and the output assembly alone (check_forward, check_output) at every shape tests/test_gpu_zzd_infer_tc.py
+records, including the networks only tc_f16 inference runs."""
 import pytest
 import torch
 
@@ -195,3 +197,183 @@ def test_half_ulp16():
     for v, want in ((1.0, 2.0 ** -11), (1.5, 2.0 ** -11), (2.0, 2.0 ** -10), (2.0 ** -14, 2.0 ** -25), (0.0, 2.0 ** -25),
                     (1e-6, 2.0 ** -25)):
         assert float(T.half_ulp16(torch.tensor([v]))) == want, v
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# the recording forward of every tensor-core network (tests/test_gpu_zzd_infer_tc.py) and its output assembly
+# ------------------------------------------------------------------------------------------------------------------------
+def emulate_forward(spec, w, x, noise, fused, bug=None):
+    """The forward half of a capture for one sub-module's rows, and y [n, rgb_dim + 1]: the row's output before any blend
+    weight, all in fp32 with fp16 rounding where the kernels round."""
+    L, layers, in_xyz, R = spec.layer_dim, spec.layers, spec.in_xyz, spec.rgb_dim
+    h = lambda t: T.h16(t.float())                                                    # noqa: E731
+    wf = {k: v.float() for k, v in w.items()}
+    n = x.shape[0]
+    pe = h(T.pe_band_fp32(x[:, :spec.xyz_dim], spec.pos_xyz_dim))
+    aux = []
+    if spec.pos_dir_dim > 0:
+        aux.append(T.pe_band_fp32(x[:, -4:-1], spec.pos_dir_dim))
+    ids = x[:, -1].long() if spec.appearance_dim > 0 else None
+    if T.app_in_dira(spec):
+        aux.append(wf['embedding_a.weight'][ids])
+    aux = h(torch.cat(aux, -1)) if aux else torch.zeros(n, 0)
+    img, cur, last32 = [], pe, None
+    for i in range(layers):
+        inp = torch.cat([pe, cur], -1) if (i in spec.skip_layers and i > 0) else cur
+        last32 = torch.relu(inp @ h(wf[f'xyz_encodings.{i}.0.weight']).t() + wf[f'xyz_encodings.{i}.0.bias'])
+        cur = h(last32)
+        img.append(cur)
+    H32 = last32 if fused else img[-1]
+    sig = (H32 @ wf['sigma.weight'].t())[:, 0] + wf['sigma.bias'] + noise.float().view(-1)
+    if spec.has_dir_a:
+        F_ = h(img[-1] @ h(wf['xyz_encoding_final.weight']).t() + wf['xyz_encoding_final.bias'])
+        G16 = h(torch.relu(torch.cat([F_, aux], -1) @ h(wf['dir_a_encoding.0.weight']).t() + wf['dir_a_encoding.0.bias']))
+        img += [F_, G16]
+        src = G16
+    else:             # the rgb head reads the last trunk image; the bug reads the (empty) G image of the record instead
+        src = torch.zeros_like(img[-1]) if bug == 'head_reads_g' else img[-1]
+    Wr = h(wf['rgb.weight']) if fused else wf['rgb.weight']
+    lin = src @ Wr.t() + wf['rgb.bias']
+    if spec.affine_appearance:
+        Tm = (wf['embedding_a.weight'][ids] @ wf['affine.weight'].t() + wf['affine.bias']).view(-1, 3, 4)
+        M3 = Tm[:, :, :3].transpose(1, 2) if bug == 'affine_transposed' else Tm[:, :, :3]
+        lin = (M3 @ lin.unsqueeze(-1)).squeeze(-1) + Tm[:, :, 3]
+    rgb = torch.sigmoid(lin) if R == 3 else lin
+    if spec.shifted_softplus:
+        sg = torch.nn.functional.softplus(sig if bug == 'softplus_unshifted' else sig - 1)
+    else:
+        sg = torch.relu(sig)
+    kpe = (in_xyz + 15) // 16 * 16
+    kaux = (aux.shape[1] + 15) // 16 * 16
+    xpe, xaux = torch.zeros(n, kpe), torch.zeros(n, kaux)
+    xpe[:, :in_xyz] = pe
+    xaux[:, :aux.shape[1]] = aux
+    tape_rgb = torch.zeros(n, 3) if spec.affine_appearance else rgb[:, :3]
+    d64 = lambda t: t.double()                                                        # noqa: E731
+    return dict(valid=torch.ones(n, dtype=torch.bool), x=d64(x), noise=d64(noise).view(-1), xpe=d64(xpe), xaux=d64(xaux),
+                img=[d64(t) for t in img], sig=d64(sig), rgb=d64(tape_rgb),
+                id=d64(x[:, -1]) if ids is not None else torch.zeros(n, dtype=torch.float64), y=torch.cat([rgb, sg.view(-1, 1)], 1))
+
+
+_G = dict(layer_dim=64, appearance_count=10)
+INFER_SPECS = {          # name: (spec, fused engine)
+    'fused64': (O.NerfSpec(**_G), True),
+    'fg128_l4': (O.NerfSpec(layer_dim=128, layers=4, skip_layers=(2,)), True),
+    'fused192': (O.NerfSpec(layer_dim=192), True),
+    'fused256_app': (O.NerfSpec(), True),
+    'fused256_d12_sh2': (O.NerfSpec(layers=12, pos_dir_dim=0, rgb_dim=27), True),
+    'affine': (O.NerfSpec(affine_appearance=True), True),
+    'affine64': (O.NerfSpec(affine_appearance=True, **_G), True),
+    'nodir_noapp': (O.NerfSpec(pos_dir_dim=0, appearance_dim=0), True),
+    'nodir_noapp128': (O.NerfSpec(pos_dir_dim=0, appearance_dim=0, layer_dim=128), True),
+    'noapp_q1': (O.NerfSpec(appearance_dim=0), True),
+    'relu_sigma': (O.NerfSpec(shifted_softplus=False), True),
+    'bg256': (O.NerfSpec(xyz_dim=4), True),
+    'sh2': (O.NerfSpec(pos_dir_dim=0, rgb_dim=27), True),
+    'fused512': (O.NerfSpec(layer_dim=512), True),
+    'layer96': (O.NerfSpec(layer_dim=96), False),
+    'layer160_nodir': (O.NerfSpec(layer_dim=160, pos_dir_dim=0, appearance_dim=0), False),
+    'layer384': (O.NerfSpec(layer_dim=384, appearance_dim=0), False),
+    'layer768': (O.NerfSpec(layer_dim=768, appearance_dim=0), False),
+    'layer2048_sh4': (O.NerfSpec(layer_dim=2048, pos_dir_dim=0, rgb_dim=75), False),
+}
+
+
+def forward_case(spec, n=300, seed=21):
+    net = O.make_net('nerf', spec, seed=seed)
+    if not spec.shifted_softplus:
+        net.weights[0]['sigma.bias'] = net.weights[0]['sigma.bias'] + 0.5
+    x = C.nerf_rows(spec, n, 31)
+    noise = torch.randn(n, 1, generator=torch.Generator().manual_seed(5))
+    return net.weights[0], x, noise
+
+
+def forward_report(spec, w, cap, fused):
+    rep = T.Report()
+    wd = {k: v.double() for k, v in w.items()}
+    with torch.no_grad():
+        T.check_forward(spec, wd, cap, fused, rep)
+        T.check_output(spec, cap['y'], [(torch.arange(cap['y'].shape[0]), None, T.slot_outputs(spec, wd, cap, fused))], rep)
+    return rep
+
+
+@pytest.mark.parametrize('vname', list(INFER_SPECS))
+def test_forward_emulation_within_bounds(vname):
+    spec, fused = INFER_SPECS[vname]
+    w, x, noise = forward_case(spec, n=128 if spec.layer_dim >= 2048 else 300)
+    with torch.no_grad():
+        cap = emulate_forward(spec, w, x, noise, fused)
+    rep = forward_report(spec, w, cap, fused)
+    print(f'\n{vname}\n{rep.text()}')
+    assert not rep.failures(), rep.failures()
+    assert any(r['stage'] == 'out rgb' and r['n'] > 0 for r in rep.rows)
+
+
+def routed_report(net, x, noise, bug=None):
+    """A MegaNeRF call emulated per sub-module (ascending, or descending under the bug) with fp32 blending, then checked."""
+    assign, wts = O.route(net, x)
+    K, R = len(net.weights), net.spec.rgb_dim
+    out = torch.zeros(x.shape[0], R + 1)
+    per = {}
+    with torch.no_grad():
+        for s in range(K):
+            rows = ((assign == s) if wts is None else (wts[:, s] > 0)).nonzero().view(-1)
+            if len(rows):
+                bw = wts[rows, s].float() if wts is not None else None
+                per[s] = (rows, bw, emulate_forward(net.spec, net.weights[s], x[rows], noise[rows], True))
+        for s in (sorted(per, reverse=True) if bug == 'combine_descending' else sorted(per)):
+            rows, bw, cap = per[s]
+            y = cap['y']
+            if bw is not None:
+                y = y * bw.view(-1, 1)
+                if bug == 'slot_w_twice':
+                    y = y * bw.view(-1, 1)
+                out[rows] = out[rows] + y
+            else:
+                out[rows] = y
+        rep = T.Report()
+        pieces = []
+        for s in sorted(per):
+            rows, bw, cap = per[s]
+            wd = {k: v.double() for k, v in net.weights[s].items()}
+            T.check_forward(net.spec, wd, cap, True, rep, tag=f'[{s}] ')
+            pieces.append((rows, bw, T.slot_outputs(net.spec, wd, cap, True)))
+        T.check_output(net.spec, out, pieces, rep)
+    return rep
+
+
+@pytest.mark.parametrize('mname', ['hard2d', 'blend2d'])
+def test_routed_emulation_within_bounds(mname):
+    net = C.mega_net(mname)
+    x = C.mega_rows(net, 1500, 13)
+    noise = torch.rand(x.shape[0], 1, generator=torch.Generator().manual_seed(6))
+    rep = routed_report(net, x, noise)
+    print(f'\n{mname}\n{rep.text()}')
+    assert not rep.failures(), rep.failures()
+
+
+FWD_BUGS = {      # bug: the network it is injected into
+    'affine_transposed': 'affine64',
+    'slot_w_twice': 'blend2d',
+    'combine_descending': 'blend2d',
+    'softplus_unshifted': 'fused64',
+    'head_reads_g': 'nodir_noapp128',
+}
+
+
+@pytest.mark.parametrize('bug', list(FWD_BUGS))
+def test_each_forward_mutation_leaves_the_bounds(bug):
+    where = FWD_BUGS[bug]
+    if where in INFER_SPECS:
+        spec, fused = INFER_SPECS[where]
+        w, x, noise = forward_case(spec)
+        with torch.no_grad():
+            cap = emulate_forward(spec, w, x, noise, fused, bug)
+        rep = forward_report(spec, w, cap, fused)
+    else:
+        net = C.mega_net(where)
+        x = C.mega_rows(net, 1500, 13)
+        rep = routed_report(net, x, torch.rand(x.shape[0], 1, generator=torch.Generator().manual_seed(6)), bug)
+    fails = rep.failures()
+    print(bug, [(r['stage'], r['fail']) for r in fails])
+    assert fails, bug
