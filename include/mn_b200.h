@@ -364,6 +364,42 @@ int mn_render_rays_bg(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays
                       const float* u_fine_bg_d, int fine_samples, int use_cascade, int sh_deg, int precision,
                       const mn_render_outputs* out, void* workspace_d, size_t workspace_bytes, void* stream);
 
+/* ---- the same through an occupancy grid (an approximate render mode the caller opts into) --------------------------------
+ * mn_render_rays / mn_render_rays_bg, except that the foreground samples of both passes (coarse and fine) that lie in a cell the
+ * grid marks empty are not queried: their raw row [rgb, sigma] (after the SH head, for one) is exactly (0, 0, 0, 0), and every
+ * later stage - composite, resampling, merge, background pass, blend - runs unchanged on it.  The background pass is never
+ * masked.  For a sample point x, per axis a: u_a = x_a * scale_a + offset_a (two separately rounded fp32 operations, no FMA),
+ * i_a = (int)floorf(u_a * reso); the sample is skipped iff 0 <= u_a < 1 on all three axes and bit (i_0 * reso + i_1) * reso + i_2
+ * (bit c & 31 of bits[c >> 5]) is 0 - so a point outside the box, or a NaN point, is always queried.  The bit order is the
+ * lattice order of mn_model_density_grid with the same offset / scale (the octree's tree.offset / tree.invradius).  With every
+ * bit set the results equal those of mn_render_rays(_bg).
+ * The queried samples are compacted on the device in ascending order and their count stays there: no host sync, the launch
+ * sequence depends on N only (CUDA-graph capturable).  counts_out_d: NULL, or int32 [2] receiving the queried foreground rows of
+ * the coarse [0] and of the fine [1] pass (the latter written only with fine_samples > 0).  N * max(coarse, fine-query samples)
+ * must stay below 2^31; reso 1 .. MN_OCC_MAX_RESO.  The grid is read during the call only. */
+#define MN_OCC_MAX_RESO 2048
+typedef struct mn_occupancy {
+    const uint32_t* bits;     /* device, ceil(reso^3 / 32) words                     */
+    int reso;
+    float offset[3];
+    float scale[3];
+} mn_occupancy;
+size_t mn_render_rays_occ_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                          int sh_deg, int precision);
+int mn_render_rays_occ(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N,
+                       const float* z_steps_d, int coarse_samples, const float* u_fine_d, int fine_samples, int use_cascade,
+                       int sh_deg, int precision, const mn_occupancy* occ, int32_t* counts_out_d, float* rgb_out_d,
+                       float* depth_out_d, float* depth_var_out_d, float* rgb_coarse_out_d, void* workspace_d,
+                       size_t workspace_bytes, void* stream);
+size_t mn_render_rays_bg_occ_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                             int use_cascade, int sh_deg, int precision);
+int mn_render_rays_bg_occ(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays_d, const float* image_indices_d, int64_t N,
+                          const float* sphere_center3_d, const float* sphere_radius3_d, int include_xyz_real, int cluster_2d,
+                          const float* z_steps_d, const float* z_steps_bg_d, int coarse_samples, const float* u_fine_d,
+                          const float* u_fine_bg_d, int fine_samples, int use_cascade, int sh_deg, int precision,
+                          const mn_occupancy* occ, int32_t* counts_out_d, const mn_render_outputs* out, void* workspace_d,
+                          size_t workspace_bytes, void* stream);
+
 /* Fused per-ray all-gather over peer memory (SURVEY.md §8e): stores this rank's (rgb, depth) rows [row0, row0+n) into
  * every buffer of peer_bufs[0..n_peers) - HOST array of device pointers to [n_total, 4] fp32 buffers, one per rank,
  * peer-mapped into this process (e.g. torch symmetric memory) - with 16-byte P2P stores.  Cross-rank ordering (nobody

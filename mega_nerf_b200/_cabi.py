@@ -44,6 +44,11 @@ class Rows(C.Structure):
                 ('dir_stride', C.c_int64), ('idx_d', C.c_void_p), ('samples_per_ray', C.c_int)]
 
 
+class Occupancy(C.Structure):
+    """mn_occupancy: a reso^3 bit grid on the device and the octree frame it lives in."""
+    _fields_ = [('bits', C.c_void_p), ('reso', C.c_int), ('offset', C.c_float * 3), ('scale', C.c_float * 3)]
+
+
 class RenderOutputs(C.Structure):
     """mn_render_outputs: device pointers (or None) named after render_rays' result keys."""
     _fields_ = [(k, C.c_void_p) for k in ('rgb', 'depth', 'depth_var', 'bg_lambda', 'fg_rgb', 'bg_rgb', 'fg_depth', 'bg_depth',
@@ -105,6 +110,12 @@ SIGNATURES = {
     'mn_render_rays_bg_workspace_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I]),
     'mn_render_rays_bg': (_I, [_P, _P, _P, _P, _P, _L, _P, _P, _I, _I, _P, _P, _I, _P, _P, _I, _I, _I, _I,
                                C.POINTER(RenderOutputs), _P, _Z, _P]),
+    'mn_render_rays_occ_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_occ': (_I, [_P, _P, _P, _P, _L, _P, _I, _P, _I, _I, _I, _I, C.POINTER(Occupancy), _P, _P, _P, _P, _P, _P, _Z,
+                                _P]),
+    'mn_render_rays_bg_occ_workspace_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_bg_occ': (_I, [_P, _P, _P, _P, _P, _L, _P, _P, _I, _I, _P, _P, _I, _P, _P, _I, _I, _I, _I,
+                                   C.POINTER(Occupancy), _P, C.POINTER(RenderOutputs), _P, _Z, _P]),
     'mn_peer_gather_store': (_I, [_P, _P, _P, _L, _L, C.POINTER(C.c_void_p), _I, _P]),
     'mn_cluster_min_dist_ratios': (_I, [_P, _P, _L, _P, _I, _P, _I, _I, _F, _P, _P, _P]),
     # training (SURVEY.md §8f-1)

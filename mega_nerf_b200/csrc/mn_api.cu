@@ -457,8 +457,9 @@ static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, Ta
 static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, int sigma_only,
                               const float* sigma_noise_d, int precision, float* out_d, void* workspace_d,
                               size_t workspace_bytes, void* tape_d, size_t tape_bytes, void* stream, int train_tc = 0,
-                              LiveRows live = LiveRows{}, int mult = 0) {
+                              LiveRows live = LiveRows{}, int mult = 0, const int* gather = nullptr) {
     if (!ctx || !m || !rows || B < 0) return MN_ERR_INVALID;
+    if (gather && rows->mode != 1) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward: a row gather needs ray-structured rows");
     const mn_model_desc& d = m->d;
     const NetDims& nd = m->nd;
     cudaStream_t st = (cudaStream_t)stream;
@@ -506,6 +507,7 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
         src.idx = rows->idx_d;
         src.idx_stride = 1;
         src.dir_quirk = (has_dir && !has_idx) ? 1 : 0;  // [xyz, dir] rows: x[:, -4:-1] = (z, dx, dy)
+        src.gather = gather;
     }
     if (B == 0) return MN_OK;
 
@@ -674,9 +676,9 @@ int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int
 }  // extern "C"
 
 int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,
-                          float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+                          float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st, const int* gather) {
     return model_forward_impl(ctx, m, rows, B, use_coarse, 0, nullptr, precision, out_d, workspace_d, workspace_bytes, nullptr, 0, st,
-                              0, live);
+                              0, live, 0, gather);
 }
 
 // ---- density grid (scripts/create_octree.py:61-105, 139-162) -------------------------------------------------------

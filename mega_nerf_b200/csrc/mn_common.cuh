@@ -104,18 +104,21 @@ struct RowSrc {
     int div;             // row -> ray divisor (1 in mode 0)
     int dir_quirk;       // models/nerf.py:146 x[:, -4:-1] with no index column: dir := (xyz_z, d_x, d_y)
     int xyz_dim;
+    const int* gather;   // mode 1 only: row r reads sample gather[r] (the queried samples of an occupancy grid); NULL = row r
 
-    __device__ __forceinline__ float xyz(int64_t row, int j) const { return x[row * cols + net_off + j]; }
-    __device__ __forceinline__ float route_xyz(int64_t row, int j) const { return x[row * cols + j]; }
+    __device__ __forceinline__ int64_t sample(int64_t row) const { return gather ? (int64_t)gather[row] : row; }
+    __device__ __forceinline__ float xyz(int64_t row, int j) const { return x[sample(row) * cols + net_off + j]; }
+    __device__ __forceinline__ float route_xyz(int64_t row, int j) const { return x[sample(row) * cols + j]; }
     __device__ __forceinline__ float dir(int64_t row, int j) const {
+        const int64_t s = sample(row);
         if (dir_quirk) {
             // columns [-4:-1] of [xyz(3), dir(3)] are (z, d_x, d_y)
-            if (j == 0) return x[row * cols + net_off + 2];
-            return dirs[(row / div) * dir_stride + (j - 1)];
+            if (j == 0) return x[s * cols + net_off + 2];
+            return dirs[(s / div) * dir_stride + (j - 1)];
         }
-        return dirs[(row / div) * dir_stride + j];
+        return dirs[(s / div) * dir_stride + j];
     }
-    __device__ __forceinline__ float index(int64_t row) const { return idx[(row / div) * idx_stride]; }
+    __device__ __forceinline__ float index(int64_t row) const { return idx[(sample(row) / div) * idx_stride]; }
 };
 
 // Rows of a call whose count lives on the device (the background pass of mn_render_rays_bg): `rays` points at a device count of

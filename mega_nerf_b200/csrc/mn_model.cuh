@@ -150,8 +150,10 @@ int mn_route_build_assigned(mn_ctx* ctx, mn_model* m, const float* rows, int64_t
                             int* slot_row, void* scratch, const float** noise_out, cudaStream_t st);
 // mn_model_forward (inference) over the first live.rows(B) of B rows: the router, the encoders and the MLP tiles see only those,
 // the launch sequence is the one for B rows (csrc/mn_api.cu)
+// gather (ray-structured rows only): row r is sample gather[r] of `rows` - point gather[r], ray gather[r] / samples_per_ray - and
+// its result goes to out_d row r (the queried samples of an occupancy grid, mn_render.cu)
 int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,
-                          float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st);
+                          float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st, const int* gather = nullptr);
 // ---- the one launch of each stage kernel (csrc/mn_sample.cu).  The public stage entry points validate their arguments and call
 // these; the render passes of mn_render_rays(_bg) call them directly, the background pass with its device ray count (`live`: rays
 // at or past it are skipped, grids stay sized for N) and the sample orders it needs: flip = reversed stratify output, flip_pts =
@@ -171,7 +173,8 @@ int mn_stage_composite(mn_ctx* ctx, const float* raw_d, const float* z_d, const 
                        LiveRows live, float* weights_out_d, float* rgb_out_d, float* depth_out_d, float* depth_var_out_d,
                        float* bg_lambda_out_d, cudaStream_t st);
 int mn_stage_sh_to_rgb(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
-                       int dir_div, int64_t B, int apply_sigmoid, LiveRows live, float* out_d, cudaStream_t st);
+                       int dir_div, int64_t B, int apply_sigmoid, LiveRows live, float* out_d, cudaStream_t st,
+                       const int* gather = nullptr);   // gather: row b's direction is that of sample gather[b] (occupancy grids)
 int mn_mlp_simt_launch(mn_ctx* ctx, const MlpArgs& a, int64_t n_tiles128, cudaStream_t st);
 int mn_mlp_bwd_launch(mn_ctx* ctx, const BwdArgs& a, int64_t n_tiles128, cudaStream_t st);
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws,

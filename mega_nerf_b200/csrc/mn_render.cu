@@ -107,6 +107,87 @@ __global__ void bg_blend_kernel(float* __restrict__ val, const float* __restrict
     val[i] = __fadd_rn(v, add);
 }
 
+// ---- occupancy grid (mn_render_rays_occ / mn_render_rays_bg_occ): the foreground samples in cells the grid marks empty are not
+// queried, their raw row is (0, 0, 0, 0).  The queried samples are compacted on the device like the background rays (a block
+// count, then a stable block scan over the counts of the blocks before), the model runs on them through a row gather with its
+// row count read from the device, and a scatter writes every raw row.
+constexpr int kOccBlock = 1024;
+
+struct OccGrid {
+    const uint32_t* bits;   // reso^3 bits, cell (i * reso + j) * reso + k at bit c & 31 of word c >> 5
+    int reso;
+    float off[3], scl[3];
+};
+
+// Whether the sample at p[0..2] is queried.  u_a = p_a * scale_a + offset_a is two separately rounded fp32 operations (no FMA,
+// __fmul_rn / __fadd_rn), the cell index floorf(u_a * reso).  A point outside [0, 1)^3 - NaN included, which fails both
+// comparisons - is always queried.  u_a < 1 keeps u_a * reso below reso in fp32 (round-to-nearest is monotone and
+// (1 - 2^-24) * reso rounds below reso), so the min() never binds; it only keeps the read inside the grid.
+__device__ __forceinline__ bool occ_queried(const OccGrid& g, const float* __restrict__ p) {
+    int64_t cell = 0;
+    for (int a = 0; a < 3; ++a) {
+        const float u = __fadd_rn(__fmul_rn(p[a], g.scl[a]), g.off[a]);
+        if (!(u >= 0.0f && u < 1.0f)) return true;
+        const int i = min((int)floorf(__fmul_rn(u, (float)g.reso)), g.reso - 1);
+        cell = cell * g.reso + i;
+    }
+    return (g.bits[cell >> 5] >> (cell & 31)) & 1u;
+}
+
+// flag[s] = 1 iff sample s of the [n, 3] points is queried; blk[b] = queried samples of block b.
+__global__ void __launch_bounds__(kOccBlock) occ_test_kernel(const float* __restrict__ xyz, int64_t n, OccGrid g, int* __restrict__ flag,
+                                                             int* __restrict__ blk) {
+    const int64_t s = (int64_t)blockIdx.x * kOccBlock + threadIdx.x;
+    bool q = false;
+    if (s < n) {
+        q = occ_queried(g, xyz + s * 3);
+        flag[s] = q ? 1 : 0;
+    }
+    const int c = __syncthreads_count(q);
+    if (threadIdx.x == 0) blk[blockIdx.x] = c;
+}
+
+// Stable compaction of the queried samples: idx[0 .. count) = their flat indices in ascending order, pos[s] = the compacted row
+// of sample s or -1, *count (and *count_out if given) = the queried samples (written by the last block).
+__global__ void __launch_bounds__(kOccBlock) occ_compact_kernel(int64_t n, const int* __restrict__ blk, int* __restrict__ pos,
+                                                                int* __restrict__ idx, int* __restrict__ count, int* __restrict__ count_out) {
+    __shared__ int wsum[32], wbase[32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int part = 0;                                           // queried samples of the blocks before this one
+    for (unsigned b = threadIdx.x; b < blockIdx.x; b += kOccBlock) part += blk[b];
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    const int64_t s = (int64_t)blockIdx.x * kOccBlock + threadIdx.x;
+    const bool q = s < n && pos[s] != 0;
+    const unsigned bal = __ballot_sync(0xffffffffu, q);
+    if (lane == 0) { wsum[warp] = part; wbase[warp] = __popc(bal); }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int run = 0;
+        for (int w = 0; w < kOccBlock / 32; ++w) run += wsum[w];
+        for (int w = 0; w < kOccBlock / 32; ++w) { const int c = wbase[w]; wbase[w] = run; run += c; }
+        if (blockIdx.x == gridDim.x - 1) {
+            *count = run;
+            if (count_out) *count_out = run;
+        }
+    }
+    __syncthreads();
+    if (s >= n) return;
+    int p = -1;
+    if (q) {
+        p = wbase[warp] + __popc(bal & ((1u << lane) - 1));
+        idx[p] = (int)s;
+    }
+    pos[s] = p;
+}
+
+// raw[s] = the compacted result row pos[s], or (0, 0, 0, 0) for a sample that was not queried.
+__global__ void occ_scatter_kernel(const float4* __restrict__ cmp, const int* __restrict__ pos, int64_t n, float4* __restrict__ raw) {
+    const int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    const int p = pos[s];
+    raw[s] = p >= 0 ? cmp[p] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
+
 // Workspace offsets: each buffer aligned on its own.
 struct Carve {
     size_t off = 0;
@@ -156,15 +237,27 @@ PassBufs carve_pass(Carve& take, const mn_model* net, int64_t N, int S, int F, i
 struct RenderPlan {
     PassBufs fg, bg;
     size_t last_delta, model_ws, model_ws_bytes, total;
+    // occupancy grid (foreground queries, sized for the larger of the two): flags / compacted rows, sample indices, block counts,
+    // the queried-row count of each pass, compacted results [rows, 4]
+    size_t occ_pos, occ_idx, occ_blk, occ_count, occ_out;
     // background split and blend; every per-ray buffer holds N rays (the compacted background rays first)
     size_t far_ov, pos, blk, count, ids, dirs, idx, ld_b, rgb_b, depth_b, rgb_cb, lam, lam_c;
 };
 
-RenderPlan make_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, int sh, int precision) {
+RenderPlan make_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, int sh, int precision,
+                     bool occ = false) {
     RenderPlan p{};
     Carve take;
     p.fg = carve_pass(take, m, N, Sc, Sf, use_cascade, sh, 3, false, precision);
     p.last_delta = take((size_t)N * 4);
+    if (occ) {
+        const int64_t rows = N * (p.fg.Sq > Sc ? p.fg.Sq : Sc);
+        p.occ_pos = take((size_t)rows * 4);
+        p.occ_idx = take((size_t)rows * 4);
+        p.occ_blk = take((size_t)mn_cdiv(rows, kOccBlock) * 4);
+        p.occ_count = take(2 * 4);
+        p.occ_out = take((size_t)rows * 16);
+    }
     p.model_ws_bytes = p.fg.model_ws_bytes;
     if (bg) {
         p.far_ov = take((size_t)N * 4);
@@ -208,7 +301,7 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
                 const float* center_d, const float* radius_d, int include_xyz_real, int cluster_2d, const float* z_steps_d,
                 const float* z_steps_bg_d, int coarse_samples, const float* u_fine_d, const float* u_fine_bg_d, int fine_samples,
                 int use_cascade, int sh_deg, int precision, const mn_render_outputs& o, void* workspace_d, size_t workspace_bytes,
-                void* stream, const char* name) {
+                void* stream, const char* name, const mn_occupancy* occ = nullptr, int* counts_out_d = nullptr) {
     const std::string nm(name);
     if (!ctx || !m || !rays_d || !z_steps_d || !o.rgb || N < 0 || coarse_samples < 1 || fine_samples < 0) return MN_ERR_INVALID;
     if (fine_samples > 0 && !u_fine_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": u_fine_d is required when fine_samples > 0");
@@ -222,9 +315,16 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
             return mn_fail(ctx, MN_ERR_INVALID, nm + ": background resampling needs u_fine_bg, >= 2 fine and >= 6 coarse samples");
         if (radius_d && !center_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": sphere radius without a center");
     }
+    if (occ) {
+        if (!occ->bits || occ->reso < 1 || occ->reso > MN_OCC_MAX_RESO)
+            return mn_fail(ctx, MN_ERR_INVALID, nm + ": the occupancy grid needs bits and a reso of 1.." + std::to_string(MN_OCC_MAX_RESO));
+        const int Sq = fine_samples > 0 ? (use_cascade ? coarse_samples + fine_samples : fine_samples) : 0;
+        if (N * (int64_t)(Sq > coarse_samples ? Sq : coarse_samples) > INT32_MAX)
+            return mn_fail(ctx, MN_ERR_INVALID, nm + ": an occupancy-grid render indexes at most 2^31 - 1 samples per pass");
+    }
     if (N == 0) return MN_OK;
     const bool sh = sh_deg >= 0;
-    const RenderPlan p = make_plan(m, bg, N, coarse_samples, fine_samples, use_cascade, sh, precision);
+    const RenderPlan p = make_plan(m, bg, N, coarse_samples, fine_samples, use_cascade, sh, precision, occ != nullptr);
     if (!workspace_d || workspace_bytes < p.total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     char* W = (char*)workspace_d;
     auto F = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
@@ -251,6 +351,53 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
         return MN_OK;
     };
 
+    // The same query of the foreground points through the occupancy grid: test and compaction of the N * S samples, the model
+    // (and the SH head) on the queried rows, whose count stays on the device, then every raw row from them or zero.  pass: 0
+    // coarse, 1 fine (the slot of the queried-row count).
+    OccGrid G{};
+    if (occ) {
+        G.bits = occ->bits;
+        G.reso = occ->reso;
+        for (int a = 0; a < 3; ++a) { G.off[a] = occ->offset[a]; G.scl[a] = occ->scale[a]; }
+    }
+    auto query_occ = [&](mn_model* net, const float* xyz, int S, int coarse, float* mlp_out, float* raw_out, const float* dirs,
+                         int64_t dstride, const float* idx, int pass) -> int {
+        const int64_t n = N * S;
+        const unsigned nblk = (unsigned)mn_cdiv(n, kOccBlock);
+        int* cnt = I(p.occ_count) + pass;
+        const int* gather = I(p.occ_idx);
+        occ_test_kernel<<<nblk, kOccBlock, 0, st>>>(xyz, n, G, I(p.occ_pos), I(p.occ_blk));
+        MN_LAUNCH_CHECK(ctx);
+        occ_compact_kernel<<<nblk, kOccBlock, 0, st>>>(n, I(p.occ_blk), I(p.occ_pos), I(p.occ_idx), cnt,
+                                                       counts_out_d ? counts_out_d + pass : nullptr);
+        MN_LAUNCH_CHECK(ctx);
+        mn_rows rows{};
+        rows.mode = 1;
+        rows.x_d = xyz;
+        rows.cols = 3;
+        rows.dirs_d = net->d.pos_dir_dim > 0 ? dirs : nullptr;
+        rows.dir_stride = dstride;
+        rows.idx_d = net->d.appearance_dim > 0 ? idx : nullptr;
+        rows.samples_per_ray = S;
+        const LiveRows lr{cnt, 1};
+        float* cmp = F(p.occ_out);
+        int r = mn_model_forward_live(ctx, net, &rows, n, lr, coarse, precision, sh ? mlp_out : cmp, W + p.model_ws, p.model_ws_bytes,
+                                      st, gather);
+        if (r) return r;
+        if (sh && (r = mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, net->nd.rgb_dim + 1, dirs, dstride, S, n, 1, lr, cmp, st, gather)))
+            return r;
+        occ_scatter_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, st>>>(reinterpret_cast<const float4*>(cmp), I(p.occ_pos), n,
+                                                                      reinterpret_cast<float4*>(raw_out));
+        MN_LAUNCH_CHECK(ctx);
+        return MN_OK;
+    };
+    // a query of pass `pass`: through the grid in the foreground pass (masked) when there is one
+    auto query_pass = [&](bool masked, mn_model* net, const float* xyz, int cols, int S, int coarse, float* mlp_out, float* raw_out,
+                          const float* dirs, int64_t dstride, const float* idx, const int* live, int pass) -> int {
+        if (masked) return query_occ(net, xyz, S, coarse, mlp_out, raw_out, dirs, dstride, idx, pass);
+        return query(net, xyz, cols, S, coarse, mlp_out, raw_out, dirs, dstride, idx, live);
+    };
+
     // The two-pass render of one network (rendering.py:176-248, render.py `_two_pass`) from the coarse depths and points the
     // caller wrote into b.z_c, b.z_c_comp, b.xyz_c and b.dreal_c.  live: the device count of the rays that hold data (background
     // pass), or null for all N.  cols: point columns.  fine_points(z, S, flip_pts, xyz, dreal) makes the fine points from the
@@ -259,10 +406,11 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
     auto two_pass = [&](mn_model* net, const PassBufs& b, const int* live, int cols, const float* last_delta, const float* u_fine,
                         const float* dirs, int64_t dstride, const float* idx, const mn_render_outputs& r, auto&& fine_points) -> int {
         const LiveRows lr{live, 1};
+        const bool masked = occ && !b.flip;   // the grid applies to the foreground pass only
         // depth scratch when only the variance is wanted: the coarse weights are dead by the time it is written
         float* depth = r.depth ? r.depth : (r.depth_var ? F(b.w_c) : nullptr);
         int e;
-        if ((e = query(net, F(b.xyz_c), cols, b.S, 1, F(b.mlp_c), F(b.raw_c), dirs, dstride, idx, live))) return e;
+        if ((e = query_pass(masked, net, F(b.xyz_c), cols, b.S, 1, F(b.mlp_c), F(b.raw_c), dirs, dstride, idx, live, 0))) return e;
         if ((e = mn_stage_composite(ctx, F(b.raw_c), F(b.z_c_comp), F(b.dreal_c), b.S, nullptr, nullptr, nullptr, 0, last_delta, N,
                                     b.flip, lr, fine ? F(b.w_c) : nullptr, use_cascade ? (fine ? r.rgb_coarse : r.rgb) : nullptr,
                                     fine ? nullptr : depth, fine ? nullptr : r.depth_var,
@@ -275,7 +423,7 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
         if (use_cascade)
             if ((e = mn_stage_sort_cat(ctx, F(b.z_c), b.S, F(b.z_f), b.F, N, 0, lr, F(b.z_q), b.flip ? F(b.z_q_comp) : nullptr, st))) return e;
         if ((e = fine_points(F(b.z_q), b.Sq, b.flip && use_cascade, F(b.xyz_f), F(b.dreal_f)))) return e;
-        if ((e = query(net, F(b.xyz_f), cols, b.Sq, 0, F(b.mlp_f), F(b.raw_f), dirs, dstride, idx, live))) return e;
+        if ((e = query_pass(masked, net, F(b.xyz_f), cols, b.Sq, 0, F(b.mlp_f), F(b.raw_f), dirs, dstride, idx, live, 1))) return e;
         if (use_cascade)
             return mn_stage_composite(ctx, F(b.raw_f), F(b.z_q_comp), F(b.dreal_f), b.Sq, nullptr, nullptr, nullptr, 0, last_delta, N,
                                       b.flip, lr, nullptr, r.rgb, depth, r.depth_var, r.bg_lambda, st);
@@ -384,6 +532,47 @@ int mn_render_rays_bg(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays
     return render_impl(ctx, fg, bg, rays_d, image_indices_d, N, sphere_center3_d, sphere_radius3_d, include_xyz_real, cluster_2d,
                        z_steps_d, z_steps_bg_d, coarse_samples, u_fine_d, u_fine_bg_d, fine_samples, use_cascade, sh_deg, precision,
                        *out, workspace_d, workspace_bytes, stream, bg ? "mn_render_rays_bg" : "mn_render_rays");
+}
+
+size_t mn_render_rays_occ_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                          int sh_deg, int precision) {
+    if (!m || N < 0 || coarse_samples < 1 || fine_samples < 0) return 0;
+    return make_plan(m, nullptr, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision, true).total;
+}
+
+int mn_render_rays_occ(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N,
+                       const float* z_steps_d, int coarse_samples, const float* u_fine_d, int fine_samples, int use_cascade,
+                       int sh_deg, int precision, const mn_occupancy* occ, int32_t* counts_out_d, float* rgb_out_d,
+                       float* depth_out_d, float* depth_var_out_d, float* rgb_coarse_out_d, void* workspace_d,
+                       size_t workspace_bytes, void* stream) {
+    if (!occ) return mn_fail(ctx, MN_ERR_INVALID, "mn_render_rays_occ: occ is NULL");
+    mn_render_outputs o{};
+    o.rgb = rgb_out_d;
+    o.depth = depth_out_d;
+    o.depth_var = depth_var_out_d;
+    o.rgb_coarse = rgb_coarse_out_d;
+    return render_impl(ctx, m, nullptr, rays_d, image_indices_d, N, nullptr, nullptr, 0, 0, z_steps_d, nullptr, coarse_samples,
+                       u_fine_d, nullptr, fine_samples, use_cascade, sh_deg, precision, o, workspace_d, workspace_bytes, stream,
+                       "mn_render_rays_occ", occ, counts_out_d);
+}
+
+size_t mn_render_rays_bg_occ_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                             int use_cascade, int sh_deg, int precision) {
+    if (!fg || !bg || N < 0 || coarse_samples < 1 || fine_samples < 0) return 0;
+    return make_plan(fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision, true).total;
+}
+
+int mn_render_rays_bg_occ(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays_d, const float* image_indices_d, int64_t N,
+                          const float* sphere_center3_d, const float* sphere_radius3_d, int include_xyz_real, int cluster_2d,
+                          const float* z_steps_d, const float* z_steps_bg_d, int coarse_samples, const float* u_fine_d,
+                          const float* u_fine_bg_d, int fine_samples, int use_cascade, int sh_deg, int precision,
+                          const mn_occupancy* occ, int32_t* counts_out_d, const mn_render_outputs* out, void* workspace_d,
+                          size_t workspace_bytes, void* stream) {
+    if (!out || !bg) return MN_ERR_INVALID;
+    if (!occ) return mn_fail(ctx, MN_ERR_INVALID, "mn_render_rays_bg_occ: occ is NULL");
+    return render_impl(ctx, fg, bg, rays_d, image_indices_d, N, sphere_center3_d, sphere_radius3_d, include_xyz_real, cluster_2d,
+                       z_steps_d, z_steps_bg_d, coarse_samples, u_fine_d, u_fine_bg_d, fine_samples, use_cascade, sh_deg, precision,
+                       *out, workspace_d, workspace_bytes, stream, "mn_render_rays_bg_occ", occ, counts_out_d);
 }
 
 }  // extern "C"

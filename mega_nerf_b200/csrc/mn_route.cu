@@ -138,7 +138,8 @@ __global__ void route_count_kernel(RowSrc src, int64_t B, LiveRows live, const f
     __syncthreads();
     const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t n = live.rows(B);
-    const bool direct = n <= 25 && K <= 25;
+    // the queried samples of an occupancy grid (src.gather) stand for the whole B-row query, whose batch size picks the path
+    const bool direct = (src.gather ? B : n) <= 25 && K <= 25;
     uint64_t mask = 0;
     if (row < n) {
         float d[KMAX], w[KMAX];

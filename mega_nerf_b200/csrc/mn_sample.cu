@@ -613,12 +613,14 @@ __device__ __forceinline__ float sh_eval(int deg, const float* s, float x, float
 }
 
 __global__ void sh_to_rgb_kernel(int deg, const float* __restrict__ coef, int64_t cstride, const float* __restrict__ dirs,
-                                 int64_t dstride, int ddiv, int64_t B, int sig, float* __restrict__ out, LiveRows live) {
+                                 int64_t dstride, int ddiv, int64_t B, int sig, float* __restrict__ out, LiveRows live,
+                                 const int* __restrict__ gather) {
     const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= live.rows(B)) return;
     const int nc = (deg + 1) * (deg + 1);
     const float* c = coef + b * cstride;
-    const float* d = dirs + (b / ddiv) * dstride;
+    // gather: row b is the compacted sample gather[b] (an occupancy-grid query), whose ray gives the direction
+    const float* d = dirs + ((gather ? (int64_t)gather[b] : b) / ddiv) * dstride;
     float s[25];
     float o[4];
     for (int ch = 0; ch < 3; ++ch) {
@@ -1052,9 +1054,9 @@ int mn_stage_composite(mn_ctx* ctx, const float* raw_d, const float* z_d, const 
 }
 
 int mn_stage_sh_to_rgb(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
-                       int dir_div, int64_t B, int apply_sigmoid, LiveRows live, float* out_d, cudaStream_t st) {
+                       int dir_div, int64_t B, int apply_sigmoid, LiveRows live, float* out_d, cudaStream_t st, const int* gather) {
     sh_to_rgb_kernel<<<(unsigned)mn_cdiv(B, 256), 256, 0, st>>>(deg, coef_d, coef_stride, dirs_d, dir_stride, dir_div, B, apply_sigmoid,
-                                                                out_d, live);
+                                                                out_d, live, gather);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }

@@ -15,6 +15,14 @@ its split.  The reference's sphere bound check (rendering.py:412-414) becomes a 
 raises the same `Exception`.
 
     g = GraphedRenderRays(nerf, hparams, 4096, dev, bg_nerf=bg, sphere_center=c, sphere_radius=r, get_bg_fg_rgb=True)
+
+With an occupancy grid (mega_nerf_b200.octree.OccupancyGrid; an approximate render mode, see render_rays_fused) the graph
+captures `render_rays_fused(..., occupancy=grid)`, with or without a background network.  The queried samples are compacted
+on the device, so one graph serves every chunk whatever the grid skips; `occupancy_counts` holds the queried foreground
+samples of the coarse and fine passes after each replay.  The graph reads the grid's words in place and keeps the grid alive;
+a different grid needs a new GraphedRenderRays.
+
+    g = GraphedRenderRays(nerf, hparams, 4096, dev, occupancy=octree.occupancy_grid(hparams, nerf, offset, invradius))
 """
 from argparse import Namespace
 from typing import Dict, Optional
@@ -30,14 +38,19 @@ class GraphedRenderRays:
     def __init__(self, nerf: nn.Module, hparams: Namespace, n_rays: int, device: torch.device, with_indices: bool = True,
                  get_depth: bool = True, get_depth_variance: bool = False, warmup: int = 2, post=None,
                  bg_nerf: Optional[nn.Module] = None, sphere_center: Optional[torch.Tensor] = None,
-                 sphere_radius: Optional[torch.Tensor] = None, get_bg_fg_rgb: bool = False):
+                 sphere_radius: Optional[torch.Tensor] = None, get_bg_fg_rgb: bool = False, occupancy=None):
         """`post(results)`, if given, runs right after render_rays INSIDE the captured region - e.g. the per-chunk
         exchange of a multi-GPU render (`torch.distributed.all_gather_into_tensor` on NCCL is capturable), so that a
         step stays one graph launch; whatever it returns is kept in `self.post_result`.
-        bg_nerf / sphere_center / sphere_radius / get_bg_fg_rgb: as for render_rays (the background path)."""
+        bg_nerf / sphere_center / sphere_radius / get_bg_fg_rgb: as for render_rays (the background path).
+        occupancy: an OccupancyGrid, as for render_rays_fused (captured once; a new grid needs a new GraphedRenderRays)."""
         if nerf.training or (bg_nerf is not None and bg_nerf.training):
             raise ValueError('GraphedRenderRays replays the inference path; call nerf.eval() first')
         _refuse_bg_ep(bg_nerf, 'GraphedRenderRays')
+        if occupancy is not None and getattr(_unwrap(nerf), '_ep', None) is not None:
+            raise ValueError('GraphedRenderRays: an occupancy grid cannot mask a network under expert parallelism')
+        self.occupancy = occupancy
+        self.occupancy_counts = torch.zeros(2, device=device, dtype=torch.int32) if occupancy is not None else None
         self.nerf, self.hparams = nerf, hparams
         self.flags = (get_depth, get_depth_variance, False)
         self.bg_nerf = bg_nerf
@@ -74,7 +87,12 @@ class GraphedRenderRays:
 
     def _run(self) -> Dict[str, torch.Tensor]:
         with torch.no_grad():      # inference path only (a recording call would switch to the fp32 training kernels)
-            if self.bg_nerf is None:
+            if self.occupancy is not None:
+                res = render_rays_fused(self.nerf, self.rays, self.indices, self.hparams, self.flags[0], self.flags[1],
+                                        bg_nerf=self.bg_nerf, sphere_center=self.center, sphere_radius=self.radius,
+                                        get_bg_fg_rgb=self.get_bg_fg_rgb, check_status=False, occupancy=self.occupancy,
+                                        occupancy_counts=self.occupancy_counts)
+            elif self.bg_nerf is None:
                 res, _ = render_rays(self.nerf, None, self.rays, self.indices, self.hparams, None, None, *self.flags)
             else:
                 # no sync inside the captured region: the status word is checked after each replay (_check)

@@ -7,6 +7,8 @@
   occupied_points<- grid[sigmas >= sigma_thresh] of _step1's masking_mode 'sigma' (create_octree.py:165-166, 176)
   lattice_points <- grid[mask] for any mask over the lattice (masking_mode 'weight': the mask from svox's grid weights)
   cell_colors    <- the rgba means of _step2 (create_octree.py:189-207), model calls on ray-structured rows
+  occupancy_grid <- _step1's sigma mask (create_octree.py:139-176) packed into an OccupancyGrid, the bit grid with which
+                    render_rays_fused / GraphedRenderRays skip the network queries of empty space (an approximate render mode)
 
 create_octree.py runs as __main__, so install() cannot reach these; INTEGRATION.md lists the lines to change there.  svox's own
 work (grid_weight_render, the in-cell sampler, refinement, merge, save) stays svox's.
@@ -159,3 +161,83 @@ def cell_colors(hparams: Namespace, nerf: nn.Module, points: torch.Tensor) -> to
         first = nerf.sub_modules[0] if isinstance(nerf, Mod.MegaNeRF) else (nerf.coarse if isinstance(nerf, Mod.Cascade) else nerf)
         return torch.empty(0, first.rgb_dim + 1, device=device)
     return torch.cat(out)
+
+
+class OccupancyGrid:
+    """A reso^3 bit grid over the octree frame (offset, scale = tree.offset, tree.invradius): the input of the occupancy render
+    mode of render_rays_fused / GraphedRenderRays.  A foreground sample x lies in cell (i_0, i_1, i_2), i_a = floor(u_a * reso)
+    with u_a = x_a * scale_a + offset_a (two fp32 roundings); it is skipped - raw (0, 0, 0, 0), no network query - iff
+    0 <= u_a < 1 on every axis and the cell's bit is 0.  Cells are ordered as density_grid's lattice: cell
+    (i * reso + j) * reso + k holds the lattice point (xx[i], yy[j], zz[k]) of lattice_axes(offset, scale, reso), so
+    `density_grid(...) >= sigma_thresh` is a mask for from_mask as it stands.
+
+    bits: int32 [ceil(reso**3 / 32)] on the device, cell c at bit c % 32 of word c // 32.  A captured CUDA graph reads these
+    words in place: it keeps this object alive, and a different grid needs a new capture."""
+
+    def __init__(self, bits: torch.Tensor, reso: int, offset, scale):
+        reso = int(reso)
+        if bits.dtype != torch.int32 or bits.dim() != 1 or bits.numel() != (reso ** 3 + 31) // 32:
+            raise ValueError(f'bits must be int32 [{(reso ** 3 + 31) // 32}] for reso {reso}')
+        self.bits = bits.contiguous()
+        self.reso = reso
+        self.offset = _axis_values(offset)
+        self.scale = _axis_values(scale)
+
+    @classmethod
+    def from_mask(cls, mask: torch.Tensor, offset, scale, device: Optional[torch.device] = None) -> 'OccupancyGrid':
+        """The grid whose occupied cells are the True entries of a boolean reso^3 mask ([reso**3] in lattice row order, or
+        [reso, reso, reso] indexed [i, j, k]), packed on the mask's device (or on `device`)."""
+        m = mask.reshape(-1).to(device if device is not None else mask.device, torch.bool)
+        reso = int(round(m.numel() ** (1.0 / 3.0)))
+        if reso < 1 or reso ** 3 != m.numel():
+            raise ValueError(f'an occupancy mask holds reso^3 cells, got {m.numel()}')
+        return cls(pack_bits(m), reso, offset, scale)
+
+    def cabi(self) -> K.Occupancy:
+        return K.Occupancy(self.bits.data_ptr(), self.reso, (C.c_float * 3)(*self.offset), (C.c_float * 3)(*self.scale))
+
+    def occupancy(self) -> float:
+        """Share of the cells that are occupied."""
+        return float(unpack_bits(self.bits, self.reso ** 3).float().mean())
+
+
+def pack_bits(mask: torch.Tensor) -> torch.Tensor:
+    """[n] bool -> int32 [ceil(n / 32)] with entry c at bit c % 32 of word c // 32 (mn_occupancy's layout)."""
+    n = mask.numel()
+    m = torch.zeros((n + 31) // 32 * 32, dtype=torch.int64, device=mask.device)
+    m[:n] = mask.reshape(-1).to(torch.int64)
+    w = (m.view(-1, 32) << torch.arange(32, device=mask.device, dtype=torch.int64)).sum(1)
+    return torch.where(w >= 2 ** 31, w - 2 ** 32, w).to(torch.int32)
+
+
+def unpack_bits(bits: torch.Tensor, n: int) -> torch.Tensor:
+    """The first n entries of pack_bits' layout, [n] bool."""
+    b = (bits.to(torch.int64).unsqueeze(1) >> torch.arange(32, device=bits.device, dtype=torch.int64)) & 1
+    return b.reshape(-1)[:n].bool()
+
+
+def occupancy_queried(xyz: torch.Tensor, grid: OccupancyGrid) -> torch.Tensor:
+    """Which of the points xyz [..., 3] (fp32) the occupancy render mode queries, [...] bool: the test of the render kernel in
+    torch fp32 ops (u = x * scale + offset as two ops, floor(u * reso), the bit of cell (i * reso + j) * reso + k)."""
+    x = xyz.to(torch.float32)
+    off = torch.tensor(grid.offset, dtype=torch.float32, device=x.device)
+    scl = torch.tensor(grid.scale, dtype=torch.float32, device=x.device)
+    u = (x * scl) + off
+    inside = ((u >= 0) & (u < 1)).all(-1)
+    i = torch.floor(u * float(grid.reso)).clamp(0, grid.reso - 1).to(torch.int64)
+    cell = (i[..., 0] * grid.reso + i[..., 1]) * grid.reso + i[..., 2]
+    cell = torch.where(inside, cell, torch.zeros_like(cell))
+    bits = grid.bits.to(x.device).to(torch.int64)
+    occupied = ((bits[cell // 32] >> (cell % 32)) & 1).bool()
+    return ~inside | occupied
+
+
+def occupancy_grid(hparams: Namespace, nerf: nn.Module, offset, invradius, reso: Optional[int] = None,
+                   alpha_thresh: Optional[float] = None) -> OccupancyGrid:
+    """_step1's occupied cells (create_octree.py:139-176) as an OccupancyGrid on the network's device: the density grid at
+    reso (default 2 ** (init_grid_depth + 1)) over the tree's box (offset = tree.offset, invradius = tree.invradius), the
+    reference's threshold sigma >= -log(1 - alpha_thresh) / (2 / reso) (default hparams.alpha_thresh), packed on the device."""
+    reso = int(reso) if reso is not None else 2 ** (hparams.init_grid_depth + 1)
+    at = hparams.alpha_thresh if alpha_thresh is None else alpha_thresh
+    sigmas = density_grid(nerf, offset, invradius, reso)
+    return OccupancyGrid.from_mask(sigmas >= _sigma_thresh(at, reso), offset, invradius)

@@ -399,16 +399,36 @@ def _refuse_bg_ep(bg: Optional[nn.Module], fn: str) -> None:
 def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Optional[torch.Tensor], hparams: Namespace,
                       get_depth: bool, get_depth_variance: bool, bg_nerf: Optional[nn.Module] = None,
                       sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None,
-                      get_bg_fg_rgb: bool = False, check_status: bool = True) -> Dict[str, torch.Tensor]:
+                      get_bg_fg_rgb: bool = False, check_status: bool = True, occupancy=None,
+                      occupancy_counts: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
     """The inference path of `render_rays(nerf, bg_nerf, ...)` as ONE library call (`mn_render_rays`, or `mn_render_rays_bg`
     with a background network): the same kernels in the same order, sequenced in C on the current stream instead of from
     Python.  Eval mode; returns the same keys and values as `render_rays(...)[0]` for the same flags.
 
     With a background network the split of the rays happens on the device (no host sync per chunk); the one sync is the
     status check at the end, where the reference checks its sphere bound too: a camera outside the ellipsoid raises its
-    `Exception`.  `check_status=False` leaves that check to the caller (CUDA-graph capture, where no sync may happen)."""
+    `Exception`.  `check_status=False` leaves that check to the caller (CUDA-graph capture, where no sync may happen).
+
+    occupancy: an octree.OccupancyGrid, an approximate render mode (`mn_render_rays_occ` / `mn_render_rays_bg_occ`): the
+    foreground samples of both passes in cells the grid marks empty are not queried and enter compositing as raw (0, 0, 0, 0),
+    which departs from the reference's results wherever the network's density there is not zero; the background pass is not
+    masked.  A grid with every cell occupied gives exactly the results without a grid.  occupancy_counts: None, or an int32
+    CUDA tensor of 2 elements that receives the queried foreground samples of the coarse and the fine pass (on the device, no
+    sync).  Not for expert-parallel networks."""
     net, bg = _nets(nerf, bg_nerf, 'render_rays_fused')
     _refuse_bg_ep(bg, 'render_rays_fused')
+    if occupancy is not None:
+        if net.training or (bg is not None and bg.training):
+            raise ValueError('render_rays_fused: an occupancy grid renders in eval mode only (no recording call)')
+        if getattr(net, '_ep', None) is not None:
+            raise ValueError('render_rays_fused: an occupancy grid cannot mask a network under expert parallelism')
+        if occupancy.bits.device != rays.device:
+            raise ValueError(f'the occupancy grid lives on {occupancy.bits.device}, the rays on {rays.device}')
+        if occupancy_counts is not None and (occupancy_counts.dtype != torch.int32 or occupancy_counts.numel() < 2
+                                             or not occupancy_counts.is_contiguous() or occupancy_counts.device != rays.device):
+            raise ValueError('occupancy_counts must be a contiguous int32 tensor of 2 elements on the rays\' device')
+    elif occupancy_counts is not None:
+        raise ValueError('occupancy_counts needs an occupancy grid')
     if net.training or (bg is not None and bg.training):
         raise ValueError('render_rays_fused is the inference path; call nerf.eval() first')
     if bool(hparams.use_cascade) != isinstance(net, Cascade):
@@ -455,7 +475,15 @@ def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
             continue                                       # coarse-only render: the final type is the coarse one
         setattr(out, field, K.ptr(res.get(key)))
     st = K.stream_of(dev)
+    occ = occupancy.cabi() if occupancy is not None else None
     if bg is None:
+        if occ is not None:
+            nbytes = int(L.mn_render_rays_occ_workspace_bytes(native.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
+            ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
+            K.check(L.mn_render_rays_occ(h, native.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(steps), Sc, K.ptr(u), Sf,
+                                         int(cascade), sh_deg, prec, C.byref(occ), K.ptr(occupancy_counts), out.rgb, out.depth,
+                                         out.depth_var, out.rgb_coarse, K.ptr(ws), ws.numel(), st), h)
+            return res
         nbytes = int(L.mn_render_rays_workspace_bytes(native.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
         ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
         K.check(L.mn_render_rays(h, native.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(steps), Sc, K.ptr(u), Sf, int(cascade),
@@ -470,11 +498,19 @@ def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
     c2d = real and getattr(net, 'cluster_dim_start', 0) == 1                          # render.py:304-305
     steps_bg = torch.linspace(0, 1, Sc // 2, device=dev)
     u_bg = torch.linspace(0, 1, Sf // 2, device=dev) if Sf > 0 else None
-    nbytes = int(L.mn_render_rays_bg_workspace_bytes(native.handle, bnative.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
-    ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
-    K.check(L.mn_render_rays_bg(h, native.handle, bnative.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(center), K.ptr(radius),
-                                int(real), int(c2d), K.ptr(steps), K.ptr(steps_bg), Sc, K.ptr(u), K.ptr(u_bg), Sf, int(cascade),
-                                sh_deg, prec, C.byref(out), K.ptr(ws), ws.numel(), st), h)
+    if occ is not None:
+        nbytes = int(L.mn_render_rays_bg_occ_workspace_bytes(native.handle, bnative.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
+        ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
+        K.check(L.mn_render_rays_bg_occ(h, native.handle, bnative.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(center), K.ptr(radius),
+                                        int(real), int(c2d), K.ptr(steps), K.ptr(steps_bg), Sc, K.ptr(u), K.ptr(u_bg), Sf,
+                                        int(cascade), sh_deg, prec, C.byref(occ), K.ptr(occupancy_counts), C.byref(out), K.ptr(ws),
+                                        ws.numel(), st), h)
+    else:
+        nbytes = int(L.mn_render_rays_bg_workspace_bytes(native.handle, bnative.handle, N, Sc, Sf, int(cascade), sh_deg, prec))
+        ws = torch.empty(max(nbytes, 256), device=dev, dtype=torch.uint8)
+        K.check(L.mn_render_rays_bg(h, native.handle, bnative.handle, K.ptr(rays), K.ptr(idx), N, K.ptr(center), K.ptr(radius),
+                                    int(real), int(c2d), K.ptr(steps), K.ptr(steps_bg), Sc, K.ptr(u), K.ptr(u_bg), Sf, int(cascade),
+                                    sh_deg, prec, C.byref(out), K.ptr(ws), ws.numel(), st), h)
     if check_status:
         # the reference raises from a host-side `.any()` over the sphere check (rendering.py:412-414)
         K.check(L.mn_check_status(h, st), h)
