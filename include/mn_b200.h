@@ -559,6 +559,45 @@ int mn_debug_tp_program_mode(const mn_model_desc* desc, int mode, unsigned int* 
 #define MN_TCL_IMG 34
 int mn_debug_tc_train_layout(const mn_model* m, int64_t B, int64_t* out, int cap);
 
+/* ---- test hook (host only, no CUDA call): where the fp32 training passes keep their intermediates ------------------------
+ * For a call of mn_model_forward_train / mn_model_backward over B rows of model m, out[] receives (indices MN_F32L_*): the
+ * slots per tape tile TM and the number of TM-slot tiles; the tiles one CTA of the weight-gradient pass sums before its fp32
+ * atomics; the tape's byte size and the byte offsets of its regions (routing counters, slot_row and slot_w or -1, the
+ * activation tape); the backward workspace's size and the byte offset of the gradient tape inside it; then the first channel
+ * of every activation-tape block (PE, aux = direction PE | embedding, trunk h_0.., F, G, rgb head output, affine Linear
+ * output, sigma pre-activation, image id) and the channels per slot, and the same for the gradient tape (dZ of every trunk
+ * layer, of F, of G, of the rgb Linear output, of the sigma pre-activation).  Channel c of slot r of tile t lies at float
+ * (t * total + c) * TM + r of its tape.  Returns MN_F32L_COUNT, or MN_ERR_WORKSPACE when cap is too small.
+ * Used by tests/test_gpu_zze_train_fp32_stages.py. */
+#define MN_F32L_TM 0
+#define MN_F32L_N_TILES 1
+#define MN_F32L_CHUNK_TILES 2
+#define MN_F32L_TAPE_BYTES 3
+#define MN_F32L_TAPE_COUNTERS 4
+#define MN_F32L_TAPE_SLOT_ROW 5
+#define MN_F32L_TAPE_SLOT_W 6
+#define MN_F32L_TAPE_ACT 7
+#define MN_F32L_BWD_BYTES 8
+#define MN_F32L_BWD_GRAD 9
+#define MN_F32L_A_PE 10
+#define MN_F32L_A_AUX 11
+#define MN_F32L_A_H 12
+#define MN_F32L_A_F 13
+#define MN_F32L_A_G 14
+#define MN_F32L_A_RGB 15
+#define MN_F32L_A_LIN 16
+#define MN_F32L_A_SIG 17
+#define MN_F32L_A_ID 18
+#define MN_F32L_A_TOTAL 19
+#define MN_F32L_G_Z 20
+#define MN_F32L_G_FINAL 21
+#define MN_F32L_G_DIRA 22
+#define MN_F32L_G_RGB 23
+#define MN_F32L_G_SIG 24
+#define MN_F32L_G_TOTAL 25
+#define MN_F32L_COUNT 26
+int mn_debug_fp32_train_layout(const mn_model* m, int64_t B, int64_t* out, int cap);
+
 /* ---- test hook: the recording forward of any network the tensor cores run --------------------------------------------
  * mn_model_forward_train_tc's forward (arguments and tape as there, laid out as mn_debug_tc_train_layout reports) for every
  * network whose tc_f16 inference runs on the tensor cores, including the shapes tensor-core training does not cover (64..192

@@ -134,6 +134,7 @@ SIGNATURES = {
     'mn_model_backward_tc': (_I, [_P, _P, _L, _I, _P, _P, _Z, _P, _P, _Z, _P]),
     'mn_debug_tc_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),
     'mn_debug_tc_forward_record': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _P, _P, _P, _Z, _P, _Z, _P]),
+    'mn_debug_fp32_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),
 }
 MN_PARAM_OFFSETS = 44
 # entries of mn_debug_tc_train_layout (MN_TCL_* in include/mn_b200.h), then 2 per record image from TCL['IMG'] on
@@ -142,6 +143,11 @@ TCL = {k: i for i, k in enumerate((
     'X_TILE', 'ACT_TILE', 'KPE', 'KAUX', 'HC', 'GC', 'F32_SIGMA', 'F32_RGB', 'F32_ID', 'F32_ROWS', 'G32_SIGMA', 'G32_RGB',
     'G32_ROWS', 'BWD_BYTES', 'BWD_DZ', 'BWD_GF32', 'BWD_EMB', 'BWD_SCALE', 'BWD_EMB_K', 'BWD_HEAD_TILES', 'BWD_DZG',
     'BWD_PP0', 'BWD_PP1', 'N_IMG', 'TRAIN', 'IMG'))}
+# entries of mn_debug_fp32_train_layout (MN_F32L_* in include/mn_b200.h)
+F32L = {k: i for i, k in enumerate((
+    'TM', 'N_TILES', 'CHUNK_TILES', 'TAPE_BYTES', 'TAPE_COUNTERS', 'TAPE_SLOT_ROW', 'TAPE_SLOT_W', 'TAPE_ACT', 'BWD_BYTES',
+    'BWD_GRAD', 'A_PE', 'A_AUX', 'A_H', 'A_F', 'A_G', 'A_RGB', 'A_LIN', 'A_SIG', 'A_ID', 'A_TOTAL', 'G_Z', 'G_FINAL', 'G_DIRA',
+    'G_RGB', 'G_SIG', 'G_TOTAL', 'COUNT'))}
 
 _lib = None
 _lock = threading.Lock()

@@ -833,6 +833,30 @@ int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const
     return mn_mlp_bwd_launch(ctx, a, slot_capacity(m, B) / MN_TILE, (cudaStream_t)stream);
 }
 
+int mn_debug_fp32_train_layout(const mn_model* m, int64_t B, int64_t* out, int cap) {
+    if (!m || !out || B < 0) return MN_ERR_INVALID;
+    if (cap < MN_F32L_COUNT) return MN_ERR_WORKSPACE;
+    const int TM = mn_tape_tm(m->nd.L);
+    char* const base = (char*)(uintptr_t)4096;      // any non-null base: tape_regions_cap returns pointers base + offset
+    TapeRegions T{};
+    auto off = [&](const void* p) -> int64_t { return p ? (int64_t)((const char*)p - base) : -1; };
+    out[MN_F32L_TM] = TM;
+    out[MN_F32L_N_TILES] = slot_capacity(m, B) / TM;
+    out[MN_F32L_CHUNK_TILES] = MN_WG_CHUNK_TILES;
+    out[MN_F32L_TAPE_BYTES] = (int64_t)tape_regions(m, B, false, base, &T);
+    out[MN_F32L_TAPE_COUNTERS] = off(T.counters);
+    out[MN_F32L_TAPE_SLOT_ROW] = off(T.slot_row);
+    out[MN_F32L_TAPE_SLOT_W] = off(T.slot_w);
+    out[MN_F32L_TAPE_ACT] = off(T.act);
+    out[MN_F32L_BWD_BYTES] = (int64_t)mn_model_backward_workspace_bytes(m, B);
+    out[MN_F32L_BWD_GRAD] = 0;                       // mn_model_backward: the gradient tape starts the workspace
+    const TapeLayout& t = m->tape;
+    const int ch[] = {t.a_pe, t.a_aux, t.a_h, t.a_f, t.a_g, t.a_rgb, t.a_lin, t.a_sig, t.a_id, t.a_total,
+                      t.g_z, t.g_final, t.g_dira, t.g_rgb, t.g_sig, t.g_total};
+    for (int i = 0; i < (int)(sizeof(ch) / sizeof(ch[0])); ++i) out[MN_F32L_A_PE + i] = ch[i];
+    return MN_F32L_COUNT;
+}
+
 // ---- tensor-core training path (precision tc_f16 for the recording forward and the backward pass) ----------------
 int mn_model_train_tc_supported(const mn_model* m) { return (m && m->train_tc_ok) ? 1 : 0; }
 

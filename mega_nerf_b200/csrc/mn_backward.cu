@@ -413,7 +413,7 @@ int mn_mlp_bwd_launch(mn_ctx* ctx, const BwdArgs& a, int64_t n_tiles128, cudaStr
     w.counters = a.counters;
     w.fixed_sub = a.fixed_sub;
     w.B = a.B;
-    w.chunk_tiles = 64;
+    w.chunk_tiles = MN_WG_CHUNK_TILES;
     const unsigned gx = (unsigned)mn_cdiv(n_tiles, w.chunk_tiles);
     const dim3 grid(gx, (unsigned)blocks, (unsigned)(a.counters ? a.n_sub : 1));
     if (TM == 64)

@@ -45,6 +45,8 @@ struct BwdLayout {
 };
 
 static inline int mn_tape_tm(int L) { return L <= 256 ? 64 : 32; }
+// TM-slot tiles one CTA of the fp32 weight-gradient kernel sums before its fp32 atomics (mlp_bwd_weight_kernel)
+#define MN_WG_CHUNK_TILES 64
 
 struct mn_model {
     mn_ctx* ctx = nullptr;
