@@ -121,6 +121,12 @@ __device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.s
 template <int N>
 __device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void st_shared_u32(unsigned char* p, uint32_t v) { *reinterpret_cast<uint32_t*>(p) = v; }
+// max(h, +0) on both halves of a packed fp16 pair (__hmax2: a NaN half gives +0, and max(-0, +0) = +0).  Rounding to fp16
+// commutes with max(., 0), so relu_h2(pack_h2(a, b)) has the bits of pack_h2(fmaxf(a, 0.0f), fmaxf(b, 0.0f)) for every a, b.
+__device__ __forceinline__ uint32_t relu_h2(uint32_t h) {
+    const __half2 r = __hmax2(*reinterpret_cast<const __half2*>(&h), __float2half2_rn(0.0f));
+    return *reinterpret_cast<const uint32_t*>(&r);
+}
 // Pins the accumulator registers at a point of the instruction stream (the compiler must not move reads or writes of them
 // across it): placed after the accumulators are initialised and after the wait that completes the MMAs writing them.
 template <int N>
@@ -626,6 +632,44 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                             }
                         };
                         constexpr int JB = NM / 8 < 8 ? NM / 8 : 8;            // column groups whose loads are issued together
+                        if constexpr (kRegAct) {
+                            // kHR: a ReLU layer without the sigma head, the ReLU on the packed fp16 pairs.  Its own copy of the
+                            // loop leaves no fp32 ReLU or sigma instructions for the compiler to predicate off: they would
+                            // still be issued.  Every column group is written, so no register keeps its old value across the
+                            // epilogue; groups past gm.n hold values that no MMA reads (the next K is at most gm.n).
+                            auto epi = [&](auto hr_tag) {
+                                constexpr bool kHR = decltype(hr_tag)::value;
+#pragma unroll
+                                for (int j0 = 0; j0 < NM / 8; j0 += JB) {
+                                    float2 bvs[JB], svs[JB];
+#pragma unroll
+                                    for (int jj = 0; jj < JB; ++jj) {
+                                        const int c = 8 * (j0 + jj) + 2 * q4;
+                                        bvs[jj] = *reinterpret_cast<const float2*>(bias + c);
+                                        svs[jj] = !kHR && want_sigma ? *reinterpret_cast<const float2*>(sw + cb + c) : make_float2(0.0f, 0.0f);
+                                    }
+#pragma unroll
+                                    for (int jj = 0; jj < JB; ++jj) {
+                                        const int j = j0 + jj;
+                                        const float2 bv = bvs[jj];
+                                        float a0 = acc[4 * j] + bv.x, a1 = acc[4 * j + 1] + bv.y, b0 = acc[4 * j + 2] + bv.x, b1 = acc[4 * j + 3] + bv.y;
+                                        if (!kHR && relu) { a0 = fmaxf(a0, 0.0f); a1 = fmaxf(a1, 0.0f); b0 = fmaxf(b0, 0.0f); b1 = fmaxf(b1, 0.0f); }
+                                        if (!kHR && want_sigma && cb + 8 * j < gm.n) {
+                                            const float2 s = svs[jj];
+                                            sacc_a = fmaf(a1, s.y, fmaf(a0, s.x, sacc_a));
+                                            sacc_b = fmaf(b1, s.y, fmaf(b0, s.x, sacc_b));
+                                        }
+                                        uint32_t ha = pack_h2(a0, a1), hb = pack_h2(b0, b1);
+                                        if constexpr (kHR) { ha = relu_h2(ha); hb = relu_h2(hb); }
+                                        hreg[2 * j] = ha;
+                                        hreg[2 * j + 1] = hb;
+                                    }
+                                }
+                            };
+                            if (relu && !want_sigma) epi(std::true_type{});
+                            else epi(std::false_type{});
+                            continue;
+                        }
 #pragma unroll
                         for (int j0 = 0; j0 < NM / 8; j0 += JB) {
                         float2 bvs[JB], svs[JB];
@@ -638,10 +682,8 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
 #pragma unroll
                         for (int jj = 0; jj < JB; ++jj) {
                             const int j = j0 + jj;
-                            // kRegAct: every column group is written, so no register keeps its old value across the
-                            // epilogue; groups past gm.n hold values that no MMA reads (the next K is at most gm.n)
                             const bool in_n = cb + 8 * j < gm.n;
-                            if (!kRegAct && !in_n) continue;
+                            if (!in_n) continue;
                             const float2 bv = bvs[jj];
                             float a0 = acc[4 * j] + bv.x, a1 = acc[4 * j + 1] + bv.y, b0 = acc[4 * j + 2] + bv.x, b1 = acc[4 * j + 3] + bv.y;
                             if (relu) { a0 = fmaxf(a0, 0.0f); a1 = fmaxf(a1, 0.0f); b0 = fmaxf(b0, 0.0f); b1 = fmaxf(b1, 0.0f); }
@@ -651,8 +693,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                                 sacc_b = fmaf(b1, s.y, fmaf(b0, s.x, sacc_b));
                             }
                             const uint32_t ha = pack_h2(a0, a1), hb = pack_h2(b0, b1);
-                            if constexpr (kRegAct) { hreg[2 * j] = ha; hreg[2 * j + 1] = hb; }
-                            else if (hold) { held[(2 * j) % (NM / 4)] = ha; held[(2 * j + 1) % (NM / 4)] = hb; }
+                            if (hold) { held[(2 * j) % (NM / 4)] = ha; held[(2 * j + 1) % (NM / 4)] = hb; }
                             else if (publish) put(cb + 8 * j + 2 * q4, ha, hb, a0, a1, b0, b1);
                         }
                         }
