@@ -450,38 +450,129 @@ static size_t tape_regions(const mn_model* m, int64_t B, bool tc, void* base, Ta
     return tape_regions_cap(m, slot_capacity(m, B), m->d.boundary_margin > 1.0f, tc, base, r);
 }
 
-// train_tc != 0: recording forward on the tensor cores (precision tc_f16) into the tensor-core tape regions; 2: the test hook's
-// recording forward (mn_debug_tc_forward_record), which also runs networks that tensor-core training does not cover.
-// live: the rows that hold data when their count lives on the device (inference only), see LiveRows.
-// mult: sub-modules per row the routing slots of this call are sized for (inference only; 0 = the model's max_multiplicity).
-static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, int sigma_only,
-                              const float* sigma_noise_d, int precision, float* out_d, void* workspace_d,
-                              size_t workspace_bytes, void* tape_d, size_t tape_bytes, void* stream, int train_tc = 0,
-                              LiveRows live = LiveRows{}, int mult = 0, const int* gather = nullptr) {
-    if (!ctx || !m || !rows || B < 0) return MN_ERR_INVALID;
-    if (gather && rows->mode != 1) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward: a row gather needs ray-structured rows");
+// The child module's shape error (models/nerf.py:121-123).
+static int shape_error(mn_ctx* ctx, int64_t rows, int cols, int expected, int xyz_dim) {
+    char buf[256];
+    snprintf(buf, sizeof(buf), "Unexpected input shape: torch.Size([%lld, %d]) (expected: %d, xyz_dim: %d)", (long long)rows, cols,
+             expected, xyz_dim);
+    return mn_fail(ctx, MN_ERR_SHAPE, buf);
+}
+
+// What a model call runs: inference at its precision, or a recording forward into the caller's tape - a training call (fp32: the
+// fp32 activation tape; tc_f16: the tensor-core records) or the test hook mn_debug_tc_forward_record (tensor-core records of every
+// network with a tensor-core forward, trained there or not).
+enum CallRun { RUN_INFER, RUN_TRAIN, RUN_TC_HOOK };
+
+// One model call, as its entry point has checked it.
+struct ModelCall {
+    RowSrc src{};
+    int64_t B = 0;                      // rows
+    int64_t cap = 0;                    // slots (slot_capacity)
+    // How rows become slots.  kind 0 / 1: every row through one sub-module (Cascade: the coarse one when use_coarse).  kind 2: the
+    // live rows routed by distance into slots sized for mult sub-modules per row, or, when id_col > 0 (the owner side of an
+    // expert-parallel query), bucketed by the sub-module id in payload column id_col (the density noise follows it if has_noise).
+    int use_coarse = 0;
+    LiveRows live{};
+    int mult = 0;
+    int id_col = 0, has_noise = 0;
+    int sigma_only = 0;
+    const float* sigma_noise = nullptr;
+    CallRun run = RUN_INFER;
+    int precision = MN_PREC_FP32;
+    TapeRegions tape{};                 // recording calls: the regions of the caller's tape
+    float* out = nullptr;
+};
+
+// Runs a checked model call: carves the workspace, builds the slots (a recording call keeps the slot mapping and this call's
+// routing counters in its tape), runs the MLP engine and combines blended rows.
+static int model_call(mn_ctx* ctx, mn_model* m, const ModelCall& c, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
     const mn_model_desc& d = m->d;
-    const NetDims& nd = m->nd;
-    cudaStream_t st = (cudaStream_t)stream;
-    const int has_dir = (!sigma_only && d.pos_dir_dim > 0) ? 1 : 0;
-    const int has_idx = (!sigma_only && d.appearance_dim > 0) ? 1 : 0;
+    const bool record = c.run != RUN_INFER;
+    MlpArgs a{};
+    a.nd = m->nd;
+    a.lay = m->lay;
+    a.packed = m->packed;
+    a.src = c.src;
+    a.n_sub = d.n_sub;
+    a.B = c.B;
+    a.sigma_only = c.sigma_only;
+    a.sigma_noise = c.sigma_noise;
+    a.out = c.out;
+    a.out_cols = c.sigma_only ? 1 : m->nd.rgb_dim + 1;
+    a.live = c.live;
+
+    char* ws = (char*)workspace_d;
+    auto carve = [&](size_t n) { char* p = ws; ws += mn_align(n); return p; };
+    int rc;
+    int* row_slots = nullptr;
+    float* slot_out = nullptr;
+    if (d.kind == 2) {
+        const bool owner = c.id_col > 0;
+        const bool blend = !owner && d.boundary_margin > 1.0f;
+        // owner training: the tape holds the slot mapping, the workspace the scratch alone, 256 bytes in
+        int* slot_row = (int*)carve(owner && record ? 256 : (size_t)c.cap * sizeof(int));
+        void* scratch = carve(owner ? mn_route_assigned_scratch_bytes(c.B) : mn_route_scratch_bytes(m, c.B));
+        float* slot_w = nullptr;
+        if (blend) {
+            slot_w = (float*)carve((size_t)c.cap * sizeof(float));
+            row_slots = (int*)carve((size_t)c.B * d.n_sub * sizeof(int));
+            slot_out = (float*)carve((size_t)c.cap * a.out_cols * sizeof(float));
+        }
+        if (record) {
+            slot_row = c.tape.slot_row;
+            slot_w = c.tape.slot_w;
+        }
+        rc = owner ? mn_route_build_assigned(ctx, m, c.src.x, c.B, c.src.cols, c.id_col, c.has_noise, c.cap, slot_row, scratch,
+                                             &a.sigma_noise, st)
+                   : mn_route_build(ctx, m, c.src, c.B, c.live, c.cap, slot_row, slot_w, row_slots, scratch, st);
+        if (rc) return rc;
+        if (record)
+            MN_CUDA(ctx, cudaMemcpyAsync(c.tape.counters, m->counters_d, CNT_TOTAL * sizeof(int), cudaMemcpyDeviceToDevice, st));
+        a.slot_row = slot_row;
+        a.slot_w = slot_w;
+        a.counters = m->counters_d;
+        a.B = c.cap;
+        a.scatter = blend ? 0 : 1;
+        if (blend) a.out = slot_out;
+    } else {
+        a.fixed_sub = (d.kind == 1) ? (c.use_coarse ? 0 : 1) : 0;
+        a.scatter = 1;
+    }
+
+    a.tape = c.tape.act;       // fp32 recording calls: the activation tape
+    if (a.tape) a.tl = m->tape;
+    const int64_t n_tiles = c.cap / MN_TILE;
+    if (record && c.precision != MN_PREC_FP32)
+        rc = mn_mlp_tc_launch_record(ctx, m, a, n_tiles, c.tape.tc, c.run == RUN_TRAIN, st);
+    else if (c.precision == MN_PREC_FP32)
+        rc = mn_mlp_simt_launch(ctx, a, n_tiles, st);
+    else
+        rc = mn_mlp_tc_launch(ctx, m, a, n_tiles, c.precision, ws, workspace_bytes - (size_t)(ws - (char*)workspace_d), st);
+    if (rc) return rc;
+    if (row_slots) return mn_route_combine(ctx, m, c.B, c.live, row_slots, slot_out, a.out_cols, c.out, st);
+    return MN_OK;
+}
+
+// A model call over mn_rows (c.src.gather: a row gather of ray-structured rows): checks the rows, the workspace and the tape (when
+// tape_d is set), then runs it.
+static int forward_rows(mn_ctx* ctx, mn_model* m, const mn_rows* rows, ModelCall c, void* workspace_d, size_t workspace_bytes,
+                        void* tape_d, size_t tape_bytes, cudaStream_t st) {
+    if (!ctx || !m || !rows || c.B < 0) return MN_ERR_INVALID;
+    if (c.src.gather && rows->mode != 1) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward: a row gather needs ray-structured rows");
+    const mn_model_desc& d = m->d;
+    const int has_dir = (!c.sigma_only && d.pos_dir_dim > 0) ? 1 : 0;
+    const int has_idx = (!c.sigma_only && d.appearance_dim > 0) ? 1 : 0;
     const int prefix = (d.kind == 2 && d.xyz_real) ? 3 : 0;
 
-    RowSrc src{};
+    RowSrc& src = c.src;
     src.xyz_dim = d.xyz_dim;
     src.net_off = prefix;
+    src.x = rows->x_d;
+    src.cols = rows->cols;
     if (rows->mode == 0) {
         const int expected = d.xyz_dim + 3 * has_dir + has_idx;
-        if (rows->cols - prefix != expected) {
-            char buf[256];
-            // the child module is what raises (models/nerf.py:121-123); it sees the row matrix minus the
-            // routing prefix, so report that shape.
-            snprintf(buf, sizeof(buf), "Unexpected input shape: torch.Size([%lld, %d]) (expected: %d, xyz_dim: %d)",
-                     (long long)B, rows->cols - prefix, expected, d.xyz_dim);
-            return mn_fail(ctx, MN_ERR_SHAPE, buf);
-        }
-        src.x = rows->x_d;
-        src.cols = rows->cols;
+        // the child module is what raises; it sees the row matrix minus the routing prefix, so report that shape.
+        if (rows->cols - prefix != expected) return shape_error(ctx, c.B, rows->cols - prefix, expected, d.xyz_dim);
         src.div = 1;
         // nerf.py:146 reads directions as x[:, -4:-1]; :149 the index as x[:, -1]
         src.dirs = rows->x_d + rows->cols - 4;
@@ -490,107 +581,42 @@ static int model_forward_impl(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
         src.idx_stride = rows->cols;
         src.dir_quirk = 0;  // the pointer arithmetic above already reproduces the slice
     } else {
-        if (rows->cols - prefix != d.xyz_dim) {
-            char buf[256];
-            snprintf(buf, sizeof(buf), "Unexpected input shape: torch.Size([%lld, %d]) (expected: %d, xyz_dim: %d)",
-                     (long long)B, rows->cols - prefix + 3 * (rows->dirs_d ? 1 : 0) + (rows->idx_d ? 1 : 0),
-                     d.xyz_dim + 3 * has_dir + has_idx, d.xyz_dim);
-            return mn_fail(ctx, MN_ERR_SHAPE, buf);
-        }
+        if (rows->cols - prefix != d.xyz_dim)
+            return shape_error(ctx, c.B, rows->cols - prefix + 3 * (rows->dirs_d ? 1 : 0) + (rows->idx_d ? 1 : 0),
+                               d.xyz_dim + 3 * has_dir + has_idx, d.xyz_dim);
         if ((has_dir && !rows->dirs_d) || (has_idx && !rows->idx_d) || rows->samples_per_ray < 1)
             return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward: ray-structured rows lack dirs / indices");
-        src.x = rows->x_d;
-        src.cols = rows->cols;
         src.div = rows->samples_per_ray;
         src.dirs = rows->dirs_d;
         src.dir_stride = rows->dir_stride;
         src.idx = rows->idx_d;
         src.idx_stride = 1;
         src.dir_quirk = (has_dir && !has_idx) ? 1 : 0;  // [xyz, dir] rows: x[:, -4:-1] = (z, dx, dy)
-        src.gather = gather;
     }
-    if (B == 0) return MN_OK;
+    if (c.B == 0) return MN_OK;
 
-    MlpArgs a{};
-    a.nd = nd;
-    a.lay = m->lay;
-    a.packed = m->packed;
-    a.src = src;
-    a.n_sub = d.n_sub;
-    a.B = B;
-    a.sigma_only = sigma_only;
-    a.sigma_noise = sigma_noise_d;
-    a.out = out_d;
-    a.out_cols = sigma_only ? 1 : nd.rgb_dim + 1;
-    a.live = live;
-
-    const int64_t cap = slot_capacity(m, B, mult);
-    const size_t need = forward_workspace_bytes(m, B, precision, mult);
+    c.cap = slot_capacity(m, c.B, c.mult);
+    // a recording call runs no tensor-core inference, so its workspace holds none
+    const size_t need = forward_workspace_bytes(m, c.B, c.run == RUN_INFER ? c.precision : MN_PREC_FP32, c.mult);
     if (need > 256 && (!workspace_d || workspace_bytes < need))
         return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward: workspace too small");
-    char* ws = (char*)workspace_d;
-    auto carve = [&](size_t n) { char* p = ws; ws += mn_align(n); return p; };
     // training forward: the routing tables and the activations outlive the call inside the caller's tape
-    TapeRegions T{};
-    if (tape_d && tape_bytes < tape_regions(m, B, train_tc != 0, tape_d, &T))
+    if (tape_d && tape_bytes < tape_regions(m, c.B, c.precision != MN_PREC_FP32, tape_d, &c.tape))
         return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward_train: tape too small");
-
-    int rc;
-    int* row_slots = nullptr;
-    float* slot_out = nullptr;
-    if (d.kind == 2) {
-        int* slot_row = (int*)carve((size_t)cap * sizeof(int));
-        void* route_scratch = carve(mn_route_scratch_bytes(m, B));
-        float* slot_w = nullptr;
-        const bool blend = d.boundary_margin > 1.0f;
-        if (blend) {
-            slot_w = (float*)carve((size_t)cap * sizeof(float));
-            row_slots = (int*)carve((size_t)B * d.n_sub * sizeof(int));
-            slot_out = (float*)carve((size_t)cap * a.out_cols * sizeof(float));
-        }
-        if (tape_d) {
-            slot_row = T.slot_row;
-            slot_w = T.slot_w;
-        }
-        if ((rc = mn_route_build(ctx, m, src, B, live, cap, slot_row, slot_w, row_slots, route_scratch, st))) return rc;
-        if (tape_d)
-            MN_CUDA(ctx, cudaMemcpyAsync(T.counters, m->counters_d, CNT_TOTAL * sizeof(int), cudaMemcpyDeviceToDevice, st));
-        a.slot_row = slot_row;
-        a.slot_w = slot_w;
-        a.counters = m->counters_d;
-        a.B = cap;
-        a.scatter = blend ? 0 : 1;
-        if (blend) a.out = slot_out;
-    } else {
-        a.fixed_sub = (d.kind == 1) ? (use_coarse ? 0 : 1) : 0;
-        a.scatter = 1;
-    }
-
-    const int64_t n_tiles = cap / MN_TILE;
-    if (tape_d && train_tc) {
-        rc = train_tc == 2 ? mn_mlp_tc_launch_record(ctx, m, a, n_tiles, T.tc, st) : mn_mlp_tc_launch_train(ctx, m, a, n_tiles, T.tc, st);
-        if (rc) return rc;
-        if (row_slots) return mn_route_combine(ctx, m, B, live, row_slots, slot_out, a.out_cols, out_d, st);
-        return MN_OK;
-    }
-    if (tape_d) {
-        a.tape = T.act;
-        a.tl = m->tape;
-    }
-    if (precision == MN_PREC_FP32)
-        rc = mn_mlp_simt_launch(ctx, a, n_tiles, st);
-    else
-        rc = mn_mlp_tc_launch(ctx, m, a, n_tiles, precision, ws, workspace_bytes - (size_t)(ws - (char*)workspace_d), st);
-    if (rc) return rc;
-    if (row_slots) return mn_route_combine(ctx, m, B, live, row_slots, slot_out, a.out_cols, out_d, st);
-    return MN_OK;
+    return model_call(ctx, m, c, workspace_d, workspace_bytes, st);
 }
 
 int mn_model_forward(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, int sigma_only,
                      const float* sigma_noise_d, int precision, float* out_d, void* workspace_d,
                      size_t workspace_bytes, void* stream) {
-    return model_forward_impl(ctx, m, rows, B, use_coarse, sigma_only, sigma_noise_d, precision, out_d, workspace_d,
-                              workspace_bytes, nullptr, 0, stream);
+    ModelCall c;
+    c.B = B;
+    c.use_coarse = use_coarse;
+    c.sigma_only = sigma_only;
+    c.sigma_noise = sigma_noise_d;
+    c.precision = precision;
+    c.out = out_d;
+    return forward_rows(ctx, m, rows, c, workspace_d, workspace_bytes, nullptr, 0, (cudaStream_t)stream);
 }
 
 // ---- owner side of an expert-parallel query (mega_nerf_b200/expert_parallel.py) ------------------------------------
@@ -604,81 +630,59 @@ size_t mn_model_forward_assigned_workspace_bytes(const mn_model* m, int64_t n, i
     return bytes;
 }
 
-// The payload rows of an owner call as the MLP kernels read them: checks the column count (the child's MN_ERR_SHAPE) and fills
-// the mode-0 RowSrc of `cols` columns inside the wider payload row - directions x[:, -4:-1], image index x[:, -1] (nerf.py:146,149).
+// The payload rows of an owner call: checks the column count (the child's MN_ERR_SHAPE) and fills the owner fields of *c - the rows,
+// the sub-module id column, and the mode-0 RowSrc of `cols` columns inside the wider payload row: directions x[:, -4:-1], image
+// index x[:, -1] (nerf.py:146,149).  Every bucketed slot runs through its own sub-module, results scattered to the rows' own indices.
 static int assigned_rows(mn_ctx* ctx, const mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, const char* who,
-                         RowSrc* src) {
+                         ModelCall* c) {
     if (m->d.kind != 2) return mn_fail(ctx, MN_ERR_INVALID, std::string(who) + ": not a MegaNeRF model");
     const mn_model_desc& d = m->d;
     const int expected = d.xyz_dim + 3 * (d.pos_dir_dim > 0 ? 1 : 0) + (d.appearance_dim > 0 ? 1 : 0);
-    if (cols != expected) {
-        char buf[256];
-        snprintf(buf, sizeof(buf), "Unexpected input shape: torch.Size([%lld, %d]) (expected: %d, xyz_dim: %d)", (long long)n, cols, expected,
-                 d.xyz_dim);
-        return mn_fail(ctx, MN_ERR_SHAPE, buf);
-    }
+    if (cols != expected) return shape_error(ctx, n, cols, expected, d.xyz_dim);
     const int stride = cols + 1 + (has_noise ? 1 : 0);
-    *src = RowSrc{};
-    src->xyz_dim = d.xyz_dim;
-    src->x = rows_d;
-    src->cols = stride;
-    src->div = 1;
-    src->dirs = rows_d + cols - 4;
-    src->dir_stride = stride;
-    src->idx = rows_d + cols - 1;
-    src->idx_stride = stride;
+    RowSrc& src = c->src;
+    src.xyz_dim = d.xyz_dim;
+    src.x = rows_d;
+    src.cols = stride;
+    src.div = 1;
+    src.dirs = rows_d + cols - 4;
+    src.dir_stride = stride;
+    src.idx = rows_d + cols - 1;
+    src.idx_stride = stride;
+    c->B = n;
+    c->id_col = cols;
+    c->has_noise = has_noise;
     return MN_OK;
-}
-
-// MlpArgs of an owner call: every bucketed slot through its own sub-module, results scattered to the rows' own indices.
-static MlpArgs assigned_args(const mn_model* m, const RowSrc& src, int64_t cap, const int* slot_row, const float* noise, float* out_d) {
-    MlpArgs a{};
-    a.nd = m->nd;
-    a.lay = m->lay;
-    a.packed = m->packed;
-    a.src = src;
-    a.n_sub = m->d.n_sub;
-    a.B = cap;
-    a.sigma_noise = noise;
-    a.out = out_d;
-    a.out_cols = m->nd.rgb_dim + 1;
-    a.slot_row = slot_row;
-    a.counters = m->counters_d;
-    a.scatter = 1;
-    return a;
 }
 
 int mn_model_forward_assigned(mn_ctx* ctx, mn_model* m, const float* rows_d, int64_t n, int cols, int has_noise, int precision,
                               float* out_d, void* workspace_d, size_t workspace_bytes, void* stream) {
     if (!ctx || !m || n < 0 || cols < 1) return MN_ERR_INVALID;
-    RowSrc src;
+    ModelCall c;
     int rc;
-    if ((rc = assigned_rows(ctx, m, rows_d, n, cols, has_noise, "mn_model_forward_assigned", &src))) return rc;
+    if ((rc = assigned_rows(ctx, m, rows_d, n, cols, has_noise, "mn_model_forward_assigned", &c))) return rc;
     if (n == 0) return MN_OK;
     if (!rows_d || !out_d) return MN_ERR_INVALID;
     if (!workspace_d || workspace_bytes < mn_model_forward_assigned_workspace_bytes(m, n, precision))
         return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_forward_assigned: workspace too small");
-    cudaStream_t st = (cudaStream_t)stream;
-    const int64_t cap = slot_capacity(m, n, 1);
-    char* ws = (char*)workspace_d;
-    auto carve = [&](size_t b) { char* p = ws; ws += mn_align(b); return p; };
-    int* slot_row = (int*)carve((size_t)cap * sizeof(int));
-    void* scratch = carve(mn_route_assigned_scratch_bytes(n));
-    const float* noise = nullptr;
-    if ((rc = mn_route_build_assigned(ctx, m, rows_d, n, src.cols, cols, has_noise, cap, slot_row, scratch, &noise, st))) return rc;
-
-    const MlpArgs a = assigned_args(m, src, cap, slot_row, noise, out_d);
-    const int64_t n_tiles = cap / MN_TILE;
-    if (precision == MN_PREC_FP32) return mn_mlp_simt_launch(ctx, a, n_tiles, st);
-    return mn_mlp_tc_launch(ctx, m, a, n_tiles, precision, ws, workspace_bytes - (size_t)(ws - (char*)workspace_d), st);
+    c.cap = slot_capacity(m, n, 1);
+    c.precision = precision;
+    c.out = out_d;
+    return model_call(ctx, m, c, workspace_d, workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"
 
 int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,
                           float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st, const int* gather) {
-    return model_forward_impl(ctx, m, rows, B, use_coarse, 0, nullptr, precision, out_d, workspace_d, workspace_bytes, nullptr, 0, st,
-                              0, live, 0, gather);
+    ModelCall c;
+    c.src.gather = gather;
+    c.B = B;
+    c.use_coarse = use_coarse;
+    c.live = live;
+    c.precision = precision;
+    c.out = out_d;
+    return forward_rows(ctx, m, rows, c, workspace_d, workspace_bytes, nullptr, 0, st);
 }
 
 // ---- density grid (scripts/create_octree.py:61-105, 139-162) -------------------------------------------------------
@@ -741,15 +745,21 @@ int mn_model_density_grid(mn_ctx* ctx, mn_model* m, int use_coarse, const float 
     rows.mode = 0;
     rows.x_d = pts;
     rows.cols = 3;
+    ModelCall c;
+    c.use_coarse = use_coarse;
+    c.sigma_only = 1;
+    // a dense box reaches past the centroid hull, where more sub-modules blend than max_multiplicity assumes: size the slots of
+    // every slab for all of them
+    c.mult = m->d.n_sub;
+    c.precision = precision;
     for (int64_t s = 0; s < n_rows; s += MN_GRID_SLAB) {
         const int64_t n = n_rows - s < MN_GRID_SLAB ? n_rows - s : MN_GRID_SLAB;
         lattice_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, st>>>(row0 + s, n, reso, offset[0], offset[1], offset[2], scale[0], scale[1],
                                                                    scale[2], pts);
         MN_LAUNCH_CHECK(ctx);
-        // a dense box reaches past the centroid hull, where more sub-modules blend than max_multiplicity assumes: size this call's
-        // slots for all of them
-        const int rc = model_forward_impl(ctx, m, &rows, n, use_coarse, 1, nullptr, precision, sigma_out_d + s, (char*)workspace_d + pts_bytes,
-                                          workspace_bytes - pts_bytes, nullptr, 0, stream, 0, LiveRows{}, m->d.n_sub);
+        c.B = n;
+        c.out = sigma_out_d + s;
+        const int rc = forward_rows(ctx, m, &rows, c, (char*)workspace_d + pts_bytes, workspace_bytes - pts_bytes, nullptr, 0, st);
         if (rc) return rc;
     }
     return MN_OK;
@@ -762,16 +772,23 @@ int mn_model_forward_train(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_
                            const float* sigma_noise_d, float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d,
                            size_t workspace_bytes, void* stream) {
     if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_train: tape is NULL");
-    return model_forward_impl(ctx, m, rows, B, use_coarse, 0, sigma_noise_d, MN_PREC_FP32, out_d, workspace_d,
-                              workspace_bytes, tape_d, tape_bytes, stream);
+    ModelCall c;
+    c.B = B;
+    c.use_coarse = use_coarse;
+    c.sigma_noise = sigma_noise_d;
+    c.run = RUN_TRAIN;
+    c.out = out_d;
+    return forward_rows(ctx, m, rows, c, workspace_d, workspace_bytes, tape_d, tape_bytes, (cudaStream_t)stream);
 }
 
-size_t mn_model_backward_workspace_bytes(const mn_model* m, int64_t B) {
-    if (!m) return 0;
-    const int64_t cap = slot_capacity(m, B);
+// Workspace of a backward pass over `cap` slots: the fp32 gradient tape, or what the tensor-core pass carves (tc).
+static size_t backward_workspace_bytes(const mn_model* m, int64_t cap, bool tc) {
+    if (tc) return 256 + mn_train_tc_backward_workspace(m, cap / MN_TILE);
     const int TM = mn_tape_tm(m->nd.L);
     return 256 + mn_align((size_t)(cap / TM) * m->tape.g_total * TM * sizeof(float));
 }
+
+size_t mn_model_backward_workspace_bytes(const mn_model* m, int64_t B) { return m ? backward_workspace_bytes(m, slot_capacity(m, B), false) : 0; }
 
 int64_t mn_model_grad_floats(const mn_model* m) { return m ? (int64_t)m->d.n_sub * m->lay.total : 0; }
 
@@ -790,10 +807,9 @@ int mn_model_param_offsets(const mn_model* m, int64_t* out, int n) {
     return MN_OK;
 }
 
-// BwdArgs fields common to both backward passes; routed models read the slot mapping and counters the forward pass saved
-// in the tape, the others run every row through one sub-module.
-static BwdArgs bwd_args(const mn_model* m, int64_t B, int use_coarse, const float* grad_out_d, float* param_grads_d,
-                        const TapeRegions& T) {
+// BwdArgs of a backward pass over B rows and `cap` slots; routed models run the slots their forward pass built (model_backward
+// points them at the slot mapping and counters saved in the tape), the others run every row through one sub-module.
+static BwdArgs bwd_args(const mn_model* m, int64_t B, int64_t cap, int use_coarse, const float* grad_out_d, float* param_grads_d) {
     const mn_model_desc& d = m->d;
     BwdArgs a{};
     a.nd = m->nd;
@@ -802,52 +818,65 @@ static BwdArgs bwd_args(const mn_model* m, int64_t B, int use_coarse, const floa
     a.packed = m->packed;
     a.packed_bwd = m->packed_bwd;
     a.n_sub = d.n_sub;
-    a.B = B;
+    a.B = d.kind == 2 ? cap : B;
     a.grad_out = grad_out_d;
+    a.grad_rows = B;
     a.out_cols = m->nd.rgb_dim + 1;
     a.gw = param_grads_d;
-    if (d.kind == 2) {
+    if (d.kind != 2) a.fixed_sub = (d.kind == 1) ? (use_coarse ? 0 : 1) : 0;
+    return a;
+}
+
+// The backward pass of a recording call over `cap` slots: checks the tape and the workspace, then runs the fp32 kernels or the
+// tensor-core pass (tc).  owner: the tape of an owner call, which holds no blend weights.  The tensor-core pass checks its
+// workspace itself; owner calls hold it to the size mn_model_backward_assigned_workspace_bytes returns.
+static int model_backward(mn_ctx* ctx, mn_model* m, BwdArgs a, int64_t cap, bool owner, bool tc, const void* tape_d,
+                          size_t tape_bytes, void* workspace_d, size_t workspace_bytes, const char* who, cudaStream_t st) {
+    TapeRegions T;
+    if (tape_bytes < tape_regions_cap(m, cap, !owner && m->d.boundary_margin > 1.0f, tc, const_cast<void*>(tape_d), &T))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": tape too small");
+    if ((owner || !tc) && (!workspace_d || workspace_bytes < backward_workspace_bytes(m, cap, tc)))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": workspace too small");
+    if (m->d.kind == 2) {
         a.slot_row = T.slot_row;
         a.slot_w = T.slot_w;
         a.counters = T.counters;
-        a.B = slot_capacity(m, B);
-    } else {
-        a.fixed_sub = (d.kind == 1) ? (use_coarse ? 0 : 1) : 0;
     }
-    return a;
+    if (tc) return mn_train_tc_backward(ctx, m, a, cap / MN_TILE, T.tc, workspace_d, workspace_bytes, st);
+    a.tl = m->tape;
+    a.act = T.act;
+    a.grad = (float*)workspace_d;
+    return mn_mlp_bwd_launch(ctx, a, cap / MN_TILE, st);
 }
 
 int mn_model_backward(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const float* grad_out_d, const void* tape_d,
                       size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream) {
     if (!ctx || !m || B < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;
     if (B == 0) return MN_OK;
-    TapeRegions T;
-    if (tape_bytes < tape_regions(m, B, false, const_cast<void*>(tape_d), &T))
-        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward: tape too small");
-    if (!workspace_d || workspace_bytes < mn_model_backward_workspace_bytes(m, B))
-        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward: workspace too small");
-    BwdArgs a = bwd_args(m, B, use_coarse, grad_out_d, param_grads_d, T);
-    a.tl = m->tape;
-    a.act = T.act;
-    a.grad = (float*)workspace_d;
-    return mn_mlp_bwd_launch(ctx, a, slot_capacity(m, B) / MN_TILE, (cudaStream_t)stream);
+    const int64_t cap = slot_capacity(m, B);
+    return model_backward(ctx, m, bwd_args(m, B, cap, use_coarse, grad_out_d, param_grads_d), cap, false, false, tape_d, tape_bytes,
+                          workspace_d, workspace_bytes, "mn_model_backward", (cudaStream_t)stream);
+}
+
+// The layout test hooks' view of the tape of a B-row call: out[0] its size, then the offsets of its regions (-1: absent) - counters,
+// slot_row, slot_w, then the fp32 activations, or the tensor-core encoder tiles, activation records and fp32 head blocks (tc).
+static_assert(MN_F32L_TAPE_ACT == MN_F32L_TAPE_BYTES + 4 && MN_TCL_TAPE_F32 == MN_TCL_TAPE_BYTES + 6, "tape_layout's order");
+static void tape_layout(const mn_model* m, int64_t B, bool tc, int64_t* out) {
+    char* const base = (char*)(uintptr_t)4096;      // any non-null base: tape_regions_cap returns pointers base + offset
+    TapeRegions T{};
+    out[0] = (int64_t)tape_regions(m, B, tc, base, &T);
+    const void* const p[] = {T.counters, T.slot_row, T.slot_w, tc ? (const void*)T.tc.xreg : T.act, T.tc.act, T.tc.f32};
+    for (int i = 0; i < (tc ? 6 : 4); ++i) out[1 + i] = p[i] ? (int64_t)((const char*)p[i] - base) : -1;
 }
 
 int mn_debug_fp32_train_layout(const mn_model* m, int64_t B, int64_t* out, int cap) {
     if (!m || !out || B < 0) return MN_ERR_INVALID;
     if (cap < MN_F32L_COUNT) return MN_ERR_WORKSPACE;
     const int TM = mn_tape_tm(m->nd.L);
-    char* const base = (char*)(uintptr_t)4096;      // any non-null base: tape_regions_cap returns pointers base + offset
-    TapeRegions T{};
-    auto off = [&](const void* p) -> int64_t { return p ? (int64_t)((const char*)p - base) : -1; };
     out[MN_F32L_TM] = TM;
     out[MN_F32L_N_TILES] = slot_capacity(m, B) / TM;
     out[MN_F32L_CHUNK_TILES] = MN_WG_CHUNK_TILES;
-    out[MN_F32L_TAPE_BYTES] = (int64_t)tape_regions(m, B, false, base, &T);
-    out[MN_F32L_TAPE_COUNTERS] = off(T.counters);
-    out[MN_F32L_TAPE_SLOT_ROW] = off(T.slot_row);
-    out[MN_F32L_TAPE_SLOT_W] = off(T.slot_w);
-    out[MN_F32L_TAPE_ACT] = off(T.act);
+    tape_layout(m, B, false, out + MN_F32L_TAPE_BYTES);
     out[MN_F32L_BWD_BYTES] = (int64_t)mn_model_backward_workspace_bytes(m, B);
     out[MN_F32L_BWD_GRAD] = 0;                       // mn_model_backward: the gradient tape starts the workspace
     const TapeLayout& t = m->tape;
@@ -867,38 +896,38 @@ int mn_model_forward_train_tc(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
                               size_t workspace_bytes, void* stream) {
     if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_train_tc: tape is NULL");
     if (!m || !m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
-    return model_forward_impl(ctx, m, rows, B, use_coarse, 0, sigma_noise_d, MN_PREC_FP32, out_d, workspace_d, workspace_bytes, tape_d,
-                              tape_bytes, stream, 1);
+    ModelCall c;
+    c.B = B;
+    c.use_coarse = use_coarse;
+    c.sigma_noise = sigma_noise_d;
+    c.run = RUN_TRAIN;
+    c.precision = MN_PREC_TC_F16;
+    c.out = out_d;
+    return forward_rows(ctx, m, rows, c, workspace_d, workspace_bytes, tape_d, tape_bytes, (cudaStream_t)stream);
 }
 
 int mn_debug_tc_forward_record(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, const float* sigma_noise_d,
                                float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes, void* stream) {
     if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_debug_tc_forward_record: tape is NULL");
-    return model_forward_impl(ctx, m, rows, B, use_coarse, 0, sigma_noise_d, MN_PREC_FP32, out_d, workspace_d, workspace_bytes, tape_d,
-                              tape_bytes, stream, 2);
+    ModelCall c;
+    c.B = B;
+    c.use_coarse = use_coarse;
+    c.sigma_noise = sigma_noise_d;
+    c.run = RUN_TC_HOOK;
+    c.precision = MN_PREC_TC_F16;
+    c.out = out_d;
+    return forward_rows(ctx, m, rows, c, workspace_d, workspace_bytes, tape_d, tape_bytes, (cudaStream_t)stream);
 }
 
-size_t mn_model_backward_workspace_bytes_tc(const mn_model* m, int64_t B) {
-    if (!m) return 0;
-    return 256 + mn_train_tc_backward_workspace(m, slot_capacity(m, B) / MN_TILE);
-}
+size_t mn_model_backward_workspace_bytes_tc(const mn_model* m, int64_t B) { return m ? backward_workspace_bytes(m, slot_capacity(m, B), true) : 0; }
 
 int mn_debug_tc_train_layout(const mn_model* m, int64_t B, int64_t* out, int cap) {
     if (!m || !out || B < 0) return MN_ERR_INVALID;
     const int64_t n_tiles = slot_capacity(m, B) / MN_TILE;
     const int rc = mn_train_tc_layout(m, n_tiles, out, cap);
     if (rc) return rc;
-    char* const base = (char*)(uintptr_t)4096;      // any non-null base: tape_regions_cap returns pointers base + offset
-    TapeRegions T{};
     out[MN_TCL_N_TILES] = n_tiles;
-    out[MN_TCL_TAPE_BYTES] = (int64_t)tape_regions(m, B, true, base, &T);
-    auto off = [&](const void* p) -> int64_t { return p ? (int64_t)((const char*)p - base) : -1; };
-    out[MN_TCL_TAPE_COUNTERS] = off(T.counters);
-    out[MN_TCL_TAPE_SLOT_ROW] = off(T.slot_row);
-    out[MN_TCL_TAPE_SLOT_W] = off(T.slot_w);
-    out[MN_TCL_TAPE_XREG] = off(T.tc.xreg);
-    out[MN_TCL_TAPE_ACT] = off(T.tc.act);
-    out[MN_TCL_TAPE_F32] = off(T.tc.f32);
+    tape_layout(m, B, true, out + MN_TCL_TAPE_BYTES);
     out[MN_TCL_BWD_BYTES] = (int64_t)mn_model_backward_workspace_bytes_tc(m, B);
     return MN_TCL_IMG + 2 * (int)out[MN_TCL_N_IMG];
 }
@@ -908,12 +937,9 @@ int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, co
     if (!ctx || !m || B < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;
     if (B == 0) return MN_OK;
     if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_model_backward_tc: unsupported network shape");
-    TapeRegions T;
-    if (tape_bytes < tape_regions(m, B, true, const_cast<void*>(tape_d), &T))
-        return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_model_backward_tc: tape too small");
-    BwdArgs a = bwd_args(m, B, use_coarse, grad_out_d, param_grads_d, T);
-    a.grad_rows = B;
-    return mn_train_tc_backward(ctx, m, a, slot_capacity(m, B) / MN_TILE, T.tc, workspace_d, workspace_bytes, (cudaStream_t)stream);
+    const int64_t cap = slot_capacity(m, B);
+    return model_backward(ctx, m, bwd_args(m, B, cap, use_coarse, grad_out_d, param_grads_d), cap, false, true, tape_d, tape_bytes,
+                          workspace_d, workspace_bytes, "mn_model_backward_tc", (cudaStream_t)stream);
 }
 
 // ---- training on the owner side of an expert-parallel query ------------------------------------------------------------
@@ -941,40 +967,30 @@ int mn_model_forward_assigned_train(mn_ctx* ctx, mn_model* m, const float* rows_
                                     void* stream) {
     if (!ctx || !m || n < 0 || cols < 1 || max_pairs < 0) return MN_ERR_INVALID;
     const char* who = "mn_model_forward_assigned_train";
-    RowSrc src;
+    ModelCall c;
     int rc;
-    if ((rc = assigned_rows(ctx, m, rows_d, n, cols, has_noise, who, &src))) return rc;
+    if ((rc = assigned_rows(ctx, m, rows_d, n, cols, has_noise, who, &c))) return rc;
     if ((rc = assigned_train_prec(ctx, m, precision, who))) return rc;
     if (n == 0) return MN_OK;
     if (!rows_d || !out_d || !tape_d) return mn_fail(ctx, MN_ERR_INVALID, std::string(who) + ": missing buffer");
-    const bool tc = precision == MN_PREC_TC_F16;
-    const int64_t cap = slot_capacity(m, max_pairs, 1);
-    TapeRegions T;
-    if (tape_bytes < tape_regions_cap(m, cap, false, tc, tape_d, &T)) return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": tape too small");
+    c.cap = slot_capacity(m, max_pairs, 1);
+    if (tape_bytes < tape_regions_cap(m, c.cap, false, precision != MN_PREC_FP32, tape_d, &c.tape))
+        return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": tape too small");
     if (!workspace_d || workspace_bytes < mn_model_forward_assigned_train_workspace_bytes(m, n))
         return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": workspace too small");
     cudaStream_t st = (cudaStream_t)stream;
     // rows whose pair finds no slot (more pairs than max_pairs: the scatter pass drops them and sets MN_STATUS_OVERFLOW) keep this
     // NaN, as do the empty rows (id -1); every other row is written by the MLP
     MN_CUDA(ctx, cudaMemsetAsync(out_d, 0xFF, (size_t)n * (m->nd.rgb_dim + 1) * sizeof(float), st));
-    const float* noise = nullptr;
-    if ((rc = mn_route_build_assigned(ctx, m, rows_d, n, src.cols, cols, has_noise, cap, T.slot_row, (char*)workspace_d + 256, &noise, st)))
-        return rc;
-    MN_CUDA(ctx, cudaMemcpyAsync(T.counters, m->counters_d, CNT_TOTAL * sizeof(int), cudaMemcpyDeviceToDevice, st));
-    MlpArgs a = assigned_args(m, src, cap, T.slot_row, noise, out_d);
-    const int64_t n_tiles = cap / MN_TILE;
-    if (tc) return mn_mlp_tc_launch_train(ctx, m, a, n_tiles, T.tc, st);
-    a.tape = T.act;
-    a.tl = m->tape;
-    return mn_mlp_simt_launch(ctx, a, n_tiles, st);
+    c.run = RUN_TRAIN;
+    c.precision = precision;
+    c.out = out_d;
+    return model_call(ctx, m, c, workspace_d, workspace_bytes, st);
 }
 
 size_t mn_model_backward_assigned_workspace_bytes(const mn_model* m, int64_t max_pairs, int precision) {
     if (!m || max_pairs < 0) return 0;
-    const int64_t cap = slot_capacity(m, max_pairs, 1);
-    if (precision != MN_PREC_FP32) return 256 + mn_train_tc_backward_workspace(m, cap / MN_TILE);
-    const int TM = mn_tape_tm(m->nd.L);
-    return 256 + mn_align((size_t)(cap / TM) * m->tape.g_total * TM * sizeof(float));
+    return backward_workspace_bytes(m, slot_capacity(m, max_pairs, 1), precision != MN_PREC_FP32);
 }
 
 int mn_model_backward_assigned(mn_ctx* ctx, mn_model* m, int64_t n, int64_t max_pairs, int precision, const float* grad_out_d,
@@ -986,21 +1002,9 @@ int mn_model_backward_assigned(mn_ctx* ctx, mn_model* m, int64_t n, int64_t max_
     int rc;
     if ((rc = assigned_train_prec(ctx, m, precision, who))) return rc;
     if (n == 0) return MN_OK;
-    const bool tc = precision == MN_PREC_TC_F16;
     const int64_t cap = slot_capacity(m, max_pairs, 1);
-    TapeRegions T;
-    if (tape_bytes < tape_regions_cap(m, cap, false, tc, const_cast<void*>(tape_d), &T))
-        return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": tape too small");
-    if (!workspace_d || workspace_bytes < mn_model_backward_assigned_workspace_bytes(m, max_pairs, precision))
-        return mn_fail(ctx, MN_ERR_WORKSPACE, std::string(who) + ": workspace too small");
-    BwdArgs a = bwd_args(m, n, 0, grad_out_d, param_grads_d, T);
-    a.B = cap;
-    a.grad_rows = n;
-    if (tc) return mn_train_tc_backward(ctx, m, a, cap / MN_TILE, T.tc, workspace_d, workspace_bytes, (cudaStream_t)stream);
-    a.tl = m->tape;
-    a.act = T.act;
-    a.grad = (float*)workspace_d;
-    return mn_mlp_bwd_launch(ctx, a, cap / MN_TILE, (cudaStream_t)stream);
+    return model_backward(ctx, m, bwd_args(m, n, cap, 0, grad_out_d, param_grads_d), cap, true, precision != MN_PREC_FP32, tape_d,
+                          tape_bytes, workspace_d, workspace_bytes, who, (cudaStream_t)stream);
 }
 
 int mn_model_last_stats(mn_ctx* ctx, mn_model* m, int64_t* slots, int64_t* tiles, void* stream) {

@@ -921,9 +921,18 @@ size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
     return mn_tc_img_off(m->nd.layers + 1, net.lin.hc) + mn_tc_img_off(1, net.lin.gc);     // ends with G (L/2 columns, padded)
 }
 
-// recording forward of either engine: encoder tiles and every layer's activations land in the caller's tape
-static int tc_record_forward(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet& net, int64_t n_tiles128, const TrainTcTape& tape,
-                             cudaStream_t st) {
+// Recording forward of either engine: encoder tiles and every layer's activations land in the caller's tape.  train: a training
+// call, whose caller has checked m->train_tc_ok; the first one allocates and packs the transposed images of the backward pass.
+// !train: the test hook mn_debug_tc_forward_record, for every network the tensor cores serve, trained there or not; it needs no
+// transposed images, so none are allocated.
+int mn_mlp_tc_launch_record(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, bool train,
+                            cudaStream_t st) {
+    const TcNet net = tc_net(*m);
+    if (!train && (net.engine == TC_NONE || !m->tc_ready))
+        return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_debug_tc_forward_record: the network has no tensor-core forward");
+    if (n_tiles128 <= 0) return MN_OK;
+    int rc;
+    if (train && (rc = tc_dgrad_ready(ctx, m, net, st))) return rc;
     if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net, n_tiles128, MN_PREC_TC_F16, nullptr, 0, st, &tape);
     TcArgs A = tc_forward_args(m, net.P, a, n_tiles128);
     A.ximg = reinterpret_cast<const __half*>(tape.xreg);
@@ -932,31 +941,12 @@ static int tc_record_forward(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const T
     A.tape_f32 = tape.f32;
     A.act_tile_bytes = (int64_t)mn_train_tc_act_tile_bytes(m);
     A.layers = a.nd.layers;
-    int rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st);
-    if (rc) return rc;
+    if ((rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st))) return rc;
     mn_prof_begin(ctx, st);
     if (A.plan.L > 256) rc = wg_launch<PP_TRAIN_FWD, false, true>(ctx, A, n_tiles128, st);
     else rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
     mn_prof_end(ctx, st);
     return rc;
-}
-
-int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
-    if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
-    if (n_tiles128 <= 0) return MN_OK;
-    const TcNet net = tc_net(*m);
-    const int rc = tc_dgrad_ready(ctx, m, net, st);
-    if (rc) return rc;
-    return tc_record_forward(ctx, m, a, net, n_tiles128, tape, st);
-}
-
-// Test hook (mn_debug_tc_forward_record): the same recording forward for every network the tensor cores serve, trained there or
-// not.  It needs no transposed images, so none are allocated.
-int mn_mlp_tc_launch_record(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st) {
-    const TcNet net = tc_net(*m);
-    if (net.engine == TC_NONE || !m->tc_ready) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_debug_tc_forward_record: the network has no tensor-core forward");
-    if (n_tiles128 <= 0) return MN_OK;
-    return tc_record_forward(ctx, m, a, net, n_tiles128, tape, st);
 }
 
 // backward workspace: [gradient images][head gradients fp32 [head_tiles][mn_tc_g32_rows(rgb_dim)][128]][embedding sums][scale,

@@ -213,9 +213,10 @@ struct TrainTcTape {
     "rgb_dim 3 or a raw SH head (rgb_dim <= 80: sh_deg <= 4), no affine appearance; use train precision 'fp32'"
 size_t mn_train_tc_x_tile_bytes(const mn_model* m);
 size_t mn_train_tc_act_tile_bytes(const mn_model* m);
-int mn_mlp_tc_launch_train(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st);
-// the same recording forward for any network with a tensor-core forward, without the training checks (test hook)
-int mn_mlp_tc_launch_record(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, cudaStream_t st);
+// the recording forward into `tape`: of a training call (train, the caller has checked train_tc_ok) or of the test hook, which
+// runs every network with a tensor-core forward
+int mn_mlp_tc_launch_record(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, bool train,
+                            cudaStream_t st);
 size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128);
 // host only (test hook mn_debug_tc_train_layout): the entries MN_TCL_ENGINE .. that the engine decides
 int mn_train_tc_layout(const mn_model* m, int64_t n_tiles128, int64_t* out, int cap);

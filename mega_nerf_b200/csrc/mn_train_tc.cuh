@@ -22,7 +22,7 @@
 //             (appearance embedding: W_e^T times the per-image sums of dZ_dira rows collected by the dgrad head stage).
 //
 // Host side (mn_mlp_tc.cu): build_dgrad_plan (the data-gradient chain and the layout of the transposed images,
-// packed by tc_dgrad_ready / tc_pack_dgrad), mn_mlp_tc_launch_train and mn_train_tc_backward, shared with the layer-GEMM engine.
+// packed by tc_dgrad_ready / tc_pack_dgrad), mn_mlp_tc_launch_record and mn_train_tc_backward, shared with the layer-GEMM engine.
 #pragma once
 
 // max |g| over the upstream gradient, spread over the machine (an SH head's grad_out has 28 columns per row): every block
