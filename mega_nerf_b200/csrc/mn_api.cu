@@ -143,6 +143,7 @@ void build_layout(mn_model* m) {
     bl.dira_f = take(nd.has_dir_a ? (nd.L / 2) * nd.L : 0);
     bl.dira_e = take(nd.app_in_dira ? (nd.L / 2) * nd.app : 0);
     bl.total = off > 0 ? off : 4;
+    m->tc = tc_net(*m);      // the tensor-core plan, from the layouts above
 }
 
 }  // namespace
@@ -434,8 +435,8 @@ static size_t tape_regions_cap(const mn_model* m, int64_t cap, bool with_w, bool
     }
     if (tc) {
         const int64_t n_tiles = cap / MN_TILE;
-        t.tc.xreg = (unsigned char*)take((size_t)n_tiles * mn_train_tc_x_tile_bytes(m));
-        t.tc.act = (unsigned char*)take((size_t)n_tiles * mn_train_tc_act_tile_bytes(m));
+        t.tc.xreg = (unsigned char*)take((size_t)n_tiles * m->tc.P.x_tile_bytes);
+        t.tc.act = (unsigned char*)take((size_t)n_tiles * m->tc.act_tile_bytes);
         t.tc.f32 = (float*)take((size_t)n_tiles * MN_TC_F32_ROWS * MN_TILE * sizeof(float));
     } else {
         const int TM = mn_tape_tm(m->nd.L);
@@ -887,7 +888,7 @@ int mn_debug_fp32_train_layout(const mn_model* m, int64_t B, int64_t* out, int c
 }
 
 // ---- tensor-core training path (precision tc_f16 for the recording forward and the backward pass) ----------------
-int mn_model_train_tc_supported(const mn_model* m) { return (m && m->train_tc_ok) ? 1 : 0; }
+int mn_model_train_tc_supported(const mn_model* m) { return (m && m->tc.train && m->tc_packed) ? 1 : 0; }
 
 size_t mn_model_tape_bytes_tc(const mn_model* m, int64_t B) { return m ? tape_regions(m, B, true, nullptr) : 0; }
 
@@ -895,7 +896,7 @@ int mn_model_forward_train_tc(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
                               const float* sigma_noise_d, float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d,
                               size_t workspace_bytes, void* stream) {
     if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_train_tc: tape is NULL");
-    if (!m || !m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
+    if (!mn_model_train_tc_supported(m)) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
     ModelCall c;
     c.B = B;
     c.use_coarse = use_coarse;
@@ -936,7 +937,7 @@ int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, co
                          size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream) {
     if (!ctx || !m || B < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;
     if (B == 0) return MN_OK;
-    if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_model_backward_tc: unsupported network shape");
+    if (!mn_model_train_tc_supported(m)) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_model_backward_tc: unsupported network shape");
     const int64_t cap = slot_capacity(m, B);
     return model_backward(ctx, m, bwd_args(m, B, cap, use_coarse, grad_out_d, param_grads_d), cap, false, true, tape_d, tape_bytes,
                           workspace_d, workspace_bytes, "mn_model_backward_tc", (cudaStream_t)stream);
@@ -948,7 +949,7 @@ int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, co
 static int assigned_train_prec(mn_ctx* ctx, const mn_model* m, int precision, const char* who) {
     if (precision == MN_PREC_FP32) return MN_OK;
     if (precision != MN_PREC_TC_F16) return mn_fail(ctx, MN_ERR_INVALID, std::string(who) + ": training precision is fp32 or tc_f16");
-    if (!m->train_tc_ok) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
+    if (!mn_model_train_tc_supported(m)) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
     return MN_OK;
 }
 

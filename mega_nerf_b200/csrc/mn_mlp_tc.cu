@@ -19,7 +19,7 @@
 // Every other network of 64..4096 wide and 1..16 trunk layers, and the spherical-harmonics heads of degree 3 and 4 (rgb_dim 48,
 // 75) at any width, run on the layer-GEMM engine instead (mn_layer_gemm.cuh).  Host side: tc_linears lists the
 // network's Linears once; tc_net picks the engine and the training coverage from that table, and builds the forward plan of
-// either engine (build_plan) and the data-gradient plan (build_dgrad_plan); every entry point below calls it once.
+// either engine (build_plan) and the data-gradient plan (build_dgrad_plan), once per model (mn_model::tc, build_layout).
 // mn_mlp_tc_pack writes the forward images of either engine, tc_dgrad_ready / tc_pack_dgrad the transposed images of the
 // backward, and mn_train_tc_backward runs the backward of either engine between one shared workspace carve, gradient scale
 // and head / embedding epilogue.
@@ -33,40 +33,10 @@
 namespace {
 
 constexpr int kTileM = MN_TILE;
-constexpr int kMaxGemm = MN_MAX_LAYERS + 2;     // layer engine: every trunk layer, xyz_encoding_final and dir_a_encoding
 
-enum { SRC_H = 0, SRC_XPE = 1, SRC_XAUX = 2 };
-enum { EPI_RELU = 0, EPI_RELU_SIGMA = 1, EPI_LINEAR = 2, EPI_RGB = 3,
-       // data-gradient chain (training, mn_train_tc.cuh): plain copy, ReLU mask from the activation tape, mask + sigma-head term
-       EPI_D_LINEAR = 4, EPI_D_MASK = 5, EPI_D_MASK_SIGMA = 6 };
 // kernel modes of tc_mlp_wg_kernel (the test hook mn_debug_tp_program_mode names them MN_TP_*)
 enum { PP_INFER = 0, PP_TRAIN_FWD = 1, PP_DGRAD = 2 };
 static_assert(PP_INFER == MN_TP_INFER && PP_TRAIN_FWD == MN_TP_TRAIN_FWD && PP_DGRAD == MN_TP_DGRAD, "mn_debug_tp_program_mode modes");
-
-struct TcGemm {
-    int n;           // MMA N = columns of the weight image (layer engine: the output columns padded to 256-column blocks)
-    int nseg;
-    int src[2];
-    int k[2];        // padded K columns per segment (multiple of 16)
-    int w_off;       // byte offset of the weight image inside one precision plane of a sub-module
-    int bias_off;    // float offset inside the sub-module's fp32 block
-    int img;         // data-gradient plan: tape image of the output (ReLU mask read from the activation record, dZ written)
-    int epi;
-};
-
-struct TcPlan {
-    int n_gemm, n_trunk;
-    TcGemm g[kMaxGemm];
-    int kpe, kaux;         // padded feature-tile widths
-    int plane_bytes;       // bytes of all weight images of one sub-module (one precision plane)
-    int f32_floats;        // fp32 block: the biases, sigma_w [L], sigma_b (4) [, the layer engine's rgb head]
-    int sigma_w_off;       // float offset of sigma_w in the fp32 block
-    int sub_bytes;         // total bytes per sub-module: planes (hi[,lo]) + fp32 block
-    int x_tile_bytes;      // bytes of one feature tile image (one plane)
-    int L;
-    int bstride;           // fused engine: floats reserved per GEMM bias in the fp32 block (256; 512 for the 512-wide network)
-    int f32_off;           // byte offset of the fp32 block inside one sub-module's pack (after the hi and lo planes)
-};
 
 int pad16(int x) { return (x + 15) / 16 * 16; }
 int pad8(int x) { return (x + 7) / 8 * 8; }
@@ -76,31 +46,6 @@ int pad8(int x) { return (x + 7) / 8 * 8; }
 // then ReLU (or none), so every GEMM reads whole K slabs and no kernel has a column tail.
 constexpr int kLgCols = 128;
 int lg_cols(int x) { return (x + kLgCols - 1) / kLgCols * kLgCols; }
-
-// ---- the network's Linears in forward order (nerf.py:115-160): trunk layers 0 .. layers-1, xyz_encoding_final,
-// dir_a_encoding, rgb.  The forward and data-gradient plans, the weight packs and the weight-gradient items of the backward all
-// walk this one table.  Linear j's SRC_H segment reads the output of Linear j - 1 (image j - 1 of a tile's activation record).
-struct TcSeg {
-    int src;             // SRC_XPE / SRC_XAUX (a segment of the feature tile) or SRC_H (the previous Linear's output)
-    int k, k_real;       // padded K columns (multiple of 16); columns that exist in the nn.Linear weight
-    int in0;             // first input column of the segment in the nn.Linear weight
-};
-struct TcLinear {
-    int n;               // output features
-    int cols;            // columns of the output's activation image (n, or lg_cols(n) on the layer engine)
-    int nseg;
-    TcSeg seg[2];
-    int kin;             // in_features
-    int w, b;            // PackedLayout float offsets of the weight and the bias (also their offsets in the gradient block)
-    int bwd;             // BwdLayout float offset of the [n][L] sub-matrix the data-gradient chain streams; -1: none
-    int epi;             // EPI_RELU, EPI_RELU_SIGMA (last trunk layer), EPI_LINEAR (xyz_encoding_final) or EPI_RGB
-};
-struct TcLinears {
-    int n, n_trunk;
-    int kpe, kaux;       // padded feature-tile widths
-    int hc, gc;          // columns of the H / F images and of the G image (L and L/2 unless padded for the layer engine)
-    TcLinear l[MN_MAX_LAYERS + 3];
-};
 
 // layer: the table of the layer engine, whose activation images are padded to lg_cols; the fused engine's are not.
 TcLinears tc_linears(const mn_model& m, bool layer) {
@@ -208,38 +153,19 @@ void build_dgrad_plan(const NetDims& nd, const TcLinears& T, bool layer, TcPlan*
     P.sub_bytes = (int)mn_align((size_t)woff + (size_t)P.f32_floats * 4, 256);
 }
 
-// ---- which engine serves a network, and whether tensor-core training covers it.  The fused engine takes rgb_dim <= 32 (its
-// N = 32 rgb GEMM) at 64..256 (a multiple of 64) and 512 wide, up to 12 trunk layers; the layer engine every other width of
-// 64..kLgMaxL and depth (up to MN_MAX_LAYERS), and the SH heads of degree 3 and 4 (rgb_dim <= MN_TC_LG_RGB_MAX).  Training
-// runs on the fused engine at 256 and 512 wide (every depth it takes, 2..12 trunk layers) and on the layer engine from 256
-// wide; it needs dir_a_encoding (its data-gradient chain ends there) and no affine appearance.  A network is trained on the
-// engine that runs its inference, so the recording forward writes the tape that engine's backward reads.
-enum { TC_NONE = 0, TC_FUSED = 1, TC_LAYER = 2 };
-constexpr int kLgMaxL = 4096;
-struct TcNet {
-    int engine;
-    bool train;          // tensor-core training covers the shape (mn_model_train_tc_supported once the weights are packed)
-    TcLinears lin;
-    TcPlan P;            // engine != TC_NONE: the forward GEMMs and the layout of the forward weight images (tc_packed)
-    TcPlan D;            // train: the data-gradient chain and the layout of the transposed weight images (tc_dgrad)
-};
-
-TcNet tc_net(const mn_model& m) {
-    const NetDims& nd = m.nd;
-    TcNet t{};
-    const bool fused_width = nd.L % 64 == 0 && (nd.L <= 256 || nd.L == 512) && nd.L >= 64;
-    if (nd.affine && nd.rgb_dim != 3) t.engine = TC_NONE;
-    else if (fused_width && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers <= 12)
-        t.engine = TC_FUSED;
-    else if (nd.L >= 64 && nd.L <= kLgMaxL && nd.rgb_dim <= MN_TC_LG_RGB_MAX && nd.layers + 2 <= kMaxGemm)
-        t.engine = TC_LAYER;
-    const bool layer = t.engine == TC_LAYER;
-    t.lin = tc_linears(m, layer);
-    if (t.engine != TC_NONE) build_plan(nd, t.lin, layer, &t.P);
-    t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.layers >= 2 &&
-              ((layer && nd.L >= 256) || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 12));
-    if (t.train) build_dgrad_plan(nd, t.lin, layer, &t.D);
-    return t;
+LgNet lg_net(const TcNet& net, const NetDims& nd) {
+    const TcPlan& P = net.P;
+    LgNet b{};
+    b.g_gemm = nd.has_dir_a ? P.n_gemm - 1 : -1;
+    b.buf_cols[LB_ACT0] = b.buf_cols[LB_ACT1] = net.lin.hc;
+    if (nd.has_dir_a) b.buf_cols[LB_G] = net.lin.gc;
+    b.h_last = (nd.layers - 1) & 1;
+    b.rgb_src = nd.has_dir_a ? LB_G : b.h_last;
+    b.sigma_k = pad8(nd.L);
+    b.rgb_k = pad8(nd.rgb_in);
+    b.rgb_w_off = P.sigma_w_off + b.sigma_k + 4;
+    b.rgb_b_off = b.rgb_w_off + nd.rgb_dim * b.rgb_k;
+    return b;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -536,49 +462,32 @@ constexpr int kSmemMax = 227 * 1024;
 
 #include "mn_mlp_wg.cuh"
 
-template <int kMode, bool kSplit, bool kWide>
-int wg_launch(mn_ctx* ctx, const TcArgs& A, int64_t n_tiles128, cudaStream_t st) {
-    const WgLayout WL = wg_layout(A.plan, kSplit, wg_reg_act(kMode, kSplit, kWide));
+// The variant of tc_mlp_wg_kernel that runs mode over plan P, and its shared-memory layout; split (tc_f16x3): inference <= 256 wide.
+struct WgVariant {
+    void (*kernel)(TcArgs);
+    WgLayout layout;
+};
+WgVariant wg_variant(int mode, bool split, const TcPlan& P) {
+    const bool wide = P.L > 256;
+    static void (*const kernel[3][2])(TcArgs) = {       // [mode][wide]
+        {tc_mlp_wg_kernel<PP_INFER, false, false>, tc_mlp_wg_kernel<PP_INFER, false, true>},
+        {tc_mlp_wg_kernel<PP_TRAIN_FWD, false, false>, tc_mlp_wg_kernel<PP_TRAIN_FWD, false, true>},
+        {tc_mlp_wg_kernel<PP_DGRAD, false, false>, tc_mlp_wg_kernel<PP_DGRAD, false, true>}};
+    return {split ? tc_mlp_wg_kernel<PP_INFER, true, false> : kernel[mode][wide], wg_layout(P, split, wg_reg_act(mode, split, wide))};
+}
+
+int wg_launch(mn_ctx* ctx, const TcArgs& A, int mode, int64_t n_tiles128, cudaStream_t st) {
+    const auto [kernel, WL] = wg_variant(mode, A.split, A.plan);
     if (WL.total > kSmemMax || WL.stages < 2) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: shared-memory budget exceeded");
-    MN_CUDA(ctx, cudaFuncSetAttribute(tc_mlp_wg_kernel<kMode, kSplit, kWide>, cudaFuncAttributeMaxDynamicSharedMemorySize, WL.total));
+    MN_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WL.total));
     const unsigned grid = (unsigned)(n_tiles128 < ctx->sm_count ? n_tiles128 : ctx->sm_count);
-    tc_mlp_wg_kernel<kMode, kSplit, kWide><<<grid, kWgmmaThreads, WL.total, st>>>(A);
+    kernel<<<grid, kWgmmaThreads, WL.total, st>>>(A);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }
 
 #include "mn_train_tc.cuh"
 #include "mn_layer_gemm.cuh"
-
-// The layer engine's activation buffers and rgb head, from the forward plan.  GEMM gi writes ping-pong buffer gi % 2 and reads
-// the other one; dir_a_encoding writes G to its own buffer: F went to the other ping-pong buffer, so the head still finds
-// H_last for sigma.  The buffers have the padded widths of the activation images (TcLinears::hc, gc).  rgb_w ([rgb_dim][rgb_k])
-// and rgb_b follow sigma_w (sigma_k floats) and sigma_b in the fp32 block (build_plan).
-enum { LB_ACT0 = 0, LB_ACT1 = 1, LB_G = 2 };
-struct LgNet {
-    int g_gemm;          // the GEMM that writes LB_G (dir_a_encoding), or -1
-    int buf_cols[3];     // columns of each activation buffer (0: unused)
-    int h_last;          // buffer of the last trunk activations
-    int rgb_src;         // buffer the rgb head reads
-    int sigma_k, rgb_k;  // columns the fp32 heads read: L and rgb_in rounded up to 8 (the padding weights are zero)
-    int rgb_w_off, rgb_b_off;
-    int in(int gi) const { return (gi + 1) & 1; }
-    int out(int gi) const { return gi == g_gemm ? LB_G : gi & 1; }
-};
-LgNet lg_net(const TcNet& net, const NetDims& nd) {
-    const TcPlan& P = net.P;
-    LgNet b{};
-    b.g_gemm = nd.has_dir_a ? P.n_gemm - 1 : -1;
-    b.buf_cols[LB_ACT0] = b.buf_cols[LB_ACT1] = net.lin.hc;
-    if (nd.has_dir_a) b.buf_cols[LB_G] = net.lin.gc;
-    b.h_last = (nd.layers - 1) & 1;
-    b.rgb_src = nd.has_dir_a ? LB_G : b.h_last;
-    b.sigma_k = pad8(nd.L);
-    b.rgb_k = pad8(nd.rgb_in);
-    b.rgb_w_off = P.sigma_w_off + b.sigma_k + 4;
-    b.rgb_b_off = b.rgb_w_off + nd.rgb_dim * b.rgb_k;
-    return b;
-}
 
 // Workspace of a forward call: per tile of a group, the feature tile and the layer engine's activation buffers, each with its lo
 // plane under tc_f16x3.  The fused engine's one group covers every tile and has no activation buffers; the layer engine's
@@ -588,16 +497,14 @@ struct TcWorkspace {
     size_t x_bytes, buf_bytes[3], total;     // per plane
     int planes;
 };
-TcWorkspace tc_workspace(const TcNet& net, const NetDims& nd, int64_t n_tiles128, int precision) {
-    const bool layer = net.engine == TC_LAYER;
-    const LgNet B = layer ? lg_net(net, nd) : LgNet{};
+TcWorkspace tc_workspace(const TcNet& net, int64_t n_tiles128, int precision) {
     TcWorkspace w{};
-    w.group_tiles = layer && n_tiles128 > kLgGroupTiles ? kLgGroupTiles : n_tiles128;
+    w.group_tiles = net.engine == TC_LAYER && n_tiles128 > kLgGroupTiles ? kLgGroupTiles : n_tiles128;
     w.planes = precision == MN_PREC_TC_F16X3 ? 2 : 1;
     w.x_bytes = mn_align((size_t)w.group_tiles * net.P.x_tile_bytes, 1024);
     w.total = w.x_bytes * w.planes;
     for (int b = 0; b < 3; ++b) {
-        w.buf_bytes[b] = mn_align((size_t)w.group_tiles * B.buf_cols[b] * kTileM * 2, 1024);
+        w.buf_bytes[b] = mn_align((size_t)w.group_tiles * net.lg.buf_cols[b] * kTileM * 2, 1024);
         w.total += w.buf_bytes[b] * w.planes;
     }
     w.total += 1024;
@@ -653,19 +560,45 @@ int lg_gemm(mn_ctx* ctx, LgArgs G, const MlpArgs& a, const TcPlan& P, const TcGe
 
 // =================================================================================================
 size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision) {
-    const TcNet net = tc_net(*m);
-    return net.engine == TC_NONE ? 0 : tc_workspace(net, m->nd, n_tiles128, precision).total;
+    return m->tc.engine == TC_NONE ? 0 : tc_workspace(m->tc, n_tiles128, precision).total;
 }
 
+// ---- which engine serves a network, and whether tensor-core training covers it.  The fused engine takes rgb_dim <= 32 (its
+// N = 32 rgb GEMM) at 64..256 (a multiple of 64) and 512 wide, up to 12 trunk layers; the layer engine every other width of
+// 64..kLgMaxL and depth (up to MN_MAX_LAYERS), and the SH heads of degree 3 and 4 (rgb_dim <= MN_TC_LG_RGB_MAX).  Training
+// runs on the fused engine at 256 and 512 wide (every depth it takes, 2..12 trunk layers) and on the layer engine from 256
+// wide; it needs dir_a_encoding (its data-gradient chain ends there) and no affine appearance.  A network is trained on the
+// engine that runs its inference, so the recording forward writes the tape that engine's backward reads.
+// Defined after mn_mlp_tc_workspace: nvcc names the anonymous namespace, so every kernel, after the first function outside it.
+constexpr int kLgMaxL = 4096;
+TcNet tc_net(const mn_model& m) {
+    const NetDims& nd = m.nd;
+    TcNet t{};
+    const bool fused_width = nd.L % 64 == 0 && (nd.L <= 256 || nd.L == 512) && nd.L >= 64;
+    if (nd.affine && nd.rgb_dim != 3) t.engine = TC_NONE;
+    else if (fused_width && nd.rgb_dim <= MN_TC_RGB_MAX && nd.layers <= 12)
+        t.engine = TC_FUSED;
+    else if (nd.L >= 64 && nd.L <= kLgMaxL && nd.rgb_dim <= MN_TC_LG_RGB_MAX && nd.layers + 2 <= kMaxGemm)
+        t.engine = TC_LAYER;
+    const bool layer = t.engine == TC_LAYER;
+    t.lin = tc_linears(m, layer);
+    if (t.engine != TC_NONE) build_plan(nd, t.lin, layer, &t.P);
+    if (layer) t.lg = lg_net(t, nd);
+    t.train = nd.has_dir_a && !nd.affine && nd.rgb_dim >= 3 && nd.layers >= 2 &&
+              ((layer && nd.L >= 256) || (t.engine == TC_FUSED && (nd.L == 256 || nd.L == 512) && nd.layers <= 12));
+    if (t.train) build_dgrad_plan(nd, t.lin, layer, &t.D);
+    t.act_tile_bytes = (int64_t)(mn_tc_img_off(nd.layers + 1, t.lin.hc) + mn_tc_img_off(1, t.lin.gc));     // ends with G (L/2 columns)
+    return t;
+}
 
 // mode: PP_INFER (the tc_f16 inference launch), PP_TRAIN_FWD (the recording forward: the forward plan in the training variant's
 // layout) or PP_DGRAD (the data-gradient chain of the backward on the transposed images); the training modes only for shapes
 // whose training runs on the fused engine.
 int mn_mlp_tp_program(const mn_model& m, int mode, unsigned int* table_out, int cap_entries, int* info8) {
-    const TcNet net = tc_net(m);
+    const TcNet& net = m.tc;
     if (net.engine != TC_FUSED || (mode != PP_INFER && !net.train)) return MN_ERR_UNSUPPORTED;
     const TcPlan& P = mode == PP_DGRAD ? net.D : net.P;
-    const WgLayout L = wg_layout(P, false, wg_reg_act(mode, false, P.L > 256));     // the tc_f16 launch's layout
+    const WgLayout L = wg_variant(mode, false, P).layout;     // the tc_f16 launch's layout
     int n = 0, n_trunk = 0;
     for (int gi = 0; gi < P.n_gemm; ++gi) {
         const int nch = (P.g[gi].n + 255) >> 8;
@@ -688,32 +621,32 @@ int mn_mlp_tp_program(const mn_model& m, int mode, unsigned int* table_out, int 
 
 // ---- transposed weight images of the data-gradient chain (build_dgrad_plan), one fp16 plane + the fp32 block per sub-module.
 // Element (n = input column, k = output channel) = W[k][n]: the [out][L] BwdLayout sub-matrix is the K-major source.
-static void tc_pack_dgrad(mn_ctx* ctx, mn_model* m, int sub, const TcNet& net) {
+static void tc_pack_dgrad(mn_ctx* ctx, mn_model* m, int sub) {
     const NetDims& nd = m->nd;
-    const TcPlan& D = net.D;
+    const TcPlan& D = m->tc.D;
     unsigned char* db = (unsigned char*)m->tc_dgrad + (size_t)sub * D.sub_bytes;
     const float* Q = m->packed_bwd + (size_t)sub * m->blay.total;
     const float* Pk = m->packed + (size_t)sub * m->lay.total;
     for (int gi = 0; gi < D.n_gemm; ++gi) {
         const TcGemm& g = D.g[gi];
-        const TcLinear& l = net.lin.l[g.img + 1];
+        const TcLinear& l = m->tc.lin.l[g.img + 1];
         const int k = g.k[0];          // l.cols: the output channels past l.n are zero rows of the image
         mn_pack_push(ctx, PackOp{Q + l.bwd, db + g.w_off, nullptr, (long long)g.n * k, PK_TC_HALF, {nd.L, l.n, g.n, k, 0, 0, 256}});
     }
     float* f32 = reinterpret_cast<float*>(db + D.f32_off);
     mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
-    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + net.lin.hc, nullptr, (long long)nd.rgb_dim * (nd.L / 2), PK_RGBW,
+    mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_w, f32 + m->tc.lin.hc, nullptr, (long long)nd.rgb_dim * (nd.L / 2), PK_RGBW,
                              {nd.L / 2, nd.rgb_dim, 0, 0, 0, 0, 0}});
 }
 
 // The transposed images cost as much as the forward images again, so they are allocated and packed by the first recording call
 // (inference-only users never hold them); from then on every mn_model_set_weights repacks them with the forward images.
-static int tc_dgrad_ready(mn_ctx* ctx, mn_model* m, const TcNet& net, cudaStream_t st) {
+static int tc_dgrad_ready(mn_ctx* ctx, mn_model* m, cudaStream_t st) {
     if (m->tc_dgrad) return MN_OK;
-    const size_t bytes = (size_t)net.D.sub_bytes * m->d.n_sub;
+    const size_t bytes = (size_t)m->tc.D.sub_bytes * m->d.n_sub;
     MN_CUDA(ctx, cudaMalloc(&m->tc_dgrad, bytes));
     MN_CUDA(ctx, cudaMemsetAsync(m->tc_dgrad, 0, bytes, st));
-    for (int s = 0; s < m->d.n_sub; ++s) tc_pack_dgrad(ctx, m, s, net);
+    for (int s = 0; s < m->d.n_sub; ++s) tc_pack_dgrad(ctx, m, s);
     return mn_pack_flush(ctx, st);
 }
 
@@ -722,11 +655,8 @@ static int tc_dgrad_ready(mn_ctx* ctx, mn_model* m, const TcNet& net, cudaStream
 // layer engine (its N is padded to 256-column blocks).  The fp32 block holds the biases, sigma_w and sigma_b, and for the layer
 // engine the rgb head.  Queued: all images of the sub-module are written by ONE launch (mn_pack_flush in mn_model_set_weights).
 int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
-    const TcNet net = tc_net(*m);
-    if (net.engine == TC_NONE) {
-        m->tc_ready = 0;
-        return MN_OK;  // configuration only served by the fp32 kernel
-    }
+    const TcNet& net = m->tc;
+    if (net.engine == TC_NONE) return MN_OK;  // configuration only served by the fp32 kernel
     const NetDims& nd = m->nd;
     const TcPlan& P = net.P;
     const size_t sub_bytes = (size_t)P.sub_bytes;
@@ -750,7 +680,7 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
         mn_pack_push(ctx, PackOp{Pk + l.b, f32 + g.bias_off, nullptr, (long long)(b_end - g.bias_off), PK_TC_F32, {l.n, 0, 0, 0, 0, 0, 0}});
     }
     const bool layer = net.engine == TC_LAYER;
-    const LgNet B = layer ? lg_net(net, nd) : LgNet{};
+    const LgNet& B = net.lg;
     const int sigma_k = layer ? B.sigma_k : nd.L;
     mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_w, f32 + P.sigma_w_off, nullptr, (long long)nd.L, PK_TC_F32, {nd.L, 0, 0, 0, 0, 0, 0}});
     mn_pack_push(ctx, PackOp{Pk + m->lay.sigma_b, f32 + P.sigma_w_off + sigma_k, nullptr, 4, PK_TC_F32, {1, 0, 0, 0, 0, 0, 0}});
@@ -760,9 +690,7 @@ int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st) {
         mn_pack_push(ctx, PackOp{Pk + m->lay.rgb_b, f32 + B.rgb_b_off, nullptr, mn_tc_lg_rgb_bound(nd.rgb_dim), PK_TC_F32,
                                  {nd.rgb_dim, 0, 0, 0, 0, 0, 0}});
     }
-    m->tc_ready = 1;
-    m->train_tc_ok = net.train ? 1 : 0;
-    if (net.train && m->tc_dgrad) tc_pack_dgrad(ctx, m, sub, net);
+    if (net.train && m->tc_dgrad) tc_pack_dgrad(ctx, m, sub);
     return MN_OK;
 }
 
@@ -798,12 +726,12 @@ static TcArgs tc_forward_args(const mn_model* m, const TcPlan& F, const MlpArgs&
 // the fp32 head blocks go to the tape instead of the workspace, which is not used.
 static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet& net, int64_t n_tiles128, int precision,
                         void* ws, size_t ws_bytes, cudaStream_t st, const TrainTcTape* tape = nullptr) {
-    if (!m->tc_ready) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: weights not packed");
+    if (!m->tc_packed) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core MLP: weights not packed");
     if (n_tiles128 <= 0) return MN_OK;
     const TcPlan& P = net.P;
-    const LgNet B = lg_net(net, m->nd);
+    const LgNet& B = net.lg;
     const int hc = net.lin.hc;
-    const TcWorkspace W = tc_workspace(net, m->nd, n_tiles128, precision);
+    const TcWorkspace W = tc_workspace(net, n_tiles128, precision);
     if (!tape && (ws_bytes < W.total || !ws)) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
     const bool split = precision == MN_PREC_TC_F16X3;
     unsigned char* wp = (unsigned char*)(((uintptr_t)ws + 1023) / 1024 * 1024);
@@ -815,7 +743,7 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet&
         buf[b] = LgImg{wp, (int64_t)B.buf_cols[b] * kTileM * 2, (int64_t)W.buf_bytes[b]};
         wp += W.buf_bytes[b] * W.planes;
     }
-    const int64_t act_tile = tape ? (int64_t)mn_train_tc_act_tile_bytes(m) : 0;
+    const int64_t act_tile = tape ? net.act_tile_bytes : 0;
 
     const size_t enc_sm = (size_t)P.x_tile_bytes * (split ? 2 : 1);
     MN_CUDA(ctx, cudaFuncSetAttribute(tc_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)enc_sm));
@@ -878,9 +806,9 @@ static int layer_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, const TcNet&
 
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws, size_t ws_bytes,
                      cudaStream_t st) {
-    const TcNet net = tc_net(*m);
+    const TcNet& net = m->tc;
     if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net, n_tiles128, precision, ws, ws_bytes, st);
-    if (net.engine != TC_FUSED || !m->tc_ready)
+    if (net.engine != TC_FUSED || !m->tc_packed)
         return mn_fail(ctx, MN_ERR_UNSUPPORTED,
                        "tensor-core MLP path covers layer_dim 64..4096 with up to 16 layers and rgb_dim <= 80 (sh_deg <= 4), without "
                        "affine appearance for rgb_dim > 3; use precision 'fp32' for this model");
@@ -889,22 +817,19 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
                        "precision 'tc_f16x3' covers layer_dim <= 256; use 'tc_f16' or 'fp32' for the 512-wide network");
     if (n_tiles128 <= 0) return MN_OK;
     TcArgs A = tc_forward_args(m, net.P, a, n_tiles128);
-    const TcPlan& P = A.plan;
     const int split = precision == MN_PREC_TC_F16X3 ? 1 : 0;
     A.split = split;
-    const TcWorkspace W = tc_workspace(net, m->nd, n_tiles128, precision);
+    const TcWorkspace W = tc_workspace(net, n_tiles128, precision);
     if (ws_bytes < W.total || !ws) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_mlp_tc_launch: workspace too small");
     uintptr_t wp = ((uintptr_t)ws + 1023) / 1024 * 1024;
     __half* ximg = reinterpret_cast<__half*>(wp);
     A.ximg = ximg;
     A.x_plane_halves = (int64_t)W.x_bytes / 2;
-    int rc = tc_encode(ctx, m, a, P, n_tiles128, split, ximg, A.x_plane_halves, st);
+    int rc = tc_encode(ctx, m, a, A.plan, n_tiles128, split, ximg, A.x_plane_halves, st);
     if (rc) return rc;
 
     mn_prof_begin(ctx, st);
-    if (split) rc = wg_launch<PP_INFER, true, false>(ctx, A, n_tiles128, st);
-    else if (P.L > 256) rc = wg_launch<PP_INFER, false, true>(ctx, A, n_tiles128, st);
-    else rc = wg_launch<PP_INFER, false, false>(ctx, A, n_tiles128, st);
+    rc = wg_launch(ctx, A, PP_INFER, n_tiles128, st);
     mn_prof_end(ctx, st);
     return rc;
 }
@@ -912,39 +837,29 @@ int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles
 // =================================================================================================
 // tensor-core training path: host side (kernels in mn_train_tc.cuh)
 // =================================================================================================
-size_t mn_train_tc_x_tile_bytes(const mn_model* m) {
-    const TcNet net = tc_net(*m);
-    return net.engine == TC_NONE ? 0 : (size_t)net.P.x_tile_bytes;
-}
-size_t mn_train_tc_act_tile_bytes(const mn_model* m) {
-    const TcNet net = tc_net(*m);
-    return mn_tc_img_off(m->nd.layers + 1, net.lin.hc) + mn_tc_img_off(1, net.lin.gc);     // ends with G (L/2 columns, padded)
-}
-
 // Recording forward of either engine: encoder tiles and every layer's activations land in the caller's tape.  train: a training
-// call, whose caller has checked m->train_tc_ok; the first one allocates and packs the transposed images of the backward pass.
-// !train: the test hook mn_debug_tc_forward_record, for every network the tensor cores serve, trained there or not; it needs no
-// transposed images, so none are allocated.
+// call, whose caller has checked m->tc.train && m->tc_packed; the first one allocates and packs the transposed images of the
+// backward pass.  !train: the test hook mn_debug_tc_forward_record, for every network the tensor cores serve, trained there or
+// not; it needs no transposed images, so none are allocated.
 int mn_mlp_tc_launch_record(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, bool train,
                             cudaStream_t st) {
-    const TcNet net = tc_net(*m);
-    if (!train && (net.engine == TC_NONE || !m->tc_ready))
+    const TcNet& net = m->tc;
+    if (!train && (net.engine == TC_NONE || !m->tc_packed))
         return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_debug_tc_forward_record: the network has no tensor-core forward");
     if (n_tiles128 <= 0) return MN_OK;
     int rc;
-    if (train && (rc = tc_dgrad_ready(ctx, m, net, st))) return rc;
+    if (train && (rc = tc_dgrad_ready(ctx, m, st))) return rc;
     if (net.engine == TC_LAYER) return layer_launch(ctx, m, a, net, n_tiles128, MN_PREC_TC_F16, nullptr, 0, st, &tape);
     TcArgs A = tc_forward_args(m, net.P, a, n_tiles128);
     A.ximg = reinterpret_cast<const __half*>(tape.xreg);
     A.x_plane_halves = 0;
     A.tape_act = tape.act;
     A.tape_f32 = tape.f32;
-    A.act_tile_bytes = (int64_t)mn_train_tc_act_tile_bytes(m);
+    A.act_tile_bytes = net.act_tile_bytes;
     A.layers = a.nd.layers;
     if ((rc = tc_encode(ctx, m, a, A.plan, n_tiles128, 0, reinterpret_cast<__half*>(tape.xreg), 0, st))) return rc;
     mn_prof_begin(ctx, st);
-    if (A.plan.L > 256) rc = wg_launch<PP_TRAIN_FWD, false, true>(ctx, A, n_tiles128, st);
-    else rc = wg_launch<PP_TRAIN_FWD, false, false>(ctx, A, n_tiles128, st);
+    rc = wg_launch(ctx, A, PP_TRAIN_FWD, n_tiles128, st);
     mn_prof_end(ctx, st);
     return rc;
 }
@@ -969,7 +884,7 @@ static TcBwdWorkspace tc_bwd_workspace(const mn_model* m, const TcNet& net, int6
         w.emb_k = pad8(nd.L / 2);
     } else {
         w.head_tiles = n_tiles128;
-        w.dz_bytes = mn_align((size_t)n_tiles128 * mn_train_tc_act_tile_bytes(m));
+        w.dz_bytes = mn_align((size_t)n_tiles128 * net.act_tile_bytes);
     }
     w.head_bytes = mn_align((size_t)w.head_tiles * mn_tc_g32_rows(nd.rgb_dim) * kTileM * sizeof(float));
     w.emb_floats = nd.app_in_dira ? (size_t)m->d.n_sub * nd.app_count * w.emb_k : 0;
@@ -977,21 +892,21 @@ static TcBwdWorkspace tc_bwd_workspace(const mn_model* m, const TcNet& net, int6
     return w;
 }
 size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128) {
-    return tc_bwd_workspace(m, tc_net(*m), n_tiles128).total;
+    return tc_bwd_workspace(m, m->tc, n_tiles128).total;
 }
 
 // Test hook (mn_debug_tc_train_layout): entries MN_TCL_ENGINE .. of the layout the two training passes share, from the same
-// tc_net / tc_bwd_workspace the passes call.  Backward-workspace offsets are relative to the 256-byte aligned base that
-// mn_train_tc_backward carves.
+// plan (mn_model::tc) and tc_bwd_workspace the passes read.  Backward-workspace offsets are relative to the 256-byte aligned
+// base that mn_train_tc_backward carves.
 int mn_train_tc_layout(const mn_model* m, int64_t n_tiles128, int64_t* out, int cap) {
-    const TcNet net = tc_net(*m);
+    const TcNet& net = m->tc;
     const NetDims& nd = m->nd;
     const int n_img = nd.has_dir_a ? nd.layers + 2 : nd.layers;      // without dir_a_encoding the record holds the trunk only
     if (cap < MN_TCL_IMG + 2 * n_img) return MN_ERR_WORKSPACE;
     out[MN_TCL_ENGINE] = net.engine;
     out[MN_TCL_TRAIN] = net.train ? 1 : 0;
     out[MN_TCL_X_TILE] = net.P.x_tile_bytes;
-    out[MN_TCL_ACT_TILE] = (int64_t)mn_train_tc_act_tile_bytes(m);
+    out[MN_TCL_ACT_TILE] = net.act_tile_bytes;
     out[MN_TCL_KPE] = net.lin.kpe;
     out[MN_TCL_KAUX] = net.lin.kaux;
     out[MN_TCL_HC] = net.lin.hc;
@@ -1051,15 +966,15 @@ static WgLinear wg_linear(const TcLinears& T, int j, int dz_off) {
 
 int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_tiles128, const TrainTcTape& tape, void* ws, size_t ws_bytes,
                          cudaStream_t st) {
-    if (!m->train_tc_ok || !m->tc_dgrad) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: unsupported network shape");
+    const TcNet& net = m->tc;
+    if (!net.train || !m->tc_packed || !m->tc_dgrad) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "tensor-core backward: unsupported network shape");
     if (n_tiles128 <= 0) return MN_OK;
-    const TcNet net = tc_net(*m);
     const TcBwdWorkspace WS = tc_bwd_workspace(m, net, n_tiles128);
     if (!ws || ws_bytes < WS.total) return mn_fail(ctx, MN_ERR_WORKSPACE, "mn_train_tc_backward: workspace too small");
     const NetDims& nd = a.nd;
     const TcLinears& lin = net.lin;
     const int L = nd.L, half = L / 2, hc = lin.hc;
-    const int64_t act_tile = (int64_t)mn_train_tc_act_tile_bytes(m);
+    const int64_t act_tile = net.act_tile_bytes;
     char* wp = (char*)(((uintptr_t)ws + 255) / 256 * 256);
     unsigned char* dz = (unsigned char*)wp;               wp += WS.dz_bytes;
     float* gf32 = (float*)wp;                             wp += WS.head_bytes;
@@ -1178,7 +1093,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         A.scale = scale;
         A.act_tile_bytes = act_tile;
         A.layers = nd.layers;
-        rc = L > 256 ? wg_launch<PP_DGRAD, false, true>(ctx, A, n_tiles128, st) : wg_launch<PP_DGRAD, false, false>(ctx, A, n_tiles128, st);
+        rc = wg_launch(ctx, A, PP_DGRAD, n_tiles128, st);
         if (rc) return rc;
         // ---- weight gradients of every Linear but rgb, straight from the gradient records.  512 wide: one launch per Linear.  A
         // single launch would be faster, but over ~80 items the chunk policy gives each CTA more tiles to sum in its accumulators,
@@ -1194,7 +1109,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         // weight gradients.  dZ of Linear j is consumed by its weight gradient before the buffer is overwritten.
         const TcPlan& P = net.P;
         const TcPlan& D = net.D;
-        const LgNet B = lg_net(net, nd);
+        const LgNet& B = net.lg;
         const int rows = mn_tc_g32_rows(nd.rgb_dim);
         const int64_t gt = WS.head_tiles;
         unsigned char* dzg = dz;                              // dZ of dir_a_encoding (gc columns)

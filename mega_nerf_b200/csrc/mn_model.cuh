@@ -48,6 +48,91 @@ static inline int mn_tape_tm(int L) { return L <= 256 ? 64 : 32; }
 // TM-slot tiles one CTA of the fp32 weight-gradient kernel sums before its fp32 atomics (mlp_bwd_weight_kernel)
 #define MN_WG_CHUNK_TILES 64
 
+// ---- tensor-core execution plan of a network (csrc/mn_mlp_tc.cu)
+constexpr int kMaxGemm = MN_MAX_LAYERS + 2;     // layer engine: every trunk layer, xyz_encoding_final and dir_a_encoding
+
+enum { SRC_H = 0, SRC_XPE = 1, SRC_XAUX = 2 };
+enum { EPI_RELU = 0, EPI_RELU_SIGMA = 1, EPI_LINEAR = 2, EPI_RGB = 3,
+       // data-gradient chain (training, mn_train_tc.cuh): plain copy, ReLU mask from the activation tape, mask + sigma-head term
+       EPI_D_LINEAR = 4, EPI_D_MASK = 5, EPI_D_MASK_SIGMA = 6 };
+
+struct TcGemm {
+    int n;           // MMA N = columns of the weight image (layer engine: the output columns padded to 256-column blocks)
+    int nseg;
+    int src[2];
+    int k[2];        // padded K columns per segment (multiple of 16)
+    int w_off;       // byte offset of the weight image inside one precision plane of a sub-module
+    int bias_off;    // float offset inside the sub-module's fp32 block
+    int img;         // data-gradient plan: tape image of the output (ReLU mask read from the activation record, dZ written)
+    int epi;
+};
+
+struct TcPlan {
+    int n_gemm, n_trunk;
+    TcGemm g[kMaxGemm];
+    int kpe, kaux;         // padded feature-tile widths
+    int plane_bytes;       // bytes of all weight images of one sub-module (one precision plane)
+    int f32_floats;        // fp32 block: the biases, sigma_w [L], sigma_b (4) [, the layer engine's rgb head]
+    int sigma_w_off;       // float offset of sigma_w in the fp32 block
+    int sub_bytes;         // total bytes per sub-module: planes (hi[,lo]) + fp32 block
+    int x_tile_bytes;      // bytes of one feature tile image (one plane)
+    int L;
+    int bstride;           // fused engine: floats reserved per GEMM bias in the fp32 block (256; 512 for the 512-wide network)
+    int f32_off;           // byte offset of the fp32 block inside one sub-module's pack (after the hi and lo planes)
+};
+
+// ---- the network's Linears in forward order (nerf.py:115-160): trunk layers 0 .. layers-1, xyz_encoding_final,
+// dir_a_encoding, rgb.  The forward and data-gradient plans, the weight packs and the weight-gradient items of the backward all
+// walk this one table.  Linear j's SRC_H segment reads the output of Linear j - 1 (image j - 1 of a tile's activation record).
+struct TcSeg {
+    int src;             // SRC_XPE / SRC_XAUX (a segment of the feature tile) or SRC_H (the previous Linear's output)
+    int k, k_real;       // padded K columns (multiple of 16); columns that exist in the nn.Linear weight
+    int in0;             // first input column of the segment in the nn.Linear weight
+};
+struct TcLinear {
+    int n;               // output features
+    int cols;            // columns of the output's activation image (n, or lg_cols(n) on the layer engine)
+    int nseg;
+    TcSeg seg[2];
+    int kin;             // in_features
+    int w, b;            // PackedLayout float offsets of the weight and the bias (also their offsets in the gradient block)
+    int bwd;             // BwdLayout float offset of the [n][L] sub-matrix the data-gradient chain streams; -1: none
+    int epi;             // EPI_RELU, EPI_RELU_SIGMA (last trunk layer), EPI_LINEAR (xyz_encoding_final) or EPI_RGB
+};
+struct TcLinears {
+    int n, n_trunk;
+    int kpe, kaux;       // padded feature-tile widths
+    int hc, gc;          // columns of the H / F images and of the G image (L and L/2 unless padded for the layer engine)
+    TcLinear l[MN_MAX_LAYERS + 3];
+};
+
+// The layer engine's activation buffers and rgb head, from the forward plan.  GEMM gi writes ping-pong buffer gi % 2 and reads
+// the other one; dir_a_encoding writes G to its own buffer: F went to the other ping-pong buffer, so the head still finds
+// H_last for sigma.  The buffers have the padded widths of the activation images (TcLinears::hc, gc).  rgb_w ([rgb_dim][rgb_k])
+// and rgb_b follow sigma_w (sigma_k floats) and sigma_b in the fp32 block (build_plan).
+enum { LB_ACT0 = 0, LB_ACT1 = 1, LB_G = 2 };
+struct LgNet {
+    int g_gemm;          // the GEMM that writes LB_G (dir_a_encoding), or -1
+    int buf_cols[3];     // columns of each activation buffer (0: unused)
+    int h_last;          // buffer of the last trunk activations
+    int rgb_src;         // buffer the rgb head reads
+    int sigma_k, rgb_k;  // columns the fp32 heads read: L and rgb_in rounded up to 8 (the padding weights are zero)
+    int rgb_w_off, rgb_b_off;
+    int in(int gi) const { return (gi + 1) & 1; }
+    int out(int gi) const { return gi == g_gemm ? LB_G : gi & 1; }
+};
+
+enum { TC_NONE = 0, TC_FUSED = 1, TC_LAYER = 2 };
+struct TcNet {
+    int engine;              // TC_NONE (fp32 only), TC_FUSED (tc_mlp_wg_kernel) or TC_LAYER (one GEMM launch per Linear)
+    bool train;              // tensor-core training covers the shape (once the weights are packed: tc_packed)
+    TcLinears lin;
+    TcPlan P;                // engine != TC_NONE: the forward GEMMs and the layout of the forward weight images (tc_packed)
+    TcPlan D;                // train: the data-gradient chain and the layout of the transposed weight images (tc_dgrad)
+    LgNet lg;                // engine == TC_LAYER: its activation buffers and rgb head
+    int64_t act_tile_bytes;  // bytes of one tile's activation record (and of the backward's gradient record)
+};
+
 struct mn_model {
     mn_ctx* ctx = nullptr;
     mn_model_desc d{};
@@ -60,12 +145,11 @@ struct mn_model {
     float* centroids_d = nullptr;     // [n_sub, 3]
     int* counters_d = nullptr;        // routing scratch: see mn_route.cu
     int max_multiplicity = 0;         // slot capacity per row for blended routing
-    // tensor-core packed weights (fp16 hi / lo images), see mn_mlp_tc.cu
+    TcNet tc{};                       // tensor-core plan: fixed by nd, lay and blay, so build_layout computes it (tc_net) once
+    // tensor-core packed weights (fp16 hi / lo images, mn_mlp_tc.cu): NULL before the first mn_model_set_weights or if TC_NONE
     void* tc_packed = nullptr;
-    int tc_ready = 0;
     // transposed fp16 weight images of the tensor-core data-gradient chain (mn_train_tc.cuh); NULL if the shape is not covered
     void* tc_dgrad = nullptr;
-    int train_tc_ok = 0;
 };
 
 // counters_d layout (ints)
@@ -182,6 +266,7 @@ int mn_mlp_bwd_launch(mn_ctx* ctx, const BwdArgs& a, int64_t n_tiles128, cudaStr
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws,
                      size_t ws_bytes, cudaStream_t st);
 size_t mn_mlp_tc_workspace(const mn_model* m, int64_t n_tiles128, int precision);
+TcNet tc_net(const mn_model& m);
 int mn_mlp_tc_pack(mn_ctx* ctx, mn_model* m, int sub, cudaStream_t st);
 // host only (test hook): mode 0 inference, 1 recording forward, 2 data-gradient chain (MN_TP_* in mn_b200.h)
 int mn_mlp_tp_program(const mn_model& m, int mode, unsigned int* table_out, int cap_entries, int* info8);
@@ -211,10 +296,8 @@ struct TrainTcTape {
 #define MN_TC_TRAIN_COVERAGE                                                                                                     \
     "tensor-core training covers layer_dim 256..4096 with 2..16 layers and a direction / appearance head, "                       \
     "rgb_dim 3 or a raw SH head (rgb_dim <= 80: sh_deg <= 4), no affine appearance; use train precision 'fp32'"
-size_t mn_train_tc_x_tile_bytes(const mn_model* m);
-size_t mn_train_tc_act_tile_bytes(const mn_model* m);
-// the recording forward into `tape`: of a training call (train, the caller has checked train_tc_ok) or of the test hook, which
-// runs every network with a tensor-core forward
+// the recording forward into `tape`: of a training call (train, the caller has checked m->tc.train && m->tc_packed) or of the
+// test hook, which runs every network with a tensor-core forward
 int mn_mlp_tc_launch_record(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, const TrainTcTape& tape, bool train,
                             cudaStream_t st);
 size_t mn_train_tc_backward_workspace(const mn_model* m, int64_t n_tiles128);
