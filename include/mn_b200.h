@@ -185,6 +185,19 @@ int mn_model_set_centroids(mn_model* m, const float* centroids_d, void* stream);
 /* (Re)pack one sub-module: transposes / pads / splits the weights into model-owned device buffers
  * (the only persistent allocation the library makes).  Call again whenever the parameters change. */
 int mn_model_set_weights(mn_model* m, int sub, const mn_nerf_weights* w, void* stream);
+/* A weight repack that a CUDA graph can replay.  mn_model_bind_weights records the tensors of *w as the sources of sub-module
+ * `sub` - they must stay allocated at the same addresses (a training step updates parameters in place) - and, once every
+ * sub-module is bound, builds the model's table of re-layouts in device memory.  It allocates the fp16 forward images if they
+ * do not exist yet, synchronises the device and uploads the table: a set-up call, not for a captured region.  The transposed
+ * images of the tensor-core backward are covered iff they exist when the sub-module is bound - the first recording call on the
+ * tensor cores allocates them; a network trained in fp32 never holds them.  Binding a sub-module again replaces its sources; a
+ * table that a graph captured earlier may read is never freed before the model (an identical table is reused).
+ * mn_model_repack then re-packs every image of every sub-module from the bound tensors - the fp32 layouts, the fp16 forward
+ * images and the transposed data-gradient images - in two launches on `stream`, with no host upload and no allocation, the same
+ * images mn_model_set_weights writes from the same values.  MN_ERR_INVALID until every sub-module is bound, and if the
+ * transposed images were allocated after a sub-module was bound (bind it again). */
+int mn_model_bind_weights(mn_model* m, int sub, const mn_nerf_weights* w);
+int mn_model_repack(mn_ctx* ctx, mn_model* m, void* stream);
 
 /* Where the per-row model inputs come from.  Mirrors the two ways the reference builds rows:
  *   mode 0 — an explicit row matrix x [B, cols] as handed to nn.Module.__call__ (nerf.py:115);
@@ -485,6 +498,42 @@ int mn_model_forward_train_tc(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int
 size_t mn_model_backward_workspace_bytes_tc(const mn_model* m, int64_t B);
 int mn_model_backward_tc(mn_ctx* ctx, mn_model* m, int64_t B, int use_coarse, const float* grad_out_d, const void* tape_d,
                          size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream);
+
+/* ---- the recording foreground render in one call ------------------------- mega_nerf/rendering.py:15-248, train mode ----
+ * render_rays(nerf, bg_nerf=None, ...) while training (runner.py:347-358): the stage entry points of the training path in their
+ * order - coarse depths with jitter, recording coarse query (+ SH head), the cascade's coarse colour, the weights of the
+ * detached coarse composite, inverse-CDF resampling, sort_cat under use_cascade, recording fine query, merge + volume
+ * rendering - sequenced on `stream` with no allocation and no host sync, the same results as those calls.  Every random input
+ * is the caller's, drawn as the reference draws it:
+ *   jitter_d [N, coarse_samples] (torch.rand; NULL iff perturb == 0); sigma_noise_coarse_d [N * coarse_samples] and
+ *   sigma_noise_fine_d [N * Sq] (Sq = fine_samples, or coarse_samples + fine_samples under use_cascade; NULL: no noise);
+ *   u_fine_d [N, fine_samples] (torch.rand, or the rows of torch.linspace(0, 1, fine_samples) when perturb == 0).
+ * fine_samples > 0; z_steps_d, use_cascade, sh_deg and image_indices_d as for mn_render_rays.  precision MN_PREC_FP32 (the
+ * kernels of mn_model_forward_train) or MN_PREC_TC_F16 (those of mn_model_forward_train_tc, same coverage and errors).
+ * Outputs: rgb_out_d [N,3] rgb_fine; depth_out_d / depth_var_out_d optional [N]; rgb_coarse_out_d [N,3], required under
+ * use_cascade.  tape_d (mn_render_rays_train_tape_bytes) receives what the backward needs - the composite inputs and both model
+ * tapes - and must stay untouched until mn_render_rays_train_backward has consumed it; its layout depends on (N, coarse_samples,
+ * fine_samples, use_cascade, sh_deg, precision) and the model only.  workspace_d: mn_render_rays_train_workspace_bytes.
+ * mn_render_rays_train_backward (same N, sample counts, flags, precision and tape): grad_rgb_d [N,3] = dL/d rgb_fine and, under
+ * use_cascade, grad_rgb_coarse_d [N,3] = dL/d rgb_coarse (NULL: no gradient, the coarse query's backward is skipped); runs the
+ * composite backward(s), then the fine and the coarse model backward, and ACCUMULATES the parameter gradients into
+ * param_grads_d as mn_model_backward does (mn_model_grad_floats, mn_model_param_offsets).  No host sync. */
+size_t mn_render_rays_train_tape_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                       int sh_deg, int precision);
+size_t mn_render_rays_train_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                            int sh_deg, int precision);
+int mn_render_rays_train(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N,
+                         const float* z_steps_d, const float* jitter_d, float perturb, int coarse_samples,
+                         const float* sigma_noise_coarse_d, const float* u_fine_d, const float* sigma_noise_fine_d, int fine_samples,
+                         int use_cascade, int sh_deg, int precision, float* rgb_out_d, float* depth_out_d, float* depth_var_out_d,
+                         float* rgb_coarse_out_d, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes,
+                         void* stream);
+size_t mn_render_rays_train_backward_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples,
+                                                     int use_cascade, int sh_deg, int precision);
+int mn_render_rays_train_backward(mn_ctx* ctx, mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                  int sh_deg, int precision, const float* grad_rgb_d, const float* grad_rgb_coarse_d,
+                                  const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d,
+                                  size_t workspace_bytes, void* stream);
 
 /* ---- test hook (host only, no CUDA call) ---------------------------------------------------------------------------
  * The stage program of the tensor-core MLP kernel (csrc/mn_mlp_wg.cuh, precision tc_f16) for one network shape: `desc` as for

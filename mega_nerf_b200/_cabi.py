@@ -86,6 +86,8 @@ SIGNATURES = {
     'mn_model_destroy': (None, [_P]),
     'mn_model_set_centroids': (_I, [_P, _P, _P]),
     'mn_model_set_weights': (_I, [_P, _I, C.POINTER(NerfWeights), _P]),
+    'mn_model_bind_weights': (_I, [_P, _I, C.POINTER(NerfWeights)]),
+    'mn_model_repack': (_I, [_P, _P, _P]),
     'mn_model_set_max_multiplicity': (_I, [_P, _I]),
     'mn_model_workspace_bytes': (_Z, [_P, _L, _I]),
     'mn_model_forward': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _I, _P, _I, _P, _P, _Z, _P]),
@@ -132,6 +134,12 @@ SIGNATURES = {
     'mn_model_forward_train_tc': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _P, _P, _P, _Z, _P, _Z, _P]),
     'mn_model_backward_workspace_bytes_tc': (_Z, [_P, _L]),
     'mn_model_backward_tc': (_I, [_P, _P, _L, _I, _P, _P, _Z, _P, _P, _Z, _P]),
+    'mn_render_rays_train_tape_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train': (_I, [_P, _P, _P, _P, _L, _P, _P, _F, _I, _P, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _Z, _P, _Z,
+                                  _P]),
+    'mn_render_rays_train_backward_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_backward': (_I, [_P, _P, _L, _I, _I, _I, _I, _I, _P, _P, _P, _Z, _P, _P, _Z, _P]),
     'mn_debug_tc_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),
     'mn_debug_tc_forward_record': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _P, _P, _P, _Z, _P, _Z, _P]),
     'mn_debug_fp32_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),

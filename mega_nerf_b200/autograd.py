@@ -112,3 +112,82 @@ class _ShFn(torch.autograd.Function):
 
 def sh_apply(sg, deg, coef, dirs, S) -> torch.Tensor:
     return _ShFn.apply(sg, deg, coef, dirs, S)
+
+
+class RenderTrainCall:
+    """One mn_render_rays_train call: its inputs (the random draws included), then its tape until the backward consumed it."""
+
+    def __init__(self, native, rays, idx, steps, jitter, perturb, noise_c, u, noise_f, Sc, Sf, cascade, sh_deg, get_depth,
+                 get_depth_variance):
+        self.native, self.rays, self.idx, self.steps, self.jitter, self.perturb = native, rays, idx, steps, jitter, perturb
+        self.noise_c, self.u, self.noise_f = noise_c, u, noise_f
+        self.Sc, self.Sf, self.cascade, self.sh_deg = Sc, Sf, cascade, sh_deg
+        self.get_depth, self.get_depth_variance = get_depth, get_depth_variance
+        # the recording kernels of set_train_precision where they cover the network (NativeModel.train_on_tensor_cores)
+        self.prec = K.PREC_TC_F16 if native.train_on_tensor_cores() else K.PREC_FP32
+        self.tape = None
+
+    def _sizes(self):
+        return (self.native.handle, self.rays.shape[0], self.Sc, self.Sf, int(self.cascade), self.sh_deg, self.prec)
+
+    def forward(self):
+        L, dev = K.lib(), self.rays.device
+        h = K.ctx(dev)
+        N = self.rays.shape[0]
+        new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
+        rgb = new(N, 3)
+        rgb_coarse = new(N, 3) if self.cascade else None
+        depth = new(N) if self.get_depth else None
+        var = new(N) if self.get_depth_variance else None
+        self.tape = torch.empty(max(int(L.mn_render_rays_train_tape_bytes(*self._sizes())), 256), device=dev, dtype=torch.uint8)
+        ws = torch.empty(max(int(L.mn_render_rays_train_workspace_bytes(*self._sizes())), 256), device=dev, dtype=torch.uint8)
+        K.check(L.mn_render_rays_train(h, self.native.handle, K.ptr(self.rays), K.ptr(self.idx), N, K.ptr(self.steps),
+                                       K.ptr(self.jitter), self.perturb, self.Sc, K.ptr(self.noise_c), K.ptr(self.u),
+                                       K.ptr(self.noise_f), self.Sf, int(self.cascade), self.sh_deg, self.prec, K.ptr(rgb),
+                                       K.ptr(depth), K.ptr(var), K.ptr(rgb_coarse), K.ptr(self.tape), self.tape.numel(), K.ptr(ws),
+                                       ws.numel(), K.stream_of(dev)), h)
+        return rgb, rgb_coarse, depth, var
+
+    def backward(self, g_rgb, g_rgb_coarse, params):
+        L, dev = K.lib(), self.rays.device
+        h = K.ctx(dev)
+        N = self.rays.shape[0]
+        gbuf = torch.zeros(int(L.mn_model_grad_floats(self.native.handle)), device=dev, dtype=torch.float32)
+        ws = torch.empty(max(int(L.mn_render_rays_train_backward_workspace_bytes(*self._sizes())), 256), device=dev,
+                         dtype=torch.uint8)
+        g_rgb = K.f32c(g_rgb) if g_rgb is not None else torch.zeros(N, 3, device=dev, dtype=torch.float32)
+        g_rgb_coarse = K.f32c(g_rgb_coarse) if g_rgb_coarse is not None else None
+        K.check(L.mn_render_rays_train_backward(h, self.native.handle, N, self.Sc, self.Sf, int(self.cascade), self.sh_deg,
+                                                self.prec, K.ptr(g_rgb), K.ptr(g_rgb_coarse), K.ptr(self.tape), self.tape.numel(),
+                                                K.ptr(gbuf), K.ptr(ws), ws.numel(), K.stream_of(dev)), h)
+        self.tape = None
+        return self.native.grad_views(gbuf, params)
+
+
+class _RenderTrainFn(torch.autograd.Function):
+    """render_rays_train (render.py): the whole recording render as one node; outputs rgb_fine, rgb_coarse (Cascade), depth and
+    depth variance (no gradient, rendering.py:381)."""
+
+    @staticmethod
+    def forward(ctx, call, *params):
+        ctx.set_materialize_grads(False)
+        rgb, rgb_coarse, depth, var = call.forward()
+        ctx.call = call
+        ctx.plist = call.native.param_list()
+        assert len(ctx.plist) == len(params)
+        nd = [t for t in (depth, var) if t is not None]
+        if nd:
+            ctx.mark_non_differentiable(*nd)
+        return rgb, rgb_coarse, depth, var
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_rgb_coarse, g_depth, g_var):
+        grads = ctx.call.backward(g_rgb, g_rgb_coarse, ctx.plist)
+        ctx.call = None
+        need = ctx.needs_input_grad[1:]
+        return (None,) + tuple(g if n else None for g, n in zip(grads, need))
+
+
+def render_train_apply(call: RenderTrainCall):
+    params = [p for _, _, p in call.native.param_list()]
+    return _RenderTrainFn.apply(call, *params)

@@ -1,61 +1,85 @@
 // Context / model management and the nn.Module-level forward entry point of the C ABI.
 #include <cuda_fp16.h>
 
+#include <cstring>
 #include <vector>
 
 #include "mn_model.cuh"
 
 namespace {
 
-__global__ void __launch_bounds__(256) pack_ops_kernel(const PackOp* __restrict__ ops) {
-    const PackOp op = ops[blockIdx.y];
+// Element i of one re-layout (PackOp).
+__device__ __forceinline__ void pack_elem(const PackOp& op, long long i) {
     const float* __restrict__ src = op.src;
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < op.count; i += (long long)gridDim.x * blockDim.x) {
-        switch (op.kind) {
-            case PK_COPY:
-                reinterpret_cast<float*>(op.dst)[i] = src[i];
-                break;
-            case PK_TRANSPOSE: {      // src [N][K] (nn.Linear weight, [out,in]) -> dst [K][N]
-                const int N = op.p[0], K = op.p[1];
-                const int k = (int)(i / N), n = (int)(i % N);
-                reinterpret_cast<float*>(op.dst)[i] = src[(long long)n * K + k];
-                break;
-            }
-            case PK_SUBMATRIX: {      // src [N][K] -> dst [N][kw] = src[:, koff : koff + kw]
-                const int K = op.p[1], koff = op.p[2], kw = op.p[3];
-                const int n = (int)(i / kw), k = (int)(i % kw);
-                reinterpret_cast<float*>(op.dst)[i] = src[(long long)n * K + koff + k];
-                break;
-            }
-            // K-major Wt[k][n_src] fp32 -> the tensor-core image [N/nw][K/8][nw][8] fp16, optional fp16 residual (lo).  Source
-            // column ks of image column k: the first k_pad0 image columns hold k_real0 source columns and zero padding, the rest
-            // follow contiguously; columns and rows past the source are zero.
-            case PK_TC_HALF: {
-                const int n_src = op.p[0], k_src = op.p[1], K = op.p[3], k_real0 = op.p[4], k_pad0 = op.p[5], nw = op.p[6];
-                const int k8 = (int)(i % 8), n = (int)((i / 8) % nw);
-                const long long rest = i / (8 * (long long)nw);
-                const int kc = (int)(rest % (K / 8)), hh = (int)(rest / (K / 8));
-                const int k = kc * 8 + k8, ng = hh * nw + n;
-                int ks;
-                if (k < k_pad0) ks = k < k_real0 ? k : -1;
-                else ks = k_real0 + (k - k_pad0);
-                float v = 0.0f;
-                if (ks >= 0 && ks < k_src && ng < n_src) v = src[(long long)ks * n_src + ng];
-                const __half h = __float2half_rn(v);
-                reinterpret_cast<__half*>(op.dst)[i] = h;
-                if (op.dst2) reinterpret_cast<__half*>(op.dst2)[i] = __float2half_rn(v - __half2float(h));
-                break;
-            }
-            case PK_TC_F32:           // copy with zero padding
-                reinterpret_cast<float*>(op.dst)[i] = i < op.p[0] ? src[i] : 0.0f;
-                break;
-            case PK_RGBW: {           // K-major Wt[k][c] -> [c][k], rows p[2] floats apart (0: K)
-                const int K = op.p[0], Cc = op.p[1], ld = op.p[2] > 0 ? op.p[2] : K;
-                reinterpret_cast<float*>(op.dst)[(i % Cc) * ld + i / Cc] = src[i];
-                break;
-            }
+    switch (op.kind) {
+        case PK_COPY:
+            reinterpret_cast<float*>(op.dst)[i] = src[i];
+            break;
+        case PK_TRANSPOSE: {      // src [N][K] (nn.Linear weight, [out,in]) -> dst [K][N]
+            const int N = op.p[0], K = op.p[1];
+            const int k = (int)(i / N), n = (int)(i % N);
+            reinterpret_cast<float*>(op.dst)[i] = src[(long long)n * K + k];
+            break;
+        }
+        case PK_SUBMATRIX: {      // src [N][K] -> dst [N][kw] = src[:, koff : koff + kw]
+            const int K = op.p[1], koff = op.p[2], kw = op.p[3];
+            const int n = (int)(i / kw), k = (int)(i % kw);
+            reinterpret_cast<float*>(op.dst)[i] = src[(long long)n * K + koff + k];
+            break;
+        }
+        // K-major Wt[k][n_src] fp32 -> the tensor-core image [N/nw][K/8][nw][8] fp16, optional fp16 residual (lo).  Source
+        // column ks of image column k: the first k_pad0 image columns hold k_real0 source columns and zero padding, the rest
+        // follow contiguously; columns and rows past the source are zero.
+        case PK_TC_HALF: {
+            const int n_src = op.p[0], k_src = op.p[1], K = op.p[3], k_real0 = op.p[4], k_pad0 = op.p[5], nw = op.p[6];
+            const int k8 = (int)(i % 8), n = (int)((i / 8) % nw);
+            const long long rest = i / (8 * (long long)nw);
+            const int kc = (int)(rest % (K / 8)), hh = (int)(rest / (K / 8));
+            const int k = kc * 8 + k8, ng = hh * nw + n;
+            int ks;
+            if (k < k_pad0) ks = k < k_real0 ? k : -1;
+            else ks = k_real0 + (k - k_pad0);
+            float v = 0.0f;
+            if (ks >= 0 && ks < k_src && ng < n_src) v = src[(long long)ks * n_src + ng];
+            const __half h = __float2half_rn(v);
+            reinterpret_cast<__half*>(op.dst)[i] = h;
+            if (op.dst2) reinterpret_cast<__half*>(op.dst2)[i] = __float2half_rn(v - __half2float(h));
+            break;
+        }
+        case PK_TC_F32:           // copy with zero padding
+            reinterpret_cast<float*>(op.dst)[i] = i < op.p[0] ? src[i] : 0.0f;
+            break;
+        case PK_RGBW: {           // K-major Wt[k][c] -> [c][k], rows p[2] floats apart (0: K)
+            const int K = op.p[0], Cc = op.p[1], ld = op.p[2] > 0 ? op.p[2] : K;
+            reinterpret_cast<float*>(op.dst)[(i % Cc) * ld + i / Cc] = src[i];
+            break;
         }
     }
+}
+
+__global__ void __launch_bounds__(256) pack_ops_kernel(const PackOp* __restrict__ ops) {
+    const PackOp op = ops[blockIdx.y];
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < op.count; i += (long long)gridDim.x * blockDim.x)
+        pack_elem(op, i);
+}
+
+// mn_model_repack: one launch over a resident table of every sub-module's re-layouts, cut into chunks of kRepackChunk elements
+// so that the blocks share the work evenly whatever the sizes of the ops (a 2048 x 2048 weight and a 1-float bias alike).
+// first[j] is the first chunk of op j (first[n_ops] = the launch's chunks); block b runs chunk b of the op that holds it.
+constexpr int kRepackChunk = 4096;
+
+__global__ void __launch_bounds__(256) repack_kernel(const PackOp* __restrict__ ops, const long long* __restrict__ first, int n_ops) {
+    const long long b = blockIdx.x;
+    int lo = 0, hi = n_ops - 1;              // the last op whose first chunk is <= b (ops of no chunk are skipped over)
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (first[mid] <= b) lo = mid;
+        else hi = mid - 1;
+    }
+    const PackOp op = ops[lo];
+    const long long i0 = (b - first[lo]) * kRepackChunk;
+    const long long i1 = op.count < i0 + kRepackChunk ? op.count : i0 + kRepackChunk;
+    for (long long i = i0 + threadIdx.x; i < i1; i += 256) pack_elem(op, i);
 }
 
 void pack_T(mn_ctx* ctx, const float* src, int N, int K, float* dst) {
@@ -305,6 +329,9 @@ void mn_model_destroy(mn_model* m) {
     if (m->counters_d) cudaFree(m->counters_d);
     if (m->tc_packed) cudaFree(m->tc_packed);
     if (m->tc_dgrad) cudaFree(m->tc_dgrad);
+    if (m->repack_ops) cudaFree(m->repack_ops);
+    if (m->repack_first) cudaFree(m->repack_first);
+    for (void* p : m->repack_retired) cudaFree(p);
     delete m;
 }
 
@@ -322,14 +349,14 @@ int mn_model_set_centroids(mn_model* m, const float* centroids_d, void* stream) 
     return MN_OK;
 }
 
-int mn_model_set_weights(mn_model* m, int sub, const mn_nerf_weights* w, void* stream) {
-    if (!m || !w || sub < 0 || sub >= m->d.n_sub) return MN_ERR_INVALID;
-    mn_ctx* ctx = m->ctx;
-    cudaStream_t st = (cudaStream_t)stream;
+}  // extern "C"
+
+// Queues the fp32 re-layouts of sub-module `sub` from the tensors of *w (ctx->pack_ops): the forward layouts and the data-gradient
+// images.  The fp16 tensor-core images (mn_mlp_tc_pack) read the forward layouts, so they go in a second launch.
+static int queue_weight_ops(mn_ctx* ctx, mn_model* m, int sub, const mn_nerf_weights* w) {
     const NetDims& nd = m->nd;
     const PackedLayout& l = m->lay;
     float* P = m->packed + (size_t)sub * l.total;
-    ctx->pack_ops.clear();
     auto copy = [&](float* dst, const float* src, size_t n) -> int {
         if (!src) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_set_weights: missing tensor");
         PackOp op{src, dst, nullptr, (long long)n, PK_COPY, {0, 0, 0, 0, 0, 0, 0}};
@@ -372,10 +399,116 @@ int mn_model_set_weights(mn_model* m, int sub, const mn_nerf_weights* w, void* s
             if (nd.app_in_dira) pack_sub(ctx, w->dir_a_w, nd.L / 2, nd.L + nd.aux, nd.L + nd.in_dir, nd.app, Q + bl.dira_e);
         }
     }
+    return MN_OK;
+}
+
+// The resident table of mn_model_repack from the bound re-layouts of every sub-module (host work and a synchronous upload).
+static int upload_repack_table(mn_ctx* ctx, mn_model* m) {
+    std::vector<PackOp> ops;
+    std::vector<long long> first;
+    int n_ops[2];
+    long long n_chunks[2];
+    for (int k = 0; k < 2; ++k) {
+        long long chunks = 0;
+        const size_t n0 = ops.size();
+        for (const auto& sub_ops : m->bound_ops[k])
+            for (const PackOp& op : sub_ops) {
+                ops.push_back(op);
+                first.push_back(chunks);
+                chunks += mn_cdiv(op.count, kRepackChunk);
+            }
+        first.push_back(chunks);
+        n_ops[k] = (int)(ops.size() - n0);
+        n_chunks[k] = chunks;
+    }
+    // A graph captured earlier holds the current table as kernel arguments: an identical table is kept, a different one goes to a
+    // new allocation and the old one stays allocated (retired) until the model is destroyed.
+    if (m->repack_ops && ops.size() == m->repack_host_ops.size() && first == m->repack_host_first &&
+        (ops.empty() || !memcmp(ops.data(), m->repack_host_ops.data(), ops.size() * sizeof(PackOp))))
+        return MN_OK;
+    PackOp* ops_d = nullptr;
+    long long* first_d = nullptr;
+    MN_CUDA(ctx, cudaMalloc(&ops_d, (ops.size() > 0 ? ops.size() : 1) * sizeof(PackOp)));
+    const cudaError_t e = cudaMalloc(&first_d, first.size() * sizeof(long long));
+    if (e != cudaSuccess) { cudaFree(ops_d); MN_CUDA(ctx, e); }
+    if (!ops.empty()) MN_CUDA(ctx, cudaMemcpy(ops_d, ops.data(), ops.size() * sizeof(PackOp), cudaMemcpyHostToDevice));
+    MN_CUDA(ctx, cudaMemcpy(first_d, first.data(), first.size() * sizeof(long long), cudaMemcpyHostToDevice));
+    if (m->repack_ops) {
+        m->repack_retired.push_back(m->repack_ops);
+        m->repack_retired.push_back(m->repack_first);
+    }
+    m->repack_ops = ops_d;
+    m->repack_first = first_d;
+    m->repack_host_ops.swap(ops);
+    m->repack_host_first.swap(first);
+    for (int k = 0; k < 2; ++k) {
+        m->repack_n[k] = n_ops[k];
+        m->repack_chunks[k] = n_chunks[k];
+    }
+    return MN_OK;
+}
+
+extern "C" {
+
+int mn_model_set_weights(mn_model* m, int sub, const mn_nerf_weights* w, void* stream) {
+    if (!m || !w || sub < 0 || sub >= m->d.n_sub) return MN_ERR_INVALID;
+    mn_ctx* ctx = m->ctx;
+    cudaStream_t st = (cudaStream_t)stream;
+    ctx->pack_ops.clear();
+    int rc;
+    if ((rc = queue_weight_ops(ctx, m, sub, w))) return rc;
     // launch 1: the fp32 layouts; launch 2 (queued by mn_mlp_tc_pack): the fp16 images that read them
     if ((rc = mn_pack_flush(ctx, st))) return rc;
     if ((rc = mn_mlp_tc_pack(ctx, m, sub, st))) { ctx->pack_ops.clear(); return rc; }
     return mn_pack_flush(ctx, st);
+}
+
+int mn_model_bind_weights(mn_model* m, int sub, const mn_nerf_weights* w) {
+    if (!m || !w || sub < 0 || sub >= m->d.n_sub) return MN_ERR_INVALID;
+    mn_ctx* ctx = m->ctx;
+    // Every image the repack writes must exist before its re-layouts are recorded: the forward images are allocated by the first
+    // mn_mlp_tc_pack below (on the legacy stream, which orders it after the caller's work).  The transposed images of the
+    // tensor-core backward are covered iff they exist, i.e. after a first recording call on the tensor cores: a network trained
+    // in fp32 never holds them.
+    MN_CUDA(ctx, cudaDeviceSynchronize());
+    ctx->pack_ops.clear();
+    int rc;
+    if ((rc = queue_weight_ops(ctx, m, sub, w))) { ctx->pack_ops.clear(); return rc; }
+    std::vector<PackOp> f32_ops;
+    f32_ops.swap(ctx->pack_ops);
+    if ((rc = mn_mlp_tc_pack(ctx, m, sub, 0))) { ctx->pack_ops.clear(); return rc; }
+    std::vector<PackOp> f16_ops;
+    f16_ops.swap(ctx->pack_ops);
+    MN_CUDA(ctx, cudaStreamSynchronize(0));
+    const int n_sub = m->d.n_sub;
+    for (int k = 0; k < 2; ++k) m->bound_ops[k].resize(n_sub);
+    m->bound.resize(n_sub, 0);
+    m->bound_ops[0][sub].swap(f32_ops);
+    m->bound_ops[1][sub].swap(f16_ops);
+    m->bound[sub] = 1;
+    m->bound_dgrad.resize(n_sub, 0);
+    m->bound_dgrad[sub] = m->tc_dgrad != nullptr;
+    for (int s = 0; s < n_sub; ++s)
+        if (!m->bound[s]) return MN_OK;     // the table is built once every sub-module is bound
+    return upload_repack_table(ctx, m);
+}
+
+int mn_model_repack(mn_ctx* ctx, mn_model* m, void* stream) {
+    if (!ctx || !m) return MN_ERR_INVALID;
+    if (!m->repack_ops) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_repack: bind the weights of every sub-module first (mn_model_bind_weights)");
+    for (char with : m->bound_dgrad)
+        if (m->tc_dgrad && !with)
+            return mn_fail(ctx, MN_ERR_INVALID, "mn_model_repack: the transposed images of the tensor-core backward were allocated "
+                                                "after the weights were bound (a first recording call on the tensor cores): bind again");
+    cudaStream_t st = (cudaStream_t)stream;
+    // launch 0: the fp32 layouts; launch 1: the fp16 images (forward and data-gradient) that read them
+    for (int k = 0, off = 0; k < 2; off += m->repack_n[k] + 1, ++k) {
+        if (m->repack_chunks[k] == 0) continue;
+        const int op0 = k == 0 ? 0 : m->repack_n[0];
+        repack_kernel<<<(unsigned)m->repack_chunks[k], 256, 0, st>>>(m->repack_ops + op0, m->repack_first + off, m->repack_n[k]);
+        MN_LAUNCH_CHECK(ctx);
+    }
+    return MN_OK;
 }
 
 // mult: sub-modules per row the slots are sized for; 0 = the model's max_multiplicity

@@ -150,6 +150,18 @@ struct mn_model {
     void* tc_packed = nullptr;
     // transposed fp16 weight images of the tensor-core data-gradient chain (mn_train_tc.cuh); NULL if the shape is not covered
     void* tc_dgrad = nullptr;
+    // weights bound by mn_model_bind_weights: per sub-module, the re-layouts of launch 0 (fp32 layouts) and launch 1 (the fp16
+    // images that read them), and, once every sub-module is bound, their resident table for mn_model_repack (csrc/mn_api.cu)
+    std::vector<std::vector<PackOp>> bound_ops[2];
+    std::vector<char> bound;
+    std::vector<char> bound_dgrad;      // per sub-module: bound with the transposed images of the backward (tc_dgrad) in its ops
+    PackOp* repack_ops = nullptr;       // [n_ops[0] + n_ops[1]]
+    long long* repack_first = nullptr;  // per launch: first chunk of each op, then the launch's chunk count [n_ops + 1]
+    int repack_n[2] = {0, 0};
+    long long repack_chunks[2] = {0, 0};
+    std::vector<PackOp> repack_host_ops;        // the table's contents
+    std::vector<long long> repack_host_first;
+    std::vector<void*> repack_retired;          // earlier tables, which captured graphs may still read (freed with the model)
 };
 
 // counters_d layout (ints)

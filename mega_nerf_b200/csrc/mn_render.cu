@@ -493,6 +493,189 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
     return MN_OK;
 }
 
+// ---- mn_render_rays_train: the recording foreground render and its backward ------------------------------------------------
+// The tape holds what the backward reads - the composite inputs (last delta, coarse and fine-query depths, raw rows), the raw SH
+// coefficients and a copy of the rays (their directions) for an SH head, and the tapes of the two model calls; the forward
+// workspace holds the rest (points, weights, the fine draws before sort_cat, the model calls' workspace); the backward workspace
+// the per-sample gradients and the model backward's workspace.
+struct TrainPlan {
+    int S, F, Sq;
+    bool tc, sh;
+    size_t last_delta, z_c, raw_c, z_q, raw_f, mlp_c, mlp_f, rays, tape_c, tape_f, tape_c_bytes, tape_f_bytes, tape_total;
+    size_t xyz_c, w_c, z_f, xyz_f, model_ws, model_ws_bytes, ws_total;
+    size_t g_raw_c, g_raw_f, g_mlp_c, g_mlp_f, bwd_ws, bwd_ws_bytes, bwd_total;
+};
+
+TrainPlan make_train_plan(const mn_model* m, int64_t N, int S, int F, int use_cascade, bool sh, bool tc) {
+    TrainPlan p{};
+    p.S = S; p.F = F; p.Sq = use_cascade ? S + F : F; p.tc = tc; p.sh = sh;
+    const int64_t Bc = N * S, Bf = N * p.Sq;
+    const int out_cols = m->nd.rgb_dim + 1;
+    Carve t;
+    p.last_delta = t((size_t)N * 4);
+    p.z_c = t((size_t)Bc * 4);
+    p.raw_c = t((size_t)Bc * 16);
+    p.z_q = t((size_t)Bf * 4);
+    p.raw_f = t((size_t)Bf * 16);
+    p.mlp_c = sh ? t((size_t)Bc * out_cols * 4) : kNone;
+    p.mlp_f = sh ? t((size_t)Bf * out_cols * 4) : kNone;
+    p.rays = sh ? t((size_t)N * 32) : kNone;
+    p.tape_c_bytes = tc ? mn_model_tape_bytes_tc(m, Bc) : mn_model_tape_bytes(m, Bc);
+    p.tape_f_bytes = tc ? mn_model_tape_bytes_tc(m, Bf) : mn_model_tape_bytes(m, Bf);
+    p.tape_c = t(p.tape_c_bytes);
+    p.tape_f = t(p.tape_f_bytes);
+    p.tape_total = t.off + 256;
+    Carve w;
+    p.xyz_c = w((size_t)Bc * 12);
+    p.w_c = w((size_t)Bc * 4);
+    p.z_f = use_cascade ? w((size_t)N * F * 4) : p.z_q;     // without cascade the fine draws are the fine-query depths (tape)
+    p.xyz_f = w((size_t)Bf * 12);
+    const size_t a = mn_model_workspace_bytes(m, Bc, MN_PREC_FP32), c = mn_model_workspace_bytes(m, Bf, MN_PREC_FP32);
+    p.model_ws_bytes = a > c ? a : c;
+    p.model_ws = w(p.model_ws_bytes);
+    p.ws_total = w.off + 256;
+    Carve b;
+    p.g_raw_c = b((size_t)Bc * 16);
+    p.g_raw_f = b((size_t)Bf * 16);
+    p.g_mlp_c = sh ? b((size_t)Bc * out_cols * 4) : kNone;
+    p.g_mlp_f = sh ? b((size_t)Bf * out_cols * 4) : kNone;
+    const size_t ba = tc ? mn_model_backward_workspace_bytes_tc(m, Bc) : mn_model_backward_workspace_bytes(m, Bc);
+    const size_t bc = tc ? mn_model_backward_workspace_bytes_tc(m, Bf) : mn_model_backward_workspace_bytes(m, Bf);
+    p.bwd_ws_bytes = ba > bc ? ba : bc;
+    p.bwd_ws = b(p.bwd_ws_bytes);
+    p.bwd_total = b.off + 256;
+    return p;
+}
+
+// The checks shared by the train render, its backward and their size queries: a foreground network that trains at `precision`.
+int check_train(mn_ctx* ctx, const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int precision, const char* name) {
+    const std::string n(name);
+    if (N < 0 || coarse_samples < 3 || fine_samples < 1)
+        return mn_fail(ctx, MN_ERR_INVALID, n + ": needs N >= 0, >= 3 coarse samples (resampling) and fine_samples > 0");
+    if (precision != MN_PREC_FP32 && precision != MN_PREC_TC_F16)
+        return mn_fail(ctx, MN_ERR_INVALID, n + ": training precision is MN_PREC_FP32 or MN_PREC_TC_F16");
+    if (precision == MN_PREC_TC_F16 && !mn_model_train_tc_supported(m)) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
+    return MN_OK;
+}
+
+int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N, const float* z_steps_d,
+               const float* jitter_d, float perturb, int S, const float* noise_c_d, const float* u_d, const float* noise_f_d, int F,
+               int use_cascade, int sh_deg, int precision, float* rgb, float* depth, float* var, float* rgb_coarse, void* tape_d,
+               size_t tape_bytes, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+    const char* name = "mn_render_rays_train";
+    const std::string nm(name);
+    if (!ctx || !m || !rays_d || !z_steps_d || !u_d || !rgb) return MN_ERR_INVALID;
+    int rc;
+    if ((rc = check_train(ctx, m, N, S, F, precision, name))) return rc;
+    if ((rc = check_net(ctx, m, use_cascade, F, sh_deg, image_indices_d, name))) return rc;
+    if (perturb > 0 && !jitter_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": perturb > 0 needs jitter_d");
+    if (use_cascade && !rgb_coarse) return mn_fail(ctx, MN_ERR_INVALID, nm + ": rgb_coarse_out_d is required under use_cascade");
+    if (N == 0) return MN_OK;
+    const bool sh = sh_deg >= 0, tc = precision == MN_PREC_TC_F16;
+    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh, tc);
+    if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
+    if (!workspace_d || workspace_bytes < p.ws_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
+    char* T = (char*)tape_d;
+    char* W = (char*)workspace_d;
+    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(T + off); };
+    auto WF = [&](size_t off) { return reinterpret_cast<float*>(W + off); };
+    const LiveRows all{};
+
+    // one recording model query on [N, Sq, 3] points -> raw [N, Sq, 4], into the model tape at `tape` (render.py `_query`)
+    auto query = [&](const float* xyz, int Sq, int coarse, const float* noise, float* mlp_out, float* raw_out, size_t tape,
+                     size_t tape_n) -> int {
+        mn_rows rows{};
+        rows.mode = 1;
+        rows.x_d = xyz;
+        rows.cols = 3;
+        rows.dirs_d = m->d.pos_dir_dim > 0 ? rays_d + 3 : nullptr;
+        rows.dir_stride = 8;
+        rows.idx_d = image_indices_d;
+        rows.samples_per_ray = Sq;
+        float* out = sh ? mlp_out : raw_out;
+        auto fn = tc ? mn_model_forward_train_tc : mn_model_forward_train;
+        int r = fn(ctx, m, &rows, N * Sq, coarse, noise, out, T + tape, tape_n, W + p.model_ws, p.model_ws_bytes, st);
+        if (r) return r;
+        if (sh) return mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, m->nd.rgb_dim + 1, rays_d + 3, 8, Sq, N * Sq, 1, all, raw_out, st);
+        return MN_OK;
+    };
+
+    fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(TF(p.last_delta), N, 1e10f);     // no background: rendering.py:33
+    MN_LAUNCH_CHECK(ctx);
+    if (sh) MN_CUDA(ctx, cudaMemcpyAsync(T + p.rays, rays_d, (size_t)N * 32, cudaMemcpyDeviceToDevice, st));
+    if ((rc = mn_sample_coarse(ctx, rays_d, nullptr, z_steps_d, jitter_d, perturb, N, S, TF(p.z_c), WF(p.xyz_c), st))) return rc;
+    if ((rc = query(WF(p.xyz_c), S, 1, noise_c_d, TF(p.mlp_c), TF(p.raw_c), p.tape_c, p.tape_c_bytes))) return rc;
+    // the cascade's coarse colour, then the resampling weights of the detached coarse composite (render.py `_two_pass`)
+    if (use_cascade)
+        if ((rc = mn_stage_composite(ctx, TF(p.raw_c), TF(p.z_c), nullptr, S, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
+                                     nullptr, rgb_coarse, nullptr, nullptr, nullptr, st)))
+            return rc;
+    if ((rc = mn_stage_composite(ctx, TF(p.raw_c), TF(p.z_c), nullptr, S, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
+                                 WF(p.w_c), nullptr, nullptr, nullptr, nullptr, st)))
+        return rc;
+    float* z_f = use_cascade ? WF(p.z_f) : TF(p.z_q);
+    if ((rc = mn_stage_sample_pdf(ctx, TF(p.z_c), WF(p.w_c), S, nullptr, u_d, F, N, S, F, all, z_f, nullptr, nullptr, st))) return rc;
+    if (use_cascade)
+        if ((rc = mn_stage_sort_cat(ctx, TF(p.z_c), S, z_f, F, N, 0, all, TF(p.z_q), nullptr, st))) return rc;
+    if ((rc = mn_points_from_z(ctx, rays_d, TF(p.z_q), N, p.Sq, WF(p.xyz_f), st))) return rc;
+    if ((rc = query(WF(p.xyz_f), p.Sq, 0, noise_f_d, TF(p.mlp_f), TF(p.raw_f), p.tape_f, p.tape_f_bytes))) return rc;
+    // depth scratch when only the variance is wanted: the coarse weights are dead by now
+    float* d = depth ? depth : (var ? WF(p.w_c) : nullptr);
+    if (use_cascade)
+        return mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_q), nullptr, p.Sq, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
+                                  nullptr, rgb, d, var, nullptr, st);
+    return mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_q), nullptr, p.Sq, TF(p.raw_c), TF(p.z_c), nullptr, S, TF(p.last_delta), N, 0,
+                              all, nullptr, rgb, d, var, nullptr, st);
+}
+
+int train_backward_impl(mn_ctx* ctx, mn_model* m, int64_t N, int S, int F, int use_cascade, int sh_deg, int precision,
+                        const float* g_rgb, const float* g_rgb_coarse, const void* tape_d, size_t tape_bytes, float* gw,
+                        void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+    const char* name = "mn_render_rays_train_backward";
+    const std::string nm(name);
+    if (!ctx || !m || !g_rgb || !gw) return MN_ERR_INVALID;
+    int rc;
+    if ((rc = check_train(ctx, m, N, S, F, precision, name))) return rc;
+    if (N == 0) return MN_OK;
+    const bool sh = sh_deg >= 0, tc = precision == MN_PREC_TC_F16;
+    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh, tc);
+    if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
+    if (!workspace_d || workspace_bytes < p.bwd_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
+    const char* T = (const char*)tape_d;
+    char* W = (char*)workspace_d;
+    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<const float*>(T + off); };
+    auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
+    const bool coarse = !use_cascade || g_rgb_coarse;     // the coarse query has a gradient
+
+    // composites: the fine one (with the coarse samples merged in, without cascade), the cascade's coarse one
+    if (use_cascade) {
+        if ((rc = mn_composite_backward(ctx, TF(p.raw_f), TF(p.z_q), p.Sq, nullptr, nullptr, 0, TF(p.last_delta), N, 0, g_rgb, nullptr,
+                                        WF(p.g_raw_f), nullptr, st)))
+            return rc;
+        if (coarse && (rc = mn_composite_backward(ctx, TF(p.raw_c), TF(p.z_c), S, nullptr, nullptr, 0, TF(p.last_delta), N, 0,
+                                                  g_rgb_coarse, nullptr, WF(p.g_raw_c), nullptr, st)))
+            return rc;
+    } else if ((rc = mn_composite_backward(ctx, TF(p.raw_f), TF(p.z_q), p.Sq, TF(p.raw_c), TF(p.z_c), S, TF(p.last_delta), N, 0, g_rgb,
+                                           nullptr, WF(p.g_raw_f), WF(p.g_raw_c), st))) {
+        return rc;
+    }
+    // the model backwards in reverse order of their forward calls, each through the SH head's backward first
+    auto model_bwd = [&](int Sq, int use_coarse, size_t mlp, size_t g_raw, size_t g_mlp, size_t tape, size_t tape_n) -> int {
+        const float* g = WF(g_raw);
+        int r;
+        if (sh) {
+            if ((r = mn_sh_to_rgb_backward(ctx, sh_deg, TF(mlp), m->nd.rgb_dim + 1, TF(p.rays) + 3, 8, Sq, N * Sq, 1, g, WF(g_mlp), st)))
+                return r;
+            g = WF(g_mlp);
+        }
+        auto fn = tc ? mn_model_backward_tc : mn_model_backward;
+        return fn(ctx, m, N * Sq, use_coarse, g, T + tape, tape_n, gw, W + p.bwd_ws, p.bwd_ws_bytes, st);
+    };
+    if ((rc = model_bwd(p.Sq, 0, p.mlp_f, p.g_raw_f, p.g_mlp_f, p.tape_f, p.tape_f_bytes))) return rc;
+    if (coarse) return model_bwd(S, 1, p.mlp_c, p.g_raw_c, p.g_mlp_c, p.tape_c, p.tape_c_bytes);
+    return MN_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -573,6 +756,44 @@ int mn_render_rays_bg_occ(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* 
     return render_impl(ctx, fg, bg, rays_d, image_indices_d, N, sphere_center3_d, sphere_radius3_d, include_xyz_real, cluster_2d,
                        z_steps_d, z_steps_bg_d, coarse_samples, u_fine_d, u_fine_bg_d, fine_samples, use_cascade, sh_deg, precision,
                        *out, workspace_d, workspace_bytes, stream, "mn_render_rays_bg_occ", occ, counts_out_d);
+}
+
+// Size queries: 0 for arguments the call would refuse.
+size_t mn_render_rays_train_tape_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                       int sh_deg, int precision) {
+    if (!m || check_train(nullptr, m, N, coarse_samples, fine_samples, precision, "")) return 0;
+    return make_train_plan(m, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16).tape_total;
+}
+
+size_t mn_render_rays_train_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                            int sh_deg, int precision) {
+    if (!m || check_train(nullptr, m, N, coarse_samples, fine_samples, precision, "")) return 0;
+    return make_train_plan(m, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16).ws_total;
+}
+
+size_t mn_render_rays_train_backward_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples,
+                                                     int use_cascade, int sh_deg, int precision) {
+    if (!m || check_train(nullptr, m, N, coarse_samples, fine_samples, precision, "")) return 0;
+    return make_train_plan(m, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16).bwd_total;
+}
+
+int mn_render_rays_train(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N,
+                         const float* z_steps_d, const float* jitter_d, float perturb, int coarse_samples,
+                         const float* sigma_noise_coarse_d, const float* u_fine_d, const float* sigma_noise_fine_d, int fine_samples,
+                         int use_cascade, int sh_deg, int precision, float* rgb_out_d, float* depth_out_d, float* depth_var_out_d,
+                         float* rgb_coarse_out_d, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes,
+                         void* stream) {
+    return train_impl(ctx, m, rays_d, image_indices_d, N, z_steps_d, jitter_d, perturb, coarse_samples, sigma_noise_coarse_d, u_fine_d,
+                      sigma_noise_fine_d, fine_samples, use_cascade, sh_deg, precision, rgb_out_d, depth_out_d, depth_var_out_d,
+                      rgb_coarse_out_d, tape_d, tape_bytes, workspace_d, workspace_bytes, (cudaStream_t)stream);
+}
+
+int mn_render_rays_train_backward(mn_ctx* ctx, mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                  int sh_deg, int precision, const float* grad_rgb_d, const float* grad_rgb_coarse_d,
+                                  const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d,
+                                  size_t workspace_bytes, void* stream) {
+    return train_backward_impl(ctx, m, N, coarse_samples, fine_samples, use_cascade, sh_deg, precision, grad_rgb_d, grad_rgb_coarse_d,
+                               tape_d, tape_bytes, param_grads_d, workspace_d, workspace_bytes, (cudaStream_t)stream);
 }
 
 }  // extern "C"

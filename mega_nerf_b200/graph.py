@@ -23,6 +23,16 @@ samples of the coarse and fine passes after each replay.  The graph reads the gr
 a different grid needs a new GraphedRenderRays.
 
     g = GraphedRenderRays(nerf, hparams, 4096, dev, occupancy=octree.occupancy_grid(hparams, nerf, offset, invradius))
+
+GraphedTrainStep does the same for a training step of a foreground network: the reference's `_training_step` and the update
+that follows it (runner.py:347-381, :265-274) - a repack of the weights from the parameters, `render_rays_train`, the loss,
+`backward()` and `optimizer.step()` - captured once and replayed with no host work besides the copy of the batch.
+
+    opt = torch.optim.Adam(nerf.parameters(), lr=torch.tensor(5e-4, device=dev), capturable=True)   # a tensor lr: schedulable
+    sched = torch.optim.lr_scheduler.ExponentialLR(opt, gamma)
+    step = GraphedTrainStep(nerf, hparams, n_rays=4096, device=dev, optimizer=opt)
+    loss, psnr, depth_variance = step.step(rays, rgbs, image_indices)   # device tensors, reused by the next step
+    sched.step()
 """
 from argparse import Namespace
 from typing import Dict, Optional
@@ -30,8 +40,11 @@ from typing import Dict, Optional
 import torch
 from torch import nn
 
+import torch.nn.functional as F
+
 from . import _cabi as K
-from .render import _refuse_bg_ep, _unwrap, render_rays, render_rays_fused
+from .modules import Cascade, MegaNeRF, NeRF
+from .render import _check_train, _refuse_bg_ep, _render_train, _unwrap, render_rays, render_rays_fused
 
 
 class GraphedRenderRays:
@@ -142,3 +155,132 @@ class GraphedRenderRays:
         self.graph.replay()
         self._check()
         return self.results
+
+
+class GraphedTrainStep:
+    def __init__(self, nerf: nn.Module, hparams: Namespace, n_rays: int, device: torch.device, optimizer: torch.optim.Optimizer,
+                 get_depth_variance: bool = True, bg_nerf: Optional[nn.Module] = None, scaler=None, warmup: int = 2):
+        """One training step of `nerf` over batches of n_rays rays as a CUDA graph.  The loss is the runner's: the MSE of rgb_fine,
+        averaged with that of rgb_coarse for a Cascade (runner.py:366-379).  `optimizer` steps every parameter it holds inside
+        the graph, so it must be capturable (`torch.optim.Adam(..., capturable=True)`).  A learning rate given as a Python number
+        is captured as a constant: to follow a schedule (the reference's ExponentialLR, runner.py:276-277) give it as a device
+        tensor, `lr=torch.tensor(5e-4, device=dev)`, which the scheduler updates in place; changing a number lr after the capture
+        raises ValueError at the next step.  The graph repacks the weights from the
+        parameters at the start of every replay, so parameters changed in place between steps (`load_state_dict`, a manual
+        edit) are what the next step trains.  Refused (ValueError): a background network (its ray split needs a host-side
+        count to draw the reference's random numbers), a network under expert parallelism or wrapped in
+        DistributedDataParallel, an optimizer that is not capturable, a GradScaler (tc_f16 scales its gradients inside the
+        library, and `scaler.step` synchronises)."""
+        if bg_nerf is not None:
+            raise ValueError('GraphedTrainStep trains a foreground network only: its background ray split needs a host-side '
+                             'count (use render_rays)')
+        if scaler is not None:
+            raise ValueError('GraphedTrainStep takes no GradScaler: scaler.step synchronises with the host')
+        if _unwrap(nerf) is not nerf or not isinstance(nerf, (NeRF, MegaNeRF, Cascade)):
+            raise ValueError('GraphedTrainStep needs a mega_nerf_b200 network itself, not a wrapper such as '
+                             'DistributedDataParallel (its gradient hooks run on the host)')
+        if getattr(nerf, '_ep', None) is not None:
+            raise ValueError('GraphedTrainStep cannot train a network under expert parallelism (its exchanges take host-side '
+                             'counts)')
+        if not all(g.get('capturable', False) for g in optimizer.param_groups):
+            raise ValueError('GraphedTrainStep needs a capturable optimizer, e.g. torch.optim.Adam(..., capturable=True)')
+        _check_train(nerf, hparams, 'GraphedTrainStep')
+        self.nerf, self.hparams, self.optimizer = nerf, hparams, optimizer
+        self.device = torch.device(device)
+        self.get_depth_variance = get_depth_variance
+        self.warmup = warmup
+        self.native = nerf._native()
+        self.rays = torch.zeros(n_rays, 8, device=self.device, dtype=torch.float32)
+        self.rgbs = torch.zeros(n_rays, 3, device=self.device, dtype=torch.float32)
+        with_indices = self.native.subs[0].appearance_dim > 0          # the network reads image indices
+        self.indices = torch.zeros(n_rays, device=self.device, dtype=torch.float32) if with_indices else None
+        self.graph: Optional[torch.cuda.CUDAGraph] = None
+        self.loss = self.psnr = self.depth_variance = None
+        self._captured_lrs = []
+
+    def _run(self, repack: bool = True):
+        """The step: repack (or, outside the graph, the host-side sync), render, loss (runner.py:366-379), backward, optimizer
+        step.  -> (loss, psnr, depth variance)."""
+        if repack:
+            self.native.repack(self.device)
+        else:
+            self.native.sync(self.device)
+        res = _render_train(self.nerf, self.native, self.rays, self.indices, self.hparams, False, self.get_depth_variance)
+        rgb = res['rgb_fine']
+        with torch.no_grad():
+            psnr = -10 * torch.log10(torch.mean((rgb - self.rgbs) ** 2))     # metrics.py:8-10, without the host read
+            dv = res['depth_variance_fine'].mean() if self.get_depth_variance else None
+        loss = F.mse_loss(rgb, self.rgbs, reduction='mean')
+        if self.hparams.use_cascade:
+            loss = (loss + F.mse_loss(res['rgb_coarse'], self.rgbs, reduction='mean')) / 2
+        loss.backward()
+        self.optimizer.step()
+        return loss.detach(), psnr, dv
+
+    def _load(self, rays, rgbs, image_indices) -> None:
+        if rays.shape != self.rays.shape or rgbs.shape != self.rgbs.shape:
+            raise ValueError(f'captured for rays {tuple(self.rays.shape)} / rgbs {tuple(self.rgbs.shape)}, got '
+                             f'{tuple(rays.shape)} / {tuple(rgbs.shape)}')
+        self.rays.copy_(rays, non_blocking=True)
+        self.rgbs.copy_(rgbs, non_blocking=True)
+        if self.indices is not None:
+            self.indices.copy_(image_indices.view(-1), non_blocking=True)   # int32 (training loaders) or float, as render_rays
+
+    def capture(self, rays, rgbs, image_indices) -> None:
+        """Warm up on a side stream (tape sizes, first launches, the optimizer's state, and on the tensor cores the transposed
+        weight images of the backward), restore the parameters, the optimizer state and the random generator as they were, bind
+        the weights - after the warm-up, so that the repack covers every image the captured step reads - then record the graph.
+        The capture itself trains nothing: the first replay is the first step."""
+        dev = self.device
+        self._load(rays, rgbs, image_indices)
+        params = [p for group in self.optimizer.param_groups for p in group['params']]
+        saved_params = [p.detach().clone() for p in params]
+        saved_state = {p: {k: v.clone() for k, v in self.optimizer.state[p].items() if torch.is_tensor(v)} for p in params
+                       if p in self.optimizer.state}
+        rng = torch.cuda.get_rng_state(dev)
+        cur = torch.cuda.current_stream(dev)
+        side = torch.cuda.Stream(dev)
+        side.wait_stream(cur)
+        with torch.cuda.stream(side):
+            for _ in range(self.warmup):
+                self.optimizer.zero_grad(set_to_none=True)
+                self._run(repack=False)
+        cur.wait_stream(side)
+        torch.cuda.synchronize(dev)
+        # The warm-up steps leave the state the capture needs (the optimizer's, allocated by its first step) but must not count
+        # as training: the parameters and the existing state go back to their values, state the warm-up created to the zeros a
+        # fresh Adam starts from, the generator to where it was.
+        with torch.no_grad():
+            for p, v in zip(params, saved_params):
+                p.copy_(v)
+            for p in params:
+                for k, v in self.optimizer.state.get(p, {}).items():
+                    if torch.is_tensor(v):
+                        v.copy_(saved_state[p][k]) if p in saved_state and k in saved_state[p] else v.zero_()
+        torch.cuda.set_rng_state(rng, dev)
+        self.optimizer.zero_grad(set_to_none=True)
+        self.native.bind(dev)
+        self.native.repack(dev)            # the restored weights, and the repack's first launch outside the capture
+        torch.cuda.synchronize(dev)
+        # a Python-number lr is a constant of the captured optimizer kernels (a tensor lr is read at every replay)
+        self._captured_lrs = [None if torch.is_tensor(g['lr']) else g['lr'] for g in self.optimizer.param_groups]
+        self.graph = torch.cuda.CUDAGraph()
+        # thread_local: other threads of the process (e.g. the NCCL watchdog polling its events) must not invalidate the capture
+        with torch.cuda.graph(self.graph, capture_error_mode='thread_local'):
+            self.loss, self.psnr, self.depth_variance = self._run()
+
+    def step(self, rays: torch.Tensor, rgbs: torch.Tensor, image_indices: Optional[torch.Tensor] = None):
+        """One training step on this batch: -> (loss, psnr, depth-variance mean or None), device tensors overwritten by the next
+        step.  Nothing is read back to the host."""
+        if self.graph is None:
+            self.capture(rays, rgbs, image_indices)
+        for g, lr in zip(self.optimizer.param_groups, self._captured_lrs):
+            if lr is not None and g['lr'] != lr:
+                raise ValueError(f'GraphedTrainStep: the learning rate changed from {lr} to {g["lr"]} after the capture, which a '
+                                 'replay cannot follow; give the optimizer a tensor lr (lr=torch.tensor(lr, device=...)), which '
+                                 'an LR scheduler updates in place')
+        self._load(rays, rgbs, image_indices)
+        self.graph.replay()
+        # the replay updated the parameters without bumping their version counters: the next eager call re-packs
+        self.native.invalidate()
+        return self.loss, self.psnr, self.depth_variance

@@ -141,6 +141,7 @@ class _Native:
         self.stamp = None
         self.keep = []
         self.max_multiplicity = None      # None: the library's geometric default (mn_model_create)
+        self._bound_centroids = None      # the centroids `repack` copies (bind)
         self.packed_subs = None           # indices of the sub-modules whose weights are packed; None: all
 
     def invalidate(self):
@@ -209,30 +210,65 @@ class _Native:
                 keep.append(c)
                 K.check(L.mn_model_set_centroids(self.handle, K.ptr(c), st), h)
             for i, sub in self._packed():
-                sd = self._sd(sub)
-                w = K.NerfWeights()
-
-                def g(name):
-                    t = sd.get(name)
-                    if t is None:
-                        return None
-                    t = K.f32c(t.detach().to(device))
-                    keep.append(t)
-                    return t.data_ptr()
-
-                for li in range(first.layers):
-                    w.xyz_w[li] = g(f'xyz_encodings.{li}.0.weight')
-                    w.xyz_b[li] = g(f'xyz_encodings.{li}.0.bias')
-                w.sigma_w, w.sigma_b = g('sigma.weight'), g('sigma.bias')
-                w.final_w, w.final_b = g('xyz_encoding_final.weight'), g('xyz_encoding_final.bias')
-                w.dir_a_w, w.dir_a_b = g('dir_a_encoding.0.weight'), g('dir_a_encoding.0.bias')
-                w.rgb_w, w.rgb_b = g('rgb.weight'), g('rgb.bias')
-                w.embedding_a = g('embedding_a.weight')
-                w.affine_w, w.affine_b = g('affine.weight'), g('affine.bias')
+                w = self._weights(sub, device, keep)
                 K.check(L.mn_model_set_weights(self.handle, i, C.byref(w), st), h)
             self.keep = keep       # packing is stream-ordered; keep sources alive until the next re-pack
             self.stamp = stamp
         return h
+
+    def _weights(self, sub: nn.Module, device: torch.device, keep: list) -> 'K.NerfWeights':
+        """mn_nerf_weights of one sub-module: its tensors as fp32 contiguous on `device` (copies where they are not; every
+        tensor handed over is appended to `keep`)."""
+        sd = self._sd(sub)
+        w = K.NerfWeights()
+
+        def g(name):
+            t = sd.get(name)
+            if t is None:
+                return None
+            t = K.f32c(t.detach().to(device))
+            keep.append((sd[name], t))
+            return t.data_ptr()
+
+        for li in range(self.subs[0].layers):
+            w.xyz_w[li] = g(f'xyz_encodings.{li}.0.weight')
+            w.xyz_b[li] = g(f'xyz_encodings.{li}.0.bias')
+        w.sigma_w, w.sigma_b = g('sigma.weight'), g('sigma.bias')
+        w.final_w, w.final_b = g('xyz_encoding_final.weight'), g('xyz_encoding_final.bias')
+        w.dir_a_w, w.dir_a_b = g('dir_a_encoding.0.weight'), g('dir_a_encoding.0.bias')
+        w.rgb_w, w.rgb_b = g('rgb.weight'), g('rgb.bias')
+        w.embedding_a = g('embedding_a.weight')
+        w.affine_w, w.affine_b = g('affine.weight'), g('affine.bias')
+        return w
+
+    def bind(self, device: torch.device) -> None:
+        """Bind the parameters themselves as the sources of `repack` (mn_model_bind_weights): a repack then reads them where
+        they are, so it sees every in-place update - optimiser steps, `load_state_dict` - with no host work.  Needs every
+        parameter (and the centroids) fp32 and contiguous on `device`; call sync(device) first."""
+        L = K.lib()
+        h = K.ctx(device)
+        for i, sub in enumerate(self.subs):
+            keep = []
+            w = self._weights(sub, device, keep)
+            for orig, t in keep:
+                if t.data_ptr() != orig.data_ptr():
+                    raise ValueError('mega_nerf_b200: binding the weights needs every parameter fp32 and contiguous on '
+                                     f'{device}')
+            K.check(L.mn_model_bind_weights(self.handle, i, C.byref(w)), h)
+        c = self.centroids
+        if c is not None and (c.device != device or c.dtype != torch.float32 or not c.is_contiguous()):
+            raise ValueError(f'mega_nerf_b200: binding the weights needs the centroids fp32 and contiguous on {device}')
+        self._bound_centroids = c
+
+    def repack(self, device: torch.device) -> None:
+        """Re-pack every weight image from the bound parameters on the current stream (mn_model_repack; CUDA-graph
+        capturable), the centroids included."""
+        L = K.lib()
+        h = K.ctx(device)
+        st = K.stream_of(device)
+        if self._bound_centroids is not None:
+            K.check(L.mn_model_set_centroids(self.handle, K.ptr(self._bound_centroids), st), h)
+        K.check(L.mn_model_repack(h, self.handle, st), h)
 
     def forward(self, rows: K.Rows, B: int, device: torch.device, use_coarse: bool, sigma_only: bool,
                 sigma_noise: Optional[torch.Tensor], out_cols: int, keep_alive=()) -> torch.Tensor:
@@ -315,6 +351,10 @@ class _Native:
         fn = L.mn_model_backward_tc if tc else L.mn_model_backward
         K.check(fn(h, self.handle, B, int(use_coarse), K.ptr(g), K.ptr(tape), tape.numel(), K.ptr(gbuf),
                    K.ptr(ws), ws.numel(), K.stream_of(device)), h)
+        return self.grad_views(gbuf, params)
+
+    def grad_views(self, gbuf: torch.Tensor, params):
+        """The gradient of each parameter of `params` (a param_list()) as a view of the [n_sub, stride] gradient block gbuf."""
         off = self._offsets()
         stride = off['stride']
         grads = []

@@ -131,6 +131,15 @@ class _Stage:
         return out
 
 
+def _density_noise(hparams: Namespace, B: int, device: torch.device) -> torch.Tensor:
+    """The density noise of a training query over B samples [B, 1]: the same draw order / shapes as the reference's per-chunk
+    torch.rand (rendering.py:294,321)."""
+    ch = hparams.model_chunk_size
+    if B == 0:
+        return torch.empty(0, 1, device=device)
+    return torch.cat([torch.rand(min(ch, B - a), 1, device=device) for a in range(0, B, ch)], 0)
+
+
 def _query(sg: _Stage, net: nn.Module, hparams: Namespace, typ: str, xyz: torch.Tensor, dirs: torch.Tensor,
            idx: Optional[torch.Tensor], call: Optional[nn.Module] = None, rays_cap: Optional[int] = None) -> torch.Tensor:
     """Model query for [n,S,C] points -> raw [n,S,4] = (rgb, sigma).  rendering.py:275-334.
@@ -141,12 +150,7 @@ def _query(sg: _Stage, net: nn.Module, hparams: Namespace, typ: str, xyz: torch.
     native = net._native()
     first = native.subs[0]
     use_dirs = hparams.pos_dir_dim != 0
-    noise = None
-    if net.training:
-        # same draw order / shapes as the reference's per-chunk torch.rand (rendering.py:294,321)
-        ch = hparams.model_chunk_size
-        noise = torch.cat([torch.rand(min(ch, B - a), 1, device=xyz.device) for a in range(0, B, ch)], 0) if B > 0 \
-            else xyz.new_empty(0, 1)
+    noise = _density_noise(hparams, B, xyz.device) if net.training else None
     rr = RayRows(xyz, S, dirs if use_dirs else None, idx)
     target = call if call is not None else net
     ep = getattr(net, '_ep', None)
@@ -514,4 +518,68 @@ def render_rays_fused(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
     if check_status:
         # the reference raises from a host-side `.any()` over the sphere check (rendering.py:412-414)
         K.check(L.mn_check_status(h, st), h)
+    return res
+
+
+def _check_train(net: nn.Module, hparams: Namespace, fn: str) -> None:
+    if not net.training:
+        raise ValueError(f'{fn} is the training path; call nerf.train() first')
+    if getattr(net, '_ep', None) is not None:
+        raise ValueError(f'{fn} cannot train a network under expert parallelism: use render_rays')
+    if bool(hparams.use_cascade) != isinstance(net, Cascade):
+        raise ValueError('hparams.use_cascade does not match the network')
+    if hparams.fine_samples <= 0:
+        raise ValueError(f'{fn} needs fine_samples > 0')
+
+
+def render_rays_train(nerf: nn.Module, rays: torch.Tensor, image_indices: Optional[torch.Tensor], hparams: Namespace,
+                      get_depth: bool, get_depth_variance: bool) -> Dict[str, torch.Tensor]:
+    """The training path of `render_rays(nerf, None, ...)` (runner.py:347-358, a foreground network in train mode) as ONE library
+    call (`mn_render_rays_train`) whose backward is one library call too (`mn_render_rays_train_backward`): the same kernels in
+    the same order, sequenced in C, at the arithmetic of `set_train_precision`.  It draws its random numbers with the calls
+    render_rays makes, in its order - the jitter, the coarse density noise, the resampling draws, the fine density noise - so
+    for the same generator state it returns the same keys and values as `render_rays(...)[0]`.  The returned colours carry one
+    autograd node; its backward accumulates every parameter's gradient as a view of one gradient block, as the stage path does.
+    Not for a background network, an expert-parallel network, a DistributedDataParallel wrapper or fine_samples == 0 (use
+    render_rays)."""
+    if _unwrap(nerf) is not nerf:
+        # the library's one call never runs the wrapper's forward, so DistributedDataParallel's reducer would not arm and every
+        # rank would keep its own gradients
+        raise ValueError('render_rays_train needs a mega_nerf_b200 network itself, not a wrapper such as DistributedDataParallel: '
+                         'use render_rays, which queries through the wrapper')
+    net, _ = _nets(nerf, None, 'render_rays_train')
+    _check_train(net, hparams, 'render_rays_train')
+    native = net._native()
+    native.sync(rays.device)
+    return _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance)
+
+
+def _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance) -> Dict[str, torch.Tensor]:
+    """render_rays_train on weights already packed (sync, or a repack inside a captured training step)."""
+    dev = rays.device
+    rays = K.f32c(rays.detach())
+    N = rays.shape[0]
+    idx = K.f32c(image_indices.to(dev)).view(-1) if image_indices is not None else None
+    Sc, Sf = hparams.coarse_samples, hparams.fine_samples
+    cascade = bool(hparams.use_cascade)
+    Sq = Sc + Sf if cascade else Sf
+    perturb = hparams.perturb
+    # the draws of render_rays in train mode, in its order (_render, then _two_pass)
+    steps = torch.linspace(0, 1, Sc, device=dev)
+    jitter = torch.rand(N, Sc, device=dev) if perturb > 0 else None
+    noise_c = _density_noise(hparams, N * Sc, dev)
+    u = torch.rand(N, Sf, device=dev) if perturb > 0 else torch.linspace(0, 1, Sf, device=dev).expand(N, Sf).contiguous()
+    noise_f = _density_noise(hparams, N * Sq, dev)
+    sh_deg = hparams.sh_deg if (hparams.pos_dir_dim == 0 and hparams.sh_deg is not None) else -1
+    call = AG.RenderTrainCall(native, rays, idx, steps, jitter, float(perturb), noise_c, u, noise_f, Sc, Sf, cascade, sh_deg,
+                              get_depth, get_depth_variance)
+    rgb, rgb_coarse, depth, var = AG.render_train_apply(call)
+    res: Dict[str, torch.Tensor] = {}
+    if cascade:
+        res['rgb_coarse'] = rgb_coarse
+    res['rgb_fine'] = rgb
+    if get_depth:
+        res['depth_fine'] = depth
+    if get_depth_variance:
+        res['depth_variance_fine'] = var
     return res
