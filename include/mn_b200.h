@@ -657,6 +657,16 @@ int mn_debug_fp32_train_layout(const mn_model* m, int64_t B, int64_t* out, int c
 int mn_debug_tc_forward_record(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, int use_coarse, const float* sigma_noise_d,
                                float* out_d, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes, void* stream);
 
+/* ---- test hook: the packed weight images of a model ------------------------------------------------------------------
+ * which: 0 the fp32 forward layout of every sub-module (n_sub x PackedLayout floats), 1 the fp32 data-gradient layout
+ * (n_sub x BwdLayout floats), 2 the fp16 hi / lo tensor-core forward images (n_sub x the plan's per-sub-module bytes), 3 the
+ * transposed tensor-core data-gradient images (allocated by the first recording call on the tensor cores).  Returns the
+ * image's byte size, 0 if it is not allocated (or `which` is out of range); with dst, copies min(size, cap) bytes device to
+ * device on `stream` (0 and mn_last_error set if the copy fails).  Every image is zeroed when it is allocated and packs write
+ * the same bytes from the same values, padding included, so two packs of equal weights are byte-identical.  Used by
+ * tests/test_gpu_zzg_train_graph_shapes.py. */
+size_t mn_debug_weight_images(const mn_model* m, int which, void* dst, size_t cap, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

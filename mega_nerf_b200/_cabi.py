@@ -143,6 +143,7 @@ SIGNATURES = {
     'mn_debug_tc_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),
     'mn_debug_tc_forward_record': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _P, _P, _P, _Z, _P, _Z, _P]),
     'mn_debug_fp32_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),
+    'mn_debug_weight_images': (_Z, [_P, _I, _P, _Z, _P]),
 }
 MN_PARAM_OFFSETS = 44
 # entries of mn_debug_tc_train_layout (MN_TCL_* in include/mn_b200.h), then 2 per record image from TCL['IMG'] on

@@ -511,6 +511,21 @@ int mn_model_repack(mn_ctx* ctx, mn_model* m, void* stream) {
     return MN_OK;
 }
 
+size_t mn_debug_weight_images(const mn_model* m, int which, void* dst, size_t cap, void* stream) {
+    if (!m || which < 0 || which > 3) return 0;
+    const size_t n_sub = (size_t)m->d.n_sub;
+    const void* src[4] = {m->packed, m->packed_bwd, m->tc_packed, m->tc_dgrad};
+    const size_t bytes[4] = {n_sub * m->lay.total * sizeof(float), n_sub * m->blay.total * sizeof(float),
+                             n_sub * (size_t)m->tc.P.sub_bytes, n_sub * (size_t)m->tc.D.sub_bytes};
+    if (!src[which]) return 0;
+    if (dst && cudaMemcpyAsync(dst, src[which], bytes[which] < cap ? bytes[which] : cap, cudaMemcpyDeviceToDevice,
+                               (cudaStream_t)stream) != cudaSuccess) {
+        mn_fail(m->ctx, MN_ERR_CUDA, "mn_debug_weight_images: copy failed");
+        return 0;
+    }
+    return bytes[which];
+}
+
 // mult: sub-modules per row the slots are sized for; 0 = the model's max_multiplicity
 static int64_t slot_capacity(const mn_model* m, int64_t B, int mult = 0) {
     if (m->d.kind != 2) return mn_cdiv(B, MN_BUCKET) * MN_BUCKET;
