@@ -535,6 +535,45 @@ int mn_render_rays_train_backward(mn_ctx* ctx, mn_model* m, int64_t N, int coars
                                   const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d,
                                   size_t workspace_bytes, void* stream);
 
+/* mn_render_rays_train_bg: the recording render of render_rays(nerf, bg_nerf, ...) in train mode (rendering.py:34-75,
+ * render.py `_render`) as ONE call: the device sphere split and stable compaction of mn_render_rays_bg, the background network's
+ * two-pass recording render over the compacted rays (their count stays on the device: every stage, the router, the encoders and
+ * the MLP tiles stop at it), the foreground's recording render with the far override, last delta and bg_lambda, then the lambda
+ * blend rgb = fg + bg_lambda * bg of the final type and, under use_cascade, of the coarse one.  No allocation, no host sync, a
+ * static launch sequence (CUDA-graph capturable); with no background ray the background kernels launch and do nothing.
+ *   fg / bg, image_indices_d, sphere_center3_d / sphere_radius3_d, include_xyz_real, cluster_2d, z_steps_d / z_steps_bg_d: as for
+ *   mn_render_rays_bg; precision / bg_precision: each network's training precision (MN_PREC_FP32 or MN_PREC_TC_F16);
+ *   foreground draws as for mn_render_rays_train; background draws jitter_bg_d [rows, coarse_samples/2] (NULL iff perturb == 0),
+ *   sigma_noise_coarse_bg_d [rows * coarse_samples/2], u_fine_bg_d [rows, fine_samples/2], sigma_noise_fine_bg_d
+ *   [rows * Sq_bg] (Sq_bg = fine_samples/2, or coarse_samples/2 + fine_samples/2 under use_cascade).  bg_draws_by_ray = 0: row p
+ *   of each block belongs to the p-th background ray in ascending ray order (rows = the background count, render_rays' stream);
+ *   1: row i belongs to ray i (rows = N), rows of rays that stay in the foreground are not read.
+ *   out: as for mn_render_rays_bg; rgb, bg_lambda required, and rgb_coarse and bg_lambda_coarse under use_cascade.
+ * A camera outside the ellipsoid sets the status word (MN_ERR_SPHERE at the next mn_check_status).  tape_d
+ * (mn_render_rays_train_bg_tape_bytes) must stay untouched until mn_render_rays_train_bg_backward has consumed it.
+ * mn_render_rays_train_bg_backward (same sizes, flags, precisions and tape): grad_rgb_d [N,3] = dL/d rgb_fine, grad_rgb_coarse_d
+ * as for mn_render_rays_train_backward; runs the blend backward, the foreground composite backward (its bg_lambda included) and
+ * model backwards, then the background composite and model backwards over the device count, and ACCUMULATES into
+ * param_grads_d (foreground) and bg_param_grads_d (background) as mn_model_backward does.  No host sync. */
+size_t mn_render_rays_train_bg_tape_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                          int use_cascade, int sh_deg, int precision, int bg_precision);
+size_t mn_render_rays_train_bg_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                               int use_cascade, int sh_deg, int precision, int bg_precision);
+int mn_render_rays_train_bg(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays_d, const float* image_indices_d, int64_t N,
+                            const float* sphere_center3_d, const float* sphere_radius3_d, int include_xyz_real, int cluster_2d,
+                            const float* z_steps_d, const float* z_steps_bg_d, const float* jitter_d, const float* jitter_bg_d,
+                            float perturb, int coarse_samples, const float* sigma_noise_coarse_d, const float* sigma_noise_coarse_bg_d,
+                            const float* u_fine_d, const float* u_fine_bg_d, const float* sigma_noise_fine_d,
+                            const float* sigma_noise_fine_bg_d, int fine_samples, int use_cascade, int sh_deg, int precision,
+                            int bg_precision, int bg_draws_by_ray, const mn_render_outputs* out, void* tape_d, size_t tape_bytes,
+                            void* workspace_d, size_t workspace_bytes, void* stream);
+size_t mn_render_rays_train_bg_backward_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples,
+                                                        int fine_samples, int use_cascade, int sh_deg, int precision, int bg_precision);
+int mn_render_rays_train_bg_backward(mn_ctx* ctx, mn_model* fg, mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                     int use_cascade, int sh_deg, int precision, int bg_precision, const float* grad_rgb_d,
+                                     const float* grad_rgb_coarse_d, const void* tape_d, size_t tape_bytes, float* param_grads_d,
+                                     float* bg_param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream);
+
 /* ---- test hook (host only, no CUDA call) ---------------------------------------------------------------------------
  * The stage program of the tensor-core MLP kernel (csrc/mn_mlp_wg.cuh, precision tc_f16) for one network shape: `desc` as for
  * mn_model_create (only the per-sub-module fields matter).  The producer and both consumer warpgroups walk this program, one

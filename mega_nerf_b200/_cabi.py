@@ -140,6 +140,12 @@ SIGNATURES = {
                                   _P]),
     'mn_render_rays_train_backward_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
     'mn_render_rays_train_backward': (_I, [_P, _P, _L, _I, _I, _I, _I, _I, _P, _P, _P, _Z, _P, _P, _Z, _P]),
+    'mn_render_rays_train_bg_tape_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_bg_workspace_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_bg': (_I, [_P, _P, _P, _P, _P, _L, _P, _P, _I, _I, _P, _P, _P, _P, _F, _I, _P, _P, _P, _P, _P, _P, _I, _I,
+                                     _I, _I, _I, _I, C.POINTER(RenderOutputs), _P, _Z, _P, _Z, _P]),
+    'mn_render_rays_train_bg_backward_workspace_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_bg_backward': (_I, [_P, _P, _P, _L, _I, _I, _I, _I, _I, _I, _P, _P, _P, _Z, _P, _P, _P, _Z, _P]),
     'mn_debug_tc_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),
     'mn_debug_tc_forward_record': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _P, _P, _P, _Z, _P, _Z, _P]),
     'mn_debug_fp32_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),

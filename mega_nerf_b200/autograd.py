@@ -9,6 +9,7 @@ arithmetic of `set_train_precision` ('fp32' CUDA-core kernels by default, or 'tc
 """
 from __future__ import annotations
 
+import ctypes as C
 from typing import Optional
 
 import torch
@@ -191,3 +192,110 @@ class _RenderTrainFn(torch.autograd.Function):
 def render_train_apply(call: RenderTrainCall):
     params = [p for _, _, p in call.native.param_list()]
     return _RenderTrainFn.apply(call, *params)
+
+
+class RenderTrainBgCall:
+    """One mn_render_rays_train_bg call: its inputs (the random draws of both networks included), its outputs, then its tape until
+    the backward consumed it.  bg_grads: whether the background parameters receive a gradient (eager, no background ray and no
+    dummy ray: None, as on the stage path)."""
+
+    def __init__(self, native, bnative, rays, idx, center, radius, real, c2d, steps, steps_bg, jitter, jitter_bg, perturb, noise_c,
+                 noise_c_bg, u, u_bg, noise_f, noise_f_bg, Sc, Sf, cascade, sh_deg, by_ray, get_depth, get_depth_variance,
+                 get_bg_fg_rgb, bg_grads=True):
+        self.native, self.bnative, self.rays, self.idx, self.center, self.radius = native, bnative, rays, idx, center, radius
+        self.real, self.c2d, self.steps, self.steps_bg, self.perturb = real, c2d, steps, steps_bg, perturb
+        self.draws = (jitter, jitter_bg, noise_c, noise_c_bg, u, u_bg, noise_f, noise_f_bg)
+        self.Sc, self.Sf, self.cascade, self.sh_deg, self.by_ray = Sc, Sf, cascade, sh_deg, by_ray
+        self.get_depth, self.get_depth_variance, self.get_bg_fg_rgb = get_depth, get_depth_variance, get_bg_fg_rgb
+        self.bg_grads = bg_grads
+        self.prec = K.PREC_TC_F16 if native.train_on_tensor_cores() else K.PREC_FP32
+        self.bprec = K.PREC_TC_F16 if bnative.train_on_tensor_cores() else K.PREC_FP32
+        self.tape = None
+
+    def _sizes(self):
+        return (self.native.handle, self.bnative.handle, self.rays.shape[0], self.Sc, self.Sf, int(self.cascade), self.sh_deg,
+                self.prec, self.bprec)
+
+    def forward(self):
+        """-> {result key: tensor} in mn_render_outputs' fields (rgb, rgb_coarse, depth, ...)."""
+        L, dev = K.lib(), self.rays.device
+        h = K.ctx(dev)
+        N = self.rays.shape[0]
+        new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
+        o = {'rgb': new(N, 3), 'bg_lambda': new(N)}
+        if self.get_depth:
+            o['depth'] = new(N)
+        if self.get_depth_variance:
+            o['depth_var'] = new(N)
+        if self.cascade:
+            o['rgb_coarse'], o['bg_lambda_coarse'] = new(N, 3), new(N)
+        if self.get_bg_fg_rgb:
+            for k in [k for k in ('rgb', 'depth', 'rgb_coarse') if k in o]:
+                pre = k[:-len('_coarse')] if k.endswith('_coarse') else k
+                post = '_coarse' if k.endswith('_coarse') else ''
+                o[f'fg_{pre}{post}'], o[f'bg_{pre}{post}'] = new(*o[k].shape), new(*o[k].shape)
+        out = K.RenderOutputs()
+        for k, v in o.items():
+            setattr(out, k, K.ptr(v))
+        self.tape = torch.empty(max(int(L.mn_render_rays_train_bg_tape_bytes(*self._sizes())), 256), device=dev, dtype=torch.uint8)
+        ws = torch.empty(max(int(L.mn_render_rays_train_bg_workspace_bytes(*self._sizes())), 256), device=dev, dtype=torch.uint8)
+        jitter, jitter_bg, noise_c, noise_c_bg, u, u_bg, noise_f, noise_f_bg = self.draws
+        K.check(L.mn_render_rays_train_bg(h, self.native.handle, self.bnative.handle, K.ptr(self.rays), K.ptr(self.idx), N,
+                                          K.ptr(self.center), K.ptr(self.radius), int(self.real), int(self.c2d), K.ptr(self.steps),
+                                          K.ptr(self.steps_bg), K.ptr(jitter), K.ptr(jitter_bg), self.perturb, self.Sc,
+                                          K.ptr(noise_c), K.ptr(noise_c_bg), K.ptr(u), K.ptr(u_bg), K.ptr(noise_f),
+                                          K.ptr(noise_f_bg), self.Sf, int(self.cascade), self.sh_deg, self.prec, self.bprec,
+                                          int(self.by_ray), C.byref(out), K.ptr(self.tape), self.tape.numel(), K.ptr(ws), ws.numel(),
+                                          K.stream_of(dev)), h)
+        return o
+
+    def backward(self, g_rgb, g_rgb_coarse, params, bparams):
+        L, dev = K.lib(), self.rays.device
+        h = K.ctx(dev)
+        N = self.rays.shape[0]
+        gbuf = torch.zeros(int(L.mn_model_grad_floats(self.native.handle)), device=dev, dtype=torch.float32)
+        gbuf_bg = torch.zeros(int(L.mn_model_grad_floats(self.bnative.handle)), device=dev, dtype=torch.float32)
+        ws = torch.empty(max(int(L.mn_render_rays_train_bg_backward_workspace_bytes(*self._sizes())), 256), device=dev,
+                         dtype=torch.uint8)
+        g_rgb = K.f32c(g_rgb) if g_rgb is not None else torch.zeros(N, 3, device=dev, dtype=torch.float32)
+        g_rgb_coarse = K.f32c(g_rgb_coarse) if g_rgb_coarse is not None else None
+        K.check(L.mn_render_rays_train_bg_backward(h, self.native.handle, self.bnative.handle, N, self.Sc, self.Sf, int(self.cascade),
+                                                   self.sh_deg, self.prec, self.bprec, K.ptr(g_rgb), K.ptr(g_rgb_coarse),
+                                                   K.ptr(self.tape), self.tape.numel(), K.ptr(gbuf), K.ptr(gbuf_bg), K.ptr(ws),
+                                                   ws.numel(), K.stream_of(dev)), h)
+        self.tape = None
+        bg = self.bnative.grad_views(gbuf_bg, bparams) if self.bg_grads else [None] * len(bparams)
+        return self.native.grad_views(gbuf, params), bg
+
+
+class _RenderTrainBgFn(torch.autograd.Function):
+    """render_rays_train with a background network (render.py): the whole recording render as one node.  Outputs rgb_fine and
+    rgb_coarse (Cascade), which carry the gradient into both networks' parameters, then the other results without one."""
+
+    @staticmethod
+    def forward(ctx, call, n_fg, *params):
+        ctx.set_materialize_grads(False)
+        o = call.forward()
+        ctx.call, ctx.n_fg = call, n_fg
+        ctx.plist = call.native.param_list()
+        ctx.blist = call.bnative.param_list()
+        assert len(ctx.plist) == n_fg and len(ctx.blist) == len(params) - n_fg
+        call.keys = [k for k in o if k not in ('rgb', 'rgb_coarse')]
+        rest = [o[k] for k in call.keys]
+        ctx.mark_non_differentiable(*rest)
+        return (o['rgb'], o.get('rgb_coarse')) + tuple(rest)
+
+    @staticmethod
+    def backward(ctx, g_rgb, g_rgb_coarse, *_):
+        grads, bgrads = ctx.call.backward(g_rgb, g_rgb_coarse, ctx.plist, ctx.blist)
+        ctx.call = None
+        need = ctx.needs_input_grad[2:]
+        return (None, None) + tuple(g if n else None for g, n in zip(grads + bgrads, need))
+
+
+def render_train_bg_apply(call: RenderTrainBgCall):
+    """-> {mn_render_outputs field: tensor}; rgb and rgb_coarse carry the graph."""
+    params = [p for _, _, p in call.native.param_list()]
+    bparams = [p for _, _, p in call.bnative.param_list()]
+    outs = _RenderTrainBgFn.apply(call, len(params), *params, *bparams)
+    return dict(zip(['rgb', 'rgb_coarse'] + call.keys, outs))

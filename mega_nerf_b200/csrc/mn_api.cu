@@ -1156,6 +1156,40 @@ int mn_model_backward_assigned(mn_ctx* ctx, mn_model* m, int64_t n, int64_t max_
                           tape_bytes, workspace_d, workspace_bytes, who, (cudaStream_t)stream);
 }
 
+}  // extern "C"
+
+int mn_model_forward_train_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse,
+                                const float* sigma_noise_d, int precision, float* out_d, void* tape_d, size_t tape_bytes,
+                                void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+    if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_train: tape is NULL");
+    if (precision == MN_PREC_TC_F16 && !mn_model_train_tc_supported(m)) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
+    ModelCall c;
+    c.B = B;
+    c.use_coarse = use_coarse;
+    c.live = live;
+    c.sigma_noise = sigma_noise_d;
+    c.run = RUN_TRAIN;
+    c.precision = precision;
+    c.out = out_d;
+    return forward_rows(ctx, m, rows, c, workspace_d, workspace_bytes, tape_d, tape_bytes, st);
+}
+
+int mn_model_backward_live(mn_ctx* ctx, mn_model* m, int64_t B, LiveRows live, int use_coarse, int precision, const float* grad_out_d,
+                           const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes,
+                           cudaStream_t st) {
+    if (!ctx || !m || B < 0 || !grad_out_d || !tape_d || !param_grads_d) return MN_ERR_INVALID;
+    if (B == 0) return MN_OK;
+    const bool tc = precision == MN_PREC_TC_F16;
+    if (tc && !mn_model_train_tc_supported(m)) return mn_fail(ctx, MN_ERR_UNSUPPORTED, "mn_model_backward_tc: unsupported network shape");
+    const int64_t cap = slot_capacity(m, B);
+    BwdArgs a = bwd_args(m, B, cap, use_coarse, grad_out_d, param_grads_d);
+    a.live = live;
+    return model_backward(ctx, m, a, cap, false, tc, tape_d, tape_bytes, workspace_d, workspace_bytes,
+                          tc ? "mn_model_backward_tc" : "mn_model_backward", st);
+}
+
+extern "C" {
+
 int mn_model_last_stats(mn_ctx* ctx, mn_model* m, int64_t* slots, int64_t* tiles, void* stream) {
     if (!ctx || !m) return MN_ERR_INVALID;
     int h[2] = {0, 0};

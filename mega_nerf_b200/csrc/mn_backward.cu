@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(256, 1) mlp_bwd_data_kernel(const BwdArgs a) {
     const int tid = threadIdx.x;
 
     const int64_t slot0 = (int64_t)blockIdx.x * TM;
-    const int64_t n_slots = a.counters ? a.counters[CNT_NSLOTS] : a.B;
+    const int64_t n_slots = a.counters ? a.counters[CNT_NSLOTS] : a.live.rows(a.B);
     if (slot0 >= n_slots) return;
     int sub = a.fixed_sub;
     if (a.counters) {
@@ -268,6 +268,7 @@ struct WgradArgs {
     const int* counters;                // saved routing counters or NULL
     int fixed_sub;
     int64_t B;                          // rows when counters == NULL
+    LiveRows live;                      // of the B rows when counters == NULL: the tiles past live.rows(B) hold no tape
     int chunk_tiles;
 };
 
@@ -285,7 +286,7 @@ __global__ void __launch_bounds__(256) mlp_bwd_weight_kernel(const WgradArgs a) 
     const int n0 = (local / kblocks) * 64, k0 = (local % kblocks) * 64;
 
     int sub = a.fixed_sub;
-    int64_t t_lo = 0, t_hi = (a.B + TM - 1) / TM;
+    int64_t t_lo = 0, t_hi = (a.live.rows(a.B) + TM - 1) / TM;
     if (a.counters) {
         sub = (int)blockIdx.z;
         t_lo = a.counters[CNT_START + sub] / TM;
@@ -413,6 +414,7 @@ int mn_mlp_bwd_launch(mn_ctx* ctx, const BwdArgs& a, int64_t n_tiles128, cudaStr
     w.counters = a.counters;
     w.fixed_sub = a.fixed_sub;
     w.B = a.B;
+    w.live = a.live;
     w.chunk_tiles = MN_WG_CHUNK_TILES;
     const unsigned gx = (unsigned)mn_cdiv(n_tiles, w.chunk_tiles);
     const dim3 grid(gx, (unsigned)blocks, (unsigned)(a.counters ? a.n_sub : 1));

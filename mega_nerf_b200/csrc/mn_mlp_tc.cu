@@ -989,7 +989,7 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     {
         const int64_t n = a.grad_rows * a.out_cols;
         const int64_t blocks = std::min<int64_t>(std::max<int64_t>(mn_cdiv(n, (int64_t)256 * 16), 1), (int64_t)ctx->sm_count * 4);
-        tc_grad_absmax_kernel<<<(unsigned)blocks, 256, 0, st>>>(a.grad_out, n, maxbits);
+        tc_grad_absmax_kernel<<<(unsigned)blocks, 256, 0, st>>>(a.grad_out, a.live, a.grad_rows, a.out_cols, maxbits);
         MN_LAUNCH_CHECK(ctx);
         tc_grad_scale_kernel<<<1, 32, 0, st>>>(maxbits, scale);
         MN_LAUNCH_CHECK(ctx);
@@ -1003,8 +1003,10 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
     mm.fixed_sub = a.fixed_sub;
     mm.B = a.B;
     mm.out_cols = a.out_cols;
+    mm.live = a.live;
     const int n_sub = a.counters ? a.n_sub : 1;
-    // tiles the forward pass really wrote: all bucketed tiles when routed, ceil(rows / 128) otherwise
+    // tiles the forward pass may have written: all bucketed tiles when routed, ceil(rows / 128) otherwise (the kernels stop at
+    // the live rows' tiles)
     const int64_t tiles_used = a.counters ? n_tiles128 : mn_cdiv(a.B, (int64_t)kTileM);
     const int wg_smem = 2 * kWgStageBytes + 6144 + 256;
     MN_CUDA(ctx, cudaFuncSetAttribute(tc_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, wg_smem));
@@ -1022,6 +1024,8 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         H.n_tiles = tiles_used;
         H.t_min = t0;
         H.t_max = t0 + nt;
+        H.live = a.live;
+        H.rows = a.B;
         H.fixed_sub = a.fixed_sub;
         H.chunk_tiles = 16;
         H.gw = a.gw;
@@ -1056,6 +1060,8 @@ int mn_train_tc_backward(mn_ctx* ctx, mn_model* m, const BwdArgs& a, int64_t n_t
         W.t_max = t0 + nt;
         W.counters = a.counters;
         W.fixed_sub = a.fixed_sub;
+        W.live = a.live;
+        W.rows = a.B;
         W.gw = a.gw;
         W.sub_stride = a.lay.total;
         W.scale = scale;

@@ -234,6 +234,9 @@ struct BwdArgs {
     const float* act;          // activation tape
     float* grad;               // gradient tape
     float* gw;                 // parameter gradients, [n_sub * lay.total], matrices stored [out][in] (nn.Linear layout)
+    // rows of grad_out that hold data, as the recording forward's (the background pass of mn_render_rays_train_bg): unrouted
+    // calls run no slot at or past live.rows(B), whose tape was never written; routed calls take their slots from the counters
+    LiveRows live;
 };
 
 int mn_route_build(mn_ctx* ctx, mn_model* m, const RowSrc& src, int64_t B, LiveRows live, int64_t cap, int* slot_row, float* slot_w,
@@ -252,6 +255,15 @@ int mn_route_build_assigned(mn_ctx* ctx, mn_model* m, const float* rows, int64_t
 // its result goes to out_d row r (the queried samples of an occupancy grid, mn_render.cu)
 int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse, int precision,
                           float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st, const int* gather = nullptr);
+// The recording forward (mn_model_forward_train(_tc), precision MN_PREC_FP32 / MN_PREC_TC_F16) and its backward (mn_model_backward(_tc))
+// over the first live.rows(B) of B rows, with the tape and workspaces of B rows: no slot at or past the live rows is encoded,
+// recorded or contracted into a weight gradient, and rows of grad_out past them are never read.
+int mn_model_forward_train_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse,
+                                const float* sigma_noise_d, int precision, float* out_d, void* tape_d, size_t tape_bytes,
+                                void* workspace_d, size_t workspace_bytes, cudaStream_t st);
+int mn_model_backward_live(mn_ctx* ctx, mn_model* m, int64_t B, LiveRows live, int use_coarse, int precision, const float* grad_out_d,
+                           const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes,
+                           cudaStream_t st);
 // ---- the one launch of each stage kernel (csrc/mn_sample.cu).  The public stage entry points validate their arguments and call
 // these; the render passes of mn_render_rays(_bg) call them directly, the background pass with its device ray count (`live`: rays
 // at or past it are skipped, grids stay sized for N) and the sample orders it needs: flip = reversed stratify output, flip_pts =
@@ -273,6 +285,12 @@ int mn_stage_composite(mn_ctx* ctx, const float* raw_d, const float* z_d, const 
 int mn_stage_sh_to_rgb(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
                        int dir_div, int64_t B, int apply_sigmoid, LiveRows live, float* out_d, cudaStream_t st,
                        const int* gather = nullptr);   // gather: row b's direction is that of sample gather[b] (occupancy grids)
+int mn_stage_composite_backward(mn_ctx* ctx, const float* raw_d, const float* z_d, int S, const float* raw2_d, const float* z2_d, int S2,
+                                const float* last_delta_d, int64_t N, int flip, LiveRows live, const float* grad_rgb_d,
+                                const float* grad_lambda_d, float* grad_raw_d, float* grad_raw2_d, cudaStream_t st);
+int mn_stage_sh_to_rgb_backward(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
+                                int dir_div, int64_t B, int apply_sigmoid, LiveRows live, const float* grad_out_d, float* grad_coef_d,
+                                cudaStream_t st);
 int mn_mlp_simt_launch(mn_ctx* ctx, const MlpArgs& a, int64_t n_tiles128, cudaStream_t st);
 int mn_mlp_bwd_launch(mn_ctx* ctx, const BwdArgs& a, int64_t n_tiles128, cudaStream_t st);
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws,

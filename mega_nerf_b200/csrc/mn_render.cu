@@ -558,28 +558,20 @@ int check_train(mn_ctx* ctx, const mn_model* m, int64_t N, int coarse_samples, i
     return MN_OK;
 }
 
-int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N, const float* z_steps_d,
-               const float* jitter_d, float perturb, int S, const float* noise_c_d, const float* u_d, const float* noise_f_d, int F,
-               int use_cascade, int sh_deg, int precision, float* rgb, float* depth, float* var, float* rgb_coarse, void* tape_d,
-               size_t tape_bytes, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
-    const char* name = "mn_render_rays_train";
-    const std::string nm(name);
-    if (!ctx || !m || !rays_d || !z_steps_d || !u_d || !rgb) return MN_ERR_INVALID;
-    int rc;
-    if ((rc = check_train(ctx, m, N, S, F, precision, name))) return rc;
-    if ((rc = check_net(ctx, m, use_cascade, F, sh_deg, image_indices_d, name))) return rc;
-    if (perturb > 0 && !jitter_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": perturb > 0 needs jitter_d");
-    if (use_cascade && !rgb_coarse) return mn_fail(ctx, MN_ERR_INVALID, nm + ": rgb_coarse_out_d is required under use_cascade");
-    if (N == 0) return MN_OK;
-    const bool sh = sh_deg >= 0, tc = precision == MN_PREC_TC_F16;
-    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh, tc);
-    if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
-    if (!workspace_d || workspace_bytes < p.ws_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
-    char* T = (char*)tape_d;
-    char* W = (char*)workspace_d;
+// The foreground's recording two-pass render into the tape T and workspace W laid out by p: coarse sampling (up to far_ov, the
+// background split's far override, when given), the recording coarse query, the detached-weights composite, resampling, sort_cat
+// under cascade, the recording fine query and the final composite.  The caller has written the last deltas into the tape.  lam /
+// lam_c: bg_lambda of the final and (cascade) the coarse type, null without a background network.
+int train_fg_pass(mn_ctx* ctx, mn_model* m, const TrainPlan& p, char* T, char* W, const float* rays_d, const float* image_indices_d,
+                  int64_t N, const float* far_ov, const float* z_steps_d, const float* jitter_d, float perturb, const float* noise_c_d,
+                  const float* u_d, const float* noise_f_d, int use_cascade, int sh_deg, float* rgb, float* depth, float* var,
+                  float* rgb_coarse, float* lam, float* lam_c, cudaStream_t st) {
+    const int S = p.S, F = p.F;
+    const bool sh = p.sh, tc = p.tc;
     auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(T + off); };
     auto WF = [&](size_t off) { return reinterpret_cast<float*>(W + off); };
     const LiveRows all{};
+    int rc;
 
     // one recording model query on [N, Sq, 3] points -> raw [N, Sq, 4], into the model tape at `tape` (render.py `_query`)
     auto query = [&](const float* xyz, int Sq, int coarse, const float* noise, float* mlp_out, float* raw_out, size_t tape,
@@ -600,15 +592,13 @@ int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image
         return MN_OK;
     };
 
-    fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(TF(p.last_delta), N, 1e10f);     // no background: rendering.py:33
-    MN_LAUNCH_CHECK(ctx);
     if (sh) MN_CUDA(ctx, cudaMemcpyAsync(T + p.rays, rays_d, (size_t)N * 32, cudaMemcpyDeviceToDevice, st));
-    if ((rc = mn_sample_coarse(ctx, rays_d, nullptr, z_steps_d, jitter_d, perturb, N, S, TF(p.z_c), WF(p.xyz_c), st))) return rc;
+    if ((rc = mn_sample_coarse(ctx, rays_d, far_ov, z_steps_d, jitter_d, perturb, N, S, TF(p.z_c), WF(p.xyz_c), st))) return rc;
     if ((rc = query(WF(p.xyz_c), S, 1, noise_c_d, TF(p.mlp_c), TF(p.raw_c), p.tape_c, p.tape_c_bytes))) return rc;
     // the cascade's coarse colour, then the resampling weights of the detached coarse composite (render.py `_two_pass`)
     if (use_cascade)
         if ((rc = mn_stage_composite(ctx, TF(p.raw_c), TF(p.z_c), nullptr, S, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
-                                     nullptr, rgb_coarse, nullptr, nullptr, nullptr, st)))
+                                     nullptr, rgb_coarse, nullptr, nullptr, lam_c, st)))
             return rc;
     if ((rc = mn_stage_composite(ctx, TF(p.raw_c), TF(p.z_c), nullptr, S, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
                                  WF(p.w_c), nullptr, nullptr, nullptr, nullptr, st)))
@@ -623,40 +613,56 @@ int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image
     float* d = depth ? depth : (var ? WF(p.w_c) : nullptr);
     if (use_cascade)
         return mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_q), nullptr, p.Sq, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
-                                  nullptr, rgb, d, var, nullptr, st);
+                                  nullptr, rgb, d, var, lam, st);
     return mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_q), nullptr, p.Sq, TF(p.raw_c), TF(p.z_c), nullptr, S, TF(p.last_delta), N, 0,
-                              all, nullptr, rgb, d, var, nullptr, st);
+                              all, nullptr, rgb, d, var, lam, st);
 }
 
-int train_backward_impl(mn_ctx* ctx, mn_model* m, int64_t N, int S, int F, int use_cascade, int sh_deg, int precision,
-                        const float* g_rgb, const float* g_rgb_coarse, const void* tape_d, size_t tape_bytes, float* gw,
-                        void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
-    const char* name = "mn_render_rays_train_backward";
+int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N, const float* z_steps_d,
+               const float* jitter_d, float perturb, int S, const float* noise_c_d, const float* u_d, const float* noise_f_d, int F,
+               int use_cascade, int sh_deg, int precision, float* rgb, float* depth, float* var, float* rgb_coarse, void* tape_d,
+               size_t tape_bytes, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+    const char* name = "mn_render_rays_train";
     const std::string nm(name);
-    if (!ctx || !m || !g_rgb || !gw) return MN_ERR_INVALID;
+    if (!ctx || !m || !rays_d || !z_steps_d || !u_d || !rgb) return MN_ERR_INVALID;
     int rc;
     if ((rc = check_train(ctx, m, N, S, F, precision, name))) return rc;
+    if ((rc = check_net(ctx, m, use_cascade, F, sh_deg, image_indices_d, name))) return rc;
+    if (perturb > 0 && !jitter_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": perturb > 0 needs jitter_d");
+    if (use_cascade && !rgb_coarse) return mn_fail(ctx, MN_ERR_INVALID, nm + ": rgb_coarse_out_d is required under use_cascade");
     if (N == 0) return MN_OK;
     const bool sh = sh_deg >= 0, tc = precision == MN_PREC_TC_F16;
     const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh, tc);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
-    if (!workspace_d || workspace_bytes < p.bwd_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
-    const char* T = (const char*)tape_d;
-    char* W = (char*)workspace_d;
+    if (!workspace_d || workspace_bytes < p.ws_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
+    char* T = (char*)tape_d;
+    fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(reinterpret_cast<float*>(T + p.last_delta), N, 1e10f);   // rendering.py:33
+    MN_LAUNCH_CHECK(ctx);
+    return train_fg_pass(ctx, m, p, T, (char*)workspace_d, rays_d, image_indices_d, N, nullptr, z_steps_d, jitter_d, perturb, noise_c_d,
+                         u_d, noise_f_d, use_cascade, sh_deg, rgb, depth, var, rgb_coarse, nullptr, nullptr, st);
+}
+
+// The backward of train_fg_pass: the composite backward(s) - with the gradients of bg_lambda (g_lam, g_lam_c; null: none) - then
+// the model backwards in reverse order of their forward calls, into gw.
+int train_fg_backward(mn_ctx* ctx, mn_model* m, const TrainPlan& p, const char* T, char* W, int64_t N, int use_cascade, int sh_deg,
+                      const float* g_rgb, const float* g_rgb_coarse, const float* g_lam, const float* g_lam_c, float* gw, cudaStream_t st) {
+    const int S = p.S;
+    const bool sh = p.sh, tc = p.tc;
     auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<const float*>(T + off); };
     auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
     const bool coarse = !use_cascade || g_rgb_coarse;     // the coarse query has a gradient
+    int rc;
 
     // composites: the fine one (with the coarse samples merged in, without cascade), the cascade's coarse one
     if (use_cascade) {
-        if ((rc = mn_composite_backward(ctx, TF(p.raw_f), TF(p.z_q), p.Sq, nullptr, nullptr, 0, TF(p.last_delta), N, 0, g_rgb, nullptr,
+        if ((rc = mn_composite_backward(ctx, TF(p.raw_f), TF(p.z_q), p.Sq, nullptr, nullptr, 0, TF(p.last_delta), N, 0, g_rgb, g_lam,
                                         WF(p.g_raw_f), nullptr, st)))
             return rc;
         if (coarse && (rc = mn_composite_backward(ctx, TF(p.raw_c), TF(p.z_c), S, nullptr, nullptr, 0, TF(p.last_delta), N, 0,
-                                                  g_rgb_coarse, nullptr, WF(p.g_raw_c), nullptr, st)))
+                                                  g_rgb_coarse, g_lam_c, WF(p.g_raw_c), nullptr, st)))
             return rc;
     } else if ((rc = mn_composite_backward(ctx, TF(p.raw_f), TF(p.z_q), p.Sq, TF(p.raw_c), TF(p.z_c), S, TF(p.last_delta), N, 0, g_rgb,
-                                           nullptr, WF(p.g_raw_f), WF(p.g_raw_c), st))) {
+                                           g_lam, WF(p.g_raw_f), WF(p.g_raw_c), st))) {
         return rc;
     }
     // the model backwards in reverse order of their forward calls, each through the SH head's backward first
@@ -673,6 +679,360 @@ int train_backward_impl(mn_ctx* ctx, mn_model* m, int64_t N, int S, int F, int u
     };
     if ((rc = model_bwd(p.Sq, 0, p.mlp_f, p.g_raw_f, p.g_mlp_f, p.tape_f, p.tape_f_bytes))) return rc;
     if (coarse) return model_bwd(S, 1, p.mlp_c, p.g_raw_c, p.g_mlp_c, p.tape_c, p.tape_c_bytes);
+    return MN_OK;
+}
+
+int train_backward_impl(mn_ctx* ctx, mn_model* m, int64_t N, int S, int F, int use_cascade, int sh_deg, int precision,
+                        const float* g_rgb, const float* g_rgb_coarse, const void* tape_d, size_t tape_bytes, float* gw,
+                        void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+    const char* name = "mn_render_rays_train_backward";
+    const std::string nm(name);
+    if (!ctx || !m || !g_rgb || !gw) return MN_ERR_INVALID;
+    int rc;
+    if ((rc = check_train(ctx, m, N, S, F, precision, name))) return rc;
+    if (N == 0) return MN_OK;
+    const bool sh = sh_deg >= 0, tc = precision == MN_PREC_TC_F16;
+    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh, tc);
+    if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
+    if (!workspace_d || workspace_bytes < p.bwd_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
+    return train_fg_backward(ctx, m, p, (const char*)tape_d, (char*)workspace_d, N, use_cascade, sh_deg, g_rgb, g_rgb_coarse, nullptr,
+                             nullptr, gw, st);
+}
+
+// ---- mn_render_rays_train_bg: the recording render with a background network and its backward ------------------------------
+// Rows of a [N, cols] draw block of ray ids -> its rows in compacted order: dst[p] = src[ids[p]] for the live background rays.
+__global__ void gather_rows_kernel(const float* __restrict__ src, const int64_t* __restrict__ ids, const int* __restrict__ count,
+                                   int64_t N, int cols, float* __restrict__ dst) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (int64_t)*count * cols) return;
+    const int64_t p = t / cols;
+    dst[t] = src[ids[p] * cols + (t - p * cols)];
+}
+
+// torch.flip(z, [-1]) of the live rows of [N, S]
+__global__ void flip_rows_kernel(const float* __restrict__ z, int64_t N, int S, LiveRows live, float* __restrict__ out) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= live.rows(N) * S) return;
+    const int64_t r = t / S;
+    out[r * S + (S - 1 - (t - r * S))] = z[t];
+}
+
+// Backward of the lambda blend val + bg_val[pos] * lam (bg_blend_kernel, torch's mul and index backwards): g_bg[pos[i]] =
+// g[i] * lam[i]; g_lam[i] = sum_c g[i, c] * bg_val[pos[i], c], 0 for a ray that stays in the foreground.
+__global__ void bg_blend_backward_kernel(const float* __restrict__ g, const float* __restrict__ lam, const float* __restrict__ bg_val,
+                                         const int* __restrict__ pos, int64_t N, float* __restrict__ g_lam, float* __restrict__ g_bg) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= N) return;
+    const int p = pos[i];
+    float gl = 0.0f;
+    if (p >= 0) {
+        const float* gi = g + i * 3;
+        const float* b = bg_val + (int64_t)p * 3;
+        for (int c = 0; c < 3; ++c) g_bg[(int64_t)p * 3 + c] = __fmul_rn(gi[c], lam[i]);
+        gl = __fadd_rn(__fadd_rn(__fmul_rn(gi[0], b[0]), __fmul_rn(gi[1], b[1])), __fmul_rn(gi[2], b[2]));
+    }
+    g_lam[i] = gl;
+}
+
+// The buffers of the background network's recording pass over N rays (the compacted background rays first), after the
+// foreground's TrainPlan in each of the three regions.  S / F: the background's coarse samples and fine draws (half the
+// foreground's), Sq: its fine-query samples.  Tape: the split (compacted positions and count), the blend's inputs (bg_lambda
+// of both types, the background colours), the composite inputs in composite order (coarse depths reversed; fine-query depths
+// reversed under cascade), the raw rows, the compacted directions and raw SH coefficients for an SH head, and the two model
+// tapes.  Workspace: the rest of the split, the depths in sample order, the points, the weights, the gathered draws of ray-indexed
+// blocks and the model calls' workspace.  Backward workspace: the blend's gradients, the per-sample gradients and the model
+// backward's workspace.
+struct BgTrainPlan {
+    TrainPlan fg;
+    int S, F, Sq, cols;
+    bool tc, sh;
+    size_t pos, count, ld_b, lam, lam_c, rgb_b, rgb_cb, dirs, z_cc, raw_c, z_qc, raw_f, mlp_c, mlp_f, tape_c, tape_f, tape_c_bytes,
+        tape_f_bytes, tape_total;
+    size_t far_ov, blk, ids, idx, z_c, xyz_c, dreal_c, w_c, z_f, z_q, xyz_f, dreal_f, depth_b, jit, u, noise_c, noise_f, model_ws,
+        model_ws_bytes, ws_total;
+    size_t g_rgb_b, g_rgb_cb, g_lam, g_lam_c, g_raw_c, g_raw_f, g_mlp_c, g_mlp_f, bwd_ws, bwd_ws_bytes, bwd_total;
+};
+
+BgTrainPlan make_bg_train_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, bool sh, bool tc,
+                               bool bg_tc) {
+    BgTrainPlan p{};
+    p.fg = make_train_plan(m, N, Sc, Sf, use_cascade, sh, tc);
+    p.S = Sc / 2; p.F = Sf / 2; p.Sq = use_cascade ? p.S + p.F : p.F; p.tc = bg_tc; p.sh = sh;
+    p.cols = bg->d.kind == 2 && bg->d.xyz_real ? 7 : 4;      // the real-xyz routing prefix, then [point, 1/r]
+    const int64_t Bc = N * p.S, Bf = N * p.Sq;
+    const int out_cols = bg->nd.rgb_dim + 1;
+    Carve t;
+    t.off = p.fg.tape_total;
+    p.pos = t((size_t)N * 4);
+    p.count = t(4);
+    p.ld_b = t((size_t)N * 4);
+    p.lam = t((size_t)N * 4);
+    p.lam_c = t((size_t)N * 4);
+    p.rgb_b = t((size_t)N * 12);
+    p.rgb_cb = t((size_t)N * 12);
+    p.dirs = t((size_t)N * 12);
+    p.z_cc = t((size_t)Bc * 4);
+    p.raw_c = t((size_t)Bc * 16);
+    p.z_qc = t((size_t)Bf * 4);
+    p.raw_f = t((size_t)Bf * 16);
+    p.mlp_c = sh ? t((size_t)Bc * out_cols * 4) : kNone;
+    p.mlp_f = sh ? t((size_t)Bf * out_cols * 4) : kNone;
+    p.tape_c_bytes = bg_tc ? mn_model_tape_bytes_tc(bg, Bc) : mn_model_tape_bytes(bg, Bc);
+    p.tape_f_bytes = bg_tc ? mn_model_tape_bytes_tc(bg, Bf) : mn_model_tape_bytes(bg, Bf);
+    p.tape_c = t(p.tape_c_bytes);
+    p.tape_f = t(p.tape_f_bytes);
+    p.tape_total = t.off + 256;
+    Carve w;
+    w.off = p.fg.ws_total;
+    p.far_ov = w((size_t)N * 4);
+    p.blk = w((size_t)mn_cdiv(N, kSplitBlock) * 4);
+    p.ids = w((size_t)N * 8);
+    p.idx = w((size_t)N * 4);
+    p.z_c = w((size_t)Bc * 4);
+    p.xyz_c = w((size_t)Bc * p.cols * 4);
+    p.dreal_c = w((size_t)Bc * 4);
+    p.w_c = w((size_t)Bc * 4);
+    p.z_f = use_cascade ? w((size_t)N * p.F * 4) : kNone;      // without cascade the fine draws are the fine-query depths (tape)
+    p.z_q = use_cascade ? w((size_t)Bf * 4) : kNone;
+    p.xyz_f = w((size_t)Bf * p.cols * 4);
+    p.dreal_f = w((size_t)Bf * 4);
+    p.depth_b = w((size_t)N * 4);
+    p.jit = w((size_t)Bc * 4);
+    p.u = w((size_t)N * p.F * 4);
+    p.noise_c = w((size_t)Bc * 4);
+    p.noise_f = w((size_t)Bf * 4);
+    const size_t a = mn_model_workspace_bytes(bg, Bc, MN_PREC_FP32), c = mn_model_workspace_bytes(bg, Bf, MN_PREC_FP32);
+    p.model_ws_bytes = a > c ? a : c;
+    p.model_ws = w(p.model_ws_bytes);
+    p.ws_total = w.off + 256;
+    Carve b;
+    b.off = p.fg.bwd_total;
+    p.g_rgb_b = b((size_t)N * 12);
+    p.g_rgb_cb = b((size_t)N * 12);
+    p.g_lam = b((size_t)N * 4);
+    p.g_lam_c = b((size_t)N * 4);
+    p.g_raw_c = b((size_t)Bc * 16);
+    p.g_raw_f = b((size_t)Bf * 16);
+    p.g_mlp_c = sh ? b((size_t)Bc * out_cols * 4) : kNone;
+    p.g_mlp_f = sh ? b((size_t)Bf * out_cols * 4) : kNone;
+    const size_t ba = bg_tc ? mn_model_backward_workspace_bytes_tc(bg, Bc) : mn_model_backward_workspace_bytes(bg, Bc);
+    const size_t bc = bg_tc ? mn_model_backward_workspace_bytes_tc(bg, Bf) : mn_model_backward_workspace_bytes(bg, Bf);
+    p.bwd_ws_bytes = ba > bc ? ba : bc;
+    p.bwd_ws = b(p.bwd_ws_bytes);
+    p.bwd_total = b.off + 256;
+    return p;
+}
+
+// The checks shared by the background train render, its backward and their size queries.
+int check_train_bg(mn_ctx* ctx, const mn_model* m, const mn_model* bg, int64_t N, int Sc, int Sf, int precision, int bg_precision,
+                   const char* name) {
+    int rc;
+    if ((rc = check_train(ctx, m, N, Sc, Sf, precision, name))) return rc;
+    if ((rc = check_train(ctx, bg, N, Sc / 2, Sf / 2, bg_precision, name))) return rc;
+    return MN_OK;
+}
+
+int train_bg_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, const float* image_indices_d, int64_t N,
+                  const float* center_d, const float* radius_d, int include_xyz_real, int cluster_2d, const float* z_steps_d,
+                  const float* z_steps_bg_d, const float* jitter_d, const float* jitter_bg_d, float perturb, int Sc,
+                  const float* noise_c_d, const float* noise_c_bg_d, const float* u_d, const float* u_bg_d, const float* noise_f_d,
+                  const float* noise_f_bg_d, int Sf, int use_cascade, int sh_deg, int precision, int bg_precision, int by_ray,
+                  const mn_render_outputs* out, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes,
+                  cudaStream_t st) {
+    const char* name = "mn_render_rays_train_bg";
+    const std::string nm(name);
+    if (!ctx || !m || !bg || !rays_d || !z_steps_d || !z_steps_bg_d || !u_d || !u_bg_d || !out || !out->rgb || !out->bg_lambda)
+        return MN_ERR_INVALID;
+    const mn_render_outputs& o = *out;
+    int rc;
+    if ((rc = check_train_bg(ctx, m, bg, N, Sc, Sf, precision, bg_precision, name))) return rc;
+    if ((rc = check_net(ctx, m, use_cascade, Sf, sh_deg, image_indices_d, name))) return rc;
+    if ((rc = check_net(ctx, bg, use_cascade, Sf, sh_deg, image_indices_d, name))) return rc;
+    if (perturb > 0 && (!jitter_d || !jitter_bg_d)) return mn_fail(ctx, MN_ERR_INVALID, nm + ": perturb > 0 needs jitter_d and jitter_bg_d");
+    if (use_cascade && (!o.rgb_coarse || !o.bg_lambda_coarse))
+        return mn_fail(ctx, MN_ERR_INVALID, nm + ": rgb_coarse and bg_lambda_coarse are required under use_cascade");
+    if (radius_d && !center_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": sphere radius without a center");
+    if (include_xyz_real != (bg->d.kind == 2 && bg->d.xyz_real ? 1 : 0))
+        return mn_fail(ctx, MN_ERR_INVALID, nm + ": include_xyz_real must match the background model's real-xyz prefix");
+    if (N == 0) return MN_OK;
+    const bool sh = sh_deg >= 0;
+    const BgTrainPlan p = make_bg_train_plan(m, bg, N, Sc, Sf, use_cascade, sh, precision == MN_PREC_TC_F16,
+                                             bg_precision == MN_PREC_TC_F16);
+    if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
+    if (!workspace_d || workspace_bytes < p.ws_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
+    char* T = (char*)tape_d;
+    char* W = (char*)workspace_d;
+    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(T + off); };
+    auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
+    int* pos = reinterpret_cast<int*>(T + p.pos);
+    const int* cnt = reinterpret_cast<const int*>(T + p.count);
+    const int64_t* ids = reinterpret_cast<const int64_t*>(W + p.ids);
+    const LiveRows lr{cnt, 1};
+
+    // ---- split and compaction (render.py:327-342): the foreground's last deltas land in its tape
+    const unsigned nblk = (unsigned)mn_cdiv(N, kSplitBlock);
+    bg_split_kernel<<<nblk, kSplitBlock, 0, st>>>(rays_d, center_d, radius_d, N, WF(p.far_ov), TF(p.fg.last_delta), pos,
+                                                 reinterpret_cast<int*>(W + p.blk), ctx->status_d);
+    MN_LAUNCH_CHECK(ctx);
+    float* bidx = image_indices_d ? WF(p.idx) : nullptr;
+    bg_compact_kernel<<<nblk, kSplitBlock, 0, st>>>(rays_d, image_indices_d, N, reinterpret_cast<int*>(W + p.blk), pos,
+                                                   reinterpret_cast<int64_t*>(W + p.ids), TF(p.dirs), bidx, reinterpret_cast<int*>(T + p.count));
+    MN_LAUNCH_CHECK(ctx);
+    fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(TF(p.ld_b), N, 1e10f);            // the background's last delta
+    MN_LAUNCH_CHECK(ctx);
+
+    // ---- the background draws in compacted order: ray-indexed blocks are gathered at the background rays
+    const float *jit = jitter_bg_d, *ub = u_bg_d, *nc = noise_c_bg_d, *nf = noise_f_bg_d;
+    if (by_ray) {
+        auto gather = [&](const float*& src, int cols, size_t dst) -> int {
+            if (!src) return MN_OK;
+            gather_rows_kernel<<<(unsigned)mn_cdiv(N * cols, 256), 256, 0, st>>>(src, ids, cnt, N, cols, WF(dst));
+            MN_LAUNCH_CHECK(ctx);
+            src = WF(dst);
+            return MN_OK;
+        };
+        if ((rc = gather(jit, p.S, p.jit)) || (rc = gather(ub, p.F, p.u)) || (rc = gather(nc, p.S, p.noise_c)) ||
+            (rc = gather(nf, p.Sq, p.noise_f)))
+            return rc;
+    }
+
+    // ---- background pass over the compacted rays (render.py `bg_pass`, `_two_pass` flipped): stratified depths in sample order
+    // and reversed, the points outside the sphere in reversed sample order, recording coarse query, composite, resampling,
+    // recording fine query, composite
+    auto outside = [&](const float* z, int S, int flip_pts, float* xyz, float* dreal) {
+        return mn_stage_points_outside(ctx, rays_d, ids, z, center_d, radius_d, N, S, include_xyz_real, cluster_2d, flip_pts, lr, xyz,
+                                       dreal, st);
+    };
+    auto bquery = [&](const float* xyz, int S, int coarse, const float* noise, float* mlp_out, float* raw_out, size_t tape,
+                      size_t tape_n) -> int {
+        mn_rows rows{};
+        rows.mode = 1;
+        rows.x_d = xyz;
+        rows.cols = p.cols;
+        rows.dirs_d = bg->d.pos_dir_dim > 0 ? TF(p.dirs) : nullptr;
+        rows.dir_stride = 3;
+        rows.idx_d = bg->d.appearance_dim > 0 ? bidx : nullptr;
+        rows.samples_per_ray = S;
+        const LiveRows lrs{cnt, S};
+        int r = mn_model_forward_train_live(ctx, bg, &rows, N * S, lrs, coarse, noise, bg_precision, sh ? mlp_out : raw_out, T + tape,
+                                            tape_n, W + p.model_ws, p.model_ws_bytes, st);
+        if (r) return r;
+        if (sh) return mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, bg->nd.rgb_dim + 1, TF(p.dirs), 3, S, N * S, 1, lrs, raw_out, st);
+        return MN_OK;
+    };
+    if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, jit, perturb, N, p.S, 0, lr, WF(p.z_c), st))) return rc;
+    flip_rows_kernel<<<(unsigned)mn_cdiv(N * p.S, 256), 256, 0, st>>>(WF(p.z_c), N, p.S, lr, TF(p.z_cc));
+    MN_LAUNCH_CHECK(ctx);
+    if ((rc = outside(WF(p.z_c), p.S, 1, WF(p.xyz_c), WF(p.dreal_c)))) return rc;
+    if ((rc = bquery(WF(p.xyz_c), p.S, 1, nc, TF(p.mlp_c), TF(p.raw_c), p.tape_c, p.tape_c_bytes))) return rc;
+    // resampling weights and, under cascade, the coarse colour: one composite (the detached one of the reference computes the same)
+    if ((rc = mn_stage_composite(ctx, TF(p.raw_c), TF(p.z_cc), WF(p.dreal_c), p.S, nullptr, nullptr, nullptr, 0, TF(p.ld_b), N, 1, lr,
+                                 WF(p.w_c), use_cascade ? TF(p.rgb_cb) : nullptr, nullptr, nullptr, nullptr, st)))
+        return rc;
+    if ((rc = mn_stage_sample_pdf(ctx, WF(p.z_c), WF(p.w_c), p.S, nullptr, ub, p.F, N, p.S, p.F, lr,
+                                  use_cascade ? WF(p.z_f) : TF(p.z_qc), nullptr, nullptr, st)))
+        return rc;
+    float* depth_b = o.depth ? WF(p.depth_b) : nullptr;
+    if (use_cascade) {
+        if ((rc = mn_stage_sort_cat(ctx, WF(p.z_c), p.S, WF(p.z_f), p.F, N, 0, lr, WF(p.z_q), TF(p.z_qc), st))) return rc;
+        if ((rc = outside(WF(p.z_q), p.Sq, 1, WF(p.xyz_f), WF(p.dreal_f)))) return rc;
+        if ((rc = bquery(WF(p.xyz_f), p.Sq, 0, nf, TF(p.mlp_f), TF(p.raw_f), p.tape_f, p.tape_f_bytes))) return rc;
+        rc = mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_qc), WF(p.dreal_f), p.Sq, nullptr, nullptr, nullptr, 0, TF(p.ld_b), N, 1, lr,
+                                nullptr, TF(p.rgb_b), depth_b, nullptr, nullptr, st);
+    } else {
+        if ((rc = outside(TF(p.z_qc), p.Sq, 0, WF(p.xyz_f), WF(p.dreal_f)))) return rc;
+        if ((rc = bquery(WF(p.xyz_f), p.Sq, 0, nf, TF(p.mlp_f), TF(p.raw_f), p.tape_f, p.tape_f_bytes))) return rc;
+        rc = mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_qc), WF(p.dreal_f), p.Sq, TF(p.raw_c), TF(p.z_cc), WF(p.dreal_c), p.S,
+                                TF(p.ld_b), N, 1, lr, nullptr, TF(p.rgb_b), depth_b, nullptr, nullptr, st);
+    }
+    if (rc) return rc;
+
+    // ---- foreground pass with the far override, the last deltas and bg_lambda of both types (render.py:344-348)
+    if ((rc = train_fg_pass(ctx, m, p.fg, T, W, rays_d, image_indices_d, N, WF(p.far_ov), z_steps_d, jitter_d, perturb, noise_c_d, u_d,
+                            noise_f_d, use_cascade, sh_deg, o.rgb, o.depth, o.depth_var, o.rgb_coarse, TF(p.lam),
+                            use_cascade ? TF(p.lam_c) : nullptr, st)))
+        return rc;
+    MN_CUDA(ctx, cudaMemcpyAsync(o.bg_lambda, TF(p.lam), (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
+    if (use_cascade) MN_CUDA(ctx, cudaMemcpyAsync(o.bg_lambda_coarse, TF(p.lam_c), (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
+
+    // ---- blend (render.py:350-376)
+    auto blend = [&](float* val, const float* bval, const float* l, int C, float* fg_out, float* bg_out) -> int {
+        bg_blend_kernel<<<(unsigned)mn_cdiv(N * C, 256), 256, 0, st>>>(val, bval, l, pos, N, C, fg_out, bg_out);
+        MN_LAUNCH_CHECK(ctx);
+        return MN_OK;
+    };
+    if ((rc = blend(o.rgb, TF(p.rgb_b), TF(p.lam), 3, o.fg_rgb, o.bg_rgb))) return rc;
+    if (o.depth)
+        if ((rc = blend(o.depth, WF(p.depth_b), TF(p.lam), 1, o.fg_depth, o.bg_depth))) return rc;
+    if (use_cascade)
+        if ((rc = blend(o.rgb_coarse, TF(p.rgb_cb), TF(p.lam_c), 3, o.fg_rgb_coarse, o.bg_rgb_coarse))) return rc;
+    return MN_OK;
+}
+
+int train_bg_backward_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, int sh_deg, int precision,
+                           int bg_precision, const float* g_rgb, const float* g_rgb_coarse, const void* tape_d, size_t tape_bytes,
+                           float* gw, float* gw_bg, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+    const char* name = "mn_render_rays_train_bg_backward";
+    const std::string nm(name);
+    if (!ctx || !m || !bg || !g_rgb || !gw || !gw_bg) return MN_ERR_INVALID;
+    int rc;
+    if ((rc = check_train_bg(ctx, m, bg, N, Sc, Sf, precision, bg_precision, name))) return rc;
+    if (N == 0) return MN_OK;
+    const bool sh = sh_deg >= 0;
+    const BgTrainPlan p = make_bg_train_plan(m, bg, N, Sc, Sf, use_cascade, sh, precision == MN_PREC_TC_F16,
+                                             bg_precision == MN_PREC_TC_F16);
+    if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
+    if (!workspace_d || workspace_bytes < p.bwd_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
+    const char* T = (const char*)tape_d;
+    char* W = (char*)workspace_d;
+    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<const float*>(T + off); };
+    auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
+    const int* pos = reinterpret_cast<const int*>(T + p.pos);
+    const int* cnt = reinterpret_cast<const int*>(T + p.count);
+    const LiveRows lr{cnt, 1};
+    const bool coarse = !use_cascade || g_rgb_coarse;     // the coarse queries have a gradient
+
+    // ---- blend backward: the background colours' and bg_lambda's gradients
+    auto blend_bwd = [&](const float* g, size_t lam, size_t bval, size_t g_lam, size_t g_bg) -> int {
+        bg_blend_backward_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(g, TF(lam), TF(bval), pos, N, WF(g_lam), WF(g_bg));
+        MN_LAUNCH_CHECK(ctx);
+        return MN_OK;
+    };
+    if ((rc = blend_bwd(g_rgb, p.lam, p.rgb_b, p.g_lam, p.g_rgb_b))) return rc;
+    if (use_cascade && coarse && (rc = blend_bwd(g_rgb_coarse, p.lam_c, p.rgb_cb, p.g_lam_c, p.g_rgb_cb))) return rc;
+
+    // ---- foreground: composites (with bg_lambda) and model backwards
+    if ((rc = train_fg_backward(ctx, m, p.fg, T, W, N, use_cascade, sh_deg, g_rgb, g_rgb_coarse, WF(p.g_lam),
+                                use_cascade && coarse ? WF(p.g_lam_c) : nullptr, gw, st)))
+        return rc;
+
+    // ---- background: composites, then the model backwards over the live rows
+    if (use_cascade) {
+        if ((rc = mn_stage_composite_backward(ctx, TF(p.raw_f), TF(p.z_qc), p.Sq, nullptr, nullptr, 0, TF(p.ld_b), N, 1, lr, WF(p.g_rgb_b),
+                                              nullptr, WF(p.g_raw_f), nullptr, st)))
+            return rc;
+        if (coarse && (rc = mn_stage_composite_backward(ctx, TF(p.raw_c), TF(p.z_cc), p.S, nullptr, nullptr, 0, TF(p.ld_b), N, 1, lr,
+                                                        WF(p.g_rgb_cb), nullptr, WF(p.g_raw_c), nullptr, st)))
+            return rc;
+    } else if ((rc = mn_stage_composite_backward(ctx, TF(p.raw_f), TF(p.z_qc), p.Sq, TF(p.raw_c), TF(p.z_cc), p.S, TF(p.ld_b), N, 1, lr,
+                                                 WF(p.g_rgb_b), nullptr, WF(p.g_raw_f), WF(p.g_raw_c), st))) {
+        return rc;
+    }
+    auto model_bwd = [&](int S, int use_coarse, size_t mlp, size_t g_raw, size_t g_mlp, size_t tape, size_t tape_n) -> int {
+        const LiveRows lrs{cnt, S};
+        const float* g = WF(g_raw);
+        int r;
+        if (sh) {
+            if ((r = mn_stage_sh_to_rgb_backward(ctx, sh_deg, TF(mlp), bg->nd.rgb_dim + 1, TF(p.dirs), 3, S, N * S, 1, lrs, g, WF(g_mlp),
+                                                 st)))
+                return r;
+            g = WF(g_mlp);
+        }
+        return mn_model_backward_live(ctx, bg, N * S, lrs, use_coarse, bg_precision, g, T + tape, tape_n, gw_bg, W + p.bwd_ws,
+                                      p.bwd_ws_bytes, st);
+    };
+    if ((rc = model_bwd(p.Sq, 0, p.mlp_f, p.g_raw_f, p.g_mlp_f, p.tape_f, p.tape_f_bytes))) return rc;
+    if (coarse) return model_bwd(p.S, 1, p.mlp_c, p.g_raw_c, p.g_mlp_c, p.tape_c, p.tape_c_bytes);
     return MN_OK;
 }
 
@@ -794,6 +1154,51 @@ int mn_render_rays_train_backward(mn_ctx* ctx, mn_model* m, int64_t N, int coars
                                   size_t workspace_bytes, void* stream) {
     return train_backward_impl(ctx, m, N, coarse_samples, fine_samples, use_cascade, sh_deg, precision, grad_rgb_d, grad_rgb_coarse_d,
                                tape_d, tape_bytes, param_grads_d, workspace_d, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t mn_render_rays_train_bg_tape_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                          int use_cascade, int sh_deg, int precision, int bg_precision) {
+    if (!fg || !bg || check_train_bg(nullptr, fg, bg, N, coarse_samples, fine_samples, precision, bg_precision, "")) return 0;
+    return make_bg_train_plan(fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
+                              bg_precision == MN_PREC_TC_F16).tape_total;
+}
+
+size_t mn_render_rays_train_bg_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                               int use_cascade, int sh_deg, int precision, int bg_precision) {
+    if (!fg || !bg || check_train_bg(nullptr, fg, bg, N, coarse_samples, fine_samples, precision, bg_precision, "")) return 0;
+    return make_bg_train_plan(fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
+                              bg_precision == MN_PREC_TC_F16).ws_total;
+}
+
+size_t mn_render_rays_train_bg_backward_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples,
+                                                        int fine_samples, int use_cascade, int sh_deg, int precision, int bg_precision) {
+    if (!fg || !bg || check_train_bg(nullptr, fg, bg, N, coarse_samples, fine_samples, precision, bg_precision, "")) return 0;
+    return make_bg_train_plan(fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
+                              bg_precision == MN_PREC_TC_F16).bwd_total;
+}
+
+int mn_render_rays_train_bg(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays_d, const float* image_indices_d, int64_t N,
+                            const float* sphere_center3_d, const float* sphere_radius3_d, int include_xyz_real, int cluster_2d,
+                            const float* z_steps_d, const float* z_steps_bg_d, const float* jitter_d, const float* jitter_bg_d,
+                            float perturb, int coarse_samples, const float* sigma_noise_coarse_d, const float* sigma_noise_coarse_bg_d,
+                            const float* u_fine_d, const float* u_fine_bg_d, const float* sigma_noise_fine_d,
+                            const float* sigma_noise_fine_bg_d, int fine_samples, int use_cascade, int sh_deg, int precision,
+                            int bg_precision, int bg_draws_by_ray, const mn_render_outputs* out, void* tape_d, size_t tape_bytes,
+                            void* workspace_d, size_t workspace_bytes, void* stream) {
+    return train_bg_impl(ctx, fg, bg, rays_d, image_indices_d, N, sphere_center3_d, sphere_radius3_d, include_xyz_real, cluster_2d,
+                         z_steps_d, z_steps_bg_d, jitter_d, jitter_bg_d, perturb, coarse_samples, sigma_noise_coarse_d,
+                         sigma_noise_coarse_bg_d, u_fine_d, u_fine_bg_d, sigma_noise_fine_d, sigma_noise_fine_bg_d, fine_samples,
+                         use_cascade, sh_deg, precision, bg_precision, bg_draws_by_ray, out, tape_d, tape_bytes, workspace_d,
+                         workspace_bytes, (cudaStream_t)stream);
+}
+
+int mn_render_rays_train_bg_backward(mn_ctx* ctx, mn_model* fg, mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                     int use_cascade, int sh_deg, int precision, int bg_precision, const float* grad_rgb_d,
+                                     const float* grad_rgb_coarse_d, const void* tape_d, size_t tape_bytes, float* param_grads_d,
+                                     float* bg_param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream) {
+    return train_bg_backward_impl(ctx, fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg, precision, bg_precision, grad_rgb_d,
+                                  grad_rgb_coarse_d, tape_d, tape_bytes, param_grads_d, bg_param_grads_d, workspace_d, workspace_bytes,
+                                  (cudaStream_t)stream);
 }
 
 }  // extern "C"

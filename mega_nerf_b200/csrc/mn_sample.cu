@@ -673,6 +673,7 @@ struct CompositeBwdArgs {
     float* grad_raw;            // [N,S,4]
     float* grad_raw2;           // [N,S2,4]
     int npad;
+    LiveRows live;              // rays at or past live.rows(N) are skipped
 };
 
 __device__ __forceinline__ double warp_incl_suffix_add(double v, int lane) {
@@ -688,7 +689,7 @@ __global__ void __launch_bounds__(128) composite_bwd_kernel(const CompositeBwdAr
     extern __shared__ unsigned char sm_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t ray = (int64_t)blockIdx.x * 4 + warp;
-    if (ray >= a.N) return;
+    if (ray >= a.live.rows(a.N)) return;
     const int n = a.S + a.S2;
     const CompositeSmem sm = composite_smem(sm_raw, warp, a.npad);
     const float* zs = sm.zs;
@@ -795,9 +796,9 @@ __device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, flo
 
 __global__ void sh_to_rgb_bwd_kernel(int deg, const float* __restrict__ coef, int64_t cstride, const float* __restrict__ dirs,
                                      int64_t dstride, int ddiv, int64_t B, int sig, const float* __restrict__ gout,
-                                     float* __restrict__ gcoef) {
+                                     float* __restrict__ gcoef, LiveRows live) {
     const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= B) return;
+    if (b >= live.rows(B)) return;
     const int nc = (deg + 1) * (deg + 1);
     const float* c = coef + b * cstride;
     const float* d = dirs + (b / ddiv) * dstride;
@@ -938,13 +939,8 @@ int mn_composite_backward(mn_ctx* ctx, const float* raw_d, const float* z_d, int
     if (!ctx || !raw_d || !z_d || !last_delta_d || !grad_rgb_d || !grad_raw_d || S < 1 || S2 < 0) return MN_ERR_INVALID;
     if (S2 > 0 && (!raw2_d || !z2_d || !grad_raw2_d)) return MN_ERR_INVALID;
     if (N == 0) return MN_OK;
-    CompositeBwdArgs a{};
-    a.raw = raw_d; a.z = z_d; a.S = S;
-    a.raw2 = raw2_d; a.z2 = z2_d; a.S2 = S2;
-    a.last_delta = last_delta_d; a.N = N; a.flip = flip;
-    a.grad_rgb = grad_rgb_d; a.grad_lambda = grad_lambda_d;
-    a.grad_raw = grad_raw_d; a.grad_raw2 = grad_raw2_d;
-    return composite_launch(ctx, composite_bwd_kernel, a, "mn_composite_backward", (cudaStream_t)stream);
+    return mn_stage_composite_backward(ctx, raw_d, z_d, S, raw2_d, z2_d, S2, last_delta_d, N, flip, LiveRows{}, grad_rgb_d, grad_lambda_d,
+                                       grad_raw_d, grad_raw2_d, (cudaStream_t)stream);
 }
 
 int mn_sh_to_rgb_backward(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d,
@@ -952,10 +948,8 @@ int mn_sh_to_rgb_backward(mn_ctx* ctx, int deg, const float* coef_d, int64_t coe
                           float* grad_coef_d, void* stream) {
     if (!ctx || !coef_d || !dirs_d || !grad_out_d || !grad_coef_d || deg < 0 || deg > 4 || dir_div < 1) return MN_ERR_INVALID;
     if (B == 0) return MN_OK;
-    sh_to_rgb_bwd_kernel<<<(unsigned)mn_cdiv(B, 256), 256, 0, (cudaStream_t)stream>>>(
-        deg, coef_d, coef_stride, dirs_d, dir_stride, dir_div, B, apply_sigmoid, grad_out_d, grad_coef_d);
-    MN_LAUNCH_CHECK(ctx);
-    return MN_OK;
+    return mn_stage_sh_to_rgb_backward(ctx, deg, coef_d, coef_stride, dirs_d, dir_stride, dir_div, B, apply_sigmoid, LiveRows{}, grad_out_d,
+                                       grad_coef_d, (cudaStream_t)stream);
 }
 
 int mn_intersect_sphere(mn_ctx* ctx, const float* rays_d, const float* center3_d, const float* radius3_d, int64_t N,
@@ -1057,6 +1051,28 @@ int mn_stage_sh_to_rgb(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_s
                        int dir_div, int64_t B, int apply_sigmoid, LiveRows live, float* out_d, cudaStream_t st, const int* gather) {
     sh_to_rgb_kernel<<<(unsigned)mn_cdiv(B, 256), 256, 0, st>>>(deg, coef_d, coef_stride, dirs_d, dir_stride, dir_div, B, apply_sigmoid,
                                                                 out_d, live, gather);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+int mn_stage_composite_backward(mn_ctx* ctx, const float* raw_d, const float* z_d, int S, const float* raw2_d, const float* z2_d, int S2,
+                                const float* last_delta_d, int64_t N, int flip, LiveRows live, const float* grad_rgb_d,
+                                const float* grad_lambda_d, float* grad_raw_d, float* grad_raw2_d, cudaStream_t st) {
+    CompositeBwdArgs a{};
+    a.raw = raw_d; a.z = z_d; a.S = S;
+    a.raw2 = raw2_d; a.z2 = z2_d; a.S2 = S2;
+    a.last_delta = last_delta_d; a.N = N; a.flip = flip;
+    a.grad_rgb = grad_rgb_d; a.grad_lambda = grad_lambda_d;
+    a.grad_raw = grad_raw_d; a.grad_raw2 = grad_raw2_d;
+    a.live = live;
+    return composite_launch(ctx, composite_bwd_kernel, a, "mn_composite_backward", st);
+}
+
+int mn_stage_sh_to_rgb_backward(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
+                                int dir_div, int64_t B, int apply_sigmoid, LiveRows live, const float* grad_out_d, float* grad_coef_d,
+                                cudaStream_t st) {
+    sh_to_rgb_bwd_kernel<<<(unsigned)mn_cdiv(B, 256), 256, 0, st>>>(deg, coef_d, coef_stride, dirs_d, dir_stride, dir_div, B, apply_sigmoid,
+                                                                    grad_out_d, grad_coef_d, live);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }

@@ -27,9 +27,11 @@
 
 // max |g| over the upstream gradient, spread over the machine (an SH head's grad_out has 28 columns per row): every block
 // folds a grid-stride share and publishes its maximum with an integer atomicMax on *maxbits (zeroed by the caller; the bit
-// patterns of non-negative floats order like the values, and fmaxf drops NaNs, so the result is max |g| exactly)
-__global__ void tc_grad_absmax_kernel(const float* __restrict__ g, int64_t n, unsigned* __restrict__ maxbits) {
+// patterns of non-negative floats order like the values, and fmaxf drops NaNs, so the result is max |g| exactly).  Only the
+// live.rows(rows) rows that hold data are read.
+__global__ void tc_grad_absmax_kernel(const float* __restrict__ g, LiveRows live, int64_t rows, int cols, unsigned* __restrict__ maxbits) {
     __shared__ float red[32];
+    const int64_t n = live.rows(rows) * cols;
     float m = 0.0f;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) m = fmaxf(m, fabsf(g[i]));
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
@@ -79,11 +81,15 @@ struct WgArgs {
     int64_t t_min, t_max;           // tiles covered by the launch
     const int* counters;            // routing counters saved by the forward pass, or NULL (all tiles belong to fixed_sub)
     int fixed_sub;
+    LiveRows live;                  // counters == NULL: tiles at or past live.rows(rows) rows hold no tape
+    int64_t rows;
     int chunk_tiles;
     float* gw;                      // [n_sub][sub_stride] fp32
     int64_t sub_stride;
     const float* scale;
 };
+// Last tile + 1 of an unrouted call whose first live.rows(rows) rows hold data.
+__device__ __forceinline__ int64_t tc_live_tiles(LiveRows live, int64_t rows) { return (live.rows(rows) + kTileM - 1) / kTileM; }
 constexpr int kWgStageBytes = 96 * 1024;
 constexpr int kWgThreads = 384;     // warpgroup 0: producer thread; warpgroups 1-2: output channels 0-63 / 64-127 of the item
 
@@ -123,6 +129,8 @@ __global__ void __launch_bounds__(kWgThreads, 1) tc_wgrad_kernel(const WgArgs A)
         sub = (int)blockIdx.z;
         t_lo = max(t_lo, (int64_t)(A.counters[CNT_START + sub] / kTileM));
         t_hi = min(t_hi, (int64_t)(A.counters[CNT_START + sub + 1] / kTileM));
+    } else {
+        t_hi = min(t_hi, tc_live_tiles(A.live, A.rows));
     }
     const int64_t t_begin = t_lo + (int64_t)blockIdx.x * A.chunk_tiles;
     const int64_t t_end = min(t_hi, t_begin + (int64_t)A.chunk_tiles);
@@ -229,6 +237,8 @@ struct HeadsArgs {
     const int* counters;
     int64_t n_tiles;
     int64_t t_min, t_max;           // tiles covered by gf32 (the layer-GEMM path's tile group; 0 .. n_tiles otherwise)
+    LiveRows live;                  // counters == NULL: tiles at or past live.rows(rows) rows hold no tape
+    int64_t rows;
     int fixed_sub, chunk_tiles;
     float* gw;
     int64_t sub_stride;
@@ -249,6 +259,8 @@ __global__ void __launch_bounds__(256) tc_heads_wgrad_kernel(const HeadsArgs A) 
         sub = (int)blockIdx.y;
         t_lo = max(t_lo, (int64_t)(A.counters[CNT_START + sub] / kTileM));
         t_hi = min(A.t_max, (int64_t)(A.counters[CNT_START + sub + 1] / kTileM));
+    } else {
+        t_hi = min(t_hi, tc_live_tiles(A.live, A.rows));
     }
     const int64_t t_begin = t_lo + (int64_t)blockIdx.x * A.chunk_tiles;
     const int64_t t_end = min(t_hi, t_begin + (int64_t)A.chunk_tiles);

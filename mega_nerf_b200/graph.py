@@ -33,6 +33,14 @@ that follows it (runner.py:347-381, :265-274) - a repack of the weights from the
     step = GraphedTrainStep(nerf, hparams, n_rays=4096, device=dev, optimizer=opt)
     loss, psnr, depth_variance = step.step(rays, rgbs, image_indices)   # device tensors, reused by the next step
     sched.step()
+
+With a background (NeRF++) network the step is the recording render of `render_rays_train(..., bg_nerf=...)`: the ray split
+runs on the device, so one graph serves every batch whatever its split, and the sphere bound check becomes a status word that
+`check()` reads.  The optimizer holds both networks' parameters.
+
+    step = GraphedTrainStep(nerf, hparams, 4096, dev, opt, bg_nerf=bg, sphere_center=c, sphere_radius=r)
+    step.step(rays, rgbs, image_indices)
+    step.check()                            # raises the reference's Exception if a replayed camera was outside the ellipsoid
 """
 from argparse import Namespace
 from typing import Dict, Optional
@@ -44,7 +52,8 @@ import torch.nn.functional as F
 
 from . import _cabi as K
 from .modules import Cascade, MegaNeRF, NeRF
-from .render import _check_train, _refuse_bg_ep, _render_train, _unwrap, render_rays, render_rays_fused
+from .render import (_check_train, _check_train_bg, _refuse_bg_ep, _render_train, _render_train_bg, _unwrap, render_rays,
+                     render_rays_fused)
 
 
 class GraphedRenderRays:
@@ -159,7 +168,8 @@ class GraphedRenderRays:
 
 class GraphedTrainStep:
     def __init__(self, nerf: nn.Module, hparams: Namespace, n_rays: int, device: torch.device, optimizer: torch.optim.Optimizer,
-                 get_depth_variance: bool = True, bg_nerf: Optional[nn.Module] = None, scaler=None, warmup: int = 2):
+                 get_depth_variance: bool = True, bg_nerf: Optional[nn.Module] = None, scaler=None, warmup: int = 2,
+                 sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None):
         """One training step of `nerf` over batches of n_rays rays as a CUDA graph.  The loss is the runner's: the MSE of rgb_fine,
         averaged with that of rgb_coarse for a Cascade (runner.py:366-379).  `optimizer` steps every parameter it holds inside
         the graph, so it must be capturable (`torch.optim.Adam(..., capturable=True)`).  A learning rate given as a Python number
@@ -167,13 +177,29 @@ class GraphedTrainStep:
         tensor, `lr=torch.tensor(5e-4, device=dev)`, which the scheduler updates in place; changing a number lr after the capture
         raises ValueError at the next step.  The graph repacks the weights from the
         parameters at the start of every replay, so parameters changed in place between steps (`load_state_dict`, a manual
-        edit) are what the next step trains.  Refused (ValueError): a background network (its ray split needs a host-side
-        count to draw the reference's random numbers), a network under expert parallelism or wrapped in
-        DistributedDataParallel, an optimizer that is not capturable, a GradScaler (tc_f16 scales its gradients inside the
+        edit) are what the next step trains.
+
+        bg_nerf / sphere_center / sphere_radius: a background network trained in the same step (both are repacked at every
+        replay).  The reference shapes the background pass's random draws by the number of rays that reach the background, a
+        count only the host knows; a replay reads nothing back, so the graph draws fixed-shape blocks instead - jitter
+        [n_rays, coarse_samples/2], resampling draws [n_rays, fine_samples/2] and density noise for every background query of
+        all n_rays rays - and background ray i uses row i.  These are the reference's distributions but not its numbers (the
+        eager render_rays_train draws the reference's stream).  A batch with no background ray gives the background parameters
+        an exactly zero gradient, and the capturable optimizer still steps them from its moments; the reference without DDP
+        leaves them untouched (with DDP its dummy ray has them stepped too).  A camera outside the ellipsoid is reported by
+        check(), not by step(), which reads nothing back.
+
+        Refused (ValueError): a background network without sphere_center / sphere_radius, under expert parallelism, wrapped in
+        DistributedDataParallel or of another kind than hparams.use_cascade says; a network under expert parallelism or wrapped
+        in DistributedDataParallel, an optimizer that is not capturable, a GradScaler (tc_f16 scales its gradients inside the
         library, and `scaler.step` synchronises)."""
         if bg_nerf is not None:
-            raise ValueError('GraphedTrainStep trains a foreground network only: its background ray split needs a host-side '
-                             'count (use render_rays)')
+            if sphere_center is None or sphere_radius is None:
+                raise ValueError('GraphedTrainStep: a background network needs sphere_center and sphere_radius')
+            if _unwrap(bg_nerf) is not bg_nerf or not isinstance(bg_nerf, (NeRF, MegaNeRF, Cascade)):
+                raise ValueError('GraphedTrainStep needs a mega_nerf_b200 background network itself, not a wrapper such as '
+                                 'DistributedDataParallel (its gradient hooks run on the host)')
+            _check_train_bg(nerf, bg_nerf, hparams, sphere_center, sphere_radius, 'GraphedTrainStep')
         if scaler is not None:
             raise ValueError('GraphedTrainStep takes no GradScaler: scaler.step synchronises with the host')
         if _unwrap(nerf) is not nerf or not isinstance(nerf, (NeRF, MegaNeRF, Cascade)):
@@ -190,22 +216,35 @@ class GraphedTrainStep:
         self.get_depth_variance = get_depth_variance
         self.warmup = warmup
         self.native = nerf._native()
+        self.bg_nerf = bg_nerf
+        self.bnative = bg_nerf._native() if bg_nerf is not None else None
+        self.center = sphere_center.to(self.device).float().contiguous() if bg_nerf is not None else None
+        self.radius = sphere_radius.to(self.device).float().contiguous() if bg_nerf is not None else None
         self.rays = torch.zeros(n_rays, 8, device=self.device, dtype=torch.float32)
         self.rgbs = torch.zeros(n_rays, 3, device=self.device, dtype=torch.float32)
-        with_indices = self.native.subs[0].appearance_dim > 0          # the network reads image indices
+        with_indices = any(nat.subs[0].appearance_dim > 0 for nat in self._natives())      # a network reads image indices
         self.indices = torch.zeros(n_rays, device=self.device, dtype=torch.float32) if with_indices else None
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.loss = self.psnr = self.depth_variance = None
         self._captured_lrs = []
 
+    def _natives(self):
+        return [nat for nat in (self.native, self.bnative) if nat is not None]
+
     def _run(self, repack: bool = True):
         """The step: repack (or, outside the graph, the host-side sync), render, loss (runner.py:366-379), backward, optimizer
         step.  -> (loss, psnr, depth variance)."""
-        if repack:
-            self.native.repack(self.device)
+        for nat in self._natives():
+            if repack:
+                nat.repack(self.device)
+            else:
+                nat.sync(self.device)
+        if self.bg_nerf is None:
+            res = _render_train(self.nerf, self.native, self.rays, self.indices, self.hparams, False, self.get_depth_variance)
         else:
-            self.native.sync(self.device)
-        res = _render_train(self.nerf, self.native, self.rays, self.indices, self.hparams, False, self.get_depth_variance)
+            res = _render_train_bg(self.nerf, self.native, self.bg_nerf, self.bnative, self.rays, self.indices, self.hparams,
+                                   self.center, self.radius, False, self.get_depth_variance, False, by_ray=True,
+                                   check_status=False)
         rgb = res['rgb_fine']
         with torch.no_grad():
             psnr = -10 * torch.log10(torch.mean((rgb - self.rgbs) ** 2))     # metrics.py:8-10, without the host read
@@ -247,6 +286,7 @@ class GraphedTrainStep:
                 self._run(repack=False)
         cur.wait_stream(side)
         torch.cuda.synchronize(dev)
+        self.check()
         # The warm-up steps leave the state the capture needs (the optimizer's, allocated by its first step) but must not count
         # as training: the parameters and the existing state go back to their values, state the warm-up created to the zeros a
         # fresh Adam starts from, the generator to where it was.
@@ -259,8 +299,9 @@ class GraphedTrainStep:
                         v.copy_(saved_state[p][k]) if p in saved_state and k in saved_state[p] else v.zero_()
         torch.cuda.set_rng_state(rng, dev)
         self.optimizer.zero_grad(set_to_none=True)
-        self.native.bind(dev)
-        self.native.repack(dev)            # the restored weights, and the repack's first launch outside the capture
+        for nat in self._natives():
+            nat.bind(dev)
+            nat.repack(dev)                # the restored weights, and the repack's first launch outside the capture
         torch.cuda.synchronize(dev)
         # a Python-number lr is a constant of the captured optimizer kernels (a tensor lr is read at every replay)
         self._captured_lrs = [None if torch.is_tensor(g['lr']) else g['lr'] for g in self.optimizer.param_groups]
@@ -282,5 +323,13 @@ class GraphedTrainStep:
         self._load(rays, rgbs, image_indices)
         self.graph.replay()
         # the replay updated the parameters without bumping their version counters: the next eager call re-packs
-        self.native.invalidate()
+        for nat in self._natives():
+            nat.invalidate()
         return self.loss, self.psnr, self.depth_variance
+
+    def check(self) -> None:
+        """With a background network: raise the reference's sphere-bound `Exception` if a camera of any replay since the last
+        check was outside the ellipsoid (those steps trained on undefined colours of its rays).  Synchronises with the device."""
+        if self.bg_nerf is not None:
+            h = K.ctx(self.device)
+            K.check(K.lib().mn_check_status(h, K.stream_of(self.device)), h)

@@ -533,25 +533,129 @@ def _check_train(net: nn.Module, hparams: Namespace, fn: str) -> None:
 
 
 def render_rays_train(nerf: nn.Module, rays: torch.Tensor, image_indices: Optional[torch.Tensor], hparams: Namespace,
-                      get_depth: bool, get_depth_variance: bool) -> Dict[str, torch.Tensor]:
-    """The training path of `render_rays(nerf, None, ...)` (runner.py:347-358, a foreground network in train mode) as ONE library
-    call (`mn_render_rays_train`) whose backward is one library call too (`mn_render_rays_train_backward`): the same kernels in
-    the same order, sequenced in C, at the arithmetic of `set_train_precision`.  It draws its random numbers with the calls
-    render_rays makes, in its order - the jitter, the coarse density noise, the resampling draws, the fine density noise - so
-    for the same generator state it returns the same keys and values as `render_rays(...)[0]`.  The returned colours carry one
-    autograd node; its backward accumulates every parameter's gradient as a view of one gradient block, as the stage path does.
-    Not for a background network, an expert-parallel network, a DistributedDataParallel wrapper or fine_samples == 0 (use
-    render_rays)."""
-    if _unwrap(nerf) is not nerf:
+                      get_depth: bool, get_depth_variance: bool, bg_nerf: Optional[nn.Module] = None,
+                      sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None,
+                      get_bg_fg_rgb: bool = False) -> Dict[str, torch.Tensor]:
+    """The training path of `render_rays(nerf, bg_nerf, ...)` (runner.py:347-358, networks in train mode) as ONE library call
+    (`mn_render_rays_train`, or `mn_render_rays_train_bg` with a background network) whose backward is one library call too: the
+    same kernels in the same order, sequenced in C, at the arithmetic of `set_train_precision`.  It draws its random numbers with
+    the calls render_rays makes, in its order - for the background network (which draws first) its jitter, coarse density noise,
+    resampling draws and fine density noise over the rays that reach the background, then the same four for the foreground - so
+    for the same generator state it returns the same keys and values as `render_rays(...)[0]`.  The returned rgb_fine (and
+    rgb_coarse for a Cascade) carry one autograd node; its backward accumulates every parameter's gradient as a view of one
+    gradient block per network, as the stage path does.  The other results (depth, variance, bg_lambda, the fg_ / bg_ terms of
+    get_bg_fg_rgb) carry no gradient.
+
+    With a background network the call reads back, once, the number of rays that reach the background - where the reference does
+    (rendering.py:37) - because the shapes of its draws depend on it.  With no such ray the background parameters get no gradient,
+    as on the stage path; under distributed training ('RANK' set) the draws of the reference's dummy background ray are consumed
+    too, and the background parameters get a zero gradient, as its dummy ray gives them.  A camera outside the ellipsoid raises
+    the reference's `Exception`.  Not for an expert-parallel network, a DistributedDataParallel wrapper, a background network
+    without sphere_center / sphere_radius, or fine_samples == 0 (use render_rays)."""
+    if _unwrap(nerf) is not nerf or (bg_nerf is not None and _unwrap(bg_nerf) is not bg_nerf):
         # the library's one call never runs the wrapper's forward, so DistributedDataParallel's reducer would not arm and every
         # rank would keep its own gradients
         raise ValueError('render_rays_train needs a mega_nerf_b200 network itself, not a wrapper such as DistributedDataParallel: '
                          'use render_rays, which queries through the wrapper')
-    net, _ = _nets(nerf, None, 'render_rays_train')
+    net, bg = _nets(nerf, bg_nerf, 'render_rays_train')
     _check_train(net, hparams, 'render_rays_train')
     native = net._native()
     native.sync(rays.device)
-    return _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance)
+    if bg is None:
+        return _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance)
+    _check_train_bg(net, bg, hparams, sphere_center, sphere_radius, 'render_rays_train')
+    bnative = bg._native()
+    bnative.sync(rays.device)
+    return _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sphere_center, sphere_radius, get_depth,
+                            get_depth_variance, get_bg_fg_rgb, by_ray=False)
+
+
+def _check_train_bg(net: nn.Module, bg: nn.Module, hparams: Namespace, center, radius, fn: str) -> None:
+    _refuse_bg_ep(bg, fn)
+    if not bg.training:
+        raise ValueError(f'{fn} is the training path; call bg_nerf.train() first')
+    if isinstance(bg, Cascade) != isinstance(net, Cascade) or bool(hparams.use_cascade) != isinstance(bg, Cascade):
+        raise ValueError('hparams.use_cascade does not match the background network')
+    if center is None or radius is None:
+        raise ValueError(f'{fn}: a background network needs sphere_center and sphere_radius')
+
+
+def _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sphere_center, sphere_radius, get_depth,
+                     get_depth_variance, get_bg_fg_rgb, by_ray: bool, check_status: bool = True) -> Dict[str, torch.Tensor]:
+    """render_rays_train with a background network, on weights already packed.  by_ray=False: the reference's random stream (the
+    background draws shaped by the background ray count, read back here); by_ray=True: fixed-shape background draws, row i for ray
+    i (GraphedTrainStep, which can read nothing back).  check_status=False leaves the sphere check to the caller."""
+    dev = rays.device
+    rays = K.f32c(rays.detach())
+    N = rays.shape[0]
+    idx = K.f32c(image_indices.to(dev)).view(-1) if image_indices is not None else None
+    center, radius = K.f32c(sphere_center.to(dev)), K.f32c(sphere_radius.to(dev))
+    Sc, Sf = hparams.coarse_samples, hparams.fine_samples
+    Sb, Fb = Sc // 2, Sf // 2
+    cascade = bool(hparams.use_cascade)
+    Sq, Sqb = (Sc + Sf, Sb + Fb) if cascade else (Sf, Fb)
+    perturb = hparams.perturb
+    real = getattr(hparams, 'container_path', None) is not None or getattr(hparams, 'train_mega_nerf', None) is not None
+    c2d = real and getattr(net, 'cluster_dim_start', 0) == 1                          # render.py:319
+    new = lambda *shape: torch.zeros(*shape, device=dev, dtype=torch.float32)
+
+    def bg_draws(n):
+        """The background pass's draws over n rows, in render_rays' order (render.py `bg_pass`, `_two_pass`)."""
+        jit = torch.rand(n, Sb, device=dev) if perturb > 0 else None
+        nc = _density_noise(hparams, n * Sb, dev)
+        u = torch.rand(n, Fb, device=dev) if perturb > 0 else torch.linspace(0, 1, Fb, device=dev).expand(n, Fb).contiguous()
+        nf = _density_noise(hparams, n * Sqb, dev)
+        return jit, nc, u, nf
+
+    bg_grads = True
+    if by_ray:
+        jit_b, nc_b, u_b, nf_b = bg_draws(N)
+    else:
+        # the reference's host sync (rendering.py:37, render.py:330), after its sphere check (rendering.py:412-414)
+        sg = _Stage(dev)
+        fg_far = torch.maximum(sg.intersect_sphere(rays, center, radius), rays[:, 6])
+        n_bg = int((rays[:, 7] > fg_far).sum())
+        if n_bg > 0:
+            jit_b, nc_b, u_b, nf_b = bg_draws(n_bg)
+        else:
+            # nothing drawn and nothing read: placeholders for the pointers the call checks
+            jit_b, nc_b, u_b, nf_b = new(1, Sb) if perturb > 0 else None, None, new(1, Fb), None
+            bg_grads = False
+    steps = torch.linspace(0, 1, Sc, device=dev)
+    steps_bg = torch.linspace(0, 1, Sb, device=dev)
+    jitter = torch.rand(N, Sc, device=dev) if perturb > 0 else None
+    noise_c = _density_noise(hparams, N * Sc, dev)
+    u = torch.rand(N, Sf, device=dev) if perturb > 0 else torch.linspace(0, 1, Sf, device=dev).expand(N, Sf).contiguous()
+    noise_f = _density_noise(hparams, N * Sq, dev)
+    if not by_ray and not bg_grads and 'RANK' in os.environ:
+        # the draws of the reference's dummy background ray (render.py:381-393), whose zero colour gives the background
+        # parameters a zero gradient
+        bg_draws(1)
+        bg_grads = True
+    sh_deg = hparams.sh_deg if (hparams.pos_dir_dim == 0 and hparams.sh_deg is not None) else -1
+    call = AG.RenderTrainBgCall(native, bnative, rays, idx, center, radius, real, c2d, steps, steps_bg, jitter, jit_b, float(perturb),
+                                noise_c, nc_b, u, u_b, noise_f, nf_b, Sc, Sf, cascade, sh_deg, by_ray, get_depth, get_depth_variance,
+                                get_bg_fg_rgb, bg_grads)
+    o = AG.render_train_bg_apply(call)
+    if check_status:
+        h = K.ctx(dev)
+        K.check(K.lib().mn_check_status(h, K.stream_of(dev)), h)
+    # render_rays' keys in its order (_two_pass, then the blend's fg_ / bg_ terms)
+    res: Dict[str, torch.Tensor] = {}
+    if cascade:
+        res['bg_lambda_coarse'] = o['bg_lambda_coarse']
+        res['rgb_coarse'] = o['rgb_coarse']
+    res['rgb_fine'] = o['rgb']
+    res['bg_lambda_fine'] = o['bg_lambda']
+    if get_depth:
+        res['depth_fine'] = o['depth']
+    if get_depth_variance:
+        res['depth_variance_fine'] = o['depth_var']
+    if get_bg_fg_rgb:
+        for name, field in (('rgb_fine', 'rgb'), ('depth_fine', 'depth'), ('rgb_coarse', 'rgb_coarse')):
+            if name in res:
+                res[f'fg_{name}'], res[f'bg_{name}'] = o[f'fg_{field}'], o[f'bg_{field}']
+    return res
 
 
 def _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance) -> Dict[str, torch.Tensor]:
