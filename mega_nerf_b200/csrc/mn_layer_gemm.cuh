@@ -17,9 +17,9 @@
 //                                  once and from L2 for the other N blocks.
 //     warpgroup 2     one thread streams K-slabs of A (the tile image, [K/8][128][8]) and of B (the N block of the weight
 //                     image, [N/256][K/8][256][8]) with 1-D cp.async.bulk copies into an mbarrier ring
-//     warpgroups 0-1  rows 0-63 / 64-127: wgmma m64n256k16, fp32 accumulators in registers; epilogue straight from the
-//                     registers: bias, ReLU (none for xyz_encoding_final), fp16, stored to the output tile image in HBM
-//                     (a quad of lanes writes one row's 16 bytes).
+//     warpgroups 0-1  rows 0-63 / 64-127: wgmma m64n256k16, fp32 accumulators in registers that start at the bias;
+//                     epilogue straight from the registers: ReLU (none for xyz_encoding_final), fp16, stored to the output
+//                     tile image in HBM (a quad of lanes writes one row's 16 bytes).
 //     kSplit (tc_f16x3): each stage carries hi and lo planes of both operands; three MMAs per K step (hi*hi + hi*lo + lo*hi),
 //     and the epilogue stores the fp16 residual of every activation in the output's lo plane.
 //   tc_layer_head_kernel   one thread per tile row, CUDA cores, fp32: sigma = the last trunk activations . sigma_w + bias
@@ -152,12 +152,19 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_layer_gemm_kernel(const L
             const int64_t lt = it / A.n_blk;
             const int nb = (int)(it - lt * A.n_blk);
             const int sub = A.m.sub_of_tile(A.tile0 + lt);
+            // kDgrad: sigma weights (last trunk layer) or nothing at bias_off
+            const float* bias = reinterpret_cast<const float*>(A.wpack + (size_t)sub * A.sub_bytes + A.f32_off) + A.bias_off + nb * kLgBlock;
+            // the forward's accumulators start at the bias (wgmma computes D = A B + D), so its epilogue has no bias to add;
+            // rows ra and ra + 8 take column c's bias: acc[4 j .. 4 j + 3] = (ra, c), (ra, c + 1), (ra + 8, c), (ra + 8, c + 1)
             float acc[128];
 #pragma unroll
-            for (int i = 0; i < 128; ++i) acc[i] = 0.0f;
+            for (int j = 0; j < 32; ++j) {
+                const float2 bv = kDgrad ? make_float2(0.0f, 0.0f) : __ldg(reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4));
+                acc[4 * j] = bv.x; acc[4 * j + 1] = bv.y; acc[4 * j + 2] = bv.x; acc[4 * j + 3] = bv.y;
+            }
             wg_fence_operand<128>(acc);
             int prev = -1;
-            uint32_t accum = 0;
+            uint32_t accum = kDgrad ? 0u : 1u;
             lg_walk(A, lt, nullptr, S::slab, [&](int kc, int, const unsigned char*, const unsigned char*) {
                 mbar_wait(&full[stage], phase);
                 const uint32_t sa = smem_s + (uint32_t)(stage * S::stage_bytes);
@@ -188,8 +195,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_layer_gemm_kernel(const L
             wg_fence_operand<128>(acc);
             if (prev >= 0 && t == 0) mbar_arrive(&empty[prev]);
 
-            // epilogue: bias, activation, fp16 [+ residual] -> output tile image in HBM
-            const float* bias = reinterpret_cast<const float*>(A.wpack + (size_t)sub * A.sub_bytes + A.f32_off) + A.bias_off + nb * kLgBlock;
+            // epilogue: activation, fp16 [+ residual] -> output tile image in HBM
             const size_t po = (size_t)nb * (kLgBlock / 8) * (kTileM * 16) + (size_t)ra * 16 + q4 * 4;
             unsigned char* o = A.out + lt * A.out_tile_bytes + po;
             if constexpr (kDgrad) {
@@ -201,7 +207,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_layer_gemm_kernel(const L
                     dsa = A.dsig[lt * A.dsig_tile_floats + ra] * S;
                     dsb = A.dsig[lt * A.dsig_tile_floats + ra + 8] * S;
                 }
-                // the mask and sigma-weight loads of JB column groups are issued together, as the forward's bias loads
+                // the mask and sigma-weight loads of JB column groups are issued together
                 constexpr int JB = 8;
 #pragma unroll
                 for (int j0 = 0; j0 < 32; j0 += JB) {
@@ -239,29 +245,20 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_layer_gemm_kernel(const L
                 }
                 continue;
             }
-            constexpr int JB = 8;                // column groups whose bias loads are issued together
 #pragma unroll
-            for (int j0 = 0; j0 < 32; j0 += JB) {
-                float2 bv[JB];
-#pragma unroll
-                for (int jj = 0; jj < JB; ++jj) bv[jj] = __ldg(reinterpret_cast<const float2*>(bias + 8 * (j0 + jj) + 2 * q4));
-#pragma unroll
-                for (int jj = 0; jj < JB; ++jj) {
-                    const int j = j0 + jj;
-                    if (nb * kLgBlock + 8 * j >= A.n_out) continue;
-                    float a0 = acc[4 * j] + bv[jj].x, a1 = acc[4 * j + 1] + bv[jj].y;
-                    float b0 = acc[4 * j + 2] + bv[jj].x, b1 = acc[4 * j + 3] + bv[jj].y;
-                    if (A.relu) { a0 = fmaxf(a0, 0.0f); a1 = fmaxf(a1, 0.0f); b0 = fmaxf(b0, 0.0f); b1 = fmaxf(b1, 0.0f); }
-                    const uint32_t ha = pack_h2(a0, a1), hb = pack_h2(b0, b1);
-                    unsigned char* p = o + (size_t)j * (kTileM * 16);
-                    *reinterpret_cast<uint32_t*>(p) = ha;
-                    *reinterpret_cast<uint32_t*>(p + 128) = hb;
-                    if (kSplit) {
-                        const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(&ha));
-                        const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(&hb));
-                        *reinterpret_cast<uint32_t*>(p + A.out_lo) = pack_h2(a0 - fa.x, a1 - fa.y);
-                        *reinterpret_cast<uint32_t*>(p + A.out_lo + 128) = pack_h2(b0 - fb.x, b1 - fb.y);
-                    }
+            for (int j = 0; j < 32; ++j) {
+                if (nb * kLgBlock + 8 * j >= A.n_out) continue;
+                float a0 = acc[4 * j], a1 = acc[4 * j + 1], b0 = acc[4 * j + 2], b1 = acc[4 * j + 3];
+                if (A.relu) { a0 = fmaxf(a0, 0.0f); a1 = fmaxf(a1, 0.0f); b0 = fmaxf(b0, 0.0f); b1 = fmaxf(b1, 0.0f); }
+                const uint32_t ha = pack_h2(a0, a1), hb = pack_h2(b0, b1);
+                unsigned char* p = o + (size_t)j * (kTileM * 16);
+                *reinterpret_cast<uint32_t*>(p) = ha;
+                *reinterpret_cast<uint32_t*>(p + 128) = hb;
+                if (kSplit) {
+                    const float2 fa = __half22float2(*reinterpret_cast<const __half2*>(&ha));
+                    const float2 fb = __half22float2(*reinterpret_cast<const __half2*>(&hb));
+                    *reinterpret_cast<uint32_t*>(p + A.out_lo) = pack_h2(a0 - fa.x, a1 - fa.y);
+                    *reinterpret_cast<uint32_t*>(p + A.out_lo + 128) = pack_h2(b0 - fb.x, b1 - fb.y);
                 }
             }
         }

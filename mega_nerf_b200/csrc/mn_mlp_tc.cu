@@ -218,7 +218,8 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 
 // rgb head epilogue shared by the tensor-core kernels (nerf.py:152-160): bias, optional per-image affine appearance
 // transform (3x4 matrix = affine(embedding_a[idx]), nerf.py:156-158), sigmoid when rgb_dim == 3, blend weight.
-// v = the row's raw fp32 accumulators of the rgb GEMM, kR >= rgb_dim of them.
+// v = the row's raw fp32 accumulators of the rgb Linear, kR >= rgb_dim of them; bias = NULL when they include the bias
+// (the fused kernel's rgb GEMM starts its accumulators at it).
 template <int kR = MN_TC_RGB_MAX>
 __device__ __forceinline__ void tc_emit_rgb(const MlpArgs& m, int sub, int64_t row, int64_t slot, const uint32_t* v,
                                             const float* bias, float sigma, float* tape_rgb = nullptr) {
@@ -239,7 +240,8 @@ __device__ __forceinline__ void tc_emit_rgb(const MlpArgs& m, int sub, int64_t r
 #pragma unroll
             for (int q = 0; q < 12; ++q) T[q] = fmaf(e, aw[j * 12 + q], T[q]);
         }
-        const float r0 = __uint_as_float(v[0]) + bias[0], r1 = __uint_as_float(v[1]) + bias[1], r2 = __uint_as_float(v[2]) + bias[2];
+        float r0 = __uint_as_float(v[0]), r1 = __uint_as_float(v[1]), r2 = __uint_as_float(v[2]);
+        if (bias) { r0 = r0 + bias[0]; r1 = r1 + bias[1]; r2 = r2 + bias[2]; }
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
             const float x = mn_sigmoid(fmaf(T[c * 4 + 2], r2, fmaf(T[c * 4 + 1], r1, T[c * 4 + 0] * r0)) + T[c * 4 + 3]);
@@ -249,7 +251,8 @@ __device__ __forceinline__ void tc_emit_rgb(const MlpArgs& m, int sub, int64_t r
 #pragma unroll
         for (int c = 0; c < kR; ++c) {
             if (c < nd.rgb_dim) {
-                float x = __uint_as_float(v[c]) + bias[c];
+                float x = __uint_as_float(v[c]);
+                if (bias) x = x + bias[c];
                 if (nd.rgb_dim == 3) x = mn_sigmoid(x);
                 if (tape_rgb && c < 3) tape_rgb[c * kTileM] = x;      // training forward: colour before the blend weight
                 m.out[o + c] = m.slot_w ? x * w : x;

@@ -6,9 +6,10 @@
 //     warpgroup 2     one thread streams the weight K-slabs of every GEMM (cp.async.bulk into an mbarrier ring) and the
 //                     feature-tile segments (positional encodings, direction + appearance) into their own buffer
 //     warpgroups 0-1  rows 0-63 / 64-127 of the tile: wgmma.mma_async m64nNk16 with A = the tile's fp16 activations (or the
-//                     feature segment) in shared memory and B = the ring stage, fp32 accumulators in registers; then the
-//                     epilogue straight from the registers: bias / ReLU -> fp16 -> the next layer's A operand, written IN
-//                     PLACE (every MMA that read the old activations has completed), sigma and rgb heads -> HBM.
+//                     feature segment) in shared memory and B = the ring stage, fp32 accumulators in registers that start at
+//                     the bias (PP_DGRAD: at 0); then the epilogue straight from the registers: ReLU -> fp16 -> the next
+//                     layer's A operand, written IN PLACE (every MMA that read the old activations has completed), sigma and
+//                     rgb heads -> HBM.
 //   kMode == PP_INFER up to 256 wide without kSplit (wg_reg_act): each warpgroup keeps its activations in registers instead,
 //   the A operand of the register form of wgmma, and the epilogue packs the accumulators straight into them.
 //   The two consumer warpgroups share the weight stream (a ring stage is released when both have read it) and never touch
@@ -329,8 +330,6 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
     uint64_t* xa_full = bars + 2 * kWgRingMax;
     uint64_t* xa_empty = xa_full + 1;
 
-    const int64_t n_slots = A.m.n_slots();
-    const int64_t n_tiles = (n_slots + kTileM - 1) / kTileM;
     const int n_gemm = A.m.sigma_only ? P.n_trunk : P.n_gemm;
     constexpr int npass = kSplit ? 3 : 1;
 
@@ -347,6 +346,8 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
         // =========================== producer ===========================
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kWgProducerRegs));
         if (threadIdx.x == 256) {
+            // the tile count is computed by each role after setmaxnreg: carried across the role split, ptxas spilled it
+            const int64_t n_tiles = (A.m.n_slots() + kTileM - 1) / kTileM;
             int stage = 0;
             uint32_t phase = 0, xphase = 0;
             const int64_t xtile_bytes = (int64_t)(P.kpe + P.kaux) * kTileM * 2;
@@ -375,6 +376,8 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
     } else {
         // =========================== consumers: MMA + epilogue ===========================
         asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kWgConsumerRegs));
+        const int64_t n_slots = A.m.n_slots();
+        const int64_t n_tiles = (n_slots + kTileM - 1) / kTileM;
         const int wg = wgi;
         const int t = threadIdx.x & 127, w = t >> 5, lane = t & 31, q4 = lane & 3;
         // accumulator fragment of m64nNk16: this thread holds rows ra, ra + 8 and, in every 8-column group j, columns 8j + 2 q4 + {0, 1}
@@ -464,12 +467,27 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                     const bool publish = !(want_sigma && A.m.sigma_only);   // nobody reads H after the last trunk layer
                     const float* sw = F32 + P.sigma_w_off;
                     float sacc_a = 0.0f, sacc_b = 0.0f;
+                    // every forward GEMM, rgb included, starts its accumulators at the bias (wgmma computes D = A B + D), so no
+                    // epilogue adds one; the data-gradient chain starts at 0.  A compile-time choice: accumulators defined by
+                    // a run-time choice of the two (zero for rgb only) make ptxas serialise the wgmma pipeline (C7515).
+                    constexpr bool biased = kMode != PP_DGRAD;
                     for (int ch = 0; ch < nch; ++ch) {
+                        if constexpr (biased) {
+                            // rows ra and rb take column c's bias: acc[4 j .. 4 j + 3] = (ra, c), (ra, c + 1), (rb, c), (rb, c + 1).
+                            // Columns past gm.n start at whatever follows the bias in shared memory; nothing reads them.
+                            const float* bias = F32 + gm.bias_off + ch * 256;
 #pragma unroll
-                        for (int i = 0; i < NM / 2; ++i) acc[i] = 0.0f;
+                            for (int j = 0; j < NM / 8; ++j) {
+                                const float2 bv = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
+                                acc[4 * j] = bv.x; acc[4 * j + 1] = bv.y; acc[4 * j + 2] = bv.x; acc[4 * j + 3] = bv.y;
+                            }
+                        } else {
+#pragma unroll
+                            for (int i = 0; i < NM / 2; ++i) acc[i] = 0.0f;
+                        }
                         wg_fence_operand<NM / 2>(acc);
                         int prev = -1;
-                        uint32_t accum = 0;
+                        uint32_t accum = biased ? 1u : 0u;
                         wg_walk_chunk(P, gi, ch, npass, slab, [&](const WgStage& st) {
                             const bool from_x = (st.flags & WS_FROM_X) != 0;
                             // lo plane of H lives right after the hi plane (split mode); the feature buffer is reloaded per pass
@@ -593,8 +611,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                             continue;
                         }
                         if (rgb) {
-                            // rgb head: the 4 lanes of a quad hold a row's 32 columns; gather them into one lane per row
-                            const float* bias = F32 + gm.bias_off;
+                            // rgb head: the 4 lanes of a quad hold a row's 32 columns (bias included); gather them into one lane per row
                             uint32_t va[32], vb[32];
 #pragma unroll
                             for (int c = 0; c < 32; ++c) {
@@ -606,14 +623,13 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                                 const int r = q4 ? rb : ra;
                                 const int64_t row = q4 ? row_b : row_a, slot = q4 ? slot_b : slot_a;
                                 float* tr = kMode == PP_TRAIN_FWD ? A.tape_f32 + (size_t)tile * MN_TC_F32_ROWS * kTileM + MN_TC_F32_RGB * kTileM + r : nullptr;
-                                if (row >= 0) tc_emit_rgb(A.m, A.m.nd.affine ? sub : 0, row, slot, q4 ? vb : va, bias, q4 ? sig_b : sig_a, tr);
+                                if (row >= 0) tc_emit_rgb(A.m, A.m.nd.affine ? sub : 0, row, slot, q4 ? vb : va, nullptr, q4 ? sig_b : sig_a, tr);
                                 else if (tr) { tr[0] = 0.5f; tr[kTileM] = 0.5f; tr[2 * kTileM] = 0.5f; }
                             }
                             continue;
                         }
                         // training forward: tape image of this GEMM's output (trunk layer gi; then F, then G)
                         unsigned char* timg = kMode == PP_TRAIN_FWD ? A.tape_act + (size_t)tile * A.act_tile_bytes + mn_tc_img_off(gi, L) : nullptr;
-                        const float* bias = F32 + gm.bias_off + cb;
                         const bool relu = gm.epi != EPI_LINEAR;
                         [[maybe_unused]] const bool hold = kWide && nch == 2 && ch == 0;
                         auto put = [&](int cc, uint32_t ha, uint32_t hb, float a0, float a1, float b0, float b1) {
@@ -641,18 +657,16 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                                 constexpr bool kHR = decltype(hr_tag)::value;
 #pragma unroll
                                 for (int j0 = 0; j0 < NM / 8; j0 += JB) {
-                                    float2 bvs[JB], svs[JB];
+                                    float2 svs[JB];
 #pragma unroll
                                     for (int jj = 0; jj < JB; ++jj) {
                                         const int c = 8 * (j0 + jj) + 2 * q4;
-                                        bvs[jj] = *reinterpret_cast<const float2*>(bias + c);
                                         svs[jj] = !kHR && want_sigma ? *reinterpret_cast<const float2*>(sw + cb + c) : make_float2(0.0f, 0.0f);
                                     }
 #pragma unroll
                                     for (int jj = 0; jj < JB; ++jj) {
                                         const int j = j0 + jj;
-                                        const float2 bv = bvs[jj];
-                                        float a0 = acc[4 * j] + bv.x, a1 = acc[4 * j + 1] + bv.y, b0 = acc[4 * j + 2] + bv.x, b1 = acc[4 * j + 3] + bv.y;
+                                        float a0 = acc[4 * j], a1 = acc[4 * j + 1], b0 = acc[4 * j + 2], b1 = acc[4 * j + 3];
                                         if (!kHR && relu) { a0 = fmaxf(a0, 0.0f); a1 = fmaxf(a1, 0.0f); b0 = fmaxf(b0, 0.0f); b1 = fmaxf(b1, 0.0f); }
                                         if (!kHR && want_sigma && cb + 8 * j < gm.n) {
                                             const float2 s = svs[jj];
@@ -672,11 +686,10 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                         }
 #pragma unroll
                         for (int j0 = 0; j0 < NM / 8; j0 += JB) {
-                        float2 bvs[JB], svs[JB];
+                        float2 svs[JB];
 #pragma unroll
                         for (int jj = 0; jj < JB; ++jj) {
                             const int c = 8 * (j0 + jj) + 2 * q4;
-                            bvs[jj] = *reinterpret_cast<const float2*>(bias + c);
                             svs[jj] = want_sigma ? *reinterpret_cast<const float2*>(sw + cb + c) : make_float2(0.0f, 0.0f);
                         }
 #pragma unroll
@@ -684,8 +697,7 @@ __global__ void __launch_bounds__(kWgmmaThreads, 1) tc_mlp_wg_kernel(const TcArg
                             const int j = j0 + jj;
                             const bool in_n = cb + 8 * j < gm.n;
                             if (!in_n) continue;
-                            const float2 bv = bvs[jj];
-                            float a0 = acc[4 * j] + bv.x, a1 = acc[4 * j + 1] + bv.y, b0 = acc[4 * j + 2] + bv.x, b1 = acc[4 * j + 3] + bv.y;
+                            float a0 = acc[4 * j], a1 = acc[4 * j + 1], b0 = acc[4 * j + 2], b1 = acc[4 * j + 3];
                             if (relu) { a0 = fmaxf(a0, 0.0f); a1 = fmaxf(a1, 0.0f); b0 = fmaxf(b0, 0.0f); b1 = fmaxf(b1, 0.0f); }
                             if (want_sigma && in_n) {
                                 const float2 s = svs[jj];
