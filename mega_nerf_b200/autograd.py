@@ -115,17 +115,30 @@ def sh_apply(sg, deg, coef, dirs, S) -> torch.Tensor:
     return _ShFn.apply(sg, deg, coef, dirs, S)
 
 
+def _grad_block(block: Optional[torch.Tensor], native, dev) -> torch.Tensor:
+    """The zeroed gradient block of `native` for a backward to accumulate into: `block` (a caller's, checked) or a new one."""
+    n = int(K.lib().mn_model_grad_floats(native.handle))
+    if block is None:
+        return torch.zeros(n, device=dev, dtype=torch.float32)
+    if block.numel() != n or block.dtype != torch.float32 or not block.is_contiguous() or block.device != dev:
+        raise ValueError(f'a gradient block of this network is {n} contiguous fp32 floats on {dev}')
+    return block.zero_()
+
+
 class RenderTrainCall:
-    """One mn_render_rays_train call: its inputs (the random draws included), then its tape until the backward consumed it."""
+    """One mn_render_rays_train call: its inputs (the random draws included), then its tape until the backward consumed it.
+    grads: None (the backward allocates the gradient block), or a caller's fp32 block of mn_model_grad_floats floats that the
+    backward zeroes and accumulates into, so that the parameters' gradients are views at a fixed address (GraphedTrainStep)."""
 
     def __init__(self, native, rays, idx, steps, jitter, perturb, noise_c, u, noise_f, Sc, Sf, cascade, sh_deg, get_depth,
-                 get_depth_variance):
+                 get_depth_variance, grads=None):
         self.native, self.rays, self.idx, self.steps, self.jitter, self.perturb = native, rays, idx, steps, jitter, perturb
         self.noise_c, self.u, self.noise_f = noise_c, u, noise_f
         self.Sc, self.Sf, self.cascade, self.sh_deg = Sc, Sf, cascade, sh_deg
         self.get_depth, self.get_depth_variance = get_depth, get_depth_variance
         # the recording kernels of set_train_precision where they cover the network (NativeModel.train_on_tensor_cores)
         self.prec = K.PREC_TC_F16 if native.train_on_tensor_cores() else K.PREC_FP32
+        self.grads = grads
         self.tape = None
 
     def _sizes(self):
@@ -153,7 +166,7 @@ class RenderTrainCall:
         L, dev = K.lib(), self.rays.device
         h = K.ctx(dev)
         N = self.rays.shape[0]
-        gbuf = torch.zeros(int(L.mn_model_grad_floats(self.native.handle)), device=dev, dtype=torch.float32)
+        gbuf = _grad_block(self.grads, self.native, dev)
         ws = torch.empty(max(int(L.mn_render_rays_train_backward_workspace_bytes(*self._sizes())), 256), device=dev,
                          dtype=torch.uint8)
         g_rgb = K.f32c(g_rgb) if g_rgb is not None else torch.zeros(N, 3, device=dev, dtype=torch.float32)
@@ -197,17 +210,19 @@ def render_train_apply(call: RenderTrainCall):
 class RenderTrainBgCall:
     """One mn_render_rays_train_bg call: its inputs (the random draws of both networks included), its outputs, then its tape until
     the backward consumed it.  bg_grads: whether the background parameters receive a gradient (eager, no background ray and no
-    dummy ray: None, as on the stage path)."""
+    dummy ray: None, as on the stage path).  grads: None, or the (foreground, background) blocks to accumulate into, as for
+    RenderTrainCall."""
 
     def __init__(self, native, bnative, rays, idx, center, radius, real, c2d, steps, steps_bg, jitter, jitter_bg, perturb, noise_c,
                  noise_c_bg, u, u_bg, noise_f, noise_f_bg, Sc, Sf, cascade, sh_deg, by_ray, get_depth, get_depth_variance,
-                 get_bg_fg_rgb, bg_grads=True):
+                 get_bg_fg_rgb, bg_grads=True, grads=None):
         self.native, self.bnative, self.rays, self.idx, self.center, self.radius = native, bnative, rays, idx, center, radius
         self.real, self.c2d, self.steps, self.steps_bg, self.perturb = real, c2d, steps, steps_bg, perturb
         self.draws = (jitter, jitter_bg, noise_c, noise_c_bg, u, u_bg, noise_f, noise_f_bg)
         self.Sc, self.Sf, self.cascade, self.sh_deg, self.by_ray = Sc, Sf, cascade, sh_deg, by_ray
         self.get_depth, self.get_depth_variance, self.get_bg_fg_rgb = get_depth, get_depth_variance, get_bg_fg_rgb
         self.bg_grads = bg_grads
+        self.grads = grads
         self.prec = K.PREC_TC_F16 if native.train_on_tensor_cores() else K.PREC_FP32
         self.bprec = K.PREC_TC_F16 if bnative.train_on_tensor_cores() else K.PREC_FP32
         self.tape = None
@@ -253,8 +268,8 @@ class RenderTrainBgCall:
         L, dev = K.lib(), self.rays.device
         h = K.ctx(dev)
         N = self.rays.shape[0]
-        gbuf = torch.zeros(int(L.mn_model_grad_floats(self.native.handle)), device=dev, dtype=torch.float32)
-        gbuf_bg = torch.zeros(int(L.mn_model_grad_floats(self.bnative.handle)), device=dev, dtype=torch.float32)
+        gbuf = _grad_block(self.grads[0] if self.grads is not None else None, self.native, dev)
+        gbuf_bg = _grad_block(self.grads[1] if self.grads is not None else None, self.bnative, dev)
         ws = torch.empty(max(int(L.mn_render_rays_train_bg_backward_workspace_bytes(*self._sizes())), 256), device=dev,
                          dtype=torch.uint8)
         g_rgb = K.f32c(g_rgb) if g_rgb is not None else torch.zeros(N, 3, device=dev, dtype=torch.float32)

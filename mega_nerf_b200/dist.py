@@ -39,6 +39,38 @@ def all_gather_rows(local: torch.Tensor, n_total: int, group=None) -> torch.Tens
     return torch.cat(pieces, 0)
 
 
+def broadcast_state(modules, group=None) -> None:
+    """DistributedDataParallel's start-up for `modules` (None entries skipped): every parameter and buffer - a MegaNeRF's
+    `centroids` included - overwritten in place by the values of the group's rank 0."""
+    src = dist.get_global_rank(group if group is not None else dist.group.WORLD, 0)
+    with torch.no_grad():
+        for m in modules:
+            if m is None:
+                continue
+            for t in list(m.parameters()) + list(m.buffers()):
+                dist.broadcast(t.detach(), src=src, group=group)
+
+
+def grad_bucket(sizes, device: torch.device) -> Tuple[torch.Tensor, list]:
+    """One zeroed fp32 allocation holding gradient blocks of the given float counts back to back, nothing between them, so that
+    one collective covers them all -> (bucket, [block views])."""
+    bucket = torch.zeros(sum(sizes), device=device, dtype=torch.float32)
+    blocks, a = [], 0
+    for n in sizes:
+        blocks.append(bucket[a:a + n])
+        a += n
+    return bucket, blocks
+
+
+def average_gradients(bucket: torch.Tensor, group=None) -> None:
+    """The mean of `bucket` over the group's ranks, in place, as DistributedDataParallel's default reduction computes it: scale
+    by the world size first, then all-reduce with SUM.  A pre-divided SUM rather than ReduceOp.AVG, which gloo does not offer:
+    one arithmetic on every backend, exact for a power-of-two world size (there DDP's multiply by 1/world gives the same bits),
+    and one elementwise pass over the bucket.  Capturable in a CUDA graph on NCCL."""
+    bucket.div_(dist.get_world_size(group))
+    dist.all_reduce(bucket, op=dist.ReduceOp.SUM, group=group)
+
+
 def render_rays_sharded(render_fn: Callable[..., Tuple[Dict[str, torch.Tensor], bool]], rays: torch.Tensor,
                         image_indices: Optional[torch.Tensor], *args, group=None, **kwargs) -> Tuple[Dict[str, torch.Tensor], bool]:
     """Every rank holds the same `rays` [N,8]; rank r renders rays[lo_r:hi_r] with `render_fn`

@@ -41,7 +41,14 @@ runs on the device, so one graph serves every batch whatever its split, and the 
     step = GraphedTrainStep(nerf, hparams, 4096, dev, opt, bg_nerf=bg, sphere_center=c, sphere_radius=r)
     step.step(rays, rgbs, image_indices)
     step.check()                            # raises the reference's Exception if a replayed camera was outside the ellipsoid
+
+Data-parallel training (one process per GPU, e.g. under torchrun, an NCCL process group): the step averages the gradients of
+both networks over the group's ranks inside the replay, with one all-reduce over one gradient bucket, as
+DistributedDataParallel would; the networks themselves are passed unwrapped.
+
+    step = GraphedTrainStep(nerf, hparams, 4096, dev, opt, process_group=dist.group.WORLD)
 """
+import gc
 from argparse import Namespace
 from typing import Dict, Optional
 
@@ -50,7 +57,10 @@ from torch import nn
 
 import torch.nn.functional as F
 
+import torch.distributed as dist
+
 from . import _cabi as K
+from . import dist as D
 from .modules import Cascade, MegaNeRF, NeRF
 from .render import (_check_train, _check_train_bg, _refuse_bg_ep, _render_train, _render_train_bg, _unwrap, render_rays,
                      render_rays_fused)
@@ -166,10 +176,25 @@ class GraphedRenderRays:
         return self.results
 
 
+def _check_group(group, device: torch.device) -> None:
+    """A process group a captured training step can average over: NCCL, with this rank on `device` - the device the group was
+    bound to (init_process_group(device_id=...)), or else the current CUDA device, which ProcessGroupNCCL takes for its rank."""
+    backend = str(dist.get_backend(group))
+    if 'nccl' not in backend:
+        raise ValueError(f'GraphedTrainStep: a CUDA graph captures NCCL collectives only; the process group is {backend!r}')
+    rank_dev = getattr(group, 'bound_device_id', None)
+    if rank_dev is None:
+        rank_dev = torch.device('cuda', torch.cuda.current_device())
+    want = device if device.index is not None else torch.device('cuda', torch.cuda.current_device())
+    if device.type != 'cuda' or rank_dev != want:
+        raise ValueError(f'GraphedTrainStep: this rank of the process group runs on {rank_dev}, the step on {device}')
+
+
 class GraphedTrainStep:
     def __init__(self, nerf: nn.Module, hparams: Namespace, n_rays: int, device: torch.device, optimizer: torch.optim.Optimizer,
                  get_depth_variance: bool = True, bg_nerf: Optional[nn.Module] = None, scaler=None, warmup: int = 2,
-                 sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None):
+                 sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None,
+                 process_group=None):
         """One training step of `nerf` over batches of n_rays rays as a CUDA graph.  The loss is the runner's: the MSE of rgb_fine,
         averaged with that of rgb_coarse for a Cascade (runner.py:366-379).  `optimizer` steps every parameter it holds inside
         the graph, so it must be capturable (`torch.optim.Adam(..., capturable=True)`).  A learning rate given as a Python number
@@ -189,10 +214,24 @@ class GraphedTrainStep:
         leaves them untouched (with DDP its dummy ray has them stepped too).  A camera outside the ellipsoid is reported by
         check(), not by step(), which reads nothing back.
 
+        process_group: None (every rank keeps its own gradients), or a torch.distributed NCCL group of one rank per GPU to train
+        data-parallel as DistributedDataParallel does.  capture() first overwrites every parameter and buffer of both networks
+        (a MegaNeRF's centroids included) with the values of the group's rank 0, as DDP's constructor does.  The backward writes
+        both networks' gradient blocks into one contiguous fp32 bucket (`self.bucket`: the foreground block, then the background
+        block), of which every `param.grad` is a view at the same address at every replay, and the replay averages the bucket over
+        the ranks between backward() and optimizer.step(): divided by the world size, then one all-reduce with ReduceOp.SUM, as
+        DDP's default reduction (`dist.average_gradients`; SUM on a pre-divided bucket rather than ReduceOp.AVG so that the same
+        arithmetic runs on every backend, and the division is exact for a power-of-two world size).  The background block is
+        averaged at every step on every rank: a rank whose batch has no background ray contributes its exactly zero gradient, so
+        no rank ever skips a collective over a count only it knows.  The reference reaches the same sum under DDP by rendering a
+        dummy background ray that it multiplies by zero (rendering.py:143-171); here the fixed-shape step needs no dummy ray.
+        loss / psnr / depth_variance and check() stay per rank.
+
         Refused (ValueError): a background network without sphere_center / sphere_radius, under expert parallelism, wrapped in
         DistributedDataParallel or of another kind than hparams.use_cascade says; a network under expert parallelism or wrapped
         in DistributedDataParallel, an optimizer that is not capturable, a GradScaler (tc_f16 scales its gradients inside the
-        library, and `scaler.step` synchronises)."""
+        library, and `scaler.step` synchronises), a process group that is not NCCL (a CUDA graph captures NCCL collectives
+        only) or whose rank's device is not `device`."""
         if bg_nerf is not None:
             if sphere_center is None or sphere_radius is None:
                 raise ValueError('GraphedTrainStep: a background network needs sphere_center and sphere_radius')
@@ -211,7 +250,12 @@ class GraphedTrainStep:
         if not all(g.get('capturable', False) for g in optimizer.param_groups):
             raise ValueError('GraphedTrainStep needs a capturable optimizer, e.g. torch.optim.Adam(..., capturable=True)')
         _check_train(nerf, hparams, 'GraphedTrainStep')
+        if process_group is not None:
+            _check_group(process_group, torch.device(device))
         self.nerf, self.hparams, self.optimizer = nerf, hparams, optimizer
+        self.process_group = process_group
+        self.bucket: Optional[torch.Tensor] = None
+        self._grads = None                     # the gradient block(s) the backward writes into, views of the bucket
         self.device = torch.device(device)
         self.get_depth_variance = get_depth_variance
         self.warmup = warmup
@@ -240,11 +284,12 @@ class GraphedTrainStep:
             else:
                 nat.sync(self.device)
         if self.bg_nerf is None:
-            res = _render_train(self.nerf, self.native, self.rays, self.indices, self.hparams, False, self.get_depth_variance)
+            res = _render_train(self.nerf, self.native, self.rays, self.indices, self.hparams, False, self.get_depth_variance,
+                                self._grads)
         else:
             res = _render_train_bg(self.nerf, self.native, self.bg_nerf, self.bnative, self.rays, self.indices, self.hparams,
                                    self.center, self.radius, False, self.get_depth_variance, False, by_ray=True,
-                                   check_status=False)
+                                   check_status=False, grads=self._grads)
         rgb = res['rgb_fine']
         with torch.no_grad():
             psnr = -10 * torch.log10(torch.mean((rgb - self.rgbs) ** 2))     # metrics.py:8-10, without the host read
@@ -253,6 +298,8 @@ class GraphedTrainStep:
         if self.hparams.use_cascade:
             loss = (loss + F.mse_loss(res['rgb_coarse'], self.rgbs, reduction='mean')) / 2
         loss.backward()
+        if self.process_group is not None:
+            D.average_gradients(self.bucket, self.process_group)
         self.optimizer.step()
         return loss.detach(), psnr, dv
 
@@ -269,9 +316,18 @@ class GraphedTrainStep:
         """Warm up on a side stream (tape sizes, first launches, the optimizer's state, and on the tensor cores the transposed
         weight images of the backward), restore the parameters, the optimizer state and the random generator as they were, bind
         the weights - after the warm-up, so that the repack covers every image the captured step reads - then record the graph.
-        The capture itself trains nothing: the first replay is the first step."""
+        The capture itself trains nothing: the first replay is the first step.  With a process group, the parameters and buffers
+        are first broadcast from the group's rank 0 and the gradient bucket is allocated."""
         dev = self.device
         self._load(rays, rgbs, image_indices)
+        if self.process_group is not None:
+            D.broadcast_state([self.nerf, self.bg_nerf], self.process_group)
+            L = K.lib()
+            for nat in self._natives():
+                nat.invalidate()           # written through NCCL: re-pack at the next sync
+                nat.sync(dev)
+            self.bucket, blocks = D.grad_bucket([int(L.mn_model_grad_floats(nat.handle)) for nat in self._natives()], dev)
+            self._grads = blocks[0] if self.bg_nerf is None else tuple(blocks)
         params = [p for group in self.optimizer.param_groups for p in group['params']]
         saved_params = [p.detach().clone() for p in params]
         saved_state = {p: {k: v.clone() for k, v in self.optimizer.state[p].items() if torch.is_tensor(v)} for p in params
@@ -306,6 +362,9 @@ class GraphedTrainStep:
         # a Python-number lr is a constant of the captured optimizer kernels (a tensor lr is read at every replay)
         self._captured_lrs = [None if torch.is_tensor(g['lr']) else g['lr'] for g in self.optimizer.param_groups]
         self.graph = torch.cuda.CUDAGraph()
+        # a network that died in a reference cycle would otherwise be collected inside the capture, whose model handle's cudaFree
+        # invalidates it
+        gc.collect()
         # thread_local: other threads of the process (e.g. the NCCL watchdog polling its events) must not invalidate the capture
         with torch.cuda.graph(self.graph, capture_error_mode='thread_local'):
             self.loss, self.psnr, self.depth_variance = self._run()

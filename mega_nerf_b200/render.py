@@ -581,10 +581,12 @@ def _check_train_bg(net: nn.Module, bg: nn.Module, hparams: Namespace, center, r
 
 
 def _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sphere_center, sphere_radius, get_depth,
-                     get_depth_variance, get_bg_fg_rgb, by_ray: bool, check_status: bool = True) -> Dict[str, torch.Tensor]:
+                     get_depth_variance, get_bg_fg_rgb, by_ray: bool, check_status: bool = True,
+                     grads=None) -> Dict[str, torch.Tensor]:
     """render_rays_train with a background network, on weights already packed.  by_ray=False: the reference's random stream (the
     background draws shaped by the background ray count, read back here); by_ray=True: fixed-shape background draws, row i for ray
-    i (GraphedTrainStep, which can read nothing back).  check_status=False leaves the sphere check to the caller."""
+    i (GraphedTrainStep, which can read nothing back).  check_status=False leaves the sphere check to the caller.  grads: None, or
+    the (foreground, background) gradient blocks the backward accumulates into (autograd.RenderTrainBgCall)."""
     dev = rays.device
     rays = K.f32c(rays.detach())
     N = rays.shape[0]
@@ -635,7 +637,7 @@ def _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sph
     sh_deg = hparams.sh_deg if (hparams.pos_dir_dim == 0 and hparams.sh_deg is not None) else -1
     call = AG.RenderTrainBgCall(native, bnative, rays, idx, center, radius, real, c2d, steps, steps_bg, jitter, jit_b, float(perturb),
                                 noise_c, nc_b, u, u_b, noise_f, nf_b, Sc, Sf, cascade, sh_deg, by_ray, get_depth, get_depth_variance,
-                                get_bg_fg_rgb, bg_grads)
+                                get_bg_fg_rgb, bg_grads, grads)
     o = AG.render_train_bg_apply(call)
     if check_status:
         h = K.ctx(dev)
@@ -658,8 +660,9 @@ def _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sph
     return res
 
 
-def _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance) -> Dict[str, torch.Tensor]:
-    """render_rays_train on weights already packed (sync, or a repack inside a captured training step)."""
+def _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance, grads=None) -> Dict[str, torch.Tensor]:
+    """render_rays_train on weights already packed (sync, or a repack inside a captured training step).  grads: None, or the
+    gradient block the backward accumulates into (autograd.RenderTrainCall)."""
     dev = rays.device
     rays = K.f32c(rays.detach())
     N = rays.shape[0]
@@ -676,7 +679,7 @@ def _render_train(net, native, rays, image_indices, hparams, get_depth, get_dept
     noise_f = _density_noise(hparams, N * Sq, dev)
     sh_deg = hparams.sh_deg if (hparams.pos_dir_dim == 0 and hparams.sh_deg is not None) else -1
     call = AG.RenderTrainCall(native, rays, idx, steps, jitter, float(perturb), noise_c, u, noise_f, Sc, Sf, cascade, sh_deg,
-                              get_depth, get_depth_variance)
+                              get_depth, get_depth_variance, grads)
     rgb, rgb_coarse, depth, var = AG.render_train_apply(call)
     res: Dict[str, torch.Tensor] = {}
     if cascade:
