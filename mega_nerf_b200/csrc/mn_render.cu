@@ -24,16 +24,44 @@ __global__ void fill_kernel(float* p, int64_t n, float v) {
 __device__ __forceinline__ float max_t(float a, float b) { return a != a ? a : (b != b ? b : (a < b ? b : a)); }
 __device__ __forceinline__ float min_t(float a, float b) { return a != a ? a : (b != b ? b : (b < a ? b : a)); }
 
-constexpr int kSplitBlock = 1024;
+// Threads per block of the split and occupancy-test kernels and of the compaction that follows each: a count per block, then a
+// stable scan over the counts of the blocks before (compact_block_scan).
+constexpr int kCompactBlock = 1024;
+
+// The stable block scan of a compaction (torch.arange(n)[mask] order) in a kCompactBlock-thread block: keep = this thread's element
+// stays, blk[b] = elements kept in block b.  Returns the element's compacted position, -1 if it is not kept; the last block writes
+// the number kept to *count (and to *count_out if given).
+__device__ __forceinline__ int compact_block_scan(const int* __restrict__ blk, bool keep, int* __restrict__ count,
+                                                  int* __restrict__ count_out) {
+    __shared__ int wsum[32], wbase[32];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    int part = 0;                                           // elements kept in the blocks before this one
+    for (unsigned b = threadIdx.x; b < blockIdx.x; b += kCompactBlock) part += blk[b];
+    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+    const unsigned bal = __ballot_sync(0xffffffffu, keep);
+    if (lane == 0) { wsum[warp] = part; wbase[warp] = __popc(bal); }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int run = 0;
+        for (int w = 0; w < kCompactBlock / 32; ++w) run += wsum[w];
+        for (int w = 0; w < kCompactBlock / 32; ++w) { const int c = wbase[w]; wbase[w] = run; run += c; }
+        if (blockIdx.x == gridDim.x - 1) {
+            *count = run;
+            if (count_out) *count_out = run;
+        }
+    }
+    __syncthreads();
+    return keep ? wbase[warp] + __popc(bal & ((1u << lane) - 1)) : -1;
+}
 
 // Background split, per ray (render.py `_render`, rendering.py:34-47): fg_far = max(sphere exit, near); the ray reaches the
 // background iff far > fg_far; its last delta (fg_far, else 1e10) and the foreground far override min(far, fg_far).  flag[i] = 1
 // for a background ray (turned into its compacted position by bg_compact_kernel); blk[b] = background rays of block b.
-__global__ void __launch_bounds__(kSplitBlock) bg_split_kernel(const float* __restrict__ rays, const float* __restrict__ center,
-                                                               const float* __restrict__ radius, int64_t N, float* __restrict__ far_ov,
-                                                               float* __restrict__ last_delta, int* __restrict__ flag,
-                                                               int* __restrict__ blk, unsigned int* status) {
-    const int64_t i = (int64_t)blockIdx.x * kSplitBlock + threadIdx.x;
+__global__ void __launch_bounds__(kCompactBlock) bg_split_kernel(const float* __restrict__ rays, const float* __restrict__ center,
+                                                                 const float* __restrict__ radius, int64_t N, float* __restrict__ far_ov,
+                                                                 float* __restrict__ last_delta, int* __restrict__ flag,
+                                                                 int* __restrict__ blk, unsigned int* status) {
+    const int64_t i = (int64_t)blockIdx.x * kCompactBlock + threadIdx.x;
     bool with_bg = false;
     if (i < N) {
         const float* r = rays + i * 8;
@@ -60,31 +88,14 @@ __global__ void __launch_bounds__(kSplitBlock) bg_split_kernel(const float* __re
 
 // Stable compaction of the background rays (torch.arange(N)[mask]): ids, directions and image indices of the compacted rays,
 // pos[i] = compacted position of ray i or -1, *count = number of background rays (written by the last block).
-__global__ void __launch_bounds__(kSplitBlock) bg_compact_kernel(const float* __restrict__ rays, const float* __restrict__ idx,
-                                                                 int64_t N, const int* __restrict__ blk, int* __restrict__ pos,
-                                                                 int64_t* __restrict__ ids, float* __restrict__ dirs,
-                                                                 float* __restrict__ cidx, int* __restrict__ count) {
-    __shared__ int wsum[32], wbase[32];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int part = 0;                                           // background rays of the blocks before this one
-    for (unsigned b = threadIdx.x; b < blockIdx.x; b += kSplitBlock) part += blk[b];
-    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-    const int64_t i = (int64_t)blockIdx.x * kSplitBlock + threadIdx.x;
-    const bool with_bg = i < N && pos[i] != 0;
-    const unsigned bal = __ballot_sync(0xffffffffu, with_bg);
-    if (lane == 0) { wsum[warp] = part; wbase[warp] = __popc(bal); }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int run = 0;
-        for (int w = 0; w < kSplitBlock / 32; ++w) run += wsum[w];
-        for (int w = 0; w < kSplitBlock / 32; ++w) { const int c = wbase[w]; wbase[w] = run; run += c; }
-        if (blockIdx.x == gridDim.x - 1) *count = run;
-    }
-    __syncthreads();
+__global__ void __launch_bounds__(kCompactBlock) bg_compact_kernel(const float* __restrict__ rays, const float* __restrict__ idx,
+                                                                   int64_t N, const int* __restrict__ blk, int* __restrict__ pos,
+                                                                   int64_t* __restrict__ ids, float* __restrict__ dirs,
+                                                                   float* __restrict__ cidx, int* __restrict__ count) {
+    const int64_t i = (int64_t)blockIdx.x * kCompactBlock + threadIdx.x;
+    const int p = compact_block_scan(blk, i < N && pos[i] != 0, count, nullptr);
     if (i >= N) return;
-    int p = -1;
-    if (with_bg) {
-        p = wbase[warp] + __popc(bal & ((1u << lane) - 1));
+    if (p >= 0) {
         ids[p] = i;
         for (int j = 0; j < 3; ++j) dirs[p * 3 + j] = rays[i * 8 + 3 + j];
         if (cidx) cidx[p] = idx[i];
@@ -111,8 +122,6 @@ __global__ void bg_blend_kernel(float* __restrict__ val, const float* __restrict
 // queried, their raw row is (0, 0, 0, 0).  The queried samples are compacted on the device like the background rays (a block
 // count, then a stable block scan over the counts of the blocks before), the model runs on them through a row gather with its
 // row count read from the device, and a scatter writes every raw row.
-constexpr int kOccBlock = 1024;
-
 struct OccGrid {
     const uint32_t* bits;   // reso^3 bits, cell (i * reso + j) * reso + k at bit c & 31 of word c >> 5
     int reso;
@@ -135,9 +144,9 @@ __device__ __forceinline__ bool occ_queried(const OccGrid& g, const float* __res
 }
 
 // flag[s] = 1 iff sample s of the [n, 3] points is queried; blk[b] = queried samples of block b.
-__global__ void __launch_bounds__(kOccBlock) occ_test_kernel(const float* __restrict__ xyz, int64_t n, OccGrid g, int* __restrict__ flag,
-                                                             int* __restrict__ blk) {
-    const int64_t s = (int64_t)blockIdx.x * kOccBlock + threadIdx.x;
+__global__ void __launch_bounds__(kCompactBlock) occ_test_kernel(const float* __restrict__ xyz, int64_t n, OccGrid g,
+                                                                 int* __restrict__ flag, int* __restrict__ blk) {
+    const int64_t s = (int64_t)blockIdx.x * kCompactBlock + threadIdx.x;
     bool q = false;
     if (s < n) {
         q = occ_queried(g, xyz + s * 3);
@@ -149,34 +158,13 @@ __global__ void __launch_bounds__(kOccBlock) occ_test_kernel(const float* __rest
 
 // Stable compaction of the queried samples: idx[0 .. count) = their flat indices in ascending order, pos[s] = the compacted row
 // of sample s or -1, *count (and *count_out if given) = the queried samples (written by the last block).
-__global__ void __launch_bounds__(kOccBlock) occ_compact_kernel(int64_t n, const int* __restrict__ blk, int* __restrict__ pos,
-                                                                int* __restrict__ idx, int* __restrict__ count, int* __restrict__ count_out) {
-    __shared__ int wsum[32], wbase[32];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    int part = 0;                                           // queried samples of the blocks before this one
-    for (unsigned b = threadIdx.x; b < blockIdx.x; b += kOccBlock) part += blk[b];
-    for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
-    const int64_t s = (int64_t)blockIdx.x * kOccBlock + threadIdx.x;
-    const bool q = s < n && pos[s] != 0;
-    const unsigned bal = __ballot_sync(0xffffffffu, q);
-    if (lane == 0) { wsum[warp] = part; wbase[warp] = __popc(bal); }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int run = 0;
-        for (int w = 0; w < kOccBlock / 32; ++w) run += wsum[w];
-        for (int w = 0; w < kOccBlock / 32; ++w) { const int c = wbase[w]; wbase[w] = run; run += c; }
-        if (blockIdx.x == gridDim.x - 1) {
-            *count = run;
-            if (count_out) *count_out = run;
-        }
-    }
-    __syncthreads();
+__global__ void __launch_bounds__(kCompactBlock) occ_compact_kernel(int64_t n, const int* __restrict__ blk, int* __restrict__ pos,
+                                                                    int* __restrict__ idx, int* __restrict__ count,
+                                                                    int* __restrict__ count_out) {
+    const int64_t s = (int64_t)blockIdx.x * kCompactBlock + threadIdx.x;
+    const int p = compact_block_scan(blk, s < n && pos[s] != 0, count, count_out);
     if (s >= n) return;
-    int p = -1;
-    if (q) {
-        p = wbase[warp] + __popc(bal & ((1u << lane) - 1));
-        idx[p] = (int)s;
-    }
+    if (p >= 0) idx[p] = (int)s;
     pos[s] = p;
 }
 
@@ -254,7 +242,7 @@ RenderPlan make_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, i
         const int64_t rows = N * (p.fg.Sq > Sc ? p.fg.Sq : Sc);
         p.occ_pos = take((size_t)rows * 4);
         p.occ_idx = take((size_t)rows * 4);
-        p.occ_blk = take((size_t)mn_cdiv(rows, kOccBlock) * 4);
+        p.occ_blk = take((size_t)mn_cdiv(rows, kCompactBlock) * 4);
         p.occ_count = take(2 * 4);
         p.occ_out = take((size_t)rows * 16);
     }
@@ -262,7 +250,7 @@ RenderPlan make_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, i
     if (bg) {
         p.far_ov = take((size_t)N * 4);
         p.pos = take((size_t)N * 4);
-        p.blk = take((size_t)mn_cdiv(N, kSplitBlock) * 4);
+        p.blk = take((size_t)mn_cdiv(N, kCompactBlock) * 4);
         p.count = take(4);
         p.ids = take((size_t)N * 8);
         p.dirs = take((size_t)N * 12);
@@ -294,6 +282,40 @@ int check_net(mn_ctx* ctx, const mn_model* m, int use_cascade, int fine_samples,
     if (!use_cascade && fine_samples == 0)
         return mn_fail(ctx, MN_ERR_INVALID, n + ": a coarse-only render composites colour only under use_cascade (rendering.py:199)");
     if (d.appearance_dim > 0 && !image_indices_d) return mn_fail(ctx, MN_ERR_INVALID, n + ": image indices are required");
+    return MN_OK;
+}
+
+// The background split and the compaction of the background rays (render.py `_render`), then the background pass's last deltas
+// (1e10: that pass has no bg_lambda).  far_ov, last_delta: the foreground's far override and last deltas; pos, blk, count, ids,
+// dirs, idx (null: no image indices): the split and the compacted rays, as bg_split_kernel / bg_compact_kernel; ld_b: the
+// background's last deltas.
+int split_bg(mn_ctx* ctx, const float* rays_d, const float* image_indices_d, int64_t N, const float* center_d, const float* radius_d,
+             float* far_ov, float* last_delta, int* pos, int* blk, int* count, int64_t* ids, float* dirs, float* idx, float* ld_b,
+             cudaStream_t st) {
+    const unsigned nblk = (unsigned)mn_cdiv(N, kCompactBlock);
+    bg_split_kernel<<<nblk, kCompactBlock, 0, st>>>(rays_d, center_d, radius_d, N, far_ov, last_delta, pos, blk, ctx->status_d);
+    MN_LAUNCH_CHECK(ctx);
+    bg_compact_kernel<<<nblk, kCompactBlock, 0, st>>>(rays_d, image_indices_d, N, blk, pos, ids, dirs, idx, count);
+    MN_LAUNCH_CHECK(ctx);
+    fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(ld_b, N, 1e10f);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
+}
+
+// The lambda blend (render.py `_render`) of o's rgb, its depth when wanted and, given lam_c, its rgb_coarse with the background
+// pass's results in bo, by bg_lambda of the final type (lam) and of the cascade's coarse type (lam_c); o's fg_* / bg_* (null:
+// not wanted) receive the two terms.
+int blend_bg(mn_ctx* ctx, const mn_render_outputs& o, const mn_render_outputs& bo, const float* lam, const float* lam_c,
+             const int* pos, int64_t N, cudaStream_t st) {
+    auto blend = [&](float* val, const float* bval, const float* l, int C, float* fg_out, float* bg_out) -> int {
+        bg_blend_kernel<<<(unsigned)mn_cdiv(N * C, 256), 256, 0, st>>>(val, bval, l, pos, N, C, fg_out, bg_out);
+        MN_LAUNCH_CHECK(ctx);
+        return MN_OK;
+    };
+    int rc;
+    if ((rc = blend(o.rgb, bo.rgb, lam, 3, o.fg_rgb, o.bg_rgb))) return rc;
+    if (o.depth && (rc = blend(o.depth, bo.depth, lam, 1, o.fg_depth, o.bg_depth))) return rc;
+    if (lam_c && o.rgb_coarse) return blend(o.rgb_coarse, bo.rgb_coarse, lam_c, 3, o.fg_rgb_coarse, o.bg_rgb_coarse);
     return MN_OK;
 }
 
@@ -363,13 +385,13 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
     auto query_occ = [&](mn_model* net, const float* xyz, int S, int coarse, float* mlp_out, float* raw_out, const float* dirs,
                          int64_t dstride, const float* idx, int pass) -> int {
         const int64_t n = N * S;
-        const unsigned nblk = (unsigned)mn_cdiv(n, kOccBlock);
+        const unsigned nblk = (unsigned)mn_cdiv(n, kCompactBlock);
         int* cnt = I(p.occ_count) + pass;
         const int* gather = I(p.occ_idx);
-        occ_test_kernel<<<nblk, kOccBlock, 0, st>>>(xyz, n, G, I(p.occ_pos), I(p.occ_blk));
+        occ_test_kernel<<<nblk, kCompactBlock, 0, st>>>(xyz, n, G, I(p.occ_pos), I(p.occ_blk));
         MN_LAUNCH_CHECK(ctx);
-        occ_compact_kernel<<<nblk, kOccBlock, 0, st>>>(n, I(p.occ_blk), I(p.occ_pos), I(p.occ_idx), cnt,
-                                                       counts_out_d ? counts_out_d + pass : nullptr);
+        occ_compact_kernel<<<nblk, kCompactBlock, 0, st>>>(n, I(p.occ_blk), I(p.occ_pos), I(p.occ_idx), cnt,
+                                                           counts_out_d ? counts_out_d + pass : nullptr);
         MN_LAUNCH_CHECK(ctx);
         mn_rows rows{};
         rows.mode = 1;
@@ -431,21 +453,16 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
                                   last_delta, N, b.flip, lr, nullptr, r.rgb, depth, r.depth_var, r.bg_lambda, st);
     };
 
+    mn_render_outputs bo{};     // the background pass's results
     if (!bg) {
         fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(F(p.last_delta), N, 1e10f);   // no background: rendering.py:33
         MN_LAUNCH_CHECK(ctx);
     } else {
         // ---- split and compaction (render.py:292-299)
-        const unsigned nblk = (unsigned)mn_cdiv(N, kSplitBlock);
-        bg_split_kernel<<<nblk, kSplitBlock, 0, st>>>(rays_d, center_d, radius_d, N, F(p.far_ov), F(p.last_delta), I(p.pos), I(p.blk),
-                                                     ctx->status_d);
-        MN_LAUNCH_CHECK(ctx);
         float* bidx = image_indices_d ? F(p.idx) : nullptr;
-        bg_compact_kernel<<<nblk, kSplitBlock, 0, st>>>(rays_d, image_indices_d, N, I(p.blk), I(p.pos),
-                                                       reinterpret_cast<int64_t*>(W + p.ids), F(p.dirs), bidx, I(p.count));
-        MN_LAUNCH_CHECK(ctx);
-        fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(F(p.ld_b), N, 1e10f);            // no bg_lambda in this pass
-        MN_LAUNCH_CHECK(ctx);
+        if ((rc = split_bg(ctx, rays_d, image_indices_d, N, center_d, radius_d, F(p.far_ov), F(p.last_delta), I(p.pos), I(p.blk),
+                           I(p.count), reinterpret_cast<int64_t*>(W + p.ids), F(p.dirs), bidx, F(p.ld_b), st)))
+            return rc;
 
         // ---- background pass over the compacted rays (render.py:300-312): coarse depths from z_steps_bg, in sample order and
         // reversed, and the points outside the sphere in reversed order
@@ -460,7 +477,6 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
         if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, nullptr, 0.0f, N, b.S, 0, lr, F(b.z_c), st))) return rc;
         if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, nullptr, 0.0f, N, b.S, 1, lr, F(b.z_c_comp), st))) return rc;
         if ((rc = outside(F(b.z_c), b.S, 1, F(b.xyz_c), F(b.dreal_c)))) return rc;
-        mn_render_outputs bo{};
         bo.rgb = F(p.rgb_b);
         bo.depth = o.depth ? F(p.depth_b) : nullptr;
         bo.rgb_coarse = F(p.rgb_cb);
@@ -480,69 +496,180 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
     if (!bg) return MN_OK;
 
     // ---- blend (render.py:320-340): the final type's rgb / depth, and rgb_coarse under cascade with fine samples
-    auto blend = [&](float* val, const float* bval, const float* l, int C, float* fg_out, float* bg_out) -> int {
-        bg_blend_kernel<<<(unsigned)mn_cdiv(N * C, 256), 256, 0, st>>>(val, bval, l, I(p.pos), N, C, fg_out, bg_out);
-        MN_LAUNCH_CHECK(ctx);
+    return blend_bg(ctx, o, bo, fo.bg_lambda, fo.bg_lambda_coarse, I(p.pos), N, st);
+}
+
+// ---- mn_render_rays_train(_bg): the recording render and its backward ------------------------------------------------------
+// The buffers of one network's recording two-pass render over N rays: S coarse samples, F fine draws, Sq (S + F under cascade, else
+// F) fine-query samples, `cols` point columns.  The tape holds what the backward reads: the depths as the composite reads them
+// (z_c_comp, z_q_comp; with flip - the background pass - the coarse depths reversed and, under cascade, the fine-query depths
+// reversed), the raw rows, the raw SH coefficients of an SH head and the two model tapes.  The workspace holds the depths in sample
+// order where they differ (z_c, z_q; kNone: the composite's buffer), the points and, with flip, their real depths, the weights, the
+// fine draws before sort_cat (z_f; kNone: the fine-query depths) and the model calls' workspace.  The backward workspace holds the
+// per-sample gradients and the model backward's workspace.
+struct TrainPassBufs {
+    int S, F, Sq, cols, flip;
+    size_t z_c_comp, raw_c, z_q_comp, raw_f, mlp_c, mlp_f, tape_c, tape_f, tape_c_bytes, tape_f_bytes;
+    size_t z_c, z_q, z_f, xyz_c, dreal_c, w_c, xyz_f, dreal_f, model_ws, model_ws_bytes;
+    size_t g_raw_c, g_raw_f, g_mlp_c, g_mlp_f, bwd_ws, bwd_ws_bytes;
+};
+
+// tc: the network trains at MN_PREC_TC_F16 (the model tapes and the backward workspace of the tensor-core pass)
+TrainPassBufs carve_train_pass(Carve& tape, Carve& ws, Carve& bwd, const mn_model* net, int64_t N, int S, int F, int use_cascade,
+                               bool sh, int cols, bool flip, bool tc) {
+    TrainPassBufs b{};
+    b.S = S; b.F = F; b.Sq = use_cascade ? S + F : F; b.cols = cols; b.flip = flip;
+    const int64_t Bc = N * S, Bf = N * b.Sq;
+    const int out_cols = net->nd.rgb_dim + 1;
+    b.z_c_comp = tape((size_t)Bc * 4);
+    b.raw_c = tape((size_t)Bc * 16);
+    b.z_q_comp = tape((size_t)Bf * 4);
+    b.raw_f = tape((size_t)Bf * 16);
+    b.mlp_c = sh ? tape((size_t)Bc * out_cols * 4) : kNone;
+    b.mlp_f = sh ? tape((size_t)Bf * out_cols * 4) : kNone;
+    b.tape_c_bytes = tc ? mn_model_tape_bytes_tc(net, Bc) : mn_model_tape_bytes(net, Bc);
+    b.tape_f_bytes = tc ? mn_model_tape_bytes_tc(net, Bf) : mn_model_tape_bytes(net, Bf);
+    b.tape_c = tape(b.tape_c_bytes);
+    b.tape_f = tape(b.tape_f_bytes);
+    b.z_c = flip ? ws((size_t)Bc * 4) : kNone;
+    b.z_q = flip && use_cascade ? ws((size_t)Bf * 4) : kNone;
+    b.z_f = use_cascade ? ws((size_t)N * F * 4) : kNone;
+    b.xyz_c = ws((size_t)Bc * cols * 4);
+    b.dreal_c = flip ? ws((size_t)Bc * 4) : kNone;
+    b.w_c = ws((size_t)Bc * 4);
+    b.xyz_f = ws((size_t)Bf * cols * 4);
+    b.dreal_f = flip ? ws((size_t)Bf * 4) : kNone;
+    const size_t a = mn_model_workspace_bytes(net, Bc, MN_PREC_FP32), c = mn_model_workspace_bytes(net, Bf, MN_PREC_FP32);
+    b.model_ws_bytes = a > c ? a : c;
+    b.model_ws = ws(b.model_ws_bytes);
+    b.g_raw_c = bwd((size_t)Bc * 16);
+    b.g_raw_f = bwd((size_t)Bf * 16);
+    b.g_mlp_c = sh ? bwd((size_t)Bc * out_cols * 4) : kNone;
+    b.g_mlp_f = sh ? bwd((size_t)Bf * out_cols * 4) : kNone;
+    const size_t ba = tc ? mn_model_backward_workspace_bytes_tc(net, Bc) : mn_model_backward_workspace_bytes(net, Bc);
+    const size_t bc = tc ? mn_model_backward_workspace_bytes_tc(net, Bf) : mn_model_backward_workspace_bytes(net, Bf);
+    b.bwd_ws_bytes = ba > bc ? ba : bc;
+    b.bwd_ws = bwd(b.bwd_ws_bytes);
+    return b;
+}
+
+// The recording two-pass render of one network (render.py `_two_pass`) into the tape T and workspace W, from the coarse depths
+// and points the caller wrote (b.z_c, b.z_c_comp, b.xyz_c, b.dreal_c): the recording coarse query, one composite for the
+// resampling weights and, under cascade, the coarse type's rgb and bg_lambda (the detached composite of the reference computes
+// the same weights), resampling, sort_cat under cascade, the fine points, the recording fine query and the final composite.
+// live: the device count of the rays that hold data (background pass), or null for all N.  u, noise_c, noise_f: the fine draws
+// and the density noise.  dirs / dstride, idx: per ray.  r and fine_points(z, S, flip_pts, xyz, dreal): as two_pass's.
+template <class Points>
+int train_two_pass(mn_ctx* ctx, mn_model* net, int precision, const TrainPassBufs& b, char* T, char* W, int64_t N, const int* live,
+                   int use_cascade, int sh_deg, const float* last_delta, const float* u, const float* noise_c, const float* noise_f,
+                   const float* dirs, int64_t dstride, const float* idx, const mn_render_outputs& r, Points&& fine_points,
+                   cudaStream_t st) {
+    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(T + off); };
+    auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
+    const LiveRows lr{live, 1};
+    const bool sh = sh_deg >= 0;
+    float* z_c = b.z_c == kNone ? TF(b.z_c_comp) : WF(b.z_c);
+    float* z_q = b.z_q == kNone ? TF(b.z_q_comp) : WF(b.z_q);
+    float* z_f = b.z_f == kNone ? z_q : WF(b.z_f);
+
+    // one recording model query on [N, S, cols] points -> raw [N, S, 4], into the model tape at `tape` (render.py `_query`)
+    auto query = [&](const float* xyz, int S, int coarse, const float* noise, float* mlp_out, float* raw_out, size_t tape,
+                     size_t tape_n) -> int {
+        mn_rows rows{};
+        rows.mode = 1;
+        rows.x_d = xyz;
+        rows.cols = b.cols;
+        rows.dirs_d = net->d.pos_dir_dim > 0 ? dirs : nullptr;
+        rows.dir_stride = dstride;
+        rows.idx_d = net->d.appearance_dim > 0 ? idx : nullptr;
+        rows.samples_per_ray = S;
+        const LiveRows lrs{live, S};
+        int e = mn_model_forward_train_live(ctx, net, &rows, N * S, lrs, coarse, noise, precision, sh ? mlp_out : raw_out, T + tape,
+                                            tape_n, W + b.model_ws, b.model_ws_bytes, st);
+        if (e) return e;
+        if (sh) return mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, net->nd.rgb_dim + 1, dirs, dstride, S, N * S, 1, lrs, raw_out, st);
         return MN_OK;
     };
-    if ((rc = blend(o.rgb, F(p.rgb_b), fo.bg_lambda, 3, o.fg_rgb, o.bg_rgb))) return rc;
-    if (o.depth)
-        if ((rc = blend(o.depth, F(p.depth_b), fo.bg_lambda, 1, o.fg_depth, o.bg_depth))) return rc;
-    if (use_cascade && fine && o.rgb_coarse)
-        if ((rc = blend(o.rgb_coarse, F(p.rgb_cb), fo.bg_lambda_coarse, 3, o.fg_rgb_coarse, o.bg_rgb_coarse))) return rc;
+
+    int rc;
+    if ((rc = query(WF(b.xyz_c), b.S, 1, noise_c, TF(b.mlp_c), TF(b.raw_c), b.tape_c, b.tape_c_bytes))) return rc;
+    if ((rc = mn_stage_composite(ctx, TF(b.raw_c), TF(b.z_c_comp), WF(b.dreal_c), b.S, nullptr, nullptr, nullptr, 0, last_delta, N,
+                                 b.flip, lr, WF(b.w_c), use_cascade ? r.rgb_coarse : nullptr, nullptr, nullptr,
+                                 use_cascade ? r.bg_lambda_coarse : nullptr, st)))
+        return rc;
+    if ((rc = mn_stage_sample_pdf(ctx, z_c, WF(b.w_c), b.S, nullptr, u, b.F, N, b.S, b.F, lr, z_f, nullptr, nullptr, st))) return rc;
+    if (use_cascade)
+        if ((rc = mn_stage_sort_cat(ctx, z_c, b.S, z_f, b.F, N, 0, lr, z_q, b.flip ? TF(b.z_q_comp) : nullptr, st))) return rc;
+    if ((rc = fine_points(z_q, b.Sq, b.flip && use_cascade, WF(b.xyz_f), WF(b.dreal_f)))) return rc;
+    if ((rc = query(WF(b.xyz_f), b.Sq, 0, noise_f, TF(b.mlp_f), TF(b.raw_f), b.tape_f, b.tape_f_bytes))) return rc;
+    // depth scratch when only the variance is wanted: the coarse weights are dead by now
+    float* depth = r.depth ? r.depth : (r.depth_var ? WF(b.w_c) : nullptr);
+    if (use_cascade)
+        return mn_stage_composite(ctx, TF(b.raw_f), TF(b.z_q_comp), WF(b.dreal_f), b.Sq, nullptr, nullptr, nullptr, 0, last_delta, N,
+                                  b.flip, lr, nullptr, r.rgb, depth, r.depth_var, r.bg_lambda, st);
+    return mn_stage_composite(ctx, TF(b.raw_f), TF(b.z_q_comp), WF(b.dreal_f), b.Sq, TF(b.raw_c), TF(b.z_c_comp), WF(b.dreal_c), b.S,
+                              last_delta, N, b.flip, lr, nullptr, r.rgb, depth, r.depth_var, r.bg_lambda, st);
+}
+
+// The backward of train_two_pass: the composite backward(s) - with the gradients of bg_lambda (g_lam, g_lam_c; null: none) - then
+// the fine and the coarse model backwards, each through the SH head's backward, into gw.  The coarse pass has no gradient under
+// cascade without g_rgb_coarse, and is skipped.  dirs / dstride: the directions the forward read.
+int train_two_pass_backward(mn_ctx* ctx, mn_model* net, int precision, const TrainPassBufs& b, const char* T, char* W, int64_t N,
+                            const int* live, int use_cascade, int sh_deg, const float* last_delta, const float* dirs, int64_t dstride,
+                            const float* g_rgb, const float* g_rgb_coarse, const float* g_lam, const float* g_lam_c, float* gw,
+                            cudaStream_t st) {
+    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<const float*>(T + off); };
+    auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
+    const LiveRows lr{live, 1};
+    const bool coarse = !use_cascade || g_rgb_coarse;
+    int rc;
+
+    // composites: the fine one (with the coarse samples merged in, without cascade), the cascade's coarse one
+    if (use_cascade) {
+        if ((rc = mn_stage_composite_backward(ctx, TF(b.raw_f), TF(b.z_q_comp), b.Sq, nullptr, nullptr, 0, last_delta, N, b.flip, lr,
+                                              g_rgb, g_lam, WF(b.g_raw_f), nullptr, st)))
+            return rc;
+        if (coarse && (rc = mn_stage_composite_backward(ctx, TF(b.raw_c), TF(b.z_c_comp), b.S, nullptr, nullptr, 0, last_delta, N,
+                                                        b.flip, lr, g_rgb_coarse, g_lam_c, WF(b.g_raw_c), nullptr, st)))
+            return rc;
+    } else if ((rc = mn_stage_composite_backward(ctx, TF(b.raw_f), TF(b.z_q_comp), b.Sq, TF(b.raw_c), TF(b.z_c_comp), b.S, last_delta,
+                                                 N, b.flip, lr, g_rgb, g_lam, WF(b.g_raw_f), WF(b.g_raw_c), st))) {
+        return rc;
+    }
+    // the model backwards in reverse order of their forward calls, each through the SH head's backward first
+    auto model_bwd = [&](int S, int use_coarse, size_t mlp, size_t g_raw, size_t g_mlp, size_t tape, size_t tape_n) -> int {
+        const LiveRows lrs{live, S};
+        const float* g = WF(g_raw);
+        int e;
+        if (sh_deg >= 0) {
+            if ((e = mn_stage_sh_to_rgb_backward(ctx, sh_deg, TF(mlp), net->nd.rgb_dim + 1, dirs, dstride, S, N * S, 1, lrs, g, WF(g_mlp),
+                                                 st)))
+                return e;
+            g = WF(g_mlp);
+        }
+        return mn_model_backward_live(ctx, net, N * S, lrs, use_coarse, precision, g, T + tape, tape_n, gw, W + b.bwd_ws,
+                                      b.bwd_ws_bytes, st);
+    };
+    if ((rc = model_bwd(b.Sq, 0, b.mlp_f, b.g_raw_f, b.g_mlp_f, b.tape_f, b.tape_f_bytes))) return rc;
+    if (coarse) return model_bwd(b.S, 1, b.mlp_c, b.g_raw_c, b.g_mlp_c, b.tape_c, b.tape_c_bytes);
     return MN_OK;
 }
 
-// ---- mn_render_rays_train: the recording foreground render and its backward ------------------------------------------------
-// The tape holds what the backward reads - the composite inputs (last delta, coarse and fine-query depths, raw rows), the raw SH
-// coefficients and a copy of the rays (their directions) for an SH head, and the tapes of the two model calls; the forward
-// workspace holds the rest (points, weights, the fine draws before sort_cat, the model calls' workspace); the backward workspace
-// the per-sample gradients and the model backward's workspace.
+// mn_render_rays_train: the foreground's pass, and in the tape its last deltas and, for an SH head, a copy of the rays (the
+// directions the backward reads).
 struct TrainPlan {
-    int S, F, Sq;
-    bool tc, sh;
-    size_t last_delta, z_c, raw_c, z_q, raw_f, mlp_c, mlp_f, rays, tape_c, tape_f, tape_c_bytes, tape_f_bytes, tape_total;
-    size_t xyz_c, w_c, z_f, xyz_f, model_ws, model_ws_bytes, ws_total;
-    size_t g_raw_c, g_raw_f, g_mlp_c, g_mlp_f, bwd_ws, bwd_ws_bytes, bwd_total;
+    TrainPassBufs pass;
+    size_t last_delta, rays, tape_total, ws_total, bwd_total;
 };
 
 TrainPlan make_train_plan(const mn_model* m, int64_t N, int S, int F, int use_cascade, bool sh, bool tc) {
     TrainPlan p{};
-    p.S = S; p.F = F; p.Sq = use_cascade ? S + F : F; p.tc = tc; p.sh = sh;
-    const int64_t Bc = N * S, Bf = N * p.Sq;
-    const int out_cols = m->nd.rgb_dim + 1;
-    Carve t;
+    Carve t, w, b;
     p.last_delta = t((size_t)N * 4);
-    p.z_c = t((size_t)Bc * 4);
-    p.raw_c = t((size_t)Bc * 16);
-    p.z_q = t((size_t)Bf * 4);
-    p.raw_f = t((size_t)Bf * 16);
-    p.mlp_c = sh ? t((size_t)Bc * out_cols * 4) : kNone;
-    p.mlp_f = sh ? t((size_t)Bf * out_cols * 4) : kNone;
+    p.pass = carve_train_pass(t, w, b, m, N, S, F, use_cascade, sh, 3, false, tc);
     p.rays = sh ? t((size_t)N * 32) : kNone;
-    p.tape_c_bytes = tc ? mn_model_tape_bytes_tc(m, Bc) : mn_model_tape_bytes(m, Bc);
-    p.tape_f_bytes = tc ? mn_model_tape_bytes_tc(m, Bf) : mn_model_tape_bytes(m, Bf);
-    p.tape_c = t(p.tape_c_bytes);
-    p.tape_f = t(p.tape_f_bytes);
     p.tape_total = t.off + 256;
-    Carve w;
-    p.xyz_c = w((size_t)Bc * 12);
-    p.w_c = w((size_t)Bc * 4);
-    p.z_f = use_cascade ? w((size_t)N * F * 4) : p.z_q;     // without cascade the fine draws are the fine-query depths (tape)
-    p.xyz_f = w((size_t)Bf * 12);
-    const size_t a = mn_model_workspace_bytes(m, Bc, MN_PREC_FP32), c = mn_model_workspace_bytes(m, Bf, MN_PREC_FP32);
-    p.model_ws_bytes = a > c ? a : c;
-    p.model_ws = w(p.model_ws_bytes);
     p.ws_total = w.off + 256;
-    Carve b;
-    p.g_raw_c = b((size_t)Bc * 16);
-    p.g_raw_f = b((size_t)Bf * 16);
-    p.g_mlp_c = sh ? b((size_t)Bc * out_cols * 4) : kNone;
-    p.g_mlp_f = sh ? b((size_t)Bf * out_cols * 4) : kNone;
-    const size_t ba = tc ? mn_model_backward_workspace_bytes_tc(m, Bc) : mn_model_backward_workspace_bytes(m, Bc);
-    const size_t bc = tc ? mn_model_backward_workspace_bytes_tc(m, Bf) : mn_model_backward_workspace_bytes(m, Bf);
-    p.bwd_ws_bytes = ba > bc ? ba : bc;
-    p.bwd_ws = b(p.bwd_ws_bytes);
     p.bwd_total = b.off + 256;
     return p;
 }
@@ -558,66 +685,6 @@ int check_train(mn_ctx* ctx, const mn_model* m, int64_t N, int coarse_samples, i
     return MN_OK;
 }
 
-// The foreground's recording two-pass render into the tape T and workspace W laid out by p: coarse sampling (up to far_ov, the
-// background split's far override, when given), the recording coarse query, the detached-weights composite, resampling, sort_cat
-// under cascade, the recording fine query and the final composite.  The caller has written the last deltas into the tape.  lam /
-// lam_c: bg_lambda of the final and (cascade) the coarse type, null without a background network.
-int train_fg_pass(mn_ctx* ctx, mn_model* m, const TrainPlan& p, char* T, char* W, const float* rays_d, const float* image_indices_d,
-                  int64_t N, const float* far_ov, const float* z_steps_d, const float* jitter_d, float perturb, const float* noise_c_d,
-                  const float* u_d, const float* noise_f_d, int use_cascade, int sh_deg, float* rgb, float* depth, float* var,
-                  float* rgb_coarse, float* lam, float* lam_c, cudaStream_t st) {
-    const int S = p.S, F = p.F;
-    const bool sh = p.sh, tc = p.tc;
-    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(T + off); };
-    auto WF = [&](size_t off) { return reinterpret_cast<float*>(W + off); };
-    const LiveRows all{};
-    int rc;
-
-    // one recording model query on [N, Sq, 3] points -> raw [N, Sq, 4], into the model tape at `tape` (render.py `_query`)
-    auto query = [&](const float* xyz, int Sq, int coarse, const float* noise, float* mlp_out, float* raw_out, size_t tape,
-                     size_t tape_n) -> int {
-        mn_rows rows{};
-        rows.mode = 1;
-        rows.x_d = xyz;
-        rows.cols = 3;
-        rows.dirs_d = m->d.pos_dir_dim > 0 ? rays_d + 3 : nullptr;
-        rows.dir_stride = 8;
-        rows.idx_d = image_indices_d;
-        rows.samples_per_ray = Sq;
-        float* out = sh ? mlp_out : raw_out;
-        auto fn = tc ? mn_model_forward_train_tc : mn_model_forward_train;
-        int r = fn(ctx, m, &rows, N * Sq, coarse, noise, out, T + tape, tape_n, W + p.model_ws, p.model_ws_bytes, st);
-        if (r) return r;
-        if (sh) return mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, m->nd.rgb_dim + 1, rays_d + 3, 8, Sq, N * Sq, 1, all, raw_out, st);
-        return MN_OK;
-    };
-
-    if (sh) MN_CUDA(ctx, cudaMemcpyAsync(T + p.rays, rays_d, (size_t)N * 32, cudaMemcpyDeviceToDevice, st));
-    if ((rc = mn_sample_coarse(ctx, rays_d, far_ov, z_steps_d, jitter_d, perturb, N, S, TF(p.z_c), WF(p.xyz_c), st))) return rc;
-    if ((rc = query(WF(p.xyz_c), S, 1, noise_c_d, TF(p.mlp_c), TF(p.raw_c), p.tape_c, p.tape_c_bytes))) return rc;
-    // the cascade's coarse colour, then the resampling weights of the detached coarse composite (render.py `_two_pass`)
-    if (use_cascade)
-        if ((rc = mn_stage_composite(ctx, TF(p.raw_c), TF(p.z_c), nullptr, S, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
-                                     nullptr, rgb_coarse, nullptr, nullptr, lam_c, st)))
-            return rc;
-    if ((rc = mn_stage_composite(ctx, TF(p.raw_c), TF(p.z_c), nullptr, S, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
-                                 WF(p.w_c), nullptr, nullptr, nullptr, nullptr, st)))
-        return rc;
-    float* z_f = use_cascade ? WF(p.z_f) : TF(p.z_q);
-    if ((rc = mn_stage_sample_pdf(ctx, TF(p.z_c), WF(p.w_c), S, nullptr, u_d, F, N, S, F, all, z_f, nullptr, nullptr, st))) return rc;
-    if (use_cascade)
-        if ((rc = mn_stage_sort_cat(ctx, TF(p.z_c), S, z_f, F, N, 0, all, TF(p.z_q), nullptr, st))) return rc;
-    if ((rc = mn_points_from_z(ctx, rays_d, TF(p.z_q), N, p.Sq, WF(p.xyz_f), st))) return rc;
-    if ((rc = query(WF(p.xyz_f), p.Sq, 0, noise_f_d, TF(p.mlp_f), TF(p.raw_f), p.tape_f, p.tape_f_bytes))) return rc;
-    // depth scratch when only the variance is wanted: the coarse weights are dead by now
-    float* d = depth ? depth : (var ? WF(p.w_c) : nullptr);
-    if (use_cascade)
-        return mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_q), nullptr, p.Sq, nullptr, nullptr, nullptr, 0, TF(p.last_delta), N, 0, all,
-                                  nullptr, rgb, d, var, lam, st);
-    return mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_q), nullptr, p.Sq, TF(p.raw_c), TF(p.z_c), nullptr, S, TF(p.last_delta), N, 0,
-                              all, nullptr, rgb, d, var, lam, st);
-}
-
 int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N, const float* z_steps_d,
                const float* jitter_d, float perturb, int S, const float* noise_c_d, const float* u_d, const float* noise_f_d, int F,
                int use_cascade, int sh_deg, int precision, float* rgb, float* depth, float* var, float* rgb_coarse, void* tape_d,
@@ -631,55 +698,26 @@ int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image
     if (perturb > 0 && !jitter_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": perturb > 0 needs jitter_d");
     if (use_cascade && !rgb_coarse) return mn_fail(ctx, MN_ERR_INVALID, nm + ": rgb_coarse_out_d is required under use_cascade");
     if (N == 0) return MN_OK;
-    const bool sh = sh_deg >= 0, tc = precision == MN_PREC_TC_F16;
-    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh, tc);
+    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
     if (!workspace_d || workspace_bytes < p.ws_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     char* T = (char*)tape_d;
-    fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(reinterpret_cast<float*>(T + p.last_delta), N, 1e10f);   // rendering.py:33
+    char* W = (char*)workspace_d;
+    float* last_delta = reinterpret_cast<float*>(T + p.last_delta);
+    fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(last_delta, N, 1e10f);   // rendering.py:33
     MN_LAUNCH_CHECK(ctx);
-    return train_fg_pass(ctx, m, p, T, (char*)workspace_d, rays_d, image_indices_d, N, nullptr, z_steps_d, jitter_d, perturb, noise_c_d,
-                         u_d, noise_f_d, use_cascade, sh_deg, rgb, depth, var, rgb_coarse, nullptr, nullptr, st);
-}
-
-// The backward of train_fg_pass: the composite backward(s) - with the gradients of bg_lambda (g_lam, g_lam_c; null: none) - then
-// the model backwards in reverse order of their forward calls, into gw.
-int train_fg_backward(mn_ctx* ctx, mn_model* m, const TrainPlan& p, const char* T, char* W, int64_t N, int use_cascade, int sh_deg,
-                      const float* g_rgb, const float* g_rgb_coarse, const float* g_lam, const float* g_lam_c, float* gw, cudaStream_t st) {
-    const int S = p.S;
-    const bool sh = p.sh, tc = p.tc;
-    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<const float*>(T + off); };
-    auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
-    const bool coarse = !use_cascade || g_rgb_coarse;     // the coarse query has a gradient
-    int rc;
-
-    // composites: the fine one (with the coarse samples merged in, without cascade), the cascade's coarse one
-    if (use_cascade) {
-        if ((rc = mn_composite_backward(ctx, TF(p.raw_f), TF(p.z_q), p.Sq, nullptr, nullptr, 0, TF(p.last_delta), N, 0, g_rgb, g_lam,
-                                        WF(p.g_raw_f), nullptr, st)))
-            return rc;
-        if (coarse && (rc = mn_composite_backward(ctx, TF(p.raw_c), TF(p.z_c), S, nullptr, nullptr, 0, TF(p.last_delta), N, 0,
-                                                  g_rgb_coarse, g_lam_c, WF(p.g_raw_c), nullptr, st)))
-            return rc;
-    } else if ((rc = mn_composite_backward(ctx, TF(p.raw_f), TF(p.z_q), p.Sq, TF(p.raw_c), TF(p.z_c), S, TF(p.last_delta), N, 0, g_rgb,
-                                           g_lam, WF(p.g_raw_f), WF(p.g_raw_c), st))) {
+    if (p.rays != kNone) MN_CUDA(ctx, cudaMemcpyAsync(T + p.rays, rays_d, (size_t)N * 32, cudaMemcpyDeviceToDevice, st));
+    if ((rc = mn_sample_coarse(ctx, rays_d, nullptr, z_steps_d, jitter_d, perturb, N, S, reinterpret_cast<float*>(T + p.pass.z_c_comp),
+                               reinterpret_cast<float*>(W + p.pass.xyz_c), st)))
         return rc;
-    }
-    // the model backwards in reverse order of their forward calls, each through the SH head's backward first
-    auto model_bwd = [&](int Sq, int use_coarse, size_t mlp, size_t g_raw, size_t g_mlp, size_t tape, size_t tape_n) -> int {
-        const float* g = WF(g_raw);
-        int r;
-        if (sh) {
-            if ((r = mn_sh_to_rgb_backward(ctx, sh_deg, TF(mlp), m->nd.rgb_dim + 1, TF(p.rays) + 3, 8, Sq, N * Sq, 1, g, WF(g_mlp), st)))
-                return r;
-            g = WF(g_mlp);
-        }
-        auto fn = tc ? mn_model_backward_tc : mn_model_backward;
-        return fn(ctx, m, N * Sq, use_coarse, g, T + tape, tape_n, gw, W + p.bwd_ws, p.bwd_ws_bytes, st);
-    };
-    if ((rc = model_bwd(p.Sq, 0, p.mlp_f, p.g_raw_f, p.g_mlp_f, p.tape_f, p.tape_f_bytes))) return rc;
-    if (coarse) return model_bwd(S, 1, p.mlp_c, p.g_raw_c, p.g_mlp_c, p.tape_c, p.tape_c_bytes);
-    return MN_OK;
+    mn_render_outputs o{};
+    o.rgb = rgb;
+    o.depth = depth;
+    o.depth_var = var;
+    o.rgb_coarse = rgb_coarse;
+    auto from_z = [&](const float* z, int Sq, int, float* xyz, float*) { return mn_points_from_z(ctx, rays_d, z, N, Sq, xyz, st); };
+    return train_two_pass(ctx, m, precision, p.pass, T, W, N, nullptr, use_cascade, sh_deg, last_delta, u_d, noise_c_d, noise_f_d,
+                          rays_d + 3, 8, image_indices_d, o, from_z, st);
 }
 
 int train_backward_impl(mn_ctx* ctx, mn_model* m, int64_t N, int S, int F, int use_cascade, int sh_deg, int precision,
@@ -691,12 +729,14 @@ int train_backward_impl(mn_ctx* ctx, mn_model* m, int64_t N, int S, int F, int u
     int rc;
     if ((rc = check_train(ctx, m, N, S, F, precision, name))) return rc;
     if (N == 0) return MN_OK;
-    const bool sh = sh_deg >= 0, tc = precision == MN_PREC_TC_F16;
-    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh, tc);
+    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
     if (!workspace_d || workspace_bytes < p.bwd_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
-    return train_fg_backward(ctx, m, p, (const char*)tape_d, (char*)workspace_d, N, use_cascade, sh_deg, g_rgb, g_rgb_coarse, nullptr,
-                             nullptr, gw, st);
+    const char* T = (const char*)tape_d;
+    const float* dirs = p.rays == kNone ? nullptr : reinterpret_cast<const float*>(T + p.rays) + 3;
+    return train_two_pass_backward(ctx, m, precision, p.pass, T, (char*)workspace_d, N, nullptr, use_cascade, sh_deg,
+                                   reinterpret_cast<const float*>(T + p.last_delta), dirs, 8, g_rgb, g_rgb_coarse, nullptr, nullptr, gw,
+                                   st);
 }
 
 // ---- mn_render_rays_train_bg: the recording render with a background network and its backward ------------------------------
@@ -734,35 +774,27 @@ __global__ void bg_blend_backward_kernel(const float* __restrict__ g, const floa
     g_lam[i] = gl;
 }
 
-// The buffers of the background network's recording pass over N rays (the compacted background rays first), after the
-// foreground's TrainPlan in each of the three regions.  S / F: the background's coarse samples and fine draws (half the
-// foreground's), Sq: its fine-query samples.  Tape: the split (compacted positions and count), the blend's inputs (bg_lambda
-// of both types, the background colours), the composite inputs in composite order (coarse depths reversed; fine-query depths
-// reversed under cascade), the raw rows, the compacted directions and raw SH coefficients for an SH head, and the two model
-// tapes.  Workspace: the rest of the split, the depths in sample order, the points, the weights, the gathered draws of ray-indexed
-// blocks and the model calls' workspace.  Backward workspace: the blend's gradients, the per-sample gradients and the model
-// backward's workspace.
+// The buffers of the recording render with a background network over N rays (the compacted background rays first), after the
+// foreground's TrainPlan in each of the three regions, then the background network's pass (half the foreground's samples).  Tape:
+// the split (compacted positions and count), the background's last deltas, the blend's inputs (bg_lambda of both types, the
+// background colours) and the compacted directions.  Workspace: the rest of the split (far override, block counts, ids, image
+// indices), the background depth and the gathered draws of ray-indexed blocks.  Backward workspace: the blend's gradients.
 struct BgTrainPlan {
     TrainPlan fg;
-    int S, F, Sq, cols;
-    bool tc, sh;
-    size_t pos, count, ld_b, lam, lam_c, rgb_b, rgb_cb, dirs, z_cc, raw_c, z_qc, raw_f, mlp_c, mlp_f, tape_c, tape_f, tape_c_bytes,
-        tape_f_bytes, tape_total;
-    size_t far_ov, blk, ids, idx, z_c, xyz_c, dreal_c, w_c, z_f, z_q, xyz_f, dreal_f, depth_b, jit, u, noise_c, noise_f, model_ws,
-        model_ws_bytes, ws_total;
-    size_t g_rgb_b, g_rgb_cb, g_lam, g_lam_c, g_raw_c, g_raw_f, g_mlp_c, g_mlp_f, bwd_ws, bwd_ws_bytes, bwd_total;
+    TrainPassBufs bg;
+    size_t pos, count, ld_b, lam, lam_c, rgb_b, rgb_cb, dirs, tape_total;
+    size_t far_ov, blk, ids, idx, depth_b, jit, u, noise_c, noise_f, ws_total;
+    size_t g_rgb_b, g_rgb_cb, g_lam, g_lam_c, bwd_total;
 };
 
 BgTrainPlan make_bg_train_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, bool sh, bool tc,
                                bool bg_tc) {
     BgTrainPlan p{};
     p.fg = make_train_plan(m, N, Sc, Sf, use_cascade, sh, tc);
-    p.S = Sc / 2; p.F = Sf / 2; p.Sq = use_cascade ? p.S + p.F : p.F; p.tc = bg_tc; p.sh = sh;
-    p.cols = bg->d.kind == 2 && bg->d.xyz_real ? 7 : 4;      // the real-xyz routing prefix, then [point, 1/r]
-    const int64_t Bc = N * p.S, Bf = N * p.Sq;
-    const int out_cols = bg->nd.rgb_dim + 1;
-    Carve t;
+    Carve t, w, b;
     t.off = p.fg.tape_total;
+    w.off = p.fg.ws_total;
+    b.off = p.fg.bwd_total;
     p.pos = t((size_t)N * 4);
     p.count = t(4);
     p.ld_b = t((size_t)N * 4);
@@ -771,54 +803,23 @@ BgTrainPlan make_bg_train_plan(const mn_model* m, const mn_model* bg, int64_t N,
     p.rgb_b = t((size_t)N * 12);
     p.rgb_cb = t((size_t)N * 12);
     p.dirs = t((size_t)N * 12);
-    p.z_cc = t((size_t)Bc * 4);
-    p.raw_c = t((size_t)Bc * 16);
-    p.z_qc = t((size_t)Bf * 4);
-    p.raw_f = t((size_t)Bf * 16);
-    p.mlp_c = sh ? t((size_t)Bc * out_cols * 4) : kNone;
-    p.mlp_f = sh ? t((size_t)Bf * out_cols * 4) : kNone;
-    p.tape_c_bytes = bg_tc ? mn_model_tape_bytes_tc(bg, Bc) : mn_model_tape_bytes(bg, Bc);
-    p.tape_f_bytes = bg_tc ? mn_model_tape_bytes_tc(bg, Bf) : mn_model_tape_bytes(bg, Bf);
-    p.tape_c = t(p.tape_c_bytes);
-    p.tape_f = t(p.tape_f_bytes);
-    p.tape_total = t.off + 256;
-    Carve w;
-    w.off = p.fg.ws_total;
     p.far_ov = w((size_t)N * 4);
-    p.blk = w((size_t)mn_cdiv(N, kSplitBlock) * 4);
+    p.blk = w((size_t)mn_cdiv(N, kCompactBlock) * 4);
     p.ids = w((size_t)N * 8);
     p.idx = w((size_t)N * 4);
-    p.z_c = w((size_t)Bc * 4);
-    p.xyz_c = w((size_t)Bc * p.cols * 4);
-    p.dreal_c = w((size_t)Bc * 4);
-    p.w_c = w((size_t)Bc * 4);
-    p.z_f = use_cascade ? w((size_t)N * p.F * 4) : kNone;      // without cascade the fine draws are the fine-query depths (tape)
-    p.z_q = use_cascade ? w((size_t)Bf * 4) : kNone;
-    p.xyz_f = w((size_t)Bf * p.cols * 4);
-    p.dreal_f = w((size_t)Bf * 4);
-    p.depth_b = w((size_t)N * 4);
-    p.jit = w((size_t)Bc * 4);
-    p.u = w((size_t)N * p.F * 4);
-    p.noise_c = w((size_t)Bc * 4);
-    p.noise_f = w((size_t)Bf * 4);
-    const size_t a = mn_model_workspace_bytes(bg, Bc, MN_PREC_FP32), c = mn_model_workspace_bytes(bg, Bf, MN_PREC_FP32);
-    p.model_ws_bytes = a > c ? a : c;
-    p.model_ws = w(p.model_ws_bytes);
-    p.ws_total = w.off + 256;
-    Carve b;
-    b.off = p.fg.bwd_total;
     p.g_rgb_b = b((size_t)N * 12);
     p.g_rgb_cb = b((size_t)N * 12);
     p.g_lam = b((size_t)N * 4);
     p.g_lam_c = b((size_t)N * 4);
-    p.g_raw_c = b((size_t)Bc * 16);
-    p.g_raw_f = b((size_t)Bf * 16);
-    p.g_mlp_c = sh ? b((size_t)Bc * out_cols * 4) : kNone;
-    p.g_mlp_f = sh ? b((size_t)Bf * out_cols * 4) : kNone;
-    const size_t ba = bg_tc ? mn_model_backward_workspace_bytes_tc(bg, Bc) : mn_model_backward_workspace_bytes(bg, Bc);
-    const size_t bc = bg_tc ? mn_model_backward_workspace_bytes_tc(bg, Bf) : mn_model_backward_workspace_bytes(bg, Bf);
-    p.bwd_ws_bytes = ba > bc ? ba : bc;
-    p.bwd_ws = b(p.bwd_ws_bytes);
+    // the real-xyz routing prefix, then [point, 1/r]
+    p.bg = carve_train_pass(t, w, b, bg, N, Sc / 2, Sf / 2, use_cascade, sh, bg->d.kind == 2 && bg->d.xyz_real ? 7 : 4, true, bg_tc);
+    p.depth_b = w((size_t)N * 4);
+    p.jit = w((size_t)N * p.bg.S * 4);
+    p.u = w((size_t)N * p.bg.F * 4);
+    p.noise_c = w((size_t)N * p.bg.S * 4);
+    p.noise_f = w((size_t)N * p.bg.Sq * 4);
+    p.tape_total = t.off + 256;
+    p.ws_total = w.off + 256;
     p.bwd_total = b.off + 256;
     return p;
 }
@@ -855,31 +856,25 @@ int train_bg_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, c
     if (include_xyz_real != (bg->d.kind == 2 && bg->d.xyz_real ? 1 : 0))
         return mn_fail(ctx, MN_ERR_INVALID, nm + ": include_xyz_real must match the background model's real-xyz prefix");
     if (N == 0) return MN_OK;
-    const bool sh = sh_deg >= 0;
-    const BgTrainPlan p = make_bg_train_plan(m, bg, N, Sc, Sf, use_cascade, sh, precision == MN_PREC_TC_F16,
+    const BgTrainPlan p = make_bg_train_plan(m, bg, N, Sc, Sf, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
                                              bg_precision == MN_PREC_TC_F16);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
     if (!workspace_d || workspace_bytes < p.ws_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     char* T = (char*)tape_d;
     char* W = (char*)workspace_d;
-    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(T + off); };
-    auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
+    auto TF = [&](size_t off) { return reinterpret_cast<float*>(T + off); };
+    auto WF = [&](size_t off) { return reinterpret_cast<float*>(W + off); };
     int* pos = reinterpret_cast<int*>(T + p.pos);
-    const int* cnt = reinterpret_cast<const int*>(T + p.count);
-    const int64_t* ids = reinterpret_cast<const int64_t*>(W + p.ids);
+    int* cnt = reinterpret_cast<int*>(T + p.count);
+    int64_t* ids = reinterpret_cast<int64_t*>(W + p.ids);
     const LiveRows lr{cnt, 1};
+    const TrainPassBufs& b = p.bg;
 
     // ---- split and compaction (render.py:327-342): the foreground's last deltas land in its tape
-    const unsigned nblk = (unsigned)mn_cdiv(N, kSplitBlock);
-    bg_split_kernel<<<nblk, kSplitBlock, 0, st>>>(rays_d, center_d, radius_d, N, WF(p.far_ov), TF(p.fg.last_delta), pos,
-                                                 reinterpret_cast<int*>(W + p.blk), ctx->status_d);
-    MN_LAUNCH_CHECK(ctx);
     float* bidx = image_indices_d ? WF(p.idx) : nullptr;
-    bg_compact_kernel<<<nblk, kSplitBlock, 0, st>>>(rays_d, image_indices_d, N, reinterpret_cast<int*>(W + p.blk), pos,
-                                                   reinterpret_cast<int64_t*>(W + p.ids), TF(p.dirs), bidx, reinterpret_cast<int*>(T + p.count));
-    MN_LAUNCH_CHECK(ctx);
-    fill_kernel<<<(unsigned)mn_cdiv(N, 256), 256, 0, st>>>(TF(p.ld_b), N, 1e10f);            // the background's last delta
-    MN_LAUNCH_CHECK(ctx);
+    if ((rc = split_bg(ctx, rays_d, image_indices_d, N, center_d, radius_d, WF(p.far_ov), TF(p.fg.last_delta), pos,
+                       reinterpret_cast<int*>(W + p.blk), cnt, ids, TF(p.dirs), bidx, TF(p.ld_b), st)))
+        return rc;
 
     // ---- the background draws in compacted order: ray-indexed blocks are gathered at the background rays
     const float *jit = jitter_bg_d, *ub = u_bg_d, *nc = noise_c_bg_d, *nf = noise_f_bg_d;
@@ -891,82 +886,46 @@ int train_bg_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, c
             src = WF(dst);
             return MN_OK;
         };
-        if ((rc = gather(jit, p.S, p.jit)) || (rc = gather(ub, p.F, p.u)) || (rc = gather(nc, p.S, p.noise_c)) ||
-            (rc = gather(nf, p.Sq, p.noise_f)))
+        if ((rc = gather(jit, b.S, p.jit)) || (rc = gather(ub, b.F, p.u)) || (rc = gather(nc, b.S, p.noise_c)) ||
+            (rc = gather(nf, b.Sq, p.noise_f)))
             return rc;
     }
 
     // ---- background pass over the compacted rays (render.py `bg_pass`, `_two_pass` flipped): stratified depths in sample order
-    // and reversed, the points outside the sphere in reversed sample order, recording coarse query, composite, resampling,
-    // recording fine query, composite
+    // and reversed, the points outside the sphere in reversed sample order
     auto outside = [&](const float* z, int S, int flip_pts, float* xyz, float* dreal) {
         return mn_stage_points_outside(ctx, rays_d, ids, z, center_d, radius_d, N, S, include_xyz_real, cluster_2d, flip_pts, lr, xyz,
                                        dreal, st);
     };
-    auto bquery = [&](const float* xyz, int S, int coarse, const float* noise, float* mlp_out, float* raw_out, size_t tape,
-                      size_t tape_n) -> int {
-        mn_rows rows{};
-        rows.mode = 1;
-        rows.x_d = xyz;
-        rows.cols = p.cols;
-        rows.dirs_d = bg->d.pos_dir_dim > 0 ? TF(p.dirs) : nullptr;
-        rows.dir_stride = 3;
-        rows.idx_d = bg->d.appearance_dim > 0 ? bidx : nullptr;
-        rows.samples_per_ray = S;
-        const LiveRows lrs{cnt, S};
-        int r = mn_model_forward_train_live(ctx, bg, &rows, N * S, lrs, coarse, noise, bg_precision, sh ? mlp_out : raw_out, T + tape,
-                                            tape_n, W + p.model_ws, p.model_ws_bytes, st);
-        if (r) return r;
-        if (sh) return mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, bg->nd.rgb_dim + 1, TF(p.dirs), 3, S, N * S, 1, lrs, raw_out, st);
-        return MN_OK;
-    };
-    if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, jit, perturb, N, p.S, 0, lr, WF(p.z_c), st))) return rc;
-    flip_rows_kernel<<<(unsigned)mn_cdiv(N * p.S, 256), 256, 0, st>>>(WF(p.z_c), N, p.S, lr, TF(p.z_cc));
+    if ((rc = mn_stage_stratify(ctx, z_steps_bg_d, 0, jit, perturb, N, b.S, 0, lr, WF(b.z_c), st))) return rc;
+    flip_rows_kernel<<<(unsigned)mn_cdiv(N * b.S, 256), 256, 0, st>>>(WF(b.z_c), N, b.S, lr, TF(b.z_c_comp));
     MN_LAUNCH_CHECK(ctx);
-    if ((rc = outside(WF(p.z_c), p.S, 1, WF(p.xyz_c), WF(p.dreal_c)))) return rc;
-    if ((rc = bquery(WF(p.xyz_c), p.S, 1, nc, TF(p.mlp_c), TF(p.raw_c), p.tape_c, p.tape_c_bytes))) return rc;
-    // resampling weights and, under cascade, the coarse colour: one composite (the detached one of the reference computes the same)
-    if ((rc = mn_stage_composite(ctx, TF(p.raw_c), TF(p.z_cc), WF(p.dreal_c), p.S, nullptr, nullptr, nullptr, 0, TF(p.ld_b), N, 1, lr,
-                                 WF(p.w_c), use_cascade ? TF(p.rgb_cb) : nullptr, nullptr, nullptr, nullptr, st)))
+    if ((rc = outside(WF(b.z_c), b.S, 1, WF(b.xyz_c), WF(b.dreal_c)))) return rc;
+    mn_render_outputs bo{};
+    bo.rgb = TF(p.rgb_b);
+    bo.depth = o.depth ? WF(p.depth_b) : nullptr;
+    bo.rgb_coarse = TF(p.rgb_cb);
+    if ((rc = train_two_pass(ctx, bg, bg_precision, b, T, W, N, cnt, use_cascade, sh_deg, TF(p.ld_b), ub, nc, nf, TF(p.dirs), 3, bidx,
+                             bo, outside, st)))
         return rc;
-    if ((rc = mn_stage_sample_pdf(ctx, WF(p.z_c), WF(p.w_c), p.S, nullptr, ub, p.F, N, p.S, p.F, lr,
-                                  use_cascade ? WF(p.z_f) : TF(p.z_qc), nullptr, nullptr, st)))
-        return rc;
-    float* depth_b = o.depth ? WF(p.depth_b) : nullptr;
-    if (use_cascade) {
-        if ((rc = mn_stage_sort_cat(ctx, WF(p.z_c), p.S, WF(p.z_f), p.F, N, 0, lr, WF(p.z_q), TF(p.z_qc), st))) return rc;
-        if ((rc = outside(WF(p.z_q), p.Sq, 1, WF(p.xyz_f), WF(p.dreal_f)))) return rc;
-        if ((rc = bquery(WF(p.xyz_f), p.Sq, 0, nf, TF(p.mlp_f), TF(p.raw_f), p.tape_f, p.tape_f_bytes))) return rc;
-        rc = mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_qc), WF(p.dreal_f), p.Sq, nullptr, nullptr, nullptr, 0, TF(p.ld_b), N, 1, lr,
-                                nullptr, TF(p.rgb_b), depth_b, nullptr, nullptr, st);
-    } else {
-        if ((rc = outside(TF(p.z_qc), p.Sq, 0, WF(p.xyz_f), WF(p.dreal_f)))) return rc;
-        if ((rc = bquery(WF(p.xyz_f), p.Sq, 0, nf, TF(p.mlp_f), TF(p.raw_f), p.tape_f, p.tape_f_bytes))) return rc;
-        rc = mn_stage_composite(ctx, TF(p.raw_f), TF(p.z_qc), WF(p.dreal_f), p.Sq, TF(p.raw_c), TF(p.z_cc), WF(p.dreal_c), p.S,
-                                TF(p.ld_b), N, 1, lr, nullptr, TF(p.rgb_b), depth_b, nullptr, nullptr, st);
-    }
-    if (rc) return rc;
 
     // ---- foreground pass with the far override, the last deltas and bg_lambda of both types (render.py:344-348)
-    if ((rc = train_fg_pass(ctx, m, p.fg, T, W, rays_d, image_indices_d, N, WF(p.far_ov), z_steps_d, jitter_d, perturb, noise_c_d, u_d,
-                            noise_f_d, use_cascade, sh_deg, o.rgb, o.depth, o.depth_var, o.rgb_coarse, TF(p.lam),
-                            use_cascade ? TF(p.lam_c) : nullptr, st)))
+    mn_render_outputs fo = o;
+    fo.bg_lambda = TF(p.lam);
+    fo.bg_lambda_coarse = use_cascade ? TF(p.lam_c) : nullptr;
+    if (p.fg.rays != kNone) MN_CUDA(ctx, cudaMemcpyAsync(T + p.fg.rays, rays_d, (size_t)N * 32, cudaMemcpyDeviceToDevice, st));
+    if ((rc = mn_sample_coarse(ctx, rays_d, WF(p.far_ov), z_steps_d, jitter_d, perturb, N, Sc, TF(p.fg.pass.z_c_comp),
+                               WF(p.fg.pass.xyz_c), st)))
         return rc;
-    MN_CUDA(ctx, cudaMemcpyAsync(o.bg_lambda, TF(p.lam), (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
-    if (use_cascade) MN_CUDA(ctx, cudaMemcpyAsync(o.bg_lambda_coarse, TF(p.lam_c), (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
+    auto from_z = [&](const float* z, int Sq, int, float* xyz, float*) { return mn_points_from_z(ctx, rays_d, z, N, Sq, xyz, st); };
+    if ((rc = train_two_pass(ctx, m, precision, p.fg.pass, T, W, N, nullptr, use_cascade, sh_deg, TF(p.fg.last_delta), u_d, noise_c_d,
+                             noise_f_d, rays_d + 3, 8, image_indices_d, fo, from_z, st)))
+        return rc;
+    MN_CUDA(ctx, cudaMemcpyAsync(o.bg_lambda, fo.bg_lambda, (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
+    if (use_cascade) MN_CUDA(ctx, cudaMemcpyAsync(o.bg_lambda_coarse, fo.bg_lambda_coarse, (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
 
     // ---- blend (render.py:350-376)
-    auto blend = [&](float* val, const float* bval, const float* l, int C, float* fg_out, float* bg_out) -> int {
-        bg_blend_kernel<<<(unsigned)mn_cdiv(N * C, 256), 256, 0, st>>>(val, bval, l, pos, N, C, fg_out, bg_out);
-        MN_LAUNCH_CHECK(ctx);
-        return MN_OK;
-    };
-    if ((rc = blend(o.rgb, TF(p.rgb_b), TF(p.lam), 3, o.fg_rgb, o.bg_rgb))) return rc;
-    if (o.depth)
-        if ((rc = blend(o.depth, WF(p.depth_b), TF(p.lam), 1, o.fg_depth, o.bg_depth))) return rc;
-    if (use_cascade)
-        if ((rc = blend(o.rgb_coarse, TF(p.rgb_cb), TF(p.lam_c), 3, o.fg_rgb_coarse, o.bg_rgb_coarse))) return rc;
-    return MN_OK;
+    return blend_bg(ctx, o, bo, fo.bg_lambda, fo.bg_lambda_coarse, pos, N, st);
 }
 
 int train_bg_backward_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, int sh_deg, int precision,
@@ -978,19 +937,16 @@ int train_bg_backward_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, int64_t N, in
     int rc;
     if ((rc = check_train_bg(ctx, m, bg, N, Sc, Sf, precision, bg_precision, name))) return rc;
     if (N == 0) return MN_OK;
-    const bool sh = sh_deg >= 0;
-    const BgTrainPlan p = make_bg_train_plan(m, bg, N, Sc, Sf, use_cascade, sh, precision == MN_PREC_TC_F16,
+    const BgTrainPlan p = make_bg_train_plan(m, bg, N, Sc, Sf, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
                                              bg_precision == MN_PREC_TC_F16);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
     if (!workspace_d || workspace_bytes < p.bwd_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     const char* T = (const char*)tape_d;
     char* W = (char*)workspace_d;
-    auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<const float*>(T + off); };
-    auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
+    auto TF = [&](size_t off) { return reinterpret_cast<const float*>(T + off); };
+    auto WF = [&](size_t off) { return reinterpret_cast<float*>(W + off); };
     const int* pos = reinterpret_cast<const int*>(T + p.pos);
-    const int* cnt = reinterpret_cast<const int*>(T + p.count);
-    const LiveRows lr{cnt, 1};
-    const bool coarse = !use_cascade || g_rgb_coarse;     // the coarse queries have a gradient
+    const bool coarse = use_cascade && g_rgb_coarse;      // the cascade's coarse type has a gradient
 
     // ---- blend backward: the background colours' and bg_lambda's gradients
     auto blend_bwd = [&](const float* g, size_t lam, size_t bval, size_t g_lam, size_t g_bg) -> int {
@@ -999,41 +955,18 @@ int train_bg_backward_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, int64_t N, in
         return MN_OK;
     };
     if ((rc = blend_bwd(g_rgb, p.lam, p.rgb_b, p.g_lam, p.g_rgb_b))) return rc;
-    if (use_cascade && coarse && (rc = blend_bwd(g_rgb_coarse, p.lam_c, p.rgb_cb, p.g_lam_c, p.g_rgb_cb))) return rc;
+    if (coarse && (rc = blend_bwd(g_rgb_coarse, p.lam_c, p.rgb_cb, p.g_lam_c, p.g_rgb_cb))) return rc;
 
     // ---- foreground: composites (with bg_lambda) and model backwards
-    if ((rc = train_fg_backward(ctx, m, p.fg, T, W, N, use_cascade, sh_deg, g_rgb, g_rgb_coarse, WF(p.g_lam),
-                                use_cascade && coarse ? WF(p.g_lam_c) : nullptr, gw, st)))
+    const float* dirs = p.fg.rays == kNone ? nullptr : TF(p.fg.rays) + 3;
+    if ((rc = train_two_pass_backward(ctx, m, precision, p.fg.pass, T, W, N, nullptr, use_cascade, sh_deg, TF(p.fg.last_delta), dirs, 8,
+                                      g_rgb, g_rgb_coarse, WF(p.g_lam), coarse ? WF(p.g_lam_c) : nullptr, gw, st)))
         return rc;
 
     // ---- background: composites, then the model backwards over the live rows
-    if (use_cascade) {
-        if ((rc = mn_stage_composite_backward(ctx, TF(p.raw_f), TF(p.z_qc), p.Sq, nullptr, nullptr, 0, TF(p.ld_b), N, 1, lr, WF(p.g_rgb_b),
-                                              nullptr, WF(p.g_raw_f), nullptr, st)))
-            return rc;
-        if (coarse && (rc = mn_stage_composite_backward(ctx, TF(p.raw_c), TF(p.z_cc), p.S, nullptr, nullptr, 0, TF(p.ld_b), N, 1, lr,
-                                                        WF(p.g_rgb_cb), nullptr, WF(p.g_raw_c), nullptr, st)))
-            return rc;
-    } else if ((rc = mn_stage_composite_backward(ctx, TF(p.raw_f), TF(p.z_qc), p.Sq, TF(p.raw_c), TF(p.z_cc), p.S, TF(p.ld_b), N, 1, lr,
-                                                 WF(p.g_rgb_b), nullptr, WF(p.g_raw_f), WF(p.g_raw_c), st))) {
-        return rc;
-    }
-    auto model_bwd = [&](int S, int use_coarse, size_t mlp, size_t g_raw, size_t g_mlp, size_t tape, size_t tape_n) -> int {
-        const LiveRows lrs{cnt, S};
-        const float* g = WF(g_raw);
-        int r;
-        if (sh) {
-            if ((r = mn_stage_sh_to_rgb_backward(ctx, sh_deg, TF(mlp), bg->nd.rgb_dim + 1, TF(p.dirs), 3, S, N * S, 1, lrs, g, WF(g_mlp),
-                                                 st)))
-                return r;
-            g = WF(g_mlp);
-        }
-        return mn_model_backward_live(ctx, bg, N * S, lrs, use_coarse, bg_precision, g, T + tape, tape_n, gw_bg, W + p.bwd_ws,
-                                      p.bwd_ws_bytes, st);
-    };
-    if ((rc = model_bwd(p.Sq, 0, p.mlp_f, p.g_raw_f, p.g_mlp_f, p.tape_f, p.tape_f_bytes))) return rc;
-    if (coarse) return model_bwd(p.S, 1, p.mlp_c, p.g_raw_c, p.g_mlp_c, p.tape_c, p.tape_c_bytes);
-    return MN_OK;
+    return train_two_pass_backward(ctx, bg, bg_precision, p.bg, T, W, N, reinterpret_cast<const int*>(T + p.count), use_cascade, sh_deg,
+                                   TF(p.ld_b), TF(p.dirs), 3, WF(p.g_rgb_b), coarse ? WF(p.g_rgb_cb) : nullptr, nullptr, nullptr,
+                                   gw_bg, st);
 }
 
 }  // namespace

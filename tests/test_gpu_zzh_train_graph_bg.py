@@ -71,22 +71,27 @@ def both_grads(pn, pb):
     return grads_of(pn), grads_of(pb)
 
 
-def stage_step(pn, pb, rays, idx, hp, target, seed):
+def fine_loss(res, target, hp):
+    """The MSE of rgb_fine alone: a Cascade's rgb_coarse gets no gradient (the one call's backward takes grad_rgb_coarse NULL)."""
+    return torch.nn.functional.mse_loss(res['rgb_fine'], target)
+
+
+def stage_step(pn, pb, rays, idx, hp, target, seed, loss=photo_loss):
     pn.zero_grad(set_to_none=True)
     pb.zero_grad(set_to_none=True)
     torch.manual_seed(seed)
     res, _ = M().render_rays(pn, pb, rays, idx, hp, CENTER.to(DEV), RADIUS.to(DEV), True, True, True)
-    photo_loss(res, target, hp).backward()
+    loss(res, target, hp).backward()
     return res, both_grads(pn, pb)
 
 
-def one_call_step(pn, pb, rays, idx, hp, target, seed):
+def one_call_step(pn, pb, rays, idx, hp, target, seed, loss=photo_loss):
     pn.zero_grad(set_to_none=True)
     pb.zero_grad(set_to_none=True)
     torch.manual_seed(seed)
     res = M().render_rays_train(pn, rays, idx, hp, True, True, bg_nerf=pb, sphere_center=CENTER.to(DEV),
                                 sphere_radius=RADIUS.to(DEV), get_bg_fg_rgb=True)
-    photo_loss(res, target, hp).backward()
+    loss(res, target, hp).backward()
     return res, both_grads(pn, pb)
 
 
@@ -111,22 +116,30 @@ def assert_grads_like_stage(got, want, again, prec, tag):
 
 
 @pytest.mark.parametrize('how', ['half', 'none', 'all'])
-@pytest.mark.parametrize('name,prec', CASES)
+# 'cascade:fine_loss': the Cascade trained on rgb_fine alone, whose backward skips both networks' coarse passes
+@pytest.mark.parametrize('name,prec', CASES + [('cascade:fine_loss', p) for p in SHAPES['cascade'][-1]])
 def test_eager_equals_the_stage_path(name, prec, how, train_precision):
     train_precision(prec)
-    net, bg, rays, idx, hp = make_case(name)
+    shape, _, fine_only = name.partition(':')
+    loss = fine_loss if fine_only else photo_loss
+    net, bg, rays, idx, hp = make_case(shape)
     rays = split(rays, how)
     pn, pb = trainable(net), trainable(bg)
     target = torch.rand(rays.shape[0], 3, generator=torch.Generator().manual_seed(2)).to(DEV)
-    res_s, (gs, gsb) = stage_step(pn, pb, rays, idx, hp, target, 7)
-    res_o, (go, gob) = one_call_step(pn, pb, rays, idx, hp, target, 7)
+    res_s, (gs, gsb) = stage_step(pn, pb, rays, idx, hp, target, 7, loss)
+    res_o, (go, gob) = one_call_step(pn, pb, rays, idx, hp, target, 7, loss)
     assert pn._native().train_on_tensor_cores() == (prec == 'tc_f16') == pb._native().train_on_tensor_cores()
     assert list(res_o) == list(res_s)
     for k in res_s:
         assert torch.equal(res_o[k], res_s[k]), (name, prec, how, k, float((res_o[k] - res_s[k]).abs().max()))
     if how == 'none':
         assert not gsb and not gob                  # no background ray: no gradient for the background, as on the stage path
-    _, (gs2, gsb2) = stage_step(pn, pb, rays, idx, hp, target, 7)
+    _, (gs2, gsb2) = stage_step(pn, pb, rays, idx, hp, target, 7, loss)
+    if fine_only:
+        # the stage path gives the coarse networks no gradient, the one call's gradient block an exactly zero one
+        for got, want in ((go, gs), (gob, gsb)):
+            for k in set(got) - set(want):
+                assert not got.pop(k).any(), (name, prec, how, k)
     assert_grads_like_stage(go, gs, gs2, prec, f'{name} {prec} {how} foreground')
     assert_grads_like_stage(gob, gsb, gsb2, prec, f'{name} {prec} {how} background')
 
