@@ -574,6 +574,63 @@ int mn_render_rays_train_bg_backward(mn_ctx* ctx, mn_model* fg, mn_model* bg, in
                                      const float* grad_rgb_coarse_d, const void* tape_d, size_t tape_bytes, float* param_grads_d,
                                      float* bg_param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream);
 
+/* ---- the training renders through an occupancy grid (an approximate training mode the caller opts into) -------------------
+ * mn_render_rays_train / mn_render_rays_train_bg, except that the foreground samples of both passes that the grid skips (the
+ * grid, the cell test and the frame of mn_render_rays_occ) are not queried: their raw row [rgb, sigma] (after the SH head, for
+ * one) is exactly (0, 0, 0, 0), and every later stage - the coarse composite and the resampling weights, the fine draws (tested
+ * and skipped the same way), the merge, the final composite, the background pass (never masked) and the blend - runs unchanged on
+ * it.  A skipped sample reaches no parameter: the backward runs the composite backward(s) over every sample, then the SH head's
+ * and the model's backward over the queried rows only, so every gradient equals that of the stage path with the skipped raw rows
+ * replaced by zero.  The random inputs are those of the unmasked call, drawn for every sample (density noise [N * S] in sample
+ * order); a queried sample uses its own draw.  With every bit set the results equal those of mn_render_rays_train(_bg).
+ * The queried samples are compacted on the device and their count stays there: no host sync, the launch sequence depends on N
+ * only (CUDA-graph capturable).  counts_out_d: NULL, or int32 [2] receiving the queried foreground rows of the coarse [0] and the
+ * fine [1] pass.  N * max(coarse_samples, Sq) must stay below 2^31; reso 1 .. MN_OCC_MAX_RESO.  The grid is read during the
+ * forward call only.  The tape also holds each pass's compacted sample indices and counts, so the size queries and the backward
+ * take the unmasked call's arguments and need no grid; a tape written by an _occ call is consumed by the _occ backward only. */
+size_t mn_render_rays_train_occ_tape_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                           int sh_deg, int precision);
+size_t mn_render_rays_train_occ_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                                int sh_deg, int precision);
+int mn_render_rays_train_occ(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N,
+                             const float* z_steps_d, const float* jitter_d, float perturb, int coarse_samples,
+                             const float* sigma_noise_coarse_d, const float* u_fine_d, const float* sigma_noise_fine_d, int fine_samples,
+                             int use_cascade, int sh_deg, int precision, const mn_occupancy* occ, int32_t* counts_out_d, float* rgb_out_d,
+                             float* depth_out_d, float* depth_var_out_d, float* rgb_coarse_out_d, void* tape_d, size_t tape_bytes,
+                             void* workspace_d, size_t workspace_bytes, void* stream);
+size_t mn_render_rays_train_occ_backward_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples,
+                                                         int use_cascade, int sh_deg, int precision);
+int mn_render_rays_train_occ_backward(mn_ctx* ctx, mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                      int sh_deg, int precision, const float* grad_rgb_d, const float* grad_rgb_coarse_d,
+                                      const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d,
+                                      size_t workspace_bytes, void* stream);
+size_t mn_render_rays_train_bg_occ_tape_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                              int use_cascade, int sh_deg, int precision, int bg_precision);
+size_t mn_render_rays_train_bg_occ_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples,
+                                                   int fine_samples, int use_cascade, int sh_deg, int precision, int bg_precision);
+int mn_render_rays_train_bg_occ(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays_d, const float* image_indices_d, int64_t N,
+                                const float* sphere_center3_d, const float* sphere_radius3_d, int include_xyz_real, int cluster_2d,
+                                const float* z_steps_d, const float* z_steps_bg_d, const float* jitter_d, const float* jitter_bg_d,
+                                float perturb, int coarse_samples, const float* sigma_noise_coarse_d,
+                                const float* sigma_noise_coarse_bg_d, const float* u_fine_d, const float* u_fine_bg_d,
+                                const float* sigma_noise_fine_d, const float* sigma_noise_fine_bg_d, int fine_samples, int use_cascade,
+                                int sh_deg, int precision, int bg_precision, const mn_occupancy* occ, int32_t* counts_out_d,
+                                int bg_draws_by_ray, const mn_render_outputs* out, void* tape_d, size_t tape_bytes, void* workspace_d,
+                                size_t workspace_bytes, void* stream);
+size_t mn_render_rays_train_bg_occ_backward_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples,
+                                                            int fine_samples, int use_cascade, int sh_deg, int precision,
+                                                            int bg_precision);
+int mn_render_rays_train_bg_occ_backward(mn_ctx* ctx, mn_model* fg, mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                         int use_cascade, int sh_deg, int precision, int bg_precision, const float* grad_rgb_d,
+                                         const float* grad_rgb_coarse_d, const void* tape_d, size_t tape_bytes, float* param_grads_d,
+                                         float* bg_param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream);
+
+/* mn_occupancy_pack: bits_d [ceil(n / 32)] = the occupancy words of n cells, cell c occupied iff sigmas_d[c] >= thresh (a NaN sigma
+ * gives an empty cell), in mn_occupancy's layout (bit c & 31 of word c >> 5; the bits past n are 0).  One warp ballot per word, no
+ * atomics, no host sync: refreshes a grid in place, e.g. from mn_model_density_grid's sigmas, between replays of a captured graph
+ * that reads it. */
+int mn_occupancy_pack(mn_ctx* ctx, const float* sigmas_d, int64_t n, float thresh, uint32_t* bits_d, void* stream);
+
 /* ---- test hook (host only, no CUDA call) ---------------------------------------------------------------------------
  * The stage program of the tensor-core MLP kernel (csrc/mn_mlp_wg.cuh, precision tc_f16) for one network shape: `desc` as for
  * mn_model_create (only the per-sub-module fields matter).  The producer and both consumer warpgroups walk this program, one

@@ -146,6 +146,19 @@ SIGNATURES = {
                                      _I, _I, _I, _I, C.POINTER(RenderOutputs), _P, _Z, _P, _Z, _P]),
     'mn_render_rays_train_bg_backward_workspace_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I, _I]),
     'mn_render_rays_train_bg_backward': (_I, [_P, _P, _P, _L, _I, _I, _I, _I, _I, _I, _P, _P, _P, _Z, _P, _P, _P, _Z, _P]),
+    'mn_render_rays_train_occ_tape_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_occ_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_occ': (_I, [_P, _P, _P, _P, _L, _P, _P, _F, _I, _P, _P, _P, _I, _I, _I, _I, C.POINTER(Occupancy), _P, _P,
+                                      _P, _P, _P, _P, _Z, _P, _Z, _P]),
+    'mn_render_rays_train_occ_backward_workspace_bytes': (_Z, [_P, _L, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_occ_backward': (_I, [_P, _P, _L, _I, _I, _I, _I, _I, _P, _P, _P, _Z, _P, _P, _Z, _P]),
+    'mn_render_rays_train_bg_occ_tape_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_bg_occ_workspace_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_bg_occ': (_I, [_P, _P, _P, _P, _P, _L, _P, _P, _I, _I, _P, _P, _P, _P, _F, _I, _P, _P, _P, _P, _P, _P, _I,
+                                         _I, _I, _I, _I, C.POINTER(Occupancy), _P, _I, C.POINTER(RenderOutputs), _P, _Z, _P, _Z, _P]),
+    'mn_render_rays_train_bg_occ_backward_workspace_bytes': (_Z, [_P, _P, _L, _I, _I, _I, _I, _I, _I]),
+    'mn_render_rays_train_bg_occ_backward': (_I, [_P, _P, _P, _L, _I, _I, _I, _I, _I, _I, _P, _P, _P, _Z, _P, _P, _P, _Z, _P]),
+    'mn_occupancy_pack': (_I, [_P, _P, _L, _F, _P, _P]),
     'mn_debug_tc_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),
     'mn_debug_tc_forward_record': (_I, [_P, _P, C.POINTER(Rows), _L, _I, _P, _P, _P, _Z, _P, _Z, _P]),
     'mn_debug_fp32_train_layout': (_I, [_P, _L, C.POINTER(_L), _I]),

@@ -128,10 +128,12 @@ def _grad_block(block: Optional[torch.Tensor], native, dev) -> torch.Tensor:
 class RenderTrainCall:
     """One mn_render_rays_train call: its inputs (the random draws included), then its tape until the backward consumed it.
     grads: None (the backward allocates the gradient block), or a caller's fp32 block of mn_model_grad_floats floats that the
-    backward zeroes and accumulates into, so that the parameters' gradients are views at a fixed address (GraphedTrainStep)."""
+    backward zeroes and accumulates into, so that the parameters' gradients are views at a fixed address (GraphedTrainStep).
+    occupancy: None, or an octree.OccupancyGrid through which the call queries (mn_render_rays_train_occ and its backward);
+    counts: None, or the int32 [2] tensor that receives the queried foreground rows of each pass."""
 
     def __init__(self, native, rays, idx, steps, jitter, perturb, noise_c, u, noise_f, Sc, Sf, cascade, sh_deg, get_depth,
-                 get_depth_variance, grads=None):
+                 get_depth_variance, grads=None, occupancy=None, counts=None):
         self.native, self.rays, self.idx, self.steps, self.jitter, self.perturb = native, rays, idx, steps, jitter, perturb
         self.noise_c, self.u, self.noise_f = noise_c, u, noise_f
         self.Sc, self.Sf, self.cascade, self.sh_deg = Sc, Sf, cascade, sh_deg
@@ -139,13 +141,18 @@ class RenderTrainCall:
         # the recording kernels of set_train_precision where they cover the network (NativeModel.train_on_tensor_cores)
         self.prec = K.PREC_TC_F16 if native.train_on_tensor_cores() else K.PREC_FP32
         self.grads = grads
+        self.occupancy, self.counts = occupancy, counts
         self.tape = None
 
     def _sizes(self):
         return (self.native.handle, self.rays.shape[0], self.Sc, self.Sf, int(self.cascade), self.sh_deg, self.prec)
 
+    def _fn(self, name: str):
+        """The entry point `name` of this call's mode: mn_render_rays_train_* or, through a grid, mn_render_rays_train_occ_*."""
+        return getattr(K.lib(), name.replace('mn_render_rays_train', 'mn_render_rays_train_occ') if self.occupancy is not None else name)
+
     def forward(self):
-        L, dev = K.lib(), self.rays.device
+        dev = self.rays.device
         h = K.ctx(dev)
         N = self.rays.shape[0]
         new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
@@ -153,25 +160,28 @@ class RenderTrainCall:
         rgb_coarse = new(N, 3) if self.cascade else None
         depth = new(N) if self.get_depth else None
         var = new(N) if self.get_depth_variance else None
-        self.tape = torch.empty(max(int(L.mn_render_rays_train_tape_bytes(*self._sizes())), 256), device=dev, dtype=torch.uint8)
-        ws = torch.empty(max(int(L.mn_render_rays_train_workspace_bytes(*self._sizes())), 256), device=dev, dtype=torch.uint8)
-        K.check(L.mn_render_rays_train(h, self.native.handle, K.ptr(self.rays), K.ptr(self.idx), N, K.ptr(self.steps),
-                                       K.ptr(self.jitter), self.perturb, self.Sc, K.ptr(self.noise_c), K.ptr(self.u),
-                                       K.ptr(self.noise_f), self.Sf, int(self.cascade), self.sh_deg, self.prec, K.ptr(rgb),
-                                       K.ptr(depth), K.ptr(var), K.ptr(rgb_coarse), K.ptr(self.tape), self.tape.numel(), K.ptr(ws),
-                                       ws.numel(), K.stream_of(dev)), h)
+        self.tape = torch.empty(max(int(self._fn('mn_render_rays_train_tape_bytes')(*self._sizes())), 256), device=dev,
+                                dtype=torch.uint8)
+        ws = torch.empty(max(int(self._fn('mn_render_rays_train_workspace_bytes')(*self._sizes())), 256), device=dev, dtype=torch.uint8)
+        args = [h, self.native.handle, K.ptr(self.rays), K.ptr(self.idx), N, K.ptr(self.steps), K.ptr(self.jitter), self.perturb,
+                self.Sc, K.ptr(self.noise_c), K.ptr(self.u), K.ptr(self.noise_f), self.Sf, int(self.cascade), self.sh_deg, self.prec]
+        if self.occupancy is not None:
+            args += [C.byref(self.occupancy.cabi()), K.ptr(self.counts)]
+        args += [K.ptr(rgb), K.ptr(depth), K.ptr(var), K.ptr(rgb_coarse), K.ptr(self.tape), self.tape.numel(), K.ptr(ws), ws.numel(),
+                 K.stream_of(dev)]
+        K.check(self._fn('mn_render_rays_train')(*args), h)
         return rgb, rgb_coarse, depth, var
 
     def backward(self, g_rgb, g_rgb_coarse, params):
-        L, dev = K.lib(), self.rays.device
+        dev = self.rays.device
         h = K.ctx(dev)
         N = self.rays.shape[0]
         gbuf = _grad_block(self.grads, self.native, dev)
-        ws = torch.empty(max(int(L.mn_render_rays_train_backward_workspace_bytes(*self._sizes())), 256), device=dev,
+        ws = torch.empty(max(int(self._fn('mn_render_rays_train_backward_workspace_bytes')(*self._sizes())), 256), device=dev,
                          dtype=torch.uint8)
         g_rgb = K.f32c(g_rgb) if g_rgb is not None else torch.zeros(N, 3, device=dev, dtype=torch.float32)
         g_rgb_coarse = K.f32c(g_rgb_coarse) if g_rgb_coarse is not None else None
-        K.check(L.mn_render_rays_train_backward(h, self.native.handle, N, self.Sc, self.Sf, int(self.cascade), self.sh_deg,
+        K.check(self._fn('mn_render_rays_train_backward')(h, self.native.handle, N, self.Sc, self.Sf, int(self.cascade), self.sh_deg,
                                                 self.prec, K.ptr(g_rgb), K.ptr(g_rgb_coarse), K.ptr(self.tape), self.tape.numel(),
                                                 K.ptr(gbuf), K.ptr(ws), ws.numel(), K.stream_of(dev)), h)
         self.tape = None
@@ -211,11 +221,11 @@ class RenderTrainBgCall:
     """One mn_render_rays_train_bg call: its inputs (the random draws of both networks included), its outputs, then its tape until
     the backward consumed it.  bg_grads: whether the background parameters receive a gradient (eager, no background ray and no
     dummy ray: None, as on the stage path).  grads: None, or the (foreground, background) blocks to accumulate into, as for
-    RenderTrainCall."""
+    RenderTrainCall.  occupancy / counts: as for RenderTrainCall (mn_render_rays_train_bg_occ and its backward)."""
 
     def __init__(self, native, bnative, rays, idx, center, radius, real, c2d, steps, steps_bg, jitter, jitter_bg, perturb, noise_c,
                  noise_c_bg, u, u_bg, noise_f, noise_f_bg, Sc, Sf, cascade, sh_deg, by_ray, get_depth, get_depth_variance,
-                 get_bg_fg_rgb, bg_grads=True, grads=None):
+                 get_bg_fg_rgb, bg_grads=True, grads=None, occupancy=None, counts=None):
         self.native, self.bnative, self.rays, self.idx, self.center, self.radius = native, bnative, rays, idx, center, radius
         self.real, self.c2d, self.steps, self.steps_bg, self.perturb = real, c2d, steps, steps_bg, perturb
         self.draws = (jitter, jitter_bg, noise_c, noise_c_bg, u, u_bg, noise_f, noise_f_bg)
@@ -223,6 +233,7 @@ class RenderTrainBgCall:
         self.get_depth, self.get_depth_variance, self.get_bg_fg_rgb = get_depth, get_depth_variance, get_bg_fg_rgb
         self.bg_grads = bg_grads
         self.grads = grads
+        self.occupancy, self.counts = occupancy, counts
         self.prec = K.PREC_TC_F16 if native.train_on_tensor_cores() else K.PREC_FP32
         self.bprec = K.PREC_TC_F16 if bnative.train_on_tensor_cores() else K.PREC_FP32
         self.tape = None
@@ -231,9 +242,13 @@ class RenderTrainBgCall:
         return (self.native.handle, self.bnative.handle, self.rays.shape[0], self.Sc, self.Sf, int(self.cascade), self.sh_deg,
                 self.prec, self.bprec)
 
+    def _fn(self, name: str):
+        """The entry point `name` of this call's mode: mn_render_rays_train_bg_* or, through a grid, mn_render_rays_train_bg_occ_*."""
+        return getattr(K.lib(), name.replace('_train_bg', '_train_bg_occ') if self.occupancy is not None else name)
+
     def forward(self):
         """-> {result key: tensor} in mn_render_outputs' fields (rgb, rgb_coarse, depth, ...)."""
-        L, dev = K.lib(), self.rays.device
+        dev = self.rays.device
         h = K.ctx(dev)
         N = self.rays.shape[0]
         new = lambda *shape: torch.empty(*shape, device=dev, dtype=torch.float32)
@@ -252,29 +267,32 @@ class RenderTrainBgCall:
         out = K.RenderOutputs()
         for k, v in o.items():
             setattr(out, k, K.ptr(v))
-        self.tape = torch.empty(max(int(L.mn_render_rays_train_bg_tape_bytes(*self._sizes())), 256), device=dev, dtype=torch.uint8)
-        ws = torch.empty(max(int(L.mn_render_rays_train_bg_workspace_bytes(*self._sizes())), 256), device=dev, dtype=torch.uint8)
+        self.tape = torch.empty(max(int(self._fn('mn_render_rays_train_bg_tape_bytes')(*self._sizes())), 256), device=dev,
+                                dtype=torch.uint8)
+        ws = torch.empty(max(int(self._fn('mn_render_rays_train_bg_workspace_bytes')(*self._sizes())), 256), device=dev,
+                         dtype=torch.uint8)
         jitter, jitter_bg, noise_c, noise_c_bg, u, u_bg, noise_f, noise_f_bg = self.draws
-        K.check(L.mn_render_rays_train_bg(h, self.native.handle, self.bnative.handle, K.ptr(self.rays), K.ptr(self.idx), N,
-                                          K.ptr(self.center), K.ptr(self.radius), int(self.real), int(self.c2d), K.ptr(self.steps),
-                                          K.ptr(self.steps_bg), K.ptr(jitter), K.ptr(jitter_bg), self.perturb, self.Sc,
-                                          K.ptr(noise_c), K.ptr(noise_c_bg), K.ptr(u), K.ptr(u_bg), K.ptr(noise_f),
-                                          K.ptr(noise_f_bg), self.Sf, int(self.cascade), self.sh_deg, self.prec, self.bprec,
-                                          int(self.by_ray), C.byref(out), K.ptr(self.tape), self.tape.numel(), K.ptr(ws), ws.numel(),
-                                          K.stream_of(dev)), h)
+        args = [h, self.native.handle, self.bnative.handle, K.ptr(self.rays), K.ptr(self.idx), N, K.ptr(self.center),
+                K.ptr(self.radius), int(self.real), int(self.c2d), K.ptr(self.steps), K.ptr(self.steps_bg), K.ptr(jitter),
+                K.ptr(jitter_bg), self.perturb, self.Sc, K.ptr(noise_c), K.ptr(noise_c_bg), K.ptr(u), K.ptr(u_bg), K.ptr(noise_f),
+                K.ptr(noise_f_bg), self.Sf, int(self.cascade), self.sh_deg, self.prec, self.bprec]
+        if self.occupancy is not None:
+            args += [C.byref(self.occupancy.cabi()), K.ptr(self.counts)]
+        args += [int(self.by_ray), C.byref(out), K.ptr(self.tape), self.tape.numel(), K.ptr(ws), ws.numel(), K.stream_of(dev)]
+        K.check(self._fn('mn_render_rays_train_bg')(*args), h)
         return o
 
     def backward(self, g_rgb, g_rgb_coarse, params, bparams):
-        L, dev = K.lib(), self.rays.device
+        dev = self.rays.device
         h = K.ctx(dev)
         N = self.rays.shape[0]
         gbuf = _grad_block(self.grads[0] if self.grads is not None else None, self.native, dev)
         gbuf_bg = _grad_block(self.grads[1] if self.grads is not None else None, self.bnative, dev)
-        ws = torch.empty(max(int(L.mn_render_rays_train_bg_backward_workspace_bytes(*self._sizes())), 256), device=dev,
+        ws = torch.empty(max(int(self._fn('mn_render_rays_train_bg_backward_workspace_bytes')(*self._sizes())), 256), device=dev,
                          dtype=torch.uint8)
         g_rgb = K.f32c(g_rgb) if g_rgb is not None else torch.zeros(N, 3, device=dev, dtype=torch.float32)
         g_rgb_coarse = K.f32c(g_rgb_coarse) if g_rgb_coarse is not None else None
-        K.check(L.mn_render_rays_train_bg_backward(h, self.native.handle, self.bnative.handle, N, self.Sc, self.Sf, int(self.cascade),
+        K.check(self._fn('mn_render_rays_train_bg_backward')(h, self.native.handle, self.bnative.handle, N, self.Sc, self.Sf, int(self.cascade),
                                                    self.sh_deg, self.prec, self.bprec, K.ptr(g_rgb), K.ptr(g_rgb_coarse),
                                                    K.ptr(self.tape), self.tape.numel(), K.ptr(gbuf), K.ptr(gbuf_bg), K.ptr(ws),
                                                    ws.numel(), K.stream_of(dev)), h)

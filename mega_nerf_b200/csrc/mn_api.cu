@@ -1160,10 +1160,11 @@ int mn_model_backward_assigned(mn_ctx* ctx, mn_model* m, int64_t n, int64_t max_
 
 int mn_model_forward_train_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse,
                                 const float* sigma_noise_d, int precision, float* out_d, void* tape_d, size_t tape_bytes,
-                                void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
+                                void* workspace_d, size_t workspace_bytes, cudaStream_t st, const int* gather) {
     if (!tape_d) return mn_fail(ctx, MN_ERR_INVALID, "mn_model_forward_train: tape is NULL");
     if (precision == MN_PREC_TC_F16 && !mn_model_train_tc_supported(m)) return mn_fail(ctx, MN_ERR_UNSUPPORTED, MN_TC_TRAIN_COVERAGE);
     ModelCall c;
+    c.src.gather = gather;
     c.B = B;
     c.use_coarse = use_coarse;
     c.live = live;

@@ -257,10 +257,11 @@ int mn_model_forward_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t
                           float* out_d, void* workspace_d, size_t workspace_bytes, cudaStream_t st, const int* gather = nullptr);
 // The recording forward (mn_model_forward_train(_tc), precision MN_PREC_FP32 / MN_PREC_TC_F16) and its backward (mn_model_backward(_tc))
 // over the first live.rows(B) of B rows, with the tape and workspaces of B rows: no slot at or past the live rows is encoded,
-// recorded or contracted into a weight gradient, and rows of grad_out past them are never read.
+// recorded or contracted into a weight gradient, and rows of grad_out past them are never read.  gather: as for
+// mn_model_forward_live; sigma_noise_d, the tape and grad_out are indexed by gathered row r, not by sample.
 int mn_model_forward_train_live(mn_ctx* ctx, mn_model* m, const mn_rows* rows, int64_t B, LiveRows live, int use_coarse,
                                 const float* sigma_noise_d, int precision, float* out_d, void* tape_d, size_t tape_bytes,
-                                void* workspace_d, size_t workspace_bytes, cudaStream_t st);
+                                void* workspace_d, size_t workspace_bytes, cudaStream_t st, const int* gather = nullptr);
 int mn_model_backward_live(mn_ctx* ctx, mn_model* m, int64_t B, LiveRows live, int use_coarse, int precision, const float* grad_out_d,
                            const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d, size_t workspace_bytes,
                            cudaStream_t st);
@@ -290,7 +291,7 @@ int mn_stage_composite_backward(mn_ctx* ctx, const float* raw_d, const float* z_
                                 const float* grad_lambda_d, float* grad_raw_d, float* grad_raw2_d, cudaStream_t st);
 int mn_stage_sh_to_rgb_backward(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
                                 int dir_div, int64_t B, int apply_sigmoid, LiveRows live, const float* grad_out_d, float* grad_coef_d,
-                                cudaStream_t st);
+                                cudaStream_t st, const int* gather = nullptr);   // gather: as for mn_stage_sh_to_rgb
 int mn_mlp_simt_launch(mn_ctx* ctx, const MlpArgs& a, int64_t n_tiles128, cudaStream_t st);
 int mn_mlp_bwd_launch(mn_ctx* ctx, const BwdArgs& a, int64_t n_tiles128, cudaStream_t st);
 int mn_mlp_tc_launch(mn_ctx* ctx, mn_model* m, const MlpArgs& a, int64_t n_tiles128, int precision, void* ws,

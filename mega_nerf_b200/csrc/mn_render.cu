@@ -157,14 +157,19 @@ __global__ void __launch_bounds__(kCompactBlock) occ_test_kernel(const float* __
 }
 
 // Stable compaction of the queried samples: idx[0 .. count) = their flat indices in ascending order, pos[s] = the compacted row
-// of sample s or -1, *count (and *count_out if given) = the queried samples (written by the last block).
+// of sample s or -1, *count (and *count_out if given) = the queried samples (written by the last block).  noise_cmp (training,
+// when given): noise_cmp[p] = noise[idx[p]], the density noise of each queried sample at its compacted row, where the MLP reads it.
 __global__ void __launch_bounds__(kCompactBlock) occ_compact_kernel(int64_t n, const int* __restrict__ blk, int* __restrict__ pos,
                                                                     int* __restrict__ idx, int* __restrict__ count,
-                                                                    int* __restrict__ count_out) {
+                                                                    int* __restrict__ count_out, const float* __restrict__ noise,
+                                                                    float* __restrict__ noise_cmp) {
     const int64_t s = (int64_t)blockIdx.x * kCompactBlock + threadIdx.x;
     const int p = compact_block_scan(blk, s < n && pos[s] != 0, count, count_out);
     if (s >= n) return;
-    if (p >= 0) idx[p] = (int)s;
+    if (p >= 0) {
+        idx[p] = (int)s;
+        if (noise_cmp) noise_cmp[p] = noise[s];
+    }
     pos[s] = p;
 }
 
@@ -174,6 +179,14 @@ __global__ void occ_scatter_kernel(const float4* __restrict__ cmp, const int* __
     if (s >= n) return;
     const int p = pos[s];
     raw[s] = p >= 0 ? cmp[p] : make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+}
+
+// bits[w] = the cells 32 w .. 32 w + 31 with sigma >= thresh (mn_occupancy_pack): lane l of a warp holds cell 32 w + l, so the
+// ballot is the word; cells past n are empty.
+__global__ void occ_pack_kernel(const float* __restrict__ sigma, int64_t n, float thresh, uint32_t* __restrict__ bits) {
+    const int64_t c = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned word = __ballot_sync(0xffffffffu, c < n && sigma[c] >= thresh);
+    if ((threadIdx.x & 31) == 0 && c < n) bits[c >> 5] = word;
 }
 
 // Workspace offsets: each buffer aligned on its own.
@@ -391,7 +404,7 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
         occ_test_kernel<<<nblk, kCompactBlock, 0, st>>>(xyz, n, G, I(p.occ_pos), I(p.occ_blk));
         MN_LAUNCH_CHECK(ctx);
         occ_compact_kernel<<<nblk, kCompactBlock, 0, st>>>(n, I(p.occ_blk), I(p.occ_pos), I(p.occ_idx), cnt,
-                                                           counts_out_d ? counts_out_d + pass : nullptr);
+                                                           counts_out_d ? counts_out_d + pass : nullptr, nullptr, nullptr);
         MN_LAUNCH_CHECK(ctx);
         mn_rows rows{};
         rows.mode = 1;
@@ -507,16 +520,22 @@ int render_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, con
 // order where they differ (z_c, z_q; kNone: the composite's buffer), the points and, with flip, their real depths, the weights, the
 // fine draws before sort_cat (z_f; kNone: the fine-query depths) and the model calls' workspace.  The backward workspace holds the
 // per-sample gradients and the model backward's workspace.
+// A pass masked by an occupancy grid (occ_idx_c != kNone) runs each model call on its queried samples only, compacted: the tape
+// also holds each query's compacted sample indices (occ_idx_c / occ_idx_f) and the two queried-row counts (occ_cnt), and the model
+// tapes and raw SH coefficients are in compacted order.  The workspace holds the test flags / compacted positions, the block
+// counts, the compacted results and the compacted density noise; the backward workspace the compacted result gradients.
 struct TrainPassBufs {
     int S, F, Sq, cols, flip;
     size_t z_c_comp, raw_c, z_q_comp, raw_f, mlp_c, mlp_f, tape_c, tape_f, tape_c_bytes, tape_f_bytes;
     size_t z_c, z_q, z_f, xyz_c, dreal_c, w_c, xyz_f, dreal_f, model_ws, model_ws_bytes;
     size_t g_raw_c, g_raw_f, g_mlp_c, g_mlp_f, bwd_ws, bwd_ws_bytes;
+    size_t occ_idx_c = kNone, occ_idx_f = kNone, occ_cnt = kNone, occ_pos, occ_blk, occ_out, occ_noise, g_cmp;
 };
 
-// tc: the network trains at MN_PREC_TC_F16 (the model tapes and the backward workspace of the tensor-core pass)
+// tc: the network trains at MN_PREC_TC_F16 (the model tapes and the backward workspace of the tensor-core pass); occ: the pass
+// is masked by an occupancy grid
 TrainPassBufs carve_train_pass(Carve& tape, Carve& ws, Carve& bwd, const mn_model* net, int64_t N, int S, int F, int use_cascade,
-                               bool sh, int cols, bool flip, bool tc) {
+                               bool sh, int cols, bool flip, bool tc, bool occ = false) {
     TrainPassBufs b{};
     b.S = S; b.F = F; b.Sq = use_cascade ? S + F : F; b.cols = cols; b.flip = flip;
     const int64_t Bc = N * S, Bf = N * b.Sq;
@@ -550,6 +569,17 @@ TrainPassBufs carve_train_pass(Carve& tape, Carve& ws, Carve& bwd, const mn_mode
     const size_t bc = tc ? mn_model_backward_workspace_bytes_tc(net, Bf) : mn_model_backward_workspace_bytes(net, Bf);
     b.bwd_ws_bytes = ba > bc ? ba : bc;
     b.bwd_ws = bwd(b.bwd_ws_bytes);
+    if (occ) {
+        const int64_t rows = Bc > Bf ? Bc : Bf;
+        b.occ_idx_c = tape((size_t)Bc * 4);
+        b.occ_idx_f = tape((size_t)Bf * 4);
+        b.occ_cnt = tape(2 * 4);
+        b.occ_pos = ws((size_t)rows * 4);
+        b.occ_blk = ws((size_t)mn_cdiv(rows, kCompactBlock) * 4);
+        b.occ_out = ws((size_t)rows * 16);
+        b.occ_noise = ws((size_t)rows * 4);
+        b.g_cmp = bwd((size_t)rows * 16);
+    }
     return b;
 }
 
@@ -559,11 +589,12 @@ TrainPassBufs carve_train_pass(Carve& tape, Carve& ws, Carve& bwd, const mn_mode
 // the same weights), resampling, sort_cat under cascade, the fine points, the recording fine query and the final composite.
 // live: the device count of the rays that hold data (background pass), or null for all N.  u, noise_c, noise_f: the fine draws
 // and the density noise.  dirs / dstride, idx: per ray.  r and fine_points(z, S, flip_pts, xyz, dreal): as two_pass's.
+// A pass carved with an occupancy grid queries through `occ` (query_occ of render_impl, recording); counts_out: as there.
 template <class Points>
 int train_two_pass(mn_ctx* ctx, mn_model* net, int precision, const TrainPassBufs& b, char* T, char* W, int64_t N, const int* live,
                    int use_cascade, int sh_deg, const float* last_delta, const float* u, const float* noise_c, const float* noise_f,
                    const float* dirs, int64_t dstride, const float* idx, const mn_render_outputs& r, Points&& fine_points,
-                   cudaStream_t st) {
+                   cudaStream_t st, const OccGrid* occ = nullptr, int* counts_out = nullptr) {
     auto TF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(T + off); };
     auto WF = [&](size_t off) { return off == kNone ? nullptr : reinterpret_cast<float*>(W + off); };
     const LiveRows lr{live, 1};
@@ -590,9 +621,49 @@ int train_two_pass(mn_ctx* ctx, mn_model* net, int precision, const TrainPassBuf
         if (sh) return mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, net->nd.rgb_dim + 1, dirs, dstride, S, N * S, 1, lrs, raw_out, st);
         return MN_OK;
     };
+    // The same through the occupancy grid: test and compaction of the N * S samples (their indices and count into the tape at
+    // idx_off / b.occ_cnt + pass, each queried sample's noise to its compacted row), the recording model call and the SH head on
+    // the compacted rows, then every raw row from them or zero.  pass: 0 coarse, 1 fine.
+    auto query_occ = [&](const float* xyz, int S, int coarse, const float* noise, float* mlp_out, float* raw_out, size_t tape,
+                         size_t tape_n, size_t idx_off, int pass) -> int {
+        const int64_t n = N * S;
+        const unsigned nblk = (unsigned)mn_cdiv(n, kCompactBlock);
+        int* pos = reinterpret_cast<int*>(W + b.occ_pos);
+        int* blk = reinterpret_cast<int*>(W + b.occ_blk);
+        int* gather = reinterpret_cast<int*>(T + idx_off);
+        int* cnt = reinterpret_cast<int*>(T + b.occ_cnt) + pass;
+        float* noise_cmp = noise ? WF(b.occ_noise) : nullptr;
+        occ_test_kernel<<<nblk, kCompactBlock, 0, st>>>(xyz, n, *occ, pos, blk);
+        MN_LAUNCH_CHECK(ctx);
+        occ_compact_kernel<<<nblk, kCompactBlock, 0, st>>>(n, blk, pos, gather, cnt, counts_out ? counts_out + pass : nullptr, noise,
+                                                           noise_cmp);
+        MN_LAUNCH_CHECK(ctx);
+        mn_rows rows{};
+        rows.mode = 1;
+        rows.x_d = xyz;
+        rows.cols = b.cols;
+        rows.dirs_d = net->d.pos_dir_dim > 0 ? dirs : nullptr;
+        rows.dir_stride = dstride;
+        rows.idx_d = net->d.appearance_dim > 0 ? idx : nullptr;
+        rows.samples_per_ray = S;
+        const LiveRows lrs{cnt, 1};
+        float* cmp = WF(b.occ_out);
+        int e = mn_model_forward_train_live(ctx, net, &rows, n, lrs, coarse, noise_cmp, precision, sh ? mlp_out : cmp, T + tape, tape_n,
+                                            W + b.model_ws, b.model_ws_bytes, st, gather);
+        if (e) return e;
+        if (sh && (e = mn_stage_sh_to_rgb(ctx, sh_deg, mlp_out, net->nd.rgb_dim + 1, dirs, dstride, S, n, 1, lrs, cmp, st, gather)))
+            return e;
+        occ_scatter_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, st>>>(reinterpret_cast<const float4*>(cmp), pos, n,
+                                                                      reinterpret_cast<float4*>(raw_out));
+        MN_LAUNCH_CHECK(ctx);
+        return MN_OK;
+    };
+    const bool masked = b.occ_idx_c != kNone;
 
     int rc;
-    if ((rc = query(WF(b.xyz_c), b.S, 1, noise_c, TF(b.mlp_c), TF(b.raw_c), b.tape_c, b.tape_c_bytes))) return rc;
+    if (masked) rc = query_occ(WF(b.xyz_c), b.S, 1, noise_c, TF(b.mlp_c), TF(b.raw_c), b.tape_c, b.tape_c_bytes, b.occ_idx_c, 0);
+    else rc = query(WF(b.xyz_c), b.S, 1, noise_c, TF(b.mlp_c), TF(b.raw_c), b.tape_c, b.tape_c_bytes);
+    if (rc) return rc;
     if ((rc = mn_stage_composite(ctx, TF(b.raw_c), TF(b.z_c_comp), WF(b.dreal_c), b.S, nullptr, nullptr, nullptr, 0, last_delta, N,
                                  b.flip, lr, WF(b.w_c), use_cascade ? r.rgb_coarse : nullptr, nullptr, nullptr,
                                  use_cascade ? r.bg_lambda_coarse : nullptr, st)))
@@ -601,7 +672,9 @@ int train_two_pass(mn_ctx* ctx, mn_model* net, int precision, const TrainPassBuf
     if (use_cascade)
         if ((rc = mn_stage_sort_cat(ctx, z_c, b.S, z_f, b.F, N, 0, lr, z_q, b.flip ? TF(b.z_q_comp) : nullptr, st))) return rc;
     if ((rc = fine_points(z_q, b.Sq, b.flip && use_cascade, WF(b.xyz_f), WF(b.dreal_f)))) return rc;
-    if ((rc = query(WF(b.xyz_f), b.Sq, 0, noise_f, TF(b.mlp_f), TF(b.raw_f), b.tape_f, b.tape_f_bytes))) return rc;
+    if (masked) rc = query_occ(WF(b.xyz_f), b.Sq, 0, noise_f, TF(b.mlp_f), TF(b.raw_f), b.tape_f, b.tape_f_bytes, b.occ_idx_f, 1);
+    else rc = query(WF(b.xyz_f), b.Sq, 0, noise_f, TF(b.mlp_f), TF(b.raw_f), b.tape_f, b.tape_f_bytes);
+    if (rc) return rc;
     // depth scratch when only the variance is wanted: the coarse weights are dead by now
     float* depth = r.depth ? r.depth : (r.depth_var ? WF(b.w_c) : nullptr);
     if (use_cascade)
@@ -611,9 +684,19 @@ int train_two_pass(mn_ctx* ctx, mn_model* net, int precision, const TrainPassBuf
                               last_delta, N, b.flip, lr, nullptr, r.rgb, depth, r.depth_var, r.bg_lambda, st);
 }
 
+// The result gradients of the queried samples in compacted order: g_cmp[p] = g_raw[idx[p]] for the *count queried rows.
+__global__ void occ_gather_grad_kernel(const float4* __restrict__ g_raw, const int* __restrict__ idx, const int* __restrict__ count,
+                                       float4* __restrict__ g_cmp) {
+    const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= *count) return;
+    g_cmp[p] = g_raw[idx[p]];
+}
+
 // The backward of train_two_pass: the composite backward(s) - with the gradients of bg_lambda (g_lam, g_lam_c; null: none) - then
 // the fine and the coarse model backwards, each through the SH head's backward, into gw.  The coarse pass has no gradient under
-// cascade without g_rgb_coarse, and is skipped.  dirs / dstride: the directions the forward read.
+// cascade without g_rgb_coarse, and is skipped.  dirs / dstride: the directions the forward read.  A pass masked by an occupancy
+// grid gathers the per-sample gradients of its queried samples into compacted order first (occ_gather_grad_kernel) and runs the
+// SH head's and the model's backward over the queried rows only; a skipped sample's gradient reaches no parameter.
 int train_two_pass_backward(mn_ctx* ctx, mn_model* net, int precision, const TrainPassBufs& b, const char* T, char* W, int64_t N,
                             const int* live, int use_cascade, int sh_deg, const float* last_delta, const float* dirs, int64_t dstride,
                             const float* g_rgb, const float* g_rgb_coarse, const float* g_lam, const float* g_lam_c, float* gw,
@@ -637,21 +720,32 @@ int train_two_pass_backward(mn_ctx* ctx, mn_model* net, int precision, const Tra
         return rc;
     }
     // the model backwards in reverse order of their forward calls, each through the SH head's backward first
-    auto model_bwd = [&](int S, int use_coarse, size_t mlp, size_t g_raw, size_t g_mlp, size_t tape, size_t tape_n) -> int {
-        const LiveRows lrs{live, S};
+    const bool masked = b.occ_idx_c != kNone;
+    auto model_bwd = [&](int S, int use_coarse, size_t mlp, size_t g_raw, size_t g_mlp, size_t tape, size_t tape_n, size_t idx_off,
+                         int pass) -> int {
+        LiveRows lrs{live, S};
         const float* g = WF(g_raw);
+        const int* gather = nullptr;
+        if (masked) {
+            gather = reinterpret_cast<const int*>(T + idx_off);
+            lrs = LiveRows{reinterpret_cast<const int*>(T + b.occ_cnt) + pass, 1};
+            occ_gather_grad_kernel<<<(unsigned)mn_cdiv(N * S, 256), 256, 0, st>>>(reinterpret_cast<const float4*>(g), gather, lrs.rays,
+                                                                                 reinterpret_cast<float4*>(WF(b.g_cmp)));
+            MN_LAUNCH_CHECK(ctx);
+            g = WF(b.g_cmp);
+        }
         int e;
         if (sh_deg >= 0) {
             if ((e = mn_stage_sh_to_rgb_backward(ctx, sh_deg, TF(mlp), net->nd.rgb_dim + 1, dirs, dstride, S, N * S, 1, lrs, g, WF(g_mlp),
-                                                 st)))
+                                                 st, gather)))
                 return e;
             g = WF(g_mlp);
         }
         return mn_model_backward_live(ctx, net, N * S, lrs, use_coarse, precision, g, T + tape, tape_n, gw, W + b.bwd_ws,
                                       b.bwd_ws_bytes, st);
     };
-    if ((rc = model_bwd(b.Sq, 0, b.mlp_f, b.g_raw_f, b.g_mlp_f, b.tape_f, b.tape_f_bytes))) return rc;
-    if (coarse) return model_bwd(b.S, 1, b.mlp_c, b.g_raw_c, b.g_mlp_c, b.tape_c, b.tape_c_bytes);
+    if ((rc = model_bwd(b.Sq, 0, b.mlp_f, b.g_raw_f, b.g_mlp_f, b.tape_f, b.tape_f_bytes, b.occ_idx_f, 1))) return rc;
+    if (coarse) return model_bwd(b.S, 1, b.mlp_c, b.g_raw_c, b.g_mlp_c, b.tape_c, b.tape_c_bytes, b.occ_idx_c, 0);
     return MN_OK;
 }
 
@@ -662,11 +756,11 @@ struct TrainPlan {
     size_t last_delta, rays, tape_total, ws_total, bwd_total;
 };
 
-TrainPlan make_train_plan(const mn_model* m, int64_t N, int S, int F, int use_cascade, bool sh, bool tc) {
+TrainPlan make_train_plan(const mn_model* m, int64_t N, int S, int F, int use_cascade, bool sh, bool tc, bool occ = false) {
     TrainPlan p{};
     Carve t, w, b;
     p.last_delta = t((size_t)N * 4);
-    p.pass = carve_train_pass(t, w, b, m, N, S, F, use_cascade, sh, 3, false, tc);
+    p.pass = carve_train_pass(t, w, b, m, N, S, F, use_cascade, sh, 3, false, tc, occ);
     p.rays = sh ? t((size_t)N * 32) : kNone;
     p.tape_total = t.off + 256;
     p.ws_total = w.off + 256;
@@ -685,11 +779,25 @@ int check_train(mn_ctx* ctx, const mn_model* m, int64_t N, int coarse_samples, i
     return MN_OK;
 }
 
+// The checks of a training render through an occupancy grid (those of render_impl), and the grid as the kernels read it.
+int check_occ(mn_ctx* ctx, const mn_occupancy* occ, int64_t N, int S, int F, int use_cascade, const char* name, OccGrid* g) {
+    const std::string n(name);
+    if (!occ->bits || occ->reso < 1 || occ->reso > MN_OCC_MAX_RESO)
+        return mn_fail(ctx, MN_ERR_INVALID, n + ": the occupancy grid needs bits and a reso of 1.." + std::to_string(MN_OCC_MAX_RESO));
+    const int Sq = use_cascade ? S + F : F;
+    if (N * (int64_t)(Sq > S ? Sq : S) > INT32_MAX)
+        return mn_fail(ctx, MN_ERR_INVALID, n + ": an occupancy-grid render indexes at most 2^31 - 1 samples per pass");
+    g->bits = occ->bits;
+    g->reso = occ->reso;
+    for (int a = 0; a < 3; ++a) { g->off[a] = occ->offset[a]; g->scl[a] = occ->scale[a]; }
+    return MN_OK;
+}
+
 int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N, const float* z_steps_d,
                const float* jitter_d, float perturb, int S, const float* noise_c_d, const float* u_d, const float* noise_f_d, int F,
                int use_cascade, int sh_deg, int precision, float* rgb, float* depth, float* var, float* rgb_coarse, void* tape_d,
-               size_t tape_bytes, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
-    const char* name = "mn_render_rays_train";
+               size_t tape_bytes, void* workspace_d, size_t workspace_bytes, cudaStream_t st, const char* name,
+               const mn_occupancy* occ = nullptr, int* counts_out = nullptr) {
     const std::string nm(name);
     if (!ctx || !m || !rays_d || !z_steps_d || !u_d || !rgb) return MN_ERR_INVALID;
     int rc;
@@ -697,8 +805,10 @@ int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image
     if ((rc = check_net(ctx, m, use_cascade, F, sh_deg, image_indices_d, name))) return rc;
     if (perturb > 0 && !jitter_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": perturb > 0 needs jitter_d");
     if (use_cascade && !rgb_coarse) return mn_fail(ctx, MN_ERR_INVALID, nm + ": rgb_coarse_out_d is required under use_cascade");
+    OccGrid G{};
+    if (occ && (rc = check_occ(ctx, occ, N, S, F, use_cascade, name, &G))) return rc;
     if (N == 0) return MN_OK;
-    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16);
+    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16, occ != nullptr);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
     if (!workspace_d || workspace_bytes < p.ws_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     char* T = (char*)tape_d;
@@ -717,19 +827,18 @@ int train_impl(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image
     o.rgb_coarse = rgb_coarse;
     auto from_z = [&](const float* z, int Sq, int, float* xyz, float*) { return mn_points_from_z(ctx, rays_d, z, N, Sq, xyz, st); };
     return train_two_pass(ctx, m, precision, p.pass, T, W, N, nullptr, use_cascade, sh_deg, last_delta, u_d, noise_c_d, noise_f_d,
-                          rays_d + 3, 8, image_indices_d, o, from_z, st);
+                          rays_d + 3, 8, image_indices_d, o, from_z, st, occ ? &G : nullptr, counts_out);
 }
 
 int train_backward_impl(mn_ctx* ctx, mn_model* m, int64_t N, int S, int F, int use_cascade, int sh_deg, int precision,
                         const float* g_rgb, const float* g_rgb_coarse, const void* tape_d, size_t tape_bytes, float* gw,
-                        void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
-    const char* name = "mn_render_rays_train_backward";
+                        void* workspace_d, size_t workspace_bytes, cudaStream_t st, const char* name, bool occ = false) {
     const std::string nm(name);
     if (!ctx || !m || !g_rgb || !gw) return MN_ERR_INVALID;
     int rc;
     if ((rc = check_train(ctx, m, N, S, F, precision, name))) return rc;
     if (N == 0) return MN_OK;
-    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16);
+    const TrainPlan p = make_train_plan(m, N, S, F, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16, occ);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
     if (!workspace_d || workspace_bytes < p.bwd_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     const char* T = (const char*)tape_d;
@@ -788,9 +897,9 @@ struct BgTrainPlan {
 };
 
 BgTrainPlan make_bg_train_plan(const mn_model* m, const mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, bool sh, bool tc,
-                               bool bg_tc) {
+                               bool bg_tc, bool occ = false) {
     BgTrainPlan p{};
-    p.fg = make_train_plan(m, N, Sc, Sf, use_cascade, sh, tc);
+    p.fg = make_train_plan(m, N, Sc, Sf, use_cascade, sh, tc, occ);
     Carve t, w, b;
     t.off = p.fg.tape_total;
     w.off = p.fg.ws_total;
@@ -839,8 +948,7 @@ int train_bg_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, c
                   const float* noise_c_d, const float* noise_c_bg_d, const float* u_d, const float* u_bg_d, const float* noise_f_d,
                   const float* noise_f_bg_d, int Sf, int use_cascade, int sh_deg, int precision, int bg_precision, int by_ray,
                   const mn_render_outputs* out, void* tape_d, size_t tape_bytes, void* workspace_d, size_t workspace_bytes,
-                  cudaStream_t st) {
-    const char* name = "mn_render_rays_train_bg";
+                  cudaStream_t st, const char* name, const mn_occupancy* occ = nullptr, int* counts_out = nullptr) {
     const std::string nm(name);
     if (!ctx || !m || !bg || !rays_d || !z_steps_d || !z_steps_bg_d || !u_d || !u_bg_d || !out || !out->rgb || !out->bg_lambda)
         return MN_ERR_INVALID;
@@ -855,9 +963,11 @@ int train_bg_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, c
     if (radius_d && !center_d) return mn_fail(ctx, MN_ERR_INVALID, nm + ": sphere radius without a center");
     if (include_xyz_real != (bg->d.kind == 2 && bg->d.xyz_real ? 1 : 0))
         return mn_fail(ctx, MN_ERR_INVALID, nm + ": include_xyz_real must match the background model's real-xyz prefix");
+    OccGrid G{};
+    if (occ && (rc = check_occ(ctx, occ, N, Sc, Sf, use_cascade, name, &G))) return rc;
     if (N == 0) return MN_OK;
     const BgTrainPlan p = make_bg_train_plan(m, bg, N, Sc, Sf, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
-                                             bg_precision == MN_PREC_TC_F16);
+                                             bg_precision == MN_PREC_TC_F16, occ != nullptr);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
     if (!workspace_d || workspace_bytes < p.ws_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     char* T = (char*)tape_d;
@@ -919,7 +1029,7 @@ int train_bg_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, c
         return rc;
     auto from_z = [&](const float* z, int Sq, int, float* xyz, float*) { return mn_points_from_z(ctx, rays_d, z, N, Sq, xyz, st); };
     if ((rc = train_two_pass(ctx, m, precision, p.fg.pass, T, W, N, nullptr, use_cascade, sh_deg, TF(p.fg.last_delta), u_d, noise_c_d,
-                             noise_f_d, rays_d + 3, 8, image_indices_d, fo, from_z, st)))
+                             noise_f_d, rays_d + 3, 8, image_indices_d, fo, from_z, st, occ ? &G : nullptr, counts_out)))
         return rc;
     MN_CUDA(ctx, cudaMemcpyAsync(o.bg_lambda, fo.bg_lambda, (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
     if (use_cascade) MN_CUDA(ctx, cudaMemcpyAsync(o.bg_lambda_coarse, fo.bg_lambda_coarse, (size_t)N * 4, cudaMemcpyDeviceToDevice, st));
@@ -930,15 +1040,15 @@ int train_bg_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, const float* rays_d, c
 
 int train_bg_backward_impl(mn_ctx* ctx, mn_model* m, mn_model* bg, int64_t N, int Sc, int Sf, int use_cascade, int sh_deg, int precision,
                            int bg_precision, const float* g_rgb, const float* g_rgb_coarse, const void* tape_d, size_t tape_bytes,
-                           float* gw, float* gw_bg, void* workspace_d, size_t workspace_bytes, cudaStream_t st) {
-    const char* name = "mn_render_rays_train_bg_backward";
+                           float* gw, float* gw_bg, void* workspace_d, size_t workspace_bytes, cudaStream_t st, const char* name,
+                           bool occ = false) {
     const std::string nm(name);
     if (!ctx || !m || !bg || !g_rgb || !gw || !gw_bg) return MN_ERR_INVALID;
     int rc;
     if ((rc = check_train_bg(ctx, m, bg, N, Sc, Sf, precision, bg_precision, name))) return rc;
     if (N == 0) return MN_OK;
     const BgTrainPlan p = make_bg_train_plan(m, bg, N, Sc, Sf, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
-                                             bg_precision == MN_PREC_TC_F16);
+                                             bg_precision == MN_PREC_TC_F16, occ);
     if (!tape_d || tape_bytes < p.tape_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": tape too small");
     if (!workspace_d || workspace_bytes < p.bwd_total) return mn_fail(ctx, MN_ERR_WORKSPACE, nm + ": workspace too small");
     const char* T = (const char*)tape_d;
@@ -1078,7 +1188,7 @@ int mn_render_rays_train(mn_ctx* ctx, mn_model* m, const float* rays_d, const fl
                          void* stream) {
     return train_impl(ctx, m, rays_d, image_indices_d, N, z_steps_d, jitter_d, perturb, coarse_samples, sigma_noise_coarse_d, u_fine_d,
                       sigma_noise_fine_d, fine_samples, use_cascade, sh_deg, precision, rgb_out_d, depth_out_d, depth_var_out_d,
-                      rgb_coarse_out_d, tape_d, tape_bytes, workspace_d, workspace_bytes, (cudaStream_t)stream);
+                      rgb_coarse_out_d, tape_d, tape_bytes, workspace_d, workspace_bytes, (cudaStream_t)stream, "mn_render_rays_train");
 }
 
 int mn_render_rays_train_backward(mn_ctx* ctx, mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
@@ -1086,7 +1196,8 @@ int mn_render_rays_train_backward(mn_ctx* ctx, mn_model* m, int64_t N, int coars
                                   const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d,
                                   size_t workspace_bytes, void* stream) {
     return train_backward_impl(ctx, m, N, coarse_samples, fine_samples, use_cascade, sh_deg, precision, grad_rgb_d, grad_rgb_coarse_d,
-                               tape_d, tape_bytes, param_grads_d, workspace_d, workspace_bytes, (cudaStream_t)stream);
+                               tape_d, tape_bytes, param_grads_d, workspace_d, workspace_bytes, (cudaStream_t)stream,
+                               "mn_render_rays_train_backward");
 }
 
 size_t mn_render_rays_train_bg_tape_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
@@ -1122,7 +1233,7 @@ int mn_render_rays_train_bg(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float
                          z_steps_d, z_steps_bg_d, jitter_d, jitter_bg_d, perturb, coarse_samples, sigma_noise_coarse_d,
                          sigma_noise_coarse_bg_d, u_fine_d, u_fine_bg_d, sigma_noise_fine_d, sigma_noise_fine_bg_d, fine_samples,
                          use_cascade, sh_deg, precision, bg_precision, bg_draws_by_ray, out, tape_d, tape_bytes, workspace_d,
-                         workspace_bytes, (cudaStream_t)stream);
+                         workspace_bytes, (cudaStream_t)stream, "mn_render_rays_train_bg");
 }
 
 int mn_render_rays_train_bg_backward(mn_ctx* ctx, mn_model* fg, mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
@@ -1131,7 +1242,106 @@ int mn_render_rays_train_bg_backward(mn_ctx* ctx, mn_model* fg, mn_model* bg, in
                                      float* bg_param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream) {
     return train_bg_backward_impl(ctx, fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg, precision, bg_precision, grad_rgb_d,
                                   grad_rgb_coarse_d, tape_d, tape_bytes, param_grads_d, bg_param_grads_d, workspace_d, workspace_bytes,
-                                  (cudaStream_t)stream);
+                                  (cudaStream_t)stream, "mn_render_rays_train_bg_backward");
+}
+
+// ---- the training renders through an occupancy grid
+size_t mn_render_rays_train_occ_tape_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                           int sh_deg, int precision) {
+    if (!m || check_train(nullptr, m, N, coarse_samples, fine_samples, precision, "")) return 0;
+    return make_train_plan(m, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16, true).tape_total;
+}
+
+size_t mn_render_rays_train_occ_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                                int sh_deg, int precision) {
+    if (!m || check_train(nullptr, m, N, coarse_samples, fine_samples, precision, "")) return 0;
+    return make_train_plan(m, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16, true).ws_total;
+}
+
+size_t mn_render_rays_train_occ_backward_workspace_bytes(const mn_model* m, int64_t N, int coarse_samples, int fine_samples,
+                                                         int use_cascade, int sh_deg, int precision) {
+    if (!m || check_train(nullptr, m, N, coarse_samples, fine_samples, precision, "")) return 0;
+    return make_train_plan(m, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16, true).bwd_total;
+}
+
+int mn_render_rays_train_occ(mn_ctx* ctx, mn_model* m, const float* rays_d, const float* image_indices_d, int64_t N,
+                             const float* z_steps_d, const float* jitter_d, float perturb, int coarse_samples,
+                             const float* sigma_noise_coarse_d, const float* u_fine_d, const float* sigma_noise_fine_d, int fine_samples,
+                             int use_cascade, int sh_deg, int precision, const mn_occupancy* occ, int32_t* counts_out_d, float* rgb_out_d,
+                             float* depth_out_d, float* depth_var_out_d, float* rgb_coarse_out_d, void* tape_d, size_t tape_bytes,
+                             void* workspace_d, size_t workspace_bytes, void* stream) {
+    if (!occ) return mn_fail(ctx, MN_ERR_INVALID, "mn_render_rays_train_occ: occ is NULL");
+    return train_impl(ctx, m, rays_d, image_indices_d, N, z_steps_d, jitter_d, perturb, coarse_samples, sigma_noise_coarse_d, u_fine_d,
+                      sigma_noise_fine_d, fine_samples, use_cascade, sh_deg, precision, rgb_out_d, depth_out_d, depth_var_out_d,
+                      rgb_coarse_out_d, tape_d, tape_bytes, workspace_d, workspace_bytes, (cudaStream_t)stream, "mn_render_rays_train_occ",
+                      occ, counts_out_d);
+}
+
+int mn_render_rays_train_occ_backward(mn_ctx* ctx, mn_model* m, int64_t N, int coarse_samples, int fine_samples, int use_cascade,
+                                      int sh_deg, int precision, const float* grad_rgb_d, const float* grad_rgb_coarse_d,
+                                      const void* tape_d, size_t tape_bytes, float* param_grads_d, void* workspace_d,
+                                      size_t workspace_bytes, void* stream) {
+    return train_backward_impl(ctx, m, N, coarse_samples, fine_samples, use_cascade, sh_deg, precision, grad_rgb_d, grad_rgb_coarse_d,
+                               tape_d, tape_bytes, param_grads_d, workspace_d, workspace_bytes, (cudaStream_t)stream,
+                               "mn_render_rays_train_occ_backward", true);
+}
+
+size_t mn_render_rays_train_bg_occ_tape_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                              int use_cascade, int sh_deg, int precision, int bg_precision) {
+    if (!fg || !bg || check_train_bg(nullptr, fg, bg, N, coarse_samples, fine_samples, precision, bg_precision, "")) return 0;
+    return make_bg_train_plan(fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
+                              bg_precision == MN_PREC_TC_F16, true).tape_total;
+}
+
+size_t mn_render_rays_train_bg_occ_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples,
+                                                   int fine_samples, int use_cascade, int sh_deg, int precision, int bg_precision) {
+    if (!fg || !bg || check_train_bg(nullptr, fg, bg, N, coarse_samples, fine_samples, precision, bg_precision, "")) return 0;
+    return make_bg_train_plan(fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
+                              bg_precision == MN_PREC_TC_F16, true).ws_total;
+}
+
+size_t mn_render_rays_train_bg_occ_backward_workspace_bytes(const mn_model* fg, const mn_model* bg, int64_t N, int coarse_samples,
+                                                            int fine_samples, int use_cascade, int sh_deg, int precision,
+                                                            int bg_precision) {
+    if (!fg || !bg || check_train_bg(nullptr, fg, bg, N, coarse_samples, fine_samples, precision, bg_precision, "")) return 0;
+    return make_bg_train_plan(fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg >= 0, precision == MN_PREC_TC_F16,
+                              bg_precision == MN_PREC_TC_F16, true).bwd_total;
+}
+
+int mn_render_rays_train_bg_occ(mn_ctx* ctx, mn_model* fg, mn_model* bg, const float* rays_d, const float* image_indices_d, int64_t N,
+                                const float* sphere_center3_d, const float* sphere_radius3_d, int include_xyz_real, int cluster_2d,
+                                const float* z_steps_d, const float* z_steps_bg_d, const float* jitter_d, const float* jitter_bg_d,
+                                float perturb, int coarse_samples, const float* sigma_noise_coarse_d,
+                                const float* sigma_noise_coarse_bg_d, const float* u_fine_d, const float* u_fine_bg_d,
+                                const float* sigma_noise_fine_d, const float* sigma_noise_fine_bg_d, int fine_samples, int use_cascade,
+                                int sh_deg, int precision, int bg_precision, const mn_occupancy* occ, int32_t* counts_out_d,
+                                int bg_draws_by_ray, const mn_render_outputs* out, void* tape_d, size_t tape_bytes, void* workspace_d,
+                                size_t workspace_bytes, void* stream) {
+    if (!occ) return mn_fail(ctx, MN_ERR_INVALID, "mn_render_rays_train_bg_occ: occ is NULL");
+    return train_bg_impl(ctx, fg, bg, rays_d, image_indices_d, N, sphere_center3_d, sphere_radius3_d, include_xyz_real, cluster_2d,
+                         z_steps_d, z_steps_bg_d, jitter_d, jitter_bg_d, perturb, coarse_samples, sigma_noise_coarse_d,
+                         sigma_noise_coarse_bg_d, u_fine_d, u_fine_bg_d, sigma_noise_fine_d, sigma_noise_fine_bg_d, fine_samples,
+                         use_cascade, sh_deg, precision, bg_precision, bg_draws_by_ray, out, tape_d, tape_bytes, workspace_d,
+                         workspace_bytes, (cudaStream_t)stream, "mn_render_rays_train_bg_occ", occ, counts_out_d);
+}
+
+int mn_render_rays_train_bg_occ_backward(mn_ctx* ctx, mn_model* fg, mn_model* bg, int64_t N, int coarse_samples, int fine_samples,
+                                         int use_cascade, int sh_deg, int precision, int bg_precision, const float* grad_rgb_d,
+                                         const float* grad_rgb_coarse_d, const void* tape_d, size_t tape_bytes, float* param_grads_d,
+                                         float* bg_param_grads_d, void* workspace_d, size_t workspace_bytes, void* stream) {
+    return train_bg_backward_impl(ctx, fg, bg, N, coarse_samples, fine_samples, use_cascade, sh_deg, precision, bg_precision, grad_rgb_d,
+                                  grad_rgb_coarse_d, tape_d, tape_bytes, param_grads_d, bg_param_grads_d, workspace_d, workspace_bytes,
+                                  (cudaStream_t)stream, "mn_render_rays_train_bg_occ_backward", true);
+}
+
+// bits = pack(sigmas >= thresh): one warp per 32 cells, each lane's comparison balloted into the cells' word.  A NaN sigma fails
+// the comparison (an empty cell), as torch's does.
+int mn_occupancy_pack(mn_ctx* ctx, const float* sigmas_d, int64_t n, float thresh, uint32_t* bits_d, void* stream) {
+    if (!ctx || n < 0 || (n > 0 && (!sigmas_d || !bits_d))) return MN_ERR_INVALID;
+    if (n == 0) return MN_OK;
+    occ_pack_kernel<<<(unsigned)mn_cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(sigmas_d, n, thresh, bits_d);
+    MN_LAUNCH_CHECK(ctx);
+    return MN_OK;
 }
 
 }  // extern "C"

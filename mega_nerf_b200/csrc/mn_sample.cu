@@ -796,12 +796,12 @@ __device__ __forceinline__ void sh_basis(int deg, float x, float y, float z, flo
 
 __global__ void sh_to_rgb_bwd_kernel(int deg, const float* __restrict__ coef, int64_t cstride, const float* __restrict__ dirs,
                                      int64_t dstride, int ddiv, int64_t B, int sig, const float* __restrict__ gout,
-                                     float* __restrict__ gcoef, LiveRows live) {
+                                     float* __restrict__ gcoef, LiveRows live, const int* __restrict__ gather) {
     const int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= live.rows(B)) return;
     const int nc = (deg + 1) * (deg + 1);
     const float* c = coef + b * cstride;
-    const float* d = dirs + (b / ddiv) * dstride;
+    const float* d = dirs + ((gather ? (int64_t)gather[b] : b) / ddiv) * dstride;     // as sh_to_rgb_kernel
     float* gc = gcoef + b * cstride;
     float Y[25], s[25];
     sh_basis(deg, d[0], d[1], d[2], Y);
@@ -1070,9 +1070,9 @@ int mn_stage_composite_backward(mn_ctx* ctx, const float* raw_d, const float* z_
 
 int mn_stage_sh_to_rgb_backward(mn_ctx* ctx, int deg, const float* coef_d, int64_t coef_stride, const float* dirs_d, int64_t dir_stride,
                                 int dir_div, int64_t B, int apply_sigmoid, LiveRows live, const float* grad_out_d, float* grad_coef_d,
-                                cudaStream_t st) {
+                                cudaStream_t st, const int* gather) {
     sh_to_rgb_bwd_kernel<<<(unsigned)mn_cdiv(B, 256), 256, 0, st>>>(deg, coef_d, coef_stride, dirs_d, dir_stride, dir_div, B, apply_sigmoid,
-                                                                    grad_out_d, grad_coef_d, live);
+                                                                    grad_out_d, grad_coef_d, live, gather);
     MN_LAUNCH_CHECK(ctx);
     return MN_OK;
 }

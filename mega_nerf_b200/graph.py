@@ -19,8 +19,9 @@ raises the same `Exception`.
 With an occupancy grid (mega_nerf_b200.octree.OccupancyGrid; an approximate render mode, see render_rays_fused) the graph
 captures `render_rays_fused(..., occupancy=grid)`, with or without a background network.  The queried samples are compacted
 on the device, so one graph serves every chunk whatever the grid skips; `occupancy_counts` holds the queried foreground
-samples of the coarse and fine passes after each replay.  The graph reads the grid's words in place and keeps the grid alive;
-a different grid needs a new GraphedRenderRays.
+samples of the coarse and fine passes after each replay.  The graph reads the grid's words in place and keeps the grid alive:
+`grid.refresh_(nerf)` rewrites them in place and the next replay follows it; a grid of another size or frame needs a new
+GraphedRenderRays.
 
     g = GraphedRenderRays(nerf, hparams, 4096, dev, occupancy=octree.occupancy_grid(hparams, nerf, offset, invradius))
 
@@ -47,6 +48,17 @@ both networks over the group's ranks inside the replay, with one all-reduce over
 DistributedDataParallel would; the networks themselves are passed unwrapped.
 
     step = GraphedTrainStep(nerf, hparams, 4096, dev, opt, process_group=dist.group.WORLD)
+
+With an occupancy grid the step trains through it (render_rays_train(..., occupancy=grid), an approximate mode): the foreground
+samples in empty cells are neither queried nor differentiated.  The grid follows the network when it is refreshed in place
+between replays, with no recapture; `occupancy_counts` holds the queried foreground samples of each pass after each replay.
+
+    grid = octree.occupancy_grid(hparams, nerf, offset, invradius)
+    step = GraphedTrainStep(nerf, hparams, 4096, dev, opt, occupancy=grid)
+    for k, (rays, rgbs, idx) in enumerate(batches):
+        step.step(rays, rgbs, idx)
+        if k % 16 == 15:
+            grid.refresh_(nerf)
 """
 import gc
 from argparse import Namespace
@@ -62,8 +74,8 @@ import torch.distributed as dist
 from . import _cabi as K
 from . import dist as D
 from .modules import Cascade, MegaNeRF, NeRF
-from .render import (_check_train, _check_train_bg, _refuse_bg_ep, _render_train, _render_train_bg, _unwrap, render_rays,
-                     render_rays_fused)
+from .render import (_check_occupancy, _check_train, _check_train_bg, _refuse_bg_ep, _render_train, _render_train_bg, _unwrap,
+                     render_rays, render_rays_fused)
 
 
 class GraphedRenderRays:
@@ -75,7 +87,8 @@ class GraphedRenderRays:
         exchange of a multi-GPU render (`torch.distributed.all_gather_into_tensor` on NCCL is capturable), so that a
         step stays one graph launch; whatever it returns is kept in `self.post_result`.
         bg_nerf / sphere_center / sphere_radius / get_bg_fg_rgb: as for render_rays (the background path).
-        occupancy: an OccupancyGrid, as for render_rays_fused (captured once; a new grid needs a new GraphedRenderRays)."""
+        occupancy: an OccupancyGrid, as for render_rays_fused (its words are read in place at every replay, so a refresh_ is
+        followed; a grid of another size or frame needs a new GraphedRenderRays)."""
         if nerf.training or (bg_nerf is not None and bg_nerf.training):
             raise ValueError('GraphedRenderRays replays the inference path; call nerf.eval() first')
         _refuse_bg_ep(bg_nerf, 'GraphedRenderRays')
@@ -194,7 +207,7 @@ class GraphedTrainStep:
     def __init__(self, nerf: nn.Module, hparams: Namespace, n_rays: int, device: torch.device, optimizer: torch.optim.Optimizer,
                  get_depth_variance: bool = True, bg_nerf: Optional[nn.Module] = None, scaler=None, warmup: int = 2,
                  sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None,
-                 process_group=None):
+                 process_group=None, occupancy=None):
         """One training step of `nerf` over batches of n_rays rays as a CUDA graph.  The loss is the runner's: the MSE of rgb_fine,
         averaged with that of rgb_coarse for a Cascade (runner.py:366-379).  `optimizer` steps every parameter it holds inside
         the graph, so it must be capturable (`torch.optim.Adam(..., capturable=True)`).  A learning rate given as a Python number
@@ -227,11 +240,18 @@ class GraphedTrainStep:
         dummy background ray that it multiplies by zero (rendering.py:143-171); here the fixed-shape step needs no dummy ray.
         loss / psnr / depth_variance and check() stay per rank.
 
+        occupancy: None, or an octree.OccupancyGrid through which the step trains the foreground network (render_rays_train's
+        occupancy mode; the background network is never masked).  The replay reads the grid's words in place, so
+        `occupancy.refresh_(nerf)` between steps - or any in-place rewrite of occupancy.bits - is what the next step trains
+        through, without a recapture.  `self.occupancy_counts` (int32 [2] on the device) receives the queried foreground samples of
+        the coarse and the fine pass at every replay.
+
         Refused (ValueError): a background network without sphere_center / sphere_radius, under expert parallelism, wrapped in
         DistributedDataParallel or of another kind than hparams.use_cascade says; a network under expert parallelism or wrapped
         in DistributedDataParallel, an optimizer that is not capturable, a GradScaler (tc_f16 scales its gradients inside the
         library, and `scaler.step` synchronises), a process group that is not NCCL (a CUDA graph captures NCCL collectives
-        only) or whose rank's device is not `device`."""
+        only) or whose rank's device is not `device`, an occupancy grid on another device or with a network under expert
+        parallelism."""
         if bg_nerf is not None:
             if sphere_center is None or sphere_radius is None:
                 raise ValueError('GraphedTrainStep: a background network needs sphere_center and sphere_radius')
@@ -250,6 +270,7 @@ class GraphedTrainStep:
         if not all(g.get('capturable', False) for g in optimizer.param_groups):
             raise ValueError('GraphedTrainStep needs a capturable optimizer, e.g. torch.optim.Adam(..., capturable=True)')
         _check_train(nerf, hparams, 'GraphedTrainStep')
+        _check_occupancy(nerf, occupancy, None, torch.device(device), 'GraphedTrainStep')
         if process_group is not None:
             _check_group(process_group, torch.device(device))
         self.nerf, self.hparams, self.optimizer = nerf, hparams, optimizer
@@ -271,6 +292,8 @@ class GraphedTrainStep:
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.loss = self.psnr = self.depth_variance = None
         self._captured_lrs = []
+        self.occupancy = occupancy
+        self.occupancy_counts = torch.zeros(2, device=self.device, dtype=torch.int32) if occupancy is not None else None
 
     def _natives(self):
         return [nat for nat in (self.native, self.bnative) if nat is not None]
@@ -285,11 +308,12 @@ class GraphedTrainStep:
                 nat.sync(self.device)
         if self.bg_nerf is None:
             res = _render_train(self.nerf, self.native, self.rays, self.indices, self.hparams, False, self.get_depth_variance,
-                                self._grads)
+                                self._grads, self.occupancy, self.occupancy_counts)
         else:
             res = _render_train_bg(self.nerf, self.native, self.bg_nerf, self.bnative, self.rays, self.indices, self.hparams,
                                    self.center, self.radius, False, self.get_depth_variance, False, by_ray=True,
-                                   check_status=False, grads=self._grads)
+                                   check_status=False, grads=self._grads, occupancy=self.occupancy,
+                                   occupancy_counts=self.occupancy_counts)
         rgb = res['rgb_fine']
         with torch.no_grad():
             psnr = -10 * torch.log10(torch.mean((rgb - self.rgbs) ** 2))     # metrics.py:8-10, without the host read

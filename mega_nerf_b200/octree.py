@@ -8,7 +8,9 @@
   lattice_points <- grid[mask] for any mask over the lattice (masking_mode 'weight': the mask from svox's grid weights)
   cell_colors    <- the rgba means of _step2 (create_octree.py:189-207), model calls on ray-structured rows
   occupancy_grid <- _step1's sigma mask (create_octree.py:139-176) packed into an OccupancyGrid, the bit grid with which
-                    render_rays_fused / GraphedRenderRays skip the network queries of empty space (an approximate render mode)
+                    render_rays_fused / GraphedRenderRays skip the network queries of empty space (an approximate render mode),
+                    and render_rays_train / GraphedTrainStep skip them in training; OccupancyGrid.refresh_ recomputes it in place
+                    from the network's current weights
 
 create_octree.py runs as __main__, so install() cannot reach these; INTEGRATION.md lists the lines to change there.  svox's own
 work (grid_weight_render, the in-cell sampler, refinement, merge, save) stays svox's.
@@ -171,10 +173,12 @@ class OccupancyGrid:
     (i * reso + j) * reso + k holds the lattice point (xx[i], yy[j], zz[k]) of lattice_axes(offset, scale, reso), so
     `density_grid(...) >= sigma_thresh` is a mask for from_mask as it stands.
 
-    bits: int32 [ceil(reso**3 / 32)] on the device, cell c at bit c % 32 of word c // 32.  A captured CUDA graph reads these
-    words in place: it keeps this object alive, and a different grid needs a new capture."""
+    bits: int32 [ceil(reso**3 / 32)] on the device, cell c at bit c % 32 of word c // 32.  A captured CUDA graph
+    (GraphedRenderRays, GraphedTrainStep) reads these words in place at every replay and keeps this object alive: refresh_, or
+    any other in-place write of `bits`, is followed by the next replay without a recapture; a grid of another reso or frame needs
+    a new capture.  alpha_thresh: the alpha threshold refresh_ applies by default (occupancy_grid sets it; None: none given)."""
 
-    def __init__(self, bits: torch.Tensor, reso: int, offset, scale):
+    def __init__(self, bits: torch.Tensor, reso: int, offset, scale, alpha_thresh: Optional[float] = None):
         reso = int(reso)
         if bits.dtype != torch.int32 or bits.dim() != 1 or bits.numel() != (reso ** 3 + 31) // 32:
             raise ValueError(f'bits must be int32 [{(reso ** 3 + 31) // 32}] for reso {reso}')
@@ -182,6 +186,7 @@ class OccupancyGrid:
         self.reso = reso
         self.offset = _axis_values(offset)
         self.scale = _axis_values(scale)
+        self.alpha_thresh = alpha_thresh
 
     @classmethod
     def from_mask(cls, mask: torch.Tensor, offset, scale, device: Optional[torch.device] = None) -> 'OccupancyGrid':
@@ -195,6 +200,26 @@ class OccupancyGrid:
 
     def cabi(self) -> K.Occupancy:
         return K.Occupancy(self.bits.data_ptr(), self.reso, (C.c_float * 3)(*self.offset), (C.c_float * 3)(*self.scale))
+
+    def refresh_(self, nerf: nn.Module, alpha_thresh: Optional[float] = None) -> 'OccupancyGrid':
+        """Recompute the grid from the network's current weights, in place: the density grid at this grid's reso / offset / scale
+        (density_grid, at the module precision, without a gradient and without changing nerf.training), thresholded at
+        sigma >= -log(1 - alpha_thresh) / (2 / reso) as occupancy_grid does (default: the grid's own alpha_thresh) and packed into
+        the same `bits` tensor on the device (mn_occupancy_pack), with no host sync.  The bits equal those of a fresh
+        occupancy_grid(..., reso=self.reso, alpha_thresh=...) over the same weights.  Returns self."""
+        at = self.alpha_thresh if alpha_thresh is None else alpha_thresh
+        if at is None:
+            raise ValueError('refresh_ needs an alpha_thresh: this grid was not made by occupancy_grid')
+        if _device_of(nerf) != self.bits.device:
+            raise ValueError(f'the network lives on {_device_of(nerf)}, the occupancy grid on {self.bits.device}')
+        with torch.no_grad():
+            sigmas = density_grid(nerf, self.offset, self.scale, self.reso)
+        dev = self.bits.device
+        h = K.ctx(dev)
+        # torch compares an fp32 tensor with a Python scalar in fp32, the scalar rounded to the nearest fp32 - as c_float rounds it
+        K.check(K.lib().mn_occupancy_pack(h, K.ptr(sigmas), sigmas.numel(), float(_sigma_thresh(at, self.reso)), K.ptr(self.bits),
+                                          K.stream_of(dev)), h)
+        return self
 
     def occupancy(self) -> float:
         """Share of the cells that are occupied."""
@@ -240,4 +265,6 @@ def occupancy_grid(hparams: Namespace, nerf: nn.Module, offset, invradius, reso:
     reso = int(reso) if reso is not None else 2 ** (hparams.init_grid_depth + 1)
     at = hparams.alpha_thresh if alpha_thresh is None else alpha_thresh
     sigmas = density_grid(nerf, offset, invradius, reso)
-    return OccupancyGrid.from_mask(sigmas >= _sigma_thresh(at, reso), offset, invradius)
+    grid = OccupancyGrid.from_mask(sigmas >= _sigma_thresh(at, reso), offset, invradius)
+    grid.alpha_thresh = at
+    return grid

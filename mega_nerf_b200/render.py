@@ -532,10 +532,26 @@ def _check_train(net: nn.Module, hparams: Namespace, fn: str) -> None:
         raise ValueError(f'{fn} needs fine_samples > 0')
 
 
+def _check_occupancy(net: nn.Module, occupancy, occupancy_counts: Optional[torch.Tensor], device: torch.device, fn: str) -> None:
+    """The refusals of a training call through an occupancy grid (those of render_rays_fused's grid)."""
+    if occupancy is None:
+        if occupancy_counts is not None:
+            raise ValueError('occupancy_counts needs an occupancy grid')
+        return
+    if getattr(net, '_ep', None) is not None:
+        raise ValueError(f'{fn}: an occupancy grid cannot mask a network under expert parallelism')
+    if occupancy.bits.device != torch.device(device):
+        raise ValueError(f'the occupancy grid lives on {occupancy.bits.device}, the rays on {device}')
+    if occupancy_counts is not None and (occupancy_counts.dtype != torch.int32 or occupancy_counts.numel() < 2
+                                         or not occupancy_counts.is_contiguous() or occupancy_counts.device != torch.device(device)):
+        raise ValueError('occupancy_counts must be a contiguous int32 tensor of 2 elements on the rays\' device')
+
+
 def render_rays_train(nerf: nn.Module, rays: torch.Tensor, image_indices: Optional[torch.Tensor], hparams: Namespace,
                       get_depth: bool, get_depth_variance: bool, bg_nerf: Optional[nn.Module] = None,
                       sphere_center: Optional[torch.Tensor] = None, sphere_radius: Optional[torch.Tensor] = None,
-                      get_bg_fg_rgb: bool = False) -> Dict[str, torch.Tensor]:
+                      get_bg_fg_rgb: bool = False, occupancy=None,
+                      occupancy_counts: Optional[torch.Tensor] = None) -> Dict[str, torch.Tensor]:
     """The training path of `render_rays(nerf, bg_nerf, ...)` (runner.py:347-358, networks in train mode) as ONE library call
     (`mn_render_rays_train`, or `mn_render_rays_train_bg` with a background network) whose backward is one library call too: the
     same kernels in the same order, sequenced in C, at the arithmetic of `set_train_precision`.  It draws its random numbers with
@@ -551,23 +567,34 @@ def render_rays_train(nerf: nn.Module, rays: torch.Tensor, image_indices: Option
     as on the stage path; under distributed training ('RANK' set) the draws of the reference's dummy background ray are consumed
     too, and the background parameters get a zero gradient, as its dummy ray gives them.  A camera outside the ellipsoid raises
     the reference's `Exception`.  Not for an expert-parallel network, a DistributedDataParallel wrapper, a background network
-    without sphere_center / sphere_radius, or fine_samples == 0 (use render_rays)."""
+    without sphere_center / sphere_radius, or fine_samples == 0 (use render_rays).
+
+    occupancy: an octree.OccupancyGrid, an approximate training mode (`mn_render_rays_train_occ` / `mn_render_rays_train_bg_occ`):
+    as in render_rays_fused, the foreground samples of both passes in cells the grid marks empty are not queried and enter
+    compositing as raw (0, 0, 0, 0); they pass no gradient to any parameter.  The background pass is not masked.  The draws are
+    those without a grid (density noise for every sample), so the results are those of render_rays with the foreground model's
+    output zeroed at the skipped samples, and with every cell occupied exactly those without a grid.  occupancy_counts: None, or
+    an int32 CUDA tensor of 2 elements that receives the queried foreground samples of the coarse and the fine pass (on the
+    device, no sync).  Not for a network under expert parallelism."""
     if _unwrap(nerf) is not nerf or (bg_nerf is not None and _unwrap(bg_nerf) is not bg_nerf):
         # the library's one call never runs the wrapper's forward, so DistributedDataParallel's reducer would not arm and every
         # rank would keep its own gradients
         raise ValueError('render_rays_train needs a mega_nerf_b200 network itself, not a wrapper such as DistributedDataParallel: '
                          'use render_rays, which queries through the wrapper')
     net, bg = _nets(nerf, bg_nerf, 'render_rays_train')
+    _check_occupancy(net, occupancy, occupancy_counts, rays.device, 'render_rays_train')
     _check_train(net, hparams, 'render_rays_train')
     native = net._native()
     native.sync(rays.device)
     if bg is None:
-        return _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance)
+        return _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance, occupancy=occupancy,
+                             occupancy_counts=occupancy_counts)
     _check_train_bg(net, bg, hparams, sphere_center, sphere_radius, 'render_rays_train')
     bnative = bg._native()
     bnative.sync(rays.device)
     return _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sphere_center, sphere_radius, get_depth,
-                            get_depth_variance, get_bg_fg_rgb, by_ray=False)
+                            get_depth_variance, get_bg_fg_rgb, by_ray=False, occupancy=occupancy,
+                            occupancy_counts=occupancy_counts)
 
 
 def _check_train_bg(net: nn.Module, bg: nn.Module, hparams: Namespace, center, radius, fn: str) -> None:
@@ -582,11 +609,12 @@ def _check_train_bg(net: nn.Module, bg: nn.Module, hparams: Namespace, center, r
 
 def _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sphere_center, sphere_radius, get_depth,
                      get_depth_variance, get_bg_fg_rgb, by_ray: bool, check_status: bool = True,
-                     grads=None) -> Dict[str, torch.Tensor]:
+                     grads=None, occupancy=None, occupancy_counts=None) -> Dict[str, torch.Tensor]:
     """render_rays_train with a background network, on weights already packed.  by_ray=False: the reference's random stream (the
     background draws shaped by the background ray count, read back here); by_ray=True: fixed-shape background draws, row i for ray
     i (GraphedTrainStep, which can read nothing back).  check_status=False leaves the sphere check to the caller.  grads: None, or
-    the (foreground, background) gradient blocks the backward accumulates into (autograd.RenderTrainBgCall)."""
+    the (foreground, background) gradient blocks the backward accumulates into (autograd.RenderTrainBgCall).  occupancy /
+    occupancy_counts: as for render_rays_train."""
     dev = rays.device
     rays = K.f32c(rays.detach())
     N = rays.shape[0]
@@ -637,7 +665,7 @@ def _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sph
     sh_deg = hparams.sh_deg if (hparams.pos_dir_dim == 0 and hparams.sh_deg is not None) else -1
     call = AG.RenderTrainBgCall(native, bnative, rays, idx, center, radius, real, c2d, steps, steps_bg, jitter, jit_b, float(perturb),
                                 noise_c, nc_b, u, u_b, noise_f, nf_b, Sc, Sf, cascade, sh_deg, by_ray, get_depth, get_depth_variance,
-                                get_bg_fg_rgb, bg_grads, grads)
+                                get_bg_fg_rgb, bg_grads, grads, occupancy, occupancy_counts)
     o = AG.render_train_bg_apply(call)
     if check_status:
         h = K.ctx(dev)
@@ -660,9 +688,11 @@ def _render_train_bg(net, native, bg, bnative, rays, image_indices, hparams, sph
     return res
 
 
-def _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance, grads=None) -> Dict[str, torch.Tensor]:
+def _render_train(net, native, rays, image_indices, hparams, get_depth, get_depth_variance, grads=None, occupancy=None,
+                  occupancy_counts=None) -> Dict[str, torch.Tensor]:
     """render_rays_train on weights already packed (sync, or a repack inside a captured training step).  grads: None, or the
-    gradient block the backward accumulates into (autograd.RenderTrainCall)."""
+    gradient block the backward accumulates into (autograd.RenderTrainCall).  occupancy / occupancy_counts: as for
+    render_rays_train."""
     dev = rays.device
     rays = K.f32c(rays.detach())
     N = rays.shape[0]
@@ -679,7 +709,7 @@ def _render_train(net, native, rays, image_indices, hparams, get_depth, get_dept
     noise_f = _density_noise(hparams, N * Sq, dev)
     sh_deg = hparams.sh_deg if (hparams.pos_dir_dim == 0 and hparams.sh_deg is not None) else -1
     call = AG.RenderTrainCall(native, rays, idx, steps, jitter, float(perturb), noise_c, u, noise_f, Sc, Sf, cascade, sh_deg,
-                              get_depth, get_depth_variance, grads)
+                              get_depth, get_depth_variance, grads, occupancy, occupancy_counts)
     rgb, rgb_coarse, depth, var = AG.render_train_apply(call)
     res: Dict[str, torch.Tensor] = {}
     if cascade:
